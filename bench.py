@@ -34,9 +34,10 @@ WORKLOADS = {
                seed=0xB25C0DE0 + 1, desc="C1: 1k docs, 100 3-term queries"),
     "c4": dict(docs=10_000_000, vocab=100_000, doclen=128, queries=4_000, tmin=8, tmax=8, zipf=1.0, k=10,
                seed=0xB25C0DE0 + 4, desc="C4: 10M docs Zipf(1), 8-term queries (4000-query subset; --no-prune = exhaustive)"),
-    "c5": dict(docs=50_000_000, vocab=100_000, doclen=128, queries=1_000_000, tmin=1, tmax=8, zipf=0.0, k=10,
+    # 25M docs: the replica (12 B per posting: postings + doc-id copy, 39 GB) fits one 80 GB H100 with room to spare
+    "c5": dict(docs=25_000_000, vocab=100_000, doclen=128, queries=1_000_000, tmin=1, tmax=8, zipf=0.0, k=10,
                seed=0xB25C0DE0 + 5, scaling="strong",
-               desc="C5: 50M docs replicated, ONE batch of 1M mixed 1-8 term queries sharded over the GPUs, top-10"),
+               desc="C5: 25M docs replicated, ONE batch of 1M mixed 1-8 term queries sharded over the GPUs, top-10"),
 }
 
 
@@ -54,11 +55,13 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-strong", action="store_true", help="skip the strong-scaling side leg of the default run")
     ap.add_argument("--no-prune", action="store_true", help="disable MaxScore-style pruning (exhaustive streaming)")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="write the result rows of the last timed step as DIR/<name>.npy (float32 / float64)")
     return ap.parse_args()
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -119,17 +122,25 @@ def effective_cores():
     return eff, {"affinity": n, "cgroup_quota": quota, "os_cpu_count": os.cpu_count()}
 
 
-def measured_traffic(workload, nq, k):
-    """dram__bytes_read.sum + dram__bytes_write.sum of the search kernel from the COMMITTED ncu capture of this exact
-    launch (profiles/*_traffic.json — newest kernel first; not measured in this run), else None."""
-    for name in ("r3_traffic.json", "r2_traffic.json"):
-        try:
-            t = json.load(open(os.path.join(ROOT, "profiles", name)))
-            if t["workload"] == workload and t["queries"] == nq and t["k"] == k:
-                return t["dram_bytes_read"] + t["dram_bytes_write"]
-        except Exception:
-            pass
-    return None
+DUMP_BYTES = 64_000_000   # --dump-outputs: larger outputs are written for a fixed, seeded sample of query rows
+
+
+def dump_outputs(d, res):
+    """Writes the result rows a caller of the batch receives (doc ids, f32 / f64 scores, counts) as DIR/<name>.npy.
+    Doc ids and counts go out as float64 (exact below 2^53)."""
+    os.makedirs(d, exist_ok=True)
+    arrays = {"doc": res["doc"].astype(np.float64), "score": res["score"].astype(np.float32),
+              "score64": res["score64"].astype(np.float64), "n": res["n"].astype(np.float64)}
+    nq = len(arrays["n"])
+    row_bytes = sum(a[:1].nbytes for a in arrays.values()) + 8   # + its entry in rows.npy
+    cap = (DUMP_BYTES - 4096) // row_bytes                       # (npy headers)
+    rows = np.arange(nq)
+    if nq > cap:
+        rows = np.sort(np.random.default_rng(0xB25D).choice(nq, cap, replace=False))
+        arrays = {name: a[rows] for name, a in arrays.items()}
+    arrays["rows"] = rows.astype(np.float64)   # which query of the batch each dumped row answers
+    for name, a in arrays.items():
+        np.save(os.path.join(d, f"{name}.npy"), a)
 
 
 def kernel_name(tmax, k, zipf=0.0):
@@ -151,7 +162,7 @@ def hbm_peak():
     try:
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s; not measured)"
 
 
 def cpu_reference(oix, q_off, q_terms, k, n, threads):
@@ -336,7 +347,7 @@ def main():
               "queries_per_gpu_per_step": nq, "terms_per_query": [wl["tmin"], wl["tmax"]], "k": k,
               "zipf_s": wl["zipf"], "postings": n_postings,
               "parallelism": f"queries sharded over {world} GPU(s), index replicated (NCCL broadcast at load)",
-              "l2": "index (8 B/posting) is far larger than the 126 MB L2; no flush needed",
+              "l2": "index (8 B/posting) is far larger than the 50 MB L2; no flush needed",
               "k_note": "BASELINE.json's metric says top-10, its configs[2] words the same 10M-doc case as top-100: "
                         "`value` is top-10, the `top100` object is the same batch at k=100",
               "gen_s": round(t_gen, 1), "index_build_s": round(t_index, 1), "replicate_s": round(t_repl, 2)}
@@ -381,6 +392,8 @@ def main():
     ev1.record(stream)
     torch.cuda.synchronize()
     ms_total = ev0.elapsed_time(ev1)
+    if rank == 0 and a.dump_outputs:
+        dump_outputs(a.dump_outputs, batch.fetch(want_f64=True))
     if world > 1:
         dist.barrier()
     torch.cuda.synchronize()
@@ -402,7 +415,7 @@ def main():
     index.search_batch(q_off, q_terms, k, want_f64=False, out=out)
     torch.cuda.synchronize()
     t0 = time.perf_counter()
-    e2e_steps = max(3, min(a.steps, 10))
+    e2e_steps = a.steps
     for _ in range(e2e_steps):
         index.search_batch(q_off, q_terms, k, want_f64=False, out=out)
     torch.cuda.synchronize()
@@ -435,7 +448,7 @@ def main():
         strong_obj = strong_leg(m, torch, dist, index, stream, qs[0], qs[1], k, rank, world, local_rank)
         if strong_obj:
             strong_obj["workload"] = (f"C5's query mix (1-8 terms, seed of configs[4]) on THIS corpus ({wl['docs']} docs): "
-                                      f"one batch of {STRONG_MIX_QUERIES} queries; the 50M-doc corpus itself: --workload c5")
+                                      f"one batch of {STRONG_MIX_QUERIES} queries; the 25M-doc corpus itself: --workload c5")
 
     t = torch.tensor([ms_total, 1e3 * e2e_s], dtype=torch.float64, device="cuda")
     if world > 1:
@@ -462,13 +475,12 @@ def main():
             "ms_per_step": ms_step, "higher_is_better": True, "scaling": "strong" if strong else "weak", "vs_baseline": None,
             "dtype": "f32 filter + f64 exact re-score (u32 doc ids)", "data": "synthetic", "config": config,
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": None if a.no_prune else measured_traffic(a.workload, nq, k), "peak_source": peak_src, "kernel": kernel_name(wl["tmax"], k, wl["zipf"]),
+                         "peak_source": peak_src, "kernel": kernel_name(wl["tmax"], k, wl["zipf"]),
                          "kernel_ms": kms, "algorithmic_bytes_per_launch": bytes_algo,
                          "postings_exhaustive": int(st.postings), "postings_streamed": fetched,
                          "pruning": "off" if a.no_prune else "on",
                          "note": "achieved = ALGORITHMIC bytes (8 B per posting, SURVEY 8d) / kernel time; the seeded kernel streams "
-                                 "doc ids only (4 B per posting), so `traffic` (DRAM bytes of the same launch, committed ncu "
-                                 "capture) is about half of that",
+                                 "doc ids only (4 B per posting), so its DRAM traffic is about half of that",
                          "skipped_frac": max(0.0, 1.0 - touched / max(1, int(st.postings)))},
             "cpu_baseline": cpu_baseline,
             "e2e": {"value": e2e_value, "unit": "queries/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,

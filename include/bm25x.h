@@ -1,5 +1,5 @@
 /*
- * bm25x.h — C ABI of the B200-native BM25 top-k engine (libbm25x.so).
+ * bm25x.h — C ABI of the H100-native BM25 top-k engine (libbm25x.so).
  *
  * This is the drop-in boundary for ONE path of tensorchord/VectorChord-bm25: the
  * ranked top-k query `bm25::search` (and, next, `bm25::evaluate`).  Each entry
@@ -10,7 +10,7 @@
  * bm25x_last_error() holds a thread-local message.
  *
  * There is NO CPU fallback: every search entry point fails with
- * BM25X_ERR_CUDA when no sm_100 device / kernel image is available.
+ * BM25X_ERR_CUDA when no sm_90 device / kernel image is available.
  */
 #ifndef BM25X_H
 #define BM25X_H
@@ -170,7 +170,7 @@ int bm25x_blake3_keyed16(const uint8_t key[32], const uint8_t *data, size_t len,
  *     out_doc u32, out_score f32 (positive; the SQL binding negates, operators.rs:54),
  *     out_score64 f64 or NULL (bit-identical to Cache::evaluate summed in ascending term order),
  *     out_payload u16[3] or NULL, out_n[i] = rows returned (<= k).
- * Host pointers; the call copies H2D, runs the sm_100a kernels, copies D2H. */
+ * Host pointers; the call copies H2D, runs the sm_90a kernels, copies D2H. */
 int bm25x_search_batch(bm25x_index *idx, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms, uint32_t k,
                        const uint8_t *allow, uint32_t *out_doc, float *out_score, double *out_score64,
                        uint16_t *out_payload, uint32_t *out_n, bm25x_search_stats *stats);

@@ -359,7 +359,7 @@ int orc_search_exhaustive(const orc_index *ix, const uint32_t *terms, int nterms
 
 /* ------------------------------------------------------------------------- */
 /* Rust std BinaryHeap restated (max-heap; library/alloc/src/collections/
- * binary_heap/mod.rs — NOT under /root/reference, written from the published
+ * binary_heap/mod.rs — NOT in the reference tree, written from the published
  * algorithm; only matters for the order of equal elements).  Generic over an
  * array of int handles with a user comparator returning <0,0,>0 like Ord::cmp. */
 

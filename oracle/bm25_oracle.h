@@ -8,7 +8,7 @@
  *
  * It is a plain-C restatement of the reference's algorithm (Rust, not
  * buildable here: no rustc/cargo/Postgres).  Every function cites the
- * reference file:line it follows (paths relative to /root/reference).
+ * reference file:line it follows (paths relative to the reference tree).
  *
  * Parity pins: the fieldnorm table, Score bit trick, the sqllogictest ranking
  * goldens and hand-checked Cache::evaluate values are pinned in

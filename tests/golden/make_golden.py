@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Regenerates tests/golden/reference_golden.json from the read-only reference tree.
 
-Run in the build container only (needs /root/reference):
-    python tests/golden/make_golden.py
+Needs a checkout of the reference tree:
+    python tests/golden/make_golden.py <path to tensorchord/VectorChord-bm25>
 Extracts every golden / known answer the reference's own tests hold for the
 BM25 top-k path (SURVEY.md §8c):
   * the literal FIELDNORM_TO_LENGTH table        crates/bm25/src/bm25.rs:15-272
@@ -18,8 +18,9 @@ the fieldnorm is exact).
 import json
 import os
 import re
+import sys
 
-REF = "/root/reference"
+REF = sys.argv[1] if len(sys.argv) > 1 else "."
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "reference_golden.json")
 
 STOP = set("""i me my myself we our ours ourselves you your yours yourself yourselves he him his himself she her

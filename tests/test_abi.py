@@ -31,12 +31,12 @@ def test_exports_every_declared_symbol(m):
         assert hasattr(lib, n), f"{n} declared in include/*.h but not exported"
 
 
-def test_library_has_only_sm100a_code(m):
+def test_library_has_only_sm90a_code(m):
     import subprocess
     out = subprocess.run(["cuobjdump", "-lelf", os.path.join(ROOT, "vectorchord-bm25_b200", "libbm25x.so")],
                          capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_(\d+a?)", out))
-    assert archs == {"100a"}, archs
+    assert archs == {"90a"}, archs
 
 
 def test_no_cpu_fallback(m):

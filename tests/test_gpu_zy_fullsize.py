@@ -83,13 +83,14 @@ def test_config4_zipf_8term_pruning_on_off(m, orc):
     ix.close()
 
 
-def test_config5_50M_docs_mixed_queries(m, orc):
-    """configs[4]: 50M docs (vocab 100k uniform, 128 terms/doc: 51 GB of postings in HBM), 1M mixed-length (1..8 term)
-    queries, top-10 — one GPU's worth here; sharding across ranks is tests/test_sharding_gloo.py + bench.py --workload c5."""
+def test_config5_25M_docs_mixed_queries(m, orc):
+    """configs[4]: 25M docs (vocab 100k uniform, 128 terms/doc: 26 GB of postings, 39 GB of index in HBM), 1M
+    mixed-length (1..8 term) queries, top-10 — one GPU's worth here; sharding across ranks is
+    tests/test_sharding_gloo.py + bench.py --workload c5."""
     import psutil
-    if psutil.virtual_memory().available < 220e9:
-        pytest.skip("needs ~200 GB of host memory for the 50M-doc CSR + the oracle's copy")
-    c = m.synth_corpus(0xB25C0DE5, 50_000_000, 100_000, 128)
+    if psutil.virtual_memory().available < 110e9:
+        pytest.skip("needs ~100 GB of host memory for the 25M-doc CSR + the oracle's copy")
+    c = m.synth_corpus(0xB25C0DE5, 25_000_000, 100_000, 128)
     q_off, q_terms = m.synth_queries(0xB25C0DE5 + 1000, 1_000_000, 100_000, 1, 8, c.post_off)
     ix = m.Index.from_corpus(c)
     res = ix.search_batch(q_off, q_terms, 10)

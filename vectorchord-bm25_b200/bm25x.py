@@ -91,7 +91,7 @@ class _Synth(C.Structure):
 
 
 def build_library(force: bool = False) -> str:
-    """nvcc -gencode arch=compute_100a,code=sm_100a build of csrc/ → libbm25x.so (in-tree)."""
+    """nvcc -gencode arch=compute_90a,code=sm_90a build of csrc/ → libbm25x.so (in-tree)."""
     srcdir = os.path.join(_HERE, "csrc")
     srcs = [os.path.join(srcdir, f) for f in os.listdir(srcdir)] + [os.path.join(_HERE, "..", "include", "bm25x.h")]
     if force or not os.path.exists(_SO) or os.path.getmtime(_SO) < max(os.path.getmtime(s) for s in srcs):

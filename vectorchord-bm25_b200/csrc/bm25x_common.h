@@ -1,4 +1,4 @@
-// bm25x_common.h — internal types shared by the host library and the sm_100a kernels.
+// bm25x_common.h — internal types shared by the host library and the sm_90a kernels.
 #pragma once
 
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-// bm25x_device.cuh — device-side building blocks of the search kernel (sm_100a): launch parameters, mbarrier / TMA
+// bm25x_device.cuh — device-side building blocks of the search kernel (sm_90a): launch parameters, mbarrier / TMA
 // bulk-copy PTX helpers, the two score functions (f32 filter, f64 exact), the tie signature and the warp-private pool.
 #pragma once
 

@@ -352,7 +352,7 @@ static cudaError_t build_champions(bm25x_index *ix) {
     ix->device_bytes += sizeof(uint64_t) * ((size_t)T + 1);
     e = cudaMemcpy(d.champ_off, h_off.data(), sizeof(uint64_t) * ((size_t)T + 1), cudaMemcpyHostToDevice);
     if (e != cudaSuccess || !T) return e;
-    const unsigned blocks = (unsigned)std::min<uint64_t>(((uint64_t)T + CHAMP_WARPS - 1) / CHAMP_WARPS, 148ull * 16ull);
+    const unsigned blocks = (unsigned)std::min<uint64_t>(((uint64_t)T + CHAMP_WARPS - 1) / CHAMP_WARPS, (uint64_t)ix->sm_count * 16ull);
     k_champions<<<blocks, CHAMP_WARPS * 32>>>(d.post_off, d.df, d.post, d.s0d, d.s1d, T, d.champ_off, d.champ);
     e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaDeviceSynchronize();
@@ -449,8 +449,8 @@ static int index_begin(const BuildMeta &m, int device, bm25x_index **ixp) {
     CU(cudaSetDevice(device));
     cudaDeviceProp prop;
     CU(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) {
-        bm25x_set_error("bm25x_index_create: device %d is sm_%d%d; this library only carries sm_100a kernels", device,
+    if (prop.major != 9 || prop.minor != 0) {
+        bm25x_set_error("bm25x_index_create: device %d is sm_%d%d; this library only carries sm_90a kernels", device,
                         prop.major, prop.minor);
         bm25x_index_destroy(ix);
         return BM25X_ERR_CUDA;
@@ -578,7 +578,7 @@ static cudaError_t index_finish_device(bm25x_index *ix) {
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) {
-        k_extract_docs<<<148 * 8, 256>>>(d.post, d.n_post_pad + BM25X_POST_SLACK, d.pdoc);
+        k_extract_docs<<<ix->sm_count * 8, 256>>>(d.post, d.n_post_pad + BM25X_POST_SLACK, d.pdoc);
         e = cudaGetLastError();
     }
     if (e == cudaSuccess && nb) {
@@ -587,7 +587,7 @@ static cudaError_t index_finish_device(bm25x_index *ix) {
         e = cudaGetLastError();
     }
     if (e == cudaSuccess && T) {
-        k_term_ub<<<(unsigned)std::min<uint32_t>(T, 148u * 16u), 256>>>(d.post_off, d.df, d.post, d.s0d, d.s1d, T, d.ubd);
+        k_term_ub<<<(unsigned)std::min<uint32_t>(T, (uint32_t)ix->sm_count * 16u), 256>>>(d.post_off, d.df, d.post, d.s0d, d.s1d, T, d.ubd);
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) e = cudaDeviceSynchronize();
@@ -1020,8 +1020,8 @@ extern "C" int bm25x_index_alloc_replica(const bm25x_index_layout *like, int dev
     CU(cudaSetDevice(device));
     cudaDeviceProp prop;
     CU(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) {
-        bm25x_set_error("bm25x_index_alloc_replica: device %d is sm_%d%d; this library only carries sm_100a kernels", device,
+    if (prop.major != 9 || prop.minor != 0) {
+        bm25x_set_error("bm25x_index_alloc_replica: device %d is sm_%d%d; this library only carries sm_90a kernels", device,
                         prop.major, prop.minor);
         bm25x_index_destroy(ix);
         return BM25X_ERR_CUDA;
@@ -1067,7 +1067,7 @@ extern "C" int bm25x_index_finalize_replica(bm25x_index *ix) {
     }
     BM25X_CUDA_TRY(cudaSetDevice(ix->device));
     // derived data that does not travel: the doc-id-only copy of the postings
-    k_extract_docs<<<148 * 8, 256>>>(ix->d.post, ix->d.n_post_pad + BM25X_POST_SLACK, ix->d.pdoc);
+    k_extract_docs<<<ix->sm_count * 8, 256>>>(ix->d.post, ix->d.n_post_pad + BM25X_POST_SLACK, ix->d.pdoc);
     BM25X_CUDA_TRY(cudaGetLastError());
     BM25X_CUDA_TRY(cudaDeviceSynchronize());
     ix->h_df.resize(ix->d.n_terms);

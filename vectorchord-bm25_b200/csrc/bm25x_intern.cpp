@@ -4,8 +4,8 @@
 //   everything else: the first 16 bytes of blake3::keyed_hash(seed, token), a zero last byte replaced by 1 so that a
 //   hashed key can never collide with a padded short token.
 //
-// The reference takes BLAKE3 from the `blake3` crate (Cargo.lock: blake3 1.8.4), which is not vendored under
-// /root/reference; the function below restates the published BLAKE3 algorithm (keyed_hash mode, full chunk tree) in
+// The reference takes BLAKE3 from the `blake3` crate (Cargo.lock: blake3 1.8.4), which is not vendored in
+// the reference tree; the function below restates the published BLAKE3 algorithm (keyed_hash mode, full chunk tree) in
 // portable C++.  Host code: keys are computed where the tokens are (the Rust side / the caller), never on the GPU.
 #include <stdint.h>
 #include <string.h>

@@ -1,4 +1,4 @@
-// bm25x_search.cu — batched BM25 top-k over the HBM-resident index (sm_100a).
+// bm25x_search.cu — batched BM25 top-k over the HBM-resident index (sm_90a).
 //
 // Replaces bm25::search (crates/bm25/src/search.rs:28-282): instead of one query walking cursors
 // over 8 KiB pages with Block-max WAND, a persistent grid streams every query's posting lists

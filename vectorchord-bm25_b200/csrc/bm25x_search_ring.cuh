@@ -1,4 +1,4 @@
-// bm25x_search_ring.cuh — kernel v6 (sm_100a): one WARP per query, ring stages + presence map, seeded flavour.
+// bm25x_search_ring.cuh — kernel v6 (sm_90a): one WARP per query, ring stages + presence map, seeded flavour.
 //
 // Replaces the per-query cursor walk of bm25::search (crates/bm25/src/search.rs:137-282) for a whole batch: every
 // warp of the persistent grid is a complete query engine (lane j owns term j of its query).
@@ -65,7 +65,7 @@ namespace {
 #define BM25X_RING_U 2
 #endif
 #ifndef BM25X_RING_MAXWARPS
-#define BM25X_RING_MAXWARPS 20  // 20 warps = 102 registers per thread (a few spills; 16: 18.5 ms, 20: 16.5 ms, 24: 19.1 ms on C3)
+#define BM25X_RING_MAXWARPS 20  // 20 warps = 102 registers per thread (a few spills; C3 on H100: 16 warps slower, 24 no faster)
 #endif
 #ifndef BM25X_RING_INIT
 #define BM25X_RING_INIT 32
@@ -77,7 +77,7 @@ namespace {
 #define BM25X_RING_SB 1  // 1: single-buffered rings (refill after the chunk, next round prefetched into L2); 0: double-buffered
 #endif
 #ifndef BM25X_RING_SUBT
-#define BM25X_RING_SUBT (1u << 30)  // classes of 8+ terms: postings per map generation (sub-window); default: off (measured: no gain, profiles/README.md)
+#define BM25X_RING_SUBT (1u << 30)  // classes of 8+ terms: postings per map generation (sub-window); default: off (no gain on C3 / C4)
 #endif
 #ifndef BM25X_RING_ADAPT
 #define BM25X_RING_ADAPT 1  // 1: ring sizes per query ∝ df; 0: M equal rings
@@ -150,7 +150,7 @@ struct RCfg {
     // which the rare terms' stay empty; queries with fewer than M terms use the whole budget.
     static constexpr int BUDGET = M_ * R;
     // Only the classes of 8+ terms size their rings per query (that is where head terms meet rare ones); for 1..4 terms
-    // the geometry stays a compile-time constant (M equal rings): runtime masks and bases cost the 3-term loop 10 %.
+    // the geometry stays a compile-time constant (M equal rings): runtime masks and bases slow the 3-term loop down.
     static constexpr bool ADAPT = (BM25X_RING_ADAPT != 0) && M_ >= 8;
     static constexpr int LOG_RMIN = 6;
     static constexpr int LOG_RMAX = (LOG_R + 2 > 10 ? 10 : LOG_R + 2) > LOG_R ? (LOG_R + 2 > 10 ? 10 : LOG_R + 2) : LOG_R;
@@ -200,7 +200,7 @@ __device__ __forceinline__ uint32_t ring_slot(uint32_t doc, uint32_t bytes) { re
 
 // lower_bound of `doc` in ring positions [a, e) (posting indices of the term; the ring holds index i at i & RM).
 // Fixed LOG_R + 1 power-of-two steps, no data-dependent branch: every lane of a verification pass searches the same run,
-// and independent searches interleave (the while-loop form cost 135 warp instructions per search, profiles/r2b).
+// and independent searches interleave (the while-loop form costs several times the instructions per search).
 __device__ __forceinline__ uint32_t ring_doc(const Posting *rg, uint32_t pos) { return rg[pos].doc; }
 __device__ __forceinline__ uint32_t ring_doc(const uint32_t *rg, uint32_t pos) { return rg[pos]; }
 template <class C, int TOP = C::LOG_RMAX>

@@ -37,6 +37,156 @@ def _compare(res, oix, q_off, q_terms, k, allow=None, what=""):
         assert np.all(res["doc"][i, n:] == 0xFFFFFFFF)
 
 
+class _PrefixOracle:
+    """OracleIndex.search_exhaustive at one large limit, memoised per (query, bitmap): the canonical order (score desc,
+    doc asc) is total, so the top-k of every smaller k is a prefix of it."""
+
+    def __init__(self, oix, kmax):
+        self.oix, self.kmax, self.memo = oix, kmax, {}
+
+    def search_exhaustive(self, q, k, allow=None):
+        assert k <= self.kmax
+        q = np.ascontiguousarray(q, dtype=np.uint32)
+        key = (q.tobytes(), None if allow is None else np.asarray(allow).tobytes())
+        if key not in self.memo:
+            self.memo[key] = self.oix.search_exhaustive(q, self.kmax, allow=allow)
+        od, os_, tg = self.memo[key]
+        return od[:k], os_[:k], tg
+
+
+def _live_queries(rng, df, counts, weighted=False):
+    """One query per entry of `counts` with exactly that many distinct terms of df > 0, ascending ids.  weighted: terms
+    drawn in proportion to df (head terms in most queries)."""
+    live = np.flatnonzero(df > 0)
+    p = df[live] / df[live].sum() if weighted else None
+    qs = [np.sort(rng.choice(live, size=n, replace=False, p=p)) for n in counts]
+    q_off = np.cumsum([0] + [len(q) for q in qs]).astype(np.uint32)
+    return q_off, np.concatenate(qs).astype(np.uint32)
+
+
+def _rows_identical(a, b, what):
+    for key in ("doc", "score", "score64", "n"):
+        assert np.array_equal(a[key], b[key]), f"{what}: {key}"
+
+
+def _csr_corpus(rng, n_docs, lists, extra_len=0):
+    """Term-major CSR from explicit posting lists [(doc ids, tfs)]; a document's length is its Σ tf plus up to
+    `extra_len` tokens of terms outside the corpus (varied norms)."""
+    off = np.zeros(len(lists) + 1, dtype=np.uint64)
+    off[1:] = np.cumsum([len(d) for d, _ in lists])
+    post_doc = np.concatenate([np.asarray(d, np.uint32) for d, _ in lists])
+    post_tf = np.concatenate([np.asarray(t, np.uint32) for _, t in lists])
+    doc_len = np.bincount(post_doc, weights=post_tf, minlength=n_docs).astype(np.uint32)
+    if extra_len:
+        doc_len += rng.integers(0, extra_len + 1, size=n_docs).astype(np.uint32)
+    return doc_len, off, post_doc, post_tf
+
+
+TWO_PASS = [
+    # uniform vocabulary: df is not monotone in the term id, so the two groups interleave in id order
+    dict(name="uniform", seed=101, n=20000, vocab=1500, lmin=8, lmax=120, zipf=0.0, weighted=False),
+    # dense: 72 terms, long documents (dense windows in pass 0)
+    dict(name="dense", seed=102, n=4000, vocab=72, lmin=60, lmax=400, zipf=0.5, weighted=False),
+    # Zipf, terms drawn by df: head terms pruned while group 1 is probed
+    dict(name="zipf", seed=103, n=30000, vocab=3000, lmin=16, lmax=96, zipf=1.0, weighted=True),
+]
+
+
+@pytest.mark.parametrize("cfg", TWO_PASS, ids=[c["name"] for c in TWO_PASS])
+def test_more_than_32_terms_two_passes(m, orc, cfg):
+    """33..64 live terms run as two passes of the 32-term kernel: the host puts the 32 rarest terms (by df, then id) first,
+    pass 0 streams them and probes the others, pass 1 streams the others and keeps only documents without a group-0 term,
+    and the exact f64 sum merges both groups back into ascending term order.  Bit-exact against the oracle for every
+    limit class, pruning on and off, with and without a prefilter bitmap, plain and two-phase options."""
+    c = m.synth_corpus(cfg["seed"], cfg["n"], cfg["vocab"], cfg["lmin"], cfg["lmax"], cfg["zipf"])
+    ix = m.Index.from_corpus(c)
+    df = ix.df()
+    rng = np.random.default_rng(cfg["seed"])
+    counts = [33, 40, 48, 63, 64] * 3
+    q_off, q_terms = _live_queries(rng, df, counts, weighted=cfg["weighted"])
+    assert np.array_equal(np.diff(q_off), counts)
+    if cfg["name"] == "uniform":  # the (df, id) split is not a cut in id order
+        inter = 0
+        for i in range(len(counts)):
+            q = q_terms[q_off[i]:q_off[i + 1]]
+            g0 = sorted(q.tolist(), key=lambda t: (df[t], t))[:32]
+            inter += max(g0) > min(set(q.tolist()) - set(g0))
+        assert inter == len(counts)
+    allow = np.packbits(rng.random(c.n_docs) < 0.3, bitorder="little")
+    ks = (1, 10, 100, 225, 1000, 1025)
+    oix = _PrefixOracle(_oracle_index(orc, c), max(ks))
+    for k in ks:
+        for al in (None, allow):
+            first = None
+            for two in (0, 1):
+                for prune in (1, 0):
+                    ix.set_option("twophase", two)
+                    ix.set_option("prune", prune)
+                    res = ix.search_batch(q_off, q_terms, k, allow=al)
+                    if first is None:
+                        first = res
+                        _compare(res, oix, q_off, q_terms, k, allow=al, what=f"{cfg['name']} k={k} allow={al is not None}")
+                    else:
+                        _rows_identical(res, first, f"{cfg['name']} k={k} twophase={two} prune={prune}")
+    ix.close()
+
+
+def test_more_than_32_terms_rarest_split_ties_and_refusals(m, orc):
+    """The rarest-32 split when many terms share the df at the 32/33 boundary (the term id decides), raw queries of 80
+    terms that reduce to <= 64 live ones (duplicates, unknown ids, TERM_MISSING: the canonical query's rows), and the
+    refusal of 65 live terms (BM25X_ERR_UNSUPPORTED)."""
+    rng = np.random.default_rng(7)
+    n_docs, T = 3000, 80
+    want_df = np.array([40] * 16 + [90] * 30 + list(rng.integers(200, 900, size=T - 46)))
+    want_df = want_df[rng.permutation(T)]  # the boundary terms sit anywhere in id order
+    lists = [(np.sort(rng.choice(n_docs, size=int(d), replace=False)), rng.integers(1, 5, size=int(d))) for d in want_df]
+    doc_len, off, pd_, pt = _csr_corpus(rng, n_docs, lists, extra_len=50)
+    ix = m.Index(n_docs, doc_len, T, off, pd_, pt)
+    oix = orc.OracleIndex(orc.Corpus(n_docs, doc_len, T, off, pd_, pt))
+    assert np.array_equal(ix.df(), want_df)
+    rare, tied, common = (np.flatnonzero(want_df == 40), np.flatnonzero(want_df == 90), np.flatnonzero(want_df >= 200))
+    qs = [np.concatenate([rare, tied, common[:18]]),                    # 64: the split cuts the df = 90 group at 16 of 30
+          np.concatenate([rare[:6], tied, common[:4]]),                 # 40: 26 of the 30 tied terms in group 0
+          np.concatenate([tied, common[:10]])]                          # 40: group 0 = the 30 tied + 2 common terms
+    q_off = np.cumsum([0] + [len(q) for q in qs]).astype(np.uint32)
+    q_terms = np.concatenate([np.sort(q) for q in qs]).astype(np.uint32)
+    for k in (1, 10, 100, 1000, 1025):
+        for prune in (1, 0):
+            ix.set_option("prune", prune)
+            _compare(ix.search_batch(q_off, q_terms, k), oix, q_off, q_terms, k, what=f"tie split k={k} prune={prune}")
+    ix.set_option("prune", 1)
+
+    # 80 raw terms, <= 64 live: the same rows as the canonical query
+    c = m.synth_corpus(104, 8000, 600, 8, 64, 0.0)
+    cix = m.Index.from_corpus(c)
+    df = cix.df()
+    live = np.flatnonzero(df > 0)
+    raws, canon = [], []
+    for n_live in (33, 60, 64):
+        q = rng.choice(live, size=n_live, replace=False)
+        junk = [m.TERM_MISSING] * 4 + [c.n_terms, c.n_terms + 7, 10 ** 6] + list(rng.choice(q, size=80 - n_live - 7))
+        raw = rng.permutation(np.concatenate([q, np.array(junk)]).astype(np.uint32))
+        assert len(raw) == 80
+        raws.append(raw)
+        canon.append(np.sort(q).astype(np.uint32))
+    r_off = np.cumsum([0] + [len(q) for q in raws]).astype(np.uint32)
+    c_off = np.cumsum([0] + [len(q) for q in canon]).astype(np.uint32)
+    c_terms = np.concatenate(canon)
+    for k in (10, 1025):
+        a = cix.search_batch(r_off, np.concatenate(raws), k)
+        b = cix.search_batch(c_off, c_terms, k)
+        _rows_identical(a, b, f"raw vs canonical k={k}")
+        _compare(b, _oracle_index(orc, c), c_off, c_terms, k, what=f"canonical k={k}")
+    # 65 live terms: refused for the whole batch (two passes of 32 lanes cover 64)
+    q65 = np.sort(rng.choice(live, size=65, replace=False)).astype(np.uint32)
+    for q in (q65, np.concatenate([q65, q65[:10], [m.TERM_MISSING]]).astype(np.uint32)):
+        with pytest.raises(m.Bm25xError) as e:
+            cix.search_batch(np.array([0, 3, 3 + len(q)], np.uint32), np.concatenate([q[:3], q]), 10)
+        assert e.value.code == 4
+    cix.close()
+    ix.close()
+
+
 CONFIGS = [
     dict(name="C1", seed=0xB25C0DE1, n=1000, vocab=1000, lmin=32, lmax=32, zipf=0.0, nq=100, tmin=3, tmax=3),
     dict(name="varlen", seed=21, n=20000, vocab=3000, lmin=1, lmax=300, zipf=0.0, nq=80, tmin=1, tmax=8),
@@ -167,16 +317,8 @@ def test_replica_same_device_identical(m, orc):
     """bm25x_index_get_layout / alloc_replica / finalize_replica on ONE GPU: the 13 replicated arrays copied device to
     device (what shard.replicate_index does with NCCL broadcasts), the derived structures (doc-id copy, champion lists)
     rebuilt by finalize_replica — the replica answers like the original, seeded and plain kernel."""
-    import ctypes
-    rt = None
-    for name in ("libcudart.so", "libcudart.so.12", "/usr/local/cuda/lib64/libcudart.so"):
-        try:
-            rt = ctypes.CDLL(name)
-            break
-        except OSError:
-            pass
-    assert rt is not None, "libcudart not found"
-    rt.cudaMemcpy.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int]
+    from util_cuda import D2D, cudart
+    rt = cudart()
     c = m.synth_corpus(95, 60000, 5000, 8, 48, 0.0)
     q_off, q_terms = m.synth_queries(96, 150, c.n_terms, 1, 8, c.post_off, 0.0)
     ix = m.Index.from_corpus(c)
@@ -187,7 +329,7 @@ def test_replica_same_device_identical(m, orc):
     rl = rep.layout()
     for i in range(len(lay.dev_ptr)):
         assert rl.bytes[i] == lay.bytes[i]
-        assert rt.cudaMemcpy(rl.dev_ptr[i], lay.dev_ptr[i], lay.bytes[i], 3) == 0  # cudaMemcpyDeviceToDevice
+        assert rt.cudaMemcpy(rl.dev_ptr[i], lay.dev_ptr[i], lay.bytes[i], D2D) == 0
     rep.finalize_replica()
     for seed in (1, 0):
         ix.set_option("seed", seed)
@@ -209,7 +351,7 @@ def test_broker_over_an_index_matches_direct_search(m, orc):
     c = m.synth_corpus(97, 30000, 2000, 6, 40, 0.5)
     q_off, q_terms = m.synth_queries(98, 96, c.n_terms, 1, 6, c.post_off, 0.5)
     ix = m.Index.from_corpus(c)
-    limits = [1, 10, 32, 40, 128, 300]
+    limits = [1, 10, 32, 40, 128, 300, 2000]
     want = {k: ix.search_batch(q_off, q_terms, k, want_payload=True) for k in limits}
     br = bm.Broker(index=ix, max_batch=64, max_wait_us=5000)
     got, errs = [None] * 96, []

@@ -635,8 +635,8 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                 parity ^= 1u;
             }
             // MaxScore (the reference's WAND pivot rule, search.rs:152-169, applied to whole terms): the terms with the
-            // smallest score bounds leave the streamed set while the sum of their bounds stays <= ALPHA · k-th score.  A
-            // document holding only such terms cannot enter; for the others the bound is added back in the filter and
+            // smallest score bounds leave the streamed set while the sum of their bounds (plus ub_oth) stays <= ALPHA · k-th
+            // score.  A document holding only such terms cannot enter; for the others the bound is added back in the filter and
             // the exact contributions are probed at verification — best bound first, giving up on a document as soon as
             // the block-level bound (SummaryTuple.wand_*, search.rs:193-203) of the probed term plus the bounds of the
             // terms still to probe cannot lift it over the threshold.
@@ -656,7 +656,10 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                     const uint32_t ness = __popc(__ballot_sync(FULL, ess));
                     if (who == 0u || ness <= 1u) break;
                     const double ub = __longlong_as_double((long long)key);
-                    if (!(ub_ne + ub <= (double)BM25X_PRUNE_ALPHA * f.Sk)) break;
+                    // pass 0 of a two-pass query: a document holding pruned terms of this group and no streamed one is
+                    // seen by neither pass (pass 1 drops every document with a group-0 term), so the bound of such a
+                    // document includes the other group's terms (ub_oth; 0 in pass 1 and for <= 32 terms)
+                    if (!(ub_ne + ub + ub_oth <= (double)BM25X_PRUNE_ALPHA * f.Sk)) break;
                     const int who_i = __ffs(who) - 1;
                     if (C::M <= 8) {
                         ne_list |= (uint32_t)who_i << (4 * n_ne);

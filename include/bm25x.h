@@ -70,7 +70,11 @@ typedef struct {
     uint64_t bytes_algo;     /* 8 B/posting + 8 B/result slot + 16 B/query term (SURVEY §8d) */
     uint32_t launches;       /* kernels launched */
     uint32_t queries;        /* live queries (>= 1 known term) */
-    uint64_t postings_fetched; /* postings actually streamed into shared memory (< postings when pruning bites) */
+    /* postings streamed into shared memory (pad slots excluded), plus the block-table entries and postings read by the
+     * probes of pruned terms and of a two-pass query's other group, plus what is read again: the ring contents a
+     * two-phase query re-reads when it resumes, and the rings re-split when terms are pruned.  With pruning and two-phase
+     * off, it equals `postings` for queries of <= 32 live terms; with pruning on it can land on either side. */
+    uint64_t postings_fetched;
 } bm25x_search_stats;
 
 /* ---- index lifetime: replaces bm25::build → flush (crates/bm25/src/build.rs:22-71, flush.rs:40-158) for the
@@ -133,7 +137,7 @@ int bm25x_index_alloc_replica(const bm25x_index_layout *like, int device, bm25x_
 int bm25x_index_finalize_replica(bm25x_index *idx);
 /* Options.  "prune" (default 1): MaxScore-style pruning in the warp-per-query kernel — terms whose summed score upper
  * bounds (the token-level WAND bound of the reference: TokenTuple.wand_fieldnorm/wand_term_frequency,
- * flush.rs:101-120, search.rs:363) stay below 5 % of the current k-th score are no longer streamed; their postings
+ * flush.rs:101-120, search.rs:363) stay at or below half the current k-th score are no longer streamed; their postings
  * are looked up in HBM only for the candidates.  Results are identical with it on or off.
  * "seed" (default 1): queries of 2..8 terms with limit <= 128 and no prefilter bitmap run through the SEEDED kernel —
  * the documents that hold a single query term come from per-term champion lists (the term's best 128 postings in
@@ -178,7 +182,11 @@ int bm25x_search_batch(bm25x_index *idx, uint32_t nq, const uint32_t *q_off, con
 /* Split form of the same call, for pipelining and for timing the device part alone:
  * prepare = canonicalise + upload queries; run = kernels only, everything resident in HBM
  * (stream = cudaStream_t as void*, NULL = the library's stream; asynchronous unless stats != NULL);
- * fetch = D2H of the results. */
+ * fetch = D2H of the results, on the stream of the last run.
+ * A batch may be run any number of times: every run rewrites every result row of its live queries.  Runs of different
+ * batches may overlap on different streams.  The only wait run adds is for the batch's upload by prepare; ordering the
+ * runs of ONE batch on different streams (and reads of bm25x_batch_device_results after a run) is the caller's job,
+ * e.g. an event recorded on the earlier run's stream and waited on by the later one. */
 int bm25x_batch_prepare(bm25x_index *idx, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms, uint32_t k,
                         const uint8_t *allow, bm25x_batch **out);
 int bm25x_batch_run(bm25x_batch *batch, void *stream, bm25x_search_stats *stats);

@@ -1,5 +1,6 @@
-"""libcudart through ctypes, for tests that copy an index's device arrays (Index.layout()) without going through the
-library: device-to-device for replicas, device-to-host to compare the arrays with a CPU computation."""
+"""libcudart through ctypes, for tests that reach device memory without going through the library: an index's arrays
+(Index.layout()) copied device-to-device for replicas or device-to-host to compare them with a CPU computation, and a
+batch's result rows (Batch.device_results()) read back or poisoned before a rerun."""
 import ctypes
 
 import numpy as np
@@ -20,6 +21,7 @@ def cudart():
                 pass
         assert _rt is not None, "libcudart not found"
         _rt.cudaMemcpy.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int]
+        _rt.cudaMemset.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_size_t]
     return _rt
 
 
@@ -28,3 +30,13 @@ def download(dev_ptr, nbytes, dtype):
     out = np.empty(nbytes, dtype=np.uint8)
     assert cudart().cudaMemcpy(out.ctypes.data, dev_ptr, nbytes, D2H) == 0
     return out.view(dtype)
+
+
+def memset(dev_ptr, value, nbytes):
+    """Every byte of [dev_ptr, dev_ptr + nbytes) set to `value`.  On the legacy default stream, which does not wait for
+    non-blocking streams (the library's): finish their work first, and call device_synchronize() before they read."""
+    assert cudart().cudaMemset(dev_ptr, value, nbytes) == 0
+
+
+def device_synchronize():
+    assert cudart().cudaDeviceSynchronize() == 0

@@ -7,7 +7,7 @@ O=gpurun_out/$TAG
 timeout 600 python -m pytest tests -q -m gpu 2>&1 | tail -5 > ${O}_pytest_gpu.log; cat ${O}_pytest_gpu.log
 # the small test corpora are dense: by default most of their queries are handed back to the plain kernel — once more with
 # every eligible query forced through the seeded kernel
-BM25X_SEED_FORCE=1 timeout 600 python -m pytest tests/test_gpu_parity.py tests/test_gpu_paths.py tests/test_gpu_margins.py tests/test_gpu_zx_stress.py tests/test_gpu_zz_growing.py -q -m gpu 2>&1 | tail -3 > ${O}_pytest_gpu_seed_forced.log; cat ${O}_pytest_gpu_seed_forced.log
+BM25X_SEED_FORCE=1 timeout 600 python -m pytest tests/test_gpu_parity.py tests/test_gpu_paths.py tests/test_gpu_margins.py tests/test_gpu_zx_stress.py tests/test_gpu_zz_growing.py tests/test_gpu_batch.py -q -m gpu 2>&1 | tail -3 > ${O}_pytest_gpu_seed_forced.log; cat ${O}_pytest_gpu_seed_forced.log
 timeout 60 python -c "import __graft_entry__ as g; g.smoke()" > ${O}_smoke.log 2>&1; tail -1 ${O}_smoke.log
 timeout 300 python bench.py --impl reference --steps 5 --warmup 2 > ${O}_bench_ref.json 2> ${O}_bench_ref.err; echo "ref rc=$?"
 timeout 300 python bench.py > ${O}_bench_c3.json 2> ${O}_bench_c3.err; echo "bench rc=$?"

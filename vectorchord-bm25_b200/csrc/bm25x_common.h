@@ -88,7 +88,7 @@ struct bm25x_index {
     std::vector<uint32_t> h_df;        // host copy for query canonicalisation
     std::vector<uint8_t> h_keys;       // [n_terms*16] sorted keys (optional)
     cudaStream_t stream = nullptr;
-    cudaStream_t copy_stream = nullptr;  // bm25x_search_batch: result downloads of one slice while the next one runs (lazy)
+    cudaStream_t copy_stream = nullptr;  // bm25x_search_batch: result downloads of one slice while the next one runs
     uint32_t slice_min = 32768;          // bm25x_search_batch cuts batches of >= 2 x this many queries into slices (0: never)
     std::vector<void *> allocs;
     int prune = 1;                     // MaxScore-style pruning in the search kernels

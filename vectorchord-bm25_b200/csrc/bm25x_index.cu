@@ -457,6 +457,8 @@ static int index_begin(const BuildMeta &m, int device, bm25x_index **ixp) {
     }
     ix->sm_count = prop.multiProcessorCount;
     CU(cudaStreamCreateWithFlags(&ix->stream, cudaStreamNonBlocking));
+    // created with the handle, never later: concurrent first calls of bm25x_search_batch must not race to create it
+    CU(cudaStreamCreateWithFlags(&ix->copy_stream, cudaStreamNonBlocking));
     {   // keep freed batch buffers cached in the default pool (bm25x_batch_* allocate stream-ordered)
         cudaMemPool_t pool;
         if (cudaDeviceGetDefaultMemPool(&pool, device) == cudaSuccess) {
@@ -1028,6 +1030,7 @@ extern "C" int bm25x_index_alloc_replica(const bm25x_index_layout *like, int dev
     }
     ix->sm_count = prop.multiProcessorCount;
     CU(cudaStreamCreateWithFlags(&ix->stream, cudaStreamNonBlocking));
+    CU(cudaStreamCreateWithFlags(&ix->copy_stream, cudaStreamNonBlocking));  // as in index_begin
     {
         cudaMemPool_t pool;
         if (cudaDeviceGetDefaultMemPool(&pool, device) == cudaSuccess) {

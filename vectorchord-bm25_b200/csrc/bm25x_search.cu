@@ -538,7 +538,6 @@ static int search_batch_sliced(bm25x_index *ix, uint32_t nq, const uint32_t *q_o
                                uint16_t *out_payload, uint32_t *out_n, bm25x_search_stats *stats, uint32_t n_slices) {
     using clk = std::chrono::steady_clock;
     BM25X_CUDA_TRY(cudaSetDevice(ix->device));
-    if (!ix->copy_stream) BM25X_CUDA_TRY(cudaStreamCreateWithFlags(&ix->copy_stream, cudaStreamNonBlocking));
     std::vector<bm25x_batch *> bs(n_slices, nullptr);
     std::vector<cudaEvent_t> done(n_slices, nullptr);
     int rc = BM25X_OK;

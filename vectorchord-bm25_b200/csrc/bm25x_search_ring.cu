@@ -36,6 +36,19 @@ int launch_ring(int device, int sm_count, const SearchParams &sp_in, cudaStream_
 
 }  // namespace
 
+#if defined(BM25X_PHASE_PROF) && BM25X_RING_KP == 64
+// diagnostic builds only (tools/phase_profile.py): copies the phase profile of the seeded k <= 32 classes to `out`
+// (PP_SLOTS values: cycles per phase, then chunks, listed candidates, hits) and zeroes it when `reset` is set
+extern "C" int bm25x_phase_prof(unsigned long long *out, int reset) {
+    if (out) BM25X_CUDA_TRY(cudaMemcpyFromSymbol(out, g_phase_prof, sizeof(g_phase_prof)));
+    if (reset) {
+        static const unsigned long long zero[PP_SLOTS] = {};
+        BM25X_CUDA_TRY(cudaMemcpyToSymbol(g_phase_prof, zero, sizeof(zero)));
+    }
+    return PP_SLOTS;
+}
+#endif
+
 #define BM25X_RING_ENTRY2(kp) bm25x_launch_ring_kp##kp
 #define BM25X_RING_ENTRY(kp) BM25X_RING_ENTRY2(kp)
 

@@ -65,7 +65,9 @@ namespace {
 #define BM25X_RING_U 2
 #endif
 #ifndef BM25X_RING_MAXWARPS
-#define BM25X_RING_MAXWARPS 20  // 20 warps = 102 registers per thread (a few spills; C3 on H100: 16 warps slower, 24 no faster)
+#define BM25X_RING_MAXWARPS 20  // 20 warps = 96 registers per thread.  C3 on H100: 16 warps slower; a cap of 24 still
+                                // builds 20 warps of the seeded 3-term class (11 KiB per warp fit 20 times), and 24 real
+                                // warps of it (seeds in registers, 80 registers) were 12 % slower (DESIGN.md §7)
 #endif
 #ifndef BM25X_RING_INIT
 #define BM25X_RING_INIT 32
@@ -103,8 +105,8 @@ namespace {
 #define BM25X_RING_K2_SHIFT 0  // the second bit of a cell word comes from hash bits [SHIFT, SHIFT + 5)
 #endif
 #ifndef BM25X_RING_K2
-#define BM25X_RING_K2 1  // bit map only: TWO bits per document inside one 32-bit cell word (blocked Bloom filter, one
-                         // shared-memory atomicOr / one load as before): false alarms ~ (fill)^2 instead of fill
+#define BM25X_RING_K2 1  // bit map only: THREE bits per document inside one 32-bit cell word (blocked Bloom filter, one
+                         // shared-memory atomicOr / one load as before): false alarms ~ (fill)^3 instead of fill
 #endif
 #ifndef BM25X_SEED_INIT_FULL
 #define BM25X_SEED_INIT_FULL 1
@@ -194,6 +196,59 @@ struct RCfg {
                   "entry format: bit 15 = dense flavour (15-bit doc offset), else 5-bit run | 10-bit ring position");
     static_assert(ACC_DOCS >= 64, "accumulator too small");
 };
+
+// -DBM25X_PHASE_PROF (diagnostic build, tools/phase_profile.py): the seeded kernel sums the SM cycles each warp spends in
+// every phase of a chunk into g_phase_prof (attribution only: the clock reads cost issue slots and order the code
+// around them).  Lane i of a warp accumulates phase i, so the whole profile costs two registers.  Without the flag the
+// macros expand to nothing.
+enum : int {
+    PP_QUERY,    // query start (terms, seeds, first round) and end (final cut, result rows)
+    PP_WAIT,     // wait for the refill round (mbar_wait)
+    PP_SETUP,    // window limits, boundary searches, dense test
+    PP_CLEAR,    // presence map clear
+    PP_SEEDS,    // seed listing
+    PP_STREAM,   // stream trips (test + mark)
+    PP_COMPACT,  // compaction of the detected postings
+    PP_VSEARCH,  // verification: ring searches
+    PP_VLOAD,    // verification: wait for the posting-word loads
+    PP_VEXACT,   // verification: filter, exact re-score, pool insert
+    PP_END,      // chunk end, refill issue
+    PP_PHASES,
+    PP_CHUNKS = PP_PHASES,  // counters after the phases: chunks, listed candidates, hits (candidates whose words are loaded)
+    PP_CANDS,
+    PP_HITS,
+    PP_SLOTS
+};
+#ifdef BM25X_PHASE_PROF
+__device__ unsigned long long g_phase_prof[PP_SLOTS];
+#define PP_MARK(ph)                                                \
+    do {                                                           \
+        if constexpr (C::SEEDED) {                                 \
+            const uint32_t pp_now_ = (uint32_t)clock();            \
+            if (lane == (ph)) pp_acc += pp_now_ - pp_t;            \
+            pp_t = pp_now_;                                        \
+        }                                                          \
+    } while (0)
+#define PP_COUNT(slot, n)                                          \
+    do {                                                           \
+        if constexpr (C::SEEDED) {                                 \
+            const uint32_t pp_n_ = (n); /* every lane takes part */ \
+            if (lane == (slot)) pp_acc += pp_n_;                   \
+        }                                                          \
+    } while (0)
+// the clock is read after the loaded words are consumed, so that the wait lands in PP_VLOAD
+#define PP_CONSUME(a, b)                                                                      \
+    do {                                                                                      \
+        if constexpr (C::SEEDED) {                                                            \
+            uint32_t pp_x_;                                                                   \
+            asm volatile("xor.b32 %0, %1, %2;" : "=r"(pp_x_) : "r"(a), "r"(b));               \
+        }                                                                                     \
+    } while (0)
+#else
+#define PP_MARK(ph) do {} while (0)
+#define PP_COUNT(slot, n) do {} while (0)
+#define PP_CONSUME(a, b) do {} while (0)
+#endif
 
 // slot of a document in a map of `bytes` cells: multiplicative hash, then the high half of hash × bytes (any size)
 __device__ __forceinline__ uint32_t ring_slot(uint32_t doc, uint32_t bytes) { return __umulhi(doc * 0x9E3779B1u, bytes); }
@@ -309,6 +364,9 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
     const float s1min = p.s1f_min;
     uint32_t parity = 0;  // mbarrier phase parity
     uint32_t gen = 0;     // generation tag of the chunk (1..255), never reset: stale tags cost false alarms only
+#ifdef BM25X_PHASE_PROF
+    uint32_t pp_acc = 0u, pp_t = (uint32_t)clock();  // lane i: cycles of phase i (or counter i) of the current query
+#endif
 
     for (;;) {
         int qi = 0;
@@ -625,6 +683,7 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
 #ifdef BM25X_WATCHDOG
         uint32_t wd_chunks = 0;
 #endif
+        PP_MARK(PP_QUERY);
         for (;;) {
 #ifdef BM25X_WATCHDOG
             if (++wd_chunks > (1u << 26)) __trap();  // debug builds: a query that never ends becomes a launch failure
@@ -634,6 +693,8 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                 mbar_wait(bar, parity);
                 parity ^= 1u;
             }
+            PP_MARK(PP_WAIT);
+            PP_COUNT(PP_CHUNKS, 1u);
             // MaxScore (the reference's WAND pivot rule, search.rs:152-169, applied to whole terms): the terms with the
             // smallest score bounds leave the streamed set while the sum of their bounds (plus ub_oth) stays <= ALPHA · k-th
             // score.  A document holding only such terms cannot enter; for the others the bound is added back in the filter and
@@ -761,6 +822,7 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                     if (act) e = ring_lower_bound<C>(myring, rmask, rd, e, hi);
                 }
             }
+            PP_MARK(PP_SETUP);
             // ---- refill: append what earlier chunks consumed (at most half a ring per round) ----
             if (!C::SB) {
                 uint32_t n = 0;
@@ -780,6 +842,7 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                 // other runs — one search per pass instead of two in a row; the even lane of a pair carries the candidate.
                 const bool pairs = C::M == 3 && !C::ADAPT && !dense && m == 3u && ne_mask == 0u;
                 const uint32_t per_pass = pairs ? 16u : 32u;
+                PP_COUNT(PP_CANDS, nc);
                 for (uint32_t base = 0; base < nc; base += per_pass) {
                     const uint32_t ci = base + (pairs ? (uint32_t)lane >> 1 : (uint32_t)lane);
                     bool has = ci < nc;
@@ -863,10 +926,14 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                             const uint32_t hitx = __shfl_xor_sync(FULL, hit ? 1u : 0u, 1);  // (every lane takes part: no short circuit)
                             const bool anyhit = hit || hitx != 0u;
                             const bool live = has && (is_seed ? !anyhit : (anyhit || solo_j));  // (same in both lanes of a pair)
+                            PP_MARK(PP_VSEARCH);
+                            PP_COUNT(PP_HITS, __popc(__ballot_sync(FULL, live && !(lane & 1))));
                             uint32_t wo = 0u;
                             if (live && hit) wo = __ldg(&(p.post + pbo)[l].w);
                             if (live && !(lane & 1) && !is_seed) own.w = __ldg(&gown->w);
                             const uint32_t wx = __shfl_xor_sync(FULL, wo, 1);  // the partner's run
+                            PP_CONSUME(wx, own.w);
+                            PP_MARK(PP_VLOAD);
                             const uint32_t ox = (lane & 1) ? (j == 0u ? 1u : 0u) : (j == 2u ? 1u : 2u);
                             has = live && !(lane & 1);
 #pragma unroll
@@ -886,12 +953,17 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                                 }
                             }
                             const bool live = has && (is_seed ? !anyhit : (by_doc || anyhit || solo_j));
+                            PP_MARK(PP_VSEARCH);
+                            PP_COUNT(PP_HITS, __popc(__ballot_sync(FULL, live)));
 #pragma unroll
                             for (int i = 0; i < C::M; ++i) {
                                 const uint64_t pbi = __shfl_sync(FULL, pbase, i);
                                 if (live && lv[i] != INF) wv[i] = __ldg(&(p.post + pbi)[lv[i]].w);
                             }
                             if (live && !by_doc && !is_seed) own.w = __ldg(&gown->w);
+#pragma unroll
+                            for (int i = 0; i < C::M; ++i) PP_CONSUME(wv[i], own.w);
+                            PP_MARK(PP_VLOAD);
                             has = live;
                         }
 #pragma unroll
@@ -1064,6 +1136,7 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                         const bool lazy = C::KP > 128 && f.tv;
                         if (pn > C::KP - 32 || (!lazy && pn >= (int)k + 32)) pool_cut();
                     }
+                    PP_MARK(PP_VEXACT);
                 }
                 __syncwarp();  // every lane has read its entries before the producers refill the list
                 nc = 0;
@@ -1105,6 +1178,7 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                     for (int i = lane; i < (int)(C::MAP_BYTES / 16u); i += 32) ((uint4 *)map)[i] = make_uint4(0, 0, 0, 0);
                     __syncwarp();
                 }
+                PP_MARK(PP_CLEAR);
                 // wlim == ~0: no single-term posting of the run can pass → the loop variant without that test; the first
                 // non-empty run has nothing to test against, the last one nobody to mark for
                 myvariant = (!C::SEEDED && wlim != 0xFFFFFFFFu ? 4 : 0) | (multi && lane != __ffs(todo) - 1 ? 2 : 0) |
@@ -1182,10 +1256,20 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                                     const uint32_t slot = __umulhi(hsh, C::MAP_BYTES * 8u);
                                     uint32_t *cell = (uint32_t *)map + (slot >> 5);
 #if BM25X_RING_K2
-                                    // second bit: low 5 bits of the hash (the shift wraps: no mask, no pre-shift)
-                                    const uint32_t msk = (1u << (slot & 31u)) | __funnelshift_l(0u, 1u, BM25X_RING_K2_SHIFT ? hsh >> BM25X_RING_K2_SHIFT : hsh);
-                                    if (TEST) c = (*cell & msk) == msk;
-                                    if (MARK && valid) atomicOr(cell, msk);
+                                    // second bit: low 5 bits of the hash (the shift wraps: no mask, no pre-shift); third
+                                    // bit: the next 5 bits
+                                    const uint32_t msk = (1u << (slot & 31u)) |
+                                                         __funnelshift_l(0u, 1u, BM25X_RING_K2_SHIFT ? hsh >> BM25X_RING_K2_SHIFT : hsh) |
+                                                         __funnelshift_l(0u, 1u, hsh >> 5);
+                                    if (TEST && MARK) {
+                                        // one atomic tests and marks: the old word also holds this run's earlier marks,
+                                        // which can only add false alarms (the verification drops them), never hide a
+                                        // mark of an earlier run
+                                        c = (atomicOr(cell, valid ? msk : 0u) & msk) == msk;
+                                    } else {
+                                        if (TEST) c = (*cell & msk) == msk;
+                                        if (MARK && valid) atomicOr(cell, msk);
+                                    }
 #else
                                     if (TEST) c = (*cell >> (slot & 31u)) & 1u;
                                     if (MARK && valid) atomicOr(cell, 1u << (slot & 31u));
@@ -1205,6 +1289,7 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                     else body(std::true_type());
                     hm |= bits << (C::PL * t);
                 }
+                PP_MARK(PP_STREAM);
                 for (;;) {  // compaction: one listed posting per lane and round
                     const uint32_t bal = __ballot_sync(FULL, hm != 0u);
                     if (!bal) break;
@@ -1217,6 +1302,7 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                     }
                     nc += __popc(bal);
                 }
+                PP_MARK(PP_COMPACT);
             };
             // Producer loop: runs (or the accumulator scan) list candidates until the list wants to be verified or the
             // window is done; ONE verification site after it.
@@ -1248,6 +1334,7 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                         nc += __popc(bal);
                     }
                     seeds_pending = ss < (uint32_t)C::M * slices;
+                    PP_MARK(PP_SEEDS);
                 }
                 if (seeds_pending) {
                     __syncwarp();  // list full: verify, then go on with the seeds
@@ -1337,6 +1424,7 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                     }
                 }
             }
+            PP_MARK(PP_END);
         }
         // ---- Results::into_sorted_vec (search.rs:281) (after the last pass; between passes: a tidy pool and threshold) ----
         if (pn > 0 && !suspended) pool_cut();
@@ -1381,6 +1469,13 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
             for (int o = 16; o > 0; o >>= 1) fetched += __shfl_xor_sync(FULL, fetched, o);
             if (lane == 0) atomicAdd(p.fetched, fetched);
         }
+#ifdef BM25X_PHASE_PROF
+        PP_MARK(PP_QUERY);
+        if constexpr (C::SEEDED) {
+            if (lane < PP_SLOTS) atomicAdd(&g_phase_prof[lane], (unsigned long long)pp_acc);
+            pp_acc = 0u;
+        }
+#endif
         __syncwarp();
     }
 }

@@ -13,9 +13,10 @@
 //             in HBM; each lane binary-searches hi in its run → exact in-window range [rd, e), nothing scanned twice.
 //   union     runs are processed in ascending order; run j first TESTS each of its documents against a presence map
 //             that holds the marks of runs < j, then MARKS it.  The map is a blocked Bloom filter: a document sets /
-//             tests two bits of one 32-bit word (one multiplicative hash; one shared-memory load, one atomicOr), cleared
-//             per window.  A document held by two runs is therefore always detected by the later run's posting (no
-//             false negatives); false alarms (both bits set by other documents) are below one per cent.
+//             tests three bits of one 32-bit word (one multiplicative hash; word and bits by shifts of it; a run that
+//             tests and marks does both with one atomicOr), cleared per window.  A document held by two runs is
+//             therefore always detected by the later run's posting (no false negatives); false alarms (all three bits
+//             set by other documents) are about 6 per 1 440-posting chunk of the seeded kernel on C3 (DESIGN.md §4.1).
 //   single    a document held by one run only can enter the top-k only if its term frequency passes the threshold:
 //             one integer compare per posting (w > wlim_j, wlim_j from the exact threshold solved for tf), plus the
 //             tie shortcut (same (run, tf, fieldnorm) signature as the k-th entry ⇒ identical score ⇒ rejected
@@ -253,6 +254,30 @@ __device__ unsigned long long g_phase_prof[PP_SLOTS];
 // slot of a document in a map of `bytes` cells: multiplicative hash, then the high half of hash × bytes (any size)
 __device__ __forceinline__ uint32_t ring_slot(uint32_t doc, uint32_t bytes) { return __umulhi(doc * 0x9E3779B1u, bytes); }
 
+// Bit map (BM25X_RING_BITMAP): the 32-bit cell word of a document (its word index) and the bits it sets / tests there.
+// Slot = high half of hash × cells; for a power-of-two map that is a plain shift of the hash (the same bits, one
+// instruction instead of IMAD.HI + mask).  The bit shifts wrap (SHF.L.W): 1 << x takes x's low 5 bits, no mask needed.
+template <class C>
+__device__ __forceinline__ uint32_t map_word(uint32_t doc, uint32_t &msk) {
+    constexpr uint32_t CELLS = C::MAP_BYTES * 8u;
+    constexpr int LOG_CELLS = 31 - __builtin_clz(CELLS);
+    const uint32_t hsh = doc * 0x9E3779B1u;
+    uint32_t slot, word;
+    if constexpr ((CELLS & (CELLS - 1u)) == 0u) {
+        slot = hsh >> (32 - LOG_CELLS);
+        // (a shift the compiler cannot merge with the caller's ×4 into shift + mask + add: one IMAD forms the address)
+        asm("shr.b32 %0, %1, %2;" : "=r"(word) : "r"(hsh), "n"(32 - LOG_CELLS + 5));
+    } else {
+        slot = __umulhi(hsh, CELLS);
+        word = slot >> 5;
+    }
+    msk = __funnelshift_l(0u, 1u, slot);
+#if BM25X_RING_K2
+    // second bit: low 5 bits of the hash (or from bit BM25X_RING_K2_SHIFT); third bit: the next 5 bits
+    msk |= __funnelshift_l(0u, 1u, BM25X_RING_K2_SHIFT ? hsh >> BM25X_RING_K2_SHIFT : hsh) | __funnelshift_l(0u, 1u, hsh >> 5);
+#endif
+    return word;
+}
 // lower_bound of `doc` in ring positions [a, e) (posting indices of the term; the ring holds index i at i & RM).
 // Fixed LOG_R + 1 power-of-two steps, no data-dependent branch: every lane of a verification pass searches the same run,
 // and independent searches interleave (the while-loop form costs several times the instructions per search).
@@ -1162,7 +1187,7 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
             // sparse window: runs in ascending order; each run tests its documents against the marks of the earlier runs,
             // then marks them.  dense window: scores summed in an f32 accumulator indexed by doc - lo (in the map's
             // memory; docs are distinct inside a run: plain read-modify-write, __syncwarp between runs), then scanned.
-            uint32_t todo = 0u, ra = 0u, ree = 0u, rnj = 0u, wl = 0u, tw = 0u, tdk = 0u, pb = 0u, genv = 0u, dbase = 0u, rm = 1u;
+            uint32_t todo = 0u, ra = 0u, ree = 0u, wl = 0u, tw = 0u, tdk = 0u, pb = 0u, genv = 0u, dbase = 0u, rm = 1u;
             int rj = -1, variant = 0;
             uint32_t ss = sub == 0u ? 0u : 0xFFFFFFFFu;  // seeded launches: next slice (term, 32 slots) of the seed table to look at in this window
             bool multi = false;
@@ -1235,7 +1260,22 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                     }
                     uint32_t bits = 0u;
                     auto body = [&](auto check_c) {
-                        constexpr bool CHECK = decltype(check_c)::value;  // trips at the ends of the range test validity
+                        // trips at the ends of the range: which of the lane's posting slots lie in [ra, ree), once per lane
+                        // and trip; the others neither mark nor test (a mark from outside the window would add false
+                        // alarms, a hit there would list a posting of another window)
+                        constexpr bool CHECK = decltype(check_c)::value;
+                        uint32_t vm = 0xFFFFFFFFu;
+                        if constexpr (CHECK) {
+                            vm = 0u;
+#pragma unroll
+                            for (int u = 0; u < C::U; ++u) {
+                                // slots below ra: at most E - 1 (a run's first trip starts at ra & ~(E - 1)); slots from
+                                // ree on: any number
+                                constexpr uint32_t ALL = (1u << C::E) - 1u;
+                                const int below = max((int)(ra - ix[u]), 0), beyond = max((int)(ix[u] + C::E - ree), 0);
+                                vm |= ((ALL << below) & (ALL >> min(beyond, C::E))) << (C::E * u);
+                            }
+                        }
 #pragma unroll
                         for (int u = 0; u < C::U; ++u) {
 #pragma unroll
@@ -1248,32 +1288,28 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                                     doc = h ? q[u].z : q[u].x;
                                     w = h ? q[u].w : q[u].y;
                                 }
-                                const bool valid = !CHECK || ix[u] + h - ra < rnj;  // unsigned: also false below ra
+                                const bool valid = (vm >> (C::E * u + h)) & 1u;
                                 bool c = false;
                                 if (TEST || MARK) {
 #if BM25X_RING_BITMAP
-                                    const uint32_t hsh = doc * 0x9E3779B1u;
-                                    const uint32_t slot = __umulhi(hsh, C::MAP_BYTES * 8u);
-                                    uint32_t *cell = (uint32_t *)map + (slot >> 5);
-#if BM25X_RING_K2
-                                    // second bit: low 5 bits of the hash (the shift wraps: no mask, no pre-shift); third
-                                    // bit: the next 5 bits
-                                    const uint32_t msk = (1u << (slot & 31u)) |
-                                                         __funnelshift_l(0u, 1u, BM25X_RING_K2_SHIFT ? hsh >> BM25X_RING_K2_SHIFT : hsh) |
-                                                         __funnelshift_l(0u, 1u, hsh >> 5);
+                                    uint32_t msk;
+                                    uint32_t *cell = (uint32_t *)map + map_word<C>(doc, msk);
+                                    // an invalid slot ORs nothing in (an atomic with an empty mask: no branch around it)
+                                    // and its test is masked off below; the word is in the map whatever the slot holds
+                                    const uint32_t mark = CHECK && !valid ? 0u : msk;
+                                    uint32_t old = 0u;
                                     if (TEST && MARK) {
                                         // one atomic tests and marks: the old word also holds this run's earlier marks,
                                         // which can only add false alarms (the verification drops them), never hide a
                                         // mark of an earlier run
-                                        c = (atomicOr(cell, valid ? msk : 0u) & msk) == msk;
+                                        old = atomicOr(cell, mark);
                                     } else {
-                                        if (TEST) c = (*cell & msk) == msk;
-                                        if (MARK && valid) atomicOr(cell, msk);
+                                        if (TEST) old = *cell;
+                                        if (MARK) atomicOr(cell, mark);
                                     }
-#else
-                                    if (TEST) c = (*cell >> (slot & 31u)) & 1u;
-                                    if (MARK && valid) atomicOr(cell, 1u << (slot & 31u));
-#endif
+                                    // hit: every bit of msk was set already (one LOP3 sets the predicate, one predicated
+                                    // add records it)
+                                    if (TEST) c = (msk & ~old) == 0u;
 #else
                                     const uint32_t slot = ring_slot(doc, C::MAP_BYTES);
                                     if (TEST) c = map[slot] == genv;
@@ -1281,24 +1317,27 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
 #endif
                                 }
                                 if (SOLO) c = c | ((w > wl) & !((w == tw) & (doc > tdk)));  // bitwise: no branches
-                                bits |= (uint32_t)(valid & c) << (C::E * u + h);
+                                if (c) bits += 1u << (C::E * u + h);
                             }
                         }
+                        if constexpr (CHECK) bits &= vm;
                     };
                     if (pb >= ra && pb + C::TRIP <= ree) body(std::false_type());
                     else body(std::true_type());
                     hm |= bits << (C::PL * t);
                 }
                 PP_MARK(PP_STREAM);
-                for (;;) {  // compaction: one listed posting per lane and round
+                // compaction: one listed posting per lane and round.  Bit b = PL·t + E·u + h of hm is posting
+                // pb0 + t·TRIP + E·(lane + 32·u) + h = pb0 + E·lane + 32·(b & ~(E - 1)) + (b & (E - 1)).
+                const uint32_t lane0 = pb0 + (uint32_t)C::E * (uint32_t)lane, rtag = (uint32_t)rj << 10;
+                for (;;) {
                     const uint32_t bal = __ballot_sync(FULL, hm != 0u);
                     if (!bal) break;
                     if (hm) {
-                        const uint32_t bpos = (uint32_t)__ffs(hm) - 1u;
+                        const uint32_t b = (uint32_t)__ffs(hm) - 1u;
                         hm &= hm - 1u;
-                        const uint32_t t = bpos / C::PL, sl = bpos % C::PL;
-                        const uint32_t idx = pb0 + t * C::TRIP + (uint32_t)C::E * (uint32_t)(lane + 32 * (sl / C::E)) + (sl % C::E);
-                        cand[nc + __popc(bal & lt_mask)] = (uint16_t)(((uint32_t)rj << 10) | (idx & rm));
+                        const uint32_t idx = lane0 + b + 31u * (b & ~((uint32_t)C::E - 1u));
+                        cand[nc + __popc(bal & lt_mask)] = (uint16_t)((idx & rm) | rtag);
                     }
                     nc += __popc(bal);
                 }
@@ -1353,7 +1392,6 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                             wl = __shfl_sync(FULL, wlim, rj);
                             tw = __shfl_sync(FULL, tiew, rj);
                             variant = __shfl_sync(FULL, myvariant, rj);
-                            rnj = ree - ra;
                             rg = (const uint4 *)(rings + ring_base(rj));
                             if constexpr (C::DOCRING) gq = (const uint4 *)(p.post + __shfl_sync(FULL, pbase, rj));
                             rm = ring_mask(rj);

@@ -234,6 +234,44 @@ int bm25x_merge_topk(uint32_t nq, uint32_t k, const uint32_t *doc_a, const float
                      const double *score64_b, const uint16_t *payload_b, const uint32_t *n_b, uint32_t doc_base_b,
                      uint32_t *out_doc, float *out_score, double *out_score64, uint16_t *out_payload, uint32_t *out_n);
 
+/* ---- document-sharded index: one sealed segment split by document range over one or more GPUs, so that its postings
+ * need not fit in one GPU's HBM.  Every shard scores with the WHOLE segment's statistics (N, avgdl, df), so its top-k is
+ * the whole index's ranking restricted to its documents; the shards' lists are merged on shard 0's device
+ * (k_merge_shards).  Results are bit-identical to bm25x_search_batch on an index created from the same corpus.  The
+ * shard handles stay internal: their df and N are not the segment's. */
+#define BM25X_MAX_SHARDS 16
+typedef struct bm25x_sharded_index bm25x_sharded_index;
+/* `whole` exactly as for bm25x_index_create.  doc_bounds[n_shards+1]: shard s holds the documents
+ * [doc_bounds[s], doc_bounds[s+1]), strictly ascending, doc_bounds[0] = 0, doc_bounds[n_shards] = n_docs; NULL = balanced
+ * by postings: b_s (0 < s < S) is the smallest d > b_{s-1} with Σ_{d' < d} c_{d'} >= ceil(s·P/S), c_d = distinct terms of
+ * document d, clamped so that every shard keeps at least one document.  devices[n_shards], or NULL = all on device 0; one
+ * device may hold several shards.  The shards are built one after the other (host memory beyond `whole`: one shard's
+ * CSR). */
+int bm25x_sharded_create(const bm25x_corpus *whole, uint32_t n_shards, const uint32_t *doc_bounds, const int *devices,
+                         bm25x_sharded_index **out);
+void bm25x_sharded_destroy(bm25x_sharded_index *sx);
+/* info as the unsharded index would report it (n_docs, n_terms, n_postings, sum_doc_len, avgdl, k1, b); device_bytes
+ * and n_blocks summed over the shards; device = shard 0's.  doc_bounds_out[n_shards+1] or NULL. */
+int bm25x_sharded_get_info(const bm25x_sharded_index *sx, bm25x_index_info *out, uint32_t *n_shards_out,
+                           uint32_t *doc_bounds_out);
+int bm25x_sharded_set_option(bm25x_sharded_index *sx, const char *name, int64_t value); /* every shard */
+int bm25x_sharded_lookup_terms(const bm25x_sharded_index *sx, const uint8_t *keys, uint32_t n, uint32_t *ordinals_out);
+/* Same contract, arguments and outputs as bm25x_search_batch on an index created from `whole`: global doc ids, `allow`
+ * over global ids, the same status codes and messages.  The shards run concurrently (one device each, or side by side
+ * on a shared one).  stats: queries = live queries of the whole index; postings, postings_fetched, launches, bytes_algo
+ * and kernel_ms are SUMS over the shards plus the merge launch — kernel_ms is summed device time, not wall time;
+ * h2d_ms = canonicalise + upload of all shards, d2h_ms = merge wait + download. */
+int bm25x_sharded_search_batch(bm25x_sharded_index *sx, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms,
+                               uint32_t k, const uint8_t *allow, uint32_t *out_doc, float *out_score, double *out_score64,
+                               uint16_t *out_payload, uint32_t *out_n, bm25x_search_stats *stats);
+/* Test / measurement hook: k_merge_shards on host rows.  Shard s's rows are doc/score/score64/payload + s·nq·k
+ * (payload: ·3) and n + s·nq, local doc ids, each row in canonical order; global id = local + doc_base[s], doc_base
+ * ascending with s.  Outputs as bm25x_search_batch; merge_ms (or NULL) = the kernel's device time. */
+int bm25x_merge_shards(int device, uint32_t n_shards, uint32_t nq, uint32_t k, const uint32_t *doc_base,
+                       const uint32_t *doc, const float *score, const double *score64, const uint16_t *payload,
+                       const uint32_t *n, uint32_t *out_doc, float *out_score, double *out_score64,
+                       uint16_t *out_payload, uint32_t *out_n, float *merge_ms);
+
 /* Invariants of the reference's vector types (crates/bm25/src/vector.rs:46-134): n vectors in CSR form, keys strictly
  * ascending inside a vector, term frequencies (tfs, NULL for Query-like vectors) non-zero — what Document::new / Query::new
  * enforce with expect("invalid data").  BM25X_ERR_INVALID names the first offending vector.  Host only. */

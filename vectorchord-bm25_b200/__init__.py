@@ -6,8 +6,9 @@ host-side interface for the path (`bm25::search` / `bm25::evaluate`, Document / 
 falls back to a CPU implementation: if the library or an H100 is missing, calls raise.
 """
 from .bm25x import (Bm25xError, Index, Batch, SearchStats, IndexLayout, synth_corpus, synth_queries, load_library, build_library,
-                    device_count, Document, Query, MAX_K, MAX_QUERY_TERMS, TERM_MISSING, merge_topk, check_vectors, Broker)
+                    device_count, Document, Query, MAX_K, MAX_QUERY_TERMS, TERM_MISSING, merge_topk, check_vectors, Broker,
+                    ShardedIndex, MAX_SHARDS, merge_shards)
 
 __all__ = ["Bm25xError", "Index", "Batch", "SearchStats", "IndexLayout", "synth_corpus", "synth_queries", "load_library",
            "build_library", "device_count", "Document", "Query", "MAX_K", "MAX_QUERY_TERMS", "TERM_MISSING", "merge_topk",
-           "check_vectors", "Broker"]
+           "check_vectors", "Broker", "ShardedIndex", "MAX_SHARDS", "merge_shards"]

@@ -153,6 +153,16 @@ def load_library():
     L.bm25x_broker_get_stats.argtypes = [vp, C.POINTER(BrokerStats)]
     L.bm25x_broker_destroy.argtypes = [vp]
     L.bm25x_broker_destroy.restype = None
+    L.bm25x_sharded_create.argtypes = [C.POINTER(_Corpus), C.c_uint32, u32p, C.POINTER(C.c_int), C.POINTER(vp)]
+    L.bm25x_sharded_destroy.argtypes = [vp]
+    L.bm25x_sharded_destroy.restype = None
+    L.bm25x_sharded_get_info.argtypes = [vp, C.POINTER(IndexInfo), u32p, u32p]
+    L.bm25x_sharded_set_option.argtypes = [vp, C.c_char_p, C.c_int64]
+    L.bm25x_sharded_lookup_terms.argtypes = [vp, u8p, C.c_uint32, u32p]
+    L.bm25x_sharded_search_batch.argtypes = [vp, C.c_uint32, u32p, u32p, C.c_uint32, u8p, u32p, f32p, f64p, u16p, u32p,
+                                             C.POINTER(SearchStats)]
+    L.bm25x_merge_shards.argtypes = [C.c_int, C.c_uint32, C.c_uint32, C.c_uint32, u32p, u32p, f32p, f64p, u16p, u32p,
+                                     u32p, f32p, f64p, u16p, u32p, f32p]
     L.bm25x_last_error.restype = C.c_char_p
     L.bm25x_device_count.restype = C.c_int
     _lib = L
@@ -510,6 +520,113 @@ def merge_topk(a, b, doc_base_b, k):
                                            _p(out["score64"], C.c_double), _p(out["payload"], C.c_uint16),
                                            _p(out["n"], C.c_uint32)))
     return out
+
+
+MAX_SHARDS = 16
+
+
+def _result_arrays(nq, k, want_f64, want_payload):
+    return {"doc": np.empty((nq, k), np.uint32), "score": np.empty((nq, k), np.float32),
+            "score64": np.empty((nq, k), np.float64) if want_f64 else None,
+            "payload": np.empty((nq, k, 3), np.uint16) if want_payload else None, "n": np.empty(nq, np.uint32)}
+
+
+class ShardedIndex:
+    """One sealed segment split by document range into `n_shards` indexes (bm25x_sharded_*), on one GPU or several, so
+    that it need not fit in one GPU's HBM.  Searches return exactly what Index.search_batch returns on the unsharded index
+    built from the same corpus: global doc ids, `allow` over global ids."""
+
+    def __init__(self, n_docs, doc_len, n_terms, post_off, post_doc, post_tf, k1=1.2, b=0.75, payload=None,
+                 term_keys=None, n_shards=2, doc_bounds=None, devices=None):
+        L = load_library()
+        keep = [np.ascontiguousarray(doc_len, dtype=np.uint32), np.ascontiguousarray(post_off, dtype=np.uint64),
+                np.ascontiguousarray(post_doc, dtype=np.uint32), np.ascontiguousarray(post_tf, dtype=np.uint32)]
+        c = _Corpus()
+        c.n_docs, c.n_terms, c.k1, c.b = int(n_docs), int(n_terms), float(k1), float(b)
+        c.doc_len, c.post_off = _p(keep[0], C.c_uint32), _p(keep[1], C.c_uint64)
+        c.post_doc, c.post_tf = _p(keep[2], C.c_uint32), _p(keep[3], C.c_uint32)
+        if payload is not None:
+            keep.append(np.ascontiguousarray(payload, dtype=np.uint16))
+            c.payload = _p(keep[-1], C.c_uint16)
+        if term_keys is not None:
+            keep.append(np.ascontiguousarray(term_keys, dtype=np.uint8))
+            c.term_key = _p(keep[-1], C.c_uint8)
+        bounds = np.ascontiguousarray(doc_bounds, dtype=np.uint32) if doc_bounds is not None else None
+        devs = (C.c_int * int(n_shards))(*[int(d) for d in devices]) if devices is not None else None
+        self.h = C.c_void_p()
+        _check(L.bm25x_sharded_create(C.byref(c), int(n_shards), _p(bounds, C.c_uint32), devs, C.byref(self.h)))
+        self.n_docs, self.n_terms = int(n_docs), int(n_terms)
+
+    @staticmethod
+    def from_corpus(c, n_shards=2, doc_bounds=None, devices=None, **kw):
+        return ShardedIndex(c.n_docs, c.doc_len, c.n_terms, c.post_off, c.post_doc, c.post_tf, getattr(c, "k1", 1.2),
+                            getattr(c, "b", 0.75), n_shards=n_shards, doc_bounds=doc_bounds, devices=devices, **kw)
+
+    def close(self):
+        if getattr(self, "h", None):
+            load_library().bm25x_sharded_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def info(self) -> IndexInfo:
+        out = IndexInfo()
+        _check(load_library().bm25x_sharded_get_info(self.h, C.byref(out), None, None))
+        return out
+
+    def doc_bounds(self):
+        n = C.c_uint32(0)
+        _check(load_library().bm25x_sharded_get_info(self.h, C.byref(IndexInfo()), C.byref(n), None))
+        out = np.zeros(n.value + 1, np.uint32)
+        _check(load_library().bm25x_sharded_get_info(self.h, C.byref(IndexInfo()), None, _p(out, C.c_uint32)))
+        return out
+
+    def set_option(self, name: str, value: int):
+        _check(load_library().bm25x_sharded_set_option(self.h, name.encode(), int(value)))
+
+    def lookup_terms(self, keys):
+        keys = np.ascontiguousarray(keys, dtype=np.uint8).reshape(-1, 16)
+        out = np.zeros(len(keys), dtype=np.uint32)
+        _check(load_library().bm25x_sharded_lookup_terms(self.h, _p(keys, C.c_uint8), len(keys), _p(out, C.c_uint32)))
+        return out
+
+    def search_batch(self, q_off, q_terms, k, allow=None, want_f64=True, want_payload=False, out=None):
+        q_off = np.ascontiguousarray(q_off, dtype=np.uint32)
+        q_terms = np.ascontiguousarray(q_terms, dtype=np.uint32)
+        nq = len(q_off) - 1
+        if out is None:
+            out = _result_arrays(nq, max(int(k), 1), want_f64, want_payload)
+        al = np.ascontiguousarray(allow, dtype=np.uint8) if allow is not None else None
+        st = SearchStats()
+        _check(load_library().bm25x_sharded_search_batch(self.h, nq, _p(q_off, C.c_uint32), _p(q_terms, C.c_uint32),
+                                                         int(k), _p(al, C.c_uint8), _p(out["doc"], C.c_uint32),
+                                                         _p(out["score"], C.c_float), _p(out["score64"], C.c_double),
+                                                         _p(out["payload"], C.c_uint16), _p(out["n"], C.c_uint32),
+                                                         C.byref(st)))
+        out["stats"] = st
+        return out
+
+
+def merge_shards(rows, doc_base, k, device=0):
+    """bm25x_merge_shards: the device merge alone on host rows.  rows = list of S result dicts (doc, score, score64,
+    payload [nq, k(, 3)] with local ids, n [nq]); returns the merged dict and the kernel's time in ms."""
+    S, nq = len(rows), len(rows[0]["n"])
+    cat = lambda key, dt: np.ascontiguousarray(np.stack([r[key] for r in rows]), dtype=dt)
+    doc, sc, s64, pay, n = (cat("doc", np.uint32), cat("score", np.float32), cat("score64", np.float64),
+                            cat("payload", np.uint16), cat("n", np.uint32))
+    base = np.ascontiguousarray(doc_base, dtype=np.uint32)
+    out = _result_arrays(nq, int(k), True, True)
+    ms = C.c_float(0.0)
+    _check(load_library().bm25x_merge_shards(int(device), S, nq, int(k), _p(base, C.c_uint32), _p(doc, C.c_uint32),
+                                             _p(sc, C.c_float), _p(s64, C.c_double), _p(pay, C.c_uint16),
+                                             _p(n, C.c_uint32), _p(out["doc"], C.c_uint32), _p(out["score"], C.c_float),
+                                             _p(out["score64"], C.c_double), _p(out["payload"], C.c_uint16),
+                                             _p(out["n"], C.c_uint32), C.byref(ms)))
+    return out, ms.value
 
 
 class Batch:

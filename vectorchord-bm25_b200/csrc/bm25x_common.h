@@ -109,3 +109,22 @@ struct bm25x_index {
     uint32_t *eval_fn_len = nullptr;
     std::mutex eval_mutex;
 };
+
+// Document-sharded index (bm25x_sharded_*): shard s is an ordinary index over the documents [bounds[s], bounds[s+1]) with
+// local ids, built with the whole segment's statistics (BuildMeta.stat_*), so it scores with the same s0 / s1 bits.
+struct bm25x_sharded_index {
+    uint32_t n_shards = 0;
+    std::vector<uint32_t> bounds;        // [n_shards+1]
+    std::vector<bm25x_index *> shards;   // [n_shards]
+    // the whole segment, as bm25x_index_get_info / query canonicalisation see it
+    uint32_t n_docs = 0, n_terms = 0;
+    uint64_t n_post = 0, sum_len = 0;
+    double k1 = 1.2, b = 0.75, avgdl = 0;
+    std::vector<uint32_t> h_df;
+};
+
+// Internal, for bm25x_sharded_search_batch (bm25x_search.cu): a run of a prepared batch on its index's stream between the
+// batch's timing events, without synchronising; after it has finished, its figures added to *acc.
+int bm25x_batch_run_timed(bm25x_batch *b);
+int bm25x_batch_add_stats(bm25x_batch *b, bm25x_search_stats *acc);
+cudaEvent_t bm25x_batch_done_event(bm25x_batch *b);

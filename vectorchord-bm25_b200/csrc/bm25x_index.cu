@@ -392,6 +392,8 @@ struct BuildMeta {
     const uint32_t *stat_df = nullptr;  // [n_terms] sealed TokenTuple.number_of_documents
     uint32_t stat_n_docs = 0;           // sealed JumpTuple.number_of_documents
     double stat_avgdl = 0.0;            // sealed sum_of_document_lengths / number_of_documents
+    // document shard (bm25x_sharded_create): global id of local document 0, for the synthesised ctid payload
+    uint32_t doc_base = 0;
 };
 
 static int check_common(const char *who, uint32_t n_docs, const void *doc_len, double k1, double b, int device) {
@@ -557,10 +559,11 @@ static int index_begin(const BuildMeta &m, int device, bm25x_index **ixp) {
     } else {
         std::vector<uint16_t> pl((size_t)N * 3);
         for (uint32_t i = 0; i < N; i++) {  // synthetic ctid: (block hi, block lo, offset) of a 291-tuple page
-            uint32_t blkno = i / 291;
+            const uint32_t g = m.doc_base + i;  // of the segment's doc id (a shard's local ids start at doc_base)
+            uint32_t blkno = g / 291;
             pl[(size_t)i * 3 + 0] = (uint16_t)(blkno >> 16);
             pl[(size_t)i * 3 + 1] = (uint16_t)(blkno & 0xFFFF);
-            pl[(size_t)i * 3 + 2] = (uint16_t)(i % 291 + 1);
+            pl[(size_t)i * 3 + 2] = (uint16_t)(g % 291 + 1);
         }
         CU(cudaMemcpy(d.payload, pl.data(), sizeof(uint16_t) * pl.size(), cudaMemcpyHostToDevice));
     }
@@ -637,18 +640,16 @@ static int upload_csr(bm25x_index *ix, const char *who, uint32_t T, uint64_t P, 
     return BM25X_OK;
 }
 
-extern "C" int bm25x_index_create(const bm25x_corpus *c, int device, bm25x_index **out) {
-    if (!c || !out) {
-        bm25x_set_error("bm25x_index_create: null argument");
-        return BM25X_ERR_INVALID;
-    }
-    *out = nullptr;
+// Host validation of a term-major CSR corpus, shared by bm25x_index_create and bm25x_sharded_create: same codes, same
+// messages.  check_device == false leaves the device check to the caller (bm25x_sharded_create checks its shard
+// arguments first, so that they are refused without a GPU).
+static int validate_corpus(const bm25x_corpus *c, int device, bool check_device) {
     if (!c->post_off || (c->post_off[c->n_terms] && (!c->post_doc || !c->post_tf))) {
         bm25x_set_error("bm25x_index_create: empty or malformed corpus");
         return BM25X_ERR_INVALID;
     }
     int rc = check_common("bm25x_index_create", c->n_docs, c->doc_len, c->k1, c->b, device);
-    if (rc != BM25X_OK) return rc;
+    if (rc != BM25X_OK && (check_device || rc != BM25X_ERR_CUDA)) return rc;
     const uint32_t N = c->n_docs, T = c->n_terms;
     const uint64_t P = c->post_off[T];
 
@@ -678,8 +679,19 @@ extern "C" int bm25x_index_create(const bm25x_corpus *c, int device, bm25x_index
         bm25x_set_error("bm25x_index_create: term frequency >= 2^24 is not supported by the packed posting layout");
         return BM25X_ERR_UNSUPPORTED;
     }
-    rc = check_keys("bm25x_index_create", c->term_key, T);
+    return check_keys("bm25x_index_create", c->term_key, T);
+}
+
+extern "C" int bm25x_index_create(const bm25x_corpus *c, int device, bm25x_index **out) {
+    if (!c || !out) {
+        bm25x_set_error("bm25x_index_create: null argument");
+        return BM25X_ERR_INVALID;
+    }
+    *out = nullptr;
+    int rc = validate_corpus(c, device, true);
     if (rc != BM25X_OK) return rc;
+    const uint32_t N = c->n_docs, T = c->n_terms;
+    const uint64_t P = c->post_off[T];
 
     std::vector<uint32_t> df(T);
     for (uint32_t t = 0; t < T; t++) df[t] = (uint32_t)(c->post_off[t + 1] - c->post_off[t]);
@@ -691,6 +703,131 @@ extern "C" int bm25x_index_create(const bm25x_corpus *c, int device, bm25x_index
     rc = upload_csr(ix, "bm25x_index_create", T, P, c->post_off, c->post_doc, c->post_tf);
     if (rc != BM25X_OK) return rc;
     *out = ix;
+    return BM25X_OK;
+}
+
+// ---- document-sharded index (DESIGN §4.7): one segment split by document range, each shard an index with local doc ids
+// that scores with the whole segment's statistics ----
+extern "C" void bm25x_sharded_destroy(bm25x_sharded_index *sx) {
+    if (!sx) return;
+    for (bm25x_index *ix : sx->shards) bm25x_index_destroy(ix);
+    delete sx;
+}
+
+extern "C" int bm25x_sharded_create(const bm25x_corpus *c, uint32_t S, const uint32_t *doc_bounds, const int *devices,
+                                    bm25x_sharded_index **out) {
+    const char *who = "bm25x_sharded_create";
+    if (!c || !out) {
+        bm25x_set_error("%s: null argument", who);
+        return BM25X_ERR_INVALID;
+    }
+    *out = nullptr;
+    // every host check before any device is used: the corpus exactly as bm25x_index_create checks it, then the shards
+    int rc = validate_corpus(c, 0, false);
+    if (rc != BM25X_OK) return rc;
+    const uint32_t N = c->n_docs, T = c->n_terms;
+    const uint64_t P = c->post_off[T];
+    if (S == 0 || S > BM25X_MAX_SHARDS) {
+        bm25x_set_error("%s: n_shards=%u must be 1..%d", who, S, BM25X_MAX_SHARDS);
+        return BM25X_ERR_INVALID;
+    }
+    if (N < S) {
+        bm25x_set_error("%s: n_docs=%u < n_shards=%u (every shard holds at least one document)", who, N, S);
+        return BM25X_ERR_INVALID;
+    }
+    std::vector<uint32_t> bounds((size_t)S + 1);
+    if (doc_bounds) {
+        bool ok = doc_bounds[0] == 0 && doc_bounds[S] == N;
+        for (uint32_t s = 0; s < S && ok; s++) ok = doc_bounds[s] < doc_bounds[s + 1];
+        if (!ok) {
+            bm25x_set_error("%s: doc_bounds must ascend strictly from 0 to n_docs=%u", who, N);
+            return BM25X_ERR_INVALID;
+        }
+        std::copy(doc_bounds, doc_bounds + S + 1, bounds.begin());
+    } else {
+        // balanced by postings: c_d = distinct terms of document d = its postings; b_s = smallest d > b_{s-1} with
+        // Σ_{d' < d} c_{d'} >= ceil(s·P/S), clamped so that the shards s..S-1 keep one document each
+        std::vector<uint64_t> cum((size_t)N + 1, 0);
+#pragma omp parallel for schedule(static) num_threads(bm25x_host_threads(0))
+        for (uint64_t p = 0; p < P; p++) {
+#pragma omp atomic
+            cum[(size_t)c->post_doc[p] + 1]++;
+        }
+        for (uint32_t d = 0; d < N; d++) cum[(size_t)d + 1] += cum[d];
+        bounds[0] = 0;
+        for (uint32_t s = 1; s < S; s++) {
+            const uint64_t target = ((uint64_t)s * P + S - 1) / S;
+            // smallest d > b_{s-1} with cum[d] >= target (cum ascends; cum[N] = P >= target)
+            uint32_t d = (uint32_t)(std::lower_bound(cum.begin() + bounds[s - 1] + 1, cum.end(), target) - cum.begin());
+            bounds[s] = std::min<uint32_t>(d, N - (S - s));
+        }
+        bounds[S] = N;
+    }
+    std::vector<int> dev(S, 0);
+    if (devices) std::copy(devices, devices + S, dev.begin());
+    for (uint32_t s = 0; s < S; s++) {
+        rc = check_common(who, N, c->doc_len, c->k1, c->b, dev[s]);
+        if (rc != BM25X_OK) return rc;
+    }
+
+    bm25x_sharded_index *sx = new bm25x_sharded_index();
+    sx->n_shards = S;
+    sx->bounds = bounds;
+    sx->n_docs = N;
+    sx->n_terms = T;
+    sx->n_post = P;
+    sx->k1 = c->k1;
+    sx->b = c->b;
+    sx->h_df.resize(T);
+    for (uint32_t t = 0; t < T; t++) sx->h_df[t] = (uint32_t)(c->post_off[t + 1] - c->post_off[t]);
+    uint64_t sum_len = 0;
+#pragma omp parallel for reduction(+ : sum_len) num_threads(bm25x_host_threads(0))
+    for (uint32_t d = 0; d < N; d++) sum_len += c->doc_len[d];
+    sx->sum_len = sum_len;
+    sx->avgdl = (double)sum_len / (double)N;  // the expression of index_begin: the shards' s1 tables are the whole index's
+
+    // one shard at a time: host memory beyond the corpus stays within one shard's CSR
+    for (uint32_t s = 0; s < S; s++) {
+        const uint32_t lo = bounds[s], hi = bounds[s + 1];
+        std::vector<uint64_t> off((size_t)T + 1, 0);
+        std::vector<uint64_t> first(T);
+#pragma omp parallel for schedule(dynamic, 256) num_threads(bm25x_host_threads(0))
+        for (uint32_t t = 0; t < T; t++) {  // the shard's range inside the term's (ascending) list
+            const uint32_t *a = c->post_doc + c->post_off[t], *e = c->post_doc + c->post_off[t + 1];
+            const uint32_t *p0 = std::lower_bound(a, e, lo), *p1 = std::lower_bound(p0, e, hi);
+            first[t] = (uint64_t)(p0 - c->post_doc);
+            off[(size_t)t + 1] = (uint64_t)(p1 - p0);
+        }
+        std::vector<uint32_t> df(T);
+        for (uint32_t t = 0; t < T; t++) {
+            df[t] = (uint32_t)off[(size_t)t + 1];
+            off[(size_t)t + 1] += off[t];
+        }
+        const uint64_t Ps = off[T];
+        std::vector<uint32_t> pdoc(Ps ? Ps : 1), ptf(Ps ? Ps : 1);
+#pragma omp parallel for schedule(dynamic, 256) num_threads(bm25x_host_threads(0))
+        for (uint32_t t = 0; t < T; t++)
+            for (uint64_t i = 0; i < off[(size_t)t + 1] - off[t]; i++) {
+                pdoc[off[t] + i] = c->post_doc[first[t] + i] - lo;
+                ptf[off[t] + i] = c->post_tf[first[t] + i];
+            }
+        // (the term keys once, with shard 0: bm25x_sharded_lookup_terms asks it)
+        BuildMeta m{hi - lo, T, c->doc_len + lo, c->payload ? c->payload + (size_t)lo * 3 : nullptr, s ? nullptr : c->term_key,
+                    c->k1, c->b, df.data(), Ps};
+        m.stat_df = sx->h_df.data();
+        m.stat_n_docs = N;
+        m.stat_avgdl = sx->avgdl;
+        m.doc_base = lo;
+        bm25x_index *ix = nullptr;
+        rc = index_begin(m, dev[s], &ix);
+        if (rc == BM25X_OK) rc = upload_csr(ix, who, T, Ps, off.data(), pdoc.data(), ptf.data());  // destroys ix on failure
+        if (rc != BM25X_OK) {
+            bm25x_sharded_destroy(sx);
+            return rc;
+        }
+        sx->shards.push_back(ix);
+    }
+    *out = sx;
     return BM25X_OK;
 }
 

@@ -531,6 +531,39 @@ extern "C" int bm25x_batch_device_results(bm25x_batch *b, void **doc, void **sco
     return BM25X_OK;
 }
 
+// Timing events around an asynchronous run on the index's stream (the slices of search_batch_sliced, the shards of
+// bm25x_sharded_search_batch); bm25x_batch_add_stats reads them once the run has finished.
+int bm25x_batch_run_timed(bm25x_batch *b) {
+    bm25x_index *ix = b->ix;
+    BM25X_CUDA_TRY(cudaSetDevice(ix->device));
+    BM25X_CUDA_TRY(cudaMemsetAsync(b->d_fetched, 0, sizeof(unsigned long long), ix->stream));
+    BM25X_CUDA_TRY(cudaEventRecord(b->ev0, ix->stream));
+    const int rc = bm25x_batch_run(b, nullptr, nullptr);
+    if (rc != BM25X_OK) return rc;
+    BM25X_CUDA_TRY(cudaEventRecord(b->ev1, ix->stream));
+    return BM25X_OK;
+}
+
+cudaEvent_t bm25x_batch_done_event(bm25x_batch *b) { return b->ev1; }
+
+int bm25x_batch_add_stats(bm25x_batch *b, bm25x_search_stats *acc) {
+    BM25X_CUDA_TRY(cudaSetDevice(b->ix->device));
+    float ms = 0.f;
+    unsigned long long fetched = 0;
+    BM25X_CUDA_TRY(cudaEventElapsedTime(&ms, b->ev0, b->ev1));
+    BM25X_CUDA_TRY(cudaMemcpy(&fetched, b->d_fetched, sizeof(fetched), cudaMemcpyDeviceToHost));
+    uint32_t launches = 0;
+    for (int c = 0; c < kNumClasses; ++c)
+        if (b->groups[c].nq) launches += b->groups[c].d_q2 ? 2u : 1u;
+    acc->kernel_ms += ms;
+    acc->postings += b->postings;
+    acc->bytes_algo += 8ull * b->postings + 8ull * (uint64_t)b->live * b->k + 16ull * b->qterms;
+    acc->launches += launches;
+    acc->queries += b->live;
+    acc->postings_fetched += fetched;
+    return BM25X_OK;
+}
+
 // Large batches run as a pipeline of slices: while slice s is on the GPU the host canonicalises and uploads slice s + 1,
 // and the results of slice s - 1 travel to the host on a second stream.  Same results, row for row.
 static int search_batch_sliced(bm25x_index *ix, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms, uint32_t k,
@@ -559,17 +592,9 @@ static int search_batch_sliced(bm25x_index *ix, uint32_t nq, const uint32_t *q_o
         host_ms += std::chrono::duration<double, std::milli>(clk::now() - t0).count();
         if (rc != BM25X_OK) break;
         bm25x_batch *b = bs[s];
-        cudaError_t ce = cudaSuccess;
-        if (stats) {
-            ce = cudaMemsetAsync(b->d_fetched, 0, sizeof(unsigned long long), ix->stream);
-            if (ce == cudaSuccess) ce = cudaEventRecord(b->ev0, ix->stream);
-        }
-        if (ce == cudaSuccess) {
-            rc = bm25x_batch_run(b, nullptr, nullptr);
-            if (rc != BM25X_OK) break;
-        }
-        if (ce == cudaSuccess && stats) ce = cudaEventRecord(b->ev1, ix->stream);
-        if (ce == cudaSuccess) ce = cudaEventCreateWithFlags(&done[s], cudaEventDisableTiming);
+        rc = stats ? bm25x_batch_run_timed(b) : bm25x_batch_run(b, nullptr, nullptr);
+        if (rc != BM25X_OK) break;
+        cudaError_t ce = cudaEventCreateWithFlags(&done[s], cudaEventDisableTiming);
         if (ce == cudaSuccess) ce = cudaEventRecord(done[s], ix->stream);
         if (ce == cudaSuccess) ce = cudaStreamWaitEvent(ix->copy_stream, done[s], 0);
         const size_t slots = (size_t)(e - a) * k, o = (size_t)a * k;
@@ -594,20 +619,8 @@ static int search_batch_sliced(bm25x_index *ix, uint32_t nq, const uint32_t *q_o
     if (stats) {
         memset(stats, 0, sizeof(*stats));
         for (uint32_t s = 0; s < n_slices; ++s) {
-            bm25x_batch *b = bs[s];
-            float ms = 0.f;
-            unsigned long long fetched = 0;
-            cudaEventElapsedTime(&ms, b->ev0, b->ev1);
-            cudaMemcpy(&fetched, b->d_fetched, sizeof(fetched), cudaMemcpyDeviceToHost);
-            uint32_t launches = 0;
-            for (int c = 0; c < kNumClasses; ++c)
-                if (b->groups[c].nq) launches += b->groups[c].d_q2 ? 2u : 1u;
-            stats->kernel_ms += ms;
-            stats->postings += b->postings;
-            stats->bytes_algo += 8ull * b->postings + 8ull * (uint64_t)b->live * b->k + 16ull * b->qterms;
-            stats->launches += launches;
-            stats->queries += b->live;
-            stats->postings_fetched += fetched;
+            rc = bm25x_batch_add_stats(bs[s], stats);
+            if (rc != BM25X_OK) return fail(rc);
         }
         stats->h2d_ms = host_ms;  // canonicalise + upload of all slices (overlapped with the kernels but for the first)
         stats->d2h_ms = std::chrono::duration<double, std::milli>(clk::now() - t2).count();  // wait for the last download

@@ -1,0 +1,442 @@
+// bm25x_shards.cu — search over a document-sharded index (DESIGN §4.7): every shard answers the batch with its own top-k
+// (the whole index's ranking restricted to its documents, because it scores with the whole segment's statistics), and
+// k_merge_shards merges the shard lists on shard 0's device into exactly the rows bm25x_search_batch returns on the
+// unsharded index.
+#include <stdlib.h>
+#include <string.h>
+
+#include <algorithm>
+#include <chrono>
+#include <vector>
+
+#include "bm25x_common.h"
+
+namespace {
+
+// Row r of shard s: (score64 x, global doc = local + base[s]).  Its rank in the merged list is r plus, for every other
+// shard s', the rows of s' ranked before it: score64 >= x for s' < s (equal scores: lower doc ranges first), score64 > x
+// for s' > s.  Every row ranks itself — no sort, no shared state; the ranks of the Σ n_s rows are a permutation.
+struct ShardRows {
+    const uint32_t *doc[BM25X_MAX_SHARDS];
+    const float *score[BM25X_MAX_SHARDS];
+    const double *score64[BM25X_MAX_SHARDS];
+    const uint16_t *payload[BM25X_MAX_SHARDS];
+    const uint32_t *n[BM25X_MAX_SHARDS];
+    uint32_t base[BM25X_MAX_SHARDS];
+};
+
+// rows of a descending list that come before x: score > x (strict) or score >= x (!strict)
+__device__ __forceinline__ uint32_t count_before(const double *__restrict__ rows, uint32_t n, double x, bool strict) {
+    uint32_t lo = 0, hi = n;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        const double v = rows[mid];
+        if (strict ? v > x : v >= x) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo;
+}
+
+// One thread per (query, shard, row slot); consecutive threads take consecutive rows of one shard.  Threads of shard 0 also
+// write out_n and fill the slots at or past it as bm25x_batch_prepare leaves them (doc 0xFFFFFFFF, zero scores, payload).
+__global__ void k_merge_shards(ShardRows in, uint32_t S, uint32_t nq, uint32_t k, uint32_t *__restrict__ out_doc,
+                               float *__restrict__ out_score, double *__restrict__ out_score64,
+                               uint16_t *__restrict__ out_payload, uint32_t *__restrict__ out_n) {
+    const uint64_t total = (uint64_t)nq * S * k, stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
+        const uint32_t r = (uint32_t)(i % k);
+        const uint64_t qs = i / k;
+        const uint32_t s = (uint32_t)(qs % S), q = (uint32_t)(qs / S);
+        const size_t row0 = (size_t)q * k;
+        const uint32_t ns = min(in.n[s][q], k);
+        if (r < ns) {
+            const double x = in.score64[s][row0 + r];
+            uint64_t pos = r;
+            for (uint32_t t = 0; t < S && pos < k; t++)
+                if (t != s) pos += count_before(in.score64[t] + row0, min(in.n[t][q], k), x, t > s);
+            if (pos < k) {
+                const size_t o = row0 + pos, src = row0 + r;
+                out_doc[o] = in.doc[s][src] + in.base[s];
+                out_score[o] = in.score[s][src];
+                out_score64[o] = x;
+                out_payload[o * 3 + 0] = in.payload[s][src * 3 + 0];
+                out_payload[o * 3 + 1] = in.payload[s][src * 3 + 1];
+                out_payload[o * 3 + 2] = in.payload[s][src * 3 + 2];
+            }
+        }
+        if (s == 0) {
+            uint64_t sum = 0;
+            for (uint32_t t = 0; t < S; t++) sum += min(in.n[t][q], k);
+            const uint32_t nout = sum < k ? (uint32_t)sum : k;
+            if (r == 0) out_n[q] = nout;
+            if (r >= nout) {
+                const size_t o = row0 + r;
+                out_doc[o] = BM25X_DOC_INF;
+                out_score[o] = 0.f;
+                out_score64[o] = 0.0;
+                out_payload[o * 3 + 0] = out_payload[o * 3 + 1] = out_payload[o * 3 + 2] = 0;
+            }
+        }
+    }
+}
+
+int launch_merge(int device, const ShardRows &in, uint32_t S, uint32_t nq, uint32_t k, uint32_t *doc, float *score,
+                 double *score64, uint16_t *payload, uint32_t *n, cudaStream_t st) {
+    const uint64_t total = (uint64_t)nq * S * k;
+    if (!total) return BM25X_OK;
+    int sms = 132;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+    const uint64_t want = (total + 255) / 256, cap = (uint64_t)sms * 32;
+    k_merge_shards<<<(unsigned)std::min(want, cap), 256, 0, st>>>(in, S, nq, k, doc, score, score64, payload, n);
+    BM25X_CUDA_TRY(cudaGetLastError());
+    return BM25X_OK;
+}
+
+// Device result buffers of the merge ([nq*k] rows, [nq] counts), stream-ordered on `st`.
+struct MergeOut {
+    uint32_t *doc = nullptr, *n = nullptr;
+    float *score = nullptr;
+    double *score64 = nullptr;
+    uint16_t *payload = nullptr;
+    cudaError_t alloc(size_t slots, uint32_t nq, cudaStream_t st) {
+        slots = slots ? slots : 1;
+        cudaError_t e = cudaMallocAsync((void **)&doc, 4 * slots, st);
+        if (e == cudaSuccess) e = cudaMallocAsync((void **)&score, 4 * slots, st);
+        if (e == cudaSuccess) e = cudaMallocAsync((void **)&score64, 8 * slots, st);
+        if (e == cudaSuccess) e = cudaMallocAsync((void **)&payload, 6 * slots, st);
+        if (e == cudaSuccess) e = cudaMallocAsync((void **)&n, 4 * (size_t)(nq ? nq : 1), st);
+        return e;
+    }
+    cudaError_t download(size_t slots, uint32_t nq, uint32_t *o_doc, float *o_score, double *o_score64,
+                         uint16_t *o_payload, uint32_t *o_n, cudaStream_t st) const {
+        cudaError_t e = cudaSuccess;
+        if (o_doc) e = cudaMemcpyAsync(o_doc, doc, 4 * slots, cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess && o_score) e = cudaMemcpyAsync(o_score, score, 4 * slots, cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess && o_score64) e = cudaMemcpyAsync(o_score64, score64, 8 * slots, cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess && o_payload) e = cudaMemcpyAsync(o_payload, payload, 6 * slots, cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess && o_n) e = cudaMemcpyAsync(o_n, n, 4 * (size_t)nq, cudaMemcpyDeviceToHost, st);
+        return e;
+    }
+    void release(cudaStream_t st) {
+        for (void *p : {(void *)doc, (void *)score, (void *)score64, (void *)payload, (void *)n})
+            if (p) cudaFreeAsync(p, st);
+        doc = n = nullptr;
+        score = nullptr;
+        score64 = nullptr;
+        payload = nullptr;
+    }
+};
+
+// Bits [lo, hi) of a bitmap over global doc ids, shifted to bit 0 (shard bounds need not be multiples of 8).
+std::vector<uint8_t> allow_slice(const uint8_t *allow, uint32_t n_docs, uint32_t lo, uint32_t hi) {
+    const size_t nb = ((size_t)(hi - lo) + 7) / 8, total = ((size_t)n_docs + 7) / 8;
+    std::vector<uint8_t> out(nb ? nb : 1, 0);
+    const size_t byte0 = lo >> 3;
+    const unsigned sh = lo & 7u;
+    for (size_t j = 0; j < nb; j++) {
+        unsigned v = allow[byte0 + j] >> sh;
+        if (sh && byte0 + j + 1 < total) v |= (unsigned)allow[byte0 + j + 1] << (8 - sh);
+        out[j] = (uint8_t)v;
+    }
+    if ((hi - lo) & 7u) out[nb - 1] &= (uint8_t)((1u << ((hi - lo) & 7u)) - 1u);  // no bits past the shard's last doc
+    return out;
+}
+
+}  // namespace
+
+// ---- the refusals of bm25x_search_batch, against the WHOLE segment's df (a query with 65 live terms is refused even when
+// no shard sees more than 64).  Mirrors bm25x_batch_prepare's checks and messages, including the query numbering inside
+// the slices bm25x_search_batch cuts large batches into.  Returns the whole index's live queries in *live_out. ----
+static int check_queries(const bm25x_sharded_index *sx, uint32_t slice_min, uint32_t nq, const uint32_t *q_off,
+                         const uint32_t *q_terms, uint32_t k, uint32_t *live_out) {
+    if (nq && (!q_off || (!q_terms && q_off[nq] != 0))) {
+        bm25x_set_error("bm25x_batch_prepare: null argument");
+        return BM25X_ERR_INVALID;
+    }
+    if (k == 0) {
+        bm25x_set_error("number of needed rows is set to 0");  // scanners/default.rs:114-116
+        return BM25X_ERR_LIMIT_ZERO;
+    }
+    if (k > BM25X_MAX_K) {
+        bm25x_set_error("bm25x_batch_prepare: k=%u > BM25X_MAX_K=%d", k, BM25X_MAX_K);
+        return BM25X_ERR_UNSUPPORTED;
+    }
+    const uint32_t n_slices = slice_min && nq >= 2ull * slice_min ? std::min<uint32_t>(16u, nq / slice_min) : 1u;
+    const uint32_t T = sx->n_terms;
+    const uint32_t *h_df = sx->h_df.data();
+    std::vector<uint8_t> kind(nq ? nq : 1, 0);  // 0 ok, 1 offsets, 2 too many live terms
+    std::vector<uint32_t> live(nq ? nq : 1, 0);
+    for (uint32_t s = 0; s < n_slices; s++) {
+        const uint32_t a = (uint32_t)(((uint64_t)nq * s) / n_slices), e = (uint32_t)(((uint64_t)nq * (s + 1)) / n_slices);
+        const size_t base0 = e > a ? q_off[a] : 0;
+        const size_t n_raw = e > a && q_off[e] >= base0 ? q_off[e] - base0 : 0;
+#pragma omp parallel for schedule(static, 1024) num_threads(e - a < 4096 ? 1 : bm25x_host_threads(16))
+        for (uint32_t i = a; i < e; i++) {
+            if (q_off[i + 1] < q_off[i] || q_off[i] < base0 || q_off[i + 1] - base0 > n_raw) {
+                kind[i] = 1;
+                continue;
+            }
+            uint32_t buf[256];
+            std::vector<uint32_t> big;
+            const uint32_t n = q_off[i + 1] - q_off[i];
+            uint32_t *dst = buf;
+            if (n > 256) {
+                big.resize(n);
+                dst = big.data();
+            }
+            uint32_t m = 0;
+            for (uint32_t j = 0; j < n; j++) {
+                const uint32_t t = q_terms[q_off[i] + j];
+                if (t < T && h_df[t] != 0) dst[m++] = t;
+            }
+            std::sort(dst, dst + m);
+            m = (uint32_t)(std::unique(dst, dst + m) - dst);
+            live[i] = m;
+            if (m > BM25X_MAX_QUERY_TERMS) kind[i] = 2;
+        }
+        int bad = -1;  // the batch reports the last offending query of the first slice that has one
+        for (uint32_t i = a; i < e; i++)
+            if (kind[i]) bad = (int)i;
+        if (bad >= 0) {
+            if (kind[bad] == 1) {
+                bm25x_set_error("bm25x_batch_prepare: q_off not monotone at %d", bad - (int)a);
+                return BM25X_ERR_INVALID;
+            }
+            bm25x_set_error("bm25x_batch_prepare: query %d has %u live terms > %d", bad - (int)a, live[bad],
+                            BM25X_MAX_QUERY_TERMS);
+            return BM25X_ERR_UNSUPPORTED;
+        }
+    }
+    uint32_t n_live = 0;
+    for (uint32_t i = 0; i < nq; i++) n_live += live[i] != 0;
+    *live_out = n_live;
+    return BM25X_OK;
+}
+
+extern "C" int bm25x_sharded_search_batch(bm25x_sharded_index *sx, uint32_t nq, const uint32_t *q_off,
+                                          const uint32_t *q_terms, uint32_t k, const uint8_t *allow, uint32_t *out_doc,
+                                          float *out_score, double *out_score64, uint16_t *out_payload, uint32_t *out_n,
+                                          bm25x_search_stats *stats) {
+    using clk = std::chrono::steady_clock;
+    if (!sx) {
+        bm25x_set_error("bm25x_sharded_search_batch: null argument");
+        return BM25X_ERR_INVALID;
+    }
+    const auto t0 = clk::now();
+    uint32_t n_live = 0;
+    int rc = check_queries(sx, sx->shards[0]->slice_min, nq, q_off, q_terms, k, &n_live);
+    if (rc != BM25X_OK) return rc;
+    const uint32_t S = sx->n_shards;
+    bm25x_index *ix0 = sx->shards[0];
+    const int dev0 = ix0->device;
+    cudaStream_t ms = ix0->stream;  // the merge runs behind shard 0's kernels on its library stream
+    std::vector<bm25x_batch *> bs(S, nullptr);
+    std::vector<void *> peer_bufs;  // results of shards on other devices, copied to dev0
+    std::vector<cudaEvent_t> evs;
+    MergeOut mo;
+    auto cleanup = [&](int code) {
+        cudaSetDevice(dev0);
+        cudaStreamSynchronize(ms);
+        for (void *p : peer_bufs) cudaFreeAsync(p, ms);
+        mo.release(ms);
+        for (cudaEvent_t e : evs) cudaEventDestroy(e);
+        for (bm25x_batch *b : bs)
+            if (b) bm25x_batch_destroy(b);
+        return code;
+    };
+    // ---- prepare + run shard after shard: the next shard's canonicalisation overlaps the kernels of the previous ----
+    for (uint32_t s = 0; s < S && rc == BM25X_OK; s++) {
+        const uint32_t lo = sx->bounds[s], hi = sx->bounds[s + 1];
+        std::vector<uint8_t> al;
+        if (allow) al = allow_slice(allow, sx->n_docs, lo, hi);
+        rc = bm25x_batch_prepare(sx->shards[s], nq, q_off, q_terms, k, allow ? al.data() : nullptr, &bs[s]);
+        if (rc == BM25X_OK) rc = bm25x_batch_run_timed(bs[s]);
+    }
+    if (rc != BM25X_OK) return cleanup(rc);
+    const auto t1 = clk::now();
+    // ---- shard rows on dev0: read in place there, copied peer to peer from the other devices ----
+    const size_t slots = (size_t)nq * k;
+    ShardRows in;
+    memset(&in, 0, sizeof(in));
+    cudaError_t e = cudaSetDevice(dev0);
+    for (uint32_t s = 0; s < S && e == cudaSuccess; s++) {
+        void *p[5];
+        bm25x_batch_device_results(bs[s], &p[0], &p[1], &p[2], &p[3], &p[4]);
+        e = cudaStreamWaitEvent(ms, bm25x_batch_done_event(bs[s]), 0);
+        const int dev = sx->shards[s]->device;
+        if (e == cudaSuccess && dev != dev0) {
+            const size_t bytes[5] = {4 * slots, 4 * slots, 8 * slots, 6 * slots, 4 * (size_t)nq};
+            for (int a = 0; a < 5 && e == cudaSuccess; a++) {
+                void *dst = nullptr;
+                e = cudaMallocAsync(&dst, bytes[a] ? bytes[a] : 4, ms);
+                if (e != cudaSuccess) break;
+                peer_bufs.push_back(dst);
+                if (bytes[a]) e = cudaMemcpyPeerAsync(dst, dev0, p[a], dev, bytes[a], ms);
+                p[a] = dst;
+            }
+        }
+        in.doc[s] = (const uint32_t *)p[0];
+        in.score[s] = (const float *)p[1];
+        in.score64[s] = (const double *)p[2];
+        in.payload[s] = (const uint16_t *)p[3];
+        in.n[s] = (const uint32_t *)p[4];
+        in.base[s] = sx->bounds[s];
+    }
+    if (e == cudaSuccess) e = mo.alloc(slots, nq, ms);
+    cudaEvent_t m0 = nullptr, m1 = nullptr;
+    if (e == cudaSuccess && stats) {
+        e = cudaEventCreate(&m0);
+        if (e == cudaSuccess) evs.push_back(m0);
+        if (e == cudaSuccess) e = cudaEventCreate(&m1);
+        if (e == cudaSuccess) evs.push_back(m1);
+        if (e == cudaSuccess) e = cudaEventRecord(m0, ms);
+    }
+    if (e != cudaSuccess) {
+        bm25x_set_error("bm25x_sharded_search_batch: %s", cudaGetErrorString(e));
+        return cleanup(e == cudaErrorMemoryAllocation ? BM25X_ERR_OOM : BM25X_ERR_CUDA);
+    }
+    rc = launch_merge(dev0, in, S, nq, k, mo.doc, mo.score, mo.score64, mo.payload, mo.n, ms);
+    if (rc != BM25X_OK) return cleanup(rc);
+    if (stats) e = cudaEventRecord(m1, ms);
+    if (e == cudaSuccess) e = mo.download(slots, nq, out_doc, out_score, out_score64, out_payload, out_n, ms);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ms);  // after the merge: every shard's kernels have finished too
+    if (e != cudaSuccess) {
+        bm25x_set_error("bm25x_sharded_search_batch: %s", cudaGetErrorString(e));
+        return cleanup(BM25X_ERR_CUDA);
+    }
+    if (stats) {
+        memset(stats, 0, sizeof(*stats));
+        for (uint32_t s = 0; s < S && rc == BM25X_OK; s++) rc = bm25x_batch_add_stats(bs[s], stats);
+        float mms = 0.f;
+        if (rc == BM25X_OK) {
+            cudaSetDevice(dev0);
+            e = cudaEventElapsedTime(&mms, m0, m1);
+            if (e != cudaSuccess) {
+                bm25x_set_error("bm25x_sharded_search_batch: %s", cudaGetErrorString(e));
+                rc = BM25X_ERR_CUDA;
+            }
+        }
+        stats->kernel_ms += mms;  // summed device time of the shards' kernels and the merge, not wall time
+        stats->launches += (uint64_t)nq * S * k ? 1u : 0u;
+        stats->queries = n_live;
+        stats->h2d_ms = std::chrono::duration<double, std::milli>(t1 - t0).count();
+        stats->d2h_ms = std::chrono::duration<double, std::milli>(clk::now() - t1).count();
+    }
+    return cleanup(rc);
+}
+
+// ---- test / measurement hook: the merge kernel alone on host rows ----
+extern "C" int bm25x_merge_shards(int device, uint32_t S, uint32_t nq, uint32_t k, const uint32_t *doc_base,
+                                  const uint32_t *doc, const float *score, const double *score64, const uint16_t *payload,
+                                  const uint32_t *n, uint32_t *out_doc, float *out_score, double *out_score64,
+                                  uint16_t *out_payload, uint32_t *out_n, float *merge_ms) {
+    const char *who = "bm25x_merge_shards";
+    if (k == 0) {
+        bm25x_set_error("number of needed rows is set to 0");
+        return BM25X_ERR_LIMIT_ZERO;
+    }
+    if (S == 0 || S > BM25X_MAX_SHARDS || k > BM25X_MAX_K) {
+        bm25x_set_error("%s: n_shards=%u must be 1..%d and k=%u <= %d", who, S, BM25X_MAX_SHARDS, k, BM25X_MAX_K);
+        return BM25X_ERR_INVALID;
+    }
+    if (nq && (!doc_base || !doc || !score || !score64 || !payload || !n)) {
+        bm25x_set_error("%s: null argument", who);
+        return BM25X_ERR_INVALID;
+    }
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) {
+        cudaGetLastError();
+        bm25x_set_error("%s: CUDA device %d not available (%d devices); there is no CPU fallback", who, device, ndev);
+        return BM25X_ERR_CUDA;
+    }
+    BM25X_CUDA_TRY(cudaSetDevice(device));
+    const size_t slots = (size_t)nq * k, all = slots * S;
+    cudaStream_t st = nullptr;
+    BM25X_CUDA_TRY(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+    MergeOut src, mo;  // the S shards' rows back to back in `src`
+    cudaEvent_t m0 = nullptr, m1 = nullptr;
+    cudaError_t e = src.alloc(all, nq * S, st);
+    if (e == cudaSuccess) e = mo.alloc(slots, nq, st);
+    auto up = [&](void *dst, const void *h, size_t bytes) {
+        if (e == cudaSuccess && bytes) e = cudaMemcpyAsync(dst, h, bytes, cudaMemcpyHostToDevice, st);
+    };
+    up(src.doc, doc, 4 * all);
+    up(src.score, score, 4 * all);
+    up(src.score64, score64, 8 * all);
+    up(src.payload, payload, 6 * all);
+    up(src.n, n, 4 * (size_t)nq * S);
+    ShardRows in;
+    memset(&in, 0, sizeof(in));
+    for (uint32_t s = 0; s < S; s++) {
+        in.doc[s] = src.doc + s * slots;
+        in.score[s] = src.score + s * slots;
+        in.score64[s] = src.score64 + s * slots;
+        in.payload[s] = src.payload + s * slots * 3;
+        in.n[s] = src.n + (size_t)s * nq;
+        in.base[s] = nq ? doc_base[s] : 0;
+    }
+    if (e == cudaSuccess) e = cudaEventCreate(&m0);
+    if (e == cudaSuccess) e = cudaEventCreate(&m1);
+    if (e == cudaSuccess) e = cudaEventRecord(m0, st);
+    int rc = BM25X_OK;
+    if (e == cudaSuccess) rc = launch_merge(device, in, S, nq, k, mo.doc, mo.score, mo.score64, mo.payload, mo.n, st);
+    if (e == cudaSuccess && rc == BM25X_OK) e = cudaEventRecord(m1, st);
+    if (e == cudaSuccess && rc == BM25X_OK) e = mo.download(slots, nq, out_doc, out_score, out_score64, out_payload, out_n, st);
+    if (e == cudaSuccess && rc == BM25X_OK) e = cudaStreamSynchronize(st);
+    if (e == cudaSuccess && rc == BM25X_OK && merge_ms) e = cudaEventElapsedTime(merge_ms, m0, m1);
+    cudaStreamSynchronize(st);
+    src.release(st);
+    mo.release(st);
+    cudaStreamSynchronize(st);
+    if (m0) cudaEventDestroy(m0);
+    if (m1) cudaEventDestroy(m1);
+    cudaStreamDestroy(st);
+    if (rc != BM25X_OK) return rc;
+    if (e != cudaSuccess) {
+        bm25x_set_error("%s: %s", who, cudaGetErrorString(e));
+        return e == cudaErrorMemoryAllocation ? BM25X_ERR_OOM : BM25X_ERR_CUDA;
+    }
+    return BM25X_OK;
+}
+
+// ---- handle queries and options ----
+extern "C" int bm25x_sharded_get_info(const bm25x_sharded_index *sx, bm25x_index_info *out, uint32_t *n_shards_out,
+                                      uint32_t *doc_bounds_out) {
+    if (!sx || !out) {
+        bm25x_set_error("bm25x_sharded_get_info: null argument");
+        return BM25X_ERR_INVALID;
+    }
+    memset(out, 0, sizeof(*out));
+    out->n_docs = sx->n_docs;
+    out->n_terms = sx->n_terms;
+    out->n_postings = sx->n_post;
+    out->sum_doc_len = sx->sum_len;
+    out->avgdl = sx->avgdl;
+    out->k1 = sx->k1;
+    out->b = sx->b;
+    for (const bm25x_index *ix : sx->shards) {
+        out->device_bytes += ix->device_bytes;
+        out->n_blocks += ix->d.n_blocks;
+    }
+    out->device = sx->shards[0]->device;
+    if (n_shards_out) *n_shards_out = sx->n_shards;
+    if (doc_bounds_out) std::copy(sx->bounds.begin(), sx->bounds.end(), doc_bounds_out);
+    return BM25X_OK;
+}
+
+extern "C" int bm25x_sharded_set_option(bm25x_sharded_index *sx, const char *name, int64_t value) {
+    if (!sx || !name) {
+        bm25x_set_error("bm25x_sharded_set_option: null argument");
+        return BM25X_ERR_INVALID;
+    }
+    for (bm25x_index *ix : sx->shards) {
+        const int rc = bm25x_index_set_option(ix, name, value);
+        if (rc != BM25X_OK) return rc;  // an unknown name fails on shard 0, before any shard changed
+    }
+    return BM25X_OK;
+}
+
+// Every shard knows every term (ordinals are the segment's); shard 0 holds the keys.
+extern "C" int bm25x_sharded_lookup_terms(const bm25x_sharded_index *sx, const uint8_t *keys, uint32_t n, uint32_t *out) {
+    return bm25x_lookup_terms(sx ? sx->shards[0] : nullptr, keys, n, out);
+}

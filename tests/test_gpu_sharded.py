@@ -224,13 +224,43 @@ def test_refusals_match_the_unsharded_index(m):
     cases = [(q_off, q_terms, 0), (q_off, q_terms, m.MAX_K + 1),
              (np.array([0, 3, 68], np.uint32), np.r_[np.uint32([1, 2, 3]), big], 10),
              (np.array([0, 2, 1], np.uint32), np.uint32([1, 2]), 10)]
-    for qo, qt, k in cases:
+
+    def refused(qo, qt, k, calls=1):
         errs = []
         for idx in (ix, sx):
-            with pytest.raises(m.Bm25xError) as e:
-                idx.search_batch(qo, qt, k)
-            errs.append((e.value.code, str(e.value)))
-        assert errs[0] == errs[1], errs
+            for _ in range(calls):
+                with pytest.raises(m.Bm25xError) as e:
+                    idx.search_batch(qo, qt, k)
+                errs.append((e.value.code, str(e.value)))
+        assert len(set(errs)) == 1, errs
+        return errs[0]
+
+    for qo, qt, k in cases:
+        refused(qo, qt, k)
+
+    def batch(nq, seed, big_at=(), backwards_at=()):
+        qo, qt = m.synth_queries(seed, nq, 100, 1, 4, c.post_off)
+        qs = [list(qt[qo[i]:qo[i + 1]]) for i in range(nq)]
+        for i in big_at:
+            qs[i] = list(big)
+        qo = np.cumsum([0] + [len(q) for q in qs]).astype(np.uint32)
+        for i in backwards_at:
+            qo[i + 1] = qo[i] - 1
+        return qo, np.array([t for q in qs for t in q], np.uint32)
+
+    # a sliced batch (4 slices of 16) whose only bad query, 40, is query 8 of the third slice
+    for idx in (ix, sx):
+        idx.set_option("slice_min", 16)
+    assert refused(*batch(64, 33, big_at=[40]), 10) == (4, "bm25x error 4: bm25x_batch_prepare: query 8 has 65 live terms > 64")
+    assert refused(*batch(64, 33, backwards_at=[40]), 10) == (1, "bm25x error 1: bm25x_batch_prepare: q_off not monotone at 8")
+    # 8192 queries in one piece, canonicalised by several threads in chunks of 1024: with bad queries in several chunks the
+    # message names the highest-numbered one, call after call
+    for idx in (ix, sx):
+        idx.set_option("slice_min", 0)
+    assert refused(*batch(8192, 34, big_at=[1500, 7000], backwards_at=[4200]), 10, calls=3) == \
+        (4, "bm25x error 4: bm25x_batch_prepare: query 7000 has 65 live terms > 64")
+    assert refused(*batch(8192, 34, big_at=[1500, 4200], backwards_at=[7000]), 10, calls=3) == \
+        (1, "bm25x error 1: bm25x_batch_prepare: q_off not monotone at 7000")
     # 65 live terms spread so that no shard sees more than 64 of them: still refused
     sx2 = m.ShardedIndex.from_corpus(c, n_shards=16)
     with pytest.raises(m.Bm25xError) as e:

@@ -196,6 +196,49 @@ def _p(a, ty):
     return a.ctypes.data_as(C.POINTER(ty)) if a is not None else None
 
 
+def _kept(keep, a, dt, ct):
+    """Pointer to `a` as a contiguous `dt` array, which `keep` holds alive until the library has copied it."""
+    a = np.ascontiguousarray(a, dtype=dt)
+    keep.append(a)
+    return _p(a, ct)
+
+
+def _corpus(keep, n_docs, doc_len, n_terms, post_off, post_doc, post_tf, k1, b, payload, term_keys):
+    c = _Corpus()
+    c.n_docs, c.n_terms, c.k1, c.b = int(n_docs), int(n_terms), float(k1), float(b)
+    c.doc_len = _kept(keep, doc_len, np.uint32, C.c_uint32)
+    c.post_off = _kept(keep, post_off, np.uint64, C.c_uint64)
+    c.post_doc = _kept(keep, post_doc, np.uint32, C.c_uint32)
+    c.post_tf = _kept(keep, post_tf, np.uint32, C.c_uint32)
+    if payload is not None:
+        c.payload = _kept(keep, payload, np.uint16, C.c_uint16)
+    if term_keys is not None:
+        c.term_key = _kept(keep, term_keys, np.uint8, C.c_uint8)
+    return c
+
+
+def _result_arrays(nq, k, want_f64, want_payload):
+    return {"doc": np.empty((nq, k), np.uint32), "score": np.empty((nq, k), np.float32),
+            "score64": np.empty((nq, k), np.float64) if want_f64 else None,
+            "payload": np.empty((nq, k, 3), np.uint16) if want_payload else None, "n": np.empty(nq, np.uint32)}
+
+
+def _search_batch(fn, h, q_off, q_terms, k, allow, want_f64, want_payload, out):
+    """bm25x_search_batch or bm25x_sharded_search_batch (the same signature) on host buffers."""
+    q_off = np.ascontiguousarray(q_off, dtype=np.uint32)
+    q_terms = np.ascontiguousarray(q_terms, dtype=np.uint32)
+    nq = len(q_off) - 1
+    if out is None:
+        out = _result_arrays(nq, max(int(k), 1), want_f64, want_payload)
+    al = np.ascontiguousarray(allow, dtype=np.uint8) if allow is not None else None
+    st = SearchStats()
+    _check(fn(h, nq, _p(q_off, C.c_uint32), _p(q_terms, C.c_uint32), int(k), _p(al, C.c_uint8),
+              _p(out["doc"], C.c_uint32), _p(out["score"], C.c_float), _p(out["score64"], C.c_double),
+              _p(out["payload"], C.c_uint16), _p(out["n"], C.c_uint32), C.byref(st)))
+    out["stats"] = st
+    return out
+
+
 def check_vectors(off, terms, tfs=None):
     """bm25x_check_vectors: the Document / Query invariants of crates/bm25/src/vector.rs:46-134 for n vectors in CSR form
     (keys strictly ascending, tfs non-zero); raises Bm25xError(1, "invalid data: ...")."""
@@ -278,27 +321,11 @@ class Index:
 
     def __init__(self, n_docs, doc_len, n_terms, post_off, post_doc, post_tf, k1=1.2, b=0.75, payload=None,
                  term_keys=None, device=0):
-        L = load_library()
-        self._keep = [np.ascontiguousarray(doc_len, dtype=np.uint32), np.ascontiguousarray(post_off, dtype=np.uint64),
-                      np.ascontiguousarray(post_doc, dtype=np.uint32), np.ascontiguousarray(post_tf, dtype=np.uint32)]
-        c = _Corpus()
-        c.n_docs, c.n_terms, c.k1, c.b = int(n_docs), int(n_terms), float(k1), float(b)
-        c.doc_len = _p(self._keep[0], C.c_uint32)
-        c.post_off = _p(self._keep[1], C.c_uint64)
-        c.post_doc = _p(self._keep[2], C.c_uint32)
-        c.post_tf = _p(self._keep[3], C.c_uint32)
-        if payload is not None:
-            pl = np.ascontiguousarray(payload, dtype=np.uint16)
-            self._keep.append(pl)
-            c.payload = _p(pl, C.c_uint16)
-        if term_keys is not None:
-            tk = np.ascontiguousarray(term_keys, dtype=np.uint8)
-            self._keep.append(tk)
-            c.term_key = _p(tk, C.c_uint8)
+        keep = []
+        c = _corpus(keep, n_docs, doc_len, n_terms, post_off, post_doc, post_tf, k1, b, payload, term_keys)
         h = C.c_void_p()
-        _check(L.bm25x_index_create(C.byref(c), device, C.byref(h)))
-        self.h = h
-        self._keep = None  # the library copied everything to the device
+        _check(load_library().bm25x_index_create(C.byref(c), device, C.byref(h)))
+        self.h, self._keep = h, None  # the library copied everything to the device
         self.n_docs, self.n_terms = int(n_docs), int(n_terms)
 
     @classmethod
@@ -308,40 +335,33 @@ class Index:
         """Index from the sealed segment as the reference stores it: per-token chains of 128-posting blocks in the
         codec of compression.rs, decoded on the GPU (bm25x_index_create_from_blocks).  Document norms come either from
         exact lengths (`doc_len`) or, as on the pages, from `doc_fieldnorm` + `sum_doc_len`."""
-        L = load_library()
         c = _Blocks()
         keep = []
-
-        def arr(a, dt, ct):
-            a = np.ascontiguousarray(a, dtype=dt)
-            keep.append(a)
-            return _p(a, ct)
-
         c.n_docs, c.n_terms, c.k1, c.b = int(n_docs), int(n_terms), float(k1), float(b)
         if doc_len is not None:
-            c.doc_len = arr(doc_len, np.uint32, C.c_uint32)
+            c.doc_len = _kept(keep, doc_len, np.uint32, C.c_uint32)
         if doc_fieldnorm is not None:
-            c.doc_fieldnorm = arr(doc_fieldnorm, np.uint8, C.c_uint8)
+            c.doc_fieldnorm = _kept(keep, doc_fieldnorm, np.uint8, C.c_uint8)
         c.sum_doc_len = int(sum_doc_len)
         if payload is not None:
-            c.payload = arr(payload, np.uint16, C.c_uint16)
+            c.payload = _kept(keep, payload, np.uint16, C.c_uint16)
         if term_keys is not None:
-            c.term_key = arr(term_keys, np.uint8, C.c_uint8)
-        c.term_blk_off = arr(term_blk_off, np.uint64, C.c_uint64)
+            c.term_key = _kept(keep, term_keys, np.uint8, C.c_uint8)
+        c.term_blk_off = _kept(keep, term_blk_off, np.uint64, C.c_uint64)
         c.n_blocks = int(keep[-1][int(n_terms)]) if len(keep[-1]) > int(n_terms) else 0
-        c.blk_min_doc = arr(blk_min_doc, np.uint32, C.c_uint32)
-        c.blk_n = arr(blk_n, np.uint32, C.c_uint32)
-        c.blk_meta_doc = arr(blk_meta_doc, np.uint8, C.c_uint8)
-        c.blk_meta_tf = arr(blk_meta_tf, np.uint8, C.c_uint8)
-        c.blk_doc_off = arr(blk_doc_off, np.uint64, C.c_uint64)
-        c.blk_tf_off = arr(blk_tf_off, np.uint64, C.c_uint64)
-        c.bytes = arr(data, np.uint8, C.c_uint8)
+        c.blk_min_doc = _kept(keep, blk_min_doc, np.uint32, C.c_uint32)
+        c.blk_n = _kept(keep, blk_n, np.uint32, C.c_uint32)
+        c.blk_meta_doc = _kept(keep, blk_meta_doc, np.uint8, C.c_uint8)
+        c.blk_meta_tf = _kept(keep, blk_meta_tf, np.uint8, C.c_uint8)
+        c.blk_doc_off = _kept(keep, blk_doc_off, np.uint64, C.c_uint64)
+        c.blk_tf_off = _kept(keep, blk_tf_off, np.uint64, C.c_uint64)
+        c.bytes = _kept(keep, data, np.uint8, C.c_uint8)
         c.n_bytes = len(keep[-1])
         if blk_wand_fieldnorm is not None and blk_wand_tf is not None:   # SummaryTuple.wand_* (checked against the blocks)
-            c.blk_wand_fieldnorm = arr(blk_wand_fieldnorm, np.uint8, C.c_uint8)
-            c.blk_wand_tf = arr(blk_wand_tf, np.uint32, C.c_uint32)
+            c.blk_wand_fieldnorm = _kept(keep, blk_wand_fieldnorm, np.uint8, C.c_uint8)
+            c.blk_wand_tf = _kept(keep, blk_wand_tf, np.uint32, C.c_uint32)
         h = C.c_void_p()
-        _check(L.bm25x_index_create_from_blocks(C.byref(c), device, C.byref(h)))
+        _check(load_library().bm25x_index_create_from_blocks(C.byref(c), device, C.byref(h)))
         return cls._adopt(h, n_docs, n_terms)
 
     @classmethod
@@ -403,24 +423,8 @@ class Index:
 
     # ---- bm25::search for a batch (host buffers in, host buffers out) ----
     def search_batch(self, q_off, q_terms, k, allow=None, want_f64=True, want_payload=False, out=None):
-        q_off = np.ascontiguousarray(q_off, dtype=np.uint32)
-        q_terms = np.ascontiguousarray(q_terms, dtype=np.uint32)
-        nq = len(q_off) - 1
-        kk = max(int(k), 1)
-        if out is None:
-            out = {"doc": np.empty((nq, kk), np.uint32), "score": np.empty((nq, kk), np.float32),
-                   "score64": np.empty((nq, kk), np.float64) if want_f64 else None,
-                   "payload": np.empty((nq, kk, 3), np.uint16) if want_payload else None,
-                   "n": np.empty(nq, np.uint32)}
-        al = np.ascontiguousarray(allow, dtype=np.uint8) if allow is not None else None
-        st = SearchStats()
-        _check(load_library().bm25x_search_batch(self.h, nq, _p(q_off, C.c_uint32), _p(q_terms, C.c_uint32), int(k),
-                                                 _p(al, C.c_uint8), _p(out["doc"], C.c_uint32),
-                                                 _p(out["score"], C.c_float), _p(out["score64"], C.c_double),
-                                                 _p(out["payload"], C.c_uint16), _p(out["n"], C.c_uint32),
-                                                 C.byref(st)))
-        out["stats"] = st
-        return out
+        return _search_batch(load_library().bm25x_search_batch, self.h, q_off, q_terms, k, allow, want_f64, want_payload,
+                             out)
 
     def search(self, query, k, allow=None):
         """One query, the shape of bm25::search(&index, k, &query, filter): [(score f64, doc id)] best first."""
@@ -437,24 +441,18 @@ class Index:
         index's statistics (bm25x_growing_create).  Search it like any index; ids are growing ordinals."""
         g = _GrowingDocs()
         keep = []
-
-        def arr(a, dt, ct):
-            a = np.ascontiguousarray(a, dtype=dt)
-            keep.append(a)
-            return _p(a, ct)
-
-        g.elem_off = arr(elem_off, np.uint64, C.c_uint64)
+        g.elem_off = _kept(keep, elem_off, np.uint64, C.c_uint64)
         g.n_docs = len(keep[-1]) - 1
-        g.elem_term = arr(elem_term, np.uint32, C.c_uint32)
-        g.elem_tf = arr(elem_tf, np.uint32, C.c_uint32)
+        g.elem_term = _kept(keep, elem_term, np.uint32, C.c_uint32)
+        g.elem_tf = _kept(keep, elem_tf, np.uint32, C.c_uint32)
         if doc_len is not None:
-            g.doc_len = arr(doc_len, np.uint32, C.c_uint32)
+            g.doc_len = _kept(keep, doc_len, np.uint32, C.c_uint32)
         if doc_fieldnorm is not None:
-            g.doc_fieldnorm = arr(doc_fieldnorm, np.uint8, C.c_uint8)
+            g.doc_fieldnorm = _kept(keep, doc_fieldnorm, np.uint8, C.c_uint8)
         if payload is not None:
-            g.payload = arr(payload, np.uint16, C.c_uint16)
+            g.payload = _kept(keep, payload, np.uint16, C.c_uint16)
         if deleted is not None:
-            g.deleted = arr(deleted, np.uint8, C.c_uint8)
+            g.deleted = _kept(keep, deleted, np.uint8, C.c_uint8)
         h = C.c_void_p()
         _check(load_library().bm25x_growing_create(self.h, C.byref(g), C.byref(h)))
         return Index._adopt(h, g.n_docs, self.n_terms)
@@ -465,9 +463,7 @@ class Index:
         q_off = np.ascontiguousarray(q_off, dtype=np.uint32)
         q_terms = np.ascontiguousarray(q_terms, dtype=np.uint32)
         nq, kk = len(q_off) - 1, int(k)
-        out = {"doc": np.empty((nq, kk), np.uint32), "score": np.empty((nq, kk), np.float32),
-               "score64": np.empty((nq, kk), np.float64),
-               "payload": np.empty((nq, kk, 3), np.uint16) if want_payload else None, "n": np.empty(nq, np.uint32)}
+        out = _result_arrays(nq, kk, True, want_payload)
         al = np.ascontiguousarray(allow, dtype=np.uint8) if allow is not None else None
         alg = np.ascontiguousarray(allow_growing, dtype=np.uint8) if allow_growing is not None else None
         st = SearchStats()
@@ -505,9 +501,7 @@ def merge_topk(a, b, doc_base_b, k):
     nq = len(a["n"])
     assert a["doc"].shape == (nq, k) and b["doc"].shape == (nq, k)
     pay = a.get("payload") is not None and b.get("payload") is not None
-    out = {"doc": np.empty((nq, k), np.uint32), "score": np.empty((nq, k), np.float32),
-           "score64": np.empty((nq, k), np.float64), "payload": np.empty((nq, k, 3), np.uint16) if pay else None,
-           "n": np.empty(nq, np.uint32)}
+    out = _result_arrays(nq, k, True, pay)
     c = lambda x, dt: np.ascontiguousarray(x, dtype=dt)
     keep = [c(a["doc"], np.uint32), c(a["score"], np.float32), c(a["score64"], np.float64),
             c(a["payload"], np.uint16) if pay else None, c(a["n"], np.uint32),
@@ -525,12 +519,6 @@ def merge_topk(a, b, doc_base_b, k):
 MAX_SHARDS = 16
 
 
-def _result_arrays(nq, k, want_f64, want_payload):
-    return {"doc": np.empty((nq, k), np.uint32), "score": np.empty((nq, k), np.float32),
-            "score64": np.empty((nq, k), np.float64) if want_f64 else None,
-            "payload": np.empty((nq, k, 3), np.uint16) if want_payload else None, "n": np.empty(nq, np.uint32)}
-
-
 class ShardedIndex:
     """One sealed segment split by document range into `n_shards` indexes (bm25x_sharded_*), on one GPU or several, so
     that it need not fit in one GPU's HBM.  Searches return exactly what Index.search_batch returns on the unsharded index
@@ -538,23 +526,13 @@ class ShardedIndex:
 
     def __init__(self, n_docs, doc_len, n_terms, post_off, post_doc, post_tf, k1=1.2, b=0.75, payload=None,
                  term_keys=None, n_shards=2, doc_bounds=None, devices=None):
-        L = load_library()
-        keep = [np.ascontiguousarray(doc_len, dtype=np.uint32), np.ascontiguousarray(post_off, dtype=np.uint64),
-                np.ascontiguousarray(post_doc, dtype=np.uint32), np.ascontiguousarray(post_tf, dtype=np.uint32)]
-        c = _Corpus()
-        c.n_docs, c.n_terms, c.k1, c.b = int(n_docs), int(n_terms), float(k1), float(b)
-        c.doc_len, c.post_off = _p(keep[0], C.c_uint32), _p(keep[1], C.c_uint64)
-        c.post_doc, c.post_tf = _p(keep[2], C.c_uint32), _p(keep[3], C.c_uint32)
-        if payload is not None:
-            keep.append(np.ascontiguousarray(payload, dtype=np.uint16))
-            c.payload = _p(keep[-1], C.c_uint16)
-        if term_keys is not None:
-            keep.append(np.ascontiguousarray(term_keys, dtype=np.uint8))
-            c.term_key = _p(keep[-1], C.c_uint8)
+        keep = []
+        c = _corpus(keep, n_docs, doc_len, n_terms, post_off, post_doc, post_tf, k1, b, payload, term_keys)
         bounds = np.ascontiguousarray(doc_bounds, dtype=np.uint32) if doc_bounds is not None else None
         devs = (C.c_int * int(n_shards))(*[int(d) for d in devices]) if devices is not None else None
         self.h = C.c_void_p()
-        _check(L.bm25x_sharded_create(C.byref(c), int(n_shards), _p(bounds, C.c_uint32), devs, C.byref(self.h)))
+        _check(load_library().bm25x_sharded_create(C.byref(c), int(n_shards), _p(bounds, C.c_uint32), devs,
+                                                   C.byref(self.h)))
         self.n_docs, self.n_terms = int(n_docs), int(n_terms)
 
     @staticmethod
@@ -595,20 +573,8 @@ class ShardedIndex:
         return out
 
     def search_batch(self, q_off, q_terms, k, allow=None, want_f64=True, want_payload=False, out=None):
-        q_off = np.ascontiguousarray(q_off, dtype=np.uint32)
-        q_terms = np.ascontiguousarray(q_terms, dtype=np.uint32)
-        nq = len(q_off) - 1
-        if out is None:
-            out = _result_arrays(nq, max(int(k), 1), want_f64, want_payload)
-        al = np.ascontiguousarray(allow, dtype=np.uint8) if allow is not None else None
-        st = SearchStats()
-        _check(load_library().bm25x_sharded_search_batch(self.h, nq, _p(q_off, C.c_uint32), _p(q_terms, C.c_uint32),
-                                                         int(k), _p(al, C.c_uint8), _p(out["doc"], C.c_uint32),
-                                                         _p(out["score"], C.c_float), _p(out["score64"], C.c_double),
-                                                         _p(out["payload"], C.c_uint16), _p(out["n"], C.c_uint32),
-                                                         C.byref(st)))
-        out["stats"] = st
-        return out
+        return _search_batch(load_library().bm25x_sharded_search_batch, self.h, q_off, q_terms, k, allow, want_f64,
+                             want_payload, out)
 
 
 def merge_shards(rows, doc_base, k, device=0):
@@ -650,10 +616,7 @@ class Batch:
         return st
 
     def fetch(self, want_f64=True, want_payload=False):
-        out = {"doc": np.empty((self.nq, self.k), np.uint32), "score": np.empty((self.nq, self.k), np.float32),
-               "score64": np.empty((self.nq, self.k), np.float64) if want_f64 else None,
-               "payload": np.empty((self.nq, self.k, 3), np.uint16) if want_payload else None,
-               "n": np.empty(self.nq, np.uint32)}
+        out = _result_arrays(self.nq, self.k, want_f64, want_payload)
         _check(load_library().bm25x_batch_fetch(self.h, _p(out["doc"], C.c_uint32), _p(out["score"], C.c_float),
                                                 _p(out["score64"], C.c_double), _p(out["payload"], C.c_uint16),
                                                 _p(out["n"], C.c_uint32)))

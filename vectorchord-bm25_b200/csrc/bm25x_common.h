@@ -4,6 +4,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
+#include <array>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -123,8 +126,92 @@ struct bm25x_sharded_index {
     std::vector<uint32_t> h_df;
 };
 
-// Internal, for bm25x_sharded_search_batch (bm25x_search.cu): a run of a prepared batch on its index's stream between the
-// batch's timing events, without synchronising; after it has finished, its figures added to *acc.
+// ---- internal to the host library (bm25x_search.cu, bm25x_shards.cu) ----
+
+// Canonical queries (sort + dedup: datatype/tsvector.rs:96-105; unknown and df-0 terms dropped: search.rs:55-62).  Query i
+// of q_off[0..nq] (absolute offsets into q_terms: q_off may be a slice of a longer array) keeps its live terms in place of
+// its raw ones, at terms[q_off[i] - q_off[0]]; a query of 33..64 live terms holds its 32 rarest first, both groups
+// ascending.  Refuses offsets that go backwards and more than BM25X_MAX_QUERY_TERMS live terms with the messages of
+// bm25x_batch_prepare, naming the highest-numbered offending query of the slice.
+struct CanonQueries {
+    std::unique_ptr<uint32_t[]> terms;
+    std::unique_ptr<uint32_t[]> live;  // live terms per query
+    std::unique_ptr<uint64_t[]> cost;  // Σ df per query
+};
+int bm25x_canonicalise(const uint32_t *h_df, uint32_t n_terms, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms,
+                       CanonQueries *out);
+
+// The slices bm25x_search_batch cuts a batch of nq queries into: min(16, nq / slice_min) of them when nq >= 2 x slice_min
+// (slice_min != 0), else one.  Slice s holds the queries [begin(s), begin(s + 1)).
+struct SlicePlan {
+    uint32_t nq, n;
+    SlicePlan(uint32_t slice_min, uint32_t nq_)
+        : nq(nq_), n(slice_min && nq_ >= 2ull * slice_min ? std::min<uint32_t>(16u, nq_ / slice_min) : 1u) {}
+    uint32_t begin(uint32_t s) const { return (uint32_t)(((uint64_t)nq * s) / n); }
+};
+
+// Result rows of a batch: per query k slots of doc id, f32 score, f64 score and payload (3 x u16), and the count n of
+// filled slots.  An empty slot is doc BM25X_DOC_INF with zeros elsewhere.  Pointers are device or host memory.
+struct ResultRows {
+    uint32_t *doc = nullptr;
+    float *score = nullptr;
+    double *score64 = nullptr;
+    uint16_t *payload = nullptr;
+    uint32_t *n = nullptr;
+
+    // bytes of the five arrays for `rows` queries
+    static std::array<size_t, 5> bytes(size_t rows, uint32_t k) {
+        const size_t slots = rows * k;
+        return {4 * slots, 4 * slots, 8 * slots, 6 * slots, 4 * rows};
+    }
+    std::array<void *, 5> arrays() const { return {doc, score, score64, payload, n}; }
+    // the rows from query `row` on (null arrays stay null)
+    ResultRows from(size_t row, uint32_t k) const {
+        ResultRows r;
+        if (doc) r.doc = doc + row * k;
+        if (score) r.score = score + row * k;
+        if (score64) r.score64 = score64 + row * k;
+        if (payload) r.payload = payload + row * k * 3;
+        if (n) r.n = n + row;
+        return r;
+    }
+    // stream-ordered device memory for `rows` queries
+    cudaError_t alloc(size_t rows, uint32_t k, cudaStream_t st) {
+        void **p[5] = {(void **)&doc, (void **)&score, (void **)&score64, (void **)&payload, (void **)&n};
+        const auto b = bytes(rows, k);
+        cudaError_t e = cudaSuccess;
+        for (int a = 0; a < 5 && e == cudaSuccess; a++) e = cudaMallocAsync(p[a], b[a] ? b[a] : 8, st);
+        return e;
+    }
+    void release(cudaStream_t st) {
+        for (void *p : arrays())
+            if (p) cudaFreeAsync(p, st);
+        *this = ResultRows();
+    }
+    // every slot empty, every count 0
+    cudaError_t reset(size_t rows, uint32_t k, cudaStream_t st) const {
+        const auto p = arrays();
+        const auto b = bytes(rows, k);
+        cudaError_t e = cudaSuccess;
+        for (int a = 0; a < 5 && e == cudaSuccess; a++) e = cudaMemsetAsync(p[a], a == 0 ? 0xFF : 0, b[a], st);
+        return e;
+    }
+    // the first `rows` queries into dst (host memory or another device's: the copy kind follows the addresses), skipping
+    // the arrays dst leaves null
+    cudaError_t copy_to(const ResultRows &dst, size_t rows, uint32_t k, cudaStream_t st) const {
+        const auto s = arrays(), d = dst.arrays();
+        const auto b = bytes(rows, k);
+        cudaError_t e = cudaSuccess;
+        for (int a = 0; a < 5 && e == cudaSuccess; a++)
+            if (d[a] && b[a]) e = cudaMemcpyAsync(d[a], s[a], b[a], cudaMemcpyDefault, st);
+        return e;
+    }
+};
+
+// A prepared batch (bm25x_batch_prepare) seen from the sharded search: its output rows; a run on its index's stream between
+// the batch's timing events, without synchronising; the event that closes that run; after it has finished, its figures
+// added to *acc.
+const ResultRows &bm25x_batch_rows(const bm25x_batch *b);
 int bm25x_batch_run_timed(bm25x_batch *b);
-int bm25x_batch_add_stats(bm25x_batch *b, bm25x_search_stats *acc);
 cudaEvent_t bm25x_batch_done_event(bm25x_batch *b);
+int bm25x_batch_add_stats(bm25x_batch *b, bm25x_search_stats *acc);

@@ -87,14 +87,11 @@ struct bm25x_batch {
     uint32_t nq = 0, k = 0;
     Group groups[kNumClasses];
     uint8_t *d_allow = nullptr;
-    uint32_t *d_out_doc = nullptr;
-    float *d_out_score = nullptr;
-    double *d_out_score64 = nullptr;
-    uint16_t *d_out_payload = nullptr;
-    uint32_t *d_out_n = nullptr;
+    ResultRows out;  // [nq] rows of k slots on the device
     unsigned long long *d_fetched = nullptr;
     uint64_t postings = 0, qterms = 0;
     uint32_t live = 0;
+    uint32_t launches = 0;  // issued by the last run
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev_ready = nullptr;
     std::vector<void *> allocs;
     void *last_stream = nullptr;
@@ -135,6 +132,7 @@ extern "C" void bm25x_batch_destroy(bm25x_batch *b) {
     cudaSetDevice(b->ix->device);
     if (b->last_stream && b->last_stream != (void *)b->ix->stream) cudaStreamSynchronize((cudaStream_t)b->last_stream);
     for (void *p : b->allocs) cudaFreeAsync(p, b->ix->stream);
+    b->out.release(b->ix->stream);
     if (b->ev0) cudaEventDestroy(b->ev0);
     if (b->ev1) cudaEventDestroy(b->ev1);
     if (b->ev_ready) cudaEventDestroy(b->ev_ready);
@@ -150,9 +148,65 @@ extern "C" void bm25x_batch_destroy(bm25x_batch *b) {
         }                            \
     } while (0)
 
-// Canonicalises the queries (sort + dedup: datatype/tsvector.rs:96-105; unknown tokens dropped: search.rs:55-62), groups
-// them by term-count class and uploads everything with ONE copy from a page-locked staging buffer cached in the index
-// handle.  OpenMP over the queries; no per-query allocation.
+// OpenMP over the queries; no per-query allocation.
+int bm25x_canonicalise(const uint32_t *h_df, uint32_t n_terms, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms,
+                       CanonQueries *out) {
+    const size_t base0 = nq ? q_off[0] : 0;
+    const size_t n_raw = nq && q_off[nq] >= base0 ? q_off[nq] - base0 : 0;
+    // not zeroed: the loop writes every query's entries (the first touch of the pages is spread over the threads)
+    out->terms.reset(new uint32_t[n_raw ? n_raw : 1]);
+    out->live.reset(new uint32_t[nq ? nq : 1]);
+    out->cost.reset(new uint64_t[nq ? nq : 1]);
+    uint32_t *const canon = out->terms.get(), *const live = out->live.get();
+    uint64_t *const cost = out->cost.get();
+    int bad = -1;  // the highest-numbered offending query, whatever the thread count
+    const int nthr = nq < 4096 ? 1 : bm25x_host_threads(16);  // small batches: a parallel region costs more than the loop
+#pragma omp parallel for schedule(static, 1024) num_threads(nthr) reduction(max : bad)
+    for (uint32_t i = 0; i < nq; ++i) {
+        if (q_off[i + 1] < q_off[i] || q_off[i] < base0 || q_off[i + 1] - base0 > n_raw) {
+            bad = std::max(bad, (int)i);
+            live[i] = 0;
+            cost[i] = 0;
+            continue;
+        }
+        uint32_t *dst = canon + (q_off[i] - base0);
+        const uint32_t n = q_off[i + 1] - q_off[i];
+        uint32_t m = 0;
+        for (uint32_t j = 0; j < n; ++j) {
+            const uint32_t t = q_terms[q_off[i] + j];
+            if (t < n_terms && h_df[t] != 0) dst[m++] = t;
+        }
+        std::sort(dst, dst + m);
+        m = (uint32_t)(std::unique(dst, dst + m) - dst);
+        uint64_t cst = 0;
+        for (uint32_t j = 0; j < m; ++j) cst += h_df[dst[j]];
+        cost[i] = cst;
+        if (m > 32 && m <= BM25X_MAX_QUERY_TERMS) {
+            // two-pass query: the 32 rarest terms first (group 0, streamed by the first pass), the others after them;
+            // both groups ascending — the kernel merges them back into ascending term order for the exact sum
+            uint32_t tmp[BM25X_MAX_QUERY_TERMS];
+            std::copy(dst, dst + m, tmp);
+            std::nth_element(tmp, tmp + 32, tmp + m, [&](uint32_t a, uint32_t b) {
+                return h_df[a] != h_df[b] ? h_df[a] < h_df[b] : a < b;
+            });
+            std::sort(tmp, tmp + 32);
+            std::sort(tmp + 32, tmp + m);
+            std::copy(tmp, tmp + m, dst);
+        }
+        if (m > BM25X_MAX_QUERY_TERMS) bad = std::max(bad, (int)i);
+        live[i] = m;
+    }
+    if (bad < 0) return BM25X_OK;
+    if (live[bad] == 0) {  // offsets (a query with too many live terms has more than 0)
+        bm25x_set_error("bm25x_batch_prepare: q_off not monotone at %d", bad);
+        return BM25X_ERR_INVALID;
+    }
+    bm25x_set_error("bm25x_batch_prepare: query %d has %u live terms > %d", bad, live[bad], BM25X_MAX_QUERY_TERMS);
+    return BM25X_ERR_UNSUPPORTED;
+}
+
+// Canonicalises the queries (bm25x_canonicalise), groups them by term-count class and uploads everything with ONE copy
+// from a page-locked staging buffer cached in the index handle.
 extern "C" int bm25x_batch_prepare(bm25x_index *ix, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms,
                                    uint32_t k, const uint8_t *allow, bm25x_batch **out) {
     if (!ix || !out || (nq && (!q_off || (!q_terms && q_off[nq] != 0)))) {
@@ -172,64 +226,14 @@ extern "C" int bm25x_batch_prepare(bm25x_index *ix, uint32_t nq, const uint32_t 
         bm25x_set_error("bm25x_batch_prepare: k=%u > BM25X_MAX_K=%d", k, BM25X_MAX_K);
         return BM25X_ERR_UNSUPPORTED;
     }
-    const uint32_t T = ix->d.n_terms;
     const uint32_t *h_df = ix->h_df.data();
-    // ---- pass 1 (parallel): canonical terms of query i written in place of its raw terms (never longer) ----
-    // (q_off may be a slice of a longer offset array: offsets are absolute into q_terms, the scratch is relative to base0)
+    CanonQueries cq;
+    const int crc = bm25x_canonicalise(h_df, ix->d.n_terms, nq, q_off, q_terms, &cq);
+    if (crc != BM25X_OK) return crc;
     const size_t base0 = nq ? q_off[0] : 0;
-    const size_t n_raw = nq && q_off[nq] >= base0 ? q_off[nq] - base0 : 0;
-    std::vector<uint32_t> canon(n_raw ? n_raw : 1);
-    std::vector<uint32_t> live(nq ? nq : 1);  // live terms of query i
-    std::vector<uint64_t> cost(nq ? nq : 1);  // Σ df of query i
-    int bad_query = -1, bad_kind = 0;
-    const int nthr = nq < 4096 ? 1 : bm25x_host_threads(16);  // small batches: a parallel region costs more than the loop
-#pragma omp parallel for schedule(static, 1024) num_threads(nthr)
-    for (uint32_t i = 0; i < nq; ++i) {
-        if (q_off[i + 1] < q_off[i] || q_off[i] < base0 || q_off[i + 1] - base0 > n_raw) {
-#pragma omp critical
-            { bad_query = (int)i; bad_kind = 1; }
-            live[i] = 0;
-            continue;
-        }
-        uint32_t *dst = canon.data() + (q_off[i] - base0);
-        const uint32_t n = q_off[i + 1] - q_off[i];
-        uint32_t m = 0;
-        for (uint32_t j = 0; j < n; ++j) {
-            const uint32_t t = q_terms[q_off[i] + j];
-            if (t < T && h_df[t] != 0) dst[m++] = t;
-        }
-        std::sort(dst, dst + m);
-        m = (uint32_t)(std::unique(dst, dst + m) - dst);
-        uint64_t cst = 0;
-        for (uint32_t j = 0; j < m; ++j) cst += h_df[dst[j]];
-        cost[i] = cst;
-        if (m > 32 && m <= BM25X_MAX_QUERY_TERMS) {
-            // two-pass query: the 32 rarest terms first (group 0, streamed by the first pass), the others after them;
-            // both groups ascending — the kernel merges them back into ascending term order for the exact sum
-            uint32_t tmp[BM25X_MAX_QUERY_TERMS];
-            std::copy(dst, dst + m, tmp);
-            std::nth_element(tmp, tmp + 32, tmp + m, [&](uint32_t a, uint32_t b) {
-                return h_df[a] != h_df[b] ? h_df[a] < h_df[b] : a < b;
-            });
-            std::sort(tmp, tmp + 32);
-            std::sort(tmp + 32, tmp + m);
-            std::copy(tmp, tmp + m, dst);
-        }
-        if (m > BM25X_MAX_QUERY_TERMS) {
-#pragma omp critical
-            { bad_query = (int)i; bad_kind = 2; }
-        }
-        live[i] = m;
-    }
-    if (bad_query >= 0) {
-        if (bad_kind == 1) {
-            bm25x_set_error("bm25x_batch_prepare: q_off not monotone at %d", bad_query);
-            return BM25X_ERR_INVALID;
-        }
-        bm25x_set_error("bm25x_batch_prepare: query %d has %u live terms > %d", bad_query, live[bad_query],
-                        BM25X_MAX_QUERY_TERMS);
-        return BM25X_ERR_UNSUPPORTED;
-    }
+    const uint32_t *const canon = cq.terms.get(), *const live = cq.live.get();
+    const uint64_t *const cost = cq.cost.get();
+    const int nthr = nq < 4096 ? 1 : bm25x_host_threads(16);
     bm25x_batch *b = new bm25x_batch();
     b->ix = ix;
     b->nq = nq;
@@ -339,7 +343,7 @@ extern "C" int bm25x_batch_prepare(bm25x_index *ix, uint32_t nq, const uint32_t 
         const int c = cls_of[m];
         hs[base_ids[c] + slot[i]] = i;
         hs[base_off[c] + slot[i] + 1] = tpos[i] + m;
-        const uint32_t *src = canon.data() + (q_off[i] - base0);
+        const uint32_t *src = canon + (q_off[i] - base0);
         uint32_t *dst = hs + base_terms[c] + tpos[i];
         for (uint32_t j = 0; j < m; ++j) {
             dst[j] = src[j];
@@ -374,20 +378,9 @@ extern "C" int bm25x_batch_prepare(bm25x_index *ix, uint32_t nq, const uint32_t 
             if (two_phase_class(ix, g.M, k)) BTRY(batch_alloc(b, &g.d_resume, (size_t)g.nq));
         }
     }
-    size_t slots = (size_t)nq * k;
-    if (slots == 0) slots = 1;
-    BTRY(batch_alloc(b, &b->d_out_doc, slots));
-    BTRY(batch_alloc(b, &b->d_out_score, slots));
-    BTRY(batch_alloc(b, &b->d_out_score64, slots));
-    BTRY(batch_alloc(b, &b->d_out_payload, slots * 3));
-    BTRY(batch_alloc(b, &b->d_out_n, nq));
     BTRY(batch_alloc(b, &b->d_fetched, 1));
-    // rows of queries without a live term are never written by a kernel
-    if (e == cudaSuccess) e = cudaMemsetAsync(b->d_out_n, 0, 4 * (size_t)(nq ? nq : 1), st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(b->d_out_doc, 0xFF, 4 * slots, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(b->d_out_score, 0, 4 * slots, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(b->d_out_score64, 0, 8 * slots, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(b->d_out_payload, 0, 6 * slots, st);
+    if (e == cudaSuccess) e = b->out.alloc(nq, k, st);
+    if (e == cudaSuccess) e = b->out.reset(nq, k, st);  // rows of queries without a live term are never written by a kernel
     if (e == cudaSuccess) e = cudaEventCreate(&b->ev0);
     if (e == cudaSuccess) e = cudaEventCreate(&b->ev1);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&b->ev_ready, cudaEventDisableTiming);
@@ -395,25 +388,22 @@ extern "C" int bm25x_batch_prepare(bm25x_index *ix, uint32_t nq, const uint32_t 
     if (e != cudaSuccess) {
         bm25x_set_error("bm25x_batch_prepare: %s", cudaGetErrorString(e));
         bm25x_batch_destroy(b);
-        return BM25X_ERR_CUDA;
+        return e == cudaErrorMemoryAllocation ? BM25X_ERR_OOM : BM25X_ERR_CUDA;
     }
     *out = b;
     return BM25X_OK;
 }
 
-extern "C" int bm25x_batch_run(bm25x_batch *b, void *stream_v, bm25x_search_stats *stats) {
-    if (!b) {
-        bm25x_set_error("bm25x_batch_run: null batch");
-        return BM25X_ERR_INVALID;
-    }
+// The launches of one run on st, counted in b->launches.  Timed: the fetched-postings counter is zeroed and the run sits
+// between the batch's events ev0 and ev1.  Does not synchronise.
+static int batch_enqueue(bm25x_batch *b, cudaStream_t st, bool timed) {
     bm25x_index *ix = b->ix;
     BM25X_CUDA_TRY(cudaSetDevice(ix->device));
-    cudaStream_t st = stream_v ? (cudaStream_t)stream_v : ix->stream;
     b->last_stream = (void *)st;
     if (st != ix->stream) BM25X_CUDA_TRY(cudaStreamWaitEvent(st, b->ev_ready, 0));  // uploads were issued on the library's stream
     const DeviceIndex &d = ix->d;
     uint32_t launches = 0;
-    if (stats) {
+    if (timed) {
         BM25X_CUDA_TRY(cudaMemsetAsync(b->d_fetched, 0, sizeof(unsigned long long), st));
         BM25X_CUDA_TRY(cudaEventRecord(b->ev0, st));
     }
@@ -449,11 +439,11 @@ extern "C" int bm25x_batch_run(bm25x_batch *b, void *stream_v, bm25x_search_stat
         sp.k = b->k;
         sp.allow = b->d_allow;
         sp.work_counter = g.d_counter;
-        sp.out_doc = b->d_out_doc;
-        sp.out_score = b->d_out_score;
-        sp.out_score64 = b->d_out_score64;
-        sp.out_payload = b->d_out_payload;
-        sp.out_n = b->d_out_n;
+        sp.out_doc = b->out.doc;
+        sp.out_score = b->out.score;
+        sp.out_score64 = b->out.score64;
+        sp.out_payload = b->out.payload;
+        sp.out_n = b->out.n;
         BM25X_CUDA_TRY(cudaMemsetAsync(g.d_counter, 0, sizeof(int), st));
         sp.q2 = g.d_q2;
         sp.resume = g.d_resume;
@@ -480,23 +470,21 @@ extern "C" int bm25x_batch_run(bm25x_batch *b, void *stream_v, bm25x_search_stat
         if (rc != BM25X_OK) return rc;
         launches++;
     }
-    if (stats) {
-        BM25X_CUDA_TRY(cudaEventRecord(b->ev1, st));
-        BM25X_CUDA_TRY(cudaEventSynchronize(b->ev1));
-        float ms = 0.f;
-        BM25X_CUDA_TRY(cudaEventElapsedTime(&ms, b->ev0, b->ev1));
-        memset(stats, 0, sizeof(*stats));
-        stats->kernel_ms = ms;
-        stats->postings = b->postings;
-        stats->bytes_algo = 8ull * b->postings + 8ull * (uint64_t)b->live * b->k + 16ull * b->qterms;
-        stats->launches = launches;
-        stats->queries = b->live;
-        unsigned long long fetched = 0;
-        BM25X_CUDA_TRY(cudaMemcpyAsync(&fetched, b->d_fetched, sizeof(fetched), cudaMemcpyDeviceToHost, st));
-        BM25X_CUDA_TRY(cudaStreamSynchronize(st));
-        stats->postings_fetched = fetched;  // 0 for the CTA kernel (always exhaustive)
-    }
+    b->launches = launches;
+    if (timed) BM25X_CUDA_TRY(cudaEventRecord(b->ev1, st));
     return BM25X_OK;
+}
+
+extern "C" int bm25x_batch_run(bm25x_batch *b, void *stream_v, bm25x_search_stats *stats) {
+    if (!b) {
+        bm25x_set_error("bm25x_batch_run: null batch");
+        return BM25X_ERR_INVALID;
+    }
+    const int rc = batch_enqueue(b, stream_v ? (cudaStream_t)stream_v : b->ix->stream, stats != nullptr);
+    if (rc != BM25X_OK || !stats) return rc;
+    BM25X_CUDA_TRY(cudaEventSynchronize(b->ev1));
+    memset(stats, 0, sizeof(*stats));
+    return bm25x_batch_add_stats(b, stats);
 }
 
 extern "C" int bm25x_batch_fetch(bm25x_batch *b, uint32_t *out_doc, float *out_score, double *out_score64,
@@ -507,12 +495,8 @@ extern "C" int bm25x_batch_fetch(bm25x_batch *b, uint32_t *out_doc, float *out_s
     }
     BM25X_CUDA_TRY(cudaSetDevice(b->ix->device));
     cudaStream_t st = b->last_stream ? (cudaStream_t)b->last_stream : b->ix->stream;
-    size_t slots = (size_t)b->nq * b->k;
-    if (out_doc) BM25X_CUDA_TRY(cudaMemcpyAsync(out_doc, b->d_out_doc, 4 * slots, cudaMemcpyDeviceToHost, st));
-    if (out_score) BM25X_CUDA_TRY(cudaMemcpyAsync(out_score, b->d_out_score, 4 * slots, cudaMemcpyDeviceToHost, st));
-    if (out_score64) BM25X_CUDA_TRY(cudaMemcpyAsync(out_score64, b->d_out_score64, 8 * slots, cudaMemcpyDeviceToHost, st));
-    if (out_payload) BM25X_CUDA_TRY(cudaMemcpyAsync(out_payload, b->d_out_payload, 6 * slots, cudaMemcpyDeviceToHost, st));
-    if (out_n) BM25X_CUDA_TRY(cudaMemcpyAsync(out_n, b->d_out_n, 4 * (size_t)b->nq, cudaMemcpyDeviceToHost, st));
+    const ResultRows host{out_doc, out_score, out_score64, out_payload, out_n};
+    BM25X_CUDA_TRY(b->out.copy_to(host, b->nq, b->k, st));
     BM25X_CUDA_TRY(cudaStreamSynchronize(st));
     return BM25X_OK;
 }
@@ -523,54 +507,44 @@ extern "C" int bm25x_batch_device_results(bm25x_batch *b, void **doc, void **sco
         bm25x_set_error("bm25x_batch_device_results: null batch");
         return BM25X_ERR_INVALID;
     }
-    if (doc) *doc = b->d_out_doc;
-    if (score) *score = b->d_out_score;
-    if (score64) *score64 = b->d_out_score64;
-    if (payload) *payload = b->d_out_payload;
-    if (n) *n = b->d_out_n;
+    void **dst[5] = {doc, score, score64, payload, n};
+    const auto p = b->out.arrays();
+    for (int a = 0; a < 5; a++)
+        if (dst[a]) *dst[a] = p[a];
     return BM25X_OK;
 }
 
-// Timing events around an asynchronous run on the index's stream (the slices of search_batch_sliced, the shards of
-// bm25x_sharded_search_batch); bm25x_batch_add_stats reads them once the run has finished.
-int bm25x_batch_run_timed(bm25x_batch *b) {
-    bm25x_index *ix = b->ix;
-    BM25X_CUDA_TRY(cudaSetDevice(ix->device));
-    BM25X_CUDA_TRY(cudaMemsetAsync(b->d_fetched, 0, sizeof(unsigned long long), ix->stream));
-    BM25X_CUDA_TRY(cudaEventRecord(b->ev0, ix->stream));
-    const int rc = bm25x_batch_run(b, nullptr, nullptr);
-    if (rc != BM25X_OK) return rc;
-    BM25X_CUDA_TRY(cudaEventRecord(b->ev1, ix->stream));
-    return BM25X_OK;
-}
+const ResultRows &bm25x_batch_rows(const bm25x_batch *b) { return b->out; }
+
+// An asynchronous timed run on the index's stream (the slices of search_batch_sliced, the shards of
+// bm25x_sharded_search_batch); bm25x_batch_add_stats reads its figures once it has finished.
+int bm25x_batch_run_timed(bm25x_batch *b) { return batch_enqueue(b, b->ix->stream, true); }
 
 cudaEvent_t bm25x_batch_done_event(bm25x_batch *b) { return b->ev1; }
 
+// The figures of the batch's last timed run, added to *acc (bm25x_batch_run fills a zeroed one).
 int bm25x_batch_add_stats(bm25x_batch *b, bm25x_search_stats *acc) {
     BM25X_CUDA_TRY(cudaSetDevice(b->ix->device));
     float ms = 0.f;
     unsigned long long fetched = 0;
     BM25X_CUDA_TRY(cudaEventElapsedTime(&ms, b->ev0, b->ev1));
     BM25X_CUDA_TRY(cudaMemcpy(&fetched, b->d_fetched, sizeof(fetched), cudaMemcpyDeviceToHost));
-    uint32_t launches = 0;
-    for (int c = 0; c < kNumClasses; ++c)
-        if (b->groups[c].nq) launches += b->groups[c].d_q2 ? 2u : 1u;
     acc->kernel_ms += ms;
     acc->postings += b->postings;
     acc->bytes_algo += 8ull * b->postings + 8ull * (uint64_t)b->live * b->k + 16ull * b->qterms;
-    acc->launches += launches;
+    acc->launches += b->launches;
     acc->queries += b->live;
-    acc->postings_fetched += fetched;
+    acc->postings_fetched += fetched;  // 0 for the CTA kernel (always exhaustive)
     return BM25X_OK;
 }
 
 // Large batches run as a pipeline of slices: while slice s is on the GPU the host canonicalises and uploads slice s + 1,
 // and the results of slice s - 1 travel to the host on a second stream.  Same results, row for row.
-static int search_batch_sliced(bm25x_index *ix, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms, uint32_t k,
-                               const uint8_t *allow, uint32_t *out_doc, float *out_score, double *out_score64,
-                               uint16_t *out_payload, uint32_t *out_n, bm25x_search_stats *stats, uint32_t n_slices) {
+static int search_batch_sliced(bm25x_index *ix, const SlicePlan &plan, const uint32_t *q_off, const uint32_t *q_terms,
+                               uint32_t k, const uint8_t *allow, const ResultRows &host, bm25x_search_stats *stats) {
     using clk = std::chrono::steady_clock;
     BM25X_CUDA_TRY(cudaSetDevice(ix->device));
+    const uint32_t n_slices = plan.n;
     std::vector<bm25x_batch *> bs(n_slices, nullptr);
     std::vector<cudaEvent_t> done(n_slices, nullptr);
     int rc = BM25X_OK;
@@ -585,25 +559,19 @@ static int search_batch_sliced(bm25x_index *ix, uint32_t nq, const uint32_t *q_o
         return code;
     };
     for (uint32_t s = 0; s < n_slices && rc == BM25X_OK; ++s) {
-        const uint32_t a = (uint32_t)(((uint64_t)nq * s) / n_slices), e = (uint32_t)(((uint64_t)nq * (s + 1)) / n_slices);
+        const uint32_t a = plan.begin(s), e = plan.begin(s + 1);
         const auto t0 = clk::now();
         // (q_off + a holds absolute offsets into q_terms: the slice is prepared in place)
         rc = bm25x_batch_prepare(ix, e - a, q_off + a, q_terms, k, allow, &bs[s]);
         host_ms += std::chrono::duration<double, std::milli>(clk::now() - t0).count();
         if (rc != BM25X_OK) break;
         bm25x_batch *b = bs[s];
-        rc = stats ? bm25x_batch_run_timed(b) : bm25x_batch_run(b, nullptr, nullptr);
+        rc = batch_enqueue(b, ix->stream, stats != nullptr);
         if (rc != BM25X_OK) break;
         cudaError_t ce = cudaEventCreateWithFlags(&done[s], cudaEventDisableTiming);
         if (ce == cudaSuccess) ce = cudaEventRecord(done[s], ix->stream);
         if (ce == cudaSuccess) ce = cudaStreamWaitEvent(ix->copy_stream, done[s], 0);
-        const size_t slots = (size_t)(e - a) * k, o = (size_t)a * k;
-        cudaStream_t cs = ix->copy_stream;
-        if (ce == cudaSuccess && out_doc) ce = cudaMemcpyAsync(out_doc + o, b->d_out_doc, 4 * slots, cudaMemcpyDeviceToHost, cs);
-        if (ce == cudaSuccess && out_score) ce = cudaMemcpyAsync(out_score + o, b->d_out_score, 4 * slots, cudaMemcpyDeviceToHost, cs);
-        if (ce == cudaSuccess && out_score64) ce = cudaMemcpyAsync(out_score64 + o, b->d_out_score64, 8 * slots, cudaMemcpyDeviceToHost, cs);
-        if (ce == cudaSuccess && out_payload) ce = cudaMemcpyAsync(out_payload + 3 * o, b->d_out_payload, 6 * slots, cudaMemcpyDeviceToHost, cs);
-        if (ce == cudaSuccess && out_n) ce = cudaMemcpyAsync(out_n + a, b->d_out_n, 4 * (size_t)(e - a), cudaMemcpyDeviceToHost, cs);
+        if (ce == cudaSuccess) ce = b->out.copy_to(host.from(a, k), e - a, k, ix->copy_stream);
         if (ce != cudaSuccess) {
             bm25x_set_error("bm25x_search_batch (slice %u): %s", s, cudaGetErrorString(ce));
             return fail(BM25X_ERR_CUDA);
@@ -637,10 +605,11 @@ extern "C" int bm25x_search_batch(bm25x_index *ix, uint32_t nq, const uint32_t *
                                   double *out_score64, uint16_t *out_payload, uint32_t *out_n,
                                   bm25x_search_stats *stats) {
     using clk = std::chrono::steady_clock;
-    if (ix && ix->slice_min && nq >= 2ull * ix->slice_min && q_off && k != 0) {
-        const uint32_t n_slices = std::min<uint32_t>(16u, nq / ix->slice_min);
-        return search_batch_sliced(ix, nq, q_off, q_terms, k, allow, out_doc, out_score, out_score64, out_payload, out_n,
-                                   stats, n_slices);
+    if (ix && q_off && k != 0) {
+        const SlicePlan plan(ix->slice_min, nq);
+        if (plan.n > 1)
+            return search_batch_sliced(ix, plan, q_off, q_terms, k, allow,
+                                       {out_doc, out_score, out_score64, out_payload, out_n}, stats);
     }
     bm25x_batch *b = nullptr;
     const auto t0 = clk::now();
@@ -703,6 +672,18 @@ extern "C" int bm25x_merge_topk(uint32_t nq, uint32_t k, const uint32_t *doc_a, 
     return BM25X_OK;
 }
 
+// Two searches of the same queries (sealed, growing) as one: times and work add up, `queries` is the first one's.
+static void add_work(bm25x_search_stats *out, const bm25x_search_stats &a, const bm25x_search_stats &b) {
+    *out = a;
+    out->kernel_ms += b.kernel_ms;
+    out->h2d_ms += b.h2d_ms;
+    out->d2h_ms += b.d2h_ms;
+    out->postings += b.postings;
+    out->bytes_algo += b.bytes_algo;
+    out->launches += b.launches;
+    out->postings_fetched += b.postings_fetched;
+}
+
 extern "C" int bm25x_search_batch_growing(bm25x_index *sealed, bm25x_index *growing, uint32_t nq, const uint32_t *q_off,
                                           const uint32_t *q_terms, uint32_t k, const uint8_t *allow_sealed,
                                           const uint8_t *allow_growing, uint32_t *out_doc, float *out_score,
@@ -737,16 +718,7 @@ extern "C" int bm25x_search_batch_growing(bm25x_index *sealed, bm25x_index *grow
                                           sc64[s].data(), out_payload ? pay[s].data() : nullptr, n[s].data(), &st[s]);
         if (rc != BM25X_OK) return rc;
     }
-    if (stats) {
-        *stats = st[0];
-        stats->kernel_ms += st[1].kernel_ms;
-        stats->h2d_ms += st[1].h2d_ms;
-        stats->d2h_ms += st[1].d2h_ms;
-        stats->postings += st[1].postings;
-        stats->bytes_algo += st[1].bytes_algo;
-        stats->launches += st[1].launches;
-        stats->postings_fetched += st[1].postings_fetched;
-    }
+    if (stats) add_work(stats, st[0], st[1]);
     return bm25x_merge_topk(nq, k, doc[0].data(), sc[0].data(), sc64[0].data(), out_payload ? pay[0].data() : nullptr,
                             n[0].data(), doc[1].data(), sc[1].data(), sc64[1].data(),
                             out_payload ? pay[1].data() : nullptr, n[1].data(), sealed->d.n_docs, out_doc, out_score,

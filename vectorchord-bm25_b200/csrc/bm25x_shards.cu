@@ -80,52 +80,27 @@ __global__ void k_merge_shards(ShardRows in, uint32_t S, uint32_t nq, uint32_t k
     }
 }
 
-int launch_merge(int device, const ShardRows &in, uint32_t S, uint32_t nq, uint32_t k, uint32_t *doc, float *score,
-                 double *score64, uint16_t *payload, uint32_t *n, cudaStream_t st) {
+int launch_merge(int device, const ShardRows &in, uint32_t S, uint32_t nq, uint32_t k, const ResultRows &out,
+                 cudaStream_t st) {
     const uint64_t total = (uint64_t)nq * S * k;
     if (!total) return BM25X_OK;
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
     const uint64_t want = (total + 255) / 256, cap = (uint64_t)sms * 32;
-    k_merge_shards<<<(unsigned)std::min(want, cap), 256, 0, st>>>(in, S, nq, k, doc, score, score64, payload, n);
+    k_merge_shards<<<(unsigned)std::min(want, cap), 256, 0, st>>>(in, S, nq, k, out.doc, out.score, out.score64,
+                                                                  out.payload, out.n);
     BM25X_CUDA_TRY(cudaGetLastError());
     return BM25X_OK;
 }
 
-// Device result buffers of the merge ([nq*k] rows, [nq] counts), stream-ordered on `st`.
-struct MergeOut {
-    uint32_t *doc = nullptr, *n = nullptr;
-    float *score = nullptr;
-    double *score64 = nullptr;
-    uint16_t *payload = nullptr;
-    cudaError_t alloc(size_t slots, uint32_t nq, cudaStream_t st) {
-        slots = slots ? slots : 1;
-        cudaError_t e = cudaMallocAsync((void **)&doc, 4 * slots, st);
-        if (e == cudaSuccess) e = cudaMallocAsync((void **)&score, 4 * slots, st);
-        if (e == cudaSuccess) e = cudaMallocAsync((void **)&score64, 8 * slots, st);
-        if (e == cudaSuccess) e = cudaMallocAsync((void **)&payload, 6 * slots, st);
-        if (e == cudaSuccess) e = cudaMallocAsync((void **)&n, 4 * (size_t)(nq ? nq : 1), st);
-        return e;
-    }
-    cudaError_t download(size_t slots, uint32_t nq, uint32_t *o_doc, float *o_score, double *o_score64,
-                         uint16_t *o_payload, uint32_t *o_n, cudaStream_t st) const {
-        cudaError_t e = cudaSuccess;
-        if (o_doc) e = cudaMemcpyAsync(o_doc, doc, 4 * slots, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess && o_score) e = cudaMemcpyAsync(o_score, score, 4 * slots, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess && o_score64) e = cudaMemcpyAsync(o_score64, score64, 8 * slots, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess && o_payload) e = cudaMemcpyAsync(o_payload, payload, 6 * slots, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess && o_n) e = cudaMemcpyAsync(o_n, n, 4 * (size_t)nq, cudaMemcpyDeviceToHost, st);
-        return e;
-    }
-    void release(cudaStream_t st) {
-        for (void *p : {(void *)doc, (void *)score, (void *)score64, (void *)payload, (void *)n})
-            if (p) cudaFreeAsync(p, st);
-        doc = n = nullptr;
-        score = nullptr;
-        score64 = nullptr;
-        payload = nullptr;
-    }
-};
+void set_shard(ShardRows &in, uint32_t s, const ResultRows &rows, uint32_t base) {
+    in.doc[s] = rows.doc;
+    in.score[s] = rows.score;
+    in.score64[s] = rows.score64;
+    in.payload[s] = rows.payload;
+    in.n[s] = rows.n;
+    in.base[s] = base;
+}
 
 // Bits [lo, hi) of a bitmap over global doc ids, shifted to bit 0 (shard bounds need not be multiples of 8).
 std::vector<uint8_t> allow_slice(const uint8_t *allow, uint32_t n_docs, uint32_t lo, uint32_t hi) {
@@ -144,11 +119,18 @@ std::vector<uint8_t> allow_slice(const uint8_t *allow, uint32_t n_docs, uint32_t
 
 }  // namespace
 
-// ---- the refusals of bm25x_search_batch, against the WHOLE segment's df (a query with 65 live terms is refused even when
-// no shard sees more than 64).  Mirrors bm25x_batch_prepare's checks and messages, including the query numbering inside
-// the slices bm25x_search_batch cuts large batches into.  Returns the whole index's live queries in *live_out. ----
-static int check_queries(const bm25x_sharded_index *sx, uint32_t slice_min, uint32_t nq, const uint32_t *q_off,
-                         const uint32_t *q_terms, uint32_t k, uint32_t *live_out) {
+extern "C" int bm25x_sharded_search_batch(bm25x_sharded_index *sx, uint32_t nq, const uint32_t *q_off,
+                                          const uint32_t *q_terms, uint32_t k, const uint8_t *allow, uint32_t *out_doc,
+                                          float *out_score, double *out_score64, uint16_t *out_payload, uint32_t *out_n,
+                                          bm25x_search_stats *stats) {
+    using clk = std::chrono::steady_clock;
+    if (!sx) {
+        bm25x_set_error("bm25x_sharded_search_batch: null argument");
+        return BM25X_ERR_INVALID;
+    }
+    const auto t0 = clk::now();
+    // ---- the refusals of bm25x_search_batch: its argument checks, then its canonicalisation slice by slice against the
+    // WHOLE segment's df (a query with 65 live terms is refused even when no shard sees more than 64) ----
     if (nq && (!q_off || (!q_terms && q_off[nq] != 0))) {
         bm25x_set_error("bm25x_batch_prepare: null argument");
         return BM25X_ERR_INVALID;
@@ -161,83 +143,30 @@ static int check_queries(const bm25x_sharded_index *sx, uint32_t slice_min, uint
         bm25x_set_error("bm25x_batch_prepare: k=%u > BM25X_MAX_K=%d", k, BM25X_MAX_K);
         return BM25X_ERR_UNSUPPORTED;
     }
-    const uint32_t n_slices = slice_min && nq >= 2ull * slice_min ? std::min<uint32_t>(16u, nq / slice_min) : 1u;
-    const uint32_t T = sx->n_terms;
-    const uint32_t *h_df = sx->h_df.data();
-    std::vector<uint8_t> kind(nq ? nq : 1, 0);  // 0 ok, 1 offsets, 2 too many live terms
-    std::vector<uint32_t> live(nq ? nq : 1, 0);
-    for (uint32_t s = 0; s < n_slices; s++) {
-        const uint32_t a = (uint32_t)(((uint64_t)nq * s) / n_slices), e = (uint32_t)(((uint64_t)nq * (s + 1)) / n_slices);
-        const size_t base0 = e > a ? q_off[a] : 0;
-        const size_t n_raw = e > a && q_off[e] >= base0 ? q_off[e] - base0 : 0;
-#pragma omp parallel for schedule(static, 1024) num_threads(e - a < 4096 ? 1 : bm25x_host_threads(16))
-        for (uint32_t i = a; i < e; i++) {
-            if (q_off[i + 1] < q_off[i] || q_off[i] < base0 || q_off[i + 1] - base0 > n_raw) {
-                kind[i] = 1;
-                continue;
-            }
-            uint32_t buf[256];
-            std::vector<uint32_t> big;
-            const uint32_t n = q_off[i + 1] - q_off[i];
-            uint32_t *dst = buf;
-            if (n > 256) {
-                big.resize(n);
-                dst = big.data();
-            }
-            uint32_t m = 0;
-            for (uint32_t j = 0; j < n; j++) {
-                const uint32_t t = q_terms[q_off[i] + j];
-                if (t < T && h_df[t] != 0) dst[m++] = t;
-            }
-            std::sort(dst, dst + m);
-            m = (uint32_t)(std::unique(dst, dst + m) - dst);
-            live[i] = m;
-            if (m > BM25X_MAX_QUERY_TERMS) kind[i] = 2;
-        }
-        int bad = -1;  // the batch reports the last offending query of the first slice that has one
-        for (uint32_t i = a; i < e; i++)
-            if (kind[i]) bad = (int)i;
-        if (bad >= 0) {
-            if (kind[bad] == 1) {
-                bm25x_set_error("bm25x_batch_prepare: q_off not monotone at %d", bad - (int)a);
-                return BM25X_ERR_INVALID;
-            }
-            bm25x_set_error("bm25x_batch_prepare: query %d has %u live terms > %d", bad - (int)a, live[bad],
-                            BM25X_MAX_QUERY_TERMS);
-            return BM25X_ERR_UNSUPPORTED;
+    uint32_t n_live = 0;  // live queries of the whole index
+    int rc = BM25X_OK;
+    {
+        const SlicePlan plan(sx->shards[0]->slice_min, nq);
+        CanonQueries cq;
+        for (uint32_t s = 0; s < plan.n && rc == BM25X_OK; s++) {
+            const uint32_t a = plan.begin(s), e = plan.begin(s + 1);
+            rc = bm25x_canonicalise(sx->h_df.data(), sx->n_terms, e - a, q_off + a, q_terms, &cq);
+            for (uint32_t i = 0; i < e - a; i++) n_live += cq.live[i] != 0;
         }
     }
-    uint32_t n_live = 0;
-    for (uint32_t i = 0; i < nq; i++) n_live += live[i] != 0;
-    *live_out = n_live;
-    return BM25X_OK;
-}
-
-extern "C" int bm25x_sharded_search_batch(bm25x_sharded_index *sx, uint32_t nq, const uint32_t *q_off,
-                                          const uint32_t *q_terms, uint32_t k, const uint8_t *allow, uint32_t *out_doc,
-                                          float *out_score, double *out_score64, uint16_t *out_payload, uint32_t *out_n,
-                                          bm25x_search_stats *stats) {
-    using clk = std::chrono::steady_clock;
-    if (!sx) {
-        bm25x_set_error("bm25x_sharded_search_batch: null argument");
-        return BM25X_ERR_INVALID;
-    }
-    const auto t0 = clk::now();
-    uint32_t n_live = 0;
-    int rc = check_queries(sx, sx->shards[0]->slice_min, nq, q_off, q_terms, k, &n_live);
     if (rc != BM25X_OK) return rc;
     const uint32_t S = sx->n_shards;
     bm25x_index *ix0 = sx->shards[0];
     const int dev0 = ix0->device;
     cudaStream_t ms = ix0->stream;  // the merge runs behind shard 0's kernels on its library stream
     std::vector<bm25x_batch *> bs(S, nullptr);
-    std::vector<void *> peer_bufs;  // results of shards on other devices, copied to dev0
+    std::vector<ResultRows> peer(S);  // rows of shards on other devices, copied to dev0
     std::vector<cudaEvent_t> evs;
-    MergeOut mo;
+    ResultRows mo;
     auto cleanup = [&](int code) {
         cudaSetDevice(dev0);
         cudaStreamSynchronize(ms);
-        for (void *p : peer_bufs) cudaFreeAsync(p, ms);
+        for (ResultRows &p : peer) p.release(ms);
         mo.release(ms);
         for (cudaEvent_t e : evs) cudaEventDestroy(e);
         for (bm25x_batch *b : bs)
@@ -255,34 +184,20 @@ extern "C" int bm25x_sharded_search_batch(bm25x_sharded_index *sx, uint32_t nq, 
     if (rc != BM25X_OK) return cleanup(rc);
     const auto t1 = clk::now();
     // ---- shard rows on dev0: read in place there, copied peer to peer from the other devices ----
-    const size_t slots = (size_t)nq * k;
     ShardRows in;
     memset(&in, 0, sizeof(in));
     cudaError_t e = cudaSetDevice(dev0);
     for (uint32_t s = 0; s < S && e == cudaSuccess; s++) {
-        void *p[5];
-        bm25x_batch_device_results(bs[s], &p[0], &p[1], &p[2], &p[3], &p[4]);
         e = cudaStreamWaitEvent(ms, bm25x_batch_done_event(bs[s]), 0);
-        const int dev = sx->shards[s]->device;
-        if (e == cudaSuccess && dev != dev0) {
-            const size_t bytes[5] = {4 * slots, 4 * slots, 8 * slots, 6 * slots, 4 * (size_t)nq};
-            for (int a = 0; a < 5 && e == cudaSuccess; a++) {
-                void *dst = nullptr;
-                e = cudaMallocAsync(&dst, bytes[a] ? bytes[a] : 4, ms);
-                if (e != cudaSuccess) break;
-                peer_bufs.push_back(dst);
-                if (bytes[a]) e = cudaMemcpyPeerAsync(dst, dev0, p[a], dev, bytes[a], ms);
-                p[a] = dst;
-            }
+        const ResultRows *rows = &bm25x_batch_rows(bs[s]);
+        if (e == cudaSuccess && sx->shards[s]->device != dev0) {
+            e = peer[s].alloc(nq, k, ms);
+            if (e == cudaSuccess) e = rows->copy_to(peer[s], nq, k, ms);
+            rows = &peer[s];
         }
-        in.doc[s] = (const uint32_t *)p[0];
-        in.score[s] = (const float *)p[1];
-        in.score64[s] = (const double *)p[2];
-        in.payload[s] = (const uint16_t *)p[3];
-        in.n[s] = (const uint32_t *)p[4];
-        in.base[s] = sx->bounds[s];
+        set_shard(in, s, *rows, sx->bounds[s]);
     }
-    if (e == cudaSuccess) e = mo.alloc(slots, nq, ms);
+    if (e == cudaSuccess) e = mo.alloc(nq, k, ms);
     cudaEvent_t m0 = nullptr, m1 = nullptr;
     if (e == cudaSuccess && stats) {
         e = cudaEventCreate(&m0);
@@ -295,10 +210,10 @@ extern "C" int bm25x_sharded_search_batch(bm25x_sharded_index *sx, uint32_t nq, 
         bm25x_set_error("bm25x_sharded_search_batch: %s", cudaGetErrorString(e));
         return cleanup(e == cudaErrorMemoryAllocation ? BM25X_ERR_OOM : BM25X_ERR_CUDA);
     }
-    rc = launch_merge(dev0, in, S, nq, k, mo.doc, mo.score, mo.score64, mo.payload, mo.n, ms);
+    rc = launch_merge(dev0, in, S, nq, k, mo, ms);
     if (rc != BM25X_OK) return cleanup(rc);
     if (stats) e = cudaEventRecord(m1, ms);
-    if (e == cudaSuccess) e = mo.download(slots, nq, out_doc, out_score, out_score64, out_payload, out_n, ms);
+    if (e == cudaSuccess) e = mo.copy_to({out_doc, out_score, out_score64, out_payload, out_n}, nq, k, ms);
     if (e == cudaSuccess) e = cudaStreamSynchronize(ms);  // after the merge: every shard's kernels have finished too
     if (e != cudaSuccess) {
         bm25x_set_error("bm25x_sharded_search_batch: %s", cudaGetErrorString(e));
@@ -350,38 +265,26 @@ extern "C" int bm25x_merge_shards(int device, uint32_t S, uint32_t nq, uint32_t 
         return BM25X_ERR_CUDA;
     }
     BM25X_CUDA_TRY(cudaSetDevice(device));
-    const size_t slots = (size_t)nq * k, all = slots * S;
     cudaStream_t st = nullptr;
     BM25X_CUDA_TRY(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-    MergeOut src, mo;  // the S shards' rows back to back in `src`
+    // the S shards' rows back to back: S * nq rows, on the host and in `src`
+    const ResultRows host{const_cast<uint32_t *>(doc), const_cast<float *>(score), const_cast<double *>(score64),
+                          const_cast<uint16_t *>(payload), const_cast<uint32_t *>(n)};
+    ResultRows src, mo;
     cudaEvent_t m0 = nullptr, m1 = nullptr;
-    cudaError_t e = src.alloc(all, nq * S, st);
-    if (e == cudaSuccess) e = mo.alloc(slots, nq, st);
-    auto up = [&](void *dst, const void *h, size_t bytes) {
-        if (e == cudaSuccess && bytes) e = cudaMemcpyAsync(dst, h, bytes, cudaMemcpyHostToDevice, st);
-    };
-    up(src.doc, doc, 4 * all);
-    up(src.score, score, 4 * all);
-    up(src.score64, score64, 8 * all);
-    up(src.payload, payload, 6 * all);
-    up(src.n, n, 4 * (size_t)nq * S);
+    cudaError_t e = src.alloc((size_t)nq * S, k, st);
+    if (e == cudaSuccess) e = mo.alloc(nq, k, st);
+    if (e == cudaSuccess) e = host.copy_to(src, (size_t)nq * S, k, st);
     ShardRows in;
     memset(&in, 0, sizeof(in));
-    for (uint32_t s = 0; s < S; s++) {
-        in.doc[s] = src.doc + s * slots;
-        in.score[s] = src.score + s * slots;
-        in.score64[s] = src.score64 + s * slots;
-        in.payload[s] = src.payload + s * slots * 3;
-        in.n[s] = src.n + (size_t)s * nq;
-        in.base[s] = nq ? doc_base[s] : 0;
-    }
+    for (uint32_t s = 0; s < S; s++) set_shard(in, s, src.from((size_t)s * nq, k), nq ? doc_base[s] : 0);
     if (e == cudaSuccess) e = cudaEventCreate(&m0);
     if (e == cudaSuccess) e = cudaEventCreate(&m1);
     if (e == cudaSuccess) e = cudaEventRecord(m0, st);
     int rc = BM25X_OK;
-    if (e == cudaSuccess) rc = launch_merge(device, in, S, nq, k, mo.doc, mo.score, mo.score64, mo.payload, mo.n, st);
+    if (e == cudaSuccess) rc = launch_merge(device, in, S, nq, k, mo, st);
     if (e == cudaSuccess && rc == BM25X_OK) e = cudaEventRecord(m1, st);
-    if (e == cudaSuccess && rc == BM25X_OK) e = mo.download(slots, nq, out_doc, out_score, out_score64, out_payload, out_n, st);
+    if (e == cudaSuccess && rc == BM25X_OK) e = mo.copy_to({out_doc, out_score, out_score64, out_payload, out_n}, nq, k, st);
     if (e == cudaSuccess && rc == BM25X_OK) e = cudaStreamSynchronize(st);
     if (e == cudaSuccess && rc == BM25X_OK && merge_ms) e = cudaEventElapsedTime(merge_ms, m0, m1);
     cudaStreamSynchronize(st);

@@ -134,7 +134,24 @@ typedef struct {
 } bm25x_index_layout;
 int bm25x_index_get_layout(const bm25x_index *idx, bm25x_index_layout *out);
 int bm25x_index_alloc_replica(const bm25x_index_layout *like, int device, bm25x_index **out);
+/* Rebuilds the derived structures below from the arrays as they are now; may be called again after a refill. */
 int bm25x_index_finalize_replica(bm25x_index *idx);
+/* Test hook: the derived structures every index builds on its own device and never replicates (finalize_replica rebuilds
+ * them), so that tests can read them back and compare them with a CPU restatement.  Device addresses, valid on `device`
+ * until the handle is destroyed or finalized again; a replica that is not finalized yet has no champion lists (NULL, 0). */
+typedef struct {
+    void *pdoc;                /* [n_postings_padded + 4] u32: post[i].doc; pad and slack slots read 0xFFFFFFFF */
+    uint64_t pdoc_bytes;
+    void *champ;               /* [n_champ] {u32 doc, u32 tf << 8 | fieldnorm}: per term its best min(df, 128) postings,
+                                  exact single-term score descending, then doc id ascending */
+    uint64_t champ_bytes;
+    void *champ_off;           /* [n_terms + 1] u64: term t's list is champ[champ_off[t] .. champ_off[t + 1]) */
+    uint64_t champ_off_bytes;
+    uint64_t n_champ;
+    float s1f_min;             /* min over the documents d of (float) s1[fieldnorm(d)] */
+    int device;
+} bm25x_index_derived;
+int bm25x_index_get_derived(const bm25x_index *idx, bm25x_index_derived *out);
 /* Options.  "prune" (default 1): MaxScore-style pruning in the warp-per-query kernel — terms whose summed score upper
  * bounds (the token-level WAND bound of the reference: TokenTuple.wand_fieldnorm/wand_term_frequency,
  * flush.rs:101-120, search.rs:363) stay at or below half the current k-th score are no longer streamed; their postings
@@ -264,6 +281,11 @@ int bm25x_sharded_lookup_terms(const bm25x_sharded_index *sx, const uint8_t *key
 int bm25x_sharded_search_batch(bm25x_sharded_index *sx, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms,
                                uint32_t k, const uint8_t *allow, uint32_t *out_doc, float *out_score, double *out_score64,
                                uint16_t *out_payload, uint32_t *out_n, bm25x_search_stats *stats);
+/* Test hook: the arrays of shard s (0 <= s < n_shards) as bm25x_index_get_layout / bm25x_index_get_derived report them
+ * for an index: local doc ids, local n_docs / n_postings / df, the whole segment's avgdl and score tables.  The shard
+ * handle itself stays internal.  Either output may be NULL. */
+int bm25x_sharded_get_shard(const bm25x_sharded_index *sx, uint32_t s, bm25x_index_layout *layout,
+                            bm25x_index_derived *derived);
 /* Test / measurement hook: k_merge_shards on host rows.  Shard s's rows are doc/score/score64/payload + s·nq·k
  * (payload: ·3) and n + s·nq, local doc ids, each row in canonical order; global id = local + doc_base[s], doc_base
  * ascending with s.  Outputs as bm25x_search_batch; merge_ms (or NULL) = the kernel's device time. */

@@ -106,6 +106,8 @@ def test_struct_layouts_match_the_header(m):
                "bm25x_index_layout": (bm.IndexLayout, ["n_docs", "n_terms", "n_postings", "n_postings_padded",
                                                        "n_blocks", "sum_doc_len", "k1", "b", "avgdl", "dev_ptr",
                                                        "bytes", "device"]),
+               "bm25x_index_derived": (bm.IndexDerived, ["pdoc", "pdoc_bytes", "champ", "champ_bytes", "champ_off",
+                                                         "champ_off_bytes", "n_champ", "s1f_min", "device"]),
                "bm25x_search_stats": (bm.SearchStats, ["kernel_ms", "h2d_ms", "d2h_ms", "postings", "bytes_algo",
                                                        "launches", "queries", "postings_fetched"])}
     prog = ['#include <stdio.h>', '#include <stddef.h>', f'#include "{HEADER}"', 'int main(void) {']

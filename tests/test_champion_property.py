@@ -45,3 +45,24 @@ def test_single_holder_results_are_champions(orc, cfg):
                     assert int(d) in champs(held[0])[:k], (cfg["seed"], i, k, int(d), held[0])
                     checked += 1
     assert checked > 50   # the property was actually exercised
+
+
+def test_restated_champion_lists_are_single_term_rankings(orc):
+    """The champion lists of the CPU restatement the GPU index tests compare with (tests/util_index.py) are each term's
+    single-term ranking by the oracle, cut to min(df, 128) — with whole tie groups at the cut (b = 0) and without."""
+    from util_index import restate
+    for b, cfg in ((0.75, (62, 6000, 900, 1, 120, 0.0)), (0.0, (61, 4000, 100, 8, 8, 0.0))):
+        c = orc.Corpus.synth(*cfg, b=b)
+        ix = orc.OracleIndex(c)
+        r = restate(orc, c.n_docs, c.post_off, c.post_doc, c.post_tf, c.k1, b, doc_len=c.doc_len)
+        champ = r.champ.reshape(-1, 2)
+        cut = 0
+        for t in range(c.n_terms):
+            lo, hi = int(r.champ_off[t]), int(r.champ_off[t + 1])
+            od, os_, _ = ix.search_exhaustive([t], 129)
+            assert np.array_equal(champ[lo:hi, 0], od[:128]), (b, t)
+            p0, p1 = int(c.post_off[t]), int(c.post_off[t + 1])
+            tf = c.post_tf[p0:p1][np.searchsorted(c.post_doc[p0:p1], od[:128])]
+            assert np.array_equal(champ[lo:hi, 1] >> 8, tf), (b, t)
+            cut += len(os_) > 128 and os_[127] == os_[128]
+        assert cut > (20 if b == 0 else -1), cut

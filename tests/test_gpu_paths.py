@@ -4,15 +4,13 @@ at the champion-list cut, k-th / (k+1)-th scores a few ulps apart, and the index
 score bounds) against a CPU restatement.  Bar as test_gpu_parity: doc ids, ranks and f64 scores bit-exact against
 OracleIndex.search_exhaustive, f32 scores = (float) f64 scores, unused rows 0xFFFFFFFF.  Two-pass (33..64-term) queries:
 test_gpu_parity.py::test_more_than_32_terms_two_passes."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
 import _pkg
 from test_gpu_parity import _compare, _csr_corpus, _live_queries, _oracle_index, _PrefixOracle, _rows_identical
 from test_gpu_zz_growing import _expect, _setup
-from util_cuda import download
+from util_index import assert_matches, read_back, restate
 
 pytestmark = pytest.mark.gpu
 
@@ -256,24 +254,10 @@ def test_near_ties_at_the_kth_score(m, orc):
     ix.close()
 
 
-ARRAYS = [("post", np.uint32), ("post_off", np.uint64), ("df", np.uint32), ("blk_off", np.uint64), ("blk", np.uint32),
-          ("s0f", np.float32), ("s0d", np.float64), ("s1d", np.float64), ("s1f", np.float32), ("fieldnorm", np.uint8),
-          ("payload", np.uint16), ("ubd", np.float64), ("blk_ub", np.float32)]
-INFLATE = np.float64(1.0 + 2.0 ** -40)
-
-
-def _f32_up(x):
-    """Smallest f32 >= each f64 of x."""
-    f = x.astype(np.float32)
-    low = f.astype(np.float64) < x
-    f[low] = np.nextafter(f[low], np.float32(np.inf))
-    return f
-
-
 @pytest.mark.parametrize("shape", ["varlen", "b0"])
 def test_index_arrays_match_cpu_restatement(m, orc, shape):
-    """The 13 device arrays of an index (Index.layout(), read back with cudaMemcpy) against numpy and the oracle's C
-    Cache / fieldnorm: postings with the fieldnorm folded in and their pad slots, offsets, block descriptors, score
+    """The 13 device arrays of an index (Index.layout(), read back with cudaMemcpy) and its derived ones against the CPU
+    restatement of tests/util_index.py (numpy and the oracle's C Cache / fieldnorm): postings with the fieldnorm folded in and their pad slots, offsets, block descriptors, score
     tables bit-equal, and the score bounds pruning trusts — ubd = (best single-posting score) x (1 + 2^-40) and blk_ub =
     the smallest f32 >= (block max) x (1 + 2^-40), bit-exact, each >= every posting score it bounds."""
     if shape == "varlen":
@@ -281,72 +265,16 @@ def test_index_arrays_match_cpu_restatement(m, orc, shape):
     else:
         c, k1, b = m.synth_corpus(261, 20000, 2000, 1, 200, 0.8), 1.2, 0.0
     ix = m.Index(c.n_docs, c.doc_len, c.n_terms, c.post_off, c.post_doc, c.post_tf, k1=k1, b=b)
-    oc = orc.Corpus(c.n_docs, c.doc_len, c.n_terms, c.post_off, c.post_doc, c.post_tf, k1=k1, b=b)
-    oix = orc.OracleIndex(oc)
+    oix = orc.OracleIndex(orc.Corpus(c.n_docs, c.doc_len, c.n_terms, c.post_off, c.post_doc, c.post_tf, k1=k1, b=b))
     L = orc.lib()
-    N, T = c.n_docs, c.n_terms
+    r = restate(orc, c.n_docs, c.post_off, c.post_doc, c.post_tf, k1, b, doc_len=c.doc_len)
     lay = ix.layout()
-    a = {name: download(lay.dev_ptr[i], lay.bytes[i], dt) for i, (name, dt) in enumerate(ARRAYS)}
-    off = oc.post_off.astype(np.int64)
-    df = np.diff(off)
-    assert (lay.n_docs, lay.n_terms, lay.n_postings) == (N, T, off[-1])
-    assert lay.sum_doc_len == int(c.doc_len.astype(np.uint64).sum()) and lay.avgdl == oix.avgdl
-    assert (lay.k1, lay.b) == (k1, b)
-
-    fn = np.array([L.orc_index_fieldnorm(oix.h, d) for d in range(N)], dtype=np.uint8)
-    assert np.array_equal(a["fieldnorm"], fn)
-    blkno = np.arange(N) // 291
-    assert np.array_equal(a["payload"].reshape(N, 3),
-                          np.stack([blkno >> 16, blkno & 0xFFFF, np.arange(N) % 291 + 1], axis=1).astype(np.uint16))
-
-    # postings: (doc, tf << 8 | fieldnorm) in CSR order, each list padded with {0xFFFFFFFF, 0} to a multiple of 4 slots,
-    # then the slack slots (all ones)
-    assert np.array_equal(a["df"], df)
-    pad = (df + 3) & ~3
-    off_pad = np.concatenate([[0], np.cumsum(pad)])
-    assert np.array_equal(a["post_off"], off_pad) and lay.n_postings_padded == off_pad[-1]
-    term = np.repeat(np.arange(T), df)
-    pos = off_pad[term] + (np.arange(off[-1]) - off[term])
-    want = np.zeros((off_pad[-1] + 4, 2), dtype=np.uint32)
-    want[:, 0] = 0xFFFFFFFF
-    want[off_pad[-1]:, 1] = 0xFFFFFFFF
-    want[pos, 0] = oc.post_doc
-    want[pos, 1] = (oc.post_tf << 8) | fn[oc.post_doc]
-    assert np.array_equal(a["post"].reshape(-1, 2), want)
-
-    # blocks of 128 postings: offsets, (first doc, last doc)
-    nb = (df + 127) // 128
-    blk_off = np.concatenate([[0], np.cumsum(nb)])
-    assert np.array_equal(a["blk_off"], blk_off)
-    bterm = np.repeat(np.arange(T), nb)
-    start = off[bterm] + 128 * (np.arange(blk_off[-1]) - blk_off[bterm])
-    end = np.minimum(start + 128, off[bterm + 1])
-    assert np.array_equal(a["blk"].reshape(-1, 2), np.stack([oc.post_doc[start], oc.post_doc[end - 1]], axis=1))
-
-    # Cache (bm25.rs:340-358) from the oracle's C code: s0 per term, s1 per fieldnorm
-    s0 = np.zeros(T)
-    s1 = (C.c_double * 256)()
-    for t in range(T):
-        s0_t = C.c_double()
-        L.orc_cache_new(N, int(df[t]), k1, b, oix.avgdl, C.byref(s0_t), s1)
-        s0[t] = s0_t.value
-    s1 = np.array(s1[:])
-    assert np.array_equal(a["s0d"], s0) and np.array_equal(a["s0f"], s0.astype(np.float32))
-    assert np.array_equal(a["s1d"], s1) and np.array_equal(a["s1f"], s1.astype(np.float32))
-
-    # every posting's exact score, Cache::evaluate's operation order (checked against the C function on a sample)
-    tfd = oc.post_tf.astype(np.float64)
-    score = (tfd * s0[term]) / (tfd + s1[fn[oc.post_doc]])
-    s1c = (C.c_double * 256)(*s1)
-    for p in np.random.default_rng(0).choice(off[-1], size=300, replace=False):
-        assert score[p] == L.orc_cache_evaluate(s0[term[p]], s1c, int(fn[oc.post_doc[p]]), int(oc.post_tf[p]))
-    bmax = np.maximum.reduceat(score, start)
-    tmax = np.zeros(T)
-    tmax[df > 0] = np.maximum.reduceat(score, off[:-1][df > 0])
-    assert np.array_equal(a["ubd"], tmax * INFLATE)
-    assert np.array_equal(a["blk_ub"], _f32_up(bmax * INFLATE))
+    assert lay.avgdl == oix.avgdl
+    assert np.array_equal(r.fieldnorm, [L.orc_index_fieldnorm(oix.h, d) for d in range(c.n_docs)])
+    der = ix.derived()
+    assert_matches(read_back(lay, der), lay, der, r, f"create {shape}")
     # what pruning relies on: no posting scores above its block's bound, no block maximum above its term's bound
-    blk_of = np.repeat(np.arange(blk_off[-1]), np.diff(np.append(start, off[-1])))
-    assert np.all(a["blk_ub"][blk_of].astype(np.float64) >= score)
-    assert np.all(a["ubd"][bterm] >= bmax) and np.all(a["ubd"][term] >= score)
+    blk_of = np.repeat(np.arange(r.n_blocks), np.diff(np.append(r.blk_start, r.n_postings)))
+    assert np.all(r.blk_ub[blk_of].astype(np.float64) >= r.score)
+    assert np.all(r.ubd[r.blk_term] >= r.block_max) and np.all(r.ubd[r.term] >= r.score)
     ix.close()

@@ -93,9 +93,11 @@ def test_default_bounds_skewed_corpus(m):
         sx.close()
 
 
-def test_adversarial_bounds(m):
-    """A one-document shard, bounds off multiples of 8, a shard where every query term has local df 0, a shard holding
-    all postings of a term, a shard with no postings at all — with and without a prefilter bitmap."""
+ADVERSARIAL_BOUNDS = [0, 997, 2001, 2002, 2003, 2301, 2600, 3333, 4000]
+
+
+def _adversarial_corpus():
+    """The corpus of test_adversarial_bounds, and its random generator for what the test draws next."""
     rng = np.random.default_rng(3)
     N = 4000
     lists = []
@@ -105,8 +107,15 @@ def test_adversarial_bounds(m):
     lists.append((np.arange(2100, 2300), rng.integers(1, 4, size=200)))     # term 60: all postings in [2003, 2301)
     lists.append((np.array([2001]), np.array([3])))                          # term 61: one document, shard [2001, 2002)
     # [2301, 2600) holds no posting at all; [2002, 2003) has no query term
-    c = _csr(N, lists, doc_len=rng.integers(1, 200, size=N).astype(np.uint32))
-    bounds = [0, 997, 2001, 2002, 2003, 2301, 2600, 3333, N]
+    return _csr(N, lists, doc_len=rng.integers(1, 200, size=N).astype(np.uint32)), rng
+
+
+def test_adversarial_bounds(m):
+    """A one-document shard, bounds off multiples of 8, a shard where every query term has local df 0, a shard holding
+    all postings of a term, a shard with no postings at all — with and without a prefilter bitmap."""
+    c, rng = _adversarial_corpus()
+    N = c["n_docs"]
+    bounds = ADVERSARIAL_BOUNDS
     ix = m.Index(**c)
     sx = m.ShardedIndex(**c, n_shards=len(bounds) - 1, doc_bounds=bounds)
     assert np.array_equal(sx.doc_bounds(), bounds)

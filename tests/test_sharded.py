@@ -119,7 +119,8 @@ def test_ctypes_declarations_match_the_header(m):
     protos = re.findall(r"\b(?:int|void)\s+(bm25x_(?:sharded_[a-z_]+|merge_shards))\s*\(([^)]*)\)\s*;", hdr)
     names = {n for n, _ in protos}
     assert names == {"bm25x_sharded_create", "bm25x_sharded_destroy", "bm25x_sharded_get_info", "bm25x_sharded_set_option",
-                     "bm25x_sharded_lookup_terms", "bm25x_sharded_search_batch", "bm25x_merge_shards"}, names
+                     "bm25x_sharded_lookup_terms", "bm25x_sharded_search_batch", "bm25x_sharded_get_shard",
+                     "bm25x_merge_shards"}, names
     lib = m.load_library()
     for name, params in protos:
         params = [" ".join(p.split()) for p in params.split(",")]

@@ -40,3 +40,10 @@ def memset(dev_ptr, value, nbytes):
 
 def device_synchronize():
     assert cudart().cudaDeviceSynchronize() == 0
+
+
+def sm_count(device=0):
+    """Streaming multiprocessors of `device` (cudaDevAttrMultiProcessorCount)."""
+    v = ctypes.c_int(0)
+    assert cudart().cudaDeviceGetAttribute(ctypes.byref(v), 16, device) == 0
+    return v.value

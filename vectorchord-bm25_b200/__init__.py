@@ -5,10 +5,10 @@ This package is the thin Python host binding used by tests and bench.py; it mirr
 host-side interface for the path (`bm25::search` / `bm25::evaluate`, Document / Query) and never
 falls back to a CPU implementation: if the library or an H100 is missing, calls raise.
 """
-from .bm25x import (Bm25xError, Index, Batch, SearchStats, IndexLayout, synth_corpus, synth_queries, load_library, build_library,
+from .bm25x import (Bm25xError, Index, Batch, SearchStats, IndexLayout, IndexDerived, synth_corpus, synth_queries, load_library, build_library,
                     device_count, Document, Query, MAX_K, MAX_QUERY_TERMS, TERM_MISSING, merge_topk, check_vectors, Broker,
                     ShardedIndex, MAX_SHARDS, merge_shards)
 
-__all__ = ["Bm25xError", "Index", "Batch", "SearchStats", "IndexLayout", "synth_corpus", "synth_queries", "load_library",
+__all__ = ["Bm25xError", "Index", "Batch", "SearchStats", "IndexLayout", "IndexDerived", "synth_corpus", "synth_queries", "load_library",
            "build_library", "device_count", "Document", "Query", "MAX_K", "MAX_QUERY_TERMS", "TERM_MISSING", "merge_topk",
            "check_vectors", "Broker", "ShardedIndex", "MAX_SHARDS", "merge_shards"]

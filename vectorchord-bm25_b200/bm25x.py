@@ -63,6 +63,12 @@ class IndexLayout(C.Structure):
                 ("bytes", C.c_uint64 * N_ARRAYS), ("device", C.c_int)]
 
 
+class IndexDerived(C.Structure):  # bm25x_index_derived: test hook, the arrays an index builds and never replicates
+    _fields_ = [("pdoc", C.c_void_p), ("pdoc_bytes", C.c_uint64), ("champ", C.c_void_p), ("champ_bytes", C.c_uint64),
+                ("champ_off", C.c_void_p), ("champ_off_bytes", C.c_uint64), ("n_champ", C.c_uint64),
+                ("s1f_min", C.c_float), ("device", C.c_int)]
+
+
 class BrokerOptions(C.Structure):  # bm25x_broker_options (include/bm25x_broker.h)
     _fields_ = [("max_batch", C.c_uint32), ("max_wait_us", C.c_uint32), ("ring_slots", C.c_uint32), ("reserved", C.c_uint32)]
 
@@ -127,6 +133,7 @@ def load_library():
     L.bm25x_index_get_layout.argtypes = [vp, C.POINTER(IndexLayout)]
     L.bm25x_index_alloc_replica.argtypes = [C.POINTER(IndexLayout), C.c_int, C.POINTER(vp)]
     L.bm25x_index_finalize_replica.argtypes = [vp]
+    L.bm25x_index_get_derived.argtypes = [vp, C.POINTER(IndexDerived)]
     L.bm25x_index_get_df.argtypes = [vp, u32p]
     L.bm25x_index_set_option.argtypes = [vp, C.c_char_p, C.c_int64]
     L.bm25x_search_batch.argtypes = [vp, C.c_uint32, u32p, u32p, C.c_uint32, u8p, u32p, f32p, f64p, u16p, u32p,
@@ -159,6 +166,7 @@ def load_library():
     L.bm25x_sharded_get_info.argtypes = [vp, C.POINTER(IndexInfo), u32p, u32p]
     L.bm25x_sharded_set_option.argtypes = [vp, C.c_char_p, C.c_int64]
     L.bm25x_sharded_lookup_terms.argtypes = [vp, u8p, C.c_uint32, u32p]
+    L.bm25x_sharded_get_shard.argtypes = [vp, C.c_uint32, C.POINTER(IndexLayout), C.POINTER(IndexDerived)]
     L.bm25x_sharded_search_batch.argtypes = [vp, C.c_uint32, u32p, u32p, C.c_uint32, u8p, u32p, f32p, f64p, u16p, u32p,
                                              C.POINTER(SearchStats)]
     L.bm25x_merge_shards.argtypes = [C.c_int, C.c_uint32, C.c_uint32, C.c_uint32, u32p, u32p, f32p, f64p, u16p, u32p,
@@ -386,6 +394,12 @@ class Index:
     def finalize_replica(self):
         _check(load_library().bm25x_index_finalize_replica(self.h))
 
+    def derived(self) -> IndexDerived:
+        """Test hook: the doc-id copy, champion lists and s1f_min this handle built on its device (never replicated)."""
+        out = IndexDerived()
+        _check(load_library().bm25x_index_get_derived(self.h, C.byref(out)))
+        return out
+
     def set_option(self, name: str, value: int):
         _check(load_library().bm25x_index_set_option(self.h, name.encode(), int(value)))
 
@@ -565,6 +579,12 @@ class ShardedIndex:
 
     def set_option(self, name: str, value: int):
         _check(load_library().bm25x_sharded_set_option(self.h, name.encode(), int(value)))
+
+    def shard_arrays(self, s: int):
+        """Test hook: (IndexLayout, IndexDerived) of shard s, whose handle stays internal (bm25x_sharded_get_shard)."""
+        lay, der = IndexLayout(), IndexDerived()
+        _check(load_library().bm25x_sharded_get_shard(self.h, int(s), C.byref(lay), C.byref(der)))
+        return lay, der
 
     def lookup_terms(self, keys):
         keys = np.ascontiguousarray(keys, dtype=np.uint8).reshape(-1, 16)

@@ -331,6 +331,8 @@ static int dev_alloc(bm25x_index *ix, T **p, size_t n) {
     return BM25X_OK;
 }
 
+// Called again for a replica that is refilled and finalized once more: the lists are rebuilt from the new postings, in the
+// same allocation when their total length has not changed.
 static cudaError_t build_champions(bm25x_index *ix) {
     DeviceIndex &d = ix->d;
     const uint32_t T = d.n_terms;
@@ -341,15 +343,32 @@ static cudaError_t build_champions(bm25x_index *ix) {
         run += std::min<uint32_t>(ix->h_df[t], BM25X_CHAMP_L);
     }
     h_off[T] = run;
+    cudaError_t e = cudaSuccess;
+    if (d.champ && run != d.n_champ) {
+        cudaFree(d.champ);
+        ix->allocs.erase(std::find(ix->allocs.begin(), ix->allocs.end(), (void *)d.champ));
+        ix->device_bytes -= sizeof(Posting) * (size_t)(d.n_champ ? d.n_champ : 1);
+        d.champ = nullptr;
+    }
     d.n_champ = run;
-    cudaError_t e = cudaMalloc((void **)&d.champ, sizeof(Posting) * (size_t)(run ? run : 1));
-    if (e != cudaSuccess) return e;
-    ix->allocs.push_back((void *)d.champ);
-    ix->device_bytes += sizeof(Posting) * (size_t)(run ? run : 1);
-    e = cudaMalloc((void **)&d.champ_off, sizeof(uint64_t) * ((size_t)T + 1));
-    if (e != cudaSuccess) return e;
-    ix->allocs.push_back((void *)d.champ_off);
-    ix->device_bytes += sizeof(uint64_t) * ((size_t)T + 1);
+    if (!d.champ) {
+        e = cudaMalloc((void **)&d.champ, sizeof(Posting) * (size_t)(run ? run : 1));
+        if (e != cudaSuccess) {
+            d.champ = nullptr;
+            return e;
+        }
+        ix->allocs.push_back((void *)d.champ);
+        ix->device_bytes += sizeof(Posting) * (size_t)(run ? run : 1);
+    }
+    if (!d.champ_off) {  // n_terms + 1 entries: the size never changes
+        e = cudaMalloc((void **)&d.champ_off, sizeof(uint64_t) * ((size_t)T + 1));
+        if (e != cudaSuccess) {
+            d.champ_off = nullptr;
+            return e;
+        }
+        ix->allocs.push_back((void *)d.champ_off);
+        ix->device_bytes += sizeof(uint64_t) * ((size_t)T + 1);
+    }
     e = cudaMemcpy(d.champ_off, h_off.data(), sizeof(uint64_t) * ((size_t)T + 1), cudaMemcpyHostToDevice);
     if (e != cudaSuccess || !T) return e;
     const unsigned blocks = (unsigned)std::min<uint64_t>(((uint64_t)T + CHAMP_WARPS - 1) / CHAMP_WARPS, (uint64_t)ix->sm_count * 16ull);
@@ -1137,6 +1156,27 @@ extern "C" int bm25x_index_get_layout(const bm25x_index *ix, bm25x_index_layout 
     return BM25X_OK;
 }
 
+extern "C" int bm25x_index_get_derived(const bm25x_index *ix, bm25x_index_derived *out) {
+    if (!ix || !out) {
+        bm25x_set_error("bm25x_index_get_derived: null argument");
+        return BM25X_ERR_INVALID;
+    }
+    const DeviceIndex &d = ix->d;
+    memset(out, 0, sizeof(*out));
+    out->pdoc = d.pdoc;
+    out->pdoc_bytes = sizeof(uint32_t) * (d.n_post_pad + BM25X_POST_SLACK);
+    if (d.champ) {  // a replica has none before its first finalize
+        out->champ = d.champ;
+        out->champ_bytes = sizeof(Posting) * d.n_champ;
+        out->champ_off = d.champ_off;
+        out->champ_off_bytes = sizeof(uint64_t) * ((uint64_t)d.n_terms + 1);
+        out->n_champ = d.n_champ;
+    }
+    out->s1f_min = ix->s1f_min;
+    out->device = ix->device;
+    return BM25X_OK;
+}
+
 extern "C" int bm25x_index_alloc_replica(const bm25x_index_layout *like, int device, bm25x_index **out) {
     if (!like || !out) {
         bm25x_set_error("bm25x_index_alloc_replica: null argument");
@@ -1213,7 +1253,7 @@ extern "C" int bm25x_index_finalize_replica(bm25x_index *ix) {
     ix->h_df.resize(ix->d.n_terms);
     if (ix->d.n_terms)
         BM25X_CUDA_TRY(cudaMemcpy(ix->h_df.data(), ix->d.df, sizeof(uint32_t) * ix->d.n_terms, cudaMemcpyDeviceToHost));
-    if (!ix->d.champ) BM25X_CUDA_TRY(build_champions(ix));  // derived data: built here from the replicated arrays
+    BM25X_CUDA_TRY(build_champions(ix));  // derived data: built here from the replicated arrays, on every call
     {   // s1f_min from the replicated arrays (see index_begin)
         std::vector<uint8_t> h_fn(ix->d.n_docs);
         float h_s1f[256];

@@ -327,6 +327,21 @@ extern "C" int bm25x_sharded_get_info(const bm25x_sharded_index *sx, bm25x_index
     return BM25X_OK;
 }
 
+extern "C" int bm25x_sharded_get_shard(const bm25x_sharded_index *sx, uint32_t s, bm25x_index_layout *layout,
+                                       bm25x_index_derived *derived) {
+    if (!sx) {
+        bm25x_set_error("bm25x_sharded_get_shard: null argument");
+        return BM25X_ERR_INVALID;
+    }
+    if (s >= sx->n_shards) {
+        bm25x_set_error("bm25x_sharded_get_shard: shard %u of %u", s, sx->n_shards);
+        return BM25X_ERR_INVALID;
+    }
+    int rc = layout ? bm25x_index_get_layout(sx->shards[s], layout) : BM25X_OK;
+    if (rc == BM25X_OK && derived) rc = bm25x_index_get_derived(sx->shards[s], derived);
+    return rc;
+}
+
 extern "C" int bm25x_sharded_set_option(bm25x_sharded_index *sx, const char *name, int64_t value) {
     if (!sx || !name) {
         bm25x_set_error("bm25x_sharded_set_option: null argument");

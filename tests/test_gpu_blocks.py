@@ -81,8 +81,8 @@ def test_blocks_from_stored_norms(m, orc):
 
 def test_blocks_wide_deltas_and_tf_limits(m, orc):
     # 26-bit deltas in a full block, 3-byte tf in a short one, tf = 2^24-1 accepted, 2^24 refused.
-    # (bit width 32 — raw ids, bitpacking_u32_ordered.rs:119-121 — needs > 2^31 documents: covered by the oracle tests
-    # and by the decoder's shared unpack path only.)
+    # (bit width 32 — raw ids, bitpacking_u32_ordered.rs:119-121 — needs > 2^31 documents: decoded on the GPU by
+    # tests/test_gpu_zy_high_doc_ids.py::test_stored_blocks_above_2_31, with a byte-width-4 tail above 2^31.)
     N = 40_000_000
     rng = np.random.default_rng(5)
     docs = np.sort(rng.choice(N, 128 + 77, replace=False)).astype(np.uint32)
@@ -210,3 +210,31 @@ def test_blocks_corruption_is_reported(m, orc):
     with pytest.raises(m.Bm25xError, match="corrupt blocks"):
         build(blk_min_doc=swap(eb.blk_min), blk_meta_doc=swap(eb.meta_doc), blk_meta_tf=swap(eb.meta_tf),
               blk_doc_off=swap(eb.doc_off), blk_tf_off=swap(eb.tf_off))
+
+    # a first delta that wraps: SummaryTuple.min_document_id 0xFFFFFFF0 + 0x20 = document 16 mod 2^32, every later id
+    # ascending and < n_docs.  The encoder always writes a first delta of 0, so only a corrupt page holds this; a decoded
+    # id below its block's min_document_id contradicts the summary.  Once in a full (bit-packed) block, once in a
+    # byte-packed tail.
+    N = 1000
+    full_docs, tail_docs = 16 + 7 * np.arange(128, dtype=np.uint32), 16 + 5 * np.arange(50, dtype=np.uint32)
+
+    def two_tokens(min_full, min_tail):
+        md0, pd0 = orc.compress_document_ids(min_full, full_docs)
+        md1, pd1 = orc.compress_document_ids(min_tail, tail_docs)
+        mt0, pt0 = orc.compress_term_frequencies(np.ones(128, np.uint32))
+        mt1, pt1 = orc.compress_term_frequencies(np.ones(50, np.uint32))
+        assert md0 >> 7 == 0 and md0 < 32 and md1 >> 7 == 1 and (md1 & 0x7F) < 4       # delta-coded, both
+        data = np.concatenate([pd0, pt0, pd1, pt1])
+        offs = np.cumsum([0, len(pd0), len(pt0), len(pd1)])
+        return m.Index.from_blocks(N, 2, [0, 1, 2], [min_full, min_tail], [128, 50], [md0, md1], [mt0, mt1],
+                                   [offs[0], offs[2]], [offs[1], offs[3]], data,
+                                   doc_fieldnorm=np.full(N, 20, dtype=np.uint8), sum_doc_len=20 * N)
+
+    ix = two_tokens(16, 16)                                            # the honest encoding: first delta 0
+    assert ix.search([0], 200)[0].tolist() == sorted(full_docs.tolist())
+    assert ix.search([1], 200)[0].tolist() == sorted(tail_docs.tolist())
+    ix.close()
+    wrap = 0xFFFFFFF0
+    for mins in ((wrap, 16), (16, wrap)):
+        with pytest.raises(m.Bm25xError, match="corrupt blocks"):
+            two_tokens(*mins)

@@ -60,7 +60,7 @@ def test_merge_topk_host():
     rng = np.random.default_rng(11)
     nq, k = 300, 7
 
-    def side(base):
+    def side(base, ids_below=1000):
         n = rng.integers(0, k + 1, nq).astype(np.uint32)
         doc = np.full((nq, k), 0xFFFFFFFF, np.uint32)
         s64 = np.zeros((nq, k))
@@ -70,25 +70,36 @@ def test_merge_topk_host():
             ids = np.zeros(n[q], np.uint32)
             for s in np.unique(sc):                                                   # ids ascend inside a tie group
                 sel = sc == s
-                ids[sel] = np.sort(rng.choice(1000, sel.sum(), replace=False))
+                ids[sel] = np.sort(rng.choice(ids_below, sel.sum(), replace=False))
             doc[q, :n[q]], s64[q, :n[q]] = ids, sc
             pay[q, :n[q], 0] = ids % 65536
             pay[q, :n[q], 2] = base
         return {"doc": doc, "score": s64.astype(np.float32), "score64": s64, "payload": pay, "n": n}
 
-    a, b = side(1), side(2)
-    out = m.merge_topk(a, b, 5000, k)
-    for q in range(nq):
-        rows = [(-a["score64"][q, i], int(a["doc"][q, i]), 1) for i in range(a["n"][q])] + \
-               [(-b["score64"][q, i], int(b["doc"][q, i]) + 5000, 2) for i in range(b["n"][q])]
-        rows.sort()
-        rows = rows[:k]
-        n = int(out["n"][q])
-        assert n == len(rows)
-        assert out["doc"][q, :n].tolist() == [r[1] for r in rows]
-        assert out["score64"][q, :n].tolist() == [-r[0] for r in rows]
-        assert out["payload"][q, :n, 2].tolist() == [r[2] for r in rows]
-        assert np.all(out["doc"][q, n:] == 0xFFFFFFFF)
+    # list b at the top of the id space: doc_base_b + k - 1 is the largest doc id, 0xFFFFFFFD (0xFFFFFFFF marks empty slots)
+    for doc_base_b, b_ids_below in ((5000, 1000), (0xFFFFFFFE - k, k)):
+        a, b = side(1), side(2, b_ids_below)
+        out = m.merge_topk(a, b, doc_base_b, k)
+        for q in range(nq):
+            rows = [(-a["score64"][q, i], int(a["doc"][q, i]), 1) for i in range(a["n"][q])] + \
+                   [(-b["score64"][q, i], int(b["doc"][q, i]) + doc_base_b, 2) for i in range(b["n"][q])]
+            rows.sort()
+            rows = rows[:k]
+            n = int(out["n"][q])
+            assert n == len(rows)
+            assert out["doc"][q, :n].tolist() == [r[1] for r in rows]
+            assert out["score64"][q, :n].tolist() == [-r[0] for r in rows]
+            assert out["payload"][q, :n, 2].tolist() == [r[2] for r in rows]
+            assert np.all(out["doc"][q, n:] == 0xFFFFFFFF)
+    assert out["doc"].max(initial=0, where=out["doc"] != 0xFFFFFFFF) == 0xFFFFFFFD
+    # one id past the largest would come back as the empty-slot marker, two past as document 0: refused
+    for over in (k, k + 1):
+        q = int(np.flatnonzero(b["n"] > 0)[0])
+        bad = {x: v.copy() for x, v in b.items()}
+        bad["doc"][q, int(b["n"][q]) - 1] = over
+        with pytest.raises(m.Bm25xError, match="exceeds the largest doc id") as e:
+            m.merge_topk(a, bad, doc_base_b, k)
+        assert e.value.code == 1
     with pytest.raises(m.Bm25xError, match="number of needed rows is set to 0"):
         m.merge_topk({x: (v[:, :0] if v.ndim > 1 else v) for x, v in a.items()},
                      {x: (v[:, :0] if v.ndim > 1 else v) for x, v in b.items()}, 0, 0)

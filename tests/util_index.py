@@ -44,10 +44,15 @@ def fieldnorms(orc, doc_len):
     return fn
 
 
-def synthetic_payload(n_docs, doc_base=0):
-    g = np.arange(n_docs, dtype=np.int64) + doc_base
+def ctid(ids):
+    """Synthetic payload of the given (global) doc ids, [len(ids), 3] u16."""
+    g = np.asarray(ids, dtype=np.int64)
     blkno = g // CTID_PER_PAGE
-    return np.stack([blkno >> 16, blkno & 0xFFFF, g % CTID_PER_PAGE + 1], axis=1).astype(np.uint16).reshape(-1)
+    return np.stack([blkno >> 16, blkno & 0xFFFF, g % CTID_PER_PAGE + 1], axis=1).astype(np.uint16)
+
+
+def synthetic_payload(n_docs, doc_base=0):
+    return ctid(np.arange(n_docs, dtype=np.int64) + doc_base).reshape(-1)
 
 
 def cache(orc, n_docs, df, k1, b, avgdl):
@@ -81,17 +86,30 @@ def restate(orc, n_docs, post_off, post_doc, post_tf, k1, b, *, doc_len=None, fi
     Returns a namespace: the arrays under their LAYOUT / DERIVED names (flat, in the dtype they are read back in), the
     layout's scalars, s1f_min, and per posting its term and exact score (for the score-bound checks)."""
     N = int(n_docs)
-    off = np.asarray(post_off, dtype=np.int64)
-    doc = np.asarray(post_doc, dtype=np.int64)
-    tf = np.asarray(post_tf, dtype=np.int64)
-    T, P = len(off) - 1, int(off[-1])
-    df = np.diff(off)
     if doc_len is not None:
         fn = fieldnorms(orc, doc_len)
         sum_len = int(np.asarray(doc_len, dtype=np.uint64).sum())
     else:
         fn = np.asarray(fieldnorm, dtype=np.uint8)
     assert len(fn) == N
+    doc = np.asarray(post_doc, dtype=np.int64)
+    r = restate_postings(orc, N, post_off, post_doc, post_tf, fn[doc], np.unique(fn), k1, b, sum_len, stat=stat)
+    r.fieldnorm = fn
+    r.payload = np.asarray(payload, dtype=np.uint16).reshape(-1) if payload is not None else synthetic_payload(N, doc_base)
+    return r
+
+
+def restate_postings(orc, n_docs, post_off, post_doc, post_tf, post_fn, norms_present, k1, b, sum_len, stat=None):
+    """The arrays restate() gives that the postings alone determine (all but fieldnorm and payload), at a cost in the
+    number of postings, whatever n_docs: post_fn is the fieldnorm of each posting's document, norms_present the distinct
+    fieldnorms of all documents (for s1f_min)."""
+    N = int(n_docs)
+    off = np.asarray(post_off, dtype=np.int64)
+    doc = np.asarray(post_doc, dtype=np.int64)
+    tf = np.asarray(post_tf, dtype=np.int64)
+    pfn = np.asarray(post_fn, dtype=np.uint8)
+    T, P = len(off) - 1, int(off[-1])
+    df = np.diff(off)
     avgdl = float(stat[2]) if stat is not None else float(sum_len) / float(N)
     s0, s1 = cache(orc, stat[0] if stat is not None else N, stat[1] if stat is not None else df, k1, b, avgdl)
     r = SimpleNamespace(n_docs=N, n_terms=T, n_postings=P, sum_doc_len=sum_len, avgdl=avgdl, k1=float(k1), b=float(b))
@@ -99,7 +117,7 @@ def restate(orc, n_docs, post_off, post_doc, post_tf, k1, b, *, doc_len=None, fi
     # postings: (doc, tf << 8 | fieldnorm) in CSR order, each list padded with {0xFFFFFFFF, 0} to a multiple of 4 slots,
     # then the slack slots (all ones)
     term = np.repeat(np.arange(T), df)
-    w = (tf << 8) | fn[doc].astype(np.int64)
+    w = (tf << 8) | pfn.astype(np.int64)
     pad = (df + ALIGN - 1) // ALIGN * ALIGN
     off_pad = np.concatenate([[0], np.cumsum(pad)]).astype(np.int64)
     pos = off_pad[term] + (np.arange(P) - off[term])
@@ -123,15 +141,13 @@ def restate(orc, n_docs, post_off, post_doc, post_tf, k1, b, *, doc_len=None, fi
     r.blk = np.stack([doc[start], doc[end - 1]], axis=1).astype(np.uint32).reshape(-1)
 
     r.s0d, r.s0f, r.s1d, r.s1f = s0, s0.astype(np.float32), s1, s1.astype(np.float32)
-    r.fieldnorm = fn
-    r.payload = np.asarray(payload, dtype=np.uint16).reshape(-1) if payload is not None else synthetic_payload(N, doc_base)
 
     # every posting's exact score, Cache::evaluate's operation order (checked against the C function on a sample)
     tfd = tf.astype(np.float64)
-    score = (tfd * s0[term]) / (tfd + s1[fn[doc]])
+    score = (tfd * s0[term]) / (tfd + s1[pfn])
     s1c = (C.c_double * 256)(*s1)
     for p in np.random.default_rng(0).choice(P, size=min(P, 300), replace=False):
-        assert score[p] == orc.lib().orc_cache_evaluate(s0[term[p]], s1c, int(fn[doc[p]]), int(tf[p]))
+        assert score[p] == orc.lib().orc_cache_evaluate(s0[term[p]], s1c, int(pfn[p]), int(tf[p]))
     r.term, r.score, r.blk_start, r.blk_term = term, score, start, bterm
     # score bounds: ubd = (best single-posting score) x (1 + 2^-40), blk_ub = the smallest f32 >= (block max) x (1 + 2^-40)
     tmax = np.zeros(T)
@@ -143,7 +159,7 @@ def restate(orc, n_docs, post_off, post_doc, post_tf, k1, b, *, doc_len=None, fi
     r.champ, r.champ_off = champion_lists(term, doc, w, score, df)
     r.champ = r.champ.reshape(-1)
     r.n_champ = int(r.champ_off[-1])
-    r.s1f_min = np.float32(r.s1f[np.unique(fn)].min())
+    r.s1f_min = np.float32(r.s1f[np.asarray(norms_present, dtype=np.int64)].min())
     return r
 
 

@@ -14,7 +14,7 @@
 
 namespace {
 
-#define BM25X_BLKERR_RANGE 1u  // doc id >= n_docs, ids not strictly ascending, tf == 0
+#define BM25X_BLKERR_RANGE 1u  // doc id >= n_docs, ids not strictly ascending or wrapped past 2^32, tf == 0
 #define BM25X_BLKERR_TF 2u     // tf >= 2^24
 
 __device__ __forceinline__ uint32_t sm_u32(const uint8_t *p) {  // payloads are byte-aligned only
@@ -32,8 +32,9 @@ __device__ __forceinline__ void unpack4(const uint8_t *sm, uint32_t bw, uint32_t
     }
 }
 
-// Decodes one stream of a block into v[0..3] (values 4*lane .. 4*lane+3).  `delta`: doc ids.
-__device__ __forceinline__ void decode_stream(const uint8_t *sm, uint8_t meta, uint32_t n, uint32_t lane, bool delta,
+// Decodes one stream of a block into v[0..3] (values 4*lane .. 4*lane+3).  `delta`: doc ids.  Returns whether the values
+// are a running sum seeded with min_doc (false: stored as is).
+__device__ __forceinline__ bool decode_stream(const uint8_t *sm, uint8_t meta, uint32_t n, uint32_t lane, bool delta,
                                               uint32_t min_doc, uint32_t v[4]) {
     const uint32_t width = meta & 0x7Fu;
     bool raw = !delta;
@@ -74,6 +75,7 @@ __device__ __forceinline__ void decode_stream(const uint8_t *sm, uint8_t meta, u
 #pragma unroll
         for (uint32_t l = 0; l < 4; l++) v[l] += base;
     }
+    return !raw;
 }
 
 constexpr int DEC_WARPS = 8;
@@ -105,9 +107,11 @@ k_decode_blocks(uint64_t n_blocks, const uint64_t *__restrict__ term_blk_off, ui
     for (uint32_t i = lane; i < nbt; i += 32) stage[warp][1][i] = stf[i];
     __syncwarp();
     uint32_t doc[4], tf[4];
-    decode_stream(stage[warp][0], md, n, lane, true, blk_min[g], doc);
+    const uint32_t min_doc = blk_min[g];
+    const bool summed = decode_stream(stage[warp][0], md, n, lane, true, min_doc, doc);
     decode_stream(stage[warp][1], mt, n, lane, false, 0u, tf);
-    // the reference trusts its pages ("data corruption" panics); here bad blocks are reported, never dereferenced
+    // the reference trusts its pages ("data corruption" panics); here bad blocks are reported, never dereferenced.  A
+    // running sum below its seed wrapped past 2^32 (a first delta the encoder never writes: it always starts at 0).
     const uint32_t prev_last = __shfl_up_sync(0xFFFFFFFFu, doc[3], 1);
     uint32_t bad = 0;
     Posting *dst = post + off_pad[lo] + (g - term_blk_off[lo]) * BM25X_BLOCK;
@@ -116,7 +120,8 @@ k_decode_blocks(uint64_t n_blocks, const uint64_t *__restrict__ term_blk_off, ui
         const uint32_t i = 4u * lane + l;
         if (i >= n) continue;
         const uint32_t before = l ? doc[l - 1] : prev_last;
-        if (doc[l] >= n_docs || (i > 0 && doc[l] <= before) || tf[l] == 0u) bad |= BM25X_BLKERR_RANGE;
+        if (doc[l] >= n_docs || (i > 0 && doc[l] <= before) || (summed && doc[l] < min_doc) || tf[l] == 0u)
+            bad |= BM25X_BLKERR_RANGE;
         if (tf[l] >= (1u << 24)) bad |= BM25X_BLKERR_TF;
         Posting p;
         p.doc = doc[l];

@@ -1023,6 +1023,13 @@ extern "C" int bm25x_growing_create(const bm25x_index *sealed, const bm25x_growi
     int rc = check_common(who, G, g->doc_len ? (const void *)g->doc_len : (const void *)g->doc_fieldnorm, sealed->k1,
                           sealed->b, sealed->device);
     if (rc != BM25X_OK) return rc;
+    // growing documents come back as sealed n_docs + ordinal (bm25x_search_batch_growing): the sum obeys check_common's
+    // bound on n_docs, so that every merged id stays below the BM25X_DOC_INF sentinel
+    if ((uint64_t)sealed->d.n_docs + G > (uint64_t)BM25X_DOC_INF - 1u) {
+        bm25x_set_error("%s: sealed n_docs=%u + growing n_docs=%u exceeds %u documents (doc ids are 32-bit, %u is reserved)",
+                        who, sealed->d.n_docs, G, BM25X_DOC_INF - 1u, BM25X_DOC_INF);
+        return BM25X_ERR_INVALID;
+    }
     // pass 1: validate the documents (vector.rs:39-75: keys strictly ascending, tf != 0) and count per-term postings
     std::vector<uint64_t> off((size_t)T + 1, 0);
     int bad = 0;

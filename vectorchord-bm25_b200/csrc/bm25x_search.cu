@@ -643,6 +643,14 @@ extern "C" int bm25x_merge_topk(uint32_t nq, uint32_t k, const uint32_t *doc_a, 
         bm25x_set_error("bm25x_merge_topk: null argument (f64 scores of both lists are required)");
         return BM25X_ERR_INVALID;
     }
+    // a shifted b id must stay a real doc id: BM25X_DOC_INF marks empty slots, and a wrapped sum would name another document
+    for (uint32_t q = 0; q < nq; q++)
+        for (uint32_t i = 0, nb = std::min(n_b[q], k); i < nb; i++)
+            if ((uint64_t)doc_b[(size_t)q * k + i] + doc_base_b > (uint64_t)BM25X_DOC_INF - 2u) {
+                bm25x_set_error("bm25x_merge_topk: doc %u of list b + doc_base_b %u exceeds the largest doc id %u",
+                                doc_b[(size_t)q * k + i], doc_base_b, BM25X_DOC_INF - 2u);
+                return BM25X_ERR_INVALID;
+            }
 #pragma omp parallel for schedule(static) num_threads(nq < 4096 ? 1 : bm25x_host_threads(16))
     for (uint32_t q = 0; q < nq; q++) {
         const size_t base = (size_t)q * k;

@@ -266,6 +266,19 @@ typedef struct bm25x_sharded_index bm25x_sharded_index;
  * CSR). */
 int bm25x_sharded_create(const bm25x_corpus *whole, uint32_t n_shards, const uint32_t *doc_bounds, const int *devices,
                          bm25x_sharded_index **out);
+/* The same document-sharded index, built from the sealed segment AS STORED (`blocks` exactly as for
+ * bm25x_index_create_from_blocks: SummaryTuple chains and BlockTuple payloads, tuples.rs:900-910,973-983, in the codec of
+ * compression.rs:36-136).  No CSR of the segment is ever built on the host: a check pass on devices[0] decodes every stored
+ * block once, in bounded chunks, with every check bm25x_index_create_from_blocks makes (the same codes and messages, the
+ * wand pair included), then each shard's device receives and decodes only the stored blocks that hold its documents.
+ * n_shards, doc_bounds and devices mean what they mean for bm25x_sharded_create (its refusals, its messages); with
+ * doc_bounds == NULL the bounds are its balanced ones, c_d counted from the decoded postings.  With doc_len the shards'
+ * arrays equal those bm25x_sharded_create builds from the decoded corpus; with doc_fieldnorm + sum_doc_len they hold the
+ * stored norms, and each shard's own sum_doc_len is the segment's.  Every host check runs before any device is used; on
+ * a refusal no handle is returned and every device allocation is freed.  The handle is an ordinary
+ * bm25x_sharded_index. */
+int bm25x_index_create_sharded_from_blocks(const bm25x_blocks *blocks, uint32_t n_shards, const uint32_t *doc_bounds,
+                                           const int *devices, bm25x_sharded_index **out);
 void bm25x_sharded_destroy(bm25x_sharded_index *sx);
 /* info as the unsharded index would report it (n_docs, n_terms, n_postings, sum_doc_len, avgdl, k1, b); device_bytes
  * and n_blocks summed over the shards; device = shard 0's.  doc_bounds_out[n_shards+1] or NULL. */

@@ -161,6 +161,8 @@ def load_library():
     L.bm25x_broker_destroy.argtypes = [vp]
     L.bm25x_broker_destroy.restype = None
     L.bm25x_sharded_create.argtypes = [C.POINTER(_Corpus), C.c_uint32, u32p, C.POINTER(C.c_int), C.POINTER(vp)]
+    L.bm25x_index_create_sharded_from_blocks.argtypes = [C.POINTER(_Blocks), C.c_uint32, u32p, C.POINTER(C.c_int),
+                                                         C.POINTER(vp)]
     L.bm25x_sharded_destroy.argtypes = [vp]
     L.bm25x_sharded_destroy.restype = None
     L.bm25x_sharded_get_info.argtypes = [vp, C.POINTER(IndexInfo), u32p, u32p]
@@ -222,6 +224,35 @@ def _corpus(keep, n_docs, doc_len, n_terms, post_off, post_doc, post_tf, k1, b, 
         c.payload = _kept(keep, payload, np.uint16, C.c_uint16)
     if term_keys is not None:
         c.term_key = _kept(keep, term_keys, np.uint8, C.c_uint8)
+    return c
+
+
+def _blocks(keep, n_docs, n_terms, term_blk_off, blk_min_doc, blk_n, blk_meta_doc, blk_meta_tf, blk_doc_off, blk_tf_off,
+            data, doc_len, doc_fieldnorm, sum_doc_len, k1, b, payload, term_keys, blk_wand_fieldnorm, blk_wand_tf):
+    c = _Blocks()
+    c.n_docs, c.n_terms, c.k1, c.b = int(n_docs), int(n_terms), float(k1), float(b)
+    if doc_len is not None:
+        c.doc_len = _kept(keep, doc_len, np.uint32, C.c_uint32)
+    if doc_fieldnorm is not None:
+        c.doc_fieldnorm = _kept(keep, doc_fieldnorm, np.uint8, C.c_uint8)
+    c.sum_doc_len = int(sum_doc_len)
+    if payload is not None:
+        c.payload = _kept(keep, payload, np.uint16, C.c_uint16)
+    if term_keys is not None:
+        c.term_key = _kept(keep, term_keys, np.uint8, C.c_uint8)
+    c.term_blk_off = _kept(keep, term_blk_off, np.uint64, C.c_uint64)
+    c.n_blocks = int(keep[-1][int(n_terms)]) if len(keep[-1]) > int(n_terms) else 0
+    c.blk_min_doc = _kept(keep, blk_min_doc, np.uint32, C.c_uint32)
+    c.blk_n = _kept(keep, blk_n, np.uint32, C.c_uint32)
+    c.blk_meta_doc = _kept(keep, blk_meta_doc, np.uint8, C.c_uint8)
+    c.blk_meta_tf = _kept(keep, blk_meta_tf, np.uint8, C.c_uint8)
+    c.blk_doc_off = _kept(keep, blk_doc_off, np.uint64, C.c_uint64)
+    c.blk_tf_off = _kept(keep, blk_tf_off, np.uint64, C.c_uint64)
+    c.bytes = _kept(keep, data, np.uint8, C.c_uint8)
+    c.n_bytes = len(keep[-1])
+    if blk_wand_fieldnorm is not None and blk_wand_tf is not None:   # SummaryTuple.wand_* (checked against the blocks)
+        c.blk_wand_fieldnorm = _kept(keep, blk_wand_fieldnorm, np.uint8, C.c_uint8)
+        c.blk_wand_tf = _kept(keep, blk_wand_tf, np.uint32, C.c_uint32)
     return c
 
 
@@ -343,31 +374,10 @@ class Index:
         """Index from the sealed segment as the reference stores it: per-token chains of 128-posting blocks in the
         codec of compression.rs, decoded on the GPU (bm25x_index_create_from_blocks).  Document norms come either from
         exact lengths (`doc_len`) or, as on the pages, from `doc_fieldnorm` + `sum_doc_len`."""
-        c = _Blocks()
         keep = []
-        c.n_docs, c.n_terms, c.k1, c.b = int(n_docs), int(n_terms), float(k1), float(b)
-        if doc_len is not None:
-            c.doc_len = _kept(keep, doc_len, np.uint32, C.c_uint32)
-        if doc_fieldnorm is not None:
-            c.doc_fieldnorm = _kept(keep, doc_fieldnorm, np.uint8, C.c_uint8)
-        c.sum_doc_len = int(sum_doc_len)
-        if payload is not None:
-            c.payload = _kept(keep, payload, np.uint16, C.c_uint16)
-        if term_keys is not None:
-            c.term_key = _kept(keep, term_keys, np.uint8, C.c_uint8)
-        c.term_blk_off = _kept(keep, term_blk_off, np.uint64, C.c_uint64)
-        c.n_blocks = int(keep[-1][int(n_terms)]) if len(keep[-1]) > int(n_terms) else 0
-        c.blk_min_doc = _kept(keep, blk_min_doc, np.uint32, C.c_uint32)
-        c.blk_n = _kept(keep, blk_n, np.uint32, C.c_uint32)
-        c.blk_meta_doc = _kept(keep, blk_meta_doc, np.uint8, C.c_uint8)
-        c.blk_meta_tf = _kept(keep, blk_meta_tf, np.uint8, C.c_uint8)
-        c.blk_doc_off = _kept(keep, blk_doc_off, np.uint64, C.c_uint64)
-        c.blk_tf_off = _kept(keep, blk_tf_off, np.uint64, C.c_uint64)
-        c.bytes = _kept(keep, data, np.uint8, C.c_uint8)
-        c.n_bytes = len(keep[-1])
-        if blk_wand_fieldnorm is not None and blk_wand_tf is not None:   # SummaryTuple.wand_* (checked against the blocks)
-            c.blk_wand_fieldnorm = _kept(keep, blk_wand_fieldnorm, np.uint8, C.c_uint8)
-            c.blk_wand_tf = _kept(keep, blk_wand_tf, np.uint32, C.c_uint32)
+        c = _blocks(keep, n_docs, n_terms, term_blk_off, blk_min_doc, blk_n, blk_meta_doc, blk_meta_tf, blk_doc_off,
+                    blk_tf_off, data, doc_len, doc_fieldnorm, sum_doc_len, k1, b, payload, term_keys, blk_wand_fieldnorm,
+                    blk_wand_tf)
         h = C.c_void_p()
         _check(load_library().bm25x_index_create_from_blocks(C.byref(c), device, C.byref(h)))
         return cls._adopt(h, n_docs, n_terms)
@@ -548,6 +558,27 @@ class ShardedIndex:
         _check(load_library().bm25x_sharded_create(C.byref(c), int(n_shards), _p(bounds, C.c_uint32), devs,
                                                    C.byref(self.h)))
         self.n_docs, self.n_terms = int(n_docs), int(n_terms)
+
+    @classmethod
+    def from_blocks(cls, n_docs, n_terms, term_blk_off, blk_min_doc, blk_n, blk_meta_doc, blk_meta_tf, blk_doc_off,
+                    blk_tf_off, data, doc_len=None, doc_fieldnorm=None, sum_doc_len=0, k1=1.2, b=0.75, payload=None,
+                    term_keys=None, blk_wand_fieldnorm=None, blk_wand_tf=None, n_shards=2, doc_bounds=None,
+                    devices=None) -> "ShardedIndex":
+        """The sharded index from the sealed segment as stored (Index.from_blocks' arguments): the blocks are checked
+        once on devices[0], then each shard's device decodes only the stored blocks that hold its documents
+        (bm25x_index_create_sharded_from_blocks)."""
+        keep = []
+        c = _blocks(keep, n_docs, n_terms, term_blk_off, blk_min_doc, blk_n, blk_meta_doc, blk_meta_tf, blk_doc_off,
+                    blk_tf_off, data, doc_len, doc_fieldnorm, sum_doc_len, k1, b, payload, term_keys, blk_wand_fieldnorm,
+                    blk_wand_tf)
+        bounds = np.ascontiguousarray(doc_bounds, dtype=np.uint32) if doc_bounds is not None else None
+        devs = (C.c_int * int(n_shards))(*[int(d) for d in devices]) if devices is not None else None
+        self = cls.__new__(cls)
+        self.h = C.c_void_p()
+        _check(load_library().bm25x_index_create_sharded_from_blocks(C.byref(c), int(n_shards), _p(bounds, C.c_uint32),
+                                                                     devs, C.byref(self.h)))
+        self.n_docs, self.n_terms = int(n_docs), int(n_terms)
+        return self
 
     @staticmethod
     def from_corpus(c, n_shards=2, doc_bounds=None, devices=None, **kw):

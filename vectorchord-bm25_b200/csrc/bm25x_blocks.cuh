@@ -16,6 +16,8 @@ namespace {
 
 #define BM25X_BLKERR_RANGE 1u  // doc id >= n_docs, ids not strictly ascending or wrapped past 2^32, tf == 0
 #define BM25X_BLKERR_TF 2u     // tf >= 2^24
+#define BM25X_BLKERR_DIR 4u    // a staged directory entry that does not describe a payload inside the staged bytes
+#define BM25X_BLKERR_WAND 8u   // SummaryTuple.wand_* is not the block's arg-max
 
 __device__ __forceinline__ uint32_t sm_u32(const uint8_t *p) {  // payloads are byte-aligned only
     return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24);
@@ -78,6 +80,33 @@ __device__ __forceinline__ bool decode_stream(const uint8_t *sm, uint8_t meta, u
     return !raw;
 }
 
+// The posting-check rule of the decoder: error bits of decoded posting i (doc, tf) of a block, `before` the id ahead of it.
+// A running sum below its seed wrapped past 2^32 (a first delta the encoder never writes: it always starts at 0).
+__device__ __forceinline__ uint32_t posting_errors(uint32_t doc, uint32_t tf, uint32_t i, uint32_t before, bool summed,
+                                                   uint32_t min_doc, uint32_t n_docs) {
+    uint32_t bad = 0;
+    if (doc >= n_docs || (i > 0 && doc <= before) || (summed && doc < min_doc) || tf == 0u) bad |= BM25X_BLKERR_RANGE;
+    if (tf >= (1u << 24)) bad |= BM25X_BLKERR_TF;
+    return bad;
+}
+
+// Cache::evaluate of one posting (bm25.rs:355-358), as k_block_desc / k_term_ub / k_champions compute it.
+__device__ __forceinline__ double posting_score(uint32_t w, double s0, const double *__restrict__ s1d) {
+    const double tfd = (double)(w >> 8);
+    return __ddiv_rn(__dmul_rn(tfd, s0), __dadd_rn(tfd, s1d[w & 0xFFu]));
+}
+
+// The stored SummaryTuple.(wand_fieldnorm, wand_term_frequency) of a block against the block's bound blk_ub (k_block_desc's
+// f32, rounded up after the 2^-40 inflation): tf() and Cache::evaluate round differently, so the last f32 ulp either way
+// is allowed.
+__device__ __forceinline__ bool wand_pair_ok(uint32_t wand_tf, uint8_t wand_fn, double s0, const double *__restrict__ s1d,
+                                             float blk_ub) {
+    const double tfd = (double)wand_tf;
+    const double v = __ddiv_rn(__dmul_rn(tfd, s0), __dadd_rn(tfd, s1d[wand_fn]));
+    const float ub = __double2float_ru(v * (1.0 + 9.094947017729282e-13));
+    return ub <= blk_ub * 1.0000003f && ub >= blk_ub * 0.9999997f;
+}
+
 constexpr int DEC_WARPS = 8;
 
 __global__ void __launch_bounds__(DEC_WARPS * 32)
@@ -110,8 +139,7 @@ k_decode_blocks(uint64_t n_blocks, const uint64_t *__restrict__ term_blk_off, ui
     const uint32_t min_doc = blk_min[g];
     const bool summed = decode_stream(stage[warp][0], md, n, lane, true, min_doc, doc);
     decode_stream(stage[warp][1], mt, n, lane, false, 0u, tf);
-    // the reference trusts its pages ("data corruption" panics); here bad blocks are reported, never dereferenced.  A
-    // running sum below its seed wrapped past 2^32 (a first delta the encoder never writes: it always starts at 0).
+    // the reference trusts its pages ("data corruption" panics); here bad blocks are reported, never dereferenced
     const uint32_t prev_last = __shfl_up_sync(0xFFFFFFFFu, doc[3], 1);
     uint32_t bad = 0;
     Posting *dst = post + off_pad[lo] + (g - term_blk_off[lo]) * BM25X_BLOCK;
@@ -119,10 +147,7 @@ k_decode_blocks(uint64_t n_blocks, const uint64_t *__restrict__ term_blk_off, ui
     for (uint32_t l = 0; l < 4; l++) {
         const uint32_t i = 4u * lane + l;
         if (i >= n) continue;
-        const uint32_t before = l ? doc[l - 1] : prev_last;
-        if (doc[l] >= n_docs || (i > 0 && doc[l] <= before) || (summed && doc[l] < min_doc) || tf[l] == 0u)
-            bad |= BM25X_BLKERR_RANGE;
-        if (tf[l] >= (1u << 24)) bad |= BM25X_BLKERR_TF;
+        bad |= posting_errors(doc[l], tf[l], i, l ? doc[l - 1] : prev_last, summed, min_doc, n_docs);
         Posting p;
         p.doc = doc[l];
         p.w = (tf[l] << 8) | (doc[l] < n_docs ? fieldnorm[doc[l]] : 0u);
@@ -144,6 +169,204 @@ __global__ void k_check_block_order(const uint64_t *__restrict__ blk_off, uint32
     }
     if (blk_off[lo] == g) return;  // first block of its token
     if (blk[g].x <= blk[g - 1].y) atomicOr(err, BM25X_BLKERR_RANGE);
+}
+
+// ---- document-sharded index from stored blocks (bm25x_index_create_sharded_from_blocks, DESIGN §4.7): the kernels below
+// read blocks gathered from the caller's directory into a staging buffer, back to back with rebased offsets ----
+
+// Bytes of one stream of an n-posting block: bit packing (flag 0) only for full blocks, 16 words of `width` <= 32 bits; byte
+// packing 1..4 bytes per value (compression.rs:43-62).  ~0u: a layout the encoder never writes.
+__host__ __device__ __forceinline__ uint32_t stream_bytes(uint8_t meta, uint32_t n) {
+    const uint32_t w = meta & 0x7Fu;
+    if ((meta >> 7) == 0) return w <= 32u && n == BM25X_BLOCK ? w * 16u : ~0u;
+    return w >= 1u && w <= 4u && n >= 1u && n <= BM25X_BLOCK ? w * n : ~0u;
+}
+
+// Copies one stream of a staged block into the warp's 512-byte stage.  False (the warp leaves, the caller reports
+// BM25X_BLKERR_DIR) when the entry does not describe a payload inside bytes[0, n_bytes).
+__device__ __forceinline__ bool stage_stream(uint8_t *stage, uint32_t lane, const uint8_t *__restrict__ bytes,
+                                             uint64_t n_bytes, uint8_t meta, uint32_t n, uint64_t off) {
+    const uint32_t nb = stream_bytes(meta, n);
+    if (nb == ~0u || off > n_bytes || nb > n_bytes - off) return false;
+    for (uint32_t i = lane; i < nb; i += 32) stage[i] = bytes[off + i];
+    return true;
+}
+
+// Whole-segment check: one warp per stored block of the chunk [g0, g0 + n_blocks) (directory arrays chunk-local).  Exactly
+// k_decode_blocks' posting checks against the segment's n_docs, without writing postings, and per block its decoded (first,
+// last) doc id: k_check_block_order's rule and the shards' block selection run on these on the host.  With wand_fn:
+// k_check_block_wand's test against the bound k_block_desc computes from the same postings (needs the segment's fieldnorm,
+// s0d, s1d).  With doc_count: every posting counted on its document (the balanced shard bounds).
+__global__ void __launch_bounds__(DEC_WARPS * 32)
+k_check_blocks(uint64_t g0, uint64_t n_blocks, const uint64_t *__restrict__ term_blk_off, uint32_t n_terms,
+               const uint32_t *__restrict__ blk_min, const uint32_t *__restrict__ blk_n,
+               const uint8_t *__restrict__ meta_doc, const uint8_t *__restrict__ meta_tf,
+               const uint64_t *__restrict__ doc_off, const uint64_t *__restrict__ tf_off, const uint8_t *__restrict__ bytes,
+               uint64_t n_bytes, const uint8_t *__restrict__ fieldnorm, uint32_t n_docs,
+               const uint8_t *__restrict__ wand_fn, const uint32_t *__restrict__ wand_tf, const double *__restrict__ s0d,
+               const double *__restrict__ s1d, uint2 *__restrict__ first_last, uint32_t *__restrict__ doc_count,
+               uint32_t *__restrict__ err) {
+    __shared__ __align__(16) uint8_t stage[DEC_WARPS][2][512];
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
+    const uint64_t j = (uint64_t)blockIdx.x * DEC_WARPS + warp;
+    if (j >= n_blocks) return;  // whole warps leave; no block-wide barrier below
+    const uint32_t n = blk_n[j];
+    const uint8_t md = meta_doc[j], mt = meta_tf[j];
+    if (!stage_stream(stage[warp][0], lane, bytes, n_bytes, md, n, doc_off[j]) ||
+        !stage_stream(stage[warp][1], lane, bytes, n_bytes, mt, n, tf_off[j])) {
+        if (lane == 0) {
+            first_last[j] = make_uint2(BM25X_DOC_INF, BM25X_DOC_INF);
+            atomicOr(err, BM25X_BLKERR_DIR);
+        }
+        return;
+    }
+    __syncwarp();
+    uint32_t doc[4], tf[4];
+    const uint32_t min_doc = blk_min[j];
+    const bool summed = decode_stream(stage[warp][0], md, n, lane, true, min_doc, doc);
+    decode_stream(stage[warp][1], mt, n, lane, false, 0u, tf);
+    const bool wand = wand_fn != nullptr;
+    double s0 = 0.0;
+    if (wand) {  // token of the block: last t with term_blk_off[t] <= g0 + j
+        const uint64_t g = g0 + j;
+        uint32_t lo = 0, hi = n_terms;
+        while (lo < hi) {
+            const uint32_t mid = (lo + hi + 1) >> 1;
+            if (term_blk_off[mid] <= g) lo = mid;
+            else hi = mid - 1;
+        }
+        s0 = s0d[lo];
+    }
+    const uint32_t prev_last = __shfl_up_sync(0xFFFFFFFFu, doc[3], 1);
+    uint32_t bad = 0, last_mine = doc[0];
+    double best = 0.0;
+#pragma unroll
+    for (uint32_t l = 0; l < 4; l++) {
+        const uint32_t i = 4u * lane + l;
+        if (i >= n) continue;
+        bad |= posting_errors(doc[l], tf[l], i, l ? doc[l - 1] : prev_last, summed, min_doc, n_docs);
+        if (i == n - 1) last_mine = doc[l];
+        const bool in = doc[l] < n_docs;
+        if (wand) {
+            const double v = posting_score((tf[l] << 8) | (in ? fieldnorm[doc[l]] : 0u), s0, s1d);
+            best = v > best ? v : best;
+        }
+        if (doc_count && in) atomicAdd(doc_count + doc[l], 1u);
+    }
+    const uint32_t first = __shfl_sync(0xFFFFFFFFu, doc[0], 0), last = __shfl_sync(0xFFFFFFFFu, last_mine, (n - 1) >> 2);
+    if (wand)
+        for (int o = 16; o > 0; o >>= 1) {
+            const double v = __shfl_xor_sync(0xFFFFFFFFu, best, o);
+            best = v > best ? v : best;
+        }
+    if (bad) atomicOr(err, bad);
+    if (lane == 0) {
+        first_last[j] = make_uint2(first, last);
+        if (wand && !wand_pair_ok(wand_tf[j], wand_fn[j], s0, s1d, __double2float_ru(best * (1.0 + 9.094947017729282e-13))))
+            atomicOr(err, BM25X_BLKERR_WAND);
+    }
+}
+
+// Per-shard count: one warp per selected block (its decoded (first, last) from the check pass): of its postings, how many
+// fall in the shard's documents [lo, hi) (.x) and how many lie below lo (.y; ids ascend inside a block, so those in range
+// are one run after them).  A block inside [lo, hi) counts n without decoding; only the blocks a bound cuts (at most two per
+// token) are decoded, doc ids only.
+__global__ void __launch_bounds__(DEC_WARPS * 32)
+k_count_shard_blocks(uint64_t n_blocks, const uint2 *__restrict__ first_last, const uint32_t *__restrict__ blk_min,
+                     const uint32_t *__restrict__ blk_n, const uint8_t *__restrict__ meta_doc,
+                     const uint64_t *__restrict__ doc_off, const uint8_t *__restrict__ bytes, uint64_t n_bytes, uint32_t lo,
+                     uint32_t hi, uint2 *__restrict__ count_skip, uint32_t *__restrict__ err) {
+    __shared__ __align__(16) uint8_t stage[DEC_WARPS][512];
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
+    const uint64_t j = (uint64_t)blockIdx.x * DEC_WARPS + warp;
+    if (j >= n_blocks) return;
+    const uint32_t n = blk_n[j];
+    const uint2 fl = first_last[j];
+    if (fl.x >= lo && fl.y < hi) {
+        if (lane == 0) count_skip[j] = make_uint2(n, 0u);
+        return;
+    }
+    const uint8_t md = meta_doc[j];
+    if (!stage_stream(stage[warp], lane, bytes, n_bytes, md, n, doc_off[j])) {
+        if (lane == 0) {
+            count_skip[j] = make_uint2(0u, 0u);
+            atomicOr(err, BM25X_BLKERR_DIR);
+        }
+        return;
+    }
+    __syncwarp();
+    uint32_t doc[4];
+    decode_stream(stage[warp], md, n, lane, true, blk_min[j], doc);
+    uint32_t in = 0, below = 0;
+#pragma unroll
+    for (uint32_t l = 0; l < 4; l++) {
+        const uint32_t i = 4u * lane + l;
+        if (i >= n) continue;
+        below += doc[l] < lo;
+        in += doc[l] >= lo && doc[l] < hi;
+    }
+    in = __reduce_add_sync(0xFFFFFFFFu, in);
+    below = __reduce_add_sync(0xFFFFFFFFu, below);
+    if (lane == 0) count_skip[j] = make_uint2(in, below);
+}
+
+// Per-shard decode: one warp per selected block; its postings in [lo, lo + n_local) written as {doc - lo, tf << 8 |
+// fieldnorm(local)} at the token's padded offset + rank[j] (the in-range postings of the token's earlier selected blocks) +
+// the posting's rank among the block's in-range ones.  The posting checks run again (n_docs: the segment's); a position
+// outside the token's shard df (a payload that decodes otherwise than it did in the count) is reported, never written.
+__global__ void __launch_bounds__(DEC_WARPS * 32)
+k_decode_shard_blocks(uint64_t n_blocks, const uint64_t *__restrict__ sel_off, uint32_t n_terms,
+                      const uint32_t *__restrict__ blk_min, const uint32_t *__restrict__ blk_n,
+                      const uint8_t *__restrict__ meta_doc, const uint8_t *__restrict__ meta_tf,
+                      const uint64_t *__restrict__ doc_off, const uint64_t *__restrict__ tf_off,
+                      const uint8_t *__restrict__ bytes, uint64_t n_bytes, const uint2 *__restrict__ count_skip,
+                      const uint32_t *__restrict__ rank, uint32_t n_docs, uint32_t lo, uint32_t n_local,
+                      const uint64_t *__restrict__ off_pad, const uint32_t *__restrict__ df,
+                      const uint8_t *__restrict__ fieldnorm, Posting *__restrict__ post, uint32_t *__restrict__ err) {
+    __shared__ __align__(16) uint8_t stage[DEC_WARPS][2][512];
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
+    const uint64_t j = (uint64_t)blockIdx.x * DEC_WARPS + warp;
+    if (j >= n_blocks) return;
+    const uint32_t n = blk_n[j];
+    const uint8_t md = meta_doc[j], mt = meta_tf[j];
+    if (!stage_stream(stage[warp][0], lane, bytes, n_bytes, md, n, doc_off[j]) ||
+        !stage_stream(stage[warp][1], lane, bytes, n_bytes, mt, n, tf_off[j])) {
+        if (lane == 0) atomicOr(err, BM25X_BLKERR_DIR);
+        return;
+    }
+    __syncwarp();
+    uint32_t t = 0, hi_t = n_terms;  // token of this block: last t with sel_off[t] <= j
+    while (t < hi_t) {
+        const uint32_t mid = (t + hi_t + 1) >> 1;
+        if (sel_off[mid] <= j) t = mid;
+        else hi_t = mid - 1;
+    }
+    uint32_t doc[4], tf[4];
+    const uint32_t min_doc = blk_min[j];
+    const bool summed = decode_stream(stage[warp][0], md, n, lane, true, min_doc, doc);
+    decode_stream(stage[warp][1], mt, n, lane, false, 0u, tf);
+    const uint32_t prev_last = __shfl_up_sync(0xFFFFFFFFu, doc[3], 1);
+    const uint32_t skip = count_skip[j].y, r0 = rank[j], n_t = df[t];
+    Posting *dst = post + off_pad[t];
+    uint32_t bad = 0;
+#pragma unroll
+    for (uint32_t l = 0; l < 4; l++) {
+        const uint32_t i = 4u * lane + l;
+        if (i >= n) continue;
+        bad |= posting_errors(doc[l], tf[l], i, l ? doc[l - 1] : prev_last, summed, min_doc, n_docs);
+        const uint32_t local = doc[l] - lo;
+        if (doc[l] < lo || local >= n_local) continue;
+        const uint64_t pos = (uint64_t)r0 + i - skip;
+        if (i < skip || pos >= n_t || tf[l] >= (1u << 24)) {
+            bad |= BM25X_BLKERR_RANGE;
+            continue;
+        }
+        Posting p;
+        p.doc = local;
+        p.w = (tf[l] << 8) | fieldnorm[local];
+        dst[pos] = p;
+    }
+    if (bad) atomicOr(err, bad);
 }
 
 }  // namespace

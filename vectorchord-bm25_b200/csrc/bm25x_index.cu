@@ -101,6 +101,20 @@ uint8_t bm25x_length_to_fieldnorm(uint32_t len) {  // bm25.rs:278-283
     return (uint8_t)(lo - 1);
 }
 
+// Cache::new (bm25.rs:340-354): s0 = idf·(k1 + 1) of a term in n of N documents (bm25.rs:285-289,348), and the s1 table,
+// identical for every term: it depends only on (k1, b, avgdl) (bm25.rs:349-352).
+static double bm25_s0(double n, double N, double k1) {
+    double idf = log((N + 1.0) / (n + 0.5));
+    return idf * (k1 + 1.0);
+}
+static void bm25_s1(double k1, double b, double avgdl, double s1d[256]) {
+    fn_init();
+    for (int f = 0; f < 256; f++) {
+        double dl = (double)g_fn_len[f];
+        s1d[f] = k1 * (1.0 - b + b * dl / avgdl);
+    }
+}
+
 // ---- device transforms ----
 
 // CSR chunk → AoS postings at their padded positions, with the fieldnorm byte folded in.
@@ -189,11 +203,7 @@ __global__ void k_check_block_wand(uint64_t n_blocks, const uint64_t *__restrict
         if (blk_off[mid] <= g) lo = mid;
         else hi = mid - 1;
     }
-    const double tfd = (double)wand_tf[g];
-    const double v = __ddiv_rn(__dmul_rn(tfd, s0d[lo]), __dadd_rn(tfd, s1d[wand_fn[g]]));
-    const float ub = __double2float_ru(v * (1.0 + 9.094947017729282e-13));
-    // tf() and Cache::evaluate round differently: allow the last f32 ulp either way
-    if (!(ub <= blk_ub[g] * 1.0000003f && ub >= blk_ub[g] * 0.9999997f)) atomicOr(err, 8u);
+    if (!wand_pair_ok(wand_tf[g], wand_fn[g], s0d[lo], s1d, blk_ub[g])) atomicOr(err, BM25X_BLKERR_WAND);
 }
 
 // Per-term upper bound of a single posting's exact score: max over the term's postings of Cache::evaluate
@@ -518,20 +528,15 @@ static int index_begin(const BuildMeta &m, int device, bm25x_index **ixp) {
         pp += (n + BM25X_POST_ALIGN - 1) & ~(uint64_t)(BM25X_POST_ALIGN - 1);
         nb += (n + BM25X_BLOCK - 1) / BM25X_BLOCK;
         const double n_stat = m.stat_df ? (double)m.stat_df[t] : (double)n, N_stat = m.stat_df ? (double)m.stat_n_docs : (double)N;
-        double idf = log((N_stat + 1.0) / (n_stat + 0.5));
-        h_s0d[t] = idf * (m.k1 + 1.0);
+        h_s0d[t] = bm25_s0(n_stat, N_stat, m.k1);
         h_s0f[t] = (float)h_s0d[t];
     }
     h_off_pad[T] = pp;
     h_blk_off[T] = nb;
-    // bm25.rs:349-352 — identical for every term: depends only on (k1, b, avgdl)
     double h_s1d[256];
     float h_s1f[256];
-    for (int f = 0; f < 256; f++) {
-        double dl = (double)g_fn_len[f];
-        h_s1d[f] = m.k1 * (1.0 - m.b + m.b * dl / ix->avgdl);
-        h_s1f[f] = (float)h_s1d[f];
-    }
+    bm25_s1(m.k1, m.b, ix->avgdl, h_s1d);
+    for (int f = 0; f < 256; f++) h_s1f[f] = (float)h_s1d[f];
     {   // smallest s1 over the documents present: the one-compare single-term test of k_search_ring needs a lower bound
         bool seen[256] = {false};
         for (uint32_t d = 0; d < N; d++) seen[h_fn[d]] = true;
@@ -733,6 +738,51 @@ extern "C" void bm25x_sharded_destroy(bm25x_sharded_index *sx) {
     delete sx;
 }
 
+// The shard arguments of a document-sharded build, by bm25x_sharded_create's rules and with its messages whichever entry
+// point is called: 1..BM25X_MAX_SHARDS shards, at least one document each, explicit bounds strictly ascending from 0 to N.
+static int check_shard_args(uint32_t N, uint32_t S, const uint32_t *doc_bounds) {
+    const char *who = "bm25x_sharded_create";
+    if (S == 0 || S > BM25X_MAX_SHARDS) {
+        bm25x_set_error("%s: n_shards=%u must be 1..%d", who, S, BM25X_MAX_SHARDS);
+        return BM25X_ERR_INVALID;
+    }
+    if (N < S) {
+        bm25x_set_error("%s: n_docs=%u < n_shards=%u (every shard holds at least one document)", who, N, S);
+        return BM25X_ERR_INVALID;
+    }
+    if (doc_bounds) {
+        bool ok = doc_bounds[0] == 0 && doc_bounds[S] == N;
+        for (uint32_t s = 0; s < S && ok; s++) ok = doc_bounds[s] < doc_bounds[s + 1];
+        if (!ok) {
+            bm25x_set_error("%s: doc_bounds must ascend strictly from 0 to n_docs=%u", who, N);
+            return BM25X_ERR_INVALID;
+        }
+    }
+    return BM25X_OK;
+}
+
+// The shard bounds of a document-sharded build: doc_bounds as given (checked by check_shard_args), or, when it is NULL,
+// balanced by postings from cum[d] = Σ_{d' < d} c_{d'} (c_d = distinct terms of document d = its postings; cum[N] = P):
+// b_s = smallest d > b_{s-1} with cum[d] >= ceil(s·P/S), clamped so that the shards s..S-1 keep one document each.
+static std::vector<uint32_t> shard_bounds(const uint32_t *doc_bounds, const std::vector<uint64_t> &cum, uint32_t N,
+                                          uint32_t S) {
+    std::vector<uint32_t> bounds((size_t)S + 1);
+    if (doc_bounds) {
+        std::copy(doc_bounds, doc_bounds + S + 1, bounds.begin());
+        return bounds;
+    }
+    const uint64_t P = cum[N];
+    bounds[0] = 0;
+    for (uint32_t s = 1; s < S; s++) {
+        const uint64_t target = ((uint64_t)s * P + S - 1) / S;
+        // smallest d > b_{s-1} with cum[d] >= target (cum ascends; cum[N] = P >= target)
+        uint32_t d = (uint32_t)(std::lower_bound(cum.begin() + bounds[s - 1] + 1, cum.end(), target) - cum.begin());
+        bounds[s] = std::min<uint32_t>(d, N - (S - s));
+    }
+    bounds[S] = N;
+    return bounds;
+}
+
 extern "C" int bm25x_sharded_create(const bm25x_corpus *c, uint32_t S, const uint32_t *doc_bounds, const int *devices,
                                     bm25x_sharded_index **out) {
     const char *who = "bm25x_sharded_create";
@@ -746,42 +796,20 @@ extern "C" int bm25x_sharded_create(const bm25x_corpus *c, uint32_t S, const uin
     if (rc != BM25X_OK) return rc;
     const uint32_t N = c->n_docs, T = c->n_terms;
     const uint64_t P = c->post_off[T];
-    if (S == 0 || S > BM25X_MAX_SHARDS) {
-        bm25x_set_error("%s: n_shards=%u must be 1..%d", who, S, BM25X_MAX_SHARDS);
-        return BM25X_ERR_INVALID;
-    }
-    if (N < S) {
-        bm25x_set_error("%s: n_docs=%u < n_shards=%u (every shard holds at least one document)", who, N, S);
-        return BM25X_ERR_INVALID;
-    }
-    std::vector<uint32_t> bounds((size_t)S + 1);
-    if (doc_bounds) {
-        bool ok = doc_bounds[0] == 0 && doc_bounds[S] == N;
-        for (uint32_t s = 0; s < S && ok; s++) ok = doc_bounds[s] < doc_bounds[s + 1];
-        if (!ok) {
-            bm25x_set_error("%s: doc_bounds must ascend strictly from 0 to n_docs=%u", who, N);
-            return BM25X_ERR_INVALID;
-        }
-        std::copy(doc_bounds, doc_bounds + S + 1, bounds.begin());
-    } else {
-        // balanced by postings: c_d = distinct terms of document d = its postings; b_s = smallest d > b_{s-1} with
-        // Σ_{d' < d} c_{d'} >= ceil(s·P/S), clamped so that the shards s..S-1 keep one document each
-        std::vector<uint64_t> cum((size_t)N + 1, 0);
+    rc = check_shard_args(N, S, doc_bounds);
+    if (rc != BM25X_OK) return rc;
+    std::vector<uint64_t> cum;
+    if (!doc_bounds) {
+        cum.assign((size_t)N + 1, 0);
 #pragma omp parallel for schedule(static) num_threads(bm25x_host_threads(0))
         for (uint64_t p = 0; p < P; p++) {
 #pragma omp atomic
             cum[(size_t)c->post_doc[p] + 1]++;
         }
         for (uint32_t d = 0; d < N; d++) cum[(size_t)d + 1] += cum[d];
-        bounds[0] = 0;
-        for (uint32_t s = 1; s < S; s++) {
-            const uint64_t target = ((uint64_t)s * P + S - 1) / S;
-            // smallest d > b_{s-1} with cum[d] >= target (cum ascends; cum[N] = P >= target)
-            uint32_t d = (uint32_t)(std::lower_bound(cum.begin() + bounds[s - 1] + 1, cum.end(), target) - cum.begin());
-            bounds[s] = std::min<uint32_t>(d, N - (S - s));
-        }
-        bounds[S] = N;
     }
+    const std::vector<uint32_t> bounds = shard_bounds(doc_bounds, cum, N, S);
+    std::vector<uint64_t>().swap(cum);
     std::vector<int> dev(S, 0);
     if (devices) std::copy(devices, devices + S, dev.begin());
     for (uint32_t s = 0; s < S; s++) {
@@ -851,13 +879,14 @@ extern "C" int bm25x_sharded_create(const bm25x_corpus *c, uint32_t S, const uin
 }
 
 // ---- f1: the sealed segment as the reference stores it (blocks in the codec of compression.rs), decoded on the GPU ----
-extern "C" int bm25x_index_create_from_blocks(const bm25x_blocks *c, int device, bm25x_index **out) {
+
+// Host validation of the stored blocks, shared by bm25x_index_create_from_blocks and
+// bm25x_index_create_sharded_from_blocks: same codes, same messages.  Gives each token's postings (df) and their total P.
+// check_device == false leaves the device check to the caller (the sharded build checks its shard arguments first, so
+// that they are refused without a GPU).
+static int validate_blocks(const bm25x_blocks *c, int device, bool check_device, std::vector<uint32_t> &df,
+                           uint64_t &n_post) {
     const char *who = "bm25x_index_create_from_blocks";
-    if (!c || !out) {
-        bm25x_set_error("%s: null argument", who);
-        return BM25X_ERR_INVALID;
-    }
-    *out = nullptr;
     const uint32_t N = c->n_docs, T = c->n_terms;
     const uint64_t NB = c->n_blocks;
     if (!c->term_blk_off || (NB && (!c->blk_min_doc || !c->blk_n || !c->blk_meta_doc || !c->blk_meta_tf ||
@@ -866,13 +895,13 @@ extern "C" int bm25x_index_create_from_blocks(const bm25x_blocks *c, int device,
         return BM25X_ERR_INVALID;
     }
     int rc = check_common(who, N, c->doc_len ? (const void *)c->doc_len : (const void *)c->doc_fieldnorm, c->k1, c->b, device);
-    if (rc != BM25X_OK) return rc;
+    if (rc != BM25X_OK && (check_device || rc != BM25X_ERR_CUDA)) return rc;
     if (c->term_blk_off[0] != 0 || c->term_blk_off[T] != NB) {
         bm25x_set_error("%s: term_blk_off must run from 0 to n_blocks", who);
         return BM25X_ERR_INVALID;
     }
     // ---- host-side validation of the block directory (payloads are validated by the decoder on the device) ----
-    std::vector<uint32_t> df(T);
+    df.assign(T, 0);
     uint64_t P = 0;
     int bad = 0;
 #pragma omp parallel for schedule(dynamic, 256) reduction(| : bad) reduction(+ : P) num_threads(bm25x_host_threads(0))
@@ -916,8 +945,46 @@ extern "C" int bm25x_index_create_from_blocks(const bm25x_blocks *c, int device,
         bm25x_set_error("%s: corrupt block metadata (bitwidth out of bound / unexpected input len)", who);
         return BM25X_ERR_INVALID;
     }
-    rc = check_keys(who, c->term_key, T);
+    n_post = P;
+    return check_keys(who, c->term_key, T);
+}
+
+// The refusal for the error bits of the decode and check kernels (bm25x_blocks.cuh), with the messages of
+// bm25x_index_create_from_blocks whichever entry point decoded the blocks.
+static int blocks_refusal(uint32_t h_err) {
+    const char *who = "bm25x_index_create_from_blocks";
+    if (h_err & BM25X_BLKERR_RANGE) {
+        bm25x_set_error("%s: corrupt blocks (doc ids must be < n_docs and strictly ascending per token, tf != 0)", who);
+        return BM25X_ERR_INVALID;
+    }
+    if (h_err & BM25X_BLKERR_TF) {
+        bm25x_set_error("%s: term frequency >= 2^24 is not supported by the packed posting layout", who);
+        return BM25X_ERR_UNSUPPORTED;
+    }
+    if (h_err & BM25X_BLKERR_WAND) {
+        bm25x_set_error("%s: corrupt blocks (SummaryTuple wand_fieldnorm/wand_term_frequency is not the block's maximum)", who);
+        return BM25X_ERR_INVALID;
+    }
+    if (h_err & BM25X_BLKERR_DIR) {  // only blocks staged by the sharded build: the caller's directory changed under it
+        bm25x_set_error("%s: corrupt block directory (block sizes, token ranges or payload offsets)", who);
+        return BM25X_ERR_INVALID;
+    }
+    return BM25X_OK;
+}
+
+extern "C" int bm25x_index_create_from_blocks(const bm25x_blocks *c, int device, bm25x_index **out) {
+    const char *who = "bm25x_index_create_from_blocks";
+    if (!c || !out) {
+        bm25x_set_error("%s: null argument", who);
+        return BM25X_ERR_INVALID;
+    }
+    *out = nullptr;
+    std::vector<uint32_t> df;
+    uint64_t P = 0;
+    int rc = validate_blocks(c, device, true, df, P);
     if (rc != BM25X_OK) return rc;
+    const uint32_t N = c->n_docs, T = c->n_terms;
+    const uint64_t NB = c->n_blocks;
 
     BuildMeta m{N, T, c->doc_len, c->payload, c->term_key, c->k1, c->b, df.data(), P};
     m.fieldnorm = c->doc_fieldnorm;
@@ -986,22 +1053,338 @@ extern "C" int bm25x_index_create_from_blocks(const bm25x_blocks *c, int device,
         bm25x_index_destroy(ix);
         return e == cudaErrorMemoryAllocation ? BM25X_ERR_OOM : BM25X_ERR_CUDA;
     }
-    if (h_err & BM25X_BLKERR_RANGE) {
-        bm25x_set_error("%s: corrupt blocks (doc ids must be < n_docs and strictly ascending per token, tf != 0)", who);
+    rc = blocks_refusal(h_err);
+    if (rc != BM25X_OK) {
         bm25x_index_destroy(ix);
-        return BM25X_ERR_INVALID;
-    }
-    if (h_err & BM25X_BLKERR_TF) {
-        bm25x_set_error("%s: term frequency >= 2^24 is not supported by the packed posting layout", who);
-        bm25x_index_destroy(ix);
-        return BM25X_ERR_UNSUPPORTED;
-    }
-    if (h_err & 8u) {
-        bm25x_set_error("%s: corrupt blocks (SummaryTuple wand_fieldnorm/wand_term_frequency is not the block's maximum)", who);
-        bm25x_index_destroy(ix);
-        return BM25X_ERR_INVALID;
+        return rc;
     }
     *out = ix;
+    return BM25X_OK;
+}
+
+// ---- a document-sharded index from the stored blocks (DESIGN §4.7): one check pass over the whole segment on shard 0's
+// device, then per shard a decode of just the stored blocks that hold its documents, on its own device ----
+
+// Device scratch of one build step on one device, freed when it goes out of scope (every refusal included).  The first
+// failure sticks in `e`; later calls do nothing.
+struct Scratch {
+    int device;
+    cudaError_t e = cudaSuccess;
+    std::vector<void *> ptrs;
+    explicit Scratch(int dev) : device(dev) {}
+    Scratch(const Scratch &) = delete;
+    ~Scratch() {
+        if (ptrs.empty()) return;
+        cudaSetDevice(device);
+        for (void *p : ptrs) cudaFree(p);
+    }
+    template <typename T>
+    T *alloc(size_t n) {
+        T *p = nullptr;
+        if (e == cudaSuccess) e = cudaMalloc((void **)&p, sizeof(T) * (n ? n : 1));
+        if (e != cudaSuccess) return nullptr;
+        ptrs.push_back(p);
+        return p;
+    }
+    template <typename T>
+    T *up(const T *h, size_t n) {
+        T *p = alloc<T>(n);
+        if (e == cudaSuccess && n) e = cudaMemcpy(p, h, sizeof(T) * n, cudaMemcpyHostToDevice);
+        return p;
+    }
+};
+
+// Directory entries and payloads of some stored blocks, gathered back to back with the offsets rebased to `bytes`: what a
+// kernel of bm25x_blocks.cuh reads for just these blocks.  The directory has passed validate_blocks.
+struct StagedBlocks {
+    std::vector<uint32_t> min, n;
+    std::vector<uint8_t> md, mt;
+    std::vector<uint64_t> doff, toff;
+    std::vector<uint8_t> bytes;
+
+    void gather(const bm25x_blocks *c, const uint64_t *ids, size_t nb) {
+        min.resize(nb);
+        n.resize(nb);
+        md.resize(nb);
+        mt.resize(nb);
+        doff.resize(nb);
+        toff.resize(nb);
+        uint64_t pos = 0;
+        for (size_t j = 0; j < nb; j++) {
+            const uint64_t g = ids[j];
+            min[j] = c->blk_min_doc[g];
+            n[j] = c->blk_n[g];
+            md[j] = c->blk_meta_doc[g];
+            mt[j] = c->blk_meta_tf[g];
+            doff[j] = pos;
+            pos += stream_bytes(md[j], n[j]);
+            toff[j] = pos;
+            pos += stream_bytes(mt[j], n[j]);
+        }
+        bytes.resize(pos ? pos : 1);
+        n_bytes = pos;
+#pragma omp parallel for schedule(static) num_threads(bm25x_host_threads(0))
+        for (size_t j = 0; j < nb; j++) {
+            const uint64_t g = ids[j];
+            memcpy(bytes.data() + doff[j], c->bytes + c->blk_doc_off[g], toff[j] - doff[j]);
+            memcpy(bytes.data() + toff[j], c->bytes + c->blk_tf_off[g], stream_bytes(mt[j], n[j]));
+        }
+    }
+    uint64_t n_bytes = 0;
+};
+
+static int scratch_failed(const char *who, cudaError_t e) {
+    bm25x_set_error("%s: block upload/decode failed: %s", who, cudaGetErrorString(e));
+    return e == cudaErrorMemoryAllocation ? BM25X_ERR_OOM : BM25X_ERR_CUDA;
+}
+
+// The check pass: every stored block decoded once on `device`, in chunks of at most 256 MiB of payload (so the compressed
+// segment never has to fit on one GPU), with every check bm25x_index_create_from_blocks makes on the device.  Gives the
+// error bits, each block's decoded (first, last) doc id, and with cum != NULL the postings of the documents < d (cum[d]).
+// fieldnorm, s0d and s1d are the segment's; they are read only to check the stored wand pairs.
+static int check_stored_blocks(const char *who, const bm25x_blocks *c, const uint8_t *fieldnorm, const double *s0d,
+                               const double *s1d, int device, std::vector<uint2> &first_last, std::vector<uint64_t> *cum,
+                               uint32_t &h_err) {
+    const uint32_t N = c->n_docs, T = c->n_terms;
+    const uint64_t NB = c->n_blocks;
+    const bool wand = c->blk_wand_fieldnorm && c->blk_wand_tf;
+    first_last.assign(NB, make_uint2(0, 0));
+    h_err = 0;
+    Scratch sc(device);
+    sc.e = cudaSetDevice(device);
+    const uint64_t *d_tbo = sc.up(c->term_blk_off, (size_t)T + 1);
+    const uint8_t *d_fn = wand ? sc.up(fieldnorm, N) : nullptr;  // the whole segment's norms: a block may straddle a bound
+    const double *d_s0d = wand ? sc.up(s0d, T) : nullptr;
+    const double *d_s1d = wand ? sc.up(s1d, 256) : nullptr;
+    uint32_t *d_cnt = cum ? sc.alloc<uint32_t>(N) : nullptr;
+    if (d_cnt && sc.e == cudaSuccess) sc.e = cudaMemset(d_cnt, 0, sizeof(uint32_t) * (size_t)N);
+    uint32_t *d_err = sc.up(&h_err, 1);
+    const uint64_t CH_BYTES = 256ull << 20, CH_BLOCKS = 1ull << 21;
+    std::vector<uint64_t> ids;
+    StagedBlocks st;
+    for (uint64_t g0 = 0; g0 < NB && sc.e == cudaSuccess;) {
+        uint64_t g1 = g0, nbytes = 0;
+        while (g1 < NB && g1 - g0 < CH_BLOCKS) {
+            const uint64_t b = (uint64_t)stream_bytes(c->blk_meta_doc[g1], c->blk_n[g1]) +
+                               stream_bytes(c->blk_meta_tf[g1], c->blk_n[g1]);
+            if (g1 > g0 && nbytes + b > CH_BYTES) break;
+            nbytes += b;
+            g1++;
+        }
+        const uint64_t nb = g1 - g0;
+        ids.resize(nb);
+        for (uint64_t j = 0; j < nb; j++) ids[j] = g0 + j;
+        st.gather(c, ids.data(), nb);
+        Scratch ch(device);
+        const uint32_t *d_min = ch.up(st.min.data(), nb), *d_n = ch.up(st.n.data(), nb);
+        const uint8_t *d_md = ch.up(st.md.data(), nb), *d_mt = ch.up(st.mt.data(), nb);
+        const uint64_t *d_doff = ch.up(st.doff.data(), nb), *d_toff = ch.up(st.toff.data(), nb);
+        const uint8_t *d_bytes = ch.up(st.bytes.data(), st.bytes.size());
+        const uint8_t *d_wfn = wand ? ch.up(c->blk_wand_fieldnorm + g0, nb) : nullptr;
+        const uint32_t *d_wtf = wand ? ch.up(c->blk_wand_tf + g0, nb) : nullptr;
+        uint2 *d_fl = ch.alloc<uint2>(nb);
+        if (ch.e == cudaSuccess) {
+            k_check_blocks<<<(unsigned)((nb + DEC_WARPS - 1) / DEC_WARPS), DEC_WARPS * 32>>>(
+                g0, nb, d_tbo, T, d_min, d_n, d_md, d_mt, d_doff, d_toff, d_bytes, st.n_bytes, d_fn, N, d_wfn, d_wtf, d_s0d,
+                d_s1d, d_fl, d_cnt, d_err);
+            ch.e = cudaGetLastError();
+        }
+        if (ch.e == cudaSuccess) ch.e = cudaMemcpy(first_last.data() + g0, d_fl, sizeof(uint2) * nb, cudaMemcpyDeviceToHost);
+        sc.e = ch.e;
+        g0 = g1;
+    }
+    if (sc.e == cudaSuccess) sc.e = cudaMemcpy(&h_err, d_err, sizeof(h_err), cudaMemcpyDeviceToHost);
+    if (sc.e == cudaSuccess && cum) {
+        std::vector<uint32_t> cnt(N);
+        sc.e = cudaMemcpy(cnt.data(), d_cnt, sizeof(uint32_t) * (size_t)N, cudaMemcpyDeviceToHost);
+        cum->assign((size_t)N + 1, 0);
+        for (uint32_t d = 0; d < N; d++) (*cum)[(size_t)d + 1] = (*cum)[d] + cnt[d];
+    }
+    if (sc.e != cudaSuccess) return scratch_failed(who, sc.e);
+    // k_check_block_order's rule on the decoded (first, last): ids ascend across the blocks of a token
+    uint32_t order = 0;
+#pragma omp parallel for schedule(dynamic, 256) reduction(| : order) num_threads(bm25x_host_threads(0))
+    for (uint32_t t = 0; t < T; t++)
+        for (uint64_t g = c->term_blk_off[t] + 1; g < c->term_blk_off[t + 1]; g++)
+            if (first_last[g].x <= first_last[g - 1].y) order |= BM25X_BLKERR_RANGE;
+    h_err |= order;
+    return BM25X_OK;
+}
+
+// Shard s of sx from the stored blocks, on `device`: the blocks whose decoded [first, last] meets [lo, hi) gathered with
+// rebased offsets (host memory beyond the caller's: this payload), counted (k_count_shard_blocks), then the shard index
+// allocated with the whole segment's statistics, decoded into place (k_decode_shard_blocks) and finished as every index is.
+static int build_shard_from_blocks(const char *who, const bm25x_blocks *c, const std::vector<uint2> &first_last,
+                                   const bm25x_sharded_index *sx, uint32_t s, int device, bm25x_index **out) {
+    *out = nullptr;
+    const uint32_t T = c->n_terms, lo = sx->bounds[s], hi = sx->bounds[s + 1];
+    // ---- select: per token the run of its blocks with last >= lo and first < hi (both ascend along the chain) ----
+    std::vector<uint64_t> sel_b0(T), sel_off((size_t)T + 1, 0);
+#pragma omp parallel for schedule(dynamic, 256) num_threads(bm25x_host_threads(0))
+    for (uint32_t t = 0; t < T; t++) {
+        const uint2 *a = first_last.data() + c->term_blk_off[t], *e = first_last.data() + c->term_blk_off[t + 1];
+        const uint2 *b0 = std::partition_point(a, e, [&](const uint2 &f) { return f.y < lo; });
+        const uint2 *b1 = std::partition_point(b0, e, [&](const uint2 &f) { return f.x < hi; });
+        sel_b0[t] = (uint64_t)(b0 - first_last.data());
+        sel_off[(size_t)t + 1] = (uint64_t)(b1 - b0);
+    }
+    for (uint32_t t = 0; t < T; t++) sel_off[(size_t)t + 1] += sel_off[t];
+    const uint64_t nsel = sel_off[T];
+    std::vector<uint64_t> ids(nsel);
+    std::vector<uint2> sel_fl(nsel);
+#pragma omp parallel for schedule(dynamic, 256) num_threads(bm25x_host_threads(0))
+    for (uint32_t t = 0; t < T; t++)
+        for (uint64_t j = sel_off[t]; j < sel_off[(size_t)t + 1]; j++) {
+            ids[j] = sel_b0[t] + (j - sel_off[t]);
+            sel_fl[j] = first_last[ids[j]];
+        }
+    StagedBlocks st;
+    st.gather(c, ids.data(), nsel);
+    std::vector<uint64_t>().swap(ids);
+    // ---- count: the shard's df, and each selected block's rank inside its token's shard list ----
+    Scratch sc(device);
+    sc.e = cudaSetDevice(device);
+    const uint32_t *d_min = sc.up(st.min.data(), nsel), *d_n = sc.up(st.n.data(), nsel);
+    const uint8_t *d_md = sc.up(st.md.data(), nsel), *d_mt = sc.up(st.mt.data(), nsel);
+    const uint64_t *d_doff = sc.up(st.doff.data(), nsel), *d_toff = sc.up(st.toff.data(), nsel);
+    const uint8_t *d_bytes = sc.up(st.bytes.data(), st.bytes.size());
+    const uint2 *d_fl = sc.up(sel_fl.data(), nsel);
+    const uint64_t *d_sel_off = sc.up(sel_off.data(), (size_t)T + 1);
+    uint2 *d_cs = sc.alloc<uint2>(nsel);
+    uint32_t h_err = 0, *d_err = sc.up(&h_err, 1);
+    const unsigned grid = (unsigned)((nsel + DEC_WARPS - 1) / DEC_WARPS);
+    if (sc.e == cudaSuccess && nsel) {
+        k_count_shard_blocks<<<grid, DEC_WARPS * 32>>>(nsel, d_fl, d_min, d_n, d_md, d_doff, d_bytes, st.n_bytes, lo, hi,
+                                                        d_cs, d_err);
+        sc.e = cudaGetLastError();
+    }
+    std::vector<uint2> cs(nsel);
+    if (sc.e == cudaSuccess && nsel) sc.e = cudaMemcpy(cs.data(), d_cs, sizeof(uint2) * nsel, cudaMemcpyDeviceToHost);
+    if (sc.e != cudaSuccess) return scratch_failed(who, sc.e);
+    std::vector<uint32_t> df(T), rank(nsel);
+    uint64_t Ps = 0;
+    for (uint32_t t = 0; t < T; t++) {
+        uint64_t run = 0;
+        for (uint64_t j = sel_off[t]; j < sel_off[(size_t)t + 1]; j++) {
+            rank[j] = (uint32_t)std::min<uint64_t>(run, 0xFFFFFFFFu);
+            run += cs[j].x;
+        }
+        df[t] = (uint32_t)std::min<uint64_t>(run, hi - lo);  // more than the shard's documents: refused by the decode
+        Ps += df[t];
+    }
+    // ---- allocate the shard as bm25x_sharded_create does (the term keys once, with shard 0) ----
+    BuildMeta m{hi - lo, T, c->doc_len ? c->doc_len + lo : nullptr, c->payload ? c->payload + (size_t)lo * 3 : nullptr,
+                s ? nullptr : c->term_key, c->k1, c->b, df.data(), Ps};
+    m.fieldnorm = c->doc_len ? nullptr : c->doc_fieldnorm + lo;
+    m.sum_len = c->sum_doc_len;  // stored norms: the pages hold the segment's sum only
+    m.stat_df = sx->h_df.data();
+    m.stat_n_docs = sx->n_docs;
+    m.stat_avgdl = sx->avgdl;
+    m.doc_base = lo;
+    bm25x_index *ix = nullptr;
+    int rc = index_begin(m, device, &ix);
+    if (rc != BM25X_OK) return rc;
+    // ---- write the postings, then what every index derives from them ----
+    const uint32_t *d_rank = sc.up(rank.data(), nsel);
+    if (sc.e == cudaSuccess && nsel) {
+        k_decode_shard_blocks<<<grid, DEC_WARPS * 32>>>(nsel, d_sel_off, T, d_min, d_n, d_md, d_mt, d_doff, d_toff, d_bytes,
+                                                         st.n_bytes, d_cs, d_rank, sx->n_docs, lo, hi - lo,
+                                                         ix->d.post_off, ix->d.df, ix->d.fieldnorm, ix->d.post, d_err);
+        sc.e = cudaGetLastError();
+    }
+    if (sc.e == cudaSuccess) sc.e = cudaMemcpy(&h_err, d_err, sizeof(h_err), cudaMemcpyDeviceToHost);
+    if (sc.e == cudaSuccess && !h_err) sc.e = index_finish_device(ix);
+    if (sc.e != cudaSuccess) {
+        rc = scratch_failed(who, sc.e);
+        bm25x_index_destroy(ix);
+        return rc;
+    }
+    rc = blocks_refusal(h_err);
+    if (rc != BM25X_OK) {
+        bm25x_index_destroy(ix);
+        return rc;
+    }
+    *out = ix;
+    return BM25X_OK;
+}
+
+extern "C" int bm25x_index_create_sharded_from_blocks(const bm25x_blocks *c, uint32_t S, const uint32_t *doc_bounds,
+                                                      const int *devices, bm25x_sharded_index **out) {
+    const char *who = "bm25x_index_create_sharded_from_blocks";
+    if (!c || !out) {
+        bm25x_set_error("%s: null argument", who);
+        return BM25X_ERR_INVALID;
+    }
+    *out = nullptr;
+    // every host check before any device is used: the blocks exactly as bm25x_index_create_from_blocks checks them, then
+    // the shard arguments exactly as bm25x_sharded_create checks them
+    std::vector<uint32_t> df;
+    uint64_t P = 0;
+    int rc = validate_blocks(c, 0, false, df, P);
+    if (rc != BM25X_OK) return rc;
+    const uint32_t N = c->n_docs, T = c->n_terms;
+    rc = check_shard_args(N, S, doc_bounds);
+    if (rc != BM25X_OK) return rc;
+    std::vector<int> dev(S, 0);
+    if (devices) std::copy(devices, devices + S, dev.begin());
+    const void *norms = c->doc_len ? (const void *)c->doc_len : (const void *)c->doc_fieldnorm;
+    for (uint32_t s = 0; s < S; s++) {
+        rc = check_common(who, N, norms, c->k1, c->b, dev[s]);
+        if (rc != BM25X_OK) return rc;
+    }
+    // ---- the segment's norms and statistics, as index_begin computes them for the unsharded index ----
+    std::vector<uint8_t> h_fn;
+    const uint8_t *fn = c->doc_fieldnorm;
+    uint64_t sum_len = c->sum_doc_len;
+    if (c->doc_len) {
+        h_fn.resize(N);
+        sum_len = 0;
+#pragma omp parallel for reduction(+ : sum_len) num_threads(bm25x_host_threads(0))
+        for (uint32_t d = 0; d < N; d++) {
+            sum_len += c->doc_len[d];
+            h_fn[d] = bm25x_length_to_fieldnorm(c->doc_len[d]);
+        }
+        fn = h_fn.data();
+    }
+    const double avgdl = (double)sum_len / (double)N;
+    std::vector<double> s0d(T);
+    for (uint32_t t = 0; t < T; t++) s0d[t] = bm25_s0((double)df[t], (double)N, c->k1);
+    double s1d[256];
+    bm25_s1(c->k1, c->b, avgdl, s1d);
+    // ---- check pass on shard 0's device: the refusals of the unsharded ingest, before any shard exists ----
+    std::vector<uint2> first_last;
+    std::vector<uint64_t> cum;
+    uint32_t h_err = 0;
+    rc = check_stored_blocks(who, c, fn, s0d.data(), s1d, dev[0], first_last, doc_bounds ? nullptr : &cum, h_err);
+    if (rc != BM25X_OK) return rc;
+    rc = blocks_refusal(h_err);
+    if (rc != BM25X_OK) return rc;
+    std::vector<uint8_t>().swap(h_fn);
+    const std::vector<uint32_t> bounds = shard_bounds(doc_bounds, cum, N, S);
+    std::vector<uint64_t>().swap(cum);
+
+    bm25x_sharded_index *sx = new bm25x_sharded_index();
+    sx->n_shards = S;
+    sx->bounds = bounds;
+    sx->n_docs = N;
+    sx->n_terms = T;
+    sx->n_post = P;
+    sx->k1 = c->k1;
+    sx->b = c->b;
+    sx->h_df = df;
+    sx->sum_len = sum_len;
+    sx->avgdl = avgdl;  // the expression of index_begin: the shards' s1 tables are the unsharded index's
+    // one shard at a time: host memory beyond the blocks stays within one shard's selected payload
+    for (uint32_t s = 0; s < S; s++) {
+        bm25x_index *ix = nullptr;
+        rc = build_shard_from_blocks(who, c, first_last, sx, s, dev[s], &ix);
+        if (rc != BM25X_OK) {
+            bm25x_sharded_destroy(sx);
+            return rc;
+        }
+        sx->shards.push_back(ix);
+    }
+    *out = sx;
     return BM25X_OK;
 }
 

@@ -21,9 +21,9 @@ LIB = os.path.join(ROOT, "vectorchord-bm25_b200", "variants", "libbm25x_phasepro
 
 # order of the PP_* enum in bm25x_search_ring.cuh
 PHASES = ["query start / end", "refill wait", "window setup", "map clear", "seed listing", "stream trips",
-          "compaction", "verify: ring searches", "verify: word-load wait", "verify: filter+exact+pool",
+          "compaction", "verify: ring searches", "flush: word-load wait", "hit append; flush: filter+exact+pool",
           "chunk end / refill issue"]
-COUNTERS = ["chunks", "listed candidates", "hits"]
+COUNTERS = ["chunks", "listed candidates", "hits", "flushes", "rows"]
 
 
 def main():
@@ -66,13 +66,14 @@ def main():
     rows = [{"phase": ph, "share": c_ / total, "cycles_per_chunk": c_ / chunks} for ph, c_ in zip(PHASES, cyc)]
     print(f"seeded k<=32 launches, {a.runs} runs of {a.queries} queries on {a.docs} docs "
           f"(profiled kernel time {min(ms):.2f} ms: not a benchmark number)")
-    print(f"{'phase':28s} {'share':>7s} {'cycles/chunk':>13s}")
+    print(f"{'phase':38s} {'share':>7s} {'cycles/chunk':>13s}")
     for r in rows:
-        print(f"{r['phase']:28s} {100 * r['share']:6.1f}% {r['cycles_per_chunk']:13.0f}")
-    print(f"{'total':28s} {100.0:6.1f}% {total / chunks:13.0f}")
+        print(f"{r['phase']:38s} {100 * r['share']:6.1f}% {r['cycles_per_chunk']:13.0f}")
+    print(f"{'total':38s} {100.0:6.1f}% {total / chunks:13.0f}")
     per_run = {k_: v_ / a.runs for k_, v_ in cnt.items()}
     print("per run: " + ", ".join(f"{k_} {v_:,.0f}" for k_, v_ in per_run.items()) +
-          f"; per chunk: {cnt['listed candidates'] / chunks:.2f} listed, {cnt['hits'] / chunks:.2f} hits")
+          f"; per chunk: {cnt['listed candidates'] / chunks:.2f} listed, {cnt['hits'] / chunks:.2f} hits"
+          f"; hit-list rows per flush: {cnt['rows'] / max(1, cnt['flushes']):.2f}")
     if a.json:
         with open(a.json, "w") as fh:
             json.dump({"rows": rows, "counters": cnt, "runs": a.runs, "kernel_ms": ms}, fh, indent=1)

@@ -38,7 +38,7 @@ int launch_ring(int device, int sm_count, const SearchParams &sp_in, cudaStream_
 
 #if defined(BM25X_PHASE_PROF) && BM25X_RING_KP == 64
 // diagnostic builds only (tools/phase_profile.py): copies the phase profile of the seeded k <= 32 classes to `out`
-// (PP_SLOTS values: cycles per phase, then chunks, listed candidates, hits) and zeroes it when `reset` is set
+// (PP_SLOTS values: cycles per phase, then chunks, listed candidates, hits, hit-list flushes and rows) and zeroes it when `reset` is set
 extern "C" int bm25x_phase_prof(unsigned long long *out, int reset) {
     if (out) BM25X_CUDA_TRY(cudaMemcpyFromSymbol(out, g_phase_prof, sizeof(g_phase_prof)));
     if (reset) {

@@ -36,7 +36,9 @@
 // top-k if it is among the first k champions of its term).  Its seeds join the candidate list of the doc window they
 // fall into and go through the ordinary verification; the stream itself then never tests a posting on its own, so the
 // rings hold doc ids only (DeviceIndex::pdoc, 4 B per posting: twice the postings per ring byte, half the HBM bytes),
-// posting words are fetched from HBM for the holders of verified documents alone, and there is no pruning: queries
+// posting words are fetched from HBM for the holders of verified documents alone — the ring searches of a verification
+// pass only list them in a per-warp hit list, scored (word loads, filter, exact score, pool) up to 32 at a time across
+// passes and windows (classes with room for 16 rows or more, RCfg::HITS) — and there is no pruning: queries
 // with a dense list or a list much longer than another one are handed back to the plain kernel (PH 4 launch behind
 // it).  PH 1 / 2 (off by default): plain kernel that suspends a query once no posting can pass alone + doc-id-only kernel
 // that resumes it.
@@ -183,13 +185,28 @@ struct RCfg {
     static constexpr uint32_t SST = KP_ <= 64 ? 32u : 128u;
     static constexpr bool SEEDS_SMEM = SEEDED;
     static constexpr size_t off_seed = (off_cand + (size_t)LCAP * 2 + 7) & ~(size_t)7;
-    static constexpr size_t off_bar = off_seed + (SEEDS_SMEM ? (size_t)M_ * SST * 8 : 0);
-    static constexpr size_t warp_bytes = (off_bar + 8 + 127) & ~(size_t)127;
+    static constexpr size_t off_hit = off_seed + (SEEDS_SMEM ? (size_t)M_ * SST * 8 : 0);
     static constexpr size_t off_s1f = 0;  // CTA-shared: 1 KiB table first, then the warps
     static constexpr size_t shared_bytes = 1024;
-    static constexpr int WARPS_FIT = (int)((227 * 1024 - shared_bytes) / warp_bytes);
     static constexpr int MAXW = M_ == 1 ? (BM25X_RING_MAXWARPS > 20 ? BM25X_RING_MAXWARPS : 20) : BM25X_RING_MAXWARPS;
+    // seeded launches: the hit list — verified documents waiting for their posting words, scored up to HCAP at a time
+    // across windows (struct of arrays: doc ids, then per run the holder's posting index, or the seed's word).  It takes
+    // what the 128-byte rounding of the warp's area leaves, up to 32 rows, and never costs a resident warp.  Classes
+    // with room for fewer than 16 rows (4 terms at k <= 32, 2 terms at k > 32, 5..8 terms) score each pass's documents
+    // right away: a pass can list 32 of them, and a short list would be flushed several times per pass.
+    static constexpr int WARPS_NOHIT = (int)((227 * 1024 - shared_bytes) / ((off_hit + 8 + 127) & ~(size_t)127)) > MAXW
+                                           ? MAXW
+                                           : (int)((227 * 1024 - shared_bytes) / ((off_hit + 8 + 127) & ~(size_t)127));
+    static constexpr size_t HIT_ROOM = (((227 * 1024 - shared_bytes) / (WARPS_NOHIT > 0 ? WARPS_NOHIT : 1)) & ~(size_t)127) - (off_hit + 24);
+    static constexpr int HROWS = HIT_ROOM / ((M_ + 1) * 4) > 32 ? 32 : (int)(HIT_ROOM / ((M_ + 1) * 4));
+    static constexpr bool HITS = SEEDED && HROWS >= 16;
+    static constexpr int HCAP = HITS ? HROWS : 0;
+    static constexpr size_t off_hst = (off_hit + (size_t)(M_ + 1) * HCAP * 4 + 7) & ~(size_t)7;  // fill state: rows, seed bits
+    static constexpr size_t off_bar = off_hst + (HITS ? 8 : 0);
+    static constexpr size_t warp_bytes = (off_bar + 8 + 127) & ~(size_t)127;
+    static constexpr int WARPS_FIT = (int)((227 * 1024 - shared_bytes) / warp_bytes);
     static constexpr int WARPS = WARPS_FIT > MAXW ? MAXW : WARPS_FIT;
+    static_assert(!HITS || WARPS == WARPS_NOHIT, "the hit list costs no resident warp");
     static constexpr size_t total = shared_bytes + warp_bytes * WARPS;
     static constexpr int THREADS = WARPS * 32;
     static_assert(WARPS >= 1, "one warp must fit");
@@ -211,13 +228,15 @@ enum : int {
     PP_STREAM,   // stream trips (test + mark)
     PP_COMPACT,  // compaction of the detected postings
     PP_VSEARCH,  // verification: ring searches
-    PP_VLOAD,    // verification: wait for the posting-word loads
-    PP_VEXACT,   // verification: filter, exact re-score, pool insert
+    PP_VLOAD,    // hit-list flush: wait for the posting-word loads
+    PP_VEXACT,   // hit-list append; flush: filter, exact re-score, pool insert
     PP_END,      // chunk end, refill issue
     PP_PHASES,
-    PP_CHUNKS = PP_PHASES,  // counters after the phases: chunks, listed candidates, hits (candidates whose words are loaded)
-    PP_CANDS,
+    PP_CHUNKS = PP_PHASES,  // counters after the phases: chunks, listed candidates, hits (candidates another run confirms,
+    PP_CANDS,               // or seeds no other run holds), flushes of the hit list and the rows they scored
     PP_HITS,
+    PP_FLUSHES,
+    PP_ROWS,
     PP_SLOTS
 };
 #ifdef BM25X_PHASE_PROF
@@ -380,6 +399,7 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
     if (lane == 0) {
         mbar_init(bar, 1);
         mbar_fence_init();
+        if constexpr (C::HITS) *(uint2 *)(ws + C::off_hst) = make_uint2(0u, 0u);  // the hit list starts empty (every query ends drained)
     }
     if (C::M > 1)
         for (int i = lane; i < (int)(C::MAP_BYTES / 16u); i += 32) ((uint4 *)map)[i] = make_uint4(0, 0, 0, 0);
@@ -432,7 +452,8 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                 continue;
             }
         }
-        unsigned long long fetched = 0;
+        // postings fetched by this lane (seeded launches: one term's list, < 2^32 — a register less; summed in 64 bits at query end)
+        typename std::conditional<C::SEEDED, uint32_t, unsigned long long>::type fetched = 0;
         uint32_t probe_steps = 0;
         // per-query pool / threshold state (warp-uniform registers)
         int pn = 0;
@@ -609,6 +630,128 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                 f.tv = true;
                 thr_new = true;
                 refresh_filter();
+            }
+        };
+        // exact score of a filtered document from its holders' posting words, in the reference's operation order
+        // (Cache::evaluate, bm25.rs:355-358, summed over ascending terms)
+        auto exact_sum = [&](bool keep, const uint32_t (&wv)[C::M], uint32_t &cnt_all) -> double {
+            double Sx = 0.0;
+#pragma unroll
+            for (int i = 0; i < C::M; ++i)
+                if (i < (int)m) {
+                    const double s0 = __shfl_sync(FULL, s0d, i);
+                    if (keep && wv[i]) {
+                        Sx = __dadd_rn(Sx, score_f64(wv[i], s0, p.s1d));
+                        cnt_all++;
+                    }
+                }
+            return Sx;
+        };
+        // a re-scored document enters the pool when it beats the k-th entry so far (score desc, doc asc)
+        auto pool_insert = [&](bool keep, double Sx, uint32_t doc, uint32_t g) {
+            keep = keep && (!f.tv || Sx > f.Sk || (Sx == f.Sk && doc < f.dk));
+            const uint32_t mk = __ballot_sync(FULL, keep);
+            if (keep) {
+                const int idx = pn + __popc(mk & lt_mask);
+                pl.s[idx] = (uint64_t)__double_as_longlong(Sx);
+                pl.d[idx] = doc;
+                pl.g[idx] = g;
+            }
+            pn += __popc(mk);
+            __syncwarp();
+            // Re-sorting a large pool is expensive (bitonic sort of KP entries): once a threshold exists,
+            // the big pool is cut only when it is about to overflow.
+            const bool lazy = C::KP > 128 && f.tv;
+            if (pn > C::KP - 32 || (!lazy && pn >= (int)k + 32)) pool_cut();
+        };
+
+        // ---- seeded launches: the hit list.  The ring searches of a verification pass decide which documents are
+        // live (every holder found, the last streamed holder emits, a seed only when no other run holds it, a streamed
+        // document only when two or more do); a live document needs no ring after that, so it waits here as a row (doc
+        // id; per run the holder's posting index relative to pbase, INF when the run does not hold it — or, for a seed,
+        // its posting word from the seed table and 0 elsewhere) and is scored with up to HCAP - 1 others, one row per
+        // lane: one DRAM latency for all their word loads, one filter / exact / pool-insert chain.  Deferring a document
+        // only lets the threshold it meets be lower (DESIGN.md §5).  The list's fill state (rows; bit r: row r is a
+        // seed) sits beside it in shared memory, not in registers held through the chunk loop.
+        auto hit_flush = [&](uint32_t hn, uint32_t hseed) {
+            const uint32_t *hl = (const uint32_t *)(ws + C::off_hit);
+            __syncwarp();  // every lane's rows are visible
+            PP_COUNT(PP_FLUSHES, 1u);
+            PP_COUNT(PP_ROWS, hn);
+            const bool has = lane < (int)hn;
+            const bool sd = (hseed >> lane) & 1u;
+            const uint32_t doc = has ? hl[lane] : 0u;
+            uint32_t wv[C::M];
+#pragma unroll
+            for (int i = 0; i < C::M; ++i) {
+                const uint32_t v = has ? hl[(i + 1) * C::HCAP + lane] : INF;
+                const uint64_t pbi = __shfl_sync(FULL, pbase, i);
+                wv[i] = sd ? v : (v != INF ? __ldg(&(p.post + pbi)[v].w) : 0u);
+            }
+#pragma unroll
+            for (int i = 0; i < C::M; ++i) PP_CONSUME(wv[i], wv[0]);
+            PP_MARK(PP_VLOAD);
+            float F = 0.f;
+            uint32_t cnt = 0, sig = SIG_NONE;
+#pragma unroll
+            for (int i = 0; i < C::M; ++i) {
+                const float s0 = __shfl_sync(FULL, s0f, i);
+                if (wv[i]) {
+                    F += score_f32(wv[i], s0, s1f);
+                    cnt++;
+                    sig = make_sig(i, wv[i]);
+                }
+            }
+            bool keep = has && wfilter_pass(f, F, cnt == 1 ? sig : SIG_NONE, doc);
+            if (keep && p.allow && !((p.allow[doc >> 3] >> (doc & 7u)) & 1u)) keep = false;
+            if (__any_sync(FULL, keep)) {
+                uint32_t cnt_all = 0;
+                const double Sx = exact_sum(keep, wv, cnt_all);
+                pool_insert(keep, Sx, doc, cnt_all == 1 ? sig : SIG_NONE);
+            }
+            __syncwarp();  // every lane has read its row before the list fills again
+            PP_MARK(PP_VEXACT);
+        };
+        // Before a pass's searches: flush when its c candidates might not fit.  A pass holds at most HCAP candidates,
+        // so its rows always fit after this, and no search result is live across a flush.
+        auto hit_room = [&](uint32_t c) {
+            uint32_t *hst = (uint32_t *)(ws + C::off_hst);
+            const uint32_t hn = hst[0];
+            if (hn != 0u && hn + c > (uint32_t)C::HCAP) {
+                hit_flush(hn, hst[1]);
+                if (lane == 0) hst[0] = hst[1] = 0u;
+                __syncwarp();
+            }
+        };
+        // append the rows of one verification pass (`row`: this lane's document is live; hv: its per-run values)
+        auto hit_append = [&](bool row, uint32_t doc, bool sd, const uint32_t (&hv)[C::M]) {
+            uint32_t *hl = (uint32_t *)(ws + C::off_hit);
+            uint32_t *hst = (uint32_t *)(ws + C::off_hst);
+            const uint32_t mk = __ballot_sync(FULL, row);
+            if (!mk) return;
+            const uint32_t hn = hst[0], r = hn + __popc(mk & lt_mask);
+            if (row) {
+                hl[r] = doc;
+#pragma unroll
+                for (int i = 0; i < C::M; ++i) hl[(i + 1) * C::HCAP + r] = hv[i];
+            }
+            const uint32_t hseed = hst[1] | __reduce_or_sync(FULL, row && sd ? 1u << r : 0u);
+            __syncwarp();
+            if (lane == 0) {
+                hst[0] = hn + __popc(mk);
+                hst[1] = hseed;
+            }
+            __syncwarp();
+        };
+        // the rows of the last windows, before the final cut
+        auto hit_drain = [&]() {
+            uint32_t *hst = (uint32_t *)(ws + C::off_hst);
+            const uint32_t hn = hst[0];
+            if (hn) {
+                PP_MARK(PP_QUERY);
+                hit_flush(hn, hst[1]);
+                if (lane == 0) hst[0] = hst[1] = 0u;
+                __syncwarp();
             }
         };
 
@@ -866,11 +1009,18 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                 // Three streamed runs (the headline class): TWO lanes per listed posting, each searches one of the two
                 // other runs — one search per pass instead of two in a row; the even lane of a pair carries the candidate.
                 const bool pairs = C::M == 3 && !C::ADAPT && !dense && m == 3u && ne_mask == 0u;
-                const uint32_t per_pass = pairs ? 16u : 32u;
+                // seeded launches with a hit list make room for a pass's candidates BEFORE its searches (a pass of
+                // the other lanes then takes at most HCAP candidates)
+                constexpr uint32_t GP = C::HITS && C::HCAP < 32 ? (uint32_t)C::HCAP : 32u;
+                const uint32_t per_pass = pairs ? 16u : GP;
                 PP_COUNT(PP_CANDS, nc);
                 for (uint32_t base = 0; base < nc; base += per_pass) {
                     const uint32_t ci = base + (pairs ? (uint32_t)lane >> 1 : (uint32_t)lane);
                     bool has = ci < nc;
+                    if constexpr (C::HITS) {
+                        has = has && ci < base + per_pass;
+                        hit_room(min(per_pass, nc - base));
+                    }
                     const uint32_t ent = has ? cand[ci] : 0u;
                     const bool by_doc = (ent >> 15) != 0u;            // dense flavour: document given as offset from lo
                     // seeded launches: run field 31 = a seed (champion of term sidx / SST, slot sidx % SST)
@@ -884,6 +1034,7 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                     // doc-id-only rings: the listed posting's word stays in HBM until something needs it — a twin was
                     // found, or run j can still pass alone (wlim): most false alarms of the map never touch HBM
                     const Posting *gown = nullptr;  // DOCRING: &post[posting index] of the listed posting
+                    [[maybe_unused]] uint32_t ownix = INF;  // DOCRING: that posting index (relative to pbase)
                     bool solo_j = false;
                     if constexpr (C::DOCRING) {
                         const uint32_t raj = __shfl_sync(FULL, rd, j & 31u);
@@ -901,7 +1052,8 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                         if (has && !by_doc && !is_seed) {
                             const uint32_t pos = ent & 0x3FFu;
                             own.doc = rings[jbase + pos];
-                            gown = p.post + pbj + (raj + ((pos - raj) & rmj));
+                            ownix = raj + ((pos - raj) & rmj);
+                            gown = p.post + pbj + ownix;
                         }
                     } else {
                         if (has && !by_doc) own = rings[jbase + (ent & 0x3FFu)];
@@ -953,6 +1105,21 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                             const bool live = has && (is_seed ? !anyhit : (anyhit || solo_j));  // (same in both lanes of a pair)
                             PP_MARK(PP_VSEARCH);
                             PP_COUNT(PP_HITS, __popc(__ballot_sync(FULL, live && !(lane & 1))));
+                            if constexpr (C::HITS) {
+                                // the even lane's row: run j (the listed posting or the seed), run o (its own search),
+                                // run ox (the partner's); it waits in the hit list unless a later run holds the document
+                                const uint32_t lx = __shfl_xor_sync(FULL, l, 1);
+                                const uint32_t ox = (lane & 1) ? (j == 0u ? 1u : 0u) : (j == 2u ? 1u : 2u);
+                                const bool later = (l != INF && o > j) || (lx != INF && ox > j);
+                                uint32_t hv[C::M];
+#pragma unroll
+                                for (int i = 0; i < C::M; ++i)
+                                    hv[i] = (uint32_t)i == j ? (is_seed ? own.w : ownix)
+                                                             : (is_seed ? 0u : ((uint32_t)i == o ? l : ((uint32_t)i == ox ? lx : INF)));
+                                hit_append(live && !(lane & 1) && !later, doc, is_seed, hv);
+                                PP_MARK(PP_VEXACT);
+                                continue;
+                            }
                             uint32_t wo = 0u;
                             if (live && hit) wo = __ldg(&(p.post + pbo)[l].w);
                             if (live && !(lane & 1) && !is_seed) own.w = __ldg(&gown->w);
@@ -980,6 +1147,21 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                             const bool live = has && (is_seed ? !anyhit : (by_doc || anyhit || solo_j));
                             PP_MARK(PP_VSEARCH);
                             PP_COUNT(PP_HITS, __popc(__ballot_sync(FULL, live)));
+                            if constexpr (C::HITS) {
+                                // a live row waits in the hit list unless a later run holds the document; a streamed
+                                // (or dense-window) document needs a second holder: one holder alone is a seed's business
+                                bool later = false;
+                                uint32_t nh = by_doc ? 0u : 1u, hv[C::M];
+#pragma unroll
+                                for (int i = 0; i < C::M; ++i) {
+                                    later |= lv[i] != INF && (uint32_t)i > j;
+                                    nh += lv[i] != INF ? 1u : 0u;
+                                    hv[i] = (uint32_t)i == j ? (is_seed ? own.w : ownix) : (is_seed ? 0u : lv[i]);
+                                }
+                                hit_append(live && !later && (is_seed || nh >= 2u), doc, is_seed, hv);
+                                PP_MARK(PP_VEXACT);
+                                continue;
+                            }
 #pragma unroll
                             for (int i = 0; i < C::M; ++i) {
                                 const uint64_t pbi = __shfl_sync(FULL, pbase, i);
@@ -1094,17 +1276,7 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                                         if (ii == i) wv[ii] = wi;
                                 }
                             }
-                            if (__any_sync(FULL, keep)) {
-#pragma unroll
-                                for (int i = 0; i < C::M; ++i)
-                                    if (i < (int)m) {
-                                        const double s0 = __shfl_sync(FULL, s0d, i);
-                                        if (keep && wv[i]) {
-                                            Sx = __dadd_rn(Sx, score_f64(wv[i], s0, p.s1d));
-                                            cnt_all++;
-                                        }
-                                    }
-                            }
+                            if (__any_sync(FULL, keep)) Sx = exact_sum(keep, wv, cnt_all);
                         } else {
                             // posting word of `doc` in a term that is no lane of this pass (two-pass queries)
                             auto probe_term = [&](uint32_t term) -> uint32_t {
@@ -1145,21 +1317,8 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                                 }
                             }
                         }
-                        keep = keep && (!f.tv || Sx > f.Sk || (Sx == f.Sk && doc < f.dk));
                         if constexpr (C::SEEDED) keep = keep && (is_seed ? cnt_all == 1u : cnt_all != 1u);  // (pruned terms probed)
-                        const uint32_t mk = __ballot_sync(FULL, keep);
-                        if (keep) {
-                            const int idx = pn + __popc(mk & lt_mask);
-                            pl.s[idx] = (uint64_t)__double_as_longlong(Sx);
-                            pl.d[idx] = doc;
-                            pl.g[idx] = cnt_all == 1 ? sig : SIG_NONE;
-                        }
-                        pn += __popc(mk);
-                        __syncwarp();
-                        // Re-sorting a large pool is expensive (bitonic sort of KP entries): once a threshold exists,
-                        // the big pool is cut only when it is about to overflow.
-                        const bool lazy = C::KP > 128 && f.tv;
-                        if (pn > C::KP - 32 || (!lazy && pn >= (int)k + 32)) pool_cut();
+                        pool_insert(keep, Sx, doc, cnt_all == 1 ? sig : SIG_NONE);
                     }
                     PP_MARK(PP_VEXACT);
                 }
@@ -1464,6 +1623,7 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
             }
             PP_MARK(PP_END);
         }
+        if constexpr (C::HITS) hit_drain();
         // ---- Results::into_sorted_vec (search.rs:281) (after the last pass; between passes: a tidy pool and threshold) ----
         if (pn > 0 && !suspended) pool_cut();
         }  // passes
@@ -1502,10 +1662,10 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
         }
         if (lane == 0) p.out_n[qid] = (uint32_t)pn;
         if (p.fetched) {
-            fetched += probe_steps;  // block-table entries / postings read by the probes of pruned terms
+            unsigned long long fsum = (unsigned long long)fetched + probe_steps;  // + block-table entries / postings read by the probes of pruned terms
 #pragma unroll
-            for (int o = 16; o > 0; o >>= 1) fetched += __shfl_xor_sync(FULL, fetched, o);
-            if (lane == 0) atomicAdd(p.fetched, fetched);
+            for (int o = 16; o > 0; o >>= 1) fsum += __shfl_xor_sync(FULL, fsum, o);
+            if (lane == 0) atomicAdd(p.fetched, fsum);
         }
 #ifdef BM25X_PHASE_PROF
         PP_MARK(PP_QUERY);

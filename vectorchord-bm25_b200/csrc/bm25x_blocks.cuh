@@ -19,6 +19,18 @@ namespace {
 #define BM25X_BLKERR_DIR 4u    // a staged directory entry that does not describe a payload inside the staged bytes
 #define BM25X_BLKERR_WAND 8u   // SummaryTuple.wand_* is not the block's arg-max
 
+// Owner of index g in an ascending offset array off[0..n]: the last t with off[t] <= g (the term of a posting, the token of a
+// block).
+__device__ __forceinline__ uint32_t owner_of(const uint64_t *__restrict__ off, uint32_t n, uint64_t g) {
+    uint32_t lo = 0, hi = n;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1) >> 1;
+        if (off[mid] <= g) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+
 __device__ __forceinline__ uint32_t sm_u32(const uint8_t *p) {  // payloads are byte-aligned only
     return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24);
 }
@@ -90,20 +102,30 @@ __device__ __forceinline__ uint32_t posting_errors(uint32_t doc, uint32_t tf, ui
     return bad;
 }
 
-// Cache::evaluate of one posting (bm25.rs:355-358), as k_block_desc / k_term_ub / k_champions compute it.
-__device__ __forceinline__ double posting_score(uint32_t w, double s0, const double *__restrict__ s1d) {
-    const double tfd = (double)(w >> 8);
-    return __ddiv_rn(__dmul_rn(tfd, s0), __dadd_rn(tfd, s1d[w & 0xFFu]));
+// Cache::evaluate (bm25.rs:355-358) of term frequency tf in a document of norm fn.  The explicit roundings keep the bits
+// of every build kernel the same whatever the compiler contracts.
+__device__ __forceinline__ double tf_score(uint32_t tf, uint32_t fn, double s0, const double *__restrict__ s1d) {
+    const double tfd = (double)tf;
+    return __ddiv_rn(__dmul_rn(tfd, s0), __dadd_rn(tfd, s1d[fn]));
 }
 
+// The same of a packed posting word w = tf << 8 | fieldnorm.
+__device__ __forceinline__ double posting_score(uint32_t w, double s0, const double *__restrict__ s1d) {
+    return tf_score(w >> 8, w & 0xFFu, s0, s1d);
+}
+
+// Score bounds are inflated by 2^-40 so that they also dominate any later re-association of the f64 sum.
+constexpr double UB_INFLATE = 1.0 + 9.094947017729282e-13;
+
+// A block's bound as stored: the inflated score rounded up to f32.
+__device__ __forceinline__ float block_bound(double v) { return __double2float_ru(v * UB_INFLATE); }
+
 // The stored SummaryTuple.(wand_fieldnorm, wand_term_frequency) of a block against the block's bound blk_ub (k_block_desc's
-// f32, rounded up after the 2^-40 inflation): tf() and Cache::evaluate round differently, so the last f32 ulp either way
-// is allowed.
+// block_bound): tf() and Cache::evaluate round differently, so the last f32 ulp either way is allowed.  wand_tf is a full
+// u32 and is never packed into a posting word.
 __device__ __forceinline__ bool wand_pair_ok(uint32_t wand_tf, uint8_t wand_fn, double s0, const double *__restrict__ s1d,
                                              float blk_ub) {
-    const double tfd = (double)wand_tf;
-    const double v = __ddiv_rn(__dmul_rn(tfd, s0), __dadd_rn(tfd, s1d[wand_fn]));
-    const float ub = __double2float_ru(v * (1.0 + 9.094947017729282e-13));
+    const float ub = block_bound(tf_score(wand_tf, wand_fn, s0, s1d));
     return ub <= blk_ub * 1.0000003f && ub >= blk_ub * 0.9999997f;
 }
 
@@ -121,12 +143,7 @@ k_decode_blocks(uint64_t n_blocks, const uint64_t *__restrict__ term_blk_off, ui
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
     const uint64_t g = (uint64_t)blockIdx.x * DEC_WARPS + warp;
     if (g >= n_blocks) return;  // whole warps leave; no block-wide barrier below
-    uint32_t lo = 0, hi = n_terms;  // token of this block: last t with term_blk_off[t] <= g
-    while (lo < hi) {
-        const uint32_t mid = (lo + hi + 1) >> 1;
-        if (term_blk_off[mid] <= g) lo = mid;
-        else hi = mid - 1;
-    }
+    const uint32_t t = owner_of(term_blk_off, n_terms, g);  // token of this block
     const uint32_t n = blk_n[g];
     const uint8_t md = meta_doc[g], mt = meta_tf[g];
     const uint32_t nbd = (md >> 7) ? (md & 0x7Fu) * n : (md & 0x7Fu) * 16u;
@@ -142,7 +159,7 @@ k_decode_blocks(uint64_t n_blocks, const uint64_t *__restrict__ term_blk_off, ui
     // the reference trusts its pages ("data corruption" panics); here bad blocks are reported, never dereferenced
     const uint32_t prev_last = __shfl_up_sync(0xFFFFFFFFu, doc[3], 1);
     uint32_t bad = 0;
-    Posting *dst = post + off_pad[lo] + (g - term_blk_off[lo]) * BM25X_BLOCK;
+    Posting *dst = post + off_pad[t] + (g - term_blk_off[t]) * BM25X_BLOCK;
 #pragma unroll
     for (uint32_t l = 0; l < 4; l++) {
         const uint32_t i = 4u * lane + l;
@@ -161,13 +178,7 @@ __global__ void k_check_block_order(const uint64_t *__restrict__ blk_off, uint32
                                     const uint2 *__restrict__ blk, uint32_t *__restrict__ err) {
     const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (g == 0 || g >= n_blocks) return;
-    uint32_t lo = 0, hi = n_terms;
-    while (lo < hi) {
-        const uint32_t mid = (lo + hi + 1) >> 1;
-        if (blk_off[mid] <= g) lo = mid;
-        else hi = mid - 1;
-    }
-    if (blk_off[lo] == g) return;  // first block of its token
+    if (blk_off[owner_of(blk_off, n_terms, g)] == g) return;  // first block of its token
     if (blk[g].x <= blk[g - 1].y) atomicOr(err, BM25X_BLKERR_RANGE);
 }
 
@@ -226,17 +237,7 @@ k_check_blocks(uint64_t g0, uint64_t n_blocks, const uint64_t *__restrict__ term
     const bool summed = decode_stream(stage[warp][0], md, n, lane, true, min_doc, doc);
     decode_stream(stage[warp][1], mt, n, lane, false, 0u, tf);
     const bool wand = wand_fn != nullptr;
-    double s0 = 0.0;
-    if (wand) {  // token of the block: last t with term_blk_off[t] <= g0 + j
-        const uint64_t g = g0 + j;
-        uint32_t lo = 0, hi = n_terms;
-        while (lo < hi) {
-            const uint32_t mid = (lo + hi + 1) >> 1;
-            if (term_blk_off[mid] <= g) lo = mid;
-            else hi = mid - 1;
-        }
-        s0 = s0d[lo];
-    }
+    const double s0 = wand ? s0d[owner_of(term_blk_off, n_terms, g0 + j)] : 0.0;  // of the block's token
     const uint32_t prev_last = __shfl_up_sync(0xFFFFFFFFu, doc[3], 1);
     uint32_t bad = 0, last_mine = doc[0];
     double best = 0.0;
@@ -262,7 +263,7 @@ k_check_blocks(uint64_t g0, uint64_t n_blocks, const uint64_t *__restrict__ term
     if (bad) atomicOr(err, bad);
     if (lane == 0) {
         first_last[j] = make_uint2(first, last);
-        if (wand && !wand_pair_ok(wand_tf[j], wand_fn[j], s0, s1d, __double2float_ru(best * (1.0 + 9.094947017729282e-13))))
+        if (wand && !wand_pair_ok(wand_tf[j], wand_fn[j], s0, s1d, block_bound(best)))
             atomicOr(err, BM25X_BLKERR_WAND);
     }
 }
@@ -335,12 +336,7 @@ k_decode_shard_blocks(uint64_t n_blocks, const uint64_t *__restrict__ sel_off, u
         return;
     }
     __syncwarp();
-    uint32_t t = 0, hi_t = n_terms;  // token of this block: last t with sel_off[t] <= j
-    while (t < hi_t) {
-        const uint32_t mid = (t + hi_t + 1) >> 1;
-        if (sel_off[mid] <= j) t = mid;
-        else hi_t = mid - 1;
-    }
+    const uint32_t t = owner_of(sel_off, n_terms, j);  // token of this block
     uint32_t doc[4], tf[4];
     const uint32_t min_doc = blk_min[j];
     const bool summed = decode_stream(stage[warp][0], md, n, lane, true, min_doc, doc);

@@ -114,7 +114,7 @@ struct bm25x_index {
 };
 
 // Document-sharded index (bm25x_sharded_*): shard s is an ordinary index over the documents [bounds[s], bounds[s+1]) with
-// local ids, built with the whole segment's statistics (BuildMeta.stat_*), so it scores with the same s0 / s1 bits.
+// local ids, built with the whole segment's statistics (one Stats object), so it scores with the same s0 / s1 bits.
 struct bm25x_sharded_index {
     uint32_t n_shards = 0;
     std::vector<uint32_t> bounds;        // [n_shards+1]

@@ -12,6 +12,8 @@
 #include <string.h>
 
 #include <algorithm>
+#include <memory>
+#include <optional>
 
 #include "bm25x_common.h"
 #include "bm25x_blocks.cuh"
@@ -115,6 +117,59 @@ static void bm25_s1(double k1, double b, double avgdl, double s1d[256]) {
     }
 }
 
+// flush.rs:52-66: the norms of N documents into fn (when not NULL) and their Σlen — quantised from the exact lengths, or,
+// without doc_len, as the stored index keeps them: the norm per document and the exact total (tuples.rs:141-160,756-762).
+static uint64_t doc_norms(uint32_t N, const uint32_t *doc_len, const uint8_t *stored_fn, uint64_t stored_sum, uint8_t *fn) {
+    fn_init();
+    if (!doc_len) {
+        if (fn) memcpy(fn, stored_fn, N);
+        return stored_sum;
+    }
+    uint64_t sum_len = 0;
+#pragma omp parallel for reduction(+ : sum_len) num_threads(bm25x_host_threads(0))
+    for (uint32_t d = 0; d < N; d++) {
+        sum_len += doc_len[d];
+        if (fn) fn[d] = bm25x_length_to_fieldnorm(doc_len[d]);
+    }
+    return sum_len;
+}
+
+// The statistics a handle scores with: avgdl and the s0 / s1 tables of a segment of N documents with the given df.  The
+// only place they are computed: the shards of a segment and its growing segment receive the segment's object, so that
+// they score with its bits (DESIGN §4.7).
+struct Stats {
+    uint64_t sum_len;
+    double avgdl;
+    std::vector<double> s0d;  // [T]
+    std::vector<float> s0f;
+    double s1d[256];
+    float s1f[256];
+
+    Stats(uint32_t N, uint64_t sum_len, double avgdl, const uint32_t *df, uint32_t T, double k1, double b)
+        : sum_len(sum_len), avgdl(avgdl), s0d(T), s0f(T) {
+        for (uint32_t t = 0; t < T; t++) {
+            s0d[t] = bm25_s0((double)df[t], (double)N, k1);
+            s0f[t] = (float)s0d[t];
+        }
+        bm25_s1(k1, b, avgdl, s1d);
+        for (int f = 0; f < 256; f++) s1f[f] = (float)s1d[f];
+    }
+    // a segment's own: avgdl = Σlen / N (flush.rs:52-66)
+    Stats(uint32_t N, uint64_t sum_len, const uint32_t *df, uint32_t T, double k1, double b)
+        : Stats(N, sum_len, (double)sum_len / (double)N, df, T, k1, b) {}
+};
+
+// Smallest s1 over the norms of the documents present: the one-compare single-term test of k_search_ring needs a lower
+// bound.
+static float s1f_min(const uint8_t *fn, uint32_t N, const float s1f[256]) {
+    bool seen[256] = {false};
+    for (uint32_t d = 0; d < N; d++) seen[fn[d]] = true;
+    float mn = 3.0e38f;
+    for (int f = 0; f < 256; f++)
+        if (seen[f] && s1f[f] < mn) mn = s1f[f];
+    return mn;
+}
+
 // ---- device transforms ----
 
 // CSR chunk → AoS postings at their padded positions, with the fieldnorm byte folded in.
@@ -125,18 +180,12 @@ __global__ void k_build_postings(const uint32_t *__restrict__ c_doc, const uint3
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= chunk_n) return;
     uint64_t gi = chunk_base + i;
-    // term = last t with off[t] <= gi
-    uint32_t lo = 0, hi = n_terms;
-    while (lo < hi) {
-        uint32_t mid = (lo + hi + 1) >> 1;
-        if (off[mid] <= gi) lo = mid;
-        else hi = mid - 1;
-    }
+    const uint32_t t = owner_of(off, n_terms, gi);
     uint32_t d = c_doc[i];
     Posting p;
     p.doc = d;
     p.w = (c_tf[i] << 8) | fieldnorm[d];
-    post[off_pad[lo] + (gi - off[lo])] = p;
+    post[off_pad[t] + (gi - off[t])] = p;
 }
 
 __global__ void k_pad_slots(const uint64_t *__restrict__ off_pad, const uint32_t *__restrict__ df, uint32_t n_terms,
@@ -160,33 +209,25 @@ __global__ void k_extract_docs(const Posting *__restrict__ post, uint64_t n, uin
 // Per 128-posting block: (first doc, last doc) = SummaryTuple.{min,max}_document_id, and the block's score bound =
 // Cache::evaluate of the block's arg-max posting, what the reference keeps as SummaryTuple.(wand_fieldnorm,
 // wand_term_frequency) (flush.rs:101-120) and evaluates per block at query time (search.rs:381,426-429).  Stored as f32
-// rounded UP after the same 2^-40 inflation as the token-level bound.
+// rounded UP after the same 2^-40 inflation as the token-level bound (block_bound).
 __global__ void k_block_desc(const uint64_t *__restrict__ off_pad, const uint32_t *__restrict__ df,
                              const uint64_t *__restrict__ blk_off, uint32_t n_terms, uint64_t n_blocks,
                              const Posting *__restrict__ post, const double *__restrict__ s0d,
                              const double *__restrict__ s1d, uint2 *__restrict__ blk, float *__restrict__ blk_ub) {
     uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= n_blocks) return;
-    uint32_t lo = 0, hi = n_terms;
-    while (lo < hi) {
-        uint32_t mid = (lo + hi + 1) >> 1;
-        if (blk_off[mid] <= g) lo = mid;
-        else hi = mid - 1;
-    }
-    uint64_t b = g - blk_off[lo];
-    uint64_t first = b * BM25X_BLOCK;
+    const uint32_t t = owner_of(blk_off, n_terms, g);
+    uint64_t first = (g - blk_off[t]) * BM25X_BLOCK;
     uint64_t last = first + BM25X_BLOCK;
-    if (last > df[lo]) last = df[lo];
-    blk[g] = make_uint2(post[off_pad[lo] + first].doc, post[off_pad[lo] + last - 1].doc);
-    const double s0 = s0d[lo];
+    if (last > df[t]) last = df[t];
+    blk[g] = make_uint2(post[off_pad[t] + first].doc, post[off_pad[t] + last - 1].doc);
+    const double s0 = s0d[t];
     double best = 0.0;
     for (uint64_t i = first; i < last; i++) {
-        const uint32_t w = post[off_pad[lo] + i].w;
-        const double tfd = (double)(w >> 8);
-        const double v = __ddiv_rn(__dmul_rn(tfd, s0), __dadd_rn(tfd, s1d[w & 0xFFu]));
+        const double v = posting_score(post[off_pad[t] + i].w, s0, s1d);
         best = v > best ? v : best;
     }
-    blk_ub[g] = __double2float_ru(best * (1.0 + 9.094947017729282e-13));
+    blk_ub[g] = block_bound(best);
 }
 
 // Ingest check: the stored SummaryTuple.(wand_fieldnorm, wand_term_frequency) of a block must evaluate to the block's
@@ -197,19 +238,13 @@ __global__ void k_check_block_wand(uint64_t n_blocks, const uint64_t *__restrict
                                    const float *__restrict__ blk_ub, uint32_t *__restrict__ err) {
     uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= n_blocks) return;
-    uint32_t lo = 0, hi = n_terms;
-    while (lo < hi) {
-        uint32_t mid = (lo + hi + 1) >> 1;
-        if (blk_off[mid] <= g) lo = mid;
-        else hi = mid - 1;
-    }
-    if (!wand_pair_ok(wand_tf[g], wand_fn[g], s0d[lo], s1d, blk_ub[g])) atomicOr(err, BM25X_BLKERR_WAND);
+    const uint32_t t = owner_of(blk_off, n_terms, g);
+    if (!wand_pair_ok(wand_tf[g], wand_fn[g], s0d[t], s1d, blk_ub[g])) atomicOr(err, BM25X_BLKERR_WAND);
 }
 
 // Per-term upper bound of a single posting's exact score: max over the term's postings of Cache::evaluate
 // (bm25.rs:355-358) — what the reference stores as the token-level (wand_fieldnorm, wand_term_frequency) arg-max
-// (flush.rs:101-120) and evaluates at query time (search.rs:363).  One block per term; inflated by 2^-40 so that the
-// bound also dominates any later re-association of the f64 sum.
+// (flush.rs:101-120) and evaluates at query time (search.rs:363).  One block per term; inflated by UB_INFLATE, in f64.
 __global__ void k_term_ub(const uint64_t *__restrict__ off_pad, const uint32_t *__restrict__ df,
                           const Posting *__restrict__ post, const double *__restrict__ s0d,
                           const double *__restrict__ s1d, uint32_t n_terms, double *__restrict__ ubd) {
@@ -219,9 +254,7 @@ __global__ void k_term_ub(const uint64_t *__restrict__ off_pad, const uint32_t *
         const double s0 = s0d[t];
         double best = 0.0;
         for (uint32_t i = threadIdx.x; i < df[t]; i += blockDim.x) {
-            uint32_t w = pp[i].w;
-            double tfd = (double)(w >> 8);
-            double v = __ddiv_rn(__dmul_rn(tfd, s0), __dadd_rn(tfd, s1d[w & 0xFFu]));
+            const double v = posting_score(pp[i].w, s0, s1d);
             best = v > best ? v : best;
         }
         red[threadIdx.x] = best;
@@ -230,7 +263,7 @@ __global__ void k_term_ub(const uint64_t *__restrict__ off_pad, const uint32_t *
             if ((int)threadIdx.x < o && red[threadIdx.x + o] > red[threadIdx.x]) red[threadIdx.x] = red[threadIdx.x + o];
             __syncthreads();
         }
-        if (threadIdx.x == 0) ubd[t] = red[0] * (1.0 + 9.094947017729282e-13);
+        if (threadIdx.x == 0) ubd[t] = red[0] * UB_INFLATE;
         __syncthreads();
     }
 }
@@ -294,8 +327,7 @@ __global__ void __launch_bounds__(CHAMP_WARPS * 32) k_champions(const uint64_t *
             double sc = -1.0;
             if (i < n) {
                 v = pp[i];
-                const double tfd = (double)(v.w >> 8);
-                sc = __ddiv_rn(__dmul_rn(tfd, s0), __dadd_rn(tfd, s1d[v.w & 0xFFu]));
+                sc = posting_score(v.w, s0, s1d);
             }
             const bool acc = i < n && (!have || sc > thr);
             const uint32_t m = __ballot_sync(0xFFFFFFFFu, acc);
@@ -329,9 +361,6 @@ __global__ void __launch_bounds__(CHAMP_WARPS * 32) k_champions(const uint64_t *
     }
 }
 
-// champ_off from the host copy of df, then the lists (index_finish_device / finalize_replica; needs post, s0d, s1d)
-static cudaError_t build_champions(bm25x_index *ix);
-
 template <typename T>
 static int dev_alloc(bm25x_index *ix, T **p, size_t n) {
     size_t bytes = sizeof(T) * (n ? n : 1);
@@ -341,6 +370,32 @@ static int dev_alloc(bm25x_index *ix, T **p, size_t n) {
     return BM25X_OK;
 }
 
+// The arrays of a handle, sized by the counts in ix->d: index_begin fills them, a replica receives them.
+static int alloc_arrays(bm25x_index *ix) {
+    DeviceIndex &d = ix->d;
+    const size_t T = d.n_terms, N = d.n_docs, PP = d.n_post_pad + BM25X_POST_SLACK;
+    int rc = BM25X_OK;
+    auto a = [&](auto **p, size_t n) {
+        if (rc == BM25X_OK) rc = dev_alloc(ix, p, n);
+    };
+    a(&d.post, PP);
+    a(&d.pdoc, PP);
+    a(&d.post_off, T + 1);
+    a(&d.df, T);
+    a(&d.blk_off, T + 1);
+    a(&d.blk, d.n_blocks);
+    a(&d.blk_ub, d.n_blocks);
+    a(&d.s0f, T);
+    a(&d.s0d, T);
+    a(&d.s1d, 256);
+    a(&d.s1f, 256);
+    a(&d.ubd, T);
+    a(&d.fieldnorm, N);
+    a(&d.payload, N * 3);
+    return rc;
+}
+
+// champ_off from the host copy of df, then the lists (index_finish_device / finalize_replica; needs post, s0d, s1d).
 // Called again for a replica that is refilled and finalized once more: the lists are rebuilt from the new postings, in the
 // same allocation when their total length has not changed.
 static cudaError_t build_champions(bm25x_index *ix) {
@@ -388,25 +443,49 @@ static cudaError_t build_champions(bm25x_index *ix) {
     return e;
 }
 
-#define TRY(x)                      \
-    do {                            \
-        int _rc = (x);              \
-        if (_rc != BM25X_OK) {      \
-            bm25x_index_destroy(ix); \
-            return _rc;             \
-        }                           \
-    } while (0)
-#define CU(x)                                                                                       \
-    do {                                                                                            \
-        cudaError_t _e = (x);                                                                       \
-        if (_e != cudaSuccess) {                                                                    \
-            bm25x_set_error("%s failed: %s (%s:%d)", #x, cudaGetErrorString(_e), __FILE__, __LINE__); \
-            bm25x_index_destroy(ix);                                                                \
-            return _e == cudaErrorMemoryAllocation ? BM25X_ERR_OOM : BM25X_ERR_CUDA;                \
-        }                                                                                           \
-    } while (0)
+// A half-built handle: an early return destroys it, release() hands it out.
+struct IndexDestroy {
+    void operator()(bm25x_index *ix) const { bm25x_index_destroy(ix); }
+};
+using IndexGuard = std::unique_ptr<bm25x_index, IndexDestroy>;
 
-// What both index sources (CSR columns, reference-format blocks) share: statistics, tables, allocations.
+// Device temporaries of one build step on one device, freed when it goes out of scope (every refusal included).  The first
+// failure sticks in `e`; later calls do nothing.
+struct Scratch {
+    int device;
+    cudaError_t e = cudaSuccess;
+    std::vector<void *> ptrs;
+    explicit Scratch(int dev) : device(dev) {}
+    Scratch(const Scratch &) = delete;
+    ~Scratch() {
+        if (ptrs.empty()) return;
+        cudaSetDevice(device);
+        for (void *p : ptrs) cudaFree(p);
+    }
+    template <typename T>
+    T *alloc(size_t n) {
+        T *p = nullptr;
+        if (e == cudaSuccess) e = cudaMalloc((void **)&p, sizeof(T) * (n ? n : 1));
+        if (e != cudaSuccess) return nullptr;
+        ptrs.push_back(p);
+        return p;
+    }
+    template <typename T>
+    T *up(const T *h, size_t n) {
+        T *p = alloc<T>(n);
+        if (e == cudaSuccess && n) e = cudaMemcpy(p, h, sizeof(T) * n, cudaMemcpyHostToDevice);
+        return p;
+    }
+};
+
+// The refusal for a failed CUDA call of a build step.
+static int cuda_refusal(const char *who, const char *step, cudaError_t e) {
+    bm25x_set_error("%s: %s failed: %s", who, step, cudaGetErrorString(e));
+    return e == cudaErrorMemoryAllocation ? BM25X_ERR_OOM : BM25X_ERR_CUDA;
+}
+
+// One handle's documents and terms, from whichever source (CSR columns, reference-format blocks, a shard of either, a
+// growing segment).
 struct BuildMeta {
     uint32_t n_docs, n_terms;
     const uint32_t *doc_len;
@@ -417,13 +496,19 @@ struct BuildMeta {
     uint64_t n_post;
     const uint8_t *fieldnorm = nullptr;  // when doc_len == NULL: DocumentTuple.fieldnorm per doc + JumpTuple.sum_of_document_lengths
     uint64_t sum_len = 0;
-    // growing segment (search.rs:66-77): score with the SEALED segment's statistics instead of the index's own
-    const uint32_t *stat_df = nullptr;  // [n_terms] sealed TokenTuple.number_of_documents
-    uint32_t stat_n_docs = 0;           // sealed JumpTuple.number_of_documents
-    double stat_avgdl = 0.0;            // sealed sum_of_document_lengths / number_of_documents
-    // document shard (bm25x_sharded_create): global id of local document 0, for the synthesised ctid payload
+    // document shard: global id of local document 0, for the synthesised ctid payload
     uint32_t doc_base = 0;
 };
+
+static int check_device(const char *who, int device) {
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) {
+        cudaGetLastError();
+        bm25x_set_error("%s: CUDA device %d not available (%d devices); there is no CPU fallback", who, device, ndev);
+        return BM25X_ERR_CUDA;
+    }
+    return BM25X_OK;
+}
 
 static int check_common(const char *who, uint32_t n_docs, const void *doc_len, double k1, double b, int device) {
     if (n_docs == 0 || n_docs == BM25X_DOC_INF || !doc_len) {
@@ -434,13 +519,7 @@ static int check_common(const char *who, uint32_t n_docs, const void *doc_len, d
         bm25x_set_error("%s: k1/b out of range", who);
         return BM25X_ERR_INVALID;
     }
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) {
-        cudaGetLastError();
-        bm25x_set_error("%s: CUDA device %d not available (%d devices); there is no CPU fallback", who, device, ndev);
-        return BM25X_ERR_CUDA;
-    }
-    return BM25X_OK;
+    return check_device(who, device);
 }
 
 static int check_keys(const char *who, const uint8_t *term_key, uint32_t T) {
@@ -453,7 +532,6 @@ static int check_keys(const char *who, const uint8_t *term_key, uint32_t T) {
     return BM25X_OK;
 }
 
-// Allocates the index and fills everything except the postings.  On failure the index is destroyed.
 // Environment overrides of the option defaults (test matrix: BM25X_SEED=0 / BM25X_TWOPHASE=1 run the same tests through
 // the other kernel paths); bm25x_index_set_option still wins.
 static void apply_env_options(bm25x_index *ix) {
@@ -467,29 +545,24 @@ static void apply_env_options(bm25x_index *ix) {
     }
 }
 
-static int index_begin(const BuildMeta &m, int device, bm25x_index **ixp) {
-    *ixp = nullptr;
-    fn_init();
-    const uint32_t N = m.n_docs, T = m.n_terms;
-    const uint64_t P = m.n_post;
-    bm25x_index *ix = new bm25x_index();
-    apply_env_options(ix);
+// A new handle on `device`: checked to be sm_90, its streams created, the pool kept, the options' defaults set.  `who`
+// names the entry point in the refusal.
+static int handle_open(const char *who, int device, IndexGuard &ix) {
+    ix.reset(new bm25x_index());
+    apply_env_options(ix.get());
     ix->device = device;
-    ix->k1 = m.k1;
-    ix->b = m.b;
-    CU(cudaSetDevice(device));
+    BM25X_CUDA_TRY(cudaSetDevice(device));
     cudaDeviceProp prop;
-    CU(cudaGetDeviceProperties(&prop, device));
+    BM25X_CUDA_TRY(cudaGetDeviceProperties(&prop, device));
     if (prop.major != 9 || prop.minor != 0) {
-        bm25x_set_error("bm25x_index_create: device %d is sm_%d%d; this library only carries sm_90a kernels", device,
-                        prop.major, prop.minor);
-        bm25x_index_destroy(ix);
+        bm25x_set_error("%s: device %d is sm_%d%d; this library only carries sm_90a kernels", who, device, prop.major,
+                        prop.minor);
         return BM25X_ERR_CUDA;
     }
     ix->sm_count = prop.multiProcessorCount;
-    CU(cudaStreamCreateWithFlags(&ix->stream, cudaStreamNonBlocking));
+    BM25X_CUDA_TRY(cudaStreamCreateWithFlags(&ix->stream, cudaStreamNonBlocking));
     // created with the handle, never later: concurrent first calls of bm25x_search_batch must not race to create it
-    CU(cudaStreamCreateWithFlags(&ix->copy_stream, cudaStreamNonBlocking));
+    BM25X_CUDA_TRY(cudaStreamCreateWithFlags(&ix->copy_stream, cudaStreamNonBlocking));
     {   // keep freed batch buffers cached in the default pool (bm25x_batch_* allocate stream-ordered)
         cudaMemPool_t pool;
         if (cudaDeviceGetDefaultMemPool(&pool, device) == cudaSuccess) {
@@ -497,89 +570,60 @@ static int index_begin(const BuildMeta &m, int device, bm25x_index **ixp) {
             cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thr);
         }
     }
+    return BM25X_OK;
+}
 
-    // ---- flush.rs:52-66: N, Σlen (exact), per-doc fieldnorm (quantised), avgdl ----
+// A handle with everything but the postings, scoring with the `given` statistics (a shard's or a growing segment's: its
+// segment's) or, when NULL, its own.  Refusals name bm25x_index_create whichever entry point builds.
+static int index_begin(const BuildMeta &m, const Stats *given, int device, IndexGuard &ix) {
+    int rc = handle_open("bm25x_index_create", device, ix);
+    if (rc != BM25X_OK) return rc;
+    const uint32_t N = m.n_docs, T = m.n_terms;
+    ix->k1 = m.k1;
+    ix->b = m.b;
     std::vector<uint8_t> h_fn(N);
-    uint64_t sum_len = 0;
-    if (m.doc_len) {
-#pragma omp parallel for reduction(+ : sum_len) num_threads(bm25x_host_threads(0))
-        for (uint32_t d = 0; d < N; d++) {
-            sum_len += m.doc_len[d];
-            h_fn[d] = bm25x_length_to_fieldnorm(m.doc_len[d]);
-        }
-    } else {  // the stored index keeps only the quantised norm per document and the exact total (tuples.rs:141-160,756-762)
-        memcpy(h_fn.data(), m.fieldnorm, N);
-        sum_len = m.sum_len;
-    }
-    ix->sum_len = sum_len;
-    ix->avgdl = m.stat_df ? m.stat_avgdl : (double)sum_len / (double)N;
+    ix->sum_len = doc_norms(N, m.doc_len, m.fieldnorm, m.sum_len, h_fn.data());
+    std::optional<Stats> own;
+    const Stats &st = given ? *given : own.emplace(N, ix->sum_len, m.df, T, m.k1, m.b);
+    ix->avgdl = st.avgdl;
+    ix->s1f_min = s1f_min(h_fn.data(), N, st.s1f);
 
-    // ---- per-term df, padded offsets, block offsets, s0 (bm25.rs:285-289,348) ----
-    ix->h_df.resize(T);
+    // ---- per-term df, padded offsets, block offsets ----
+    ix->h_df.assign(m.df, m.df + T);
     std::vector<uint64_t> h_off_pad(T + 1), h_blk_off(T + 1);
-    std::vector<double> h_s0d(T);
-    std::vector<float> h_s0f(T);
     uint64_t pp = 0, nb = 0;
     for (uint32_t t = 0; t < T; t++) {
-        uint64_t n = m.df[t];
-        ix->h_df[t] = (uint32_t)n;
+        const uint64_t n = m.df[t];
         h_off_pad[t] = pp;
         h_blk_off[t] = nb;
         pp += (n + BM25X_POST_ALIGN - 1) & ~(uint64_t)(BM25X_POST_ALIGN - 1);
         nb += (n + BM25X_BLOCK - 1) / BM25X_BLOCK;
-        const double n_stat = m.stat_df ? (double)m.stat_df[t] : (double)n, N_stat = m.stat_df ? (double)m.stat_n_docs : (double)N;
-        h_s0d[t] = bm25_s0(n_stat, N_stat, m.k1);
-        h_s0f[t] = (float)h_s0d[t];
     }
     h_off_pad[T] = pp;
     h_blk_off[T] = nb;
-    double h_s1d[256];
-    float h_s1f[256];
-    bm25_s1(m.k1, m.b, ix->avgdl, h_s1d);
-    for (int f = 0; f < 256; f++) h_s1f[f] = (float)h_s1d[f];
-    {   // smallest s1 over the documents present: the one-compare single-term test of k_search_ring needs a lower bound
-        bool seen[256] = {false};
-        for (uint32_t d = 0; d < N; d++) seen[h_fn[d]] = true;
-        float mn = 3.0e38f;
-        for (int f = 0; f < 256; f++)
-            if (seen[f] && h_s1f[f] < mn) mn = h_s1f[f];
-        ix->s1f_min = mn;
-    }
     if (m.term_key) ix->h_keys.assign(m.term_key, m.term_key + (size_t)T * 16);
 
     DeviceIndex &d = ix->d;
     d.n_docs = N;
     d.n_terms = T;
-    d.n_post = P;
+    d.n_post = m.n_post;
     d.n_post_pad = pp;
     d.n_blocks = nb;
-    TRY(dev_alloc(ix, &d.post, pp + BM25X_POST_SLACK));
-    TRY(dev_alloc(ix, &d.pdoc, pp + BM25X_POST_SLACK));
-    TRY(dev_alloc(ix, &d.post_off, (size_t)T + 1));
-    TRY(dev_alloc(ix, &d.df, T));
-    TRY(dev_alloc(ix, &d.blk_off, (size_t)T + 1));
-    TRY(dev_alloc(ix, &d.blk, nb));
-    TRY(dev_alloc(ix, &d.blk_ub, nb));
-    TRY(dev_alloc(ix, &d.s0f, T));
-    TRY(dev_alloc(ix, &d.s0d, T));
-    TRY(dev_alloc(ix, &d.s1d, 256));
-    TRY(dev_alloc(ix, &d.s1f, 256));
-    TRY(dev_alloc(ix, &d.ubd, T));
-    TRY(dev_alloc(ix, &d.fieldnorm, N));
-    TRY(dev_alloc(ix, &d.payload, (size_t)N * 3));
-    CU(cudaMemset((void *)(d.post + pp), 0xFF, BM25X_POST_SLACK * sizeof(Posting)));  // the slack slots read as exhausted cursors
-    CU(cudaMemcpy(d.post_off, h_off_pad.data(), sizeof(uint64_t) * (T + 1), cudaMemcpyHostToDevice));
-    CU(cudaMemcpy(d.blk_off, h_blk_off.data(), sizeof(uint64_t) * (T + 1), cudaMemcpyHostToDevice));
+    rc = alloc_arrays(ix.get());
+    if (rc != BM25X_OK) return rc;
+    BM25X_CUDA_TRY(cudaMemset((void *)(d.post + pp), 0xFF, BM25X_POST_SLACK * sizeof(Posting)));  // the slack slots read as exhausted cursors
+    BM25X_CUDA_TRY(cudaMemcpy(d.post_off, h_off_pad.data(), sizeof(uint64_t) * (T + 1), cudaMemcpyHostToDevice));
+    BM25X_CUDA_TRY(cudaMemcpy(d.blk_off, h_blk_off.data(), sizeof(uint64_t) * (T + 1), cudaMemcpyHostToDevice));
     if (T) {
-        CU(cudaMemcpy(d.df, ix->h_df.data(), sizeof(uint32_t) * T, cudaMemcpyHostToDevice));
-        CU(cudaMemcpy(d.s0d, h_s0d.data(), sizeof(double) * T, cudaMemcpyHostToDevice));
-        CU(cudaMemcpy(d.s0f, h_s0f.data(), sizeof(float) * T, cudaMemcpyHostToDevice));
+        BM25X_CUDA_TRY(cudaMemcpy(d.df, ix->h_df.data(), sizeof(uint32_t) * T, cudaMemcpyHostToDevice));
+        BM25X_CUDA_TRY(cudaMemcpy(d.s0d, st.s0d.data(), sizeof(double) * T, cudaMemcpyHostToDevice));
+        BM25X_CUDA_TRY(cudaMemcpy(d.s0f, st.s0f.data(), sizeof(float) * T, cudaMemcpyHostToDevice));
     }
-    CU(cudaMemcpy(d.s1d, h_s1d, sizeof(h_s1d), cudaMemcpyHostToDevice));
-    CU(cudaMemcpy(d.s1f, h_s1f, sizeof(h_s1f), cudaMemcpyHostToDevice));
-    CU(cudaMemcpy(d.fieldnorm, h_fn.data(), N, cudaMemcpyHostToDevice));
+    BM25X_CUDA_TRY(cudaMemcpy(d.s1d, st.s1d, sizeof(st.s1d), cudaMemcpyHostToDevice));
+    BM25X_CUDA_TRY(cudaMemcpy(d.s1f, st.s1f, sizeof(st.s1f), cudaMemcpyHostToDevice));
+    BM25X_CUDA_TRY(cudaMemcpy(d.fieldnorm, h_fn.data(), N, cudaMemcpyHostToDevice));
     if (m.payload) {
-        CU(cudaMemcpy(d.payload, m.payload, sizeof(uint16_t) * 3 * (size_t)N, cudaMemcpyHostToDevice));
+        BM25X_CUDA_TRY(cudaMemcpy(d.payload, m.payload, sizeof(uint16_t) * 3 * (size_t)N, cudaMemcpyHostToDevice));
     } else {
         std::vector<uint16_t> pl((size_t)N * 3);
         for (uint32_t i = 0; i < N; i++) {  // synthetic ctid: (block hi, block lo, offset) of a 291-tuple page
@@ -589,10 +633,8 @@ static int index_begin(const BuildMeta &m, int device, bm25x_index **ixp) {
             pl[(size_t)i * 3 + 1] = (uint16_t)(blkno & 0xFFFF);
             pl[(size_t)i * 3 + 2] = (uint16_t)(g % 291 + 1);
         }
-        CU(cudaMemcpy(d.payload, pl.data(), sizeof(uint16_t) * pl.size(), cudaMemcpyHostToDevice));
+        BM25X_CUDA_TRY(cudaMemcpy(d.payload, pl.data(), sizeof(uint16_t) * pl.size(), cudaMemcpyHostToDevice));
     }
-
-    *ixp = ix;
     return BM25X_OK;
 }
 
@@ -625,43 +667,26 @@ static cudaError_t index_finish_device(bm25x_index *ix) {
 }
 
 // Postings of a term-major CSR: chunked H2D of the columns + device transform to the padded AoS, then the derived arrays.
-// Destroys the index on failure.
 static int upload_csr(bm25x_index *ix, const char *who, uint32_t T, uint64_t P, const uint64_t *post_off,
                       const uint32_t *post_doc, const uint32_t *post_tf) {
     DeviceIndex &d = ix->d;
-    // ---- postings: chunked H2D of the CSR columns + device transform to the padded AoS ----
-    {
-        uint64_t *d_off = nullptr;
-        uint32_t *d_cdoc = nullptr, *d_ctf = nullptr;
-        const uint64_t CH = 64ull << 20;  // postings per chunk
-        uint64_t chn = std::min<uint64_t>(CH, P ? P : 1);
-        cudaError_t e1 = cudaMalloc((void **)&d_off, sizeof(uint64_t) * ((size_t)T + 1));
-        cudaError_t e2 = cudaMalloc((void **)&d_cdoc, sizeof(uint32_t) * chn);
-        cudaError_t e3 = cudaMalloc((void **)&d_ctf, sizeof(uint32_t) * chn);
-        cudaError_t e = e1 != cudaSuccess ? e1 : (e2 != cudaSuccess ? e2 : e3);
-        if (e == cudaSuccess) e = cudaMemcpy(d_off, post_off, sizeof(uint64_t) * ((size_t)T + 1), cudaMemcpyHostToDevice);
-        for (uint64_t base = 0; base < P && e == cudaSuccess; base += CH) {
-            uint64_t n = std::min<uint64_t>(CH, P - base);
-            e = cudaMemcpy(d_cdoc, post_doc + base, sizeof(uint32_t) * n, cudaMemcpyHostToDevice);
-            if (e == cudaSuccess) e = cudaMemcpy(d_ctf, post_tf + base, sizeof(uint32_t) * n, cudaMemcpyHostToDevice);
-            if (e == cudaSuccess) {
-                k_build_postings<<<(unsigned)((n + 255) / 256), 256>>>(d_cdoc, d_ctf, base, n, d_off, d.post_off, T,
-                                                                       d.fieldnorm, d.post);
-                e = cudaGetLastError();
-            }
-            if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    const uint64_t CH = 64ull << 20;  // postings per chunk
+    Scratch sc(ix->device);
+    const uint64_t *d_off = sc.up(post_off, (size_t)T + 1);
+    uint32_t *d_cdoc = sc.alloc<uint32_t>(std::min<uint64_t>(CH, P)), *d_ctf = sc.alloc<uint32_t>(std::min<uint64_t>(CH, P));
+    for (uint64_t base = 0; base < P && sc.e == cudaSuccess; base += CH) {
+        const uint64_t n = std::min<uint64_t>(CH, P - base);
+        sc.e = cudaMemcpy(d_cdoc, post_doc + base, sizeof(uint32_t) * n, cudaMemcpyHostToDevice);
+        if (sc.e == cudaSuccess) sc.e = cudaMemcpy(d_ctf, post_tf + base, sizeof(uint32_t) * n, cudaMemcpyHostToDevice);
+        if (sc.e == cudaSuccess) {
+            k_build_postings<<<(unsigned)((n + 255) / 256), 256>>>(d_cdoc, d_ctf, base, n, d_off, d.post_off, T, d.fieldnorm,
+                                                                   d.post);
+            sc.e = cudaGetLastError();
         }
-        if (e == cudaSuccess) e = index_finish_device(ix);
-        cudaFree(d_off);
-        cudaFree(d_cdoc);
-        cudaFree(d_ctf);
-        if (e != cudaSuccess) {
-            bm25x_set_error("%s: posting upload failed: %s", who, cudaGetErrorString(e));
-            bm25x_index_destroy(ix);
-            return e == cudaErrorMemoryAllocation ? BM25X_ERR_OOM : BM25X_ERR_CUDA;
-        }
+        if (sc.e == cudaSuccess) sc.e = cudaDeviceSynchronize();
     }
-    return BM25X_OK;
+    if (sc.e == cudaSuccess) sc.e = index_finish_device(ix);
+    return sc.e == cudaSuccess ? BM25X_OK : cuda_refusal(who, "posting upload", sc.e);
 }
 
 // Host validation of a term-major CSR corpus, shared by bm25x_index_create and bm25x_sharded_create: same codes, same
@@ -720,14 +745,11 @@ extern "C" int bm25x_index_create(const bm25x_corpus *c, int device, bm25x_index
     std::vector<uint32_t> df(T);
     for (uint32_t t = 0; t < T; t++) df[t] = (uint32_t)(c->post_off[t + 1] - c->post_off[t]);
     BuildMeta m{N, T, c->doc_len, c->payload, c->term_key, c->k1, c->b, df.data(), P};
-    bm25x_index *ix = nullptr;
-    rc = index_begin(m, device, &ix);
-    if (rc != BM25X_OK) return rc;
-
-    rc = upload_csr(ix, "bm25x_index_create", T, P, c->post_off, c->post_doc, c->post_tf);
-    if (rc != BM25X_OK) return rc;
-    *out = ix;
-    return BM25X_OK;
+    IndexGuard ix;
+    rc = index_begin(m, nullptr, device, ix);
+    if (rc == BM25X_OK) rc = upload_csr(ix.get(), "bm25x_index_create", T, P, c->post_off, c->post_doc, c->post_tf);
+    if (rc == BM25X_OK) *out = ix.release();
+    return rc;
 }
 
 // ---- document-sharded index (DESIGN §4.7): one segment split by document range, each shard an index with local doc ids
@@ -783,6 +805,47 @@ static std::vector<uint32_t> shard_bounds(const uint32_t *doc_bounds, const std:
     return bounds;
 }
 
+// The container of a document-sharded build, for both sources: after the host checks of the segment c (P postings, df, the
+// statistics st), every shard's device is checked with who's message; then prepare(device of shard 0, cum) runs the
+// host work and refusals that need a device and, when doc_bounds is NULL, gives the postings per document for the balanced
+// bounds (shard_bounds); then the shards are built one at a time by build(s, device, lo, hi, ix).  On the first failure
+// everything built so far is destroyed.
+template <typename Segment, typename Prepare, typename Build>
+static int sharded_build(const char *who, const Segment *c, uint64_t P, const std::vector<uint32_t> &df, const Stats &st,
+                         uint32_t S, const uint32_t *doc_bounds, const int *devices, Prepare prepare, Build build,
+                         bm25x_sharded_index **out) {
+    std::vector<int> dev(S, 0);
+    if (devices) std::copy(devices, devices + S, dev.begin());
+    for (uint32_t s = 0; s < S; s++) {
+        const int rc = check_device(who, dev[s]);
+        if (rc != BM25X_OK) return rc;
+    }
+    std::vector<uint64_t> cum;
+    int rc = prepare(dev[0], doc_bounds ? nullptr : &cum);
+    if (rc != BM25X_OK) return rc;
+    std::unique_ptr<bm25x_sharded_index, void (*)(bm25x_sharded_index *)> sx(new bm25x_sharded_index(),
+                                                                             bm25x_sharded_destroy);
+    sx->n_shards = S;
+    sx->bounds = shard_bounds(doc_bounds, cum, c->n_docs, S);
+    std::vector<uint64_t>().swap(cum);
+    sx->n_docs = c->n_docs;
+    sx->n_terms = c->n_terms;
+    sx->n_post = P;
+    sx->k1 = c->k1;
+    sx->b = c->b;
+    sx->h_df = df;
+    sx->sum_len = st.sum_len;
+    sx->avgdl = st.avgdl;
+    for (uint32_t s = 0; s < S; s++) {
+        IndexGuard ix;
+        rc = build(s, dev[s], sx->bounds[s], sx->bounds[s + 1], ix);
+        if (rc != BM25X_OK) return rc;
+        sx->shards.push_back(ix.release());
+    }
+    *out = sx.release();
+    return BM25X_OK;
+}
+
 extern "C" int bm25x_sharded_create(const bm25x_corpus *c, uint32_t S, const uint32_t *doc_bounds, const int *devices,
                                     bm25x_sharded_index **out) {
     const char *who = "bm25x_sharded_create";
@@ -798,44 +861,22 @@ extern "C" int bm25x_sharded_create(const bm25x_corpus *c, uint32_t S, const uin
     const uint64_t P = c->post_off[T];
     rc = check_shard_args(N, S, doc_bounds);
     if (rc != BM25X_OK) return rc;
-    std::vector<uint64_t> cum;
-    if (!doc_bounds) {
-        cum.assign((size_t)N + 1, 0);
+    std::vector<uint32_t> df(T);
+    for (uint32_t t = 0; t < T; t++) df[t] = (uint32_t)(c->post_off[t + 1] - c->post_off[t]);
+    const Stats st(N, doc_norms(N, c->doc_len, nullptr, 0, nullptr), df.data(), T, c->k1, c->b);
+    auto count = [&](int, std::vector<uint64_t> *cum) {
+        if (!cum) return BM25X_OK;
+        cum->assign((size_t)N + 1, 0);
 #pragma omp parallel for schedule(static) num_threads(bm25x_host_threads(0))
         for (uint64_t p = 0; p < P; p++) {
 #pragma omp atomic
-            cum[(size_t)c->post_doc[p] + 1]++;
+            (*cum)[(size_t)c->post_doc[p] + 1]++;
         }
-        for (uint32_t d = 0; d < N; d++) cum[(size_t)d + 1] += cum[d];
-    }
-    const std::vector<uint32_t> bounds = shard_bounds(doc_bounds, cum, N, S);
-    std::vector<uint64_t>().swap(cum);
-    std::vector<int> dev(S, 0);
-    if (devices) std::copy(devices, devices + S, dev.begin());
-    for (uint32_t s = 0; s < S; s++) {
-        rc = check_common(who, N, c->doc_len, c->k1, c->b, dev[s]);
-        if (rc != BM25X_OK) return rc;
-    }
-
-    bm25x_sharded_index *sx = new bm25x_sharded_index();
-    sx->n_shards = S;
-    sx->bounds = bounds;
-    sx->n_docs = N;
-    sx->n_terms = T;
-    sx->n_post = P;
-    sx->k1 = c->k1;
-    sx->b = c->b;
-    sx->h_df.resize(T);
-    for (uint32_t t = 0; t < T; t++) sx->h_df[t] = (uint32_t)(c->post_off[t + 1] - c->post_off[t]);
-    uint64_t sum_len = 0;
-#pragma omp parallel for reduction(+ : sum_len) num_threads(bm25x_host_threads(0))
-    for (uint32_t d = 0; d < N; d++) sum_len += c->doc_len[d];
-    sx->sum_len = sum_len;
-    sx->avgdl = (double)sum_len / (double)N;  // the expression of index_begin: the shards' s1 tables are the whole index's
-
+        for (uint32_t d = 0; d < N; d++) (*cum)[(size_t)d + 1] += (*cum)[d];
+        return BM25X_OK;
+    };
     // one shard at a time: host memory beyond the corpus stays within one shard's CSR
-    for (uint32_t s = 0; s < S; s++) {
-        const uint32_t lo = bounds[s], hi = bounds[s + 1];
+    auto build = [&](uint32_t s, int device, uint32_t lo, uint32_t hi, IndexGuard &ix) {
         std::vector<uint64_t> off((size_t)T + 1, 0);
         std::vector<uint64_t> first(T);
 #pragma omp parallel for schedule(dynamic, 256) num_threads(bm25x_host_threads(0))
@@ -845,9 +886,9 @@ extern "C" int bm25x_sharded_create(const bm25x_corpus *c, uint32_t S, const uin
             first[t] = (uint64_t)(p0 - c->post_doc);
             off[(size_t)t + 1] = (uint64_t)(p1 - p0);
         }
-        std::vector<uint32_t> df(T);
+        std::vector<uint32_t> df_s(T);
         for (uint32_t t = 0; t < T; t++) {
-            df[t] = (uint32_t)off[(size_t)t + 1];
+            df_s[t] = (uint32_t)off[(size_t)t + 1];
             off[(size_t)t + 1] += off[t];
         }
         const uint64_t Ps = off[T];
@@ -860,22 +901,12 @@ extern "C" int bm25x_sharded_create(const bm25x_corpus *c, uint32_t S, const uin
             }
         // (the term keys once, with shard 0: bm25x_sharded_lookup_terms asks it)
         BuildMeta m{hi - lo, T, c->doc_len + lo, c->payload ? c->payload + (size_t)lo * 3 : nullptr, s ? nullptr : c->term_key,
-                    c->k1, c->b, df.data(), Ps};
-        m.stat_df = sx->h_df.data();
-        m.stat_n_docs = N;
-        m.stat_avgdl = sx->avgdl;
+                    c->k1, c->b, df_s.data(), Ps};
         m.doc_base = lo;
-        bm25x_index *ix = nullptr;
-        rc = index_begin(m, dev[s], &ix);
-        if (rc == BM25X_OK) rc = upload_csr(ix, who, T, Ps, off.data(), pdoc.data(), ptf.data());  // destroys ix on failure
-        if (rc != BM25X_OK) {
-            bm25x_sharded_destroy(sx);
-            return rc;
-        }
-        sx->shards.push_back(ix);
-    }
-    *out = sx;
-    return BM25X_OK;
+        const int rc = index_begin(m, &st, device, ix);
+        return rc == BM25X_OK ? upload_csr(ix.get(), who, T, Ps, off.data(), pdoc.data(), ptf.data()) : rc;
+    };
+    return sharded_build(who, c, P, df, st, S, doc_bounds, devices, count, build, out);
 }
 
 // ---- f1: the sealed segment as the reference stores it (blocks in the codec of compression.rs), decoded on the GPU ----
@@ -989,110 +1020,48 @@ extern "C" int bm25x_index_create_from_blocks(const bm25x_blocks *c, int device,
     BuildMeta m{N, T, c->doc_len, c->payload, c->term_key, c->k1, c->b, df.data(), P};
     m.fieldnorm = c->doc_fieldnorm;
     m.sum_len = c->sum_doc_len;
-    bm25x_index *ix = nullptr;
-    rc = index_begin(m, device, &ix);
+    IndexGuard ix;
+    rc = index_begin(m, nullptr, device, ix);
     if (rc != BM25X_OK) return rc;
     DeviceIndex &d = ix->d;
 
     // ---- upload the directory + payloads, decode on the device ----
-    uint64_t *d_tbo = nullptr, *d_doff = nullptr, *d_toff = nullptr;
-    uint32_t *d_min = nullptr, *d_n = nullptr, *d_err = nullptr;
-    uint8_t *d_md = nullptr, *d_mt = nullptr, *d_bytes = nullptr;
     uint32_t h_err = 0;
-    cudaError_t e = cudaSuccess;
-    auto up = [&](auto **dp, const auto *hp, size_t n) {
-        using E = std::remove_pointer_t<std::remove_pointer_t<decltype(dp)>>;
-        if (e != cudaSuccess) return;
-        e = cudaMalloc((void **)dp, sizeof(E) * (n ? n : 1));
-        if (e == cudaSuccess && n) e = cudaMemcpy(*dp, hp, sizeof(E) * n, cudaMemcpyHostToDevice);
-    };
-    up(&d_tbo, c->term_blk_off, (size_t)T + 1);
-    up(&d_min, c->blk_min_doc, NB);
-    up(&d_n, c->blk_n, NB);
-    up(&d_md, c->blk_meta_doc, NB);
-    up(&d_mt, c->blk_meta_tf, NB);
-    up(&d_doff, c->blk_doc_off, NB);
-    up(&d_toff, c->blk_tf_off, NB);
-    up(&d_bytes, c->bytes, c->n_bytes);
-    up(&d_err, &h_err, 1);
-    if (e == cudaSuccess && NB) {
+    Scratch sc(device);
+    const uint64_t *d_tbo = sc.up(c->term_blk_off, (size_t)T + 1);
+    const uint32_t *d_min = sc.up(c->blk_min_doc, NB), *d_n = sc.up(c->blk_n, NB);
+    const uint8_t *d_md = sc.up(c->blk_meta_doc, NB), *d_mt = sc.up(c->blk_meta_tf, NB);
+    const uint64_t *d_doff = sc.up(c->blk_doc_off, NB), *d_toff = sc.up(c->blk_tf_off, NB);
+    const uint8_t *d_bytes = sc.up(c->bytes, c->n_bytes);
+    uint32_t *d_err = sc.up(&h_err, 1);
+    if (sc.e == cudaSuccess && NB) {
         k_decode_blocks<<<(unsigned)((NB + DEC_WARPS - 1) / DEC_WARPS), DEC_WARPS * 32>>>(
             NB, d_tbo, T, d_min, d_n, d_md, d_mt, d_doff, d_toff, d_bytes, d.post_off, d.fieldnorm, N, d.post, d_err);
-        e = cudaGetLastError();
+        sc.e = cudaGetLastError();
     }
-    if (e == cudaSuccess) e = index_finish_device(ix);
-    uint8_t *d_wfn = nullptr;
-    uint32_t *d_wtf = nullptr;
+    if (sc.e == cudaSuccess) sc.e = index_finish_device(ix.get());
     if (c->blk_wand_fieldnorm && c->blk_wand_tf) {  // the stored per-block bounds must be those of the decoded postings
-        up(&d_wfn, c->blk_wand_fieldnorm, NB);
-        up(&d_wtf, c->blk_wand_tf, NB);
-        if (e == cudaSuccess && NB) {
+        const uint8_t *d_wfn = sc.up(c->blk_wand_fieldnorm, NB);
+        const uint32_t *d_wtf = sc.up(c->blk_wand_tf, NB);
+        if (sc.e == cudaSuccess && NB) {
             k_check_block_wand<<<(unsigned)((NB + 255) / 256), 256>>>(NB, d.blk_off, T, d_wfn, d_wtf, d.s0d, d.s1d, d.blk_ub,
                                                                      d_err);
-            e = cudaGetLastError();
+            sc.e = cudaGetLastError();
         }
     }
-    if (e == cudaSuccess && NB > 1) {
+    if (sc.e == cudaSuccess && NB > 1) {
         k_check_block_order<<<(unsigned)((NB + 255) / 256), 256>>>(d.blk_off, T, NB, d.blk, d_err);
-        e = cudaGetLastError();
+        sc.e = cudaGetLastError();
     }
-    if (e == cudaSuccess) e = cudaMemcpy(&h_err, d_err, sizeof(h_err), cudaMemcpyDeviceToHost);
-    cudaFree(d_wfn);
-    cudaFree(d_wtf);
-    cudaFree(d_tbo);
-    cudaFree(d_min);
-    cudaFree(d_n);
-    cudaFree(d_md);
-    cudaFree(d_mt);
-    cudaFree(d_doff);
-    cudaFree(d_toff);
-    cudaFree(d_bytes);
-    cudaFree(d_err);
-    if (e != cudaSuccess) {
-        bm25x_set_error("%s: block upload/decode failed: %s", who, cudaGetErrorString(e));
-        bm25x_index_destroy(ix);
-        return e == cudaErrorMemoryAllocation ? BM25X_ERR_OOM : BM25X_ERR_CUDA;
-    }
+    if (sc.e == cudaSuccess) sc.e = cudaMemcpy(&h_err, d_err, sizeof(h_err), cudaMemcpyDeviceToHost);
+    if (sc.e != cudaSuccess) return cuda_refusal(who, "block upload/decode", sc.e);
     rc = blocks_refusal(h_err);
-    if (rc != BM25X_OK) {
-        bm25x_index_destroy(ix);
-        return rc;
-    }
-    *out = ix;
-    return BM25X_OK;
+    if (rc == BM25X_OK) *out = ix.release();
+    return rc;
 }
 
 // ---- a document-sharded index from the stored blocks (DESIGN §4.7): one check pass over the whole segment on shard 0's
 // device, then per shard a decode of just the stored blocks that hold its documents, on its own device ----
-
-// Device scratch of one build step on one device, freed when it goes out of scope (every refusal included).  The first
-// failure sticks in `e`; later calls do nothing.
-struct Scratch {
-    int device;
-    cudaError_t e = cudaSuccess;
-    std::vector<void *> ptrs;
-    explicit Scratch(int dev) : device(dev) {}
-    Scratch(const Scratch &) = delete;
-    ~Scratch() {
-        if (ptrs.empty()) return;
-        cudaSetDevice(device);
-        for (void *p : ptrs) cudaFree(p);
-    }
-    template <typename T>
-    T *alloc(size_t n) {
-        T *p = nullptr;
-        if (e == cudaSuccess) e = cudaMalloc((void **)&p, sizeof(T) * (n ? n : 1));
-        if (e != cudaSuccess) return nullptr;
-        ptrs.push_back(p);
-        return p;
-    }
-    template <typename T>
-    T *up(const T *h, size_t n) {
-        T *p = alloc<T>(n);
-        if (e == cudaSuccess && n) e = cudaMemcpy(p, h, sizeof(T) * n, cudaMemcpyHostToDevice);
-        return p;
-    }
-};
 
 // Directory entries and payloads of some stored blocks, gathered back to back with the offsets rebased to `bytes`: what a
 // kernel of bm25x_blocks.cuh reads for just these blocks.  The directory has passed validate_blocks.
@@ -1133,18 +1102,12 @@ struct StagedBlocks {
     uint64_t n_bytes = 0;
 };
 
-static int scratch_failed(const char *who, cudaError_t e) {
-    bm25x_set_error("%s: block upload/decode failed: %s", who, cudaGetErrorString(e));
-    return e == cudaErrorMemoryAllocation ? BM25X_ERR_OOM : BM25X_ERR_CUDA;
-}
-
 // The check pass: every stored block decoded once on `device`, in chunks of at most 256 MiB of payload (so the compressed
 // segment never has to fit on one GPU), with every check bm25x_index_create_from_blocks makes on the device.  Gives the
 // error bits, each block's decoded (first, last) doc id, and with cum != NULL the postings of the documents < d (cum[d]).
-// fieldnorm, s0d and s1d are the segment's; they are read only to check the stored wand pairs.
-static int check_stored_blocks(const char *who, const bm25x_blocks *c, const uint8_t *fieldnorm, const double *s0d,
-                               const double *s1d, int device, std::vector<uint2> &first_last, std::vector<uint64_t> *cum,
-                               uint32_t &h_err) {
+// fieldnorm and the s0 / s1 tables of stats are the segment's; they are read only to check the stored wand pairs.
+static int check_stored_blocks(const char *who, const bm25x_blocks *c, const uint8_t *fieldnorm, const Stats &stats,
+                               int device, std::vector<uint2> &first_last, std::vector<uint64_t> *cum, uint32_t &h_err) {
     const uint32_t N = c->n_docs, T = c->n_terms;
     const uint64_t NB = c->n_blocks;
     const bool wand = c->blk_wand_fieldnorm && c->blk_wand_tf;
@@ -1154,8 +1117,8 @@ static int check_stored_blocks(const char *who, const bm25x_blocks *c, const uin
     sc.e = cudaSetDevice(device);
     const uint64_t *d_tbo = sc.up(c->term_blk_off, (size_t)T + 1);
     const uint8_t *d_fn = wand ? sc.up(fieldnorm, N) : nullptr;  // the whole segment's norms: a block may straddle a bound
-    const double *d_s0d = wand ? sc.up(s0d, T) : nullptr;
-    const double *d_s1d = wand ? sc.up(s1d, 256) : nullptr;
+    const double *d_s0d = wand ? sc.up(stats.s0d.data(), T) : nullptr;
+    const double *d_s1d = wand ? sc.up(stats.s1d, 256) : nullptr;
     uint32_t *d_cnt = cum ? sc.alloc<uint32_t>(N) : nullptr;
     if (d_cnt && sc.e == cudaSuccess) sc.e = cudaMemset(d_cnt, 0, sizeof(uint32_t) * (size_t)N);
     uint32_t *d_err = sc.up(&h_err, 1);
@@ -1200,7 +1163,7 @@ static int check_stored_blocks(const char *who, const bm25x_blocks *c, const uin
         cum->assign((size_t)N + 1, 0);
         for (uint32_t d = 0; d < N; d++) (*cum)[(size_t)d + 1] = (*cum)[d] + cnt[d];
     }
-    if (sc.e != cudaSuccess) return scratch_failed(who, sc.e);
+    if (sc.e != cudaSuccess) return cuda_refusal(who, "block upload/decode", sc.e);
     // k_check_block_order's rule on the decoded (first, last): ids ascend across the blocks of a token
     uint32_t order = 0;
 #pragma omp parallel for schedule(dynamic, 256) reduction(| : order) num_threads(bm25x_host_threads(0))
@@ -1211,13 +1174,13 @@ static int check_stored_blocks(const char *who, const bm25x_blocks *c, const uin
     return BM25X_OK;
 }
 
-// Shard s of sx from the stored blocks, on `device`: the blocks whose decoded [first, last] meets [lo, hi) gathered with
-// rebased offsets (host memory beyond the caller's: this payload), counted (k_count_shard_blocks), then the shard index
-// allocated with the whole segment's statistics, decoded into place (k_decode_shard_blocks) and finished as every index is.
+// Shard s, documents [lo, hi), from the stored blocks, on `device`: the blocks whose decoded [first, last] meets [lo, hi)
+// gathered with rebased offsets (host memory beyond the caller's: this payload), counted (k_count_shard_blocks), then the
+// shard index allocated with the whole segment's statistics, decoded into place (k_decode_shard_blocks) and finished as
+// every index is.
 static int build_shard_from_blocks(const char *who, const bm25x_blocks *c, const std::vector<uint2> &first_last,
-                                   const bm25x_sharded_index *sx, uint32_t s, int device, bm25x_index **out) {
-    *out = nullptr;
-    const uint32_t T = c->n_terms, lo = sx->bounds[s], hi = sx->bounds[s + 1];
+                                   const Stats &stats, uint32_t s, uint32_t lo, uint32_t hi, int device, IndexGuard &ix) {
+    const uint32_t T = c->n_terms;
     // ---- select: per token the run of its blocks with last >= lo and first < hi (both ascend along the chain) ----
     std::vector<uint64_t> sel_b0(T), sel_off((size_t)T + 1, 0);
 #pragma omp parallel for schedule(dynamic, 256) num_threads(bm25x_host_threads(0))
@@ -1260,7 +1223,7 @@ static int build_shard_from_blocks(const char *who, const bm25x_blocks *c, const
     }
     std::vector<uint2> cs(nsel);
     if (sc.e == cudaSuccess && nsel) sc.e = cudaMemcpy(cs.data(), d_cs, sizeof(uint2) * nsel, cudaMemcpyDeviceToHost);
-    if (sc.e != cudaSuccess) return scratch_failed(who, sc.e);
+    if (sc.e != cudaSuccess) return cuda_refusal(who, "block upload/decode", sc.e);
     std::vector<uint32_t> df(T), rank(nsel);
     uint64_t Ps = 0;
     for (uint32_t t = 0; t < T; t++) {
@@ -1277,35 +1240,20 @@ static int build_shard_from_blocks(const char *who, const bm25x_blocks *c, const
                 s ? nullptr : c->term_key, c->k1, c->b, df.data(), Ps};
     m.fieldnorm = c->doc_len ? nullptr : c->doc_fieldnorm + lo;
     m.sum_len = c->sum_doc_len;  // stored norms: the pages hold the segment's sum only
-    m.stat_df = sx->h_df.data();
-    m.stat_n_docs = sx->n_docs;
-    m.stat_avgdl = sx->avgdl;
     m.doc_base = lo;
-    bm25x_index *ix = nullptr;
-    int rc = index_begin(m, device, &ix);
+    const int rc = index_begin(m, &stats, device, ix);
     if (rc != BM25X_OK) return rc;
     // ---- write the postings, then what every index derives from them ----
     const uint32_t *d_rank = sc.up(rank.data(), nsel);
     if (sc.e == cudaSuccess && nsel) {
         k_decode_shard_blocks<<<grid, DEC_WARPS * 32>>>(nsel, d_sel_off, T, d_min, d_n, d_md, d_mt, d_doff, d_toff, d_bytes,
-                                                         st.n_bytes, d_cs, d_rank, sx->n_docs, lo, hi - lo,
+                                                         st.n_bytes, d_cs, d_rank, c->n_docs, lo, hi - lo,
                                                          ix->d.post_off, ix->d.df, ix->d.fieldnorm, ix->d.post, d_err);
         sc.e = cudaGetLastError();
     }
     if (sc.e == cudaSuccess) sc.e = cudaMemcpy(&h_err, d_err, sizeof(h_err), cudaMemcpyDeviceToHost);
-    if (sc.e == cudaSuccess && !h_err) sc.e = index_finish_device(ix);
-    if (sc.e != cudaSuccess) {
-        rc = scratch_failed(who, sc.e);
-        bm25x_index_destroy(ix);
-        return rc;
-    }
-    rc = blocks_refusal(h_err);
-    if (rc != BM25X_OK) {
-        bm25x_index_destroy(ix);
-        return rc;
-    }
-    *out = ix;
-    return BM25X_OK;
+    if (sc.e == cudaSuccess && !h_err) sc.e = index_finish_device(ix.get());
+    return sc.e != cudaSuccess ? cuda_refusal(who, "block upload/decode", sc.e) : blocks_refusal(h_err);
 }
 
 extern "C" int bm25x_index_create_sharded_from_blocks(const bm25x_blocks *c, uint32_t S, const uint32_t *doc_bounds,
@@ -1325,67 +1273,24 @@ extern "C" int bm25x_index_create_sharded_from_blocks(const bm25x_blocks *c, uin
     const uint32_t N = c->n_docs, T = c->n_terms;
     rc = check_shard_args(N, S, doc_bounds);
     if (rc != BM25X_OK) return rc;
-    std::vector<int> dev(S, 0);
-    if (devices) std::copy(devices, devices + S, dev.begin());
-    const void *norms = c->doc_len ? (const void *)c->doc_len : (const void *)c->doc_fieldnorm;
-    for (uint32_t s = 0; s < S; s++) {
-        rc = check_common(who, N, norms, c->k1, c->b, dev[s]);
-        if (rc != BM25X_OK) return rc;
-    }
-    // ---- the segment's norms and statistics, as index_begin computes them for the unsharded index ----
-    std::vector<uint8_t> h_fn;
-    const uint8_t *fn = c->doc_fieldnorm;
-    uint64_t sum_len = c->sum_doc_len;
-    if (c->doc_len) {
-        h_fn.resize(N);
-        sum_len = 0;
-#pragma omp parallel for reduction(+ : sum_len) num_threads(bm25x_host_threads(0))
-        for (uint32_t d = 0; d < N; d++) {
-            sum_len += c->doc_len[d];
-            h_fn[d] = bm25x_length_to_fieldnorm(c->doc_len[d]);
-        }
-        fn = h_fn.data();
-    }
-    const double avgdl = (double)sum_len / (double)N;
-    std::vector<double> s0d(T);
-    for (uint32_t t = 0; t < T; t++) s0d[t] = bm25_s0((double)df[t], (double)N, c->k1);
-    double s1d[256];
-    bm25_s1(c->k1, c->b, avgdl, s1d);
-    // ---- check pass on shard 0's device: the refusals of the unsharded ingest, before any shard exists ----
+    // the segment's norms (the stored ones, or quantised for the check pass) and statistics
+    std::vector<uint8_t> h_fn(c->doc_len ? N : 0);
+    const uint8_t *fn = c->doc_len ? h_fn.data() : c->doc_fieldnorm;
+    const Stats st(N, doc_norms(N, c->doc_len, c->doc_fieldnorm, c->sum_doc_len, c->doc_len ? h_fn.data() : nullptr),
+                   df.data(), T, c->k1, c->b);
     std::vector<uint2> first_last;
-    std::vector<uint64_t> cum;
-    uint32_t h_err = 0;
-    rc = check_stored_blocks(who, c, fn, s0d.data(), s1d, dev[0], first_last, doc_bounds ? nullptr : &cum, h_err);
-    if (rc != BM25X_OK) return rc;
-    rc = blocks_refusal(h_err);
-    if (rc != BM25X_OK) return rc;
-    std::vector<uint8_t>().swap(h_fn);
-    const std::vector<uint32_t> bounds = shard_bounds(doc_bounds, cum, N, S);
-    std::vector<uint64_t>().swap(cum);
-
-    bm25x_sharded_index *sx = new bm25x_sharded_index();
-    sx->n_shards = S;
-    sx->bounds = bounds;
-    sx->n_docs = N;
-    sx->n_terms = T;
-    sx->n_post = P;
-    sx->k1 = c->k1;
-    sx->b = c->b;
-    sx->h_df = df;
-    sx->sum_len = sum_len;
-    sx->avgdl = avgdl;  // the expression of index_begin: the shards' s1 tables are the unsharded index's
+    // ---- check pass on shard 0's device: the refusals of the unsharded ingest, before any shard exists ----
+    auto check = [&](int device, std::vector<uint64_t> *cum) {
+        uint32_t h_err = 0;
+        const int rc = check_stored_blocks(who, c, fn, st, device, first_last, cum, h_err);
+        std::vector<uint8_t>().swap(h_fn);
+        return rc != BM25X_OK ? rc : blocks_refusal(h_err);
+    };
     // one shard at a time: host memory beyond the blocks stays within one shard's selected payload
-    for (uint32_t s = 0; s < S; s++) {
-        bm25x_index *ix = nullptr;
-        rc = build_shard_from_blocks(who, c, first_last, sx, s, dev[s], &ix);
-        if (rc != BM25X_OK) {
-            bm25x_sharded_destroy(sx);
-            return rc;
-        }
-        sx->shards.push_back(ix);
-    }
-    *out = sx;
-    return BM25X_OK;
+    auto build = [&](uint32_t s, int device, uint32_t lo, uint32_t hi, IndexGuard &ix) {
+        return build_shard_from_blocks(who, c, first_last, st, s, lo, hi, device, ix);
+    };
+    return sharded_build(who, c, P, df, st, S, doc_bounds, devices, check, build, out);
 }
 
 // ---- f3: the growing segment (documents inserted since the last seal, search.rs:83-135) as a second, small index that
@@ -1469,16 +1374,14 @@ extern "C" int bm25x_growing_create(const bm25x_index *sealed, const bm25x_growi
     BuildMeta m{G, T, g->doc_len, g->payload, sealed->h_keys.empty() ? nullptr : sealed->h_keys.data(), sealed->k1,
                 sealed->b, df.data(), P};
     m.fieldnorm = g->doc_fieldnorm;
-    m.stat_df = sealed->h_df.data();
-    m.stat_n_docs = sealed->d.n_docs;
-    m.stat_avgdl = sealed->avgdl;
-    bm25x_index *ix = nullptr;
-    rc = index_begin(m, sealed->device, &ix);
-    if (rc != BM25X_OK) return rc;
-    rc = upload_csr(ix, who, T, P, off.data(), post_doc.data(), post_tf.data());
+    // search.rs:66-77: scored with the SEALED segment's statistics, not its own
+    const Stats st(sealed->d.n_docs, sealed->sum_len, sealed->avgdl, sealed->h_df.data(), T, sealed->k1, sealed->b);
+    IndexGuard ix;
+    rc = index_begin(m, &st, sealed->device, ix);
+    if (rc == BM25X_OK) rc = upload_csr(ix.get(), who, T, P, off.data(), post_doc.data(), post_tf.data());
     if (rc != BM25X_OK) return rc;
     ix->prune = sealed->prune;
-    *out = ix;
+    *out = ix.release();
     return BM25X_OK;
 }
 
@@ -1579,55 +1482,22 @@ extern "C" int bm25x_index_alloc_replica(const bm25x_index_layout *like, int dev
         bm25x_set_error("bm25x_index_alloc_replica: CUDA device %d not available; there is no CPU fallback", device);
         return BM25X_ERR_CUDA;
     }
-    bm25x_index *ix = new bm25x_index();
-    apply_env_options(ix);
-    ix->device = device;
+    IndexGuard ix;
+    int rc = handle_open("bm25x_index_alloc_replica", device, ix);
+    if (rc != BM25X_OK) return rc;
     ix->k1 = like->k1;
     ix->b = like->b;
     ix->avgdl = like->avgdl;
     ix->sum_len = like->sum_doc_len;
-    CU(cudaSetDevice(device));
-    cudaDeviceProp prop;
-    CU(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 9 || prop.minor != 0) {
-        bm25x_set_error("bm25x_index_alloc_replica: device %d is sm_%d%d; this library only carries sm_90a kernels", device,
-                        prop.major, prop.minor);
-        bm25x_index_destroy(ix);
-        return BM25X_ERR_CUDA;
-    }
-    ix->sm_count = prop.multiProcessorCount;
-    CU(cudaStreamCreateWithFlags(&ix->stream, cudaStreamNonBlocking));
-    CU(cudaStreamCreateWithFlags(&ix->copy_stream, cudaStreamNonBlocking));  // as in index_begin
-    {
-        cudaMemPool_t pool;
-        if (cudaDeviceGetDefaultMemPool(&pool, device) == cudaSuccess) {
-            uint64_t thr = ~0ull;
-            cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thr);
-        }
-    }
     DeviceIndex &d = ix->d;
     d.n_docs = like->n_docs;
     d.n_terms = like->n_terms;
     d.n_post = like->n_postings;
     d.n_post_pad = like->n_postings_padded;
     d.n_blocks = like->n_blocks;
-    const size_t T = d.n_terms, N = d.n_docs;
-    TRY(dev_alloc(ix, &d.post, d.n_post_pad + BM25X_POST_SLACK));
-    TRY(dev_alloc(ix, &d.pdoc, d.n_post_pad + BM25X_POST_SLACK));
-    TRY(dev_alloc(ix, &d.post_off, T + 1));
-    TRY(dev_alloc(ix, &d.df, T));
-    TRY(dev_alloc(ix, &d.blk_off, T + 1));
-    TRY(dev_alloc(ix, &d.blk, d.n_blocks));
-    TRY(dev_alloc(ix, &d.blk_ub, d.n_blocks));
-    TRY(dev_alloc(ix, &d.s0f, T));
-    TRY(dev_alloc(ix, &d.s0d, T));
-    TRY(dev_alloc(ix, &d.s1d, 256));
-    TRY(dev_alloc(ix, &d.s1f, 256));
-    TRY(dev_alloc(ix, &d.fieldnorm, N));
-    TRY(dev_alloc(ix, &d.payload, N * 3));
-    TRY(dev_alloc(ix, &d.ubd, T));
-    *out = ix;
-    return BM25X_OK;
+    rc = alloc_arrays(ix.get());
+    if (rc == BM25X_OK) *out = ix.release();
+    return rc;
 }
 
 extern "C" int bm25x_index_finalize_replica(bm25x_index *ix) {
@@ -1644,18 +1514,12 @@ extern "C" int bm25x_index_finalize_replica(bm25x_index *ix) {
     if (ix->d.n_terms)
         BM25X_CUDA_TRY(cudaMemcpy(ix->h_df.data(), ix->d.df, sizeof(uint32_t) * ix->d.n_terms, cudaMemcpyDeviceToHost));
     BM25X_CUDA_TRY(build_champions(ix));  // derived data: built here from the replicated arrays, on every call
-    {   // s1f_min from the replicated arrays (see index_begin)
-        std::vector<uint8_t> h_fn(ix->d.n_docs);
-        float h_s1f[256];
-        BM25X_CUDA_TRY(cudaMemcpy(h_fn.data(), ix->d.fieldnorm, ix->d.n_docs, cudaMemcpyDeviceToHost));
-        BM25X_CUDA_TRY(cudaMemcpy(h_s1f, ix->d.s1f, sizeof(h_s1f), cudaMemcpyDeviceToHost));
-        bool seen[256] = {false};
-        for (uint32_t d = 0; d < ix->d.n_docs; d++) seen[h_fn[d]] = true;
-        float mn = 3.0e38f;
-        for (int f = 0; f < 256; f++)
-            if (seen[f] && h_s1f[f] < mn) mn = h_s1f[f];
-        ix->s1f_min = mn;
-    }
+    // s1f_min from the replicated arrays
+    std::vector<uint8_t> h_fn(ix->d.n_docs);
+    float h_s1f[256];
+    BM25X_CUDA_TRY(cudaMemcpy(h_fn.data(), ix->d.fieldnorm, ix->d.n_docs, cudaMemcpyDeviceToHost));
+    BM25X_CUDA_TRY(cudaMemcpy(h_s1f, ix->d.s1f, sizeof(h_s1f), cudaMemcpyDeviceToHost));
+    ix->s1f_min = s1f_min(h_fn.data(), ix->d.n_docs, h_s1f);
     return BM25X_OK;
 }
 

@@ -36,7 +36,7 @@ CASES = {
     "class_16": (dict(m=15, k=10, n_docs=1000000), PATHS["plain"], 1),        # filter_term loop
     "class_32": (dict(m=31, k=10, n_docs=1000000), PATHS["plain"], 1),
     "seeded_4_lanes": (dict(m=3, k=10, n_docs=1000000), PATHS["seeded"], 2),  # seeded launch + (empty) hand-back launch
-    "two_phase": (dict(m=3, k=10, n_docs=1000000), PATHS["twophase"], 2),     # PH 1 suspends, PH 2 (doc ids) finds B
+    "two_phase": (dict(m=3, k=10, n_docs=1000000), PATHS["twophase"], 2),     # suspend launch, resume launch (doc ids) finds B
     "two_pass": (dict(m=8, k=10, n_docs=1000000, n_rare=32), PATHS["plain"], 1),  # 41 lanes: B holds group 1 only
     "dense_window": (dict(m=4, k=10, n_docs=60000, binade=8.0, dense=True), PATHS["plain"], 1),
     "hbm_pool": (dict(m=3, k=1025, n_docs=1000000), PATHS["plain"], 1),       # k = 1025: pool in HBM, lazy cut

@@ -1,4 +1,4 @@
-"""GPU: the seeded kernel's hit list.  A seeded launch (RCfg::PH 3) does its ring searches per verification pass but
+"""GPU: the seeded kernel's hit list.  A seeded launch (RING_SEEDED) does its ring searches per verification pass but
 scores the documents they confirm later, several passes and windows at a time (word loads, f32 filter, exact f64 score,
 pool insert); the list is flushed when a pass's rows might not fit and once at query end.  These corpora make the list
 fill many times per window and across windows (correlated lists: most documents of a query hold two or three of its

@@ -20,12 +20,14 @@
 #define BM25X_CHAMP_L 128u          // champion list: the best min(df, 128) postings of every term by single-term score
 #define BM25X_POST_SLACK 4u         // slack slots behind the last list, reading as exhausted cursors
 
-#ifndef BM25X_SEED_MAX_TERMS
-#define BM25X_SEED_MAX_TERMS 8
-#endif
-#ifndef BM25X_TWOPHASE_DEFAULT
-#define BM25X_TWOPHASE_DEFAULT 0
-#endif
+// The five launch flavours of the search kernel k_search_ring (bm25x_search_ring.cuh, RCfg::FLAVOUR).
+enum RingFlavour : int {
+    RING_PLAIN = 0,     // one launch answers its queries (8-byte postings in the rings, MaxScore pruning)
+    RING_SUSPEND = 1,   // two-phase launches, first: the plain kernel, which suspends a query once no posting can pass alone
+    RING_RESUME = 2,    // two-phase launches, second: doc-id-only rings resume the suspended queries
+    RING_SEEDED = 3,    // single-term documents from the champion lists, doc-id-only rings, no pruning
+    RING_HANDBACK = 4,  // the plain kernel over the queries a seeded launch handed back
+};
 
 void bm25x_set_error(const char *fmt, ...);
 // Host threads this process may really use: the affinity mask capped by the cgroup CPU quota (omp_get_max_threads()
@@ -97,9 +99,9 @@ struct bm25x_index {
     int prune = 1;                     // MaxScore-style pruning in the search kernels
     uint32_t seed_dense_div = 64;      // seeded launches hand queries with a list of n_docs / 64 postings or more to the plain kernel
     uint32_t seed_prune_min = 32768;   // seeded launches hand queries with a list this long (and 8x their shortest) to the pruning kernel
-    int seed_max_terms = BM25X_SEED_MAX_TERMS;  // widest term-count class that runs seeded (4 or 8)
+    int seed_max_terms = 8;            // widest term-count class that runs seeded (4 or 8)
     int seed = 1;                      // 2..4-term classes, k <= BM25X_CHAMP_L, no prefilter: pools seeded from the champion lists
-    int twophase = BM25X_TWOPHASE_DEFAULT;  // 2..4-term classes, k <= 224: two launches (8-byte postings, then doc ids only)
+    int twophase = 0;                  // 2..4-term classes, k <= 224: two launches (8-byte postings, then doc ids only)
     // page-locked staging buffer of bm25x_batch_prepare (grow-only, shared by the batches of this index)
     uint32_t *h_stage = nullptr;
     size_t h_stage_words = 0;

@@ -4,8 +4,8 @@
 
 #include "bm25x_common.h"
 
-// Two-phase launches of the 2..4-term classes (bm25x_search_ring.cuh, RCfg::PH): what the first phase hands over when it
-// suspends a query — the pool entries themselves travel in the query's output rows.
+// Two-phase launches of the 2..4-term classes (bm25x_search_ring.cuh, RING_SUSPEND then RING_RESUME): what the first
+// phase hands over when it suspends a query — the pool entries themselves travel in the query's output rows.
 struct ResumeRec {
     double Sk, ub_ne;
     unsigned long long fetched_unused;
@@ -79,13 +79,7 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t *bar, uint32_t by
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
     uint32_t addr = smem_u32(bar);
     uint32_t ok;
-#ifdef BM25X_WATCHDOG
-    uint32_t spins = 0;
-#endif
     do {
-#ifdef BM25X_WATCHDOG
-        if (++spins > (1u << 26)) __trap();  // debug builds: turn a pipeline deadlock into a launch failure
-#endif
         asm volatile(
             "{\n\t.reg .pred p;\n\t"
             "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"

@@ -98,25 +98,25 @@ struct bm25x_batch {
 };
 
 // kernel v6 (bm25x_search_ring.cu: warp per query, ring stages + presence map), one entry per pool capacity
-// phase: 0 = the launch answers its queries; 1 / 2 = the two launches of a two-phase class (RCfg::PH)
-int bm25x_launch_ring_kp64(int device, int sm_count, const SearchParams &sp, int M, int phase, cudaStream_t stream);
-int bm25x_launch_ring_kp256(int device, int sm_count, const SearchParams &sp, int M, int phase, cudaStream_t stream);
-int bm25x_launch_ring_kp2048(int device, int sm_count, const SearchParams &sp, int M, int phase, cudaStream_t stream);
-int bm25x_launch_ring_kp131072(int device, int sm_count, const SearchParams &sp, int M, int phase, cudaStream_t stream);
+// flavour: which launch of the class this is (RingFlavour, bm25x_common.h)
+int bm25x_launch_ring_kp64(int device, int sm_count, const SearchParams &sp, int M, RingFlavour flavour, cudaStream_t stream);
+int bm25x_launch_ring_kp256(int device, int sm_count, const SearchParams &sp, int M, RingFlavour flavour, cudaStream_t stream);
+int bm25x_launch_ring_kp2048(int device, int sm_count, const SearchParams &sp, int M, RingFlavour flavour, cudaStream_t stream);
+int bm25x_launch_ring_kp131072(int device, int sm_count, const SearchParams &sp, int M, RingFlavour flavour, cudaStream_t stream);
 
 // Two launches per class: 2..4 terms with the pool in shared memory (k <= 224).
 static bool two_phase_class(const bm25x_index *ix, int M, uint32_t k) { return ix->twophase && M >= 2 && M <= 4 && k <= 224; }
-// One seeded launch (phase 3): 2..4 terms, k within the champion lists, no prefilter bitmap (a filtered-out champion would
+// One seeded launch (RING_SEEDED): 2..4 terms, k within the champion lists, no prefilter bitmap (a filtered-out champion would
 // have to be replaced by the next one of its term: such batches take the unseeded kernels).
 static bool seeded_class(const bm25x_index *ix, int M, uint32_t k, const uint8_t *allow) {
     return ix->seed && ix->d.champ && !allow && M >= 2 && M <= ix->seed_max_terms && k <= BM25X_CHAMP_L;
 }
 
-static int launch_ring_k(const bm25x_index *ix, const SearchParams &sp, int M, int phase, cudaStream_t stream) {
-    if (sp.k <= 32) return bm25x_launch_ring_kp64(ix->device, ix->sm_count, sp, M, phase, stream);
-    if (sp.k <= 224) return bm25x_launch_ring_kp256(ix->device, ix->sm_count, sp, M, phase, stream);
-    if (sp.k <= 1024) return bm25x_launch_ring_kp2048(ix->device, ix->sm_count, sp, M, 0, stream);
-    return bm25x_launch_ring_kp131072(ix->device, ix->sm_count, sp, M, 0, stream);  // candidate pools in HBM
+static int launch_ring_k(const bm25x_index *ix, const SearchParams &sp, int M, RingFlavour flavour, cudaStream_t stream) {
+    if (sp.k <= 32) return bm25x_launch_ring_kp64(ix->device, ix->sm_count, sp, M, flavour, stream);
+    if (sp.k <= 224) return bm25x_launch_ring_kp256(ix->device, ix->sm_count, sp, M, flavour, stream);
+    if (sp.k <= 1024) return bm25x_launch_ring_kp2048(ix->device, ix->sm_count, sp, M, RING_PLAIN, stream);
+    return bm25x_launch_ring_kp131072(ix->device, ix->sm_count, sp, M, RING_PLAIN, stream);  // candidate pools in HBM
 }
 
 template <typename T>
@@ -452,20 +452,20 @@ static int batch_enqueue(bm25x_batch *b, cudaStream_t st, bool timed) {
             // seeded launch (champion lists + doc-id-only stream, no pruning); the queries it hands back (a list much
             // longer than another: pruning pays) go through the plain kernel
             BM25X_CUDA_TRY(cudaMemsetAsync(g.d_q2, 0, 2 * sizeof(uint32_t), st));
-            rc = launch_ring_k(ix, sp, g.M, 3, st);
+            rc = launch_ring_k(ix, sp, g.M, RING_SEEDED, st);
             if (rc != BM25X_OK) return rc;
             launches++;
-            rc = launch_ring_k(ix, sp, g.M, 4, st);
+            rc = launch_ring_k(ix, sp, g.M, RING_HANDBACK, st);
         } else if (g.d_q2 && g.d_resume && ix->twophase) {
             // first phase: 8-byte postings until no posting can enter the top-k alone; second phase: the suspended
-            // queries go on with doc ids only (bm25x_search_ring.cuh, RCfg::PH)
+            // queries go on with doc ids only (bm25x_search_ring.cuh, RING_SUSPEND / RING_RESUME)
             BM25X_CUDA_TRY(cudaMemsetAsync(g.d_q2, 0, 2 * sizeof(uint32_t), st));
-            rc = launch_ring_k(ix, sp, g.M, 1, st);
+            rc = launch_ring_k(ix, sp, g.M, RING_SUSPEND, st);
             if (rc != BM25X_OK) return rc;
             launches++;
-            rc = launch_ring_k(ix, sp, g.M, 2, st);
+            rc = launch_ring_k(ix, sp, g.M, RING_RESUME, st);
         } else {
-            rc = launch_ring_k(ix, sp, g.M, 0, st);
+            rc = launch_ring_k(ix, sp, g.M, RING_PLAIN, st);
         }
         if (rc != BM25X_OK) return rc;
         launches++;

@@ -34,6 +34,42 @@ int launch_ring(int device, int sm_count, const SearchParams &sp_in, cudaStream_
     return BM25X_OK;
 }
 
+// a flavour / term-count class pair that is not built
+int no_launch(int M) {
+    bm25x_set_error("k_search_ring: no two-phase launch for %d terms / pool %d", M, (int)BM25X_RING_KP);
+    return BM25X_ERR_INVALID;
+}
+
+// The term-count classes flavour F is built for: every class for the plain kernel (M = 64: two passes of the 32-term
+// kernel); 2..4 terms for the two-phase flavours; 2..4 and 8 terms for the seeded launch and its hand-back.  The flavours
+// other than plain only exist with the pool in shared memory (KP <= 256).
+template <int F>
+int launch_flavour(int device, int sm_count, const SearchParams &sp, int M, cudaStream_t stream) {
+    constexpr int KP = BM25X_RING_KP;
+    if constexpr (F == RING_PLAIN) {
+        switch (M) {
+            case 1: return launch_ring<RCfg<1, KP, F>>(device, sm_count, sp, stream);
+            case 2: return launch_ring<RCfg<2, KP, F>>(device, sm_count, sp, stream);
+            case 3: return launch_ring<RCfg<3, KP, F>>(device, sm_count, sp, stream);
+            case 4: return launch_ring<RCfg<4, KP, F>>(device, sm_count, sp, stream);
+            case 8: return launch_ring<RCfg<8, KP, F>>(device, sm_count, sp, stream);
+            case 16: return launch_ring<RCfg<16, KP, F>>(device, sm_count, sp, stream);
+            default: return launch_ring<RCfg<32, KP, F>>(device, sm_count, sp, stream);
+        }
+    } else if constexpr (KP <= 256) {
+        switch (M) {
+            case 2: return launch_ring<RCfg<2, KP, F>>(device, sm_count, sp, stream);
+            case 3: return launch_ring<RCfg<3, KP, F>>(device, sm_count, sp, stream);
+            case 4: return launch_ring<RCfg<4, KP, F>>(device, sm_count, sp, stream);
+            case 8:
+                if constexpr (F == RING_SEEDED || F == RING_HANDBACK) return launch_ring<RCfg<8, KP, F>>(device, sm_count, sp, stream);
+                break;
+            default: break;
+        }
+    }
+    return no_launch(M);
+}
+
 }  // namespace
 
 #if defined(BM25X_PHASE_PROF) && BM25X_RING_KP == 64
@@ -52,47 +88,15 @@ extern "C" int bm25x_phase_prof(unsigned long long *out, int reset) {
 #define BM25X_RING_ENTRY2(kp) bm25x_launch_ring_kp##kp
 #define BM25X_RING_ENTRY(kp) BM25X_RING_ENTRY2(kp)
 
-// M = term-count class of the launch (1, 2, 3, 4, 8, 16, 32); phase = RCfg::PH (1 / 2 only for 2..4 terms, KP <= 256)
-int BM25X_RING_ENTRY(BM25X_RING_KP)(int device, int sm_count, const SearchParams &sp, int M, int phase, cudaStream_t stream) {
-#if BM25X_RING_KP <= 256
-    if (phase == 1) switch (M) {
-            case 2: return launch_ring<RCfg<2, BM25X_RING_KP, 1>>(device, sm_count, sp, stream);
-            case 3: return launch_ring<RCfg<3, BM25X_RING_KP, 1>>(device, sm_count, sp, stream);
-            case 4: return launch_ring<RCfg<4, BM25X_RING_KP, 1>>(device, sm_count, sp, stream);
-            default: break;
-        }
-    if (phase == 2) switch (M) {
-            case 2: return launch_ring<RCfg<2, BM25X_RING_KP, 2>>(device, sm_count, sp, stream);
-            case 3: return launch_ring<RCfg<3, BM25X_RING_KP, 2>>(device, sm_count, sp, stream);
-            case 4: return launch_ring<RCfg<4, BM25X_RING_KP, 2>>(device, sm_count, sp, stream);
-            default: break;
-        }
-    if (phase == 3) switch (M) {
-            case 2: return launch_ring<RCfg<2, BM25X_RING_KP, 3>>(device, sm_count, sp, stream);
-            case 3: return launch_ring<RCfg<3, BM25X_RING_KP, 3>>(device, sm_count, sp, stream);
-            case 4: return launch_ring<RCfg<4, BM25X_RING_KP, 3>>(device, sm_count, sp, stream);
-            case 8: return launch_ring<RCfg<8, BM25X_RING_KP, 3>>(device, sm_count, sp, stream);
-            default: break;
-        }
-    if (phase == 4) switch (M) {
-            case 2: return launch_ring<RCfg<2, BM25X_RING_KP, 4>>(device, sm_count, sp, stream);
-            case 3: return launch_ring<RCfg<3, BM25X_RING_KP, 4>>(device, sm_count, sp, stream);
-            case 4: return launch_ring<RCfg<4, BM25X_RING_KP, 4>>(device, sm_count, sp, stream);
-            case 8: return launch_ring<RCfg<8, BM25X_RING_KP, 4>>(device, sm_count, sp, stream);
-            default: break;
-        }
-#endif
-    if (phase != 0) {
-        bm25x_set_error("k_search_ring: no two-phase launch for %d terms / pool %d", M, (int)BM25X_RING_KP);
-        return BM25X_ERR_INVALID;
+// M = term-count class of the launch (1, 2, 3, 4, 8, 16, 32)
+int BM25X_RING_ENTRY(BM25X_RING_KP)(int device, int sm_count, const SearchParams &sp, int M, RingFlavour flavour,
+                                    cudaStream_t stream) {
+    switch (flavour) {
+        case RING_PLAIN: return launch_flavour<RING_PLAIN>(device, sm_count, sp, M, stream);
+        case RING_SUSPEND: return launch_flavour<RING_SUSPEND>(device, sm_count, sp, M, stream);
+        case RING_RESUME: return launch_flavour<RING_RESUME>(device, sm_count, sp, M, stream);
+        case RING_SEEDED: return launch_flavour<RING_SEEDED>(device, sm_count, sp, M, stream);
+        case RING_HANDBACK: return launch_flavour<RING_HANDBACK>(device, sm_count, sp, M, stream);
     }
-    switch (M) {
-        case 1: return launch_ring<RCfg<1, BM25X_RING_KP>>(device, sm_count, sp, stream);
-        case 2: return launch_ring<RCfg<2, BM25X_RING_KP>>(device, sm_count, sp, stream);
-        case 3: return launch_ring<RCfg<3, BM25X_RING_KP>>(device, sm_count, sp, stream);
-        case 4: return launch_ring<RCfg<4, BM25X_RING_KP>>(device, sm_count, sp, stream);
-        case 8: return launch_ring<RCfg<8, BM25X_RING_KP>>(device, sm_count, sp, stream);
-        case 16: return launch_ring<RCfg<16, BM25X_RING_KP>>(device, sm_count, sp, stream);
-        default: return launch_ring<RCfg<32, BM25X_RING_KP>>(device, sm_count, sp, stream);
-    }
+    return no_launch(M);
 }

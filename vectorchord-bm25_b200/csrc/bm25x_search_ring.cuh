@@ -3,12 +3,12 @@
 // Replaces the per-query cursor walk of bm25::search (crates/bm25/src/search.rs:137-282) for a whole batch: every
 // warp of the persistent grid is a complete query engine (lane j owns term j of its query).
 //
-//   rings     each term ("run") owns a ring of postings in shared memory (the warp's ring budget is split per query in
-//             proportion to the terms' df), filled by TMA bulk copies
+//   rings     each term ("run") owns a ring of postings in shared memory (the classes of 8+ terms split the warp's ring
+//             budget per query in proportion to the terms' df), filled by TMA bulk copies
 //             (cp.async.bulk + mbarrier).  A refill appends exactly as many postings as earlier chunks consumed, so
 //             every posting crosses L2 → shared memory once (the v5 kernel re-fetched the unconsumed tail of every
-//             chunk: 1.66 postings loaded per posting consumed).  One refill round is in flight while the previous
-//             one is processed.
+//             chunk: 1.66 postings loaded per posting consumed).  A ring is one window, refilled after its chunk from
+//             bytes an L2 prefetch issued one round earlier has already pulled into L2.
 //   window    chunk = doc window [lo, hi): hi = the smallest "last landed doc" over the runs that still have postings
 //             in HBM; each lane binary-searches hi in its run → exact in-window range [rd, e), nothing scanned twice.
 //   union     runs are processed in ascending order; run j first TESTS each of its documents against a presence map
@@ -30,8 +30,9 @@
 //             doc - lo instead (the window is clamped to the accumulator size: a ring can be consumed partially).
 //   pruning   MaxScore-style, as v5 (token-level bounds; non-streamed terms are probed in HBM for candidates).
 //
-// Flavours (RCfg::PH).  The above is the PLAIN kernel (PH 0; PH 4 = the same, fed from a device-side query list).  The
-// SEEDED kernel (PH 3; 2..8 terms, k <= 128, no prefilter) takes the documents that hold a single query term from per-term
+// Flavours (RCfg::FLAVOUR, RingFlavour in bm25x_common.h).  The above is the PLAIN kernel (RING_PLAIN; RING_HANDBACK =
+// the same, fed from a device-side query list).  The
+// SEEDED kernel (RING_SEEDED; 2..8 terms, k <= 128, no prefilter) takes the documents that hold a single query term from per-term
 // champion lists (DeviceIndex::champ: a term's best postings in result order — such a document can only be in the
 // top-k if it is among the first k champions of its term).  Its seeds join the candidate list of the doc window they
 // fall into and go through the ordinary verification; the stream itself then never tests a posting on its own, so the
@@ -39,9 +40,9 @@
 // posting words are fetched from HBM for the holders of verified documents alone — the ring searches of a verification
 // pass only list them in a per-warp hit list, scored (word loads, filter, exact score, pool) up to 32 at a time across
 // passes and windows (classes with room for 16 rows or more, RCfg::HITS) — and there is no pruning: queries
-// with a dense list or a list much longer than another one are handed back to the plain kernel (PH 4 launch behind
-// it).  PH 1 / 2 (off by default): plain kernel that suspends a query once no posting can pass alone + doc-id-only kernel
-// that resumes it.
+// with a dense list or a list much longer than another one are handed back to the plain kernel (RING_HANDBACK launch
+// behind it).  Two-phase launches (option "twophase", off by default; 2..4 terms): RING_SUSPEND = the plain kernel,
+// which suspends a query once no posting can pass alone, then RING_RESUME = doc-id-only rings that resume it.
 //
 // Exactness (DESIGN.md §5): the f32 filter only rejects F < Sk·(1-2^-18) and exact-score ties by signature;
 // everything else is ranked by (f64 score desc, doc id asc).
@@ -53,13 +54,6 @@ namespace {
 
 #ifndef BM25X_RING_LOG_R
 #define BM25X_RING_LOG_R -1
-#endif
-#ifndef BM25X_RING_BITMAP
-#define BM25X_RING_BITMAP 1  // 1: the presence map is a BIT map (one bit per cell, marks by shared-memory atomicOr, cleared
-                             // per window) — 8x the cells of the byte map in the same memory; 0: byte map with generation tags
-#endif
-#ifndef BM25X_RING_MAPBYTES
-#define BM25X_RING_MAPBYTES 0  // presence map bytes when not a power of two (multiple of 16); 0: 2^BM25X_RING_LOG_S
 #endif
 #ifndef BM25X_RING_LOG_S
 #define BM25X_RING_LOG_S -1  // log2 of the map bytes; -1: per class (2 KiB of bit cells up to 4 terms, 8 KiB beyond)
@@ -78,20 +72,6 @@ namespace {
 #ifndef BM25X_RING_DENSE_T
 #define BM25X_RING_DENSE_T 48
 #endif
-#ifndef BM25X_RING_SB
-#define BM25X_RING_SB 1  // 1: single-buffered rings (refill after the chunk, next round prefetched into L2); 0: double-buffered
-#endif
-#ifndef BM25X_RING_SUBT
-#define BM25X_RING_SUBT (1u << 30)  // classes of 8+ terms: postings per map generation (sub-window); default: off (no gain on C3 / C4)
-#endif
-#ifndef BM25X_RING_ADAPT
-#define BM25X_RING_ADAPT 1  // 1: ring sizes per query ∝ df; 0: M equal rings
-#endif
-#ifndef BM25X_DOCRING
-#define BM25X_DOCRING 0  // 1: the 2..4-term classes stream DOC IDS ONLY (4 B per posting, SearchParams::pdoc): their hot loop
-                         // never reads tf / fieldnorm once no single-term posting can pass; the posting word is fetched
-                         // from HBM for the few postings that reach the verification.  Twice the postings per ring byte.
-#endif
 #ifndef BM25X_DOCRING_LOG_R
 #define BM25X_DOCRING_LOG_R 9  // doc ids per run of a DOCRING class (2 KiB per run, as 256 8-byte postings)
 #endif
@@ -104,16 +84,6 @@ namespace {
 #ifndef BM25X_DOCRING_LOG_S
 #define BM25X_DOCRING_LOG_S 11  // log2 of the presence map bytes of a DOCRING class
 #endif
-#ifndef BM25X_RING_K2_SHIFT
-#define BM25X_RING_K2_SHIFT 0  // the second bit of a cell word comes from hash bits [SHIFT, SHIFT + 5)
-#endif
-#ifndef BM25X_RING_K2
-#define BM25X_RING_K2 1  // bit map only: THREE bits per document inside one 32-bit cell word (blocked Bloom filter, one
-                         // shared-memory atomicOr / one load as before): false alarms ~ (fill)^3 instead of fill
-#endif
-#ifndef BM25X_SEED_INIT_FULL
-#define BM25X_SEED_INIT_FULL 1
-#endif
 #ifndef BM25X_SUSPEND_MIN
 #define BM25X_SUSPEND_MIN 4096  // first phase: a query is handed to the doc-id-only phase when at least this many postings remain
 #endif
@@ -121,31 +91,38 @@ namespace {
 #define BM25X_PRUNE_ALPHA 0.5  // terms leave the streamed set while the sum of their score bounds stays <= ALPHA · k-th score
 #endif
 
-// PH_: 0 = one launch answers the query.  Two-phase launches of the 2..4-term classes: 1 = first phase (8-byte postings in
-// the rings: every posting's tf / fieldnorm word is at hand while single-term postings can still enter the top-k), which
-// SUSPENDS a query as soon as no posting can pass alone any more; 2 = second phase (doc-id-only rings: twice the postings
-// per ring byte, half the bytes from HBM), which resumes the suspended queries.
-template <int M_, int KP_, int PH_ = 0>
+// FLAVOUR_ (a RingFlavour, kept an int so that the kernel names stay plain numbers):
+//   RING_PLAIN     one launch answers the query.
+//   RING_SUSPEND   two-phase launches of the 2..4-term classes, first phase (8-byte postings in the rings: every posting's
+//                  tf / fieldnorm word is at hand while single-term postings can still enter the top-k), which SUSPENDS a
+//                  query as soon as no posting can pass alone any more;
+//   RING_RESUME    second phase (doc-id-only rings: twice the postings per ring byte, half the bytes from HBM), which
+//                  resumes the suspended queries.
+//   RING_SEEDED    one seeded launch (2..8 terms).
+//   RING_HANDBACK  the plain kernel behind a seeded launch, over the queries it handed back.
+template <int M_, int KP_, int FLAVOUR_>
 struct RCfg {
     static constexpr int M = M_;    // max live terms (lanes 0..M-1 own the terms)
-    static constexpr int PH = PH_;
-    static_assert(PH_ == 0 || (M_ >= 2 && M_ <= 8 && KP_ <= 256), "phased launches: 2..8 terms, pools in shared memory");
-    static_assert((PH_ != 1 && PH_ != 2) || M_ <= 4, "two-phase hand-over record: 4 runs");
+    static constexpr int FLAVOUR = FLAVOUR_;
+    static_assert(FLAVOUR_ == RING_PLAIN || (M_ >= 2 && M_ <= 8 && KP_ <= 256),
+                  "flavours other than plain: 2..8 terms, pools in shared memory");
+    static_assert((FLAVOUR_ != RING_SUSPEND && FLAVOUR_ != RING_RESUME) || M_ <= 4, "two-phase hand-over record: 4 runs");
     static constexpr int KP = KP_;  // pool capacity (power of two >= k + 32)
     // pools beyond 2048 entries (k > 1024, up to the reference's bm25.limit maximum of 65535, src/index/gucs.rs:37-46)
     // live in HBM: one KP-entry slice of SearchParams::pool_scratch per warp
     static constexpr bool POOL_GLOBAL = KP_ > 2048;
     static constexpr size_t POOL_SMEM = POOL_GLOBAL ? 0 : (size_t)KP_;
-    // ring postings per run: half a ring is in flight while the other half is processed
-    // doc-id-only rings (2..4 terms): ring element = u32 doc id, the posting word comes from HBM on demand
-    static constexpr bool DOCRING = PH_ == 2 || PH_ == 3 || (PH_ == 0 && (BM25X_DOCRING != 0) && M_ >= 2 && M_ <= 4);
-    // PH_ = 4: the plain kernel (as PH_ = 0) over the queries a seeded launch handed back (SearchParams::q2)
-    static constexpr bool FROM_Q2 = PH_ == 2 || PH_ == 4;
-    // PH_ = 3: one SEEDED launch — the documents that hold a single query term come from the terms' champion lists
+    // doc-id-only rings (the resume and seeded flavours): ring element = u32 doc id (SearchParams::pdoc, 4 B per
+    // posting: twice the postings per ring byte); the posting word comes from HBM for the few postings that reach the
+    // verification
+    static constexpr bool DOCRING = FLAVOUR_ == RING_RESUME || FLAVOUR_ == RING_SEEDED;
+    // the queries come from the list another launch handed over (SearchParams::q2), not from the batch's work counter
+    static constexpr bool FROM_Q2 = FLAVOUR_ == RING_RESUME || FLAVOUR_ == RING_HANDBACK;
+    // one SEEDED launch — the documents that hold a single query term come from the terms' champion lists
     // (DeviceIndex::champ) before the stream starts, so the stream (doc ids only) never tests a posting on its own
     // A seeded launch never prunes terms (no single-posting test, no probes: a leaner loop) — queries that would gain
-    // from pruning (one list much longer than another) are handed back for the plain kernel (PH_ = 4).
-    static constexpr bool SEEDED = PH_ == 3;
+    // from pruning (one list much longer than another) are handed back for the plain kernel (RING_HANDBACK).
+    static constexpr bool SEEDED = FLAVOUR_ == RING_SEEDED;
     using RT = typename std::conditional<DOCRING, uint32_t, Posting>::type;  // ring element
     static constexpr uint32_t AL = DOCRING ? 4u : 2u;                        // ring elements per 16 bytes (TMA granularity)
     static constexpr int LOG_R = DOCRING ? BM25X_DOCRING_LOG_R : (BM25X_RING_LOG_R > 0 ? BM25X_RING_LOG_R : (M_ <= 8 ? 8 : 7));
@@ -156,11 +133,12 @@ struct RCfg {
     static constexpr int BUDGET = M_ * R;
     // Only the classes of 8+ terms size their rings per query (that is where head terms meet rare ones); for 1..4 terms
     // the geometry stays a compile-time constant (M equal rings): runtime masks and bases slow the 3-term loop down.
-    static constexpr bool ADAPT = (BM25X_RING_ADAPT != 0) && M_ >= 8;
+    static constexpr bool ADAPT = M_ >= 8;
     static constexpr int LOG_RMIN = 6;
-    static constexpr int LOG_RMAX = (LOG_R + 2 > 10 ? 10 : LOG_R + 2) > LOG_R ? (LOG_R + 2 > 10 ? 10 : LOG_R + 2) : LOG_R;
-    static constexpr int LOG_S = M_ == 1 ? 8 : (DOCRING && M_ <= 4) ? BM25X_DOCRING_LOG_S : (BM25X_RING_LOG_S > 0 ? BM25X_RING_LOG_S : (BM25X_RING_BITMAP && M_ <= 4 ? 11 : 13));  // presence map bytes = dense accumulator bytes (unused for one term)
-    static constexpr uint32_t MAP_BYTES = M_ == 1 ? 256u : (BM25X_RING_MAPBYTES ? (uint32_t)BM25X_RING_MAPBYTES : (1u << LOG_S));
+    static constexpr int LOG_RMAX = LOG_R + 2 < 10 ? LOG_R + 2 : 10;
+    // log2 of the presence map bytes = dense accumulator bytes (unused for one term)
+    static constexpr int LOG_S = M_ == 1 ? 8 : (DOCRING && M_ <= 4) ? BM25X_DOCRING_LOG_S : (BM25X_RING_LOG_S > 0 ? BM25X_RING_LOG_S : (M_ <= 4 ? 11 : 13));
+    static constexpr uint32_t MAP_BYTES = 1u << LOG_S;
     static constexpr uint32_t ACC_DOCS = MAP_BYTES / 4u;
     static constexpr int U = DOCRING ? BM25X_DOCRING_G : BM25X_RING_U;  // 16-byte shared loads per lane and trip
     static constexpr int E = DOCRING ? 4 : 2;       // postings per 16-byte load
@@ -171,10 +149,6 @@ struct RCfg {
     static_assert(PL * TMAX <= 32, "one detection bit per posting slot of a lane between two compactions");
     static constexpr int LCAP = TMAX * TRIP + 64;   // candidate list entries, 16 bits each (verified when > 64 are listed)
     static constexpr int INIT = BM25X_RING_INIT;    // postings per run in the very first load (a threshold exists early)
-    // Single-buffered: the whole ring is one window; it is refilled AFTER the chunk (the load is exposed, but it comes
-    // from L2: the bytes were prefetched while the chunk was processed) — half the ring memory per posting in flight,
-    // i.e. more resident warps.  Double-buffered (default): half a ring in flight while the other half is processed.
-    static constexpr bool SB = BM25X_RING_SB != 0;
     static constexpr size_t off_ring = 0;
     static constexpr size_t off_map = off_ring + (size_t)M_ * R * sizeof(RT);
     static constexpr size_t off_pool_s = off_map + (size_t)MAP_BYTES;
@@ -183,9 +157,8 @@ struct RCfg {
     static constexpr size_t off_cand = off_pool_g + POOL_SMEM * 4;
     // seeded launches: the first k champions of the query's terms (doc, w) in shared memory, SST slots per term
     static constexpr uint32_t SST = KP_ <= 64 ? 32u : 128u;
-    static constexpr bool SEEDS_SMEM = SEEDED;
     static constexpr size_t off_seed = (off_cand + (size_t)LCAP * 2 + 7) & ~(size_t)7;
-    static constexpr size_t off_hit = off_seed + (SEEDS_SMEM ? (size_t)M_ * SST * 8 : 0);
+    static constexpr size_t off_hit = off_seed + (SEEDED ? (size_t)M_ * SST * 8 : 0);
     static constexpr size_t off_s1f = 0;  // CTA-shared: 1 KiB table first, then the warps
     static constexpr size_t shared_bytes = 1024;
     static constexpr int MAXW = M_ == 1 ? (BM25X_RING_MAXWARPS > 20 ? BM25X_RING_MAXWARPS : 20) : BM25X_RING_MAXWARPS;
@@ -210,7 +183,7 @@ struct RCfg {
     static constexpr size_t total = shared_bytes + warp_bytes * WARPS;
     static constexpr int THREADS = WARPS * 32;
     static_assert(WARPS >= 1, "one warp must fit");
-    static_assert(LOG_RMAX <= 10 && LOG_R >= LOG_RMIN && M_ <= 32 && MAP_BYTES / 4u <= 32768u && MAP_BYTES % 16u == 0u,
+    static_assert(LOG_R <= LOG_RMAX && LOG_R >= LOG_RMIN && M_ <= 32 && MAP_BYTES / 4u <= 32768u && MAP_BYTES % 16u == 0u,
                   "entry format: bit 15 = dense flavour (15-bit doc offset), else 5-bit run | 10-bit ring position");
     static_assert(ACC_DOCS >= 64, "accumulator too small");
 };
@@ -270,31 +243,22 @@ __device__ unsigned long long g_phase_prof[PP_SLOTS];
 #define PP_CONSUME(a, b) do {} while (0)
 #endif
 
-// slot of a document in a map of `bytes` cells: multiplicative hash, then the high half of hash × bytes (any size)
-__device__ __forceinline__ uint32_t ring_slot(uint32_t doc, uint32_t bytes) { return __umulhi(doc * 0x9E3779B1u, bytes); }
-
-// Bit map (BM25X_RING_BITMAP): the 32-bit cell word of a document (its word index) and the bits it sets / tests there.
-// Slot = high half of hash × cells; for a power-of-two map that is a plain shift of the hash (the same bits, one
-// instruction instead of IMAD.HI + mask).  The bit shifts wrap (SHF.L.W): 1 << x takes x's low 5 bits, no mask needed.
+// Presence map: the 32-bit cell word of a document (its word index) and the THREE bits it sets / tests there (a blocked
+// Bloom filter: one shared-memory atomicOr or load per posting; false alarms ~ fill^3).  Multiplicative hash; the slot
+// is its top log2(cells) bits (the high half of hash × cells of a power-of-two map, one instruction instead of IMAD.HI +
+// mask), the second bit comes from its low 5 bits, the third from the next 5.  The bit shifts wrap (SHF.L.W): 1 << x
+// takes x's low 5 bits, no mask needed.
 template <class C>
 __device__ __forceinline__ uint32_t map_word(uint32_t doc, uint32_t &msk) {
-    constexpr uint32_t CELLS = C::MAP_BYTES * 8u;
-    constexpr int LOG_CELLS = 31 - __builtin_clz(CELLS);
+    static_assert((C::MAP_BYTES & (C::MAP_BYTES - 1u)) == 0u, "the presence map is a power of two bytes");
+    constexpr int LOG_CELLS = 31 - __builtin_clz(C::MAP_BYTES * 8u);
     const uint32_t hsh = doc * 0x9E3779B1u;
-    uint32_t slot, word;
-    if constexpr ((CELLS & (CELLS - 1u)) == 0u) {
-        slot = hsh >> (32 - LOG_CELLS);
-        // (a shift the compiler cannot merge with the caller's ×4 into shift + mask + add: one IMAD forms the address)
-        asm("shr.b32 %0, %1, %2;" : "=r"(word) : "r"(hsh), "n"(32 - LOG_CELLS + 5));
-    } else {
-        slot = __umulhi(hsh, CELLS);
-        word = slot >> 5;
-    }
+    const uint32_t slot = hsh >> (32 - LOG_CELLS);
+    uint32_t word;
+    // (a shift the compiler cannot merge with the caller's ×4 into shift + mask + add: one IMAD forms the address)
+    asm("shr.b32 %0, %1, %2;" : "=r"(word) : "r"(hsh), "n"(32 - LOG_CELLS + 5));
     msk = __funnelshift_l(0u, 1u, slot);
-#if BM25X_RING_K2
-    // second bit: low 5 bits of the hash (or from bit BM25X_RING_K2_SHIFT); third bit: the next 5 bits
-    msk |= __funnelshift_l(0u, 1u, BM25X_RING_K2_SHIFT ? hsh >> BM25X_RING_K2_SHIFT : hsh) | __funnelshift_l(0u, 1u, hsh >> 5);
-#endif
+    msk |= __funnelshift_l(0u, 1u, hsh) | __funnelshift_l(0u, 1u, hsh >> 5);
     return word;
 }
 // lower_bound of `doc` in ring positions [a, e) (posting indices of the term; the ring holds index i at i & RM).
@@ -313,19 +277,13 @@ __device__ __forceinline__ uint32_t ring_lower_bound(const typename C::RT *rg, u
     }
     return pos;
 }
-// posting word of `doc` in [a, e), 0 when absent.  gpost = the term's postings in HBM (posting index = ring index):
-// doc-id-only rings fetch the word from there.
+// posting word of `doc` in [a, e), 0 when absent (8-byte rings)
 template <class C, int TOP = C::LOG_RMAX>
-__device__ __forceinline__ uint32_t ring_find(const typename C::RT *rg, uint32_t mask, uint32_t a, uint32_t e, uint32_t doc,
-                                              const Posting *gpost) {
+__device__ __forceinline__ uint32_t ring_find(const Posting *rg, uint32_t mask, uint32_t a, uint32_t e, uint32_t doc) {
     const uint32_t l = ring_lower_bound<C, TOP>(rg, mask, a, e, doc);
     if (l < e) {
-        if constexpr (C::DOCRING) {
-            if (rg[l & mask] == doc) return __ldg(&gpost[l].w);
-        } else {
-            const Posting v = rg[l & mask];
-            if (v.doc == doc) return v.w;
-        }
+        const Posting v = rg[l & mask];
+        if (v.doc == doc) return v.w;
     }
     return 0u;
 }
@@ -408,7 +366,6 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
     const double kEps = 1.0 / 262144.0;
     const float s1min = p.s1f_min;
     uint32_t parity = 0;  // mbarrier phase parity
-    uint32_t gen = 0;     // generation tag of the chunk (1..255), never reset: stale tags cost false alarms only
 #ifdef BM25X_PHASE_PROF
     uint32_t pp_acc = 0u, pp_t = (uint32_t)clock();  // lane i: cycles of phase i (or counter i) of the current query
 #endif
@@ -583,9 +540,6 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
         float FloT = -1.f;         // filter threshold on the score over ALL terms (f.Flo: over the streamed terms only)
         bool thr_new = false;     // the threshold moved since the pruned set was last reconsidered
         uint32_t wlim = C::SEEDED ? 0xFFFFFFFFu : 255u;  // lane j: single-term postings of run j can pass only if w > wlim  (tf >= 1: all)
-#ifdef BM25X_DIAG_NOSOLO
-        wlim = 0xFFFFFFFFu;
-#endif
         uint32_t tiew = 0xFFFFFFFFu;  // lane j: posting word of the tie signature when it belongs to run j
 
         // f32 filter constants from (Sk, tie signature, pruned set)
@@ -610,9 +564,6 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
             // the term's best posting (its token-level bound) stays below the threshold: no posting of this run can
             // enter alone, the hot loop drops the single-term test altogether
             if (lane < (int)m && ubd < flo) wlim = 0xFFFFFFFFu;
-#ifdef BM25X_DIAG_NOSOLO  // timing diagnostics only (wrong results): no posting ever passes alone
-            wlim = 0xFFFFFFFFu;
-#endif
             tiew = (f.tie_dk != INF && (f.tie_sig >> 27) == (uint32_t)lane) ? (f.tie_sig & 0x07FFFFFFu) : 0xFFFFFFFFu;
             if constexpr (C::SEEDED) {  // single-term documents come from the champion lists: the stream lists no posting on its own
                 wlim = 0xFFFFFFFFu;
@@ -778,16 +729,14 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                 else src = p.post + pbase + wr;
                 tma_load_1d(myring + off, src, n1 * (uint32_t)sizeof(RT), bar);
                 if (n > n1) tma_load_1d(myring, src + n1, (n - n1) * (uint32_t)sizeof(RT), bar);
-#ifndef BM25X_DIAG_SOLOFRAC
                 fetched += min(wr + n, dfj) - min(wr, dfj);  // the pad slots of a list are not postings
-#endif
                 wr += n;
             }
             return true;
         };
 
         bool inflight;
-        if constexpr (C::PH == 2) {
+        if constexpr (C::FLAVOUR == RING_RESUME) {
             // ---- resume: cursors, threshold, pruned set from the record; the pool entries from the query's output rows ----
             const ResumeRec *rec = p.resume + qi;
             const size_t ob = (size_t)qid * k;
@@ -815,7 +764,7 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
             inflight = issue_round(lane < (int)m && !((ne_mask >> lane) & 1u) ? min(rsize, dfpad - wr) : 0u);
         } else {
             // (a seeded launch needs no early threshold: whole rings from the start)
-            inflight = issue_round(lane < (int)m ? min(dfpad, C::SEEDED && BM25X_SEED_INIT_FULL ? rsize : (uint32_t)C::INIT) : 0u);
+            inflight = issue_round(lane < (int)m ? min(dfpad, C::SEEDED ? rsize : (uint32_t)C::INIT) : 0u);
         }
         // ---- seeds: a document that holds ONE query term can only be in the top-k if it is among the first k champions
         // of that term (DeviceIndex::champ: every posting ranked before it in (single-term score desc, doc asc) belongs
@@ -831,31 +780,23 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                 ncj = min(dfj, min(k, (uint32_t)BM25X_CHAMP_L));
                 coff = p.champ_off[p.q_terms[t0 + lane]];
             }
-            if constexpr (C::SEEDS_SMEM) {
-                seeds = (Posting *)(ws + C::off_seed);
+            seeds = (Posting *)(ws + C::off_seed);
 #pragma unroll
-                for (int jj = 0; jj < C::M; ++jj) {
-                    const uint32_t nj = __shfl_sync(FULL, ncj, jj);
-                    const uint64_t cj = __shfl_sync(FULL, coff, jj);
-                    for (uint32_t r = (uint32_t)lane; r < C::SST && r < ((k + 31u) & ~31u); r += 32) {
-                        Posting v;
-                        v.doc = INF;  // slots beyond the list: never inside a window
-                        v.w = 0u;
-                        if (r < nj) v = p.champ[cj + r];
-                        seeds[jj * C::SST + r] = v;
-                    }
+            for (int jj = 0; jj < C::M; ++jj) {
+                const uint32_t nj = __shfl_sync(FULL, ncj, jj);
+                const uint64_t cj = __shfl_sync(FULL, coff, jj);
+                for (uint32_t r = (uint32_t)lane; r < C::SST && r < ((k + 31u) & ~31u); r += 32) {
+                    Posting v;
+                    v.doc = INF;  // slots beyond the list: never inside a window
+                    v.w = 0u;
+                    if (r < nj) v = p.champ[cj + r];
+                    seeds[jj * C::SST + r] = v;
                 }
-                __syncwarp();
             }
+            __syncwarp();
         }
-#ifdef BM25X_WATCHDOG
-        uint32_t wd_chunks = 0;
-#endif
         PP_MARK(PP_QUERY);
         for (;;) {
-#ifdef BM25X_WATCHDOG
-            if (++wd_chunks > (1u << 26)) __trap();  // debug builds: a query that never ends becomes a launch failure
-#endif
             // ---- chunk boundary: the outstanding round has landed ----
             if (inflight) {
                 mbar_wait(bar, parity);
@@ -901,7 +842,7 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                 }
                 if (changed) {
                     refresh_filter();
-                    if (C::ADAPT && C::SB) {
+                    if (C::ADAPT) {
                         // the pruned terms' rings go back to the budget: the streamed terms get wider windows.  Their rings
                         // move, so what they held beyond rd is fetched again (a few hundred postings, a few times per query)
                         alloc_rings(~ne_mask);
@@ -918,7 +859,7 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                 }
             }
             const bool act = lane < (int)m && !((ne_mask >> lane) & 1u);
-            if constexpr (C::PH == 1) {
+            if constexpr (C::FLAVOUR == RING_SUSPEND) {
                 // ---- hand-over: no posting of a streamed run can enter the top-k alone any more (wlim), so the rest of the
                 // query only needs doc ids — suspend it for the second phase.  Nothing is in flight here (the round has
                 // landed); the pool travels in the query's own output rows, the rest in the record.
@@ -973,11 +914,10 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
             }
             // ---- dense or sparse?  (expected number of documents held by two runs in this window) ----
             bool dense = false;
-            uint32_t span = 0, chunk_postings = 0;
+            uint32_t span = 0;
             if (C::M > 1) {
                 const uint32_t n = e - rd;
                 const uint32_t S = __reduce_add_sync(FULL, n);
-                chunk_postings = S;
                 const uint32_t S2 = __reduce_add_sync(FULL, n * n);
                 uint32_t hi_eff = hi;
                 if (last) hi_eff = __reduce_max_sync(FULL, n ? ring_doc(myring, (e - 1u) & rmask) + 1u : 0u);
@@ -991,17 +931,6 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                 }
             }
             PP_MARK(PP_SETUP);
-            // ---- refill: append what earlier chunks consumed (at most half a ring per round) ----
-            if (!C::SB) {
-                uint32_t n = 0;
-                if (act && wr < dfpad) {
-                    const uint32_t fr = rsize - (wr - rd);
-                    n = min(min(fr, rsize / 2) & ~(C::AL - 1u), dfpad - wr);
-                    // no small top-ups while the run still holds a quarter ring beyond this chunk
-                    if (n < rsize / 8 && wr - e >= rsize / 4) n = 0;
-                }
-                inflight = issue_round(n);
-            }
 
             uint32_t nc = 0;  // listed candidates (warp-uniform)
             // ---- verification: 32 listed postings at a time ----
@@ -1042,11 +971,8 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                         solo_j = __shfl_sync(FULL, wlim, j & 31u) != 0xFFFFFFFFu;
                         // seeded launch: a lone streamed holder only matters when a pruned term may hold the document too
                         if constexpr (C::SEEDED) solo_j = false;
-                        if constexpr (C::SEEDS_SMEM) {
+                        if constexpr (C::SEEDED) {
                             if (is_seed) own = seeds[sidx];
-                        } else if constexpr (C::SEEDED) {
-                            const uint64_t cjs = __shfl_sync(FULL, coff, j & 31u);
-                            if (is_seed) own = p.champ[cjs + (sidx % C::SST)];
                         }
                         const uint32_t rmj = C::ADAPT ? __shfl_sync(FULL, rmask, j & 31u) : (uint32_t)C::R - 1u;
                         if (has && !by_doc && !is_seed) {
@@ -1066,12 +992,14 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                     uint32_t wv[KEEPW ? C::M : 1];
 #pragma unroll
                     for (int i = 0; i < (KEEPW ? C::M : 1); ++i) wv[i] = 0u;
+                    // posting word of run i's holder of the document (8-byte rings; the doc-id-only flavours search with
+                    // ring_find_pos and never call this)
                     auto holder = [&](int i, uint32_t ib, uint32_t im, uint32_t ai, uint32_t ei) -> uint32_t {
-                        const Posting *gi = nullptr;
-                        if constexpr (C::DOCRING) gi = p.post + __shfl_sync(FULL, pbase, i);  // (not reached: DOCRING has its own front end)
-                        return (uint32_t)i == j ? own.w
-                                                : (small_rings ? ring_find<C, C::LOG_R>(rings + ib, im, ai, ei, doc, gi)
-                                                               : ring_find<C>(rings + ib, im, ai, ei, doc, gi));
+                        if constexpr (C::DOCRING) return 0u;
+                        else
+                            return (uint32_t)i == j ? own.w
+                                                    : (small_rings ? ring_find<C, C::LOG_R>(rings + ib, im, ai, ei, doc)
+                                                                   : ring_find<C>(rings + ib, im, ai, ei, doc));
                     };
                     auto filter_term = [&](int i) {
                         const uint32_t ai = __shfl_sync(FULL, rd, i), ei = __shfl_sync(FULL, e, i);
@@ -1195,7 +1123,7 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                             const uint32_t o = (lane & 1) ? (j == 2u ? 1u : 2u) : (j == 0u ? 1u : 0u);
                             const uint32_t ao = __shfl_sync(FULL, rd, o), eo = __shfl_sync(FULL, e, o);
                             uint32_t wo = 0u;
-                            if (has) wo = ring_find<C, C::LOG_R>(rings + o * C::R, C::R - 1u, ao, eo, doc, nullptr);
+                            if (has) wo = ring_find<C, C::LOG_R>(rings + o * C::R, C::R - 1u, ao, eo, doc);
                             const uint32_t wx = __shfl_xor_sync(FULL, wo, 1);  // the partner's run
                             const uint32_t ox = (lane & 1) ? (j == 0u ? 1u : 0u) : (j == 2u ? 1u : 2u);
                             has = has && !(lane & 1);
@@ -1326,29 +1254,13 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                 nc = 0;
             };
 
-
-            // Classes of 8+ terms unite a few thousand postings per chunk: the presence map would be a quarter full and a
-            // tenth of all postings false alarms.  The chunk is therefore walked in doc SUB-WINDOWS of about SUBT postings,
-            // each with its own map generation (one more boundary search per run and sub-window, lanes in parallel).
-            uint32_t nsub = 1;
-            if (C::M >= 8 && !dense) nsub = min(8u, (chunk_postings + BM25X_RING_SUBT - 1u) / BM25X_RING_SUBT);
-            if (nsub < 1u) nsub = 1u;
-            const uint32_t e_full = e;
-            for (uint32_t sub = 0; sub < nsub; ++sub) {
-            if (nsub > 1u) {
-                e = e_full;
-                if (sub + 1u < nsub) {
-                    const uint32_t hs = lo + (uint32_t)(((unsigned long long)span * (sub + 1u)) / nsub);
-                    e = act ? ring_lower_bound<C>(myring, rmask, rd, e_full, hs) : rd;
-                }
-            }
             // ---- candidate production (resumable) + ONE verification site ----
             // sparse window: runs in ascending order; each run tests its documents against the marks of the earlier runs,
             // then marks them.  dense window: scores summed in an f32 accumulator indexed by doc - lo (in the map's
             // memory; docs are distinct inside a run: plain read-modify-write, __syncwarp between runs), then scanned.
-            uint32_t todo = 0u, ra = 0u, ree = 0u, wl = 0u, tw = 0u, tdk = 0u, pb = 0u, genv = 0u, dbase = 0u, rm = 1u;
+            uint32_t todo = 0u, ra = 0u, ree = 0u, wl = 0u, tw = 0u, tdk = 0u, pb = 0u, dbase = 0u, rm = 1u;
             int rj = -1, variant = 0;
-            uint32_t ss = sub == 0u ? 0u : 0xFFFFFFFFu;  // seeded launches: next slice (term, 32 slots) of the seed table to look at in this window
+            uint32_t ss = 0u;  // seeded launches: next slice (term, 32 slots) of the seed table to look at in this window
             bool multi = false;
             const uint4 *rg = nullptr;
             const uint4 *gq = nullptr;  // DOCRING: the current run's 8-byte postings in HBM (single-term test only)
@@ -1356,9 +1268,7 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
             if (!dense) {
                 todo = __ballot_sync(FULL, act && e > rd);
                 multi = C::M > 1 && __popc(todo) > 1;
-                if (multi) gen = gen % 255u + 1u;
-                genv = gen;
-                if (BM25X_RING_BITMAP && multi) {  // bit cells carry no generation: clear the map for this window
+                if (multi) {  // clear the map for this window
                     for (int i = lane; i < (int)(C::MAP_BYTES / 16u); i += 32) ((uint4 *)map)[i] = make_uint4(0, 0, 0, 0);
                     __syncwarp();
                 }
@@ -1450,7 +1360,6 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                                 const bool valid = (vm >> (C::E * u + h)) & 1u;
                                 bool c = false;
                                 if (TEST || MARK) {
-#if BM25X_RING_BITMAP
                                     uint32_t msk;
                                     uint32_t *cell = (uint32_t *)map + map_word<C>(doc, msk);
                                     // an invalid slot ORs nothing in (an atomic with an empty mask: no branch around it)
@@ -1469,11 +1378,6 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                                     // hit: every bit of msk was set already (one LOP3 sets the predicate, one predicated
                                     // add records it)
                                     if (TEST) c = (msk & ~old) == 0u;
-#else
-                                    const uint32_t slot = ring_slot(doc, C::MAP_BYTES);
-                                    if (TEST) c = map[slot] == genv;
-                                    if (MARK && valid) map[slot] = (uint8_t)genv;
-#endif
                                 }
                                 if (SOLO) c = c | ((w > wl) & !((w == tw) & (doc > tdk)));  // bitwise: no branches
                                 if (c) bits += 1u << (C::E * u + h);
@@ -1511,11 +1415,7 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                     // the seeds of this doc window join the candidate list first (entry: run field 31 | seed slot); the
                     // rings hold every run's postings of the window, so the ONE verification site below tells whether
                     // another term holds the document
-#ifdef BM25X_DIAG_NOSEEDS  // timing diagnostics only (wrong results): the seeds never join
-                    const uint32_t slices = 0u;
-#else
                     const uint32_t slices = (min(k, (uint32_t)BM25X_CHAMP_L) + 31u) >> 5;  // per term
-#endif
 #pragma unroll 1
                     while (ss < (uint32_t)C::M * slices && nc <= 64u) {
                         uint32_t jj = ss, r = (uint32_t)lane;
@@ -1595,30 +1495,26 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                 }
                 if (nc) verify();
             }
-#ifdef BM25X_DIAG_SOLOFRAC  // statistics diagnostics: `fetched` counts the postings consumed while some run can pass alone
-            if (__any_sync(FULL, act && wlim != 0xFFFFFFFFu)) fetched += e - rd;
-#endif
             rd = e;
-            }  // sub-windows
             lo = hi;
             if (last) break;
-            if (C::SB) {  // single-buffered: refill everything this chunk freed; the bytes should already sit in L2
-                uint32_t n = 0;
-                if (act && wr < dfpad) {
-                    n = min((rsize - (wr - rd)) & ~(C::AL - 1u), dfpad - wr);
-                    if (n < rsize / 4 && wr - rd >= rsize / 4) n = 0;  // no small top-ups
-                }
-                inflight = issue_round(n);
-                if (n > 0 && wr < dfpad) {  // the round after this one: into L2 while this chunk's successor is processed
-                    const uint32_t pn_ = min(rsize, dfpad - wr);
-                    if constexpr (C::DOCRING) {
-                        asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p.pdoc + pbase + wr), "r"(pn_ * 4u) : "memory");
-                        // while postings of this run can still pass alone, the loop also reads their tf / fieldnorm words
-                        if (wlim != 0xFFFFFFFFu)
-                            asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p.post + pbase + wr), "r"(pn_ * 8u) : "memory");
-                    } else {
+            // ---- refill: everything this chunk freed (the ring is one window, refilled after it: the load is exposed,
+            // but the bytes should already sit in L2 — half the ring memory per posting in flight, i.e. more resident warps)
+            uint32_t n = 0;
+            if (act && wr < dfpad) {
+                n = min((rsize - (wr - rd)) & ~(C::AL - 1u), dfpad - wr);
+                if (n < rsize / 4 && wr - rd >= rsize / 4) n = 0;  // no small top-ups
+            }
+            inflight = issue_round(n);
+            if (n > 0 && wr < dfpad) {  // the round after this one: into L2 while this chunk's successor is processed
+                const uint32_t pn_ = min(rsize, dfpad - wr);
+                if constexpr (C::DOCRING) {
+                    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p.pdoc + pbase + wr), "r"(pn_ * 4u) : "memory");
+                    // while postings of this run can still pass alone, the loop also reads their tf / fieldnorm words
+                    if (wlim != 0xFFFFFFFFu)
                         asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p.post + pbase + wr), "r"(pn_ * 8u) : "memory");
-                    }
+                } else {
+                    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p.post + pbase + wr), "r"(pn_ * 8u) : "memory");
                 }
             }
             PP_MARK(PP_END);

@@ -221,8 +221,8 @@ void bm25x_batch_destroy(bm25x_batch *batch);
  * k1, b, sealed avgdl) (search.rs:49-51,66-77; `insert` does not update them) — and shares the Results heap with the
  * sealed documents.  Here the growing documents are inverted once into a second, small index handle that carries
  * the sealed statistics, so the same kernels unite their postings; a query then is two top-k searches + a merge.
- * Doc ids of the growing handle are growing ordinals (insertion order).  Re-create the handle after inserts/deletes
- * (it is as cheap as the segment is small); `maintain`/seal = build a new sealed index. */
+ * Doc ids of the growing handle are growing ordinals (insertion order).  The handle is immutable: a segment that takes
+ * inserts and deletes in place is bm25x_growing_segment below; `maintain`/seal = build a new sealed index. */
 typedef struct {
     uint32_t n_docs;               /* growing documents, in VectorTuple-chain order */
     const uint32_t *doc_len;       /* [n_docs] exact lengths, or NULL: then doc_fieldnorm */
@@ -239,7 +239,9 @@ int bm25x_growing_create(const bm25x_index *sealed, const bm25x_growing_docs *do
 /* bm25::search over sealed + growing: bm25x_search_batch on both handles and the merge below.  `growing` may be NULL
  * (sealed only).  Doc ids >= n_docs(sealed) denote growing ordinal (id - n_docs(sealed)); on equal scores sealed
  * documents come first, then ascending id (the reference's order of equal scores is not pinned, see bm25x_search_batch).
- * allow_growing: optional prefilter bitmap over growing ordinals. */
+ * allow_growing: optional prefilter bitmap over growing ordinals.  Both lists are merged on the device
+ * (k_merge_shards): stats are those of bm25x_sharded_search_batch (sums over both handles plus the merge launch, so
+ * `launches` and `kernel_ms` include the merge), except `queries` = the sealed search's live queries. */
 int bm25x_search_batch_growing(bm25x_index *sealed, bm25x_index *growing, uint32_t nq, const uint32_t *q_off,
                                const uint32_t *q_terms, uint32_t k, const uint8_t *allow_sealed,
                                const uint8_t *allow_growing, uint32_t *out_doc, float *out_score, double *out_score64,
@@ -250,6 +252,54 @@ int bm25x_merge_topk(uint32_t nq, uint32_t k, const uint32_t *doc_a, const float
                      const uint16_t *payload_a, const uint32_t *n_a, const uint32_t *doc_b, const float *score_b,
                      const double *score64_b, const uint16_t *payload_b, const uint32_t *n_b, uint32_t doc_base_b,
                      uint32_t *out_doc, float *out_score, double *out_score64, uint16_t *out_payload, uint32_t *out_n);
+
+/* ---- the mutable growing segment: the documents inserted since the last seal, owned by the library and indexed on the
+ * sealed index's device.  bm25x_growing_insert appends documents (`insert`, crates/bm25/src/insert.rs) and
+ * bm25x_growing_delete sets their deleted flag (`bulkdelete`, bulkdelete.rs); both cost host work in proportion to what
+ * they change.  A refresh brings the segment's index handle up to date on the device: the surviving postings of the
+ * current handle and the inserted ones are spliced into a new handle built beside it, which then replaces it.  A search
+ * over sealed + growing is one call (both handles' kernels, one device merge, one download) and refreshes first when
+ * anything is pending.  Every call may come from any thread: a search sees one state of the segment, with every insert
+ * and delete that returned before it started and never part of one; a handle a running search still holds is destroyed
+ * when that search ends.  The sealed index must outlive the segment. */
+typedef struct bm25x_growing_segment bm25x_growing_segment;
+typedef struct {
+    uint32_t n_docs;        /* ordinals handed out (deleted ones included) */
+    uint32_t n_deleted;
+    uint64_t n_postings;    /* postings in the segment's handle (as of the last refresh) */
+    uint64_t device_bytes;  /* HBM held by the segment's handle */
+    uint32_t pending;       /* 1: inserts or deletes since the last refresh */
+    int device;             /* the sealed index's */
+} bm25x_growing_info;
+/* An empty segment on the sealed index's device, scoring with its statistics. */
+int bm25x_growing_open(bm25x_index *sealed, bm25x_growing_segment **out);
+/* Appends docs as ordinals n_docs .. n_docs + docs->n_docs - 1 (deleted flags included).  Refuses what
+ * bm25x_growing_create refuses, with its codes and messages (terms not ascending, tf = 0, tf >= 2^24, sealed n_docs +
+ * growing n_docs above 2^32 - 2), and documents in the other norm form than the segment's first insert (doc_len vs
+ * doc_fieldnorm, BM25X_ERR_INVALID).  A refused insert changes nothing.  Without a payload a document gets the synthetic
+ * ctid of its ordinal, as bm25x_growing_create gives it. */
+int bm25x_growing_insert(bm25x_growing_segment *g, const bm25x_growing_docs *docs);
+/* Marks ordinals deleted (bulkdelete).  An ordinal >= n_docs is refused (BM25X_ERR_INVALID, naming the first one) and
+ * nothing is applied; deleting a deleted ordinal is a no-op.  Sealed documents are filtered with allow_sealed. */
+int bm25x_growing_delete(bm25x_growing_segment *g, uint32_t n, const uint32_t *ordinals);
+/* Brings the handle up to date (a no-op when nothing is pending).  Optional: the search refreshes too.  Its arrays are
+ * those bm25x_growing_create builds over all documents inserted so far with their deleted flags. */
+int bm25x_growing_refresh(bm25x_growing_segment *g);
+int bm25x_growing_get_info(const bm25x_growing_segment *g, bm25x_growing_info *out);
+/* The contract, refusals and rows of bm25x_search_batch_growing on a handle bm25x_growing_create builds from the
+ * segment's documents: sealed ids as they are, growing ordinal o as n_docs(sealed) + o; score desc, on equal scores
+ * sealed first, then ascending id.  allow_growing covers ordinals [0, allow_growing_docs): ordinals at or past it are
+ * filtered out (NULL = all pass).  A pending refresh runs first and counts in h2d_ms.  stats: sums over both
+ * searches plus the merge launch (queries included); before the first insert, the call is bm25x_search_batch on the
+ * sealed index, stats included. */
+int bm25x_growing_search_batch(bm25x_growing_segment *g, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms,
+                               uint32_t k, const uint8_t *allow_sealed, const uint8_t *allow_growing,
+                               uint32_t allow_growing_docs, uint32_t *out_doc, float *out_score, double *out_score64,
+                               uint16_t *out_payload, uint32_t *out_n, bm25x_search_stats *stats);
+/* Test hook: the arrays of the segment's current handle, as bm25x_sharded_get_shard reports a shard's (either output may
+ * be NULL); valid until the next refresh or close.  Refused before the first refresh of a non-empty segment. */
+int bm25x_growing_get_index(const bm25x_growing_segment *g, bm25x_index_layout *layout, bm25x_index_derived *derived);
+void bm25x_growing_close(bm25x_growing_segment *g);
 
 /* ---- document-sharded index: one sealed segment split by document range over one or more GPUs, so that its postings
  * need not fit in one GPU's HBM.  Every shard scores with the WHOLE segment's statistics (N, avgdl, df), so its top-k is

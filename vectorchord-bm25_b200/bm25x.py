@@ -47,6 +47,11 @@ class _GrowingDocs(C.Structure):
                 ("elem_tf", C.POINTER(C.c_uint32))]
 
 
+class GrowingInfo(C.Structure):  # bm25x_growing_info
+    _fields_ = [("n_docs", C.c_uint32), ("n_deleted", C.c_uint32), ("n_postings", C.c_uint64),
+                ("device_bytes", C.c_uint64), ("pending", C.c_uint32), ("device", C.c_int)]
+
+
 class IndexInfo(C.Structure):
     _fields_ = [("n_docs", C.c_uint32), ("n_terms", C.c_uint32), ("n_postings", C.c_uint64),
                 ("sum_doc_len", C.c_uint64), ("avgdl", C.c_double), ("k1", C.c_double), ("b", C.c_double),
@@ -124,6 +129,16 @@ def load_library():
     L.bm25x_growing_create.argtypes = [vp, C.POINTER(_GrowingDocs), C.POINTER(vp)]
     L.bm25x_search_batch_growing.argtypes = [vp, vp, C.c_uint32, u32p, u32p, C.c_uint32, u8p, u8p, u32p, f32p, f64p,
                                              u16p, u32p, C.POINTER(SearchStats)]
+    L.bm25x_growing_open.argtypes = [vp, C.POINTER(vp)]
+    L.bm25x_growing_insert.argtypes = [vp, C.POINTER(_GrowingDocs)]
+    L.bm25x_growing_delete.argtypes = [vp, C.c_uint32, u32p]
+    L.bm25x_growing_refresh.argtypes = [vp]
+    L.bm25x_growing_get_info.argtypes = [vp, C.POINTER(GrowingInfo)]
+    L.bm25x_growing_search_batch.argtypes = [vp, C.c_uint32, u32p, u32p, C.c_uint32, u8p, u8p, C.c_uint32, u32p, f32p,
+                                             f64p, u16p, u32p, C.POINTER(SearchStats)]
+    L.bm25x_growing_get_index.argtypes = [vp, C.POINTER(IndexLayout), C.POINTER(IndexDerived)]
+    L.bm25x_growing_close.argtypes = [vp]
+    L.bm25x_growing_close.restype = None
     L.bm25x_merge_topk.argtypes = [C.c_uint32, C.c_uint32, u32p, f32p, f64p, u16p, u32p, u32p, f32p, f64p, u16p, u32p,
                                    C.c_uint32, u32p, f32p, f64p, u16p, u32p]
     L.bm25x_index_destroy.argtypes = [vp]
@@ -463,23 +478,16 @@ class Index:
         """Handle over the growing documents (doc-major: document g holds elements elem_off[g]..elem_off[g+1], term
         ordinals of THIS sealed index ascending, TERM_MISSING for tokens it does not know) that scores with this
         index's statistics (bm25x_growing_create).  Search it like any index; ids are growing ordinals."""
-        g = _GrowingDocs()
         keep = []
-        g.elem_off = _kept(keep, elem_off, np.uint64, C.c_uint64)
-        g.n_docs = len(keep[-1]) - 1
-        g.elem_term = _kept(keep, elem_term, np.uint32, C.c_uint32)
-        g.elem_tf = _kept(keep, elem_tf, np.uint32, C.c_uint32)
-        if doc_len is not None:
-            g.doc_len = _kept(keep, doc_len, np.uint32, C.c_uint32)
-        if doc_fieldnorm is not None:
-            g.doc_fieldnorm = _kept(keep, doc_fieldnorm, np.uint8, C.c_uint8)
-        if payload is not None:
-            g.payload = _kept(keep, payload, np.uint16, C.c_uint16)
-        if deleted is not None:
-            g.deleted = _kept(keep, deleted, np.uint8, C.c_uint8)
+        g = _growing_docs(keep, elem_off, elem_term, elem_tf, doc_len, doc_fieldnorm, payload, deleted)
         h = C.c_void_p()
         _check(load_library().bm25x_growing_create(self.h, C.byref(g), C.byref(h)))
         return Index._adopt(h, g.n_docs, self.n_terms)
+
+    def growing_segment(self) -> "GrowingSegment":
+        """An empty mutable growing segment on this index's device (bm25x_growing_open): insert / delete in place,
+        search sealed + growing in one call.  This index must stay open while the segment is."""
+        return GrowingSegment(self)
 
     def search_batch_growing(self, growing, q_off, q_terms, k, allow=None, allow_growing=None, want_payload=False):
         """bm25::search over this sealed index + a growing handle (None = sealed only): ids >= n_docs are growing
@@ -518,6 +526,88 @@ class Index:
 
     def evaluate(self, document: Document, query: Query) -> float:
         return float(self.evaluate_batch([document], [query])[0])
+
+
+def _growing_docs(keep, elem_off, elem_term, elem_tf, doc_len, doc_fieldnorm, payload, deleted):
+    g = _GrowingDocs()
+    g.elem_off = _kept(keep, elem_off, np.uint64, C.c_uint64)
+    g.n_docs = len(keep[-1]) - 1
+    g.elem_term = _kept(keep, elem_term, np.uint32, C.c_uint32)
+    g.elem_tf = _kept(keep, elem_tf, np.uint32, C.c_uint32)
+    if doc_len is not None:
+        g.doc_len = _kept(keep, doc_len, np.uint32, C.c_uint32)
+    if doc_fieldnorm is not None:
+        g.doc_fieldnorm = _kept(keep, doc_fieldnorm, np.uint8, C.c_uint8)
+    if payload is not None:
+        g.payload = _kept(keep, payload, np.uint16, C.c_uint16)
+    if deleted is not None:
+        g.deleted = _kept(keep, deleted, np.uint8, C.c_uint8)
+    return g
+
+
+class GrowingSegment:
+    """The growing segment as the library keeps it (bm25x_growing_*): documents inserted and deleted in place, indexed on
+    the sealed index's device by a refresh, searched together with the sealed index.  Growing ordinal o comes back as
+    doc id sealed.n_docs + o."""
+
+    def __init__(self, sealed: Index):
+        self.sealed = sealed
+        self.h = C.c_void_p()
+        _check(load_library().bm25x_growing_open(sealed.h, C.byref(self.h)))
+
+    def insert(self, elem_off, elem_term, elem_tf, doc_len=None, doc_fieldnorm=None, payload=None, deleted=None):
+        """Appends documents, arguments as Index.growing (bm25x_growing_insert)."""
+        keep = []
+        g = _growing_docs(keep, elem_off, elem_term, elem_tf, doc_len, doc_fieldnorm, payload, deleted)
+        _check(load_library().bm25x_growing_insert(self.h, C.byref(g)))
+
+    def delete(self, ordinals):
+        o = np.ascontiguousarray(ordinals, dtype=np.uint32)
+        _check(load_library().bm25x_growing_delete(self.h, len(o), _p(o, C.c_uint32)))
+
+    def refresh(self):
+        _check(load_library().bm25x_growing_refresh(self.h))
+
+    def info(self) -> GrowingInfo:
+        out = GrowingInfo()
+        _check(load_library().bm25x_growing_get_info(self.h, C.byref(out)))
+        return out
+
+    def arrays(self):
+        """Test hook: (IndexLayout, IndexDerived) of the segment's current handle (bm25x_growing_get_index)."""
+        lay, der = IndexLayout(), IndexDerived()
+        _check(load_library().bm25x_growing_get_index(self.h, C.byref(lay), C.byref(der)))
+        return lay, der
+
+    def search_batch(self, q_off, q_terms, k, allow=None, allow_growing=None, allow_growing_docs=None,
+                     want_payload=False):
+        """Sealed + growing, the rows of Index.search_batch_growing.  allow_growing covers the ordinals
+        [0, allow_growing_docs) (default: 8 x its length)."""
+        q_off = np.ascontiguousarray(q_off, dtype=np.uint32)
+        q_terms = np.ascontiguousarray(q_terms, dtype=np.uint32)
+        nq, kk = len(q_off) - 1, int(k)
+        out = _result_arrays(nq, max(kk, 1), True, want_payload)
+        al = np.ascontiguousarray(allow, dtype=np.uint8) if allow is not None else None
+        alg = np.ascontiguousarray(allow_growing, dtype=np.uint8) if allow_growing is not None else None
+        n_alg = (8 * len(alg) if allow_growing_docs is None else int(allow_growing_docs)) if alg is not None else 0
+        st = SearchStats()
+        _check(load_library().bm25x_growing_search_batch(
+            self.h, nq, _p(q_off, C.c_uint32), _p(q_terms, C.c_uint32), kk, _p(al, C.c_uint8), _p(alg, C.c_uint8), n_alg,
+            _p(out["doc"], C.c_uint32), _p(out["score"], C.c_float), _p(out["score64"], C.c_double),
+            _p(out["payload"], C.c_uint16), _p(out["n"], C.c_uint32), C.byref(st)))
+        out["stats"] = st
+        return out
+
+    def close(self):
+        if getattr(self, "h", None):
+            load_library().bm25x_growing_close(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 def merge_topk(a, b, doc_base_b, k):

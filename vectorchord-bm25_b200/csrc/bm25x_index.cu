@@ -12,11 +12,13 @@
 #include <string.h>
 
 #include <algorithm>
+#include <chrono>
 #include <memory>
 #include <optional>
 
 #include "bm25x_common.h"
 #include "bm25x_blocks.cuh"
+#include "bm25x_growing.cuh"
 
 static thread_local char g_err[512] = "";
 
@@ -573,6 +575,14 @@ static int handle_open(const char *who, int device, IndexGuard &ix) {
     return BM25X_OK;
 }
 
+// The payload of a document created without one: a synthetic ctid (block hi, block lo, offset) of a 291-tuple page.
+static void synth_ctid(uint32_t g, uint16_t *out) {
+    const uint32_t blkno = g / 291;
+    out[0] = (uint16_t)(blkno >> 16);
+    out[1] = (uint16_t)(blkno & 0xFFFF);
+    out[2] = (uint16_t)(g % 291 + 1);
+}
+
 // A handle with everything but the postings, scoring with the `given` statistics (a shard's or a growing segment's: its
 // segment's) or, when NULL, its own.  Refusals name bm25x_index_create whichever entry point builds.
 static int index_begin(const BuildMeta &m, const Stats *given, int device, IndexGuard &ix) {
@@ -626,13 +636,8 @@ static int index_begin(const BuildMeta &m, const Stats *given, int device, Index
         BM25X_CUDA_TRY(cudaMemcpy(d.payload, m.payload, sizeof(uint16_t) * 3 * (size_t)N, cudaMemcpyHostToDevice));
     } else {
         std::vector<uint16_t> pl((size_t)N * 3);
-        for (uint32_t i = 0; i < N; i++) {  // synthetic ctid: (block hi, block lo, offset) of a 291-tuple page
-            const uint32_t g = m.doc_base + i;  // of the segment's doc id (a shard's local ids start at doc_base)
-            uint32_t blkno = g / 291;
-            pl[(size_t)i * 3 + 0] = (uint16_t)(blkno >> 16);
-            pl[(size_t)i * 3 + 1] = (uint16_t)(blkno & 0xFFFF);
-            pl[(size_t)i * 3 + 2] = (uint16_t)(g % 291 + 1);
-        }
+        // of the segment's doc id (a shard's local ids start at doc_base)
+        for (uint32_t i = 0; i < N; i++) synth_ctid(m.doc_base + i, &pl[(size_t)i * 3]);
         BM25X_CUDA_TRY(cudaMemcpy(d.payload, pl.data(), sizeof(uint16_t) * pl.size(), cudaMemcpyHostToDevice));
     }
     return BM25X_OK;
@@ -1295,14 +1300,22 @@ extern "C" int bm25x_index_create_sharded_from_blocks(const bm25x_blocks *c, uin
 
 // ---- f3: the growing segment (documents inserted since the last seal, search.rs:83-135) as a second, small index that
 // scores with the sealed segment's statistics.  The reference scans these documents one by one per query; here they
-// are inverted once (term-major postings over growing ordinals) so that the same kernels unite them. ----
-extern "C" int bm25x_growing_create(const bm25x_index *sealed, const bm25x_growing_docs *g, bm25x_index **out) {
+// are inverted (term-major postings over growing ordinals) so that the same kernels unite them. ----
+
+// Live postings of a batch of growing documents, term-major: the terms that hold any, ascending, and term[i]'s postings
+// doc / tf[off[i] .. off[i + 1]) with ordinals ascending.
+struct GrowingCsr {
+    std::vector<uint32_t> term;
+    std::vector<uint64_t> off{0};
+    std::vector<uint32_t> doc, tf;
+};
+
+// The checks of growing documents (vector.rs:39-75: keys strictly ascending, tf != 0; tf < 2^24; every merged id below
+// the BM25X_DOC_INF sentinel) and their inversion, for bm25x_growing_create and bm25x_growing_insert alike: the same codes
+// and messages.  Document i becomes ordinal first + i; `first` growing documents already exist.  A deleted document, a
+// BM25X_TERM_MISSING token and a term without sealed postings give no posting.
+static int invert_growing(const bm25x_index *sealed, const bm25x_growing_docs *g, uint32_t first, GrowingCsr &out) {
     const char *who = "bm25x_growing_create";
-    if (!sealed || !g || !out) {
-        bm25x_set_error("%s: null argument", who);
-        return BM25X_ERR_INVALID;
-    }
-    *out = nullptr;
     const uint32_t G = g->n_docs, T = sealed->d.n_terms;
     if (!g->elem_off || (g->elem_off[G] && (!g->elem_term || !g->elem_tf))) {
         bm25x_set_error("%s: empty or malformed corpus", who);
@@ -1313,13 +1326,18 @@ extern "C" int bm25x_growing_create(const bm25x_index *sealed, const bm25x_growi
     if (rc != BM25X_OK) return rc;
     // growing documents come back as sealed n_docs + ordinal (bm25x_search_batch_growing): the sum obeys check_common's
     // bound on n_docs, so that every merged id stays below the BM25X_DOC_INF sentinel
-    if ((uint64_t)sealed->d.n_docs + G > (uint64_t)BM25X_DOC_INF - 1u) {
-        bm25x_set_error("%s: sealed n_docs=%u + growing n_docs=%u exceeds %u documents (doc ids are 32-bit, %u is reserved)",
-                        who, sealed->d.n_docs, G, BM25X_DOC_INF - 1u, BM25X_DOC_INF);
+    if ((uint64_t)sealed->d.n_docs + first + G > (uint64_t)BM25X_DOC_INF - 1u) {
+        bm25x_set_error("%s: sealed n_docs=%u + growing n_docs=%llu exceeds %u documents (doc ids are 32-bit, %u is reserved)",
+                        who, sealed->d.n_docs, (unsigned long long)first + G, BM25X_DOC_INF - 1u, BM25X_DOC_INF);
         return BM25X_ERR_INVALID;
     }
-    // pass 1: validate the documents (vector.rs:39-75: keys strictly ascending, tf != 0) and count per-term postings
-    std::vector<uint64_t> off((size_t)T + 1, 0);
+    // a batch with many postings against the vocabulary is grouped by counting over every term (O(T + P)), a small one by
+    // a sort of its own postings (O(P log P)), so that an insert of one document costs no O(T) pass
+    const uint64_t E = g->elem_off[G] >= g->elem_off[0] ? g->elem_off[G] - g->elem_off[0] : 0;
+    const bool dense = E * 8 >= T;
+    std::vector<uint64_t> cnt(dense ? (size_t)T + 1 : 0, 0);
+    // pass 1: validate the documents and count their live postings (per term when dense)
+    uint64_t P = 0;
     int bad = 0;
     for (uint32_t d = 0; d < G; d++) {
         const uint64_t e0 = g->elem_off[d], e1 = g->elem_off[d + 1];
@@ -1339,7 +1357,8 @@ extern "C" int bm25x_growing_create(const bm25x_index *sealed, const bm25x_growi
             prev = t;
             if (t >= T || sealed->h_df[t] == 0) continue;
             if (f >= (1u << 24)) bad |= 2;
-            off[(size_t)t + 1]++;
+            P++;
+            if (dense) cnt[(size_t)t + 1]++;
         }
     }
     if (bad & 1) {
@@ -1350,39 +1369,349 @@ extern "C" int bm25x_growing_create(const bm25x_index *sealed, const bm25x_growi
         bm25x_set_error("%s: term frequency >= 2^24 is not supported by the packed posting layout", who);
         return BM25X_ERR_UNSUPPORTED;
     }
-    std::vector<uint32_t> df(T);
-    for (uint32_t t = 0; t < T; t++) {
-        df[t] = (uint32_t)off[(size_t)t + 1];
-        off[(size_t)t + 1] += off[t];
-    }
-    const uint64_t P = off[T];
-    // pass 2: invert (documents are visited in ascending ordinal, so every term's list comes out ascending)
-    std::vector<uint32_t> post_doc(P ? P : 1), post_tf(P ? P : 1);
-    {
-        std::vector<uint64_t> cur(off.begin(), off.end() - 1);
-        for (uint32_t d = 0; d < G; d++) {
-            if (g->deleted && g->deleted[d]) continue;
-            for (uint64_t e = g->elem_off[d]; e < g->elem_off[d + 1]; e++) {
-                const uint32_t t = g->elem_term[e];
-                if (t == BM25X_TERM_MISSING || t >= T || sealed->h_df[t] == 0) continue;
-                post_doc[cur[t]] = d;
-                post_tf[cur[t]] = g->elem_tf[e];
-                cur[t]++;
+    // pass 2: invert.  Documents are visited in ascending ordinal and grouped stably, so every list comes out ascending.
+    auto live = [&](uint32_t d, uint64_t e) {
+        const uint32_t t = g->elem_term[e];
+        return !(g->deleted && g->deleted[d]) && t != BM25X_TERM_MISSING && t < T && sealed->h_df[t] != 0;
+    };
+    out = GrowingCsr();
+    out.doc.resize(P);
+    out.tf.resize(P);
+    if (dense) {
+        for (uint32_t t = 0; t < T; t++) cnt[(size_t)t + 1] += cnt[t];
+        std::vector<uint64_t> cur(cnt.begin(), cnt.end() - 1);
+        for (uint32_t d = 0; d < G; d++)
+            for (uint64_t e = g->elem_off[d]; e < g->elem_off[d + 1]; e++)
+                if (live(d, e)) {
+                    const uint64_t p = cur[g->elem_term[e]]++;
+                    out.doc[p] = first + d;
+                    out.tf[p] = g->elem_tf[e];
+                }
+        for (uint32_t t = 0; t < T; t++)
+            if (cnt[(size_t)t + 1] > cnt[t]) {
+                out.term.push_back(t);
+                out.off.push_back(cnt[(size_t)t + 1]);
             }
-        }
+        return BM25X_OK;
     }
+    std::vector<uint64_t> src;  // element index of each live posting, in document order
+    src.reserve(P);
+    for (uint32_t d = 0; d < G; d++)
+        for (uint64_t e = g->elem_off[d]; e < g->elem_off[d + 1]; e++)
+            if (live(d, e)) src.push_back(e);
+    std::vector<uint32_t> owner(P);
+    for (uint32_t d = 0, p = 0; d < G; d++)
+        for (uint64_t e = g->elem_off[d]; e < g->elem_off[d + 1]; e++)
+            if (live(d, e)) owner[p++] = first + d;
+    std::vector<uint32_t> perm(P);
+    for (uint32_t p = 0; p < P; p++) perm[p] = p;
+    std::stable_sort(perm.begin(), perm.end(), [&](uint32_t a, uint32_t b) { return g->elem_term[src[a]] < g->elem_term[src[b]]; });
+    for (uint64_t i = 0; i < P; i++) {
+        const uint32_t t = g->elem_term[src[perm[i]]];
+        if (out.term.empty() || out.term.back() != t) {
+            if (!out.term.empty()) out.off.push_back(i);
+            out.term.push_back(t);
+        }
+        out.doc[i] = owner[perm[i]];
+        out.tf[i] = g->elem_tf[src[perm[i]]];
+    }
+    if (!out.term.empty()) out.off.push_back(P);
+    return BM25X_OK;
+}
+
+// Options of a growing segment's handle: the sealed index's `prune`, over the environment overrides handle_open applied,
+// so that its searches take the sealed handle's kernel paths.
+static void growing_options(bm25x_index *ix, const bm25x_index *sealed) { ix->prune = sealed->prune; }
+
+// The growing segment's scoring statistics: the SEALED segment's (search.rs:66-77), not its own.
+static Stats sealed_stats(const bm25x_index *sealed) {
+    return Stats(sealed->d.n_docs, sealed->sum_len, sealed->avgdl, sealed->h_df.data(), sealed->d.n_terms, sealed->k1,
+                 sealed->b);
+}
+
+extern "C" int bm25x_growing_create(const bm25x_index *sealed, const bm25x_growing_docs *g, bm25x_index **out) {
+    const char *who = "bm25x_growing_create";
+    if (!sealed || !g || !out) {
+        bm25x_set_error("%s: null argument", who);
+        return BM25X_ERR_INVALID;
+    }
+    *out = nullptr;
+    const uint32_t G = g->n_docs, T = sealed->d.n_terms;
+    GrowingCsr csr;
+    int rc = invert_growing(sealed, g, 0, csr);
+    if (rc != BM25X_OK) return rc;
+    std::vector<uint32_t> df(T, 0);
+    std::vector<uint64_t> off((size_t)T + 1, 0);
+    for (size_t i = 0; i < csr.term.size(); i++) df[csr.term[i]] = (uint32_t)(csr.off[i + 1] - csr.off[i]);
+    for (uint32_t t = 0; t < T; t++) off[(size_t)t + 1] = off[t] + df[t];
+    const uint64_t P = off[T];
     BuildMeta m{G, T, g->doc_len, g->payload, sealed->h_keys.empty() ? nullptr : sealed->h_keys.data(), sealed->k1,
                 sealed->b, df.data(), P};
     m.fieldnorm = g->doc_fieldnorm;
-    // search.rs:66-77: scored with the SEALED segment's statistics, not its own
-    const Stats st(sealed->d.n_docs, sealed->sum_len, sealed->avgdl, sealed->h_df.data(), T, sealed->k1, sealed->b);
+    const Stats st = sealed_stats(sealed);
     IndexGuard ix;
     rc = index_begin(m, &st, sealed->device, ix);
-    if (rc == BM25X_OK) rc = upload_csr(ix.get(), who, T, P, off.data(), post_doc.data(), post_tf.data());
+    if (rc == BM25X_OK) rc = upload_csr(ix.get(), who, T, P, off.data(), csr.doc.data(), csr.tf.data());
     if (rc != BM25X_OK) return rc;
-    ix->prune = sealed->prune;
+    growing_options(ix.get(), sealed);
     *out = ix.release();
     return BM25X_OK;
+}
+
+// ---- the mutable growing segment (DESIGN §4.5): the documents on the host as the reference's VectorTuples keep them
+// (norm, payload, deleted bit), their postings in one index handle on the sealed index's device, brought up to date by a
+// refresh ----
+struct bm25x_growing_segment {
+    bm25x_index *sealed;
+    Stats stats;                       // the sealed segment's, computed once
+    mutable std::mutex mu;             // guards everything below; a refresh runs under it
+    int norm_form = -1;                // -1: no insert yet; 1: doc_len; 0: doc_fieldnorm
+    std::vector<uint8_t> fieldnorm;    // per ordinal
+    std::vector<uint32_t> doc_len;     // per ordinal (doc_len form only)
+    std::vector<uint16_t> payload;     // per ordinal x 3: the given ctid, or the synthetic one of the ordinal
+    std::vector<uint8_t> deleted;      // per ordinal
+    uint32_t n_deleted = 0;
+    // postings inserted since the last refresh, one entry per posting: each insert's term-major CSR appended as it came,
+    // so that the postings of one term are in insertion order, hence ordinals ascending
+    std::vector<uint32_t> pend_term, pend_doc, pend_tf;
+    bool pending = false;              // inserts or deletes since the last refresh
+    // the current handle over ordinals [0, n_indexed); a running search keeps its own reference, so that a refresh can
+    // replace it meanwhile and the last holder destroys it
+    std::shared_ptr<bm25x_index> cur;
+
+    explicit bm25x_growing_segment(bm25x_index *s) : sealed(s), stats(sealed_stats(s)) {}
+    uint32_t n_docs() const { return (uint32_t)deleted.size(); }
+};
+
+extern "C" int bm25x_growing_open(bm25x_index *sealed, bm25x_growing_segment **out) {
+    if (!sealed || !out) {
+        bm25x_set_error("bm25x_growing_open: null argument");
+        return BM25X_ERR_INVALID;
+    }
+    *out = nullptr;
+    if (sealed->h_df.size() != sealed->d.n_terms) {
+        bm25x_set_error("bm25x_growing_open: replica not finalized (bm25x_index_finalize_replica)");
+        return BM25X_ERR_INVALID;
+    }
+    *out = new bm25x_growing_segment(sealed);
+    return BM25X_OK;
+}
+
+extern "C" void bm25x_growing_close(bm25x_growing_segment *g) { delete g; }
+
+extern "C" int bm25x_growing_insert(bm25x_growing_segment *g, const bm25x_growing_docs *docs) {
+    if (!g || !docs) {
+        bm25x_set_error("bm25x_growing_insert: null argument");
+        return BM25X_ERR_INVALID;
+    }
+    std::lock_guard<std::mutex> lock(g->mu);
+    const int form = docs->doc_len ? 1 : docs->doc_fieldnorm ? 0 : -1;
+    if (g->norm_form >= 0 && form >= 0 && form != g->norm_form) {
+        bm25x_set_error("bm25x_growing_insert: documents with %s into a segment whose documents carry %s",
+                        form ? "doc_len" : "doc_fieldnorm", form ? "doc_fieldnorm" : "doc_len");
+        return BM25X_ERR_INVALID;
+    }
+    const uint32_t first = g->n_docs(), G = docs->n_docs;
+    GrowingCsr csr;
+    const int rc = invert_growing(g->sealed, docs, first, csr);
+    if (rc != BM25X_OK) return rc;
+    g->norm_form = form;
+    g->fieldnorm.resize((size_t)first + G);
+    if (form) {
+        g->doc_len.insert(g->doc_len.end(), docs->doc_len, docs->doc_len + G);
+        for (uint32_t d = 0; d < G; d++) g->fieldnorm[(size_t)first + d] = bm25x_length_to_fieldnorm(docs->doc_len[d]);
+    } else {
+        std::copy(docs->doc_fieldnorm, docs->doc_fieldnorm + G, g->fieldnorm.begin() + first);
+    }
+    g->payload.resize(((size_t)first + G) * 3);
+    for (uint32_t d = 0; d < G; d++) {
+        uint16_t *p = &g->payload[((size_t)first + d) * 3];
+        if (docs->payload) std::copy(docs->payload + (size_t)d * 3, docs->payload + (size_t)d * 3 + 3, p);
+        else synth_ctid(first + d, p);
+    }
+    g->deleted.resize((size_t)first + G, 0);
+    for (uint32_t d = 0; docs->deleted && d < G; d++)
+        if (docs->deleted[d]) {
+            g->deleted[(size_t)first + d] = 1;
+            g->n_deleted++;
+        }
+    for (size_t i = 0; i < csr.term.size(); i++)
+        g->pend_term.insert(g->pend_term.end(), csr.off[i + 1] - csr.off[i], csr.term[i]);
+    g->pend_doc.insert(g->pend_doc.end(), csr.doc.begin(), csr.doc.end());
+    g->pend_tf.insert(g->pend_tf.end(), csr.tf.begin(), csr.tf.end());
+    g->pending = true;
+    return BM25X_OK;
+}
+
+extern "C" int bm25x_growing_delete(bm25x_growing_segment *g, uint32_t n, const uint32_t *ordinals) {
+    if (!g || (n && !ordinals)) {
+        bm25x_set_error("bm25x_growing_delete: null argument");
+        return BM25X_ERR_INVALID;
+    }
+    std::lock_guard<std::mutex> lock(g->mu);
+    const uint32_t N = g->n_docs();
+    for (uint32_t i = 0; i < n; i++)
+        if (ordinals[i] >= N) {
+            bm25x_set_error("bm25x_growing_delete: ordinal %u (entry %u) >= n_docs=%u", ordinals[i], i, N);
+            return BM25X_ERR_INVALID;
+        }
+    for (uint32_t i = 0; i < n; i++)
+        if (!g->deleted[ordinals[i]]) {
+            g->deleted[ordinals[i]] = 1;
+            g->n_deleted++;
+            g->pending = true;
+        }
+    return BM25X_OK;
+}
+
+// The refresh, under g->mu: the next handle is built beside the current one (which running searches may still read)
+// from its surviving postings and the inserted ones, then replaces it.  On a refusal nothing changes.
+static int growing_refresh_locked(bm25x_growing_segment *g) {
+    const char *who = "bm25x_growing_refresh";
+    if (!g->pending) return BM25X_OK;
+    const bm25x_index *sealed = g->sealed;
+    const uint32_t N = g->n_docs(), T = sealed->d.n_terms;
+    const int device = sealed->device;
+    // the inserted postings as one term-major CSR: a stable counting sort by term keeps each term's ordinals ascending
+    const uint64_t PP = g->pend_term.size();
+    std::vector<uint64_t> pend_off((size_t)T + 1, 0);
+    for (uint64_t p = 0; p < PP; p++) pend_off[(size_t)g->pend_term[p] + 1]++;
+    for (uint32_t t = 0; t < T; t++) pend_off[(size_t)t + 1] += pend_off[t];
+    std::vector<uint32_t> pend_doc(PP), pend_tf(PP);
+    {
+        std::vector<uint64_t> cur(pend_off.begin(), pend_off.end() - 1);
+        for (uint64_t p = 0; p < PP; p++) {
+            const uint64_t at = cur[g->pend_term[p]]++;
+            pend_doc[at] = g->pend_doc[p];
+            pend_tf[at] = g->pend_tf[p];
+        }
+    }
+    std::vector<uint32_t> bits(((size_t)N + 31) / 32, 0);
+    for (uint32_t o = 0; o < N; o++)
+        if (g->deleted[o]) bits[o >> 5] |= 1u << (o & 31);
+    // ---- new df: the survivors of the current lists and of the inserted ones ----
+    Scratch sc(device);
+    sc.e = cudaSetDevice(device);
+    const uint64_t *d_pend_off = sc.up(pend_off.data(), (size_t)T + 1);
+    const uint32_t *d_pend_doc = sc.up(pend_doc.data(), PP), *d_pend_tf = sc.up(pend_tf.data(), PP);
+    const uint32_t *d_del = sc.up(bits.data(), bits.size());
+    uint32_t *d_df = sc.alloc<uint32_t>(T);
+    const bm25x_index *old = g->cur.get();
+    const Posting *old_post = old ? old->d.post : nullptr;
+    const uint64_t *old_off = old ? old->d.post_off : nullptr;
+    const uint32_t *old_df = old ? old->d.df : nullptr;
+    const unsigned grid = (unsigned)std::min<uint64_t>(((uint64_t)T + 7) / 8, (uint64_t)sealed->sm_count * 32ull);
+    if (sc.e == cudaSuccess && T) {
+        k_growing_count<<<grid, 256>>>(T, old_post, old_off, old_df, d_pend_off, d_pend_doc, d_del, d_df);
+        sc.e = cudaGetLastError();
+    }
+    std::vector<uint32_t> df(T);
+    if (sc.e == cudaSuccess && T) sc.e = cudaMemcpy(df.data(), d_df, sizeof(uint32_t) * T, cudaMemcpyDeviceToHost);
+    if (sc.e != cudaSuccess) return cuda_refusal(who, "count", sc.e);
+    uint64_t P = 0;
+    for (uint32_t t = 0; t < T; t++) P += df[t];
+    // ---- the new handle, built as bm25x_growing_create builds one over all N ordinals ----
+    BuildMeta m{N, T, g->norm_form ? g->doc_len.data() : nullptr, g->payload.data(),
+                sealed->h_keys.empty() ? nullptr : sealed->h_keys.data(), sealed->k1, sealed->b, df.data(), P};
+    m.fieldnorm = g->norm_form ? nullptr : g->fieldnorm.data();
+    IndexGuard ix;
+    int rc = index_begin(m, &g->stats, device, ix);
+    if (rc != BM25X_OK) return rc;
+    if (T) {
+        k_growing_splice<<<grid, 256>>>(T, old_post, old_off, old_df, d_pend_off, d_pend_doc, d_pend_tf, d_del,
+                                        ix->d.fieldnorm, ix->d.post_off, ix->d.post);
+        sc.e = cudaGetLastError();
+    }
+    if (sc.e == cudaSuccess) sc.e = cudaDeviceSynchronize();
+    if (sc.e == cudaSuccess) sc.e = index_finish_device(ix.get());
+    if (sc.e != cudaSuccess) return cuda_refusal(who, "splice", sc.e);
+    growing_options(ix.get(), sealed);
+    g->cur.reset(ix.release(), IndexDestroy());
+    std::vector<uint32_t>().swap(g->pend_term);
+    std::vector<uint32_t>().swap(g->pend_doc);
+    std::vector<uint32_t>().swap(g->pend_tf);
+    g->pending = false;
+    return BM25X_OK;
+}
+
+extern "C" int bm25x_growing_refresh(bm25x_growing_segment *g) {
+    if (!g) {
+        bm25x_set_error("bm25x_growing_refresh: null argument");
+        return BM25X_ERR_INVALID;
+    }
+    std::lock_guard<std::mutex> lock(g->mu);
+    return growing_refresh_locked(g);
+}
+
+extern "C" int bm25x_growing_get_info(const bm25x_growing_segment *g, bm25x_growing_info *out) {
+    if (!g || !out) {
+        bm25x_set_error("bm25x_growing_get_info: null argument");
+        return BM25X_ERR_INVALID;
+    }
+    std::lock_guard<std::mutex> lock(g->mu);
+    memset(out, 0, sizeof(*out));
+    out->n_docs = g->n_docs();
+    out->n_deleted = g->n_deleted;
+    out->n_postings = g->cur ? g->cur->d.n_post : 0;
+    out->device_bytes = g->cur ? g->cur->device_bytes : 0;
+    out->pending = g->pending ? 1u : 0u;
+    out->device = g->sealed->device;
+    return BM25X_OK;
+}
+
+extern "C" int bm25x_growing_get_index(const bm25x_growing_segment *g, bm25x_index_layout *layout,
+                                       bm25x_index_derived *derived) {
+    if (!g) {
+        bm25x_set_error("bm25x_growing_get_index: null argument");
+        return BM25X_ERR_INVALID;
+    }
+    std::lock_guard<std::mutex> lock(g->mu);
+    if (!g->cur) {
+        bm25x_set_error("bm25x_growing_get_index: no document has been indexed yet (insert, then refresh)");
+        return BM25X_ERR_INVALID;
+    }
+    int rc = layout ? bm25x_index_get_layout(g->cur.get(), layout) : BM25X_OK;
+    if (rc == BM25X_OK && derived) rc = bm25x_index_get_derived(g->cur.get(), derived);
+    return rc;
+}
+
+extern "C" int bm25x_growing_search_batch(bm25x_growing_segment *g, uint32_t nq, const uint32_t *q_off,
+                                          const uint32_t *q_terms, uint32_t k, const uint8_t *allow_sealed,
+                                          const uint8_t *allow_growing, uint32_t allow_growing_docs, uint32_t *out_doc,
+                                          float *out_score, double *out_score64, uint16_t *out_payload, uint32_t *out_n,
+                                          bm25x_search_stats *stats) {
+    if (!g) {
+        bm25x_set_error("bm25x_growing_search_batch: null argument");
+        return BM25X_ERR_INVALID;
+    }
+    if (k == 0) {
+        bm25x_set_error("number of needed rows is set to 0");  // scanners/default.rs:114-116
+        return BM25X_ERR_LIMIT_ZERO;
+    }
+    const auto t0 = std::chrono::steady_clock::now();
+    std::shared_ptr<bm25x_index> cur;  // this search's state of the segment
+    {
+        std::lock_guard<std::mutex> lock(g->mu);
+        const int rc = growing_refresh_locked(g);
+        if (rc != BM25X_OK) return rc;
+        cur = g->cur;
+    }
+    if (!cur)  // nothing inserted yet: the sealed search alone
+        return bm25x_search_batch(g->sealed, nq, q_off, q_terms, k, allow_sealed, out_doc, out_score, out_score64,
+                                  out_payload, out_n, stats);
+    bm25x_index *ix[2] = {g->sealed, cur.get()};
+    const uint32_t base[2] = {0, g->sealed->d.n_docs};
+    const uint8_t *allow[2] = {allow_sealed, nullptr};
+    std::vector<uint8_t> ag;  // allow_growing over the handle's ordinals: the caller's bits below allow_growing_docs
+    if (allow_growing) {
+        const uint32_t N = cur->d.n_docs, n = std::min(N, allow_growing_docs);
+        ag.assign(((size_t)N + 7) / 8, 0);
+        std::copy(allow_growing, allow_growing + ((size_t)n + 7) / 8, ag.begin());
+        if (n & 7u) ag[n >> 3] &= (uint8_t)((1u << (n & 7u)) - 1u);
+        allow[1] = ag.data();
+    }
+    return bm25x_merged_search("bm25x_growing_search_batch", 2, ix, base, allow, nq, q_off, q_terms, k,
+                               {out_doc, out_score, out_score64, out_payload, out_n}, stats, t0, nullptr);
 }
 
 extern "C" void bm25x_index_destroy(bm25x_index *ix) {

@@ -680,18 +680,6 @@ extern "C" int bm25x_merge_topk(uint32_t nq, uint32_t k, const uint32_t *doc_a, 
     return BM25X_OK;
 }
 
-// Two searches of the same queries (sealed, growing) as one: times and work add up, `queries` is the first one's.
-static void add_work(bm25x_search_stats *out, const bm25x_search_stats &a, const bm25x_search_stats &b) {
-    *out = a;
-    out->kernel_ms += b.kernel_ms;
-    out->h2d_ms += b.h2d_ms;
-    out->d2h_ms += b.d2h_ms;
-    out->postings += b.postings;
-    out->bytes_algo += b.bytes_algo;
-    out->launches += b.launches;
-    out->postings_fetched += b.postings_fetched;
-}
-
 extern "C" int bm25x_search_batch_growing(bm25x_index *sealed, bm25x_index *growing, uint32_t nq, const uint32_t *q_off,
                                           const uint32_t *q_terms, uint32_t k, const uint8_t *allow_sealed,
                                           const uint8_t *allow_growing, uint32_t *out_doc, float *out_score,
@@ -708,29 +696,16 @@ extern "C" int bm25x_search_batch_growing(bm25x_index *sealed, bm25x_index *grow
         bm25x_set_error("number of needed rows is set to 0");
         return BM25X_ERR_LIMIT_ZERO;
     }
-    const size_t slots = (size_t)nq * k;
-    std::vector<uint32_t> doc[2], n[2];
-    std::vector<float> sc[2];
-    std::vector<double> sc64[2];
-    std::vector<uint16_t> pay[2];
-    bm25x_search_stats st[2];
+    // both top-k lists merged on the device: equal scores keep the sealed list first (its ids are all below the base)
     bm25x_index *seg[2] = {sealed, growing};
+    const uint32_t base[2] = {0, sealed->d.n_docs};
     const uint8_t *allow[2] = {allow_sealed, allow_growing};
-    for (int s = 0; s < 2; s++) {
-        doc[s].resize(slots ? slots : 1);
-        n[s].resize(nq ? nq : 1);
-        sc[s].resize(slots ? slots : 1);
-        sc64[s].resize(slots ? slots : 1);
-        if (out_payload) pay[s].resize(slots ? slots * 3 : 1);
-        const int rc = bm25x_search_batch(seg[s], nq, q_off, q_terms, k, allow[s], doc[s].data(), sc[s].data(),
-                                          sc64[s].data(), out_payload ? pay[s].data() : nullptr, n[s].data(), &st[s]);
-        if (rc != BM25X_OK) return rc;
-    }
-    if (stats) add_work(stats, st[0], st[1]);
-    return bm25x_merge_topk(nq, k, doc[0].data(), sc[0].data(), sc64[0].data(), out_payload ? pay[0].data() : nullptr,
-                            n[0].data(), doc[1].data(), sc[1].data(), sc64[1].data(),
-                            out_payload ? pay[1].data() : nullptr, n[1].data(), sealed->d.n_docs, out_doc, out_score,
-                            out_score64, out_payload, out_n);
+    uint32_t live[2] = {0, 0};
+    const int rc = bm25x_merged_search("bm25x_search_batch_growing", 2, seg, base, allow, nq, q_off, q_terms, k,
+                                       {out_doc, out_score, out_score64, out_payload, out_n}, stats,
+                                       std::chrono::steady_clock::now(), live);
+    if (rc == BM25X_OK && stats) stats->queries = live[0];  // the sealed search's: a growing live query is a sealed one
+    return rc;
 }
 
 // ---------------------------------------------------------------------------------------------

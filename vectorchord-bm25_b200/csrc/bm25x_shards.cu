@@ -119,16 +119,110 @@ std::vector<uint8_t> allow_slice(const uint8_t *allow, uint32_t n_docs, uint32_t
 
 }  // namespace
 
+// The rows of S handles over consecutive doc ranges (list s: ids + base[s], base ascending) merged into one top-k list:
+// every handle's batch is prepared and run on its own library stream (the next one's canonicalisation overlaps the
+// kernels of the previous), the merge stream (handle 0's) waits for each run's done event and runs k_merge_shards, then
+// ONE copy brings the merged rows to `host`.  Rows of handles on other devices are copied peer to peer first.  stats:
+// sums over the handles plus the merge launch; h2d_ms = from t0 to the last run enqueued, d2h_ms = merge wait +
+// download; queries = sum of the handles' live queries (live[s] = handle s's, when live != NULL).
+int bm25x_merged_search(const char *who, uint32_t S, bm25x_index *const *handles, const uint32_t *base,
+                        const uint8_t *const *allow, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms,
+                        uint32_t k, const ResultRows &host, bm25x_search_stats *stats,
+                        std::chrono::steady_clock::time_point t0, uint32_t *live) {
+    using clk = std::chrono::steady_clock;
+    bm25x_index *ix0 = handles[0];
+    const int dev0 = ix0->device;
+    cudaStream_t ms = ix0->stream;  // the merge runs behind handle 0's kernels on its library stream
+    std::vector<bm25x_batch *> bs(S, nullptr);
+    std::vector<ResultRows> peer(S);  // rows of handles on other devices, copied to dev0
+    std::vector<cudaEvent_t> evs;
+    ResultRows mo;
+    auto cleanup = [&](int code) {
+        cudaSetDevice(dev0);
+        cudaStreamSynchronize(ms);
+        for (ResultRows &p : peer) p.release(ms);
+        mo.release(ms);
+        for (cudaEvent_t e : evs) cudaEventDestroy(e);
+        for (bm25x_batch *b : bs)
+            if (b) bm25x_batch_destroy(b);
+        return code;
+    };
+    int rc = BM25X_OK;
+    for (uint32_t s = 0; s < S && rc == BM25X_OK; s++) {
+        rc = bm25x_batch_prepare(handles[s], nq, q_off, q_terms, k, allow[s], &bs[s]);
+        if (rc == BM25X_OK) rc = bm25x_batch_run_timed(bs[s]);
+    }
+    if (rc != BM25X_OK) return cleanup(rc);
+    const auto t1 = clk::now();
+    // ---- every handle's rows on dev0: read in place there, copied peer to peer from the other devices ----
+    ShardRows in;
+    memset(&in, 0, sizeof(in));
+    cudaError_t e = cudaSetDevice(dev0);
+    for (uint32_t s = 0; s < S && e == cudaSuccess; s++) {
+        e = cudaStreamWaitEvent(ms, bm25x_batch_done_event(bs[s]), 0);
+        const ResultRows *rows = &bm25x_batch_rows(bs[s]);
+        if (e == cudaSuccess && handles[s]->device != dev0) {
+            e = peer[s].alloc(nq, k, ms);
+            if (e == cudaSuccess) e = rows->copy_to(peer[s], nq, k, ms);
+            rows = &peer[s];
+        }
+        set_shard(in, s, *rows, base[s]);
+    }
+    if (e == cudaSuccess) e = mo.alloc(nq, k, ms);
+    cudaEvent_t m0 = nullptr, m1 = nullptr;
+    if (e == cudaSuccess && stats) {
+        e = cudaEventCreate(&m0);
+        if (e == cudaSuccess) evs.push_back(m0);
+        if (e == cudaSuccess) e = cudaEventCreate(&m1);
+        if (e == cudaSuccess) evs.push_back(m1);
+        if (e == cudaSuccess) e = cudaEventRecord(m0, ms);
+    }
+    if (e != cudaSuccess) {
+        bm25x_set_error("%s: %s", who, cudaGetErrorString(e));
+        return cleanup(e == cudaErrorMemoryAllocation ? BM25X_ERR_OOM : BM25X_ERR_CUDA);
+    }
+    rc = launch_merge(dev0, in, S, nq, k, mo, ms);
+    if (rc != BM25X_OK) return cleanup(rc);
+    if (stats) e = cudaEventRecord(m1, ms);
+    if (e == cudaSuccess) e = mo.copy_to(host, nq, k, ms);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ms);  // after the merge: every handle's kernels have finished too
+    if (e != cudaSuccess) {
+        bm25x_set_error("%s: %s", who, cudaGetErrorString(e));
+        return cleanup(BM25X_ERR_CUDA);
+    }
+    if (stats) {
+        memset(stats, 0, sizeof(*stats));
+        for (uint32_t s = 0; s < S && rc == BM25X_OK; s++) {
+            const uint32_t q0 = stats->queries;
+            rc = bm25x_batch_add_stats(bs[s], stats);
+            if (live) live[s] = stats->queries - q0;
+        }
+        float mms = 0.f;
+        if (rc == BM25X_OK) {
+            cudaSetDevice(dev0);
+            e = cudaEventElapsedTime(&mms, m0, m1);
+            if (e != cudaSuccess) {
+                bm25x_set_error("%s: %s", who, cudaGetErrorString(e));
+                rc = BM25X_ERR_CUDA;
+            }
+        }
+        stats->kernel_ms += mms;  // summed device time of the handles' kernels and the merge, not wall time
+        stats->launches += (uint64_t)nq * S * k ? 1u : 0u;
+        stats->h2d_ms = std::chrono::duration<double, std::milli>(t1 - t0).count();
+        stats->d2h_ms = std::chrono::duration<double, std::milli>(clk::now() - t1).count();
+    }
+    return cleanup(rc);
+}
+
 extern "C" int bm25x_sharded_search_batch(bm25x_sharded_index *sx, uint32_t nq, const uint32_t *q_off,
                                           const uint32_t *q_terms, uint32_t k, const uint8_t *allow, uint32_t *out_doc,
                                           float *out_score, double *out_score64, uint16_t *out_payload, uint32_t *out_n,
                                           bm25x_search_stats *stats) {
-    using clk = std::chrono::steady_clock;
     if (!sx) {
         bm25x_set_error("bm25x_sharded_search_batch: null argument");
         return BM25X_ERR_INVALID;
     }
-    const auto t0 = clk::now();
+    const auto t0 = std::chrono::steady_clock::now();
     // ---- the refusals of bm25x_search_batch: its argument checks, then its canonicalisation slice by slice against the
     // WHOLE segment's df (a query with 65 live terms is refused even when no shard sees more than 64) ----
     if (nq && (!q_off || (!q_terms && q_off[nq] != 0))) {
@@ -156,88 +250,16 @@ extern "C" int bm25x_sharded_search_batch(bm25x_sharded_index *sx, uint32_t nq, 
     }
     if (rc != BM25X_OK) return rc;
     const uint32_t S = sx->n_shards;
-    bm25x_index *ix0 = sx->shards[0];
-    const int dev0 = ix0->device;
-    cudaStream_t ms = ix0->stream;  // the merge runs behind shard 0's kernels on its library stream
-    std::vector<bm25x_batch *> bs(S, nullptr);
-    std::vector<ResultRows> peer(S);  // rows of shards on other devices, copied to dev0
-    std::vector<cudaEvent_t> evs;
-    ResultRows mo;
-    auto cleanup = [&](int code) {
-        cudaSetDevice(dev0);
-        cudaStreamSynchronize(ms);
-        for (ResultRows &p : peer) p.release(ms);
-        mo.release(ms);
-        for (cudaEvent_t e : evs) cudaEventDestroy(e);
-        for (bm25x_batch *b : bs)
-            if (b) bm25x_batch_destroy(b);
-        return code;
-    };
-    // ---- prepare + run shard after shard: the next shard's canonicalisation overlaps the kernels of the previous ----
-    for (uint32_t s = 0; s < S && rc == BM25X_OK; s++) {
-        const uint32_t lo = sx->bounds[s], hi = sx->bounds[s + 1];
-        std::vector<uint8_t> al;
-        if (allow) al = allow_slice(allow, sx->n_docs, lo, hi);
-        rc = bm25x_batch_prepare(sx->shards[s], nq, q_off, q_terms, k, allow ? al.data() : nullptr, &bs[s]);
-        if (rc == BM25X_OK) rc = bm25x_batch_run_timed(bs[s]);
+    std::vector<std::vector<uint8_t>> al(allow ? S : 0);
+    std::vector<const uint8_t *> as(S, nullptr);
+    for (uint32_t s = 0; s < S && allow; s++) {
+        al[s] = allow_slice(allow, sx->n_docs, sx->bounds[s], sx->bounds[s + 1]);
+        as[s] = al[s].data();
     }
-    if (rc != BM25X_OK) return cleanup(rc);
-    const auto t1 = clk::now();
-    // ---- shard rows on dev0: read in place there, copied peer to peer from the other devices ----
-    ShardRows in;
-    memset(&in, 0, sizeof(in));
-    cudaError_t e = cudaSetDevice(dev0);
-    for (uint32_t s = 0; s < S && e == cudaSuccess; s++) {
-        e = cudaStreamWaitEvent(ms, bm25x_batch_done_event(bs[s]), 0);
-        const ResultRows *rows = &bm25x_batch_rows(bs[s]);
-        if (e == cudaSuccess && sx->shards[s]->device != dev0) {
-            e = peer[s].alloc(nq, k, ms);
-            if (e == cudaSuccess) e = rows->copy_to(peer[s], nq, k, ms);
-            rows = &peer[s];
-        }
-        set_shard(in, s, *rows, sx->bounds[s]);
-    }
-    if (e == cudaSuccess) e = mo.alloc(nq, k, ms);
-    cudaEvent_t m0 = nullptr, m1 = nullptr;
-    if (e == cudaSuccess && stats) {
-        e = cudaEventCreate(&m0);
-        if (e == cudaSuccess) evs.push_back(m0);
-        if (e == cudaSuccess) e = cudaEventCreate(&m1);
-        if (e == cudaSuccess) evs.push_back(m1);
-        if (e == cudaSuccess) e = cudaEventRecord(m0, ms);
-    }
-    if (e != cudaSuccess) {
-        bm25x_set_error("bm25x_sharded_search_batch: %s", cudaGetErrorString(e));
-        return cleanup(e == cudaErrorMemoryAllocation ? BM25X_ERR_OOM : BM25X_ERR_CUDA);
-    }
-    rc = launch_merge(dev0, in, S, nq, k, mo, ms);
-    if (rc != BM25X_OK) return cleanup(rc);
-    if (stats) e = cudaEventRecord(m1, ms);
-    if (e == cudaSuccess) e = mo.copy_to({out_doc, out_score, out_score64, out_payload, out_n}, nq, k, ms);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ms);  // after the merge: every shard's kernels have finished too
-    if (e != cudaSuccess) {
-        bm25x_set_error("bm25x_sharded_search_batch: %s", cudaGetErrorString(e));
-        return cleanup(BM25X_ERR_CUDA);
-    }
-    if (stats) {
-        memset(stats, 0, sizeof(*stats));
-        for (uint32_t s = 0; s < S && rc == BM25X_OK; s++) rc = bm25x_batch_add_stats(bs[s], stats);
-        float mms = 0.f;
-        if (rc == BM25X_OK) {
-            cudaSetDevice(dev0);
-            e = cudaEventElapsedTime(&mms, m0, m1);
-            if (e != cudaSuccess) {
-                bm25x_set_error("bm25x_sharded_search_batch: %s", cudaGetErrorString(e));
-                rc = BM25X_ERR_CUDA;
-            }
-        }
-        stats->kernel_ms += mms;  // summed device time of the shards' kernels and the merge, not wall time
-        stats->launches += (uint64_t)nq * S * k ? 1u : 0u;
-        stats->queries = n_live;
-        stats->h2d_ms = std::chrono::duration<double, std::milli>(t1 - t0).count();
-        stats->d2h_ms = std::chrono::duration<double, std::milli>(clk::now() - t1).count();
-    }
-    return cleanup(rc);
+    rc = bm25x_merged_search("bm25x_sharded_search_batch", S, sx->shards.data(), sx->bounds.data(), as.data(), nq, q_off,
+                             q_terms, k, {out_doc, out_score, out_score64, out_payload, out_n}, stats, t0, nullptr);
+    if (rc == BM25X_OK && stats) stats->queries = n_live;
+    return rc;
 }
 
 // ---- test / measurement hook: the merge kernel alone on host rows ----

@@ -222,7 +222,7 @@ void bm25x_batch_destroy(bm25x_batch *batch);
  * sealed documents.  Here the growing documents are inverted once into a second, small index handle that carries
  * the sealed statistics, so the same kernels unite their postings; a query then is two top-k searches + a merge.
  * Doc ids of the growing handle are growing ordinals (insertion order).  The handle is immutable: a segment that takes
- * inserts and deletes in place is bm25x_growing_segment below; `maintain`/seal = build a new sealed index. */
+ * inserts and deletes in place is bm25x_growing_segment below; `maintain`/seal = bm25x_growing_seal on that segment. */
 typedef struct {
     uint32_t n_docs;               /* growing documents, in VectorTuple-chain order */
     const uint32_t *doc_len;       /* [n_docs] exact lengths, or NULL: then doc_fieldnorm */
@@ -300,6 +300,39 @@ int bm25x_growing_search_batch(bm25x_growing_segment *g, uint32_t nq, const uint
  * be NULL); valid until the next refresh or close.  Refused before the first refresh of a non-empty segment. */
 int bm25x_growing_get_index(const bm25x_growing_segment *g, bm25x_index_layout *layout, bm25x_index_derived *derived);
 void bm25x_growing_close(bm25x_growing_segment *g);
+
+/* ---- the seal (`maintain`, crates/bm25/src/maintain.rs:27-311, called from amvacuumcleanup): a NEW sealed index on the
+ * sealed index's device from the sealed documents not marked deleted (ascending old id, relabelled densely) followed by
+ * the segment's surviving documents (ascending ordinal), with fresh statistics (N, Σlen, df, blocks, bounds).  Every
+ * document keeps its stored payload (the synthetic ctid of its OLD id / ordinal when none was given).  Lengths: a
+ * sealed survivor's is the number of postings it holds in the sealed segment (add_element adds 1 per posting,
+ * maintain.rs:356-360), a growing survivor's its doc_len, or in doc_fieldnorm form the saturating Σ tf over all its
+ * elements, BM25X_TERM_MISSING ones included (Document::length, vector.rs:77-83).  Vocabulary: an inserted ordinal >=
+ * n_terms(sealed) becomes a term, BM25X_TERM_MISSING never does.  Keyless index: ordinals are stable, the new n_terms
+ * = max(n_terms(sealed), 1 + the largest ordinal inserted), a term without surviving posting stays with df 0.  Keyed
+ * index: ordinal n_terms(sealed) + i has key new_keys[i]; the new terms are the keys with df > 0, ascending.  The
+ * segment takes its state (refreshing first) under its lock and builds outside it: inserts, deletes and searches go on
+ * meanwhile and the seal covers exactly ordinals [0, n_growing).  The sealed index and the segment are not changed; the
+ * new index has bm25x_index_create's option defaults.  Refusals (nothing changes, *out = NULL): null arguments; no
+ * surviving document (BM25X_ERR_INVALID); new_keys on a keyless index; a new key equal to a sealed or another new key;
+ * on a keyed index an inserted ordinal >= n_terms(sealed) + n_new_keys (the first one is named); a non-NULL map whose
+ * cap is below what the seal writes (n_growing and n_source_terms are set for a retry); a surviving posting with
+ * tf >= 2^24 (BM25X_ERR_UNSUPPORTED); BM25X_ERR_OOM when the new index does not fit. */
+typedef struct {
+    const uint8_t *sealed_deleted; /* in: [ceil(n_docs(sealed)/8)] bit d set = sealed document d is deleted
+                                      (DocumentTuple.deleted, bulkdelete.rs), the bit layout of `allow`; NULL = none */
+    const uint8_t *new_keys;       /* in, keyed sealed index only: [n_new_keys*16] key of token ordinal n_terms(sealed)+i */
+    uint32_t n_new_keys;
+    uint32_t *sealed_map;          /* out [n_docs(sealed)]: new doc id, or 0xFFFFFFFF if deleted; or NULL */
+    uint32_t *growing_map;         /* out [growing_cap]: new doc id of growing ordinal o < n_growing, or 0xFFFFFFFF; or NULL */
+    uint32_t growing_cap;
+    uint32_t *term_map;            /* out [term_cap]: new ordinal of source term t < n_source_terms, or BM25X_TERM_MISSING;
+                                      or NULL */
+    uint32_t term_cap;
+    uint32_t n_growing;            /* out: ordinals [0, n_growing) were folded in */
+    uint32_t n_source_terms;       /* out: keyless: the new n_terms; keyed: n_terms(sealed) + n_new_keys */
+} bm25x_seal_args;
+int bm25x_growing_seal(bm25x_growing_segment *g, bm25x_seal_args *args, bm25x_index **out);
 
 /* ---- document-sharded index: one sealed segment split by document range over one or more GPUs, so that its postings
  * need not fit in one GPU's HBM.  Every shard scores with the WHOLE segment's statistics (N, avgdl, df), so its top-k is

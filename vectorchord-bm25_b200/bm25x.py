@@ -52,6 +52,13 @@ class GrowingInfo(C.Structure):  # bm25x_growing_info
                 ("device_bytes", C.c_uint64), ("pending", C.c_uint32), ("device", C.c_int)]
 
 
+class SealArgs(C.Structure):  # bm25x_seal_args
+    _fields_ = [("sealed_deleted", C.POINTER(C.c_uint8)), ("new_keys", C.POINTER(C.c_uint8)), ("n_new_keys", C.c_uint32),
+                ("sealed_map", C.POINTER(C.c_uint32)), ("growing_map", C.POINTER(C.c_uint32)), ("growing_cap", C.c_uint32),
+                ("term_map", C.POINTER(C.c_uint32)), ("term_cap", C.c_uint32), ("n_growing", C.c_uint32),
+                ("n_source_terms", C.c_uint32)]
+
+
 class IndexInfo(C.Structure):
     _fields_ = [("n_docs", C.c_uint32), ("n_terms", C.c_uint32), ("n_postings", C.c_uint64),
                 ("sum_doc_len", C.c_uint64), ("avgdl", C.c_double), ("k1", C.c_double), ("b", C.c_double),
@@ -139,6 +146,7 @@ def load_library():
     L.bm25x_growing_get_index.argtypes = [vp, C.POINTER(IndexLayout), C.POINTER(IndexDerived)]
     L.bm25x_growing_close.argtypes = [vp]
     L.bm25x_growing_close.restype = None
+    L.bm25x_growing_seal.argtypes = [vp, C.POINTER(SealArgs), C.POINTER(vp)]
     L.bm25x_merge_topk.argtypes = [C.c_uint32, C.c_uint32, u32p, f32p, f64p, u16p, u32p, u32p, f32p, f64p, u16p, u32p,
                                    C.c_uint32, u32p, f32p, f64p, u16p, u32p]
     L.bm25x_index_destroy.argtypes = [vp]
@@ -597,6 +605,37 @@ class GrowingSegment:
             _p(out["payload"], C.c_uint16), _p(out["n"], C.c_uint32), C.byref(st)))
         out["stats"] = st
         return out
+
+    def seal(self, sealed_deleted=None, new_keys=None):
+        """`maintain` (bm25x_growing_seal): a new sealed Index of the surviving sealed documents (ascending old id) and
+        the surviving growing ones (ascending ordinal).  sealed_deleted: bitmap over sealed ids, the layout of `allow`;
+        new_keys: keyed index only, [n, 16] keys of the token ordinals sealed.n_terms + i.  Returns (index, sealed_map,
+        growing_map, term_map): new id of each sealed id / growing ordinal (0xFFFFFFFF: deleted) and new ordinal of each
+        source term (TERM_MISSING: vanished); growing_map covers the ordinals the seal took, which may be fewer than
+        info().n_docs when other threads insert meanwhile.  The segment and this sealed index stay as they are."""
+        L = load_library()
+        dele = np.ascontiguousarray(sealed_deleted, dtype=np.uint8) if sealed_deleted is not None else None
+        keys = np.ascontiguousarray(new_keys, dtype=np.uint8).reshape(-1, 16) if new_keys is not None else None
+        n_keys = len(keys) if keys is not None else 0
+        smap = np.empty(self.sealed.n_docs, np.uint32)
+        g_cap, t_cap = int(self.info().n_docs), self.sealed.n_terms + n_keys
+        while True:  # a cap below what the seal writes is refused with the sizes it needs (inserts may run meanwhile)
+            gmap, tmap = np.empty(max(g_cap, 1), np.uint32), np.empty(max(t_cap, 1), np.uint32)
+            a = SealArgs()
+            a.sealed_deleted, a.new_keys, a.n_new_keys = _p(dele, C.c_uint8), _p(keys, C.c_uint8), n_keys
+            a.sealed_map = _p(smap, C.c_uint32)
+            a.growing_map, a.growing_cap = _p(gmap, C.c_uint32), g_cap
+            a.term_map, a.term_cap = _p(tmap, C.c_uint32), t_cap
+            h = C.c_void_p()
+            rc = L.bm25x_growing_seal(self.h, C.byref(a), C.byref(h))
+            if rc != 0 and (a.n_growing > g_cap or a.n_source_terms > t_cap):
+                g_cap, t_cap = max(g_cap, int(a.n_growing)), max(t_cap, int(a.n_source_terms))
+                continue
+            _check(rc)
+            info = IndexInfo()
+            _check(L.bm25x_index_get_info(h, C.byref(info)))
+            ix = Index._adopt(h, info.n_docs, info.n_terms)
+            return ix, smap, gmap[:a.n_growing].copy(), tmap[:a.n_source_terms].copy()
 
     def close(self):
         if getattr(self, "h", None):

@@ -15,10 +15,12 @@
 #include <chrono>
 #include <memory>
 #include <optional>
+#include <unordered_set>
 
 #include "bm25x_common.h"
 #include "bm25x_blocks.cuh"
 #include "bm25x_growing.cuh"
+#include "bm25x_seal.cuh"
 
 static thread_local char g_err[512] = "";
 
@@ -1475,6 +1477,15 @@ struct bm25x_growing_segment {
     // so that the postings of one term are in insertion order, hence ordinals ascending
     std::vector<uint32_t> pend_term, pend_doc, pend_tf;
     bool pending = false;              // inserts or deletes since the last refresh
+    // what only the seal reads (bm25x_growing_seal): the "dormant" postings the handle never holds (terms >= the sealed
+    // n_terms, terms without sealed postings) of every document not inserted deleted, as (term, ordinal, tf) appended per
+    // insert; in doc_fieldnorm form each ordinal's saturating Σ tf over all its elements (Document::length,
+    // vector.rs:77-83); the inserted ordinals >= the sealed n_terms, each once, in the order they first came
+    std::vector<uint32_t> dorm_term, dorm_doc, dorm_tf;
+    std::vector<uint32_t> sum_tf;
+    std::vector<uint32_t> new_terms;
+    std::unordered_set<uint32_t> new_seen;
+    uint32_t term_end = 0;             // 1 + the largest ordinal in new_terms (0: none)
     // the current handle over ordinals [0, n_indexed); a running search keeps its own reference, so that a refresh can
     // replace it meanwhile and the last holder destroys it
     std::shared_ptr<bm25x_index> cur;
@@ -1539,6 +1550,28 @@ extern "C" int bm25x_growing_insert(bm25x_growing_segment *g, const bm25x_growin
         g->pend_term.insert(g->pend_term.end(), csr.off[i + 1] - csr.off[i], csr.term[i]);
     g->pend_doc.insert(g->pend_doc.end(), csr.doc.begin(), csr.doc.end());
     g->pend_tf.insert(g->pend_tf.end(), csr.tf.begin(), csr.tf.end());
+    // the seal's share: dormant postings, Σ tf (doc_fieldnorm form), new ordinals
+    const bm25x_index *sealed = g->sealed;
+    const uint32_t T = sealed->d.n_terms;
+    for (uint32_t d = 0; d < G; d++) {
+        const bool live = !(docs->deleted && docs->deleted[d]);
+        uint64_t sum = 0;
+        for (uint64_t e = docs->elem_off[d]; e < docs->elem_off[d + 1]; e++) {
+            const uint32_t t = docs->elem_term[e];
+            sum += docs->elem_tf[e];
+            if (t == BM25X_TERM_MISSING) continue;
+            if (t >= T && g->new_seen.insert(t).second) {
+                g->new_terms.push_back(t);
+                g->term_end = std::max(g->term_end, t + 1);
+            }
+            if (live && (t >= T || sealed->h_df[t] == 0)) {
+                g->dorm_term.push_back(t);
+                g->dorm_doc.push_back(first + d);
+                g->dorm_tf.push_back(docs->elem_tf[e]);
+            }
+        }
+        if (!form) g->sum_tf.push_back((uint32_t)std::min<uint64_t>(sum, 0xFFFFFFFFu));
+    }
     g->pending = true;
     return BM25X_OK;
 }
@@ -1712,6 +1745,222 @@ extern "C" int bm25x_growing_search_batch(bm25x_growing_segment *g, uint32_t nq,
     }
     return bm25x_merged_search("bm25x_growing_search_batch", 2, ix, base, allow, nq, q_off, q_terms, k,
                                {out_doc, out_score, out_score64, out_payload, out_n}, stats, t0, nullptr);
+}
+
+// ---- the seal (`maintain`, maintain.rs:27-311; DESIGN §4.5): a new sealed index from the sealed survivors and the
+// segment's, built on the device from the arrays already there ----
+
+// What the seal reads of the segment, copied under its lock right after a refresh.
+struct SealSnapshot {
+    uint32_t n = 0;                    // ordinals
+    std::shared_ptr<bm25x_index> cur;  // the refreshed handle over them (NULL: none)
+    std::vector<uint8_t> deleted;
+    std::vector<uint32_t> len;         // rule 4 length per ordinal: doc_len, or Σ tf in doc_fieldnorm form
+    std::vector<uint16_t> payload;
+    std::vector<uint32_t> dorm_term, dorm_doc, dorm_tf;
+};
+
+extern "C" int bm25x_growing_seal(bm25x_growing_segment *g, bm25x_seal_args *a, bm25x_index **out) {
+    const char *who = "bm25x_growing_seal";
+    if (!g || !a || !out || (a->n_new_keys && !a->new_keys)) {
+        bm25x_set_error("%s: null argument", who);
+        return BM25X_ERR_INVALID;
+    }
+    *out = nullptr;
+    const bm25x_index *sealed = g->sealed;
+    const uint32_t NS = sealed->d.n_docs, T = sealed->d.n_terms, K = a->n_new_keys;
+    const int device = sealed->device;
+    const bool keyed = !sealed->h_keys.empty();
+    // ---- the new keys: each unlike every sealed key and every other new key ----
+    if (a->new_keys && !keyed) {
+        bm25x_set_error("%s: new_keys given, but the sealed index was created without term keys", who);
+        return BM25X_ERR_INVALID;
+    }
+    const uint8_t *skeys = sealed->h_keys.data();
+    auto key_of = [&](uint32_t t) { return t < T ? skeys + (size_t)t * 16 : a->new_keys + (size_t)(t - T) * 16; };
+    auto key_less = [&](uint32_t x, uint32_t y) { return memcmp(key_of(x), key_of(y), 16) < 0; };
+    if (K) {
+        std::vector<uint32_t> order(K);
+        for (uint32_t i = 0; i < K; i++) order[i] = T + i;
+        std::sort(order.begin(), order.end(), key_less);
+        for (uint32_t i = 1; i < K; i++)
+            if (memcmp(key_of(order[i - 1]), key_of(order[i]), 16) == 0) {
+                const uint32_t x = std::min(order[i - 1], order[i]) - T, y = std::max(order[i - 1], order[i]) - T;
+                bm25x_set_error("%s: new key %u equals new key %u", who, x, y);
+                return BM25X_ERR_INVALID;
+            }
+        for (uint32_t i = 0; i < K; i++) {  // address_tokens::read over the sealed keys, as bm25x_lookup_terms
+            uint32_t lo = 0, hi = T;
+            while (lo < hi) {
+                const uint32_t mid = (lo + hi) >> 1;
+                if (memcmp(skeys + (size_t)mid * 16, key_of(T + i), 16) < 0) lo = mid + 1;
+                else hi = mid;
+            }
+            if (lo < T && memcmp(skeys + (size_t)lo * 16, key_of(T + i), 16) == 0) {
+                bm25x_set_error("%s: new key %u equals the key of sealed term %u", who, i, lo);
+                return BM25X_ERR_INVALID;
+            }
+        }
+    }
+    // ---- rule 1: the sealed survivors in ascending old id ----
+    std::vector<uint32_t> smap(NS);
+    uint32_t ns_keep = 0;
+    for (uint32_t d = 0; d < NS; d++)
+        smap[d] = a->sealed_deleted && ((a->sealed_deleted[d >> 3] >> (d & 7u)) & 1u) ? BM25X_DOC_INF : ns_keep++;
+    // ---- the snapshot: every refusal that depends on the segment first, then a refresh and a copy ----
+    SealSnapshot s;
+    uint32_t n_src;
+    {
+        std::lock_guard<std::mutex> lock(g->mu);
+        const uint32_t NG = g->n_docs();
+        n_src = keyed ? T + K : std::max(T, g->term_end);
+        if (keyed)
+            for (uint32_t t : g->new_terms)
+                if (t >= T + K) {
+                    bm25x_set_error("%s: inserted term ordinal %u >= n_terms(sealed)=%u + n_new_keys=%u (it has no key)", who,
+                                    t, T, K);
+                    return BM25X_ERR_INVALID;
+                }
+        if ((a->growing_map && NG > a->growing_cap) || (a->term_map && n_src > a->term_cap)) {
+            a->n_growing = NG;
+            a->n_source_terms = n_src;
+            bm25x_set_error("%s: growing_cap=%u / term_cap=%u below n_growing=%u / n_source_terms=%u", who, a->growing_cap,
+                            a->term_cap, NG, n_src);
+            return BM25X_ERR_INVALID;
+        }
+        if (ns_keep == 0 && NG == g->n_deleted) {
+            bm25x_set_error("%s: no document survives (every sealed and growing document is deleted)", who);
+            return BM25X_ERR_INVALID;
+        }
+        for (size_t i = 0; i < g->dorm_tf.size(); i++)
+            if (g->dorm_tf[i] >= (1u << 24) && !g->deleted[g->dorm_doc[i]]) {
+                bm25x_set_error("%s: term frequency >= 2^24 is not supported by the packed posting layout", who);
+                return BM25X_ERR_UNSUPPORTED;
+            }
+        const int rc = growing_refresh_locked(g);
+        if (rc != BM25X_OK) return rc;
+        s.n = NG;
+        s.cur = g->cur;
+        s.deleted = g->deleted;
+        s.len = g->norm_form == 1 ? g->doc_len : g->sum_tf;
+        s.payload = g->payload;
+        s.dorm_term = g->dorm_term;
+        s.dorm_doc = g->dorm_doc;
+        s.dorm_tf = g->dorm_tf;
+    }
+    // ---- rule 1: the growing survivors after the sealed ones, in ascending ordinal ----
+    const uint32_t NG = s.n;
+    std::vector<uint32_t> gmap(NG);
+    uint32_t N = ns_keep;
+    for (uint32_t o = 0; o < NG; o++) gmap[o] = s.deleted[o] ? BM25X_DOC_INF : N++;
+    // the dormant postings as a CSR over the source terms: a stable counting sort keeps each term's ordinals ascending
+    const uint64_t PD = s.dorm_term.size();
+    std::vector<uint64_t> dorm_off((size_t)n_src + 1, 0);
+    for (uint64_t p = 0; p < PD; p++) dorm_off[(size_t)s.dorm_term[p] + 1]++;
+    for (uint32_t t = 0; t < n_src; t++) dorm_off[(size_t)t + 1] += dorm_off[t];
+    std::vector<uint32_t> dorm_doc(PD), dorm_tf(PD);
+    {
+        std::vector<uint64_t> cur(dorm_off.begin(), dorm_off.end() - 1);
+        for (uint64_t p = 0; p < PD; p++) {
+            const uint64_t at = cur[s.dorm_term[p]]++;
+            dorm_doc[at] = s.dorm_doc[p];
+            dorm_tf[at] = s.dorm_tf[p];
+        }
+    }
+    std::vector<uint32_t> sbits(((size_t)NS + 31) / 32, 0), gbits(((size_t)NG + 31) / 32, 0);
+    if (a->sealed_deleted) memcpy(sbits.data(), a->sealed_deleted, ((size_t)NS + 7) / 8);  // little-endian: bit d of word d >> 5
+    for (uint32_t o = 0; o < NG; o++)
+        if (s.deleted[o]) gbits[o >> 5] |= 1u << (o & 31);
+    // ---- rule 3 lengths and rule 5 df on the device ----
+    Scratch sc(device);
+    sc.e = cudaSetDevice(device);
+    const uint32_t *d_sdel = sc.up(sbits.data(), sbits.size()), *d_gdel = sc.up(gbits.data(), gbits.size());
+    const uint32_t *d_smap = sc.up(smap.data(), NS), *d_gmap = sc.up(gmap.data(), NG);
+    const uint64_t *d_dorm_off = sc.up(dorm_off.data(), (size_t)n_src + 1);
+    const uint32_t *d_dorm_doc = sc.up(dorm_doc.data(), PD), *d_dorm_tf = sc.up(dorm_tf.data(), PD);
+    uint32_t *d_cnt = sc.alloc<uint32_t>(NS), *d_df = sc.alloc<uint32_t>(n_src);
+    const bm25x_index *gh = s.cur.get();
+    const Posting *g_post = gh ? gh->d.post : nullptr;
+    const uint64_t *g_off = gh ? gh->d.post_off : nullptr;
+    const uint32_t *g_df = gh ? gh->d.df : nullptr;
+    const DeviceIndex &sd = sealed->d;
+    auto grid = [&](uint32_t n) {
+        return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(((uint64_t)n + 7) / 8, (uint64_t)sealed->sm_count * 32ull));
+    };
+    if (sc.e == cudaSuccess) sc.e = cudaMemset(d_cnt, 0, sizeof(uint32_t) * (size_t)NS);
+    if (sc.e == cudaSuccess && T) {
+        k_seal_doc_postings<<<grid(T), 256>>>(T, sd.pdoc, sd.post_off, sd.df, d_sdel, d_cnt);
+        sc.e = cudaGetLastError();
+    }
+    if (sc.e == cudaSuccess && n_src) {
+        k_seal_df<<<grid(n_src), 256>>>(n_src, T, sd.pdoc, sd.post_off, sd.df, d_sdel, g_post, g_off, g_df, d_gdel,
+                                        d_dorm_off, d_dorm_doc, d_df);
+        sc.e = cudaGetLastError();
+    }
+    std::vector<uint32_t> cnt(NS), df_src(n_src);
+    std::vector<uint16_t> spay((size_t)NS * 3);
+    if (sc.e == cudaSuccess) sc.e = cudaMemcpy(cnt.data(), d_cnt, sizeof(uint32_t) * (size_t)NS, cudaMemcpyDeviceToHost);
+    if (sc.e == cudaSuccess && n_src) sc.e = cudaMemcpy(df_src.data(), d_df, sizeof(uint32_t) * n_src, cudaMemcpyDeviceToHost);
+    if (sc.e == cudaSuccess)
+        sc.e = cudaMemcpy(spay.data(), sd.payload, sizeof(uint16_t) * 3 * (size_t)NS, cudaMemcpyDeviceToHost);
+    if (sc.e != cudaSuccess) return cuda_refusal(who, "count", sc.e);
+    // ---- rules 2-4: per new document its length and its stored payload ----
+    std::vector<uint32_t> len(N);
+    std::vector<uint16_t> pay((size_t)N * 3);
+#pragma omp parallel for schedule(static) num_threads(bm25x_host_threads(0))
+    for (uint32_t d = 0; d < NS; d++)
+        if (smap[d] != BM25X_DOC_INF) {
+            len[smap[d]] = cnt[d];
+            memcpy(&pay[(size_t)smap[d] * 3], &spay[(size_t)d * 3], 6);
+        }
+    for (uint32_t o = 0; o < NG; o++)
+        if (gmap[o] != BM25X_DOC_INF) {
+            len[gmap[o]] = s.len[o];
+            memcpy(&pay[(size_t)gmap[o] * 3], &s.payload[(size_t)o * 3], 6);
+        }
+    // ---- rule 6: the vocabulary ----
+    std::vector<uint32_t> src_of;  // new term -> source term
+    if (keyed) {
+        for (uint32_t t = 0; t < n_src; t++)
+            if (df_src[t]) src_of.push_back(t);
+        std::sort(src_of.begin(), src_of.end(), key_less);
+    } else {
+        src_of.resize(n_src);
+        for (uint32_t t = 0; t < n_src; t++) src_of[t] = t;
+    }
+    const uint32_t TN = (uint32_t)src_of.size();
+    std::vector<uint32_t> df(TN), tmap(n_src, BM25X_TERM_MISSING);
+    std::vector<uint8_t> keys(keyed ? (size_t)TN * 16 : 0);
+    uint64_t P = 0;
+    for (uint32_t j = 0; j < TN; j++) {
+        df[j] = df_src[src_of[j]];
+        tmap[src_of[j]] = j;
+        P += df[j];
+        if (keyed) memcpy(&keys[(size_t)j * 16], key_of(src_of[j]), 16);
+    }
+    // ---- rule 5 and 7: the new handle with its own statistics, the postings spliced into it, then what every index
+    // derives from them ----
+    BuildMeta m{N, TN, len.data(), pay.data(), keyed ? keys.data() : nullptr, sealed->k1, sealed->b, df.data(), P};
+    IndexGuard ix;
+    int rc = index_begin(m, nullptr, device, ix);
+    if (rc != BM25X_OK) return rc;
+    const uint32_t *d_src_of = sc.up(src_of.data(), TN);
+    if (sc.e == cudaSuccess && TN) {
+        k_seal_splice<<<grid(TN), 256>>>(TN, d_src_of, T, sd.post, sd.post_off, sd.df, d_sdel, d_smap, g_post, g_off, g_df,
+                                         d_gdel, d_gmap, d_dorm_off, d_dorm_doc, d_dorm_tf, ix->d.fieldnorm, ix->d.post_off,
+                                         ix->d.post);
+        sc.e = cudaGetLastError();
+    }
+    if (sc.e == cudaSuccess) sc.e = cudaDeviceSynchronize();
+    if (sc.e == cudaSuccess) sc.e = index_finish_device(ix.get());
+    if (sc.e != cudaSuccess) return cuda_refusal(who, "splice", sc.e);
+    a->n_growing = NG;
+    a->n_source_terms = n_src;
+    if (a->sealed_map) std::copy(smap.begin(), smap.end(), a->sealed_map);
+    if (a->growing_map) std::copy(gmap.begin(), gmap.end(), a->growing_map);
+    if (a->term_map) std::copy(tmap.begin(), tmap.end(), a->term_map);
+    *out = ix.release();
+    return BM25X_OK;
 }
 
 extern "C" void bm25x_index_destroy(bm25x_index *ix) {

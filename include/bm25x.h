@@ -271,7 +271,9 @@ typedef struct {
     uint32_t pending;       /* 1: inserts or deletes since the last refresh */
     int device;             /* the sealed index's */
 } bm25x_growing_info;
-/* An empty segment on the sealed index's device, scoring with its statistics. */
+/* An empty segment on the sealed index's device, scoring with its statistics.  Any finalized handle serves; a finalized
+ * replica holds no term keys (they do not travel with the 13 arrays), so a keyed index's replica seals as a keyless one:
+ * stable ordinals, new_keys refused. */
 int bm25x_growing_open(bm25x_index *sealed, bm25x_growing_segment **out);
 /* Appends docs as ordinals n_docs .. n_docs + docs->n_docs - 1 (deleted flags included).  Refuses what
  * bm25x_growing_create refuses, with its codes and messages (terms not ascending, tf = 0, tf >= 2^24, sealed n_docs +

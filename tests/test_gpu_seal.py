@@ -38,16 +38,18 @@ def m():
 class World:
     """A sealed index and what the restatement needs of it."""
 
-    def __init__(self, m, n_docs, off, doc, tf, doc_len, payload, keys, ix=None):
+    def __init__(self, m, n_docs, off, doc, tf, doc_len, payload, keys, ix=None, k1=1.2, b=0.75):
         self.n_docs, self.n_terms = int(n_docs), len(off) - 1
         self.off, self.doc, self.tf, self.doc_len, self.payload, self.keys = off, doc, tf, doc_len, payload, keys
-        self.ix = ix or m.Index(n_docs, doc_len, self.n_terms, off, doc, tf, payload=payload, term_keys=keys)
+        self.k1, self.b = k1, b
+        self.ix = ix or m.Index(n_docs, doc_len, self.n_terms, off, doc, tf, k1=k1, b=b, payload=payload, term_keys=keys)
         self.df = np.diff(off.astype(np.int64))
+        self.sum_len = int(np.asarray(doc_len, np.uint64).sum())   # what a growing segment's avgdl comes from
 
     @staticmethod
-    def from_restated(m, r, ix):
+    def from_restated(m, r, ix, k1=1.2, b=0.75):
         """The restated corpus r, whose index is the seal's result ix."""
-        return World(m, r.n_docs, r.post_off, r.post_doc, r.post_tf, r.doc_len, r.payload, r.term_keys, ix)
+        return World(m, r.n_docs, r.post_off, r.post_doc, r.post_tf, r.doc_len, r.payload, r.term_keys, ix, k1, b)
 
 
 def _keys(rng, n, taken=()):
@@ -61,9 +63,9 @@ def _keys(rng, n, taken=()):
     return np.array(out, np.uint8).reshape(-1, 16)
 
 
-def _sealed_world(m, orc, rng, n_docs, T, keyed, with_payload):
-    """Zipf-like documents over T terms, a few terms left without postings, a document with one term at tf 3 and an
-    empty one."""
+def _sealed_docs(rng, n_docs, T):
+    """Zipf-like documents ({term: tf}) over T terms, a few terms left without postings (returned, sorted), a document
+    with one term at tf 3 and an empty one."""
     p = 1.0 / np.arange(1, T + 1)
     p /= p.sum()
     dead = set(rng.choice(np.arange(T // 2, T), size=4, replace=False).tolist())
@@ -74,11 +76,17 @@ def _sealed_world(m, orc, rng, n_docs, T, keyed, with_payload):
         docs.append({int(t): int(rng.integers(1, 6)) for t in terms})
     docs[1] = {2: 3}
     docs[2] = {}
+    return docs, sorted(dead)
+
+
+def _sealed_world(m, orc, rng, n_docs, T, keyed, with_payload):
+    """An index over _sealed_docs, its lengths a few tokens above Σ tf."""
+    docs, dead = _sealed_docs(rng, n_docs, T)
     c = orc.Corpus.from_docs(docs, n_terms=T)
     doc_len = c.doc_len + rng.integers(0, 5, size=n_docs).astype(np.uint32)
     payload = rng.integers(0, 65536, size=(n_docs, 3)).astype(np.uint16) if with_payload else None
     keys = np.array(sorted(_keys(rng, T).tolist()), np.uint8) if keyed else None
-    return World(m, n_docs, c.post_off, c.post_doc, c.post_tf, doc_len, payload, keys), sorted(dead)
+    return World(m, n_docs, c.post_off, c.post_doc, c.post_tf, doc_len, payload, keys), dead
 
 
 class Docs:
@@ -153,18 +161,19 @@ def _pack(bits):
     return np.packbits(np.asarray(bits, np.uint8), bitorder="little")
 
 
-def _check_result(m, orc, got_ix, maps, r, what):
-    """The sealed result against bm25x_index_create over the restated corpus and against the CPU restatement."""
+def _check_result(m, orc, got_ix, maps, r, what, k1=1.2, b=0.75):
+    """The sealed result against bm25x_index_create over the restated corpus (built with k1, b) and against the CPU
+    restatement, which is returned."""
     smap, gmap, tmap = maps
     assert np.array_equal(smap, r.sealed_map), f"{what}: sealed_map"
     assert np.array_equal(gmap, r.growing_map), f"{what}: growing_map"
     assert np.array_equal(tmap, r.term_map), f"{what}: term_map"
-    ref = m.Index(r.n_docs, r.doc_len, r.n_terms, r.post_off, r.post_doc, r.post_tf, payload=r.payload,
+    ref = m.Index(r.n_docs, r.doc_len, r.n_terms, r.post_off, r.post_doc, r.post_tf, k1=k1, b=b, payload=r.payload,
                   term_keys=r.term_keys)
     try:
         lay, der = got_ix.layout(), got_ix.derived()
         got = read_back(lay, der)
-        rs = restate(orc, r.n_docs, r.post_off, r.post_doc, r.post_tf, 1.2, 0.75, doc_len=r.doc_len, payload=r.payload)
+        rs = restate(orc, r.n_docs, r.post_off, r.post_doc, r.post_tf, k1, b, doc_len=r.doc_len, payload=r.payload)
         assert_matches(got, lay, der, rs, what)
         want = read_back(ref.layout(), ref.derived())
         for key in want:
@@ -176,23 +185,25 @@ def _check_result(m, orc, got_ix, maps, r, what):
             assert getattr(a, f) == getattr(b, f), f"{what}: info.{f}"
         if r.term_keys is not None and r.n_terms:
             assert np.array_equal(got_ix.lookup_terms(r.term_keys), np.arange(r.n_terms, dtype=np.uint32))
+        return rs
     finally:
         ref.close()
 
 
-def _check_searches(orc, got_ix, r, rng, what):
-    """Searches on the result against the oracle's exhaustive scorer over the restated corpus, on every kernel path."""
+def _check_searches(orc, got_ix, r, rng, what, k1=1.2, b=0.75, ks=KS, modes=MODES):
+    """Searches on the result against the oracle's exhaustive scorer (k1, b) over the restated corpus, at every limit of
+    `ks` under every option set of `modes`."""
     df = np.diff(r.post_off.astype(np.int64))
     if not (df > 0).any():
         return
-    oix = orc.OracleIndex(orc.Corpus(r.n_docs, r.doc_len, r.n_terms, r.post_off, r.post_doc, r.post_tf))
-    po = _PrefixOracle(oix, max(KS))
+    oix = orc.OracleIndex(orc.Corpus(r.n_docs, r.doc_len, r.n_terms, r.post_off, r.post_doc, r.post_tf, k1, b))
+    po = _PrefixOracle(oix, max(ks))
     q_off, q_terms = _live_queries(rng, df, [1, 2, 2, 3, 3, 4, 5, 8, 12, 40][: 10 if (df > 0).sum() >= 40 else 6])
     try:
-        for mode, opts in MODES.items():
+        for mode, opts in modes.items():
             for name, v in {**DEFAULTS, **opts}.items():
                 got_ix.set_option(name, v)
-            for k in KS:
+            for k in ks:
                 _compare(got_ix.search_batch(q_off, q_terms, k), po, q_off, q_terms, k, what=f"{what} {mode} k={k}")
     finally:
         for name, v in DEFAULTS.items():

@@ -1,5 +1,9 @@
-"""GPU: the f32 filter's safety margin kEps (bm25x_search_ring.cuh refresh_filter) is load-bearing on every kernel path:
-a kernel built with kEps = 0 fails every case of this module.
+"""GPU: the f32 filter's safety margin kEps (bm25x_search_ring.cuh refresh_filter) is load-bearing on the kernel paths
+below — the plain 8-, 16- and 32-term classes, a two-pass query, a dense window and the HBM pool, the seeded 4-term class
+(no hit list) and the two-phase launches, all at k = 10 but the HBM pool: a kernel built with kEps = 0 fails every case
+of this module.  test_gpu_margin_paths.py covers the other instantiations that score candidates (the seeded hit list,
+the seeded 2- and 8-term classes, dense windows in doc-id-only rings, the hand-back launch, the 256- and 2048-entry
+shared pools, dense windows in the 16- and 32-term classes).
 
 Each case is a corpus built by util_filter.near_threshold_case: document A is the k-th entry once the pool has been cut
 with A and the better documents in it (whichever order a kernel verifies the early candidates in, later low-scoring

@@ -180,7 +180,33 @@ def _next_up(f):
     return float(np.nextafter(F32(f), F32(np.inf)))
 
 
-def near_threshold_case(orc, m, k, n_docs, *, binade=16.0, dense=False, n_rare=0, seed=0, tries=3000):
+def pool_capacity(k):
+    """KP of the launch that answers a limit of k (bm25x_search.cu launch_ring_k): the warp's candidate pool, in shared
+    memory up to 2048 entries, in HBM beyond."""
+    return 64 if k <= 32 else 256 if k <= 224 else 2048 if k <= 1024 else 131072
+
+
+def cut_trigger(k, kp, threshold):
+    """The pool size at which pool_insert cuts the pool back to k (k_search_ring): always above KP − 32 entries; before
+    that, at k + 32 entries, unless the pool is a large one (KP > 128) that already has a threshold (the lazy cut)."""
+    lazy = kp > 128 and threshold
+    return kp - 31 if lazy else min(kp - 31, k + 32)
+
+
+def late_count(k, n_low, hit_rows=0):
+    """Late low documents of near_threshold_case.  A kernel may cut the pool first with A (or some high documents)
+    missing; after that cut the pool holds k entries and has a threshold.  A enters, and every late low document beats
+    that threshold, so once pool_insert has cut again at cut_trigger(k, KP, True) entries A is the k-th: that takes
+    cut_trigger − k late documents.  The seeded kernel's hit list (hit_rows rows, RCfg::HCAP) keeps up to hit_rows − 1
+    of them waiting across windows until the flush that scores B: their insertion comes after B's filter, so hit_rows
+    more.  An HBM pool (KP > 2048) is cut lazily only beyond KP − 32 = 131 040 entries, more than a list here holds:
+    there the cases rest on the first cut, which the n_low early low documents force at k + 32 entries.  Never fewer
+    than n_low, the count the fixtures of k <= 32 without a hit list were built with."""
+    kp = pool_capacity(k)
+    return n_low if kp > 2048 else max(n_low, cut_trigger(k, kp, True) - k + hit_rows)
+
+
+def near_threshold_case(orc, m, k, n_docs, *, binade=16.0, dense=False, n_rare=0, hit_rows=0, seed=0, tries=3000):
     """A corpus (b = 0, k1 = 2: exact regime) in which the margin kEps alone decides whether a top-k document survives.
 
     Query terms: ids 0 … m − 1 (B's terms), m (term x, A's knob) and, with n_rare, m + 1 … m + n_rare (df 1: the rarest,
@@ -188,39 +214,94 @@ def near_threshold_case(orc, m, k, n_docs, *, binade=16.0, dense=False, n_rare=0
     everything else); with n_rare, one document holding the rare terms; document A (term x at a large tf, a few of B's
     terms at tf <= 3, searched so that next_f32(F_B) <= S_A < S_B); 40 "low" documents (terms 0 and 1, tf 1); the fillers —
     single-term documents spread evenly (sparse) or, with `dense`, a block of documents holding every B term with tf 1 —
-    with 40 "late low" documents (terms 0 and 1, tf 3: above every low document and filler, below S_A) halfway through
-    them; and last, document B (B's m terms, tf 2).  The late low documents make the threshold S_A whatever order the
-    early candidates were verified in: a kernel may cut the pool for the first time before the high documents or A are
-    in it (the seeded kernel verifies its champion seeds and the documents of the lower runs first), and then, with
-    nothing else above that first threshold, the k-th score would stay below S_A until B.  With them, the pool overflows
-    again once A and the high documents are in, and is cut to exactly those k.  B's exact score beats S_A while B's f32
-    filter score is below f32_rd(S_A): a kernel without the margin drops B.
+    with late_count(k, 40, hit_rows) "late low" documents (terms 0 and 1, tf 3: above every low document and filler,
+    below S_A) halfway through them; and last, document B (B's m terms, tf 2).  The late low documents make the threshold S_A
+    whatever order the early candidates were verified in: a kernel may cut the pool for the first time before the high
+    documents or A are in it (the seeded kernel verifies its champion seeds and the documents of the lower runs first),
+    and then, with nothing else above that first threshold, the k-th score would stay below S_A until B.  With them, the
+    pool overflows again once A and the high documents are in, and is cut to exactly those k.  B's exact score beats S_A
+    while B's f32 filter score is below f32_rd(S_A): a kernel without the margin drops B.
 
     B's dfs are searched among the terms whose s0 (just above `binade`) rounds down most in f32, in the order that leaves
-    F_B furthest below S_B."""
+    F_B furthest below S_B.  m = 2: B's two tfs are searched too (tf 6 or 14 where tf 2 cannot lose enough).
+
+    m = 1 (a 2-term query): B holds term x too, so that it has two holders (a document of one holder would be a seed or a
+    single-term posting).  Two terms at tf 2 cannot lose more than one f32 ulp, so B's tfs and A's tf on term 0 are
+    searched as well, and term x's df is solved so that A's large tf on x lands S_A in the window (_pair_case).  Its late
+    low documents hold term 0 at tf 1 and x at tf 2 (tf 3 on both would beat B)."""
     rng = np.random.default_rng(seed)
     k1, b = 2.0, 0.0
     n_high = k - 1 - (1 if n_rare else 0)
-    n_low = 40  # also the number of late low documents
+    n_low = 40
+    n_late = late_count(k, n_low, hit_rows)
     # s0 = 3 ln((N + 1) / (df + 0.5)) in [binade, 1.1 binade]
     cand = np.arange(int(n_docs * np.exp(-1.1 * binade / 3)) + 1, int(n_docs * np.exp(-binade / 3)))
     s0c, s1d = cache(orc, n_docs, cand, k1, b)
     assert np.all(s1d == 2.0) and len(cand) >= 2 * m
     rel = (s0c - s0c.astype(F32).astype(np.float64)) / s0c
+    if m == 1:
+        assert not n_rare and not dense
+        return _pair_case(orc, cand, s0c, s1d, k, n_docs, n_high, n_low, n_late, rng)
     pool = np.argsort(-rel)[:max(60, 2 * m)]
+    # two terms at tf 2 lose at most one ulp of their f32 sum (each s0f / 2 is exact, the sum rounds once): with two
+    # terms B's tfs are searched too (tf + 2 a power of two: 6 and 14 round tf·s0f as well)
+    tfbs = [(2,) * m] if m > 2 else [(6, 6), (2, 6), (6, 2), (6, 14), (14, 6)]
     found = {}
     for _ in range(tries):
         pick = tuple(rng.choice(pool, size=m, replace=False))
         q = Query(s0c[list(pick)], s1d)
-        F = float(q.filter_score([2] * m)[0])
-        S = q.exact([2] * m)
-        if S > _next_up(F):
-            found[pick] = (S - _next_up(F)) / S
-    for pick in sorted(found, key=lambda p: -found[p])[:40]:
-        case = _with_a(orc, np.array(pick), cand, s0c, s1d, m, k, n_docs, n_high, n_low, dense, n_rare, rng)
+        for tfb in tfbs:
+            F = float(q.filter_score(tfb)[0])
+            S = q.exact(tfb)
+            if S > _next_up(F):
+                found[pick, tfb] = (S - _next_up(F)) / S
+    for pick, tfb in sorted(found, key=lambda p: -found[p])[:40]:
+        case = _with_a(orc, np.array(pick), cand, s0c, s1d, m, k, n_docs, n_high, n_low, n_late, dense, n_rare, rng,
+                       list(tfb))
         if case is not None and (case["tight_pruned"] or m + 1 > 8 or n_rare):
             return case
     raise AssertionError(f"no near-threshold fixture for m={m}")
+
+
+def _pair_case(orc, cand, s0c, s1d, k, n_docs, n_high, n_low, n_late, rng):
+    """The 2-term fixture: B = (tf t0 on term 0, tf tx on x), A = (tf a on term 0, a large tf T on x).  With T large,
+    S_A = s0_0·a/(a + 2) + s0_x·(1 − 2/(T + 2)) reaches S_B = s0_0·t0/(t0 + 2) + s0_x·tx/(tx + 2) only when
+    s0_x·2/(tx + 2) is just above s0_0·(t0/(t0 + 2) − a/(a + 2)): x's df is taken from that neighbourhood, and T solved."""
+    need = n_high + n_low + n_late + 16  # postings of each term: high, low, late documents, A, B and a few fillers
+    cand_x = np.arange(need, n_docs // 8)
+    for t0, tx, a in ((6, 2, 1), (14, 2, 1), (6, 6, 2), (14, 6, 2), (6, 2, 2), (2, 6, 1), (14, 2, 2)):
+        c = t0 / (t0 + 2) - a / (a + 2)
+        for i in rng.permutation(len(cand))[:400]:
+            if cand[i] < need:
+                continue
+            s0_0 = float(s0c[i])
+            target = (tx + 2) / 2 * s0_0 * c  # s0_x at which T would be infinite
+            d0 = int((n_docs + 1) * np.exp(-target / 3))
+            dfx = cand_x[(cand_x >= d0 - 40) & (cand_x <= d0 + 2)]
+            if len(dfx) == 0:
+                continue
+            s0x, _ = cache(orc, n_docs, dfx, 2.0, 0.0)
+            for d, s0_x in zip(dfx, s0x):
+                q = Query(np.array([s0_0, s0_x]), s1d)
+                F_b = float(q.filter_score([t0, tx])[0])
+                S_b = q.exact([t0, tx])
+                lo_w = _next_up(F_b)
+                if not S_b > lo_w:
+                    continue
+                part = float(score64(a, s0_0, 2.0))
+                R = lo_w - part
+                if not s0_x > R:
+                    continue
+                t_0 = 2.0 * R / (s0_x - R)
+                if not (1 << 12) <= t_0 <= (1 << 24) - 8:
+                    continue
+                for T in range(int(t_0) - 3, int(t_0) + 5):
+                    if lo_w <= sum64([part, score64(T, s0_x, 2.0)]) < S_b:
+                        case = _corpus(orc, np.array([cand[i], d]), np.array([s0_0, s0_x]), s1d, 1, k, n_docs, n_high,
+                                       n_low, n_late, False, 0, rng, [t0, tx], [a, T], F_b, S_b, late_tf=(1, 2))
+                        if case["tight_pruned"]:
+                            return case
+    raise AssertionError("no near-threshold fixture for a 2-term query")
 
 
 def _find_a(orc, q, m, n_docs, lo_w, hi_w, rng, configs=300):
@@ -257,19 +338,25 @@ def _find_a(orc, q, m, n_docs, lo_w, hi_w, rng, configs=300):
     return None
 
 
-def _with_a(orc, pick, cand, s0c, s1d, m, k, n_docs, n_high, n_low, dense, n_rare, rng):
+def _with_a(orc, pick, cand, s0c, s1d, m, k, n_docs, n_high, n_low, n_late, dense, n_rare, rng, tf_b):
     q = Query(s0c[pick], s1d)
-    tf_b = [2] * m
     F_b = float(q.filter_score(tf_b)[0])
     S_b = q.exact(tf_b)
     got = _find_a(orc, q, m, n_docs, _next_up(F_b), S_b, rng)
     if got is None:
         return None
     df_x, tf_a, s0_x = got
-    qa = Query(np.append(q.s0d, s0_x), s1d)
+    return _corpus(orc, np.append(cand[pick], df_x), np.append(q.s0d, s0_x), s1d, m, k, n_docs, n_high, n_low, n_late,
+                   dense, n_rare, rng, tf_b, tf_a, F_b, S_b)
+
+
+def _corpus(orc, dfs, s0d, s1d, m, k, n_docs, n_high, n_low, n_late, dense, n_rare, rng, tf_b, tf_a, F_b, S_b,
+            late_tf=(3, 3)):
+    """The documents of near_threshold_case around B (tfs tf_b on lanes 0 … len(tf_b) − 1) and A (tf_a on lanes 0 … m)."""
+    bl = len(tf_b)  # B's lanes: m, or m + 1 when B holds x as well
+    qa = Query(s0d, s1d)
     S_a = qa.exact(tf_a)
     assert _next_up(F_b) <= S_a < S_b
-    dfs = np.append(cand[pick], df_x)
     T = m + 1 + n_rare
     a_doc = n_high + (1 if n_rare else 0)
     low0 = a_doc + 1
@@ -282,7 +369,7 @@ def _with_a(orc, pick, cand, s0c, s1d, m, k, n_docs, n_high, n_low, dense, n_rar
         lists[t][1].append(int(tf))
 
     for d in range(n_high):
-        for t in range(m):
+        for t in range(bl):
             put(d, t, 30)
     for t in range(m + 1, T):
         put(n_high, t, 1)
@@ -292,29 +379,29 @@ def _with_a(orc, pick, cand, s0c, s1d, m, k, n_docs, n_high, n_low, dense, n_rar
     for d in range(low0, first):
         put(d, 0, 1)
         put(d, 1, 1)
-    used = np.array([len(lists[t][0]) + (n_low if t < 2 else 0) + (1 if t < m else 0) for t in range(m + 1)])  # late, B
-    region = int(min(dfs[:m] - used[:m])) - 8 if dense else 0
-    extra = dfs - used - np.append(np.full(m, region), 0)
+    used = np.array([len(lists[t][0]) + (n_late if t < 2 else 0) + (1 if t < bl else 0) for t in range(m + 1)])  # late, B
+    region = int(min(dfs[:bl] - used[:bl])) - 8 if dense else 0
+    extra = dfs - used - np.append(np.full(bl, region), np.zeros(m + 1 - bl, int))
     assert np.all(extra >= 0)
     singles = np.repeat(np.arange(m + 1), extra)
     rng.shuffle(singles)
     stop = b_doc - region
     late0 = (first + stop) // 2
-    late = np.arange(late0, late0 + n_low)
+    late = np.arange(late0, late0 + n_late)
     free = np.setdiff1d(np.arange(first, stop), late)
     stride = len(free) // (len(singles) + 1)
     assert stride >= 1
     docs = [(int(d), int(t), 1) for d, t in zip(free[np.arange(len(singles)) * stride], singles)]
-    docs += [(int(d), t, 3) for d in late for t in (0, 1)]
+    docs += [(int(d), t, late_tf[t]) for d in late for t in (0, 1)]
     for d, t, tf in sorted(docs):
         put(d, t, tf)
-    S_late = float(score64(3, qa.s0d[0], 2.0) + score64(3, qa.s0d[1], 2.0))
+    S_late = float(score64(late_tf[0], qa.s0d[0], 2.0) + score64(late_tf[1], qa.s0d[1], 2.0))
     assert S_late < S_a
     for d in range(stop, b_doc):
-        for t in range(m):
+        for t in range(bl):
             put(d, t, 1)
-    for t in range(m):
-        put(b_doc, t, 2)
+    for t in range(bl):
+        put(b_doc, t, tf_b[t])
     post_off = np.zeros(T + 1, np.uint64)
     post_off[1:] = np.cumsum([len(d) for d, _ in lists])
     for t, (d, _) in enumerate(lists):
@@ -325,15 +412,15 @@ def _with_a(orc, pick, cand, s0c, s1d, m, k, n_docs, n_high, n_low, dense, n_rar
     # bounds (k_term_ub) and the pruned set at Sk = S_A over the m + 1 lanes of a single-pass query
     ubd = [float(max(score64(np.asarray(lists[t][1]), qa.s0d[t], 2.0))) * (1.0 + 2.0 ** -40) for t in range(m + 1)]
     pruned = pruned_lanes(ubd, S_a) if not n_rare else []
-    tfb1 = tf_b + [0]
+    tfb1 = list(tf_b) + [0] * (m + 1 - bl)
     F_probe = float(qa.filter_score(tfb1, order=probe_order(m + 1, pruned))[0])
-    F_str = float(qa.filter_score(tfb1, order=[i for i in range(m + 1) if i not in pruned])[0]) if len(pruned) < m else None
+    F_str = float(qa.filter_score(tfb1, order=[i for i in range(m + 1) if i not in pruned])[0]) if len(pruned) < bl else None
     Flo, _ = thresholds(S_a)
     Flo_p, FloT = thresholds(S_a, sum(ubd[i] for i in pruned))
     return dict(m=m, k=k, n_docs=n_docs, doc_len=doc_len, n_terms=T, post_off=post_off, post_doc=post_doc,
                 post_tf=post_tf, query=np.arange(T, dtype=np.uint32), a_doc=a_doc, b_doc=b_doc, tf_a=tf_a, df=dfs,
                 S_a=S_a, S_b=S_b, F_b=F_b, F_probe=F_probe, pruned=pruned, dense_from=stop, stride=stride,
-                late=late, S_late=S_late,
+                late=late, S_late=S_late, tf_b=list(tf_b), ubd=ubd,
                 # kEps = 0 drops B, the shipped margin keeps it: without pruning (F_B against Flo), and with the terms
                 # pruned at Sk = S_A (the streamed part against Flo − ub_ne, then the probe loop's Fres against FloT)
                 tight=F_b < f32_rd(S_a), keeps=F_b >= Flo,

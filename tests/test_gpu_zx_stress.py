@@ -1,6 +1,7 @@
 """GPU parity stress: many small random corpora / query shapes / limits against the exhaustive oracle, bit for bit —
-ring wrap-around, single-posting terms, head terms next to rare ones (dense windows, pruning and the re-split of the
-rings), duplicate-heavy vocabularies (tie floods), every term-count class, pruning on and off."""
+ring wrap-around, single-posting terms, head terms next to rare ones (dense windows, and pruning where a draw happens to
+reach it), duplicate-heavy vocabularies (tie floods), every term-count class, pruning on and off.  Nothing here asserts
+that a query pruned or that its rings were split again: test_gpu_prune_points.py builds those cases on purpose."""
 import numpy as np
 import pytest
 

@@ -1,6 +1,6 @@
-"""GPU: the refresh and the seal of a growing segment on a constructed corpus, not a random one.  k_growing_splice and
-k_seal_splice walk every source of a term (refresh: the current handle's list, then the pending one; seal: the sealed list,
-then the growing handle's, or the dormant list alone) in 32-posting steps with a ballot / popc compaction, each source
+"""GPU: the refresh and the seal of a growing segment on a constructed corpus, not a random one.  k_splice walks every
+source of a term (refresh: the current handle's list, then the pending one; seal: the sealed list, then the growing
+handle's, or the dormant list alone) in 32-posting steps with a ballot / popc compaction, each source
 starting at whatever position the one before left.  TABLE chooses per term how many postings each source holds and which
 of them are deleted; the documents are built from it, `coverage` derives from the built lists what every kernel step
 sees (length, survivors, start position) and test_table_covers_every_case asserts the cases, so an edit that loses one

@@ -1,6 +1,6 @@
-"""GPU: the refresh and the seal of a growing segment at the vocabulary size they are built for.  k_growing_count,
-k_growing_splice, k_seal_doc_postings, k_seal_df and k_seal_splice take one warp per term in a grid capped at 32 blocks of
-8 warps per SM and loop `t += warps`; with T = 3 x sm_count x 256 terms (101 376 on a 132-SM H100) every warp of every
+"""GPU: the refresh and the seal of a growing segment at the vocabulary size they are built for.  k_splice_count,
+k_splice and k_seal_doc_postings take one warp per term in a grid capped at 32 blocks of 8 warps per SM and loop
+`t += warps`; with T = 3 x sm_count x 256 terms (101 376 on a 132-SM H100) every warp of every
 one of them takes three trips, on whatever card runs this.  Sealed: ~400 k documents of 16-48 terms, Zipf 0.8, the upper
 half of the vocabulary thinned to 0-3 postings per term (head lists of ~200 k postings: thousands of 32-posting steps).
 Growing: 40 k documents over the same vocabulary, 2000 new ordinals (keyed: new keys that interleave with the sealed
@@ -113,7 +113,7 @@ def test_more_terms_than_warps(m, orc, kind):
         got = seg.seal(sealed_deleted=_pack(sdel), new_keys=new_keys)
         r = maintain(w.n_docs, w.off, w.doc, w.tf, docs.restated(orc, "doc_len", True), sealed_deleted=sdel,
                      sealed_keys=w.keys, new_keys=new_keys)
-        assert r.n_terms >= 3 * sms * 256, "k_seal_splice's term loop takes fewer than three trips"
+        assert r.n_terms >= 3 * sms * 256, "k_splice's term loop takes fewer than three trips"
         rs = _check_result(m, orc, got[0], got[1:], r, f"{kind}, seal")
         assert np.array_equal(got[0].df(), rs.df), f"{kind}: bm25x_index_get_df of the seal's result"
         ref = m.Index(r.n_docs, r.doc_len, r.n_terms, r.post_off, r.post_doc, r.post_tf, payload=r.payload,

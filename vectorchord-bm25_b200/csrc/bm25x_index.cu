@@ -19,8 +19,7 @@
 
 #include "bm25x_common.h"
 #include "bm25x_blocks.cuh"
-#include "bm25x_growing.cuh"
-#include "bm25x_seal.cuh"
+#include "bm25x_splice.cuh"
 
 static thread_local char g_err[512] = "";
 
@@ -1597,6 +1596,88 @@ extern "C" int bm25x_growing_delete(bm25x_growing_segment *g, uint32_t n, const 
     return BM25X_OK;
 }
 
+// ---- the splice of the refresh and the seal (bm25x_splice.cuh): the sources described, their survivors counted per
+// term, a handle opened with that df, the survivors written into it ----
+
+// The grid of a one-warp-per-term launch over n > 0 terms: 8 warps per block, at most 32 blocks per SM.
+static unsigned splice_grid(uint32_t n, int sm_count) {
+    return (unsigned)std::min<uint64_t>(((uint64_t)n + 7) / 8, (uint64_t)sm_count * 32ull);
+}
+
+// The deleted bitmap of a byte-per-document vector: bit d of word d >> 5 set = deleted[d] != 0.
+static std::vector<uint32_t> deleted_bitmap(const std::vector<uint8_t> &deleted) {
+    std::vector<uint32_t> bits((deleted.size() + 31) / 32, 0);
+    for (size_t d = 0; d < deleted.size(); d++)
+        if (deleted[d]) bits[d >> 5] |= 1u << (d & 31);
+    return bits;
+}
+
+// An index handle's lists as a splice source (h == NULL: no source).
+static SpliceSrc handle_source(const bm25x_index *h, const uint32_t *del, const uint32_t *map) {
+    SpliceSrc s{};
+    if (h) {
+        s.off = h->d.post_off;
+        s.df = h->d.df;
+        s.doc = h->d.pdoc;
+        s.post = h->d.post;
+        s.n_terms = h->d.n_terms;
+    }
+    s.del = del;
+    s.map = map;
+    return s;
+}
+
+// A (term, doc, tf) list, appended so that each term's docs ascend, grouped over n terms and uploaded as a splice source:
+// a stable counting sort by term keeps each term's docs in order.  Failures stick in sc.e.
+static SpliceSrc grouped_source(Scratch &sc, uint32_t n, const std::vector<uint32_t> &term, const std::vector<uint32_t> &doc,
+                                const std::vector<uint32_t> &tf, const uint32_t *del, const uint32_t *map) {
+    const uint64_t P = term.size();
+    std::vector<uint64_t> off((size_t)n + 1, 0);
+    for (uint64_t p = 0; p < P; p++) off[(size_t)term[p] + 1]++;
+    for (uint32_t t = 0; t < n; t++) off[(size_t)t + 1] += off[t];
+    std::vector<uint32_t> gdoc(P), gtf(P);
+    std::vector<uint64_t> at(off.begin(), off.end() - 1);
+    for (uint64_t p = 0; p < P; p++) {
+        const uint64_t i = at[term[p]]++;
+        gdoc[i] = doc[p];
+        gtf[i] = tf[p];
+    }
+    SpliceSrc s{};
+    s.off = sc.up(off.data(), off.size());
+    s.doc = sc.up(gdoc.data(), P);
+    s.tf = sc.up(gtf.data(), P);
+    s.del = del;
+    s.map = map;
+    s.n_terms = n;
+    return s;
+}
+
+// df[t] = the surviving postings of term t < n over src: k_splice_count, then the download.  Failures stick in sc.e.
+static std::vector<uint32_t> splice_count(Scratch &sc, int sm_count, uint32_t n, const SpliceSources &src) {
+    std::vector<uint32_t> df(n);
+    uint32_t *d_df = sc.alloc<uint32_t>(n);
+    if (sc.e == cudaSuccess && n) {
+        k_splice_count<<<splice_grid(n, sm_count), 256>>>(n, src, d_df);
+        sc.e = cudaGetLastError();
+    }
+    if (sc.e == cudaSuccess && n) sc.e = cudaMemcpy(df.data(), d_df, sizeof(uint32_t) * n, cudaMemcpyDeviceToHost);
+    return df;
+}
+
+// The survivors of src written into ix, opened by index_begin with the df splice_count gave (new term j from source term
+// src_of[j]; src_of == NULL: j), then what every index derives from them.  A CUDA failure, here or earlier in sc.e, is
+// refused as step "splice" of `who`.
+static int splice_finish(Scratch &sc, const char *who, bm25x_index *ix, const uint32_t *src_of, const SpliceSources &src) {
+    const uint32_t n = ix->d.n_terms;
+    if (sc.e == cudaSuccess && n) {
+        k_splice<<<splice_grid(n, ix->sm_count), 256>>>(n, src_of, src, ix->d.fieldnorm, ix->d.post_off, ix->d.post);
+        sc.e = cudaGetLastError();
+    }
+    if (sc.e == cudaSuccess) sc.e = cudaDeviceSynchronize();
+    if (sc.e == cudaSuccess) sc.e = index_finish_device(ix);
+    return sc.e == cudaSuccess ? BM25X_OK : cuda_refusal(who, "splice", sc.e);
+}
+
 // The refresh, under g->mu: the next handle is built beside the current one (which running searches may still read)
 // from its surviving postings and the inserted ones, then replaces it.  On a refusal nothing changes.
 static int growing_refresh_locked(bm25x_growing_segment *g) {
@@ -1605,41 +1686,16 @@ static int growing_refresh_locked(bm25x_growing_segment *g) {
     const bm25x_index *sealed = g->sealed;
     const uint32_t N = g->n_docs(), T = sealed->d.n_terms;
     const int device = sealed->device;
-    // the inserted postings as one term-major CSR: a stable counting sort by term keeps each term's ordinals ascending
-    const uint64_t PP = g->pend_term.size();
-    std::vector<uint64_t> pend_off((size_t)T + 1, 0);
-    for (uint64_t p = 0; p < PP; p++) pend_off[(size_t)g->pend_term[p] + 1]++;
-    for (uint32_t t = 0; t < T; t++) pend_off[(size_t)t + 1] += pend_off[t];
-    std::vector<uint32_t> pend_doc(PP), pend_tf(PP);
-    {
-        std::vector<uint64_t> cur(pend_off.begin(), pend_off.end() - 1);
-        for (uint64_t p = 0; p < PP; p++) {
-            const uint64_t at = cur[g->pend_term[p]]++;
-            pend_doc[at] = g->pend_doc[p];
-            pend_tf[at] = g->pend_tf[p];
-        }
-    }
-    std::vector<uint32_t> bits(((size_t)N + 31) / 32, 0);
-    for (uint32_t o = 0; o < N; o++)
-        if (g->deleted[o]) bits[o >> 5] |= 1u << (o & 31);
-    // ---- new df: the survivors of the current lists and of the inserted ones ----
+    // ---- the sources: the current handle's lists, then the postings inserted since, against the deleted ordinals ----
     Scratch sc(device);
     sc.e = cudaSetDevice(device);
-    const uint64_t *d_pend_off = sc.up(pend_off.data(), (size_t)T + 1);
-    const uint32_t *d_pend_doc = sc.up(pend_doc.data(), PP), *d_pend_tf = sc.up(pend_tf.data(), PP);
+    const std::vector<uint32_t> bits = deleted_bitmap(g->deleted);
     const uint32_t *d_del = sc.up(bits.data(), bits.size());
-    uint32_t *d_df = sc.alloc<uint32_t>(T);
-    const bm25x_index *old = g->cur.get();
-    const Posting *old_post = old ? old->d.post : nullptr;
-    const uint64_t *old_off = old ? old->d.post_off : nullptr;
-    const uint32_t *old_df = old ? old->d.df : nullptr;
-    const unsigned grid = (unsigned)std::min<uint64_t>(((uint64_t)T + 7) / 8, (uint64_t)sealed->sm_count * 32ull);
-    if (sc.e == cudaSuccess && T) {
-        k_growing_count<<<grid, 256>>>(T, old_post, old_off, old_df, d_pend_off, d_pend_doc, d_del, d_df);
-        sc.e = cudaGetLastError();
-    }
-    std::vector<uint32_t> df(T);
-    if (sc.e == cudaSuccess && T) sc.e = cudaMemcpy(df.data(), d_df, sizeof(uint32_t) * T, cudaMemcpyDeviceToHost);
+    SpliceSources src{};
+    src.s[0] = handle_source(g->cur.get(), d_del, nullptr);
+    src.s[1] = grouped_source(sc, T, g->pend_term, g->pend_doc, g->pend_tf, d_del, nullptr);
+    // ---- new df: the survivors of the current lists and of the inserted ones ----
+    const std::vector<uint32_t> df = splice_count(sc, sealed->sm_count, T, src);
     if (sc.e != cudaSuccess) return cuda_refusal(who, "count", sc.e);
     uint64_t P = 0;
     for (uint32_t t = 0; t < T; t++) P += df[t];
@@ -1649,15 +1705,8 @@ static int growing_refresh_locked(bm25x_growing_segment *g) {
     m.fieldnorm = g->norm_form ? nullptr : g->fieldnorm.data();
     IndexGuard ix;
     int rc = index_begin(m, &g->stats, device, ix);
+    if (rc == BM25X_OK) rc = splice_finish(sc, who, ix.get(), nullptr, src);
     if (rc != BM25X_OK) return rc;
-    if (T) {
-        k_growing_splice<<<grid, 256>>>(T, old_post, old_off, old_df, d_pend_off, d_pend_doc, d_pend_tf, d_del,
-                                        ix->d.fieldnorm, ix->d.post_off, ix->d.post);
-        sc.e = cudaGetLastError();
-    }
-    if (sc.e == cudaSuccess) sc.e = cudaDeviceSynchronize();
-    if (sc.e == cudaSuccess) sc.e = index_finish_device(ix.get());
-    if (sc.e != cudaSuccess) return cuda_refusal(who, "splice", sc.e);
     growing_options(ix.get(), sealed);
     g->cur.reset(ix.release(), IndexDestroy());
     std::vector<uint32_t>().swap(g->pend_term);
@@ -1853,54 +1902,30 @@ extern "C" int bm25x_growing_seal(bm25x_growing_segment *g, bm25x_seal_args *a, 
     std::vector<uint32_t> gmap(NG);
     uint32_t N = ns_keep;
     for (uint32_t o = 0; o < NG; o++) gmap[o] = s.deleted[o] ? BM25X_DOC_INF : N++;
-    // the dormant postings as a CSR over the source terms: a stable counting sort keeps each term's ordinals ascending
-    const uint64_t PD = s.dorm_term.size();
-    std::vector<uint64_t> dorm_off((size_t)n_src + 1, 0);
-    for (uint64_t p = 0; p < PD; p++) dorm_off[(size_t)s.dorm_term[p] + 1]++;
-    for (uint32_t t = 0; t < n_src; t++) dorm_off[(size_t)t + 1] += dorm_off[t];
-    std::vector<uint32_t> dorm_doc(PD), dorm_tf(PD);
-    {
-        std::vector<uint64_t> cur(dorm_off.begin(), dorm_off.end() - 1);
-        for (uint64_t p = 0; p < PD; p++) {
-            const uint64_t at = cur[s.dorm_term[p]]++;
-            dorm_doc[at] = s.dorm_doc[p];
-            dorm_tf[at] = s.dorm_tf[p];
-        }
-    }
-    std::vector<uint32_t> sbits(((size_t)NS + 31) / 32, 0), gbits(((size_t)NG + 31) / 32, 0);
+    // ---- the sources: the sealed lists, the growing handle's, the dormant postings; the deleted bitmaps and the maps ----
+    std::vector<uint32_t> sbits(((size_t)NS + 31) / 32, 0);
     if (a->sealed_deleted) memcpy(sbits.data(), a->sealed_deleted, ((size_t)NS + 7) / 8);  // little-endian: bit d of word d >> 5
-    for (uint32_t o = 0; o < NG; o++)
-        if (s.deleted[o]) gbits[o >> 5] |= 1u << (o & 31);
-    // ---- rule 3 lengths and rule 5 df on the device ----
+    const std::vector<uint32_t> gbits = deleted_bitmap(s.deleted);
     Scratch sc(device);
     sc.e = cudaSetDevice(device);
     const uint32_t *d_sdel = sc.up(sbits.data(), sbits.size()), *d_gdel = sc.up(gbits.data(), gbits.size());
-    const uint32_t *d_smap = sc.up(smap.data(), NS), *d_gmap = sc.up(gmap.data(), NG);
-    const uint64_t *d_dorm_off = sc.up(dorm_off.data(), (size_t)n_src + 1);
-    const uint32_t *d_dorm_doc = sc.up(dorm_doc.data(), PD), *d_dorm_tf = sc.up(dorm_tf.data(), PD);
-    uint32_t *d_cnt = sc.alloc<uint32_t>(NS), *d_df = sc.alloc<uint32_t>(n_src);
-    const bm25x_index *gh = s.cur.get();
-    const Posting *g_post = gh ? gh->d.post : nullptr;
-    const uint64_t *g_off = gh ? gh->d.post_off : nullptr;
-    const uint32_t *g_df = gh ? gh->d.df : nullptr;
+    const uint32_t *d_gmap = sc.up(gmap.data(), NG);
+    SpliceSources src{};
+    src.s[0] = handle_source(sealed, d_sdel, sc.up(smap.data(), NS));
+    src.s[1] = handle_source(s.cur.get(), d_gdel, d_gmap);
+    src.s[2] = grouped_source(sc, n_src, s.dorm_term, s.dorm_doc, s.dorm_tf, d_gdel, d_gmap);
+    // ---- rule 3 lengths and rule 5 df on the device ----
+    uint32_t *d_cnt = sc.alloc<uint32_t>(NS);
     const DeviceIndex &sd = sealed->d;
-    auto grid = [&](uint32_t n) {
-        return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(((uint64_t)n + 7) / 8, (uint64_t)sealed->sm_count * 32ull));
-    };
     if (sc.e == cudaSuccess) sc.e = cudaMemset(d_cnt, 0, sizeof(uint32_t) * (size_t)NS);
     if (sc.e == cudaSuccess && T) {
-        k_seal_doc_postings<<<grid(T), 256>>>(T, sd.pdoc, sd.post_off, sd.df, d_sdel, d_cnt);
+        k_seal_doc_postings<<<splice_grid(T, sealed->sm_count), 256>>>(T, sd.pdoc, sd.post_off, sd.df, d_sdel, d_cnt);
         sc.e = cudaGetLastError();
     }
-    if (sc.e == cudaSuccess && n_src) {
-        k_seal_df<<<grid(n_src), 256>>>(n_src, T, sd.pdoc, sd.post_off, sd.df, d_sdel, g_post, g_off, g_df, d_gdel,
-                                        d_dorm_off, d_dorm_doc, d_df);
-        sc.e = cudaGetLastError();
-    }
-    std::vector<uint32_t> cnt(NS), df_src(n_src);
+    const std::vector<uint32_t> df_src = splice_count(sc, sealed->sm_count, n_src, src);
+    std::vector<uint32_t> cnt(NS);
     std::vector<uint16_t> spay((size_t)NS * 3);
     if (sc.e == cudaSuccess) sc.e = cudaMemcpy(cnt.data(), d_cnt, sizeof(uint32_t) * (size_t)NS, cudaMemcpyDeviceToHost);
-    if (sc.e == cudaSuccess && n_src) sc.e = cudaMemcpy(df_src.data(), d_df, sizeof(uint32_t) * n_src, cudaMemcpyDeviceToHost);
     if (sc.e == cudaSuccess)
         sc.e = cudaMemcpy(spay.data(), sd.payload, sizeof(uint16_t) * 3 * (size_t)NS, cudaMemcpyDeviceToHost);
     if (sc.e != cudaSuccess) return cuda_refusal(who, "count", sc.e);
@@ -1943,17 +1968,8 @@ extern "C" int bm25x_growing_seal(bm25x_growing_segment *g, bm25x_seal_args *a, 
     BuildMeta m{N, TN, len.data(), pay.data(), keyed ? keys.data() : nullptr, sealed->k1, sealed->b, df.data(), P};
     IndexGuard ix;
     int rc = index_begin(m, nullptr, device, ix);
+    if (rc == BM25X_OK) rc = splice_finish(sc, who, ix.get(), sc.up(src_of.data(), TN), src);
     if (rc != BM25X_OK) return rc;
-    const uint32_t *d_src_of = sc.up(src_of.data(), TN);
-    if (sc.e == cudaSuccess && TN) {
-        k_seal_splice<<<grid(TN), 256>>>(TN, d_src_of, T, sd.post, sd.post_off, sd.df, d_sdel, d_smap, g_post, g_off, g_df,
-                                         d_gdel, d_gmap, d_dorm_off, d_dorm_doc, d_dorm_tf, ix->d.fieldnorm, ix->d.post_off,
-                                         ix->d.post);
-        sc.e = cudaGetLastError();
-    }
-    if (sc.e == cudaSuccess) sc.e = cudaDeviceSynchronize();
-    if (sc.e == cudaSuccess) sc.e = index_finish_device(ix.get());
-    if (sc.e != cudaSuccess) return cuda_refusal(who, "splice", sc.e);
     a->n_growing = NG;
     a->n_source_terms = n_src;
     if (a->sealed_map) std::copy(smap.begin(), smap.end(), a->sealed_map);

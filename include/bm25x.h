@@ -379,6 +379,28 @@ int bm25x_sharded_lookup_terms(const bm25x_sharded_index *sx, const uint8_t *key
 int bm25x_sharded_search_batch(bm25x_sharded_index *sx, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms,
                                uint32_t k, const uint8_t *allow, uint32_t *out_doc, float *out_score, double *out_score64,
                                uint16_t *out_payload, uint32_t *out_n, bm25x_search_stats *stats);
+/* A growing segment over a document-sharded index.  It scores with the whole segment's statistics (as every shard
+ * does).  Its handle lives on the LAST shard's device.  After this call the segment is an ordinary
+ * bm25x_growing_segment: insert, delete, refresh, get_info, get_index, search_batch and close take it unchanged, with
+ * "the sealed index" meaning the whole segment (n_docs, n_terms, df, keys, Σlen / avgdl) and
+ * bm25x_growing_info.device the last shard's.  bm25x_growing_search_batch then has the refusals of
+ * bm25x_sharded_search_batch (the whole segment's canonicalisation first) and merges the shards' lists and the growing
+ * handle's, growing ordinal o as n_docs(whole) + o, allow_sealed over global ids; stats: queries = live queries of the
+ * whole segment plus the growing handle's, the rest sums over the shards, the growing handle and the merge launch.
+ * Before the first insert it is bm25x_sharded_search_batch, stats included.  The sharded index must outlive the segment;
+ * bm25x_growing_seal refuses the segment (BM25X_ERR_INVALID). */
+int bm25x_growing_open_sharded(bm25x_sharded_index *sealed, bm25x_growing_segment **out);
+/* The seal of a segment opened with bm25x_growing_open_sharded.  The result is a new document-sharded index.  args,
+ * refusals and concurrency are bm25x_growing_seal's (sealed_deleted over global ids, the maps give new global ids, equal
+ * to those of bm25x_growing_seal on an unsharded index over the same corpus).  New shard j comes from an old shard and
+ * holds its surviving documents in ascending old id; the old LAST shard also takes the growing survivors after its own.
+ * An old shard left with no document is dropped; the rest keep their order and devices, the new bounds are the prefix
+ * sums of the survivors.  Every shard scores with the new segment's statistics; the keys, when keyed, are with shard 0;
+ * options are bm25x_sharded_create's defaults.  Each shard is rebuilt on its own device from its own arrays: at the peak a
+ * device holds its old and new shards, the last one also the growing handle.  BM25X_ERR_OOM when a new shard does not
+ * fit (bounds are not rebalanced).  The old sharded index and the segment are not changed; an unsharded segment is
+ * refused (BM25X_ERR_INVALID). */
+int bm25x_growing_seal_sharded(bm25x_growing_segment *g, bm25x_seal_args *args, bm25x_sharded_index **out);
 /* Test hook: the arrays of shard s (0 <= s < n_shards) as bm25x_index_get_layout / bm25x_index_get_derived report them
  * for an index: local doc ids, local n_docs / n_postings / df, the whole segment's avgdl and score tables.  The shard
  * handle itself stays internal.  Either output may be NULL. */

@@ -147,6 +147,8 @@ def load_library():
     L.bm25x_growing_close.argtypes = [vp]
     L.bm25x_growing_close.restype = None
     L.bm25x_growing_seal.argtypes = [vp, C.POINTER(SealArgs), C.POINTER(vp)]
+    L.bm25x_growing_open_sharded.argtypes = [vp, C.POINTER(vp)]
+    L.bm25x_growing_seal_sharded.argtypes = [vp, C.POINTER(SealArgs), C.POINTER(vp)]
     L.bm25x_merge_topk.argtypes = [C.c_uint32, C.c_uint32, u32p, f32p, f64p, u16p, u32p, u32p, f32p, f64p, u16p, u32p,
                                    C.c_uint32, u32p, f32p, f64p, u16p, u32p]
     L.bm25x_index_destroy.argtypes = [vp]
@@ -556,12 +558,15 @@ def _growing_docs(keep, elem_off, elem_term, elem_tf, doc_len, doc_fieldnorm, pa
 class GrowingSegment:
     """The growing segment as the library keeps it (bm25x_growing_*): documents inserted and deleted in place, indexed on
     the sealed index's device by a refresh, searched together with the sealed index.  Growing ordinal o comes back as
-    doc id sealed.n_docs + o."""
+    doc id sealed.n_docs + o.  The sealed side is an Index or a ShardedIndex (bm25x_growing_open_sharded: the segment
+    lives on the last shard's device, ids and allow_sealed are global)."""
 
-    def __init__(self, sealed: Index):
+    def __init__(self, sealed):
         self.sealed = sealed
+        self.sharded = isinstance(sealed, ShardedIndex)
         self.h = C.c_void_p()
-        _check(load_library().bm25x_growing_open(sealed.h, C.byref(self.h)))
+        L = load_library()
+        _check((L.bm25x_growing_open_sharded if self.sharded else L.bm25x_growing_open)(sealed.h, C.byref(self.h)))
 
     def insert(self, elem_off, elem_term, elem_tf, doc_len=None, doc_fieldnorm=None, payload=None, deleted=None):
         """Appends documents, arguments as Index.growing (bm25x_growing_insert)."""
@@ -612,7 +617,8 @@ class GrowingSegment:
         new_keys: keyed index only, [n, 16] keys of the token ordinals sealed.n_terms + i.  Returns (index, sealed_map,
         growing_map, term_map): new id of each sealed id / growing ordinal (0xFFFFFFFF: deleted) and new ordinal of each
         source term (TERM_MISSING: vanished); growing_map covers the ordinals the seal took, which may be fewer than
-        info().n_docs when other threads insert meanwhile.  The segment and this sealed index stay as they are."""
+        info().n_docs when other threads insert meanwhile.  The segment and this sealed index stay as they are.  Over a
+        ShardedIndex (bm25x_growing_seal_sharded) the index returned is a new ShardedIndex and the ids are global."""
         L = load_library()
         dele = np.ascontiguousarray(sealed_deleted, dtype=np.uint8) if sealed_deleted is not None else None
         keys = np.ascontiguousarray(new_keys, dtype=np.uint8).reshape(-1, 16) if new_keys is not None else None
@@ -627,14 +633,18 @@ class GrowingSegment:
             a.growing_map, a.growing_cap = _p(gmap, C.c_uint32), g_cap
             a.term_map, a.term_cap = _p(tmap, C.c_uint32), t_cap
             h = C.c_void_p()
-            rc = L.bm25x_growing_seal(self.h, C.byref(a), C.byref(h))
+            rc = (L.bm25x_growing_seal_sharded if self.sharded else L.bm25x_growing_seal)(self.h, C.byref(a), C.byref(h))
             if rc != 0 and (a.n_growing > g_cap or a.n_source_terms > t_cap):
                 g_cap, t_cap = max(g_cap, int(a.n_growing)), max(t_cap, int(a.n_source_terms))
                 continue
             _check(rc)
             info = IndexInfo()
-            _check(L.bm25x_index_get_info(h, C.byref(info)))
-            ix = Index._adopt(h, info.n_docs, info.n_terms)
+            if self.sharded:
+                _check(L.bm25x_sharded_get_info(h, C.byref(info), None, None))
+                ix = ShardedIndex._adopt(h, info.n_docs, info.n_terms)
+            else:
+                _check(L.bm25x_index_get_info(h, C.byref(info)))
+                ix = Index._adopt(h, info.n_docs, info.n_terms)
             return ix, smap, gmap[:a.n_growing].copy(), tmap[:a.n_source_terms].copy()
 
     def close(self):
@@ -708,6 +718,17 @@ class ShardedIndex:
                                                                      devs, C.byref(self.h)))
         self.n_docs, self.n_terms = int(n_docs), int(n_terms)
         return self
+
+    @classmethod
+    def _adopt(cls, handle, n_docs, n_terms):
+        self = cls.__new__(cls)
+        self.h, self.n_docs, self.n_terms = handle, int(n_docs), int(n_terms)
+        return self
+
+    def growing_segment(self) -> "GrowingSegment":
+        """An empty mutable growing segment over this sharded index, on its last shard's device
+        (bm25x_growing_open_sharded); seal() gives a new ShardedIndex.  This index must stay open while the segment is."""
+        return GrowingSegment(self)
 
     @staticmethod
     def from_corpus(c, n_shards=2, doc_bounds=None, devices=None, **kw):

@@ -1303,6 +1303,40 @@ extern "C" int bm25x_index_create_sharded_from_blocks(const bm25x_blocks *c, uin
 // scores with the sealed segment's statistics.  The reference scans these documents one by one per query; here they
 // are inverted (term-major postings over growing ordinals) so that the same kernels unite them. ----
 
+// One sealed handle's documents as the seal reads them: the handle, the id of its local document 0 in the whole segment,
+// its documents.
+struct SealPart {
+    const bm25x_index *h;
+    uint32_t first, n;
+};
+
+// The sealed side of a growing segment: one index (ix), or a document-sharded index (sx).  It answers for the whole
+// segment (n_docs, n_terms, df, Σlen, avgdl, keys: shard 0 holds them) and names the handle the growing segment lives
+// beside, `home`: the index, or the LAST shard (device, SM count, options), where the growing documents sit in id order.
+struct SealedSide {
+    bm25x_index *ix = nullptr;
+    bm25x_sharded_index *sx = nullptr;
+
+    const bm25x_index &home() const { return sx ? *sx->shards.back() : *ix; }
+    uint32_t n_docs() const { return sx ? sx->n_docs : ix->d.n_docs; }
+    uint32_t n_terms() const { return sx ? sx->n_terms : ix->d.n_terms; }
+    const std::vector<uint32_t> &df() const { return sx ? sx->h_df : ix->h_df; }
+    const std::vector<uint8_t> &keys() const { return sx ? sx->shards[0]->h_keys : ix->h_keys; }
+    // the statistics of the whole sealed segment: the growing segment scores with them (search.rs:66-77), not its own
+    Stats stats() const {
+        const bm25x_index &h = home();
+        return sx ? Stats(sx->n_docs, sx->sum_len, sx->avgdl, sx->h_df.data(), sx->n_terms, h.k1, h.b)
+                  : Stats(ix->d.n_docs, ix->sum_len, ix->avgdl, ix->h_df.data(), ix->d.n_terms, h.k1, h.b);
+    }
+    std::vector<SealPart> parts() const {
+        if (!sx) return {{ix, 0, ix->d.n_docs}};
+        std::vector<SealPart> p;
+        for (uint32_t s = 0; s < sx->n_shards; s++)
+            p.push_back({sx->shards[s], sx->bounds[s], sx->bounds[s + 1] - sx->bounds[s]});
+        return p;
+    }
+};
+
 // Live postings of a batch of growing documents, term-major: the terms that hold any, ascending, and term[i]'s postings
 // doc / tf[off[i] .. off[i + 1]) with ordinals ascending.
 struct GrowingCsr {
@@ -1315,21 +1349,22 @@ struct GrowingCsr {
 // the BM25X_DOC_INF sentinel) and their inversion, for bm25x_growing_create and bm25x_growing_insert alike: the same codes
 // and messages.  Document i becomes ordinal first + i; `first` growing documents already exist.  A deleted document, a
 // BM25X_TERM_MISSING token and a term without sealed postings give no posting.
-static int invert_growing(const bm25x_index *sealed, const bm25x_growing_docs *g, uint32_t first, GrowingCsr &out) {
+static int invert_growing(const SealedSide &sealed, const bm25x_growing_docs *g, uint32_t first, GrowingCsr &out) {
     const char *who = "bm25x_growing_create";
-    const uint32_t G = g->n_docs, T = sealed->d.n_terms;
+    const uint32_t G = g->n_docs, T = sealed.n_terms(), NS = sealed.n_docs();
+    const std::vector<uint32_t> &sdf = sealed.df();
     if (!g->elem_off || (g->elem_off[G] && (!g->elem_term || !g->elem_tf))) {
         bm25x_set_error("%s: empty or malformed corpus", who);
         return BM25X_ERR_INVALID;
     }
-    int rc = check_common(who, G, g->doc_len ? (const void *)g->doc_len : (const void *)g->doc_fieldnorm, sealed->k1,
-                          sealed->b, sealed->device);
+    int rc = check_common(who, G, g->doc_len ? (const void *)g->doc_len : (const void *)g->doc_fieldnorm,
+                          sealed.home().k1, sealed.home().b, sealed.home().device);
     if (rc != BM25X_OK) return rc;
     // growing documents come back as sealed n_docs + ordinal (bm25x_search_batch_growing): the sum obeys check_common's
     // bound on n_docs, so that every merged id stays below the BM25X_DOC_INF sentinel
-    if ((uint64_t)sealed->d.n_docs + first + G > (uint64_t)BM25X_DOC_INF - 1u) {
+    if ((uint64_t)NS + first + G > (uint64_t)BM25X_DOC_INF - 1u) {
         bm25x_set_error("%s: sealed n_docs=%u + growing n_docs=%llu exceeds %u documents (doc ids are 32-bit, %u is reserved)",
-                        who, sealed->d.n_docs, (unsigned long long)first + G, BM25X_DOC_INF - 1u, BM25X_DOC_INF);
+                        who, NS, (unsigned long long)first + G, BM25X_DOC_INF - 1u, BM25X_DOC_INF);
         return BM25X_ERR_INVALID;
     }
     // a batch with many postings against the vocabulary is grouped by counting over every term (O(T + P)), a small one by
@@ -1356,7 +1391,7 @@ static int invert_growing(const bm25x_index *sealed, const bm25x_growing_docs *g
             if (have_prev && t <= prev) bad |= 1;
             have_prev = true;
             prev = t;
-            if (t >= T || sealed->h_df[t] == 0) continue;
+            if (t >= T || sdf[t] == 0) continue;
             if (f >= (1u << 24)) bad |= 2;
             P++;
             if (dense) cnt[(size_t)t + 1]++;
@@ -1373,7 +1408,7 @@ static int invert_growing(const bm25x_index *sealed, const bm25x_growing_docs *g
     // pass 2: invert.  Documents are visited in ascending ordinal and grouped stably, so every list comes out ascending.
     auto live = [&](uint32_t d, uint64_t e) {
         const uint32_t t = g->elem_term[e];
-        return !(g->deleted && g->deleted[d]) && t != BM25X_TERM_MISSING && t < T && sealed->h_df[t] != 0;
+        return !(g->deleted && g->deleted[d]) && t != BM25X_TERM_MISSING && t < T && sdf[t] != 0;
     };
     out = GrowingCsr();
     out.doc.resize(P);
@@ -1420,15 +1455,9 @@ static int invert_growing(const bm25x_index *sealed, const bm25x_growing_docs *g
     return BM25X_OK;
 }
 
-// Options of a growing segment's handle: the sealed index's `prune`, over the environment overrides handle_open applied,
-// so that its searches take the sealed handle's kernel paths.
-static void growing_options(bm25x_index *ix, const bm25x_index *sealed) { ix->prune = sealed->prune; }
-
-// The growing segment's scoring statistics: the SEALED segment's (search.rs:66-77), not its own.
-static Stats sealed_stats(const bm25x_index *sealed) {
-    return Stats(sealed->d.n_docs, sealed->sum_len, sealed->avgdl, sealed->h_df.data(), sealed->d.n_terms, sealed->k1,
-                 sealed->b);
-}
+// Options of a growing segment's handle: the sealed side's `prune`, over the environment overrides handle_open applied,
+// so that its searches take the sealed handles' kernel paths.
+static void growing_options(bm25x_index *ix, const SealedSide &sealed) { ix->prune = sealed.home().prune; }
 
 extern "C" int bm25x_growing_create(const bm25x_index *sealed, const bm25x_growing_docs *g, bm25x_index **out) {
     const char *who = "bm25x_growing_create";
@@ -1438,8 +1467,10 @@ extern "C" int bm25x_growing_create(const bm25x_index *sealed, const bm25x_growi
     }
     *out = nullptr;
     const uint32_t G = g->n_docs, T = sealed->d.n_terms;
+    SealedSide side;
+    side.ix = const_cast<bm25x_index *>(sealed);  // read only
     GrowingCsr csr;
-    int rc = invert_growing(sealed, g, 0, csr);
+    int rc = invert_growing(side, g, 0, csr);
     if (rc != BM25X_OK) return rc;
     std::vector<uint32_t> df(T, 0);
     std::vector<uint64_t> off((size_t)T + 1, 0);
@@ -1449,21 +1480,21 @@ extern "C" int bm25x_growing_create(const bm25x_index *sealed, const bm25x_growi
     BuildMeta m{G, T, g->doc_len, g->payload, sealed->h_keys.empty() ? nullptr : sealed->h_keys.data(), sealed->k1,
                 sealed->b, df.data(), P};
     m.fieldnorm = g->doc_fieldnorm;
-    const Stats st = sealed_stats(sealed);
+    const Stats st = side.stats();
     IndexGuard ix;
     rc = index_begin(m, &st, sealed->device, ix);
     if (rc == BM25X_OK) rc = upload_csr(ix.get(), who, T, P, off.data(), csr.doc.data(), csr.tf.data());
     if (rc != BM25X_OK) return rc;
-    growing_options(ix.get(), sealed);
+    growing_options(ix.get(), side);
     *out = ix.release();
     return BM25X_OK;
 }
 
 // ---- the mutable growing segment (DESIGN §4.5): the documents on the host as the reference's VectorTuples keep them
-// (norm, payload, deleted bit), their postings in one index handle on the sealed index's device, brought up to date by a
-// refresh ----
+// (norm, payload, deleted bit), their postings in one index handle on the sealed side's home device, brought up to date
+// by a refresh ----
 struct bm25x_growing_segment {
-    bm25x_index *sealed;
+    SealedSide sealed;
     Stats stats;                       // the sealed segment's, computed once
     mutable std::mutex mu;             // guards everything below; a refresh runs under it
     int norm_form = -1;                // -1: no insert yet; 1: doc_len; 0: doc_fieldnorm
@@ -1489,7 +1520,7 @@ struct bm25x_growing_segment {
     // replace it meanwhile and the last holder destroys it
     std::shared_ptr<bm25x_index> cur;
 
-    explicit bm25x_growing_segment(bm25x_index *s) : sealed(s), stats(sealed_stats(s)) {}
+    explicit bm25x_growing_segment(const SealedSide &s) : sealed(s), stats(s.stats()) {}
     uint32_t n_docs() const { return (uint32_t)deleted.size(); }
 };
 
@@ -1503,7 +1534,21 @@ extern "C" int bm25x_growing_open(bm25x_index *sealed, bm25x_growing_segment **o
         bm25x_set_error("bm25x_growing_open: replica not finalized (bm25x_index_finalize_replica)");
         return BM25X_ERR_INVALID;
     }
-    *out = new bm25x_growing_segment(sealed);
+    SealedSide side;
+    side.ix = sealed;
+    *out = new bm25x_growing_segment(side);
+    return BM25X_OK;
+}
+
+extern "C" int bm25x_growing_open_sharded(bm25x_sharded_index *sealed, bm25x_growing_segment **out) {
+    if (!sealed || !out) {
+        bm25x_set_error("bm25x_growing_open_sharded: null argument");
+        return BM25X_ERR_INVALID;
+    }
+    *out = nullptr;
+    SealedSide side;
+    side.sx = sealed;
+    *out = new bm25x_growing_segment(side);
     return BM25X_OK;
 }
 
@@ -1550,8 +1595,8 @@ extern "C" int bm25x_growing_insert(bm25x_growing_segment *g, const bm25x_growin
     g->pend_doc.insert(g->pend_doc.end(), csr.doc.begin(), csr.doc.end());
     g->pend_tf.insert(g->pend_tf.end(), csr.tf.begin(), csr.tf.end());
     // the seal's share: dormant postings, Σ tf (doc_fieldnorm form), new ordinals
-    const bm25x_index *sealed = g->sealed;
-    const uint32_t T = sealed->d.n_terms;
+    const uint32_t T = g->sealed.n_terms();
+    const std::vector<uint32_t> &sdf = g->sealed.df();
     for (uint32_t d = 0; d < G; d++) {
         const bool live = !(docs->deleted && docs->deleted[d]);
         uint64_t sum = 0;
@@ -1563,7 +1608,7 @@ extern "C" int bm25x_growing_insert(bm25x_growing_segment *g, const bm25x_growin
                 g->new_terms.push_back(t);
                 g->term_end = std::max(g->term_end, t + 1);
             }
-            if (live && (t >= T || sealed->h_df[t] == 0)) {
+            if (live && (t >= T || sdf[t] == 0)) {
                 g->dorm_term.push_back(t);
                 g->dorm_doc.push_back(first + d);
                 g->dorm_tf.push_back(docs->elem_tf[e]);
@@ -1683,9 +1728,10 @@ static int splice_finish(Scratch &sc, const char *who, bm25x_index *ix, const ui
 static int growing_refresh_locked(bm25x_growing_segment *g) {
     const char *who = "bm25x_growing_refresh";
     if (!g->pending) return BM25X_OK;
-    const bm25x_index *sealed = g->sealed;
-    const uint32_t N = g->n_docs(), T = sealed->d.n_terms;
-    const int device = sealed->device;
+    const bm25x_index &home = g->sealed.home();
+    const std::vector<uint8_t> &keys = g->sealed.keys();
+    const uint32_t N = g->n_docs(), T = g->sealed.n_terms();
+    const int device = home.device;
     // ---- the sources: the current handle's lists, then the postings inserted since, against the deleted ordinals ----
     Scratch sc(device);
     sc.e = cudaSetDevice(device);
@@ -1695,19 +1741,19 @@ static int growing_refresh_locked(bm25x_growing_segment *g) {
     src.s[0] = handle_source(g->cur.get(), d_del, nullptr);
     src.s[1] = grouped_source(sc, T, g->pend_term, g->pend_doc, g->pend_tf, d_del, nullptr);
     // ---- new df: the survivors of the current lists and of the inserted ones ----
-    const std::vector<uint32_t> df = splice_count(sc, sealed->sm_count, T, src);
+    const std::vector<uint32_t> df = splice_count(sc, home.sm_count, T, src);
     if (sc.e != cudaSuccess) return cuda_refusal(who, "count", sc.e);
     uint64_t P = 0;
     for (uint32_t t = 0; t < T; t++) P += df[t];
     // ---- the new handle, built as bm25x_growing_create builds one over all N ordinals ----
-    BuildMeta m{N, T, g->norm_form ? g->doc_len.data() : nullptr, g->payload.data(),
-                sealed->h_keys.empty() ? nullptr : sealed->h_keys.data(), sealed->k1, sealed->b, df.data(), P};
+    BuildMeta m{N, T, g->norm_form ? g->doc_len.data() : nullptr, g->payload.data(), keys.empty() ? nullptr : keys.data(),
+                home.k1, home.b, df.data(), P};
     m.fieldnorm = g->norm_form ? nullptr : g->fieldnorm.data();
     IndexGuard ix;
     int rc = index_begin(m, &g->stats, device, ix);
     if (rc == BM25X_OK) rc = splice_finish(sc, who, ix.get(), nullptr, src);
     if (rc != BM25X_OK) return rc;
-    growing_options(ix.get(), sealed);
+    growing_options(ix.get(), g->sealed);
     g->cur.reset(ix.release(), IndexDestroy());
     std::vector<uint32_t>().swap(g->pend_term);
     std::vector<uint32_t>().swap(g->pend_doc);
@@ -1737,7 +1783,7 @@ extern "C" int bm25x_growing_get_info(const bm25x_growing_segment *g, bm25x_grow
     out->n_postings = g->cur ? g->cur->d.n_post : 0;
     out->device_bytes = g->cur ? g->cur->device_bytes : 0;
     out->pending = g->pending ? 1u : 0u;
-    out->device = g->sealed->device;
+    out->device = g->sealed.home().device;
     return BM25X_OK;
 }
 
@@ -1778,22 +1824,29 @@ extern "C" int bm25x_growing_search_batch(bm25x_growing_segment *g, uint32_t nq,
         if (rc != BM25X_OK) return rc;
         cur = g->cur;
     }
+    const ResultRows host{out_doc, out_score, out_score64, out_payload, out_n};
+    bm25x_sharded_index *sx = g->sealed.sx;
     if (!cur)  // nothing inserted yet: the sealed search alone
-        return bm25x_search_batch(g->sealed, nq, q_off, q_terms, k, allow_sealed, out_doc, out_score, out_score64,
-                                  out_payload, out_n, stats);
-    bm25x_index *ix[2] = {g->sealed, cur.get()};
-    const uint32_t base[2] = {0, g->sealed->d.n_docs};
-    const uint8_t *allow[2] = {allow_sealed, nullptr};
+        return sx ? bm25x_sharded_search_batch(sx, nq, q_off, q_terms, k, allow_sealed, out_doc, out_score, out_score64,
+                                               out_payload, out_n, stats)
+                  : bm25x_search_batch(g->sealed.ix, nq, q_off, q_terms, k, allow_sealed, out_doc, out_score, out_score64,
+                                       out_payload, out_n, stats);
     std::vector<uint8_t> ag;  // allow_growing over the handle's ordinals: the caller's bits below allow_growing_docs
     if (allow_growing) {
         const uint32_t N = cur->d.n_docs, n = std::min(N, allow_growing_docs);
         ag.assign(((size_t)N + 7) / 8, 0);
         std::copy(allow_growing, allow_growing + ((size_t)n + 7) / 8, ag.begin());
         if (n & 7u) ag[n >> 3] &= (uint8_t)((1u << (n & 7u)) - 1u);
-        allow[1] = ag.data();
     }
-    return bm25x_merged_search("bm25x_growing_search_batch", 2, ix, base, allow, nq, q_off, q_terms, k,
-                               {out_doc, out_score, out_score64, out_payload, out_n}, stats, t0, nullptr);
+    const uint8_t *alg = allow_growing ? ag.data() : nullptr;
+    if (sx)
+        return bm25x_sharded_merged_search("bm25x_growing_search_batch", sx, cur.get(), alg, nq, q_off, q_terms, k,
+                                           allow_sealed, host, stats, t0);
+    bm25x_index *ix[2] = {g->sealed.ix, cur.get()};
+    const uint32_t base[2] = {0, g->sealed.n_docs()};
+    const uint8_t *allow[2] = {allow_sealed, alg};
+    return bm25x_merged_search("bm25x_growing_search_batch", 2, ix, base, allow, nq, q_off, q_terms, k, host, stats, t0,
+                               nullptr);
 }
 
 // ---- the seal (`maintain`, maintain.rs:27-311; DESIGN §4.5): a new sealed index from the sealed survivors and the
@@ -1809,23 +1862,31 @@ struct SealSnapshot {
     std::vector<uint32_t> dorm_term, dorm_doc, dorm_tf;
 };
 
-extern "C" int bm25x_growing_seal(bm25x_growing_segment *g, bm25x_seal_args *a, bm25x_index **out) {
-    const char *who = "bm25x_growing_seal";
-    if (!g || !a || !out || (a->n_new_keys && !a->new_keys)) {
-        bm25x_set_error("%s: null argument", who);
-        return BM25X_ERR_INVALID;
-    }
-    *out = nullptr;
-    const bm25x_index *sealed = g->sealed;
-    const uint32_t NS = sealed->d.n_docs, T = sealed->d.n_terms, K = a->n_new_keys;
-    const int device = sealed->device;
-    const bool keyed = !sealed->h_keys.empty();
+// The new segment of a seal: its handles in id order (one per sealed part that keeps a document), their bounds, and what
+// it answers as a whole.
+struct SealResult {
+    std::vector<IndexGuard> shards;
+    std::vector<uint32_t> bounds;  // [shards + 1]
+    uint32_t n_docs = 0, n_terms = 0;
+    uint64_t n_post = 0, sum_len = 0;
+    double k1 = 1.2, b = 0.75, avgdl = 0;
+    std::vector<uint32_t> df;
+};
+
+// The seal of g over its sealed side's parts (one index: one part; a document-sharded index: its shards).  New part j
+// holds the survivors of an old part in ascending old id, the last one also the growing survivors after its own; a part
+// left without a document is dropped.  Each part is counted and spliced on its own device from its own arrays; the host
+// sums df over the parts, settles the vocabulary and builds ONE Stats for the new segment, with which every new handle
+// is opened.  Refusals and maps are bm25x_growing_seal's, named by `who`.
+static int seal_segment(const char *who, bm25x_growing_segment *g, bm25x_seal_args *a, SealResult &out) {
+    const uint32_t NS = g->sealed.n_docs(), T = g->sealed.n_terms(), K = a->n_new_keys;
+    const bool keyed = !g->sealed.keys().empty();
     // ---- the new keys: each unlike every sealed key and every other new key ----
     if (a->new_keys && !keyed) {
         bm25x_set_error("%s: new_keys given, but the sealed index was created without term keys", who);
         return BM25X_ERR_INVALID;
     }
-    const uint8_t *skeys = sealed->h_keys.data();
+    const uint8_t *skeys = g->sealed.keys().data();
     auto key_of = [&](uint32_t t) { return t < T ? skeys + (size_t)t * 16 : a->new_keys + (size_t)(t - T) * 16; };
     auto key_less = [&](uint32_t x, uint32_t y) { return memcmp(key_of(x), key_of(y), 16) < 0; };
     if (K) {
@@ -1902,42 +1963,71 @@ extern "C" int bm25x_growing_seal(bm25x_growing_segment *g, bm25x_seal_args *a, 
     std::vector<uint32_t> gmap(NG);
     uint32_t N = ns_keep;
     for (uint32_t o = 0; o < NG; o++) gmap[o] = s.deleted[o] ? BM25X_DOC_INF : N++;
-    // ---- the sources: the sealed lists, the growing handle's, the dormant postings; the deleted bitmaps and the maps ----
-    std::vector<uint32_t> sbits(((size_t)NS + 31) / 32, 0);
-    if (a->sealed_deleted) memcpy(sbits.data(), a->sealed_deleted, ((size_t)NS + 7) / 8);  // little-endian: bit d of word d >> 5
-    const std::vector<uint32_t> gbits = deleted_bitmap(s.deleted);
-    Scratch sc(device);
-    sc.e = cudaSetDevice(device);
-    const uint32_t *d_sdel = sc.up(sbits.data(), sbits.size()), *d_gdel = sc.up(gbits.data(), gbits.size());
-    const uint32_t *d_gmap = sc.up(gmap.data(), NG);
-    SpliceSources src{};
-    src.s[0] = handle_source(sealed, d_sdel, sc.up(smap.data(), NS));
-    src.s[1] = handle_source(s.cur.get(), d_gdel, d_gmap);
-    src.s[2] = grouped_source(sc, n_src, s.dorm_term, s.dorm_doc, s.dorm_tf, d_gdel, d_gmap);
-    // ---- rule 3 lengths and rule 5 df on the device ----
-    uint32_t *d_cnt = sc.alloc<uint32_t>(NS);
-    const DeviceIndex &sd = sealed->d;
-    if (sc.e == cudaSuccess) sc.e = cudaMemset(d_cnt, 0, sizeof(uint32_t) * (size_t)NS);
-    if (sc.e == cudaSuccess && T) {
-        k_seal_doc_postings<<<splice_grid(T, sealed->sm_count), 256>>>(T, sd.pdoc, sd.post_off, sd.df, d_sdel, d_cnt);
-        sc.e = cudaGetLastError();
+    // ---- per part: its survivors' new ids [new_lo, new_lo + n_new) (the last part's include the growing survivors) ----
+    const std::vector<SealPart> parts = g->sealed.parts();
+    const uint32_t NP = (uint32_t)parts.size();
+    std::vector<uint32_t> new_lo(NP + 1, 0);
+    for (uint32_t p = 0; p < NP; p++) {
+        uint32_t kept = 0;
+        for (uint32_t d = parts[p].first; d < parts[p].first + parts[p].n; d++) kept += smap[d] != BM25X_DOC_INF;
+        new_lo[p + 1] = new_lo[p] + kept;
     }
-    const std::vector<uint32_t> df_src = splice_count(sc, sealed->sm_count, n_src, src);
-    std::vector<uint32_t> cnt(NS);
-    std::vector<uint16_t> spay((size_t)NS * 3);
-    if (sc.e == cudaSuccess) sc.e = cudaMemcpy(cnt.data(), d_cnt, sizeof(uint32_t) * (size_t)NS, cudaMemcpyDeviceToHost);
-    if (sc.e == cudaSuccess)
-        sc.e = cudaMemcpy(spay.data(), sd.payload, sizeof(uint16_t) * 3 * (size_t)NS, cudaMemcpyDeviceToHost);
-    if (sc.e != cudaSuccess) return cuda_refusal(who, "count", sc.e);
-    // ---- rules 2-4: per new document its length and its stored payload ----
-    std::vector<uint32_t> len(N);
+    new_lo[NP] = N;
+    // ---- per part, on its own device with its local ids: the sources (its sealed lists; the last part also the growing
+    // handle's and the dormant postings), the local deleted bitmaps and maps, rule 3 lengths and rule 5 df ----
+    const std::vector<uint32_t> gbits = deleted_bitmap(s.deleted);
+    std::vector<std::unique_ptr<Scratch>> scs(NP);
+    std::vector<SpliceSources> srcs(NP);
+    std::vector<std::vector<uint32_t>> df_part(NP);
+    std::vector<uint32_t> df_src(n_src, 0), len(N);
     std::vector<uint16_t> pay((size_t)N * 3);
-#pragma omp parallel for schedule(static) num_threads(bm25x_host_threads(0))
-    for (uint32_t d = 0; d < NS; d++)
-        if (smap[d] != BM25X_DOC_INF) {
-            len[smap[d]] = cnt[d];
-            memcpy(&pay[(size_t)smap[d] * 3], &spay[(size_t)d * 3], 6);
+    for (uint32_t p = 0; p < NP; p++) {
+        const SealPart &pt = parts[p];
+        const bool last = p + 1 == NP;
+        Scratch &sc = *(scs[p] = std::make_unique<Scratch>(pt.h->device));
+        sc.e = cudaSetDevice(pt.h->device);
+        std::vector<uint32_t> sbits(((size_t)pt.n + 31) / 32, 0), lmap(pt.n);
+        for (uint32_t d = 0; d < pt.n; d++) {
+            const uint32_t nd = smap[pt.first + d];
+            lmap[d] = nd == BM25X_DOC_INF ? nd : nd - new_lo[p];
+            if (nd == BM25X_DOC_INF) sbits[d >> 5] |= 1u << (d & 31);
         }
+        const uint32_t *d_sdel = sc.up(sbits.data(), sbits.size());
+        SpliceSources &src = srcs[p];
+        src = SpliceSources{};
+        src.s[0] = handle_source(pt.h, d_sdel, sc.up(lmap.data(), pt.n));
+        if (last) {
+            std::vector<uint32_t> glmap(NG);
+            for (uint32_t o = 0; o < NG; o++) glmap[o] = gmap[o] == BM25X_DOC_INF ? gmap[o] : gmap[o] - new_lo[p];
+            const uint32_t *d_gdel = sc.up(gbits.data(), gbits.size()), *d_gmap = sc.up(glmap.data(), NG);
+            src.s[1] = handle_source(s.cur.get(), d_gdel, d_gmap);
+            src.s[2] = grouped_source(sc, n_src, s.dorm_term, s.dorm_doc, s.dorm_tf, d_gdel, d_gmap);
+        }
+        uint32_t *d_cnt = sc.alloc<uint32_t>(pt.n);
+        const DeviceIndex &sd = pt.h->d;
+        if (sc.e == cudaSuccess) sc.e = cudaMemset(d_cnt, 0, sizeof(uint32_t) * (size_t)pt.n);
+        if (sc.e == cudaSuccess && T) {
+            k_seal_doc_postings<<<splice_grid(T, pt.h->sm_count), 256>>>(T, sd.pdoc, sd.post_off, sd.df, d_sdel, d_cnt);
+            sc.e = cudaGetLastError();
+        }
+        df_part[p] = splice_count(sc, pt.h->sm_count, n_src, src);
+        std::vector<uint32_t> cnt(pt.n);
+        std::vector<uint16_t> spay((size_t)pt.n * 3);
+        if (sc.e == cudaSuccess) sc.e = cudaMemcpy(cnt.data(), d_cnt, sizeof(uint32_t) * (size_t)pt.n, cudaMemcpyDeviceToHost);
+        if (sc.e == cudaSuccess)
+            sc.e = cudaMemcpy(spay.data(), sd.payload, sizeof(uint16_t) * 3 * (size_t)pt.n, cudaMemcpyDeviceToHost);
+        if (sc.e != cudaSuccess) return cuda_refusal(who, "count", sc.e);
+        for (uint32_t t = 0; t < n_src; t++) df_src[t] += df_part[p][t];
+        // ---- rules 2-4: per new document its length and its stored payload ----
+#pragma omp parallel for schedule(static) num_threads(bm25x_host_threads(0))
+        for (uint32_t d = 0; d < pt.n; d++) {
+            const uint32_t nd = smap[pt.first + d];
+            if (nd != BM25X_DOC_INF) {
+                len[nd] = cnt[d];
+                memcpy(&pay[(size_t)nd * 3], &spay[(size_t)d * 3], 6);
+            }
+        }
+    }
     for (uint32_t o = 0; o < NG; o++)
         if (gmap[o] != BM25X_DOC_INF) {
             len[gmap[o]] = s.len[o];
@@ -1956,26 +2046,100 @@ extern "C" int bm25x_growing_seal(bm25x_growing_segment *g, bm25x_seal_args *a, 
     const uint32_t TN = (uint32_t)src_of.size();
     std::vector<uint32_t> df(TN), tmap(n_src, BM25X_TERM_MISSING);
     std::vector<uint8_t> keys(keyed ? (size_t)TN * 16 : 0);
-    uint64_t P = 0;
+    uint64_t P = 0, sum_len = 0;
     for (uint32_t j = 0; j < TN; j++) {
         df[j] = df_src[src_of[j]];
         tmap[src_of[j]] = j;
         P += df[j];
         if (keyed) memcpy(&keys[(size_t)j * 16], key_of(src_of[j]), 16);
     }
-    // ---- rule 5 and 7: the new handle with its own statistics, the postings spliced into it, then what every index
-    // derives from them ----
-    BuildMeta m{N, TN, len.data(), pay.data(), keyed ? keys.data() : nullptr, sealed->k1, sealed->b, df.data(), P};
-    IndexGuard ix;
-    int rc = index_begin(m, nullptr, device, ix);
-    if (rc == BM25X_OK) rc = splice_finish(sc, who, ix.get(), sc.up(src_of.data(), TN), src);
-    if (rc != BM25X_OK) return rc;
+    for (uint32_t d = 0; d < N; d++) sum_len += len[d];
+    // ---- rules 5 and 7: ONE set of statistics for the new segment; per part that keeps a document, a new handle on its
+    // device scoring with them, its survivors spliced into it, then what every index derives from them ----
+    const double k1 = g->sealed.home().k1, b = g->sealed.home().b;
+    const Stats st(N, sum_len, df.data(), TN, k1, b);
+    SealResult res;
+    res.bounds.push_back(0);
+    for (uint32_t p = 0; p < NP; p++) {
+        const uint32_t lo = new_lo[p], n = new_lo[p + 1] - lo;
+        if (!n) continue;  // a part left without a document is dropped
+        std::vector<uint32_t> dfp(TN);
+        uint64_t Pp = 0;
+        for (uint32_t j = 0; j < TN; j++) Pp += dfp[j] = df_part[p][src_of[j]];
+        // (the term keys once, with the new shard 0)
+        BuildMeta m{n, TN, len.data() + lo, pay.data() + (size_t)lo * 3, keyed && res.shards.empty() ? keys.data() : nullptr,
+                    k1, b, dfp.data(), Pp};
+        IndexGuard ix;
+        Scratch &sc = *scs[p];
+        int rc = index_begin(m, &st, parts[p].h->device, ix);
+        if (rc == BM25X_OK) rc = splice_finish(sc, who, ix.get(), sc.up(src_of.data(), TN), srcs[p]);
+        if (rc != BM25X_OK) return rc;
+        res.shards.push_back(std::move(ix));
+        res.bounds.push_back(lo + n);
+    }
+    res.n_docs = N;
+    res.n_terms = TN;
+    res.n_post = P;
+    res.k1 = k1;
+    res.b = b;
+    res.df = std::move(df);
+    res.sum_len = sum_len;
+    res.avgdl = st.avgdl;
     a->n_growing = NG;
     a->n_source_terms = n_src;
     if (a->sealed_map) std::copy(smap.begin(), smap.end(), a->sealed_map);
     if (a->growing_map) std::copy(gmap.begin(), gmap.end(), a->growing_map);
     if (a->term_map) std::copy(tmap.begin(), tmap.end(), a->term_map);
-    *out = ix.release();
+    out = std::move(res);
+    return BM25X_OK;
+}
+
+extern "C" int bm25x_growing_seal(bm25x_growing_segment *g, bm25x_seal_args *a, bm25x_index **out) {
+    const char *who = "bm25x_growing_seal";
+    if (!g || !a || !out || (a->n_new_keys && !a->new_keys)) {
+        bm25x_set_error("%s: null argument", who);
+        return BM25X_ERR_INVALID;
+    }
+    *out = nullptr;
+    if (g->sealed.sx) {
+        bm25x_set_error("%s: the segment was opened over a document-sharded index: seal it with bm25x_growing_seal_sharded",
+                        who);
+        return BM25X_ERR_INVALID;
+    }
+    SealResult res;
+    const int rc = seal_segment(who, g, a, res);
+    if (rc != BM25X_OK) return rc;
+    *out = res.shards[0].release();
+    return BM25X_OK;
+}
+
+extern "C" int bm25x_growing_seal_sharded(bm25x_growing_segment *g, bm25x_seal_args *a, bm25x_sharded_index **out) {
+    const char *who = "bm25x_growing_seal_sharded";
+    if (!g || !a || !out || (a->n_new_keys && !a->new_keys)) {
+        bm25x_set_error("%s: null argument", who);
+        return BM25X_ERR_INVALID;
+    }
+    *out = nullptr;
+    if (!g->sealed.sx) {
+        bm25x_set_error("%s: the segment was opened over an unsharded index: seal it with bm25x_growing_seal", who);
+        return BM25X_ERR_INVALID;
+    }
+    SealResult res;
+    const int rc = seal_segment(who, g, a, res);
+    if (rc != BM25X_OK) return rc;
+    bm25x_sharded_index *sx = new bm25x_sharded_index();
+    sx->n_shards = (uint32_t)res.shards.size();
+    sx->bounds = std::move(res.bounds);
+    for (IndexGuard &ix : res.shards) sx->shards.push_back(ix.release());
+    sx->n_docs = res.n_docs;
+    sx->n_terms = res.n_terms;
+    sx->n_post = res.n_post;
+    sx->k1 = res.k1;
+    sx->b = res.b;
+    sx->h_df = std::move(res.df);
+    sx->sum_len = res.sum_len;
+    sx->avgdl = res.avgdl;
+    *out = sx;
     return BM25X_OK;
 }
 

@@ -17,12 +17,12 @@ namespace {
 // shard s', the rows of s' ranked before it: score64 >= x for s' < s (equal scores: lower doc ranges first), score64 > x
 // for s' > s.  Every row ranks itself — no sort, no shared state; the ranks of the Σ n_s rows are a permutation.
 struct ShardRows {
-    const uint32_t *doc[BM25X_MAX_SHARDS];
-    const float *score[BM25X_MAX_SHARDS];
-    const double *score64[BM25X_MAX_SHARDS];
-    const uint16_t *payload[BM25X_MAX_SHARDS];
-    const uint32_t *n[BM25X_MAX_SHARDS];
-    uint32_t base[BM25X_MAX_SHARDS];
+    const uint32_t *doc[BM25X_MAX_LISTS];
+    const float *score[BM25X_MAX_LISTS];
+    const double *score64[BM25X_MAX_LISTS];
+    const uint16_t *payload[BM25X_MAX_LISTS];
+    const uint32_t *n[BM25X_MAX_LISTS];
+    uint32_t base[BM25X_MAX_LISTS];
 };
 
 // rows of a descending list that come before x: score > x (strict) or score >= x (!strict)
@@ -130,6 +130,10 @@ int bm25x_merged_search(const char *who, uint32_t S, bm25x_index *const *handles
                         uint32_t k, const ResultRows &host, bm25x_search_stats *stats,
                         std::chrono::steady_clock::time_point t0, uint32_t *live) {
     using clk = std::chrono::steady_clock;
+    if (S == 0 || S > BM25X_MAX_LISTS) {
+        bm25x_set_error("%s: %u lists to merge, must be 1..%d", who, S, BM25X_MAX_LISTS);
+        return BM25X_ERR_INVALID;
+    }
     bm25x_index *ix0 = handles[0];
     const int dev0 = ix0->device;
     cudaStream_t ms = ix0->stream;  // the merge runs behind handle 0's kernels on its library stream
@@ -214,15 +218,10 @@ int bm25x_merged_search(const char *who, uint32_t S, bm25x_index *const *handles
     return cleanup(rc);
 }
 
-extern "C" int bm25x_sharded_search_batch(bm25x_sharded_index *sx, uint32_t nq, const uint32_t *q_off,
-                                          const uint32_t *q_terms, uint32_t k, const uint8_t *allow, uint32_t *out_doc,
-                                          float *out_score, double *out_score64, uint16_t *out_payload, uint32_t *out_n,
-                                          bm25x_search_stats *stats) {
-    if (!sx) {
-        bm25x_set_error("bm25x_sharded_search_batch: null argument");
-        return BM25X_ERR_INVALID;
-    }
-    const auto t0 = std::chrono::steady_clock::now();
+int bm25x_sharded_merged_search(const char *who, bm25x_sharded_index *sx, bm25x_index *growing,
+                                const uint8_t *allow_growing, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms,
+                                uint32_t k, const uint8_t *allow, const ResultRows &host, bm25x_search_stats *stats,
+                                std::chrono::steady_clock::time_point t0) {
     // ---- the refusals of bm25x_search_batch: its argument checks, then its canonicalisation slice by slice against the
     // WHOLE segment's df (a query with 65 live terms is refused even when no shard sees more than 64) ----
     if (nq && (!q_off || (!q_terms && q_off[nq] != 0))) {
@@ -249,17 +248,37 @@ extern "C" int bm25x_sharded_search_batch(bm25x_sharded_index *sx, uint32_t nq, 
         }
     }
     if (rc != BM25X_OK) return rc;
-    const uint32_t S = sx->n_shards;
+    const uint32_t S = sx->n_shards, L = S + (growing ? 1u : 0u);
     std::vector<std::vector<uint8_t>> al(allow ? S : 0);
-    std::vector<const uint8_t *> as(S, nullptr);
+    std::vector<const uint8_t *> as(L, nullptr);
     for (uint32_t s = 0; s < S && allow; s++) {
         al[s] = allow_slice(allow, sx->n_docs, sx->bounds[s], sx->bounds[s + 1]);
         as[s] = al[s].data();
     }
-    rc = bm25x_merged_search("bm25x_sharded_search_batch", S, sx->shards.data(), sx->bounds.data(), as.data(), nq, q_off,
-                             q_terms, k, {out_doc, out_score, out_score64, out_payload, out_n}, stats, t0, nullptr);
-    if (rc == BM25X_OK && stats) stats->queries = n_live;
+    // the lists: the shards at their bounds, then the growing handle at n_docs(sx) (= bounds[S])
+    std::vector<bm25x_index *> hs(sx->shards.begin(), sx->shards.end());
+    if (growing) {
+        hs.push_back(growing);
+        as[S] = allow_growing;
+    }
+    std::vector<uint32_t> live(L, 0);
+    rc = bm25x_merged_search(who, L, hs.data(), sx->bounds.data(), as.data(), nq, q_off, q_terms, k, host, stats, t0,
+                             live.data());
+    if (rc == BM25X_OK && stats) stats->queries = n_live + (growing ? live[S] : 0u);
     return rc;
+}
+
+extern "C" int bm25x_sharded_search_batch(bm25x_sharded_index *sx, uint32_t nq, const uint32_t *q_off,
+                                          const uint32_t *q_terms, uint32_t k, const uint8_t *allow, uint32_t *out_doc,
+                                          float *out_score, double *out_score64, uint16_t *out_payload, uint32_t *out_n,
+                                          bm25x_search_stats *stats) {
+    if (!sx) {
+        bm25x_set_error("bm25x_sharded_search_batch: null argument");
+        return BM25X_ERR_INVALID;
+    }
+    return bm25x_sharded_merged_search("bm25x_sharded_search_batch", sx, nullptr, nullptr, nq, q_off, q_terms, k, allow,
+                                       {out_doc, out_score, out_score64, out_payload, out_n}, stats,
+                                       std::chrono::steady_clock::now());
 }
 
 // ---- test / measurement hook: the merge kernel alone on host rows ----

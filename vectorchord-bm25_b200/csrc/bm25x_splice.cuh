@@ -6,7 +6,8 @@
 // map) are above every earlier source's, so a term's survivors stay ascending when written source by source:
 //   - refresh: the current growing handle's list, then the pending list;
 //   - seal: the sealed handle's list, then the growing handle's, then the dormant list (the postings the growing handle
-//     leaves out: terms >= the sealed n_terms, terms without sealed postings).
+//     leaves out: terms >= the sealed n_terms, terms without sealed postings).  Over a document-sharded index each old
+//     shard is one such splice on its own device, with local ids; only the last one has the growing sources.
 // A posting survives when its document is not deleted.  Every kernel takes one warp per term.
 #pragma once
 

@@ -10,7 +10,7 @@
 // layout {doc, tf << 8 | fieldnorm(doc)}.
 #pragma once
 
-#include "bm25x_common.h"
+#include "bm25x_build.h"
 
 namespace {
 
@@ -18,18 +18,6 @@ namespace {
 #define BM25X_BLKERR_TF 2u     // tf >= 2^24
 #define BM25X_BLKERR_DIR 4u    // a staged directory entry that does not describe a payload inside the staged bytes
 #define BM25X_BLKERR_WAND 8u   // SummaryTuple.wand_* is not the block's arg-max
-
-// Owner of index g in an ascending offset array off[0..n]: the last t with off[t] <= g (the term of a posting, the token of a
-// block).
-__device__ __forceinline__ uint32_t owner_of(const uint64_t *__restrict__ off, uint32_t n, uint64_t g) {
-    uint32_t lo = 0, hi = n;
-    while (lo < hi) {
-        const uint32_t mid = (lo + hi + 1) >> 1;
-        if (off[mid] <= g) lo = mid;
-        else hi = mid - 1;
-    }
-    return lo;
-}
 
 __device__ __forceinline__ uint32_t sm_u32(const uint8_t *p) {  // payloads are byte-aligned only
     return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24);
@@ -101,24 +89,6 @@ __device__ __forceinline__ uint32_t posting_errors(uint32_t doc, uint32_t tf, ui
     if (tf >= (1u << 24)) bad |= BM25X_BLKERR_TF;
     return bad;
 }
-
-// Cache::evaluate (bm25.rs:355-358) of term frequency tf in a document of norm fn.  The explicit roundings keep the bits
-// of every build kernel the same whatever the compiler contracts.
-__device__ __forceinline__ double tf_score(uint32_t tf, uint32_t fn, double s0, const double *__restrict__ s1d) {
-    const double tfd = (double)tf;
-    return __ddiv_rn(__dmul_rn(tfd, s0), __dadd_rn(tfd, s1d[fn]));
-}
-
-// The same of a packed posting word w = tf << 8 | fieldnorm.
-__device__ __forceinline__ double posting_score(uint32_t w, double s0, const double *__restrict__ s1d) {
-    return tf_score(w >> 8, w & 0xFFu, s0, s1d);
-}
-
-// Score bounds are inflated by 2^-40 so that they also dominate any later re-association of the f64 sum.
-constexpr double UB_INFLATE = 1.0 + 9.094947017729282e-13;
-
-// A block's bound as stored: the inflated score rounded up to f32.
-__device__ __forceinline__ float block_bound(double v) { return __double2float_ru(v * UB_INFLATE); }
 
 // The stored SummaryTuple.(wand_fieldnorm, wand_term_frequency) of a block against the block's bound blk_ub (k_block_desc's
 // block_bound): tf() and Cache::evaluate round differently, so the last f32 ulp either way is allowed.  wand_tf is a full
@@ -366,3 +336,15 @@ k_decode_shard_blocks(uint64_t n_blocks, const uint64_t *__restrict__ sel_off, u
 }
 
 }  // namespace
+
+// Ingest check: the stored SummaryTuple.(wand_fieldnorm, wand_term_frequency) of a block must evaluate to the block's
+// real maximum (it is the arg-max of the block's own postings, flush.rs:101-110); anything else is a corrupt index.
+__global__ void k_check_block_wand(uint64_t n_blocks, const uint64_t *__restrict__ blk_off, uint32_t n_terms,
+                                   const uint8_t *__restrict__ wand_fn, const uint32_t *__restrict__ wand_tf,
+                                   const double *__restrict__ s0d, const double *__restrict__ s1d,
+                                   const float *__restrict__ blk_ub, uint32_t *__restrict__ err) {
+    uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= n_blocks) return;
+    const uint32_t t = owner_of(blk_off, n_terms, g);
+    if (!wand_pair_ok(wand_tf[g], wand_fn[g], s0d[t], s1d, blk_ub[g])) atomicOr(err, BM25X_BLKERR_WAND);
+}

@@ -1,0 +1,177 @@
+// bm25x_build.h — the build contract of every index handle, internal to the library (DESIGN §3).
+//
+// A builder opens the handle with index_begin (df, statistics, norms, payloads: every array but the postings), writes the
+// postings at their padded offsets d.post_off, then calls index_finish_device (pad slots, doc-id copy, block descriptors,
+// score bounds, champion lists).  Builders: the CSR builds (bm25x_index.cu), the stored-block ingests (bm25x_blocks.cu),
+// the growing segment's create, refresh and seal (bm25x_growing.cu).
+#pragma once
+
+#include <memory>
+#include <vector>
+
+#include "bm25x_common.h"
+
+namespace {
+
+// Owner of index g in an ascending offset array off[0..n]: the last t with off[t] <= g (the term of a posting, the token of a
+// block).
+__device__ __forceinline__ uint32_t owner_of(const uint64_t *__restrict__ off, uint32_t n, uint64_t g) {
+    uint32_t lo = 0, hi = n;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1) >> 1;
+        if (off[mid] <= g) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+
+// Cache::evaluate (bm25.rs:355-358) of term frequency tf in a document of norm fn.  The explicit roundings keep the bits
+// of every build kernel the same whatever the compiler contracts.
+__device__ __forceinline__ double tf_score(uint32_t tf, uint32_t fn, double s0, const double *__restrict__ s1d) {
+    const double tfd = (double)tf;
+    return __ddiv_rn(__dmul_rn(tfd, s0), __dadd_rn(tfd, s1d[fn]));
+}
+
+// The same of a packed posting word w = tf << 8 | fieldnorm.
+__device__ __forceinline__ double posting_score(uint32_t w, double s0, const double *__restrict__ s1d) {
+    return tf_score(w >> 8, w & 0xFFu, s0, s1d);
+}
+
+// Score bounds are inflated by 2^-40 so that they also dominate any later re-association of the f64 sum.
+constexpr double UB_INFLATE = 1.0 + 9.094947017729282e-13;
+
+// A block's bound as stored: the inflated score rounded up to f32.
+__device__ __forceinline__ float block_bound(double v) { return __double2float_ru(v * UB_INFLATE); }
+
+}  // namespace
+
+// The statistics a handle scores with: avgdl and the s0 / s1 tables of a segment of N documents with the given df.  The
+// only place they are computed is the constructors (bm25x_index.cu): the shards of a segment and its growing segment
+// receive the segment's object, so that they score with its bits (DESIGN §4.7).
+struct Stats {
+    uint64_t sum_len;
+    double avgdl;
+    std::vector<double> s0d;  // [T]
+    std::vector<float> s0f;
+    double s1d[256];
+    float s1f[256];
+
+    Stats(uint32_t N, uint64_t sum_len, double avgdl, const uint32_t *df, uint32_t T, double k1, double b);
+    // a segment's own: avgdl = Σlen / N (flush.rs:52-66)
+    Stats(uint32_t N, uint64_t sum_len, const uint32_t *df, uint32_t T, double k1, double b);
+};
+
+// A half-built handle: an early return destroys it, release() hands it out.
+struct IndexDestroy {
+    void operator()(bm25x_index *ix) const { bm25x_index_destroy(ix); }
+};
+using IndexGuard = std::unique_ptr<bm25x_index, IndexDestroy>;
+
+// Device temporaries of one build step on one device, freed when it goes out of scope (every refusal included).  The first
+// failure sticks in `e`; later calls do nothing.
+struct Scratch {
+    int device;
+    cudaError_t e = cudaSuccess;
+    std::vector<void *> ptrs;
+    explicit Scratch(int dev) : device(dev) {}
+    Scratch(const Scratch &) = delete;
+    ~Scratch() {
+        if (ptrs.empty()) return;
+        cudaSetDevice(device);
+        for (void *p : ptrs) cudaFree(p);
+    }
+    template <typename T>
+    T *alloc(size_t n) {
+        T *p = nullptr;
+        if (e == cudaSuccess) e = cudaMalloc((void **)&p, sizeof(T) * (n ? n : 1));
+        if (e != cudaSuccess) return nullptr;
+        ptrs.push_back(p);
+        return p;
+    }
+    template <typename T>
+    T *up(const T *h, size_t n) {
+        T *p = alloc<T>(n);
+        if (e == cudaSuccess && n) e = cudaMemcpy(p, h, sizeof(T) * n, cudaMemcpyHostToDevice);
+        return p;
+    }
+};
+
+// One handle's documents and terms, from whichever source (CSR columns, reference-format blocks, a shard of either, a
+// growing segment).
+struct BuildMeta {
+    uint32_t n_docs, n_terms;
+    const uint32_t *doc_len;
+    const uint16_t *payload;
+    const uint8_t *term_key;
+    double k1, b;
+    const uint32_t *df;  // [n_terms]
+    uint64_t n_post;
+    const uint8_t *fieldnorm = nullptr;  // when doc_len == NULL: DocumentTuple.fieldnorm per doc + JumpTuple.sum_of_document_lengths
+    uint64_t sum_len = 0;
+    // document shard: global id of local document 0, for the synthesised ctid payload
+    uint32_t doc_base = 0;
+};
+
+// ---- the build core (bm25x_index.cu) ----
+
+// A handle with everything but the postings, scoring with `given` or, when NULL, its own statistics.
+int index_begin(const BuildMeta &m, const Stats *given, int device, IndexGuard &ix);
+// After the postings are in place: everything derived from them.
+cudaError_t index_finish_device(bm25x_index *ix);
+// The postings of a term-major CSR uploaded, then index_finish_device; a CUDA failure is refused as `who`'s.
+int upload_csr(bm25x_index *ix, const char *who, uint32_t T, uint64_t P, const uint64_t *post_off,
+               const uint32_t *post_doc, const uint32_t *post_tf);
+
+// ---- host checks and helpers shared by the builders, with the messages their refusals give ----
+
+int cuda_refusal(const char *who, const char *step, cudaError_t e);
+int check_device(const char *who, int device);
+int check_common(const char *who, uint32_t n_docs, const void *doc_len, double k1, double b, int device);
+int check_keys(const char *who, const uint8_t *term_key, uint32_t T);
+int check_shard_args(uint32_t N, uint32_t S, const uint32_t *doc_bounds);
+std::vector<uint32_t> shard_bounds(const uint32_t *doc_bounds, const std::vector<uint64_t> &cum, uint32_t N,
+                                   uint32_t S);
+uint8_t bm25x_length_to_fieldnorm(uint32_t len);
+uint64_t doc_norms(uint32_t N, const uint32_t *doc_len, const uint8_t *stored_fn, uint64_t stored_sum, uint8_t *fn);
+void synth_ctid(uint32_t g, uint16_t *out);
+
+// The container of a document-sharded build, for both sources: after the host checks of the segment c (P postings, df, the
+// statistics st), every shard's device is checked with who's message; then prepare(device of shard 0, cum) runs the
+// host work and refusals that need a device and, when doc_bounds is NULL, gives the postings per document for the balanced
+// bounds (shard_bounds); then the shards are built one at a time by build(s, device, lo, hi, ix).  On the first failure
+// everything built so far is destroyed.
+template <typename Segment, typename Prepare, typename Build>
+int sharded_build(const char *who, const Segment *c, uint64_t P, const std::vector<uint32_t> &df, const Stats &st,
+                  uint32_t S, const uint32_t *doc_bounds, const int *devices, Prepare prepare, Build build,
+                  bm25x_sharded_index **out) {
+    std::vector<int> dev(S, 0);
+    if (devices) std::copy(devices, devices + S, dev.begin());
+    for (uint32_t s = 0; s < S; s++) {
+        const int rc = check_device(who, dev[s]);
+        if (rc != BM25X_OK) return rc;
+    }
+    std::vector<uint64_t> cum;
+    int rc = prepare(dev[0], doc_bounds ? nullptr : &cum);
+    if (rc != BM25X_OK) return rc;
+    std::unique_ptr<bm25x_sharded_index, void (*)(bm25x_sharded_index *)> sx(new bm25x_sharded_index(),
+                                                                             bm25x_sharded_destroy);
+    sx->n_shards = S;
+    sx->bounds = shard_bounds(doc_bounds, cum, c->n_docs, S);
+    std::vector<uint64_t>().swap(cum);
+    sx->n_docs = c->n_docs;
+    sx->n_terms = c->n_terms;
+    sx->n_post = P;
+    sx->k1 = c->k1;
+    sx->b = c->b;
+    sx->h_df = df;
+    sx->sum_len = st.sum_len;
+    sx->avgdl = st.avgdl;
+    for (uint32_t s = 0; s < S; s++) {
+        IndexGuard ix;
+        rc = build(s, dev[s], sx->bounds[s], sx->bounds[s + 1], ix);
+        if (rc != BM25X_OK) return rc;
+        sx->shards.push_back(ix.release());
+    }
+    *out = sx.release();
+    return BM25X_OK;
+}

@@ -9,7 +9,7 @@
 #include <chrono>
 #include <vector>
 
-#include "bm25x_common.h"
+#include "bm25x_build.h"
 
 namespace {
 
@@ -299,12 +299,7 @@ extern "C" int bm25x_merge_shards(int device, uint32_t S, uint32_t nq, uint32_t 
         bm25x_set_error("%s: null argument", who);
         return BM25X_ERR_INVALID;
     }
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) {
-        cudaGetLastError();
-        bm25x_set_error("%s: CUDA device %d not available (%d devices); there is no CPU fallback", who, device, ndev);
-        return BM25X_ERR_CUDA;
-    }
+    if (const int rc = check_device(who, device); rc != BM25X_OK) return rc;
     BM25X_CUDA_TRY(cudaSetDevice(device));
     cudaStream_t st = nullptr;
     BM25X_CUDA_TRY(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));

@@ -14,8 +14,9 @@ import numpy as np
 import pytest
 
 import _pkg
-from test_gpu_parity import _compare, _live_queries, _oracle_index, _PrefixOracle, _rows_identical
+from test_gpu_parity import _compare, _live_queries, _oracle_index, _PrefixOracle
 from util_cuda import device_synchronize, download, memset
+from util_parity import same_rows
 
 pytestmark = pytest.mark.gpu
 
@@ -125,12 +126,6 @@ def _poison(batch, live):
     device_synchronize()
 
 
-def _same(got, want, what):
-    _rows_identical(got, want, what)
-    if got.get("payload") is not None:
-        assert np.array_equal(got["payload"], want["payload"]), f"{what}: payload"
-
-
 def _check_oracle(res, oix, canon, k, allow, what):
     c_off, c_terms = _csr(canon)
     _compare(res, oix, c_off, c_terms, k, allow=allow, what=what)
@@ -197,11 +192,11 @@ def test_rerun_rewrites_every_row(m, ix, oix, mixed, path):
                 for r in range(3):
                     _poison(b, live)
                     b.run(timed=False)
-                    _same(b.fetch(want_payload=True), want, f"{what} run {r}")
+                    same_rows(b.fetch(want_payload=True), want, f"{what} run {r}")
                 _poison(b, live)
                 for _ in range(5):
                     b.run(timed=False)
-                _same(b.fetch(want_payload=True), want, f"{what} 5 runs back to back")
+                same_rows(b.fetch(want_payload=True), want, f"{what} 5 runs back to back")
                 b.close()
     ix.set_option("prune", 1)
 
@@ -226,7 +221,7 @@ def test_caller_streams_and_interleaved_batches(m, ix, mixed):
         for b, s in zip(bs, streams):
             b.run(stream=s, timed=False)
     for b, w, (k, _) in zip(bs, want, specs):
-        _same(b.fetch(want_payload=True), w, f"k={k} interleaved")
+        same_rows(b.fetch(want_payload=True), w, f"k={k} interleaved")
 
     b = bs[0]
     _poison(b, live)
@@ -235,13 +230,13 @@ def test_caller_streams_and_interleaved_batches(m, ix, mixed):
     ev.record(s1)
     s2.wait_event(ev)
     b.run(stream=s2.cuda_stream, timed=False)  # fetch reads on the stream of the last run
-    _same(b.fetch(want_payload=True), want[0], "second stream after an event wait")
+    same_rows(b.fetch(want_payload=True), want[0], "second stream after an event wait")
     for b in bs:
         b.close()
 
     fresh = ix.prepare(q_off, q_terms, 200, allow=allow)
     fresh.run(stream=s1.cuda_stream, timed=False)
-    _same(fresh.fetch(want_payload=True), want[1], "caller stream right after prepare")
+    same_rows(fresh.fetch(want_payload=True), want[1], "caller stream right after prepare")
     st = fresh.run(stream=s2.cuda_stream, timed=True)
     assert _fields(st) == _fields(want[1]["stats"]) and st.kernel_ms > 0
     fresh.close()
@@ -289,7 +284,7 @@ def test_device_results_and_partial_fetch(m, ix, mixed):
             _set(ix, prune=prune_run, **run)
             st = b.run(timed=True)
             what = f"prepared {prep} prune={prune_prep}, run {run} prune={prune_run}"
-            _same(b.fetch(want_payload=True), want, what)
+            same_rows(b.fetch(want_payload=True), want, what)
             assert st.launches == _launches(canon, k, None, prep, run), what
             b.close()
     assert _launches(canon, k, None, PATHS["handback"], PATHS["plain"]) == len({_cls(len(c)) for c in canon if len(c)})
@@ -300,7 +295,7 @@ def test_device_results_and_partial_fetch(m, ix, mixed):
         sub = ix.prepare(q_off[a:e + 1], q_terms, k)
         st = sub.run(timed=True)
         got = sub.fetch(want_payload=True)
-        _same(got, {key: want[key][a:e] for key in ("doc", "score", "score64", "payload", "n")}, f"slice [{a}, {e})")
+        same_rows(got, {key: want[key][a:e] for key in ("doc", "score", "score64", "payload", "n")}, f"slice [{a}, {e})")
         assert _fields(st) == _restated(canon[a:e], ix.df(), k, None, PATHS["handback"]), (a, e)
         sub.close()
 
@@ -451,7 +446,7 @@ def test_concurrent_threads_one_index(m, corpus, ix, mixed):
     got = run_threads(index, plans, refuse=True)
     for t in range(len(plans)):
         for j, (g, w) in enumerate(zip(got[t], wants[t])):
-            _same(g, w, f"thread {t} call {j} ({plans[t][j][0]}, k={plans[t][j][2]})")
+            same_rows(g, w, f"thread {t} call {j} ({plans[t][j][0]}, k={plans[t][j][2]})")
     index.close()
 
     # every thread's first call is sliced, on indexes that have served no call yet
@@ -463,7 +458,7 @@ def test_concurrent_threads_one_index(m, corpus, ix, mixed):
         got = run_threads(index, plans, refuse=False)
         for t in range(len(plans)):
             for j, (g, w) in enumerate(zip(got[t], wants[t])):
-                _same(g, w, f"fresh index {r} thread {t} call {j}")
+                same_rows(g, w, f"fresh index {r} thread {t} call {j}")
         index.close()
     _set(ix, slice_min=0)
 
@@ -489,7 +484,7 @@ def test_prepare_refusals(m, corpus, ix, mixed):
             assert e.value.code == code, (code, str(e.value))
         b = ix.prepare(q_off, q_terms, 10)
         b.run(timed=False)
-        _same(b.fetch(want_payload=True), want, f"prepare after a code-{code} refusal")
+        same_rows(b.fetch(want_payload=True), want, f"prepare after a code-{code} refusal")
         b.close()
     b = ix.prepare(np.array([0, len(dup64)], np.uint32), dup64, 10)
     assert b.run(timed=True).queries == 1

@@ -14,6 +14,7 @@ from test_gpu_parity import _oracle_index
 from test_gpu_zz_growing import _expect
 from util_cuda import cudart
 from util_index import CHAMP_L, assert_matches, fieldnorms, read_back, restate
+from util_parity import same_rows
 
 pytestmark = pytest.mark.gpu
 
@@ -140,12 +141,6 @@ def _queries(rng, T, nq, lo=1, hi=8):
     return q_off, np.array([t for q in qs for t in q], np.uint32)
 
 
-def _same_rows(a, b, what):
-    for key in ("doc", "score", "score64", "payload", "n"):
-        if a.get(key) is not None or b.get(key) is not None:
-            assert np.array_equal(a[key], b[key]), f"{what}: {key}"
-
-
 def _search_both(seg, ix, ref, q_off, q_terms, k, allow=None, allow_g=None, allow_g_docs=None):
     got = seg.search_batch(q_off, q_terms, k, allow=allow, allow_growing=allow_g, allow_growing_docs=allow_g_docs,
                            want_payload=True)
@@ -234,13 +229,13 @@ def run_script(orc, w, form, with_payload, prune, seed):
                 allow_g = np.packbits(rng.random(docs.n) < 0.6, bitorder="little")
                 for k in KS:
                     got, want = _search_both(seg, ix, ref, q_off, q_terms, k)
-                    _same_rows(got, want, f"{what} k={k}")
+                    same_rows(got, want, f"{what} k={k}")
                 for k in (10, 129):
                     got, want = _search_both(seg, ix, ref, q_off, q_terms, k, allow=allow, allow_g=allow_g)
-                    _same_rows(got, want, f"{what} k={k} prefiltered")
+                    same_rows(got, want, f"{what} k={k} prefiltered")
                     short = max(0, docs.n - 5)
                     got, want = _search_both(seg, ix, ref, q_off, q_terms, k, allow_g=allow_g, allow_g_docs=short)
-                    _same_rows(got, want, f"{what} k={k} allow_growing_docs={short}")
+                    same_rows(got, want, f"{what} k={k} allow_growing_docs={short}")
             finally:
                 ref.close()
         # the oracle's restatement of search.rs:83-135 + the sealed scan, on a subset
@@ -267,14 +262,14 @@ def test_empty_all_deleted_and_refusals(m, orc, world):
     alone = ix.search_batch(q_off, q_terms, 50, want_payload=True)
     seg = ix.growing_segment()
     try:
-        _same_rows(seg.search_batch(q_off, q_terms, 50, want_payload=True), alone, "opened, empty")
+        same_rows(seg.search_batch(q_off, q_terms, 50, want_payload=True), alone, "opened, empty")
         docs = Docs()
         _new_docs(rng, w, docs, 300)
         seg.insert(**_kw(docs, "doc_len", False))
         seg.delete(np.arange(docs.n))
         seg.delete(np.arange(docs.n))                       # again: a no-op
         assert seg.info().n_deleted == docs.n
-        _same_rows(seg.search_batch(q_off, q_terms, 50, want_payload=True), alone, "every document deleted")
+        same_rows(seg.search_batch(q_off, q_terms, 50, want_payload=True), alone, "every document deleted")
         assert seg.info().n_postings == 0
         # a live segment, then every refusal: the segment and its rows stay as they were
         lo = docs.n
@@ -300,7 +295,7 @@ def test_empty_all_deleted_and_refusals(m, orc, world):
         refused(lambda: seg.search_batch(q_off, q_terms, 65536), 4, "k=65536")
         wide = np.arange(65, dtype=np.uint32)
         refused(lambda: seg.search_batch(np.array([0, 65], np.uint32), wide, 10), 4, "65 live terms")
-        _same_rows(seg.search_batch(q_off, q_terms, 50, want_payload=True), before, "after the refusals")
+        same_rows(seg.search_batch(q_off, q_terms, 50, want_payload=True), before, "after the refusals")
         # the same refusals as bm25x_growing_create's, codes and messages
         for terms, tfs in (([5, 4], [1, 1]), ([4, 5], [1, 1 << 24])):
             with pytest.raises(m.Bm25xError) as a:

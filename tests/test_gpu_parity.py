@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 
 import _pkg
-from util_parity import check_topk
+from util_parity import check_topk, same_rows
 
 pytestmark = pytest.mark.gpu
 
@@ -61,11 +61,6 @@ def _live_queries(rng, df, counts, weighted=False):
     qs = [np.sort(rng.choice(live, size=n, replace=False, p=p)) for n in counts]
     q_off = np.cumsum([0] + [len(q) for q in qs]).astype(np.uint32)
     return q_off, np.concatenate(qs).astype(np.uint32)
-
-
-def _rows_identical(a, b, what):
-    for key in ("doc", "score", "score64", "n"):
-        assert np.array_equal(a[key], b[key]), f"{what}: {key}"
 
 
 def _csr_corpus(rng, n_docs, lists, extra_len=0):
@@ -126,7 +121,7 @@ def test_more_than_32_terms_two_passes(m, orc, cfg):
                         first = res
                         _compare(res, oix, q_off, q_terms, k, allow=al, what=f"{cfg['name']} k={k} allow={al is not None}")
                     else:
-                        _rows_identical(res, first, f"{cfg['name']} k={k} twophase={two} prune={prune}")
+                        same_rows(res, first, f"{cfg['name']} k={k} twophase={two} prune={prune}")
     ix.close()
 
 
@@ -174,7 +169,7 @@ def test_more_than_32_terms_rarest_split_ties_and_refusals(m, orc):
     for k in (10, 1025):
         a = cix.search_batch(r_off, np.concatenate(raws), k)
         b = cix.search_batch(c_off, c_terms, k)
-        _rows_identical(a, b, f"raw vs canonical k={k}")
+        same_rows(a, b, f"raw vs canonical k={k}")
         _compare(b, _oracle_index(orc, c), c_off, c_terms, k, what=f"canonical k={k}")
     # 65 live terms: refused for the whole batch (two passes of 32 lanes cover 64)
     q65 = np.sort(rng.choice(live, size=65, replace=False)).astype(np.uint32)

@@ -8,7 +8,8 @@ import numpy as np
 import pytest
 
 import _pkg
-from test_gpu_parity import _compare, _csr_corpus, _live_queries, _oracle_index, _PrefixOracle, _rows_identical
+from test_gpu_parity import _compare, _csr_corpus, _live_queries, _oracle_index, _PrefixOracle
+from util_parity import same_rows
 from test_gpu_zz_growing import _expect, _setup
 from util_index import assert_matches, read_back, restate
 
@@ -55,7 +56,7 @@ def test_class_boundary_matrix_sliced(m, orc):
         ix.set_option("slice_min", 8)  # 74 queries: 9 slices
         cut = ix.search_batch(q_off, q_terms, k, want_payload=True)
         assert cut["stats"].launches > one["stats"].launches
-        _rows_identical(one, cut, f"sliced k={k}")
+        same_rows(one, cut, f"sliced k={k}")
         assert np.array_equal(one["payload"], cut["payload"])
         _compare(one, oix, q_off, q_terms, k, what=f"class matrix k={k}")
     ix.close()
@@ -90,7 +91,7 @@ def test_limits_above_1024_hbm_pools(m, orc):
             on = ix.search_batch(q_off, q_terms, k, allow=al)
             ix.set_option("prune", 0)
             off = ix.search_batch(q_off, q_terms, k, allow=al)
-            _rows_identical(on, off, f"prune on/off k={k} allow={al is not None}")
+            same_rows(on, off, f"prune on/off k={k} allow={al is not None}")
             _compare(on, oix, q_off, q_terms, k, allow=al, what=f"hbm pool k={k} allow={al is not None}")
     ix.set_option("prune", 1)
     ix.close()
@@ -137,7 +138,7 @@ def test_seeded_5_to_8_terms(m, orc):
                 _set(ix, prune=prune, **opts)
                 got[name, prune] = ix.search_batch(q_off, q_terms, k)
         for key, res in got.items():
-            _rows_identical(res, got["off", 1], f"{key} k={k}")
+            same_rows(res, got["off", 1], f"{key} k={k}")
         # one class (8) in the batch: a seeded launch and the launch of its hand-back list, else one launch
         assert got["seed8", 1]["stats"].launches == (2 if k <= 128 else 1)
         assert got["seed4", 1]["stats"].launches == 1
@@ -166,7 +167,7 @@ def test_k1_b_edges(m, orc, k1, b):
                 _set(ix, prune=prune, **opts)
                 got[name, prune] = ix.search_batch(q_off, q_terms, k)
         for key, res in got.items():
-            _rows_identical(res, got["plain", 1], f"{key} k={k}")
+            same_rows(res, got["plain", 1], f"{key} k={k}")
         _compare(got["seeded", 1], oix, q_off, q_terms, k, what=f"k1={k1} b={b} k={k}")
     ix.close()
 
@@ -201,7 +202,7 @@ def test_b0_tie_flood_at_champion_cut(m, orc):
                     _set(ix, prune=prune, **PATHS[name])
                     got[name, prune] = ix.search_batch(q_off, q_terms, k)
             for key, res in got.items():
-                _rows_identical(res, got["plain", 1], f"{key} k1={k1} k={k}")
+                same_rows(res, got["plain", 1], f"{key} k1={k1} k={k}")
             _compare(got["seeded", 1], oix, q_off, q_terms, k, what=f"tie flood k1={k1} k={k}")
             if k < 1000:  # the cut is inside a tie group: the last row of [0, 1] ties with rows it excludes
                 assert got["plain", 1]["score64"][1, k - 1] == oix.search_exhaustive(qs[1], k + 1)[1][k]
@@ -250,7 +251,7 @@ def test_near_ties_at_the_kth_score(m, orc):
                         assert np.array_equal(res["score64"][j], os_[:k]), f"q{qi} k={k}: f64 scores"
                         assert np.array_equal(res["score"][j], os_[:k].astype(np.float32)), f"q{qi} k={k}: f32 scores"
                 else:
-                    _rows_identical(res, first, f"near tie k={k} {name} prune={prune}")
+                    same_rows(res, first, f"near tie k={k} {name} prune={prune}")
     ix.close()
 
 

@@ -28,7 +28,8 @@ import pytest
 import _pkg
 import util_filter as uf
 import util_prune as up
-from test_gpu_parity import _compare, _PrefixOracle, _rows_identical
+from test_gpu_parity import _compare, _PrefixOracle
+from util_parity import same_rows
 from test_gpu_margin_paths import _hands_back
 from test_gpu_paths import _set
 
@@ -74,7 +75,7 @@ def _run_both(ix, oix, q_off, q_terms, k, opts, launches, what):
         assert res["stats"].launches == launches, (what, prune, res["stats"].launches)
         _compare(res, oix, q_off, q_terms, k, what=f"{what} prune={prune}")
         got.append(res)
-    _rows_identical(got[0], got[1], f"{what}: pruning on / off")
+    same_rows(got[0], got[1], f"{what}: pruning on / off")
     return got
 
 

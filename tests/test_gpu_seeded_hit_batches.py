@@ -9,7 +9,8 @@ import numpy as np
 import pytest
 
 import _pkg
-from test_gpu_parity import _compare, _csr_corpus, _PrefixOracle, _rows_identical
+from test_gpu_parity import _compare, _csr_corpus, _PrefixOracle
+from util_parity import same_rows
 
 pytestmark = pytest.mark.gpu
 
@@ -46,7 +47,7 @@ def _both_paths(m, ix, oix, qs, what, ks=KS):
                 _set(ix, prune=prune, **opts)
                 got[name, prune] = ix.search_batch(q_off, q_terms, k)
         for key, res in got.items():
-            _rows_identical(res, got["plain", 1], f"{what} {key} k={k}")
+            same_rows(res, got["plain", 1], f"{what} {key} k={k}")
             assert np.all(res["doc"][np.arange(k)[None, :] >= res["n"][:, None]] == 0xFFFFFFFF), f"{what} {key} k={k}"
         _compare(got["seeded", 0], oix, q_off, q_terms, k, what=f"{what} k={k}")
 

@@ -8,10 +8,10 @@ import pytest
 
 import _pkg
 from test_gpu_parity import CONFIGS, TWO_PASS, _live_queries
+from util_parity import ROWS, same_rows
 
 pytestmark = pytest.mark.gpu
 
-KEYS = ("doc", "score", "score64", "payload", "n")
 
 
 @pytest.fixture(scope="module")
@@ -22,18 +22,10 @@ def m():
     return mod
 
 
-def _identical(a, b, what):
-    for key in KEYS:
-        assert a[key].shape == b[key].shape, f"{what}: {key} shape"
-        if not np.array_equal(a[key], b[key]):
-            bad = np.argwhere(a[key] != b[key])[:3]
-            raise AssertionError(f"{what}: `{key}` differs at {bad.tolist()}")
-
-
 def _both(ix, sx, q_off, q_terms, k, allow=None, what=""):
     want = ix.search_batch(q_off, q_terms, k, allow=allow, want_payload=True)
     got = sx.search_batch(q_off, q_terms, k, allow=allow, want_payload=True)
-    _identical(got, want, what)
+    same_rows(got, want, what)
     return got, want
 
 
@@ -342,7 +334,7 @@ def test_eight_threads_on_one_sharded_index(m):
         try:
             q_off, q_terms, k, want = work[t]
             for _ in range(4):
-                _identical(sx.search_batch(q_off, q_terms, k, want_payload=True), want, f"thread {t}")
+                same_rows(sx.search_batch(q_off, q_terms, k, want_payload=True), want, f"thread {t}")
         except Exception as e:  # noqa: BLE001 — reported below
             errors.append(e)
 
@@ -405,7 +397,7 @@ def test_merge_kernel_against_a_fold_of_the_host_merge(m):
         acc["doc"] = np.where(np.arange(k)[None, :] < acc["n"][:, None], acc["doc"] + np.uint32(bases[0]), acc["doc"])
         for s in range(1, S):
             acc = m.merge_topk(acc, rows[s], bases[s], k)
-        for key in KEYS:
+        for key in ROWS:
             assert np.array_equal(got[key], acc[key]), (S, nq, k, key)
         assert np.array_equal(got["n"], np.minimum(sum(r["n"].astype(np.int64) for r in rows), k))
 

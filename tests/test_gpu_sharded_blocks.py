@@ -10,9 +10,10 @@ import pytest
 import _pkg
 from test_gpu_blocks import CONFIGS
 from test_gpu_index_arrays import _check_shards, _local_csr
-from test_gpu_sharded import ADVERSARIAL_BOUNDS, PATHS, _adversarial_corpus, _identical
+from test_gpu_sharded import ADVERSARIAL_BOUNDS, PATHS, _adversarial_corpus
 from util_cuda import cudart
 from util_index import DERIVED, LAYOUT, SCALARS, read_back, restate, assert_matches
+from util_parity import same_rows
 
 pytestmark = pytest.mark.gpu
 
@@ -65,7 +66,7 @@ def _same_info(sx, ix, what):
 def _rows(ix, sx, q_off, q_terms, k, allow=None, what=""):
     want = ix.search_batch(q_off, q_terms, k, allow=allow, want_payload=True)
     got = sx.search_batch(q_off, q_terms, k, allow=allow, want_payload=True)
-    _identical(got, want, what)
+    same_rows(got, want, what)
 
 
 # ---- 1. arrays: byte-identical to bm25x_sharded_create on the decoded CSR ----

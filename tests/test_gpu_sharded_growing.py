@@ -18,10 +18,10 @@ from test_gpu_seal import (DEFAULTS, KS, MODES, NONE, Docs, World, _free_bytes, 
                            m)  # noqa: F401  (m: the module fixture)
 from util_index import read_back
 from util_maintain import MISSING, maintain
+from util_parity import ROWS, same_rows
 
 pytestmark = pytest.mark.gpu
 
-ROWS = ("doc", "score", "score64", "payload", "n")
 
 
 def _bounds(kind, S, n_docs):
@@ -41,11 +41,6 @@ def _set_options(handles, opts):
     for h in handles:
         for name, v in {**DEFAULTS, **opts}.items():
             h.set_option(name, v)
-
-
-def _same_rows(a, b, what):
-    for key in ROWS:
-        assert np.array_equal(a[key], b[key]), f"{what}: {key} differs"
 
 
 def _same_arrays(a, b, what):
@@ -73,7 +68,7 @@ def _search_pair(seg, twin, rng, w, q_off, q_terms, k, what, allow=True):
                              want_payload=True)
         b = twin.search_batch(q_off, q_terms, k, allow=al, allow_growing=ag, allow_growing_docs=max(n_g - 3, 0),
                               want_payload=True)
-        _same_rows(a, b, f"{what} allow={al is not None}")
+        same_rows(a, b, f"{what} allow={al is not None}")
         assert (a["stats"].queries, a["stats"].postings) == (b["stats"].queries, b["stats"].postings), what
 
 
@@ -99,7 +94,7 @@ def test_search_parity(m, orc, S, kind, k):
         # before the first insert: the sharded search itself, stats included
         a = seg.search_batch(q_off, q_terms, k, want_payload=True)
         b = sx.search_batch(q_off, q_terms, k, want_payload=True)
-        _same_rows(a, b, f"{what} empty")
+        same_rows(a, b, f"{what} empty")
         for f in ("queries", "postings", "postings_fetched", "launches", "bytes_algo"):
             assert getattr(a["stats"], f) == getattr(b["stats"], f), f"{what} empty: stats.{f}"
         assert seg.info().device == 0
@@ -173,7 +168,7 @@ def _check_sealed(m, orc, got, twin_got, r, old_bounds, sdel, old_devices, rng, 
         for mode, opts in modes.items():
             _set_options((sx, tix), opts)
             for k in ks:
-                _same_rows(sx.search_batch(q_off, q_terms, k, want_payload=True),
+                same_rows(sx.search_batch(q_off, q_terms, k, want_payload=True),
                            tix.search_batch(q_off, q_terms, k, want_payload=True), f"{what} {mode} k={k}")
     finally:
         _set_options((sx, tix), {})
@@ -220,7 +215,7 @@ def test_seal_matches_restatement(m, orc, kind, form, with_payload, S):
             made.append(got[0])
             twin_got = twin.seal(sealed_deleted=_pack(sdel), new_keys=new_keys)
             made.append(twin_got[0])
-            _same_rows(before, seg.search_batch(q_off, q_terms, 40, want_payload=True), f"{what}: the old segment")
+            same_rows(before, seg.search_batch(q_off, q_terms, 40, want_payload=True), f"{what}: the old segment")
             r = maintain(w.n_docs, w.off, w.doc, w.tf, docs.restated(orc, form, with_payload), sealed_deleted=sdel,
                          sealed_payload=w.payload, sealed_keys=w.keys, new_keys=new_keys)
             _check_sealed(m, orc, got, twin_got, r, old_bounds, sdel, [0] * (len(old_bounds) - 1), rng, what)
@@ -307,7 +302,7 @@ def test_refusals(m, orc):
                 fn()
             assert e.value.code == code and text in str(e.value), str(e.value)
             assert _snapshot(seg) == info
-            _same_rows(rows, seg.search_batch(q_off, q_terms, 20, want_payload=True), text)
+            same_rows(rows, seg.search_batch(q_off, q_terms, 20, want_payload=True), text)
 
         first = next(t for t in docs.term if w.n_terms + 2 <= t != MISSING)
         who = "bm25x_growing_seal_sharded: "
@@ -351,7 +346,7 @@ def test_refusals(m, orc):
         msg = L.bm25x_last_error().decode()
         assert msg.startswith(who) and msg.endswith("with bm25x_growing_seal"), msg
         assert _snapshot(seg) == info
-        _same_rows(rows, seg.search_batch(q_off, q_terms, 20, want_payload=True), "after the cross-kind refusals")
+        same_rows(rows, seg.search_batch(q_off, q_terms, 20, want_payload=True), "after the cross-kind refusals")
     finally:
         seg.close()
         plain.close()

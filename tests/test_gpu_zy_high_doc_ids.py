@@ -22,6 +22,7 @@ import pytest
 import _pkg
 from util_cuda import cudart, download
 from util_index import LAYOUT, ctid
+from util_parity import same_rows
 from util_sparse import (DOC_INF, FN_EMPTY, FN_TIE, MAX_N_DOCS, T31, SparseReference, assert_rows, full_fieldnorm,
                          high_id_corpus, reference, sum_len_of)
 
@@ -153,11 +154,6 @@ def _set_path(ix, name):
     ix.set_option("seed_dense_div", div)
 
 
-def _rows_identical(a, b, what):
-    for key in ("doc", "score", "score64", "n", "payload"):
-        assert np.array_equal(a[key], b[key]), f"{what}: {key}"
-
-
 def _slices(n):
     """First 4 KiB, the 4 KiB around 2^31 and the last 4 KiB of the doc ids [0, n)."""
     return [(0, 4096), (T31 - 2048, T31 + 2048), (n - 4096, n)]
@@ -235,7 +231,7 @@ def test_index_a_kernel_paths(index_a, corpus_a):
                 got[name, prune] = ix.search_batch(q_off, q_terms, k, want_payload=True)
                 assert got[name, prune]["stats"].launches >= 1
         for key, res in got.items():
-            _rows_identical(res, got["plain", 1], f"{key} k={k}")
+            same_rows(res, got["plain", 1], f"{key} k={k}")
         assert_rows(got["seeded", 1], pref, qs, k, f"paths k={k}")
     _set_path(ix, "seeded")
     ix.set_option("seed_prune_min", 32768)

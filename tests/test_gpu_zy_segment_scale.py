@@ -25,6 +25,7 @@ from test_gpu_seal import World, _check_result, _keys, _pack
 from test_gpu_segment_steps import check_segment, docs_from_postings, first_docs
 from util_cuda import cudart, sm_count
 from util_maintain import MISSING, maintain
+from util_parity import same_rows
 
 pytestmark = pytest.mark.gpu
 
@@ -70,11 +71,6 @@ def _growing(m, orc, rng, T):
     return docs
 
 
-def _same_rows(a, b, what):
-    for key in ROWS:
-        assert np.array_equal(a[key], b[key]), f"{what}: {key}"
-
-
 @pytest.mark.parametrize("kind", ["keyless", "keyed"])
 def test_more_terms_than_warps(m, orc, kind):
     sms = sm_count()
@@ -100,7 +96,7 @@ def test_more_terms_than_warps(m, orc, kind):
                 g = w.ix.growing(**docs.kw(orc, "doc_len", True))
                 try:
                     for k in KS:
-                        _same_rows(seg.search_batch(q_off, q_terms, k), w.ix.search_batch_growing(g, q_off, q_terms, k),
+                        same_rows(seg.search_batch(q_off, q_terms, k), w.ix.search_batch_growing(g, q_off, q_terms, k),
                                    f"{kind}, segment k={k}")
                 finally:
                     g.close()
@@ -128,7 +124,7 @@ def test_more_terms_than_warps(m, orc, kind):
         oix = orc.OracleIndex(orc.Corpus(r.n_docs, r.doc_len, r.n_terms, r.post_off, r.post_doc, r.post_tf))
         for k in KS:
             rows = got[0].search_batch(q_off, q_new, k)
-            _same_rows(rows, ref.search_batch(q_off, q_new, k), f"{kind}, result k={k}")
+            same_rows(rows, ref.search_batch(q_off, q_new, k), f"{kind}, result k={k}")
             first = {key: rows[key][:50] for key in ROWS}
             _compare(first, oix, q_off[:51], q_new, k, what=f"{kind}, result against the oracle k={k}")
     finally:

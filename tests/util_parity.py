@@ -4,6 +4,21 @@ score differs from both neighbours; (iii) inside a tie group returned ids must b
 oracle's full tie group (checked by rescoring through `score_of`)."""
 import numpy as np
 
+ROWS = ("doc", "score", "score64", "payload", "n")
+
+
+def same_rows(a, b, what):
+    """Two result dicts hold the same rows: every row array that either holds is in both, with the same shape and
+    values."""
+    for key in ROWS:
+        x, y = a.get(key), b.get(key)
+        if x is None and y is None:
+            continue
+        assert x is not None and y is not None, f"{what}: `{key}` in one result only"
+        assert x.shape == y.shape, f"{what}: `{key}` shape {x.shape} != {y.shape}"
+        if not np.array_equal(x, y):
+            raise AssertionError(f"{what}: `{key}` differs at {np.argwhere(x != y)[:3].tolist()}")
+
 
 def check_topk(docs, scores, o_docs, o_scores, rtol, score_of=None, canonical=False, what=""):
     docs = np.asarray(docs)

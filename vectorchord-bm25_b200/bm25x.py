@@ -287,6 +287,12 @@ def _result_arrays(nq, k, want_f64, want_payload):
             "payload": np.empty((nq, k, 3), np.uint16) if want_payload else None, "n": np.empty(nq, np.uint32)}
 
 
+def _rows_args(out):
+    """The five result arrays of a dict of _result_arrays as the out_doc .. out_n arguments of a search or merge."""
+    return (_p(out["doc"], C.c_uint32), _p(out["score"], C.c_float), _p(out["score64"], C.c_double),
+            _p(out["payload"], C.c_uint16), _p(out["n"], C.c_uint32))
+
+
 def _search_batch(fn, h, q_off, q_terms, k, allow, want_f64, want_payload, out):
     """bm25x_search_batch or bm25x_sharded_search_batch (the same signature) on host buffers."""
     q_off = np.ascontiguousarray(q_off, dtype=np.uint32)
@@ -296,9 +302,8 @@ def _search_batch(fn, h, q_off, q_terms, k, allow, want_f64, want_payload, out):
         out = _result_arrays(nq, max(int(k), 1), want_f64, want_payload)
     al = np.ascontiguousarray(allow, dtype=np.uint8) if allow is not None else None
     st = SearchStats()
-    _check(fn(h, nq, _p(q_off, C.c_uint32), _p(q_terms, C.c_uint32), int(k), _p(al, C.c_uint8),
-              _p(out["doc"], C.c_uint32), _p(out["score"], C.c_float), _p(out["score64"], C.c_double),
-              _p(out["payload"], C.c_uint16), _p(out["n"], C.c_uint32), C.byref(st)))
+    _check(fn(h, nq, _p(q_off, C.c_uint32), _p(q_terms, C.c_uint32), int(k), _p(al, C.c_uint8), *_rows_args(out),
+              C.byref(st)))
     out["stats"] = st
     return out
 
@@ -511,8 +516,7 @@ class Index:
         st = SearchStats()
         _check(load_library().bm25x_search_batch_growing(
             self.h, growing.h if growing is not None else None, nq, _p(q_off, C.c_uint32), _p(q_terms, C.c_uint32), kk,
-            _p(al, C.c_uint8), _p(alg, C.c_uint8), _p(out["doc"], C.c_uint32), _p(out["score"], C.c_float),
-            _p(out["score64"], C.c_double), _p(out["payload"], C.c_uint16), _p(out["n"], C.c_uint32), C.byref(st)))
+            _p(al, C.c_uint8), _p(alg, C.c_uint8), *_rows_args(out), C.byref(st)))
         out["stats"] = st
         return out
 
@@ -606,8 +610,7 @@ class GrowingSegment:
         st = SearchStats()
         _check(load_library().bm25x_growing_search_batch(
             self.h, nq, _p(q_off, C.c_uint32), _p(q_terms, C.c_uint32), kk, _p(al, C.c_uint8), _p(alg, C.c_uint8), n_alg,
-            _p(out["doc"], C.c_uint32), _p(out["score"], C.c_float), _p(out["score64"], C.c_double),
-            _p(out["payload"], C.c_uint16), _p(out["n"], C.c_uint32), C.byref(st)))
+            *_rows_args(out), C.byref(st)))
         out["stats"] = st
         return out
 
@@ -673,9 +676,7 @@ def merge_topk(a, b, doc_base_b, k):
     ty = [C.c_uint32, C.c_float, C.c_double, C.c_uint16, C.c_uint32] * 2
     _check(load_library().bm25x_merge_topk(nq, int(k), *[_p(x, t) for x, t in zip(keep[:5], ty[:5])],
                                            *[_p(x, t) for x, t in zip(keep[5:], ty[5:])], int(doc_base_b),
-                                           _p(out["doc"], C.c_uint32), _p(out["score"], C.c_float),
-                                           _p(out["score64"], C.c_double), _p(out["payload"], C.c_uint16),
-                                           _p(out["n"], C.c_uint32)))
+                                           *_rows_args(out)))
     return out
 
 
@@ -790,9 +791,7 @@ def merge_shards(rows, doc_base, k, device=0):
     ms = C.c_float(0.0)
     _check(load_library().bm25x_merge_shards(int(device), S, nq, int(k), _p(base, C.c_uint32), _p(doc, C.c_uint32),
                                              _p(sc, C.c_float), _p(s64, C.c_double), _p(pay, C.c_uint16),
-                                             _p(n, C.c_uint32), _p(out["doc"], C.c_uint32), _p(out["score"], C.c_float),
-                                             _p(out["score64"], C.c_double), _p(out["payload"], C.c_uint16),
-                                             _p(out["n"], C.c_uint32), C.byref(ms)))
+                                             _p(n, C.c_uint32), *_rows_args(out), C.byref(ms)))
     return out, ms.value
 
 
@@ -818,9 +817,7 @@ class Batch:
 
     def fetch(self, want_f64=True, want_payload=False):
         out = _result_arrays(self.nq, self.k, want_f64, want_payload)
-        _check(load_library().bm25x_batch_fetch(self.h, _p(out["doc"], C.c_uint32), _p(out["score"], C.c_float),
-                                                _p(out["score64"], C.c_double), _p(out["payload"], C.c_uint16),
-                                                _p(out["n"], C.c_uint32)))
+        _check(load_library().bm25x_batch_fetch(self.h, *_rows_args(out)))
         return out
 
     def device_results(self):

@@ -135,7 +135,52 @@ uint8_t bm25x_length_to_fieldnorm(uint32_t len);
 uint64_t doc_norms(uint32_t N, const uint32_t *doc_len, const uint8_t *stored_fn, uint64_t stored_sum, uint8_t *fn);
 void synth_ctid(uint32_t g, uint16_t *out);
 
-// The container of a document-sharded build, for both sources: after the host checks of the segment c (P postings, df, the
+// One sealed handle's documents: the handle, the id of its local document 0 in the whole segment, its documents.
+struct SealPart {
+    bm25x_index *h;
+    uint32_t first, n;
+};
+
+// The sealed side of a growing segment or a search: one index (ix), or a document-sharded index (sx).  It answers for the
+// whole segment (n_docs, n_terms, df, Σlen, avgdl, keys: shard 0 holds them) and names the handle the growing segment
+// lives beside, `home`: the index, or the LAST shard (device, SM count, options), where the growing documents sit in id
+// order.
+struct SealedSide {
+    bm25x_index *ix = nullptr;
+    bm25x_sharded_index *sx = nullptr;
+
+    const bm25x_index &home() const { return sx ? *sx->shards.back() : *ix; }
+    uint32_t n_docs() const { return sx ? sx->n_docs : ix->d.n_docs; }
+    uint32_t n_terms() const { return sx ? sx->n_terms : ix->d.n_terms; }
+    const std::vector<uint32_t> &df() const { return sx ? sx->h_df : ix->h_df; }
+    const std::vector<uint8_t> &keys() const { return sx ? sx->shards[0]->h_keys : ix->h_keys; }
+    // the statistics of the whole sealed segment: the growing segment scores with them (search.rs:66-77), not its own
+    Stats stats() const {
+        const bm25x_index &h = home();
+        return sx ? Stats(sx->n_docs, sx->sum_len, sx->avgdl, sx->h_df.data(), sx->n_terms, h.k1, h.b)
+                  : Stats(ix->d.n_docs, ix->sum_len, ix->avgdl, ix->h_df.data(), ix->d.n_terms, h.k1, h.b);
+    }
+    std::vector<SealPart> parts() const {
+        if (!sx) return {{ix, 0, ix->d.n_docs}};
+        std::vector<SealPart> p;
+        for (uint32_t s = 0; s < sx->n_shards; s++)
+            p.push_back({sx->shards[s], sx->bounds[s], sx->bounds[s + 1] - sx->bounds[s]});
+        return p;
+    }
+};
+
+// The search of a sealed side and, when `growing` is given, a growing handle over ids n_docs() + ordinal (bm25x_shards.cu).
+// One index without a growing handle: bm25x_search_batch.  Otherwise every part's top-k with its slice of allow_sealed
+// (global ids) and the growing handle's with allow_growing (its ordinals), merged on the device.  A sharded side first
+// makes bm25x_search_batch's request checks and canonicalises the queries against the whole segment, so that its
+// refusals are those of the unsharded index.  stats->queries = the live queries of the whole sealed segment, plus the
+// growing handle's when count_growing; h2d_ms is counted from t0.  CUDA failures are named by `who`.
+int sealed_side_search(const char *who, const SealedSide &sealed, bm25x_index *growing, const uint8_t *allow_sealed,
+                       const uint8_t *allow_growing, bool count_growing, uint32_t nq, const uint32_t *q_off,
+                       const uint32_t *q_terms, uint32_t k, const ResultRows &host, bm25x_search_stats *stats,
+                       std::chrono::steady_clock::time_point t0);
+
+// The container of a document-sharded build, for both sources:after the host checks of the segment c (P postings, df, the
 // statistics st), every shard's device is checked with who's message; then prepare(device of shard 0, cum) runs the
 // host work and refusals that need a device and, when doc_bounds is NULL, gives the postings per document for the balanced
 // bounds (shard_bounds); then the shards are built one at a time by build(s, device, lo, hi, ix).  On the first failure

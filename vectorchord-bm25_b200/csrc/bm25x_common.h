@@ -129,7 +129,7 @@ struct bm25x_sharded_index {
     std::vector<uint32_t> h_df;
 };
 
-// ---- internal to the host library (bm25x_search.cu, bm25x_shards.cu) ----
+// ---- internal to the host library (bm25x_search.cu, bm25x_shards.cu, bm25x_growing.cu) ----
 
 // Canonical queries (sort + dedup: datatype/tsvector.rs:96-105; unknown and df-0 terms dropped: search.rs:55-62).  Query i
 // of q_off[0..nq] (absolute offsets into q_terms: q_off may be a slice of a longer array) keeps its live terms in place of
@@ -219,25 +219,8 @@ int bm25x_batch_run_timed(bm25x_batch *b);
 cudaEvent_t bm25x_batch_done_event(bm25x_batch *b);
 int bm25x_batch_add_stats(bm25x_batch *b, bm25x_search_stats *acc);
 
-// Lists one merge takes at most: the shards of a document-sharded index and its growing segment's handle.
-#define BM25X_MAX_LISTS (BM25X_MAX_SHARDS + 1)
-
-// The search over S handles that hold consecutive doc ranges of one ranking (the shards of a document-sharded index;
-// a sealed index and its growing segment's handle; both): each handle's top-k with its own allow[s] (NULL = all pass),
-// merged on handle 0's device by k_merge_shards with list s's ids shifted by base[s] (ascending), one copy of the merged
-// rows to `host`.  More than BM25X_MAX_LISTS handles are refused (BM25X_ERR_INVALID).  Refusals of bm25x_batch_prepare,
-// CUDA failures named by `who`.  stats (or NULL): sums over the handles plus the merge launch, h2d_ms counted from t0;
-// live[s] (or NULL) = live queries of handle s.
-int bm25x_merged_search(const char *who, uint32_t S, bm25x_index *const *handles, const uint32_t *base,
-                        const uint8_t *const *allow, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms,
-                        uint32_t k, const ResultRows &host, bm25x_search_stats *stats,
-                        std::chrono::steady_clock::time_point t0, uint32_t *live);
-
-// bm25x_sharded_search_batch (growing == NULL), or the search of a growing segment over sx: the shards' lists and, after
-// them, the growing handle's over ids n_docs(sx) + ordinal, filtered by allow_growing (over its ordinals, or NULL).  The
-// refusals are bm25x_sharded_search_batch's, the whole segment's canonicalisation first; stats->queries = live queries of
-// the whole segment plus the growing handle's.  CUDA failures are named by `who`.
-int bm25x_sharded_merged_search(const char *who, bm25x_sharded_index *sx, bm25x_index *growing,
-                                const uint8_t *allow_growing, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms,
-                                uint32_t k, const uint8_t *allow, const ResultRows &host, bm25x_search_stats *stats,
-                                std::chrono::steady_clock::time_point t0);
+// The request checks of the searches and merges, with bm25x_search_batch's messages (bm25x_search.cu).  check_queries:
+// q_off when nq > 0, q_terms unless every query is empty.  check_k: k == 0, the reference's refusal
+// (scanners/default.rs:114-116), then, when max_k, k <= BM25X_MAX_K.
+int check_queries(uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms);
+int check_k(uint32_t k, bool max_k);

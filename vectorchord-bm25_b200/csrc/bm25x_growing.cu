@@ -15,40 +15,6 @@
 // scores with the sealed segment's statistics.  The reference scans these documents one by one per query; here they
 // are inverted (term-major postings over growing ordinals) so that the same kernels unite them. ----
 
-// One sealed handle's documents as the seal reads them: the handle, the id of its local document 0 in the whole segment,
-// its documents.
-struct SealPart {
-    const bm25x_index *h;
-    uint32_t first, n;
-};
-
-// The sealed side of a growing segment: one index (ix), or a document-sharded index (sx).  It answers for the whole
-// segment (n_docs, n_terms, df, Σlen, avgdl, keys: shard 0 holds them) and names the handle the growing segment lives
-// beside, `home`: the index, or the LAST shard (device, SM count, options), where the growing documents sit in id order.
-struct SealedSide {
-    bm25x_index *ix = nullptr;
-    bm25x_sharded_index *sx = nullptr;
-
-    const bm25x_index &home() const { return sx ? *sx->shards.back() : *ix; }
-    uint32_t n_docs() const { return sx ? sx->n_docs : ix->d.n_docs; }
-    uint32_t n_terms() const { return sx ? sx->n_terms : ix->d.n_terms; }
-    const std::vector<uint32_t> &df() const { return sx ? sx->h_df : ix->h_df; }
-    const std::vector<uint8_t> &keys() const { return sx ? sx->shards[0]->h_keys : ix->h_keys; }
-    // the statistics of the whole sealed segment: the growing segment scores with them (search.rs:66-77), not its own
-    Stats stats() const {
-        const bm25x_index &h = home();
-        return sx ? Stats(sx->n_docs, sx->sum_len, sx->avgdl, sx->h_df.data(), sx->n_terms, h.k1, h.b)
-                  : Stats(ix->d.n_docs, ix->sum_len, ix->avgdl, ix->h_df.data(), ix->d.n_terms, h.k1, h.b);
-    }
-    std::vector<SealPart> parts() const {
-        if (!sx) return {{ix, 0, ix->d.n_docs}};
-        std::vector<SealPart> p;
-        for (uint32_t s = 0; s < sx->n_shards; s++)
-            p.push_back({sx->shards[s], sx->bounds[s], sx->bounds[s + 1] - sx->bounds[s]});
-        return p;
-    }
-};
-
 // Live postings of a batch of growing documents, term-major: the terms that hold any, ascending, and term[i]'s postings
 // doc / tf[off[i] .. off[i + 1]) with ordinals ascending.
 struct GrowingCsr {
@@ -524,41 +490,25 @@ extern "C" int bm25x_growing_search_batch(bm25x_growing_segment *g, uint32_t nq,
         bm25x_set_error("bm25x_growing_search_batch: null argument");
         return BM25X_ERR_INVALID;
     }
-    if (k == 0) {
-        bm25x_set_error("number of needed rows is set to 0");  // scanners/default.rs:114-116
-        return BM25X_ERR_LIMIT_ZERO;
-    }
+    if (const int rc = check_k(k, false); rc != BM25X_OK) return rc;  // before the refresh: a refused call leaves it pending
     const auto t0 = std::chrono::steady_clock::now();
-    std::shared_ptr<bm25x_index> cur;  // this search's state of the segment
+    std::shared_ptr<bm25x_index> cur;  // this search's state of the segment (NULL: nothing inserted yet)
     {
         std::lock_guard<std::mutex> lock(g->mu);
         const int rc = growing_refresh_locked(g);
         if (rc != BM25X_OK) return rc;
         cur = g->cur;
     }
-    const ResultRows host{out_doc, out_score, out_score64, out_payload, out_n};
-    bm25x_sharded_index *sx = g->sealed.sx;
-    if (!cur)  // nothing inserted yet: the sealed search alone
-        return sx ? bm25x_sharded_search_batch(sx, nq, q_off, q_terms, k, allow_sealed, out_doc, out_score, out_score64,
-                                               out_payload, out_n, stats)
-                  : bm25x_search_batch(g->sealed.ix, nq, q_off, q_terms, k, allow_sealed, out_doc, out_score, out_score64,
-                                       out_payload, out_n, stats);
     std::vector<uint8_t> ag;  // allow_growing over the handle's ordinals: the caller's bits below allow_growing_docs
-    if (allow_growing) {
+    if (cur && allow_growing) {
         const uint32_t N = cur->d.n_docs, n = std::min(N, allow_growing_docs);
         ag.assign(((size_t)N + 7) / 8, 0);
         std::copy(allow_growing, allow_growing + ((size_t)n + 7) / 8, ag.begin());
         if (n & 7u) ag[n >> 3] &= (uint8_t)((1u << (n & 7u)) - 1u);
     }
-    const uint8_t *alg = allow_growing ? ag.data() : nullptr;
-    if (sx)
-        return bm25x_sharded_merged_search("bm25x_growing_search_batch", sx, cur.get(), alg, nq, q_off, q_terms, k,
-                                           allow_sealed, host, stats, t0);
-    bm25x_index *ix[2] = {g->sealed.ix, cur.get()};
-    const uint32_t base[2] = {0, g->sealed.n_docs()};
-    const uint8_t *allow[2] = {allow_sealed, alg};
-    return bm25x_merged_search("bm25x_growing_search_batch", 2, ix, base, allow, nq, q_off, q_terms, k, host, stats, t0,
-                               nullptr);
+    return sealed_side_search("bm25x_growing_search_batch", g->sealed, cur.get(), allow_sealed,
+                              cur && allow_growing ? ag.data() : nullptr, true, nq, q_off, q_terms, k,
+                              {out_doc, out_score, out_score64, out_payload, out_n}, stats, t0);
 }
 
 // ---- the seal (`maintain`, maintain.rs:27-311; DESIGN §4.5): a new sealed index from the sealed survivors and the

@@ -20,7 +20,7 @@
 #include <mutex>
 #include <vector>
 
-#include "bm25x_common.h"
+#include "bm25x_build.h"
 
 #include "bm25x_device.cuh"
 
@@ -205,27 +205,41 @@ int bm25x_canonicalise(const uint32_t *h_df, uint32_t n_terms, uint32_t nq, cons
     return BM25X_ERR_UNSUPPORTED;
 }
 
+int check_queries(uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms) {
+    if (nq && (!q_off || (!q_terms && q_off[nq] != 0))) {
+        bm25x_set_error("bm25x_batch_prepare: null argument");
+        return BM25X_ERR_INVALID;
+    }
+    return BM25X_OK;
+}
+
+int check_k(uint32_t k, bool max_k) {
+    if (k == 0) {
+        bm25x_set_error("number of needed rows is set to 0");  // scanners/default.rs:114-116
+        return BM25X_ERR_LIMIT_ZERO;
+    }
+    if (max_k && k > BM25X_MAX_K) {
+        bm25x_set_error("bm25x_batch_prepare: k=%u > BM25X_MAX_K=%d", k, BM25X_MAX_K);
+        return BM25X_ERR_UNSUPPORTED;
+    }
+    return BM25X_OK;
+}
+
 // Canonicalises the queries (bm25x_canonicalise), groups them by term-count class and uploads everything with ONE copy
 // from a page-locked staging buffer cached in the index handle.
 extern "C" int bm25x_batch_prepare(bm25x_index *ix, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms,
                                    uint32_t k, const uint8_t *allow, bm25x_batch **out) {
-    if (!ix || !out || (nq && (!q_off || (!q_terms && q_off[nq] != 0)))) {
+    if (!ix || !out) {
         bm25x_set_error("bm25x_batch_prepare: null argument");
         return BM25X_ERR_INVALID;
     }
+    if (const int rc = check_queries(nq, q_off, q_terms); rc != BM25X_OK) return rc;
     *out = nullptr;
     if (ix->h_df.size() != ix->d.n_terms) {
         bm25x_set_error("bm25x_batch_prepare: replica not finalized (bm25x_index_finalize_replica)");
         return BM25X_ERR_INVALID;
     }
-    if (k == 0) {
-        bm25x_set_error("number of needed rows is set to 0");  // scanners/default.rs:114-116
-        return BM25X_ERR_LIMIT_ZERO;
-    }
-    if (k > BM25X_MAX_K) {
-        bm25x_set_error("bm25x_batch_prepare: k=%u > BM25X_MAX_K=%d", k, BM25X_MAX_K);
-        return BM25X_ERR_UNSUPPORTED;
-    }
+    if (const int rc = check_k(k, true); rc != BM25X_OK) return rc;
     const uint32_t *h_df = ix->h_df.data();
     CanonQueries cq;
     const int crc = bm25x_canonicalise(h_df, ix->d.n_terms, nq, q_off, q_terms, &cq);
@@ -394,6 +408,33 @@ extern "C" int bm25x_batch_prepare(bm25x_index *ix, uint32_t nq, const uint32_t 
     return BM25X_OK;
 }
 
+// The fields of the search kernels' parameters that depend on the index handle alone: its device arrays and options.
+static SearchParams index_params(const bm25x_index *ix) {
+    const DeviceIndex &d = ix->d;
+    SearchParams sp;
+    sp.post = d.post;
+    sp.pdoc = d.pdoc;
+    sp.champ = d.champ;
+    sp.champ_off = d.champ_off;
+    sp.seed_prune_min = ix->seed_prune_min;
+    sp.seed_dense_div = ix->seed_dense_div;
+    sp.post_off = d.post_off;
+    sp.df = d.df;
+    sp.blk_off = d.blk_off;
+    sp.blk = d.blk;
+    sp.blk_ub = d.blk_ub;
+    sp.s0f = d.s0f;
+    sp.s0d = d.s0d;
+    sp.s1d = d.s1d;
+    sp.s1f = d.s1f;
+    sp.payload = d.payload;
+    sp.ubd = d.ubd;
+    sp.prune = ix->prune;
+    sp.s1f_min = ix->s1f_min;
+    sp.n_docs = d.n_docs;
+    return sp;
+}
+
 // The launches of one run on st, counted in b->launches.  Timed: the fetched-postings counter is zeroed and the run sits
 // between the batch's events ev0 and ev1.  Does not synchronise.
 static int batch_enqueue(bm25x_batch *b, cudaStream_t st, bool timed) {
@@ -401,52 +442,31 @@ static int batch_enqueue(bm25x_batch *b, cudaStream_t st, bool timed) {
     BM25X_CUDA_TRY(cudaSetDevice(ix->device));
     b->last_stream = (void *)st;
     if (st != ix->stream) BM25X_CUDA_TRY(cudaStreamWaitEvent(st, b->ev_ready, 0));  // uploads were issued on the library's stream
-    const DeviceIndex &d = ix->d;
     uint32_t launches = 0;
     if (timed) {
         BM25X_CUDA_TRY(cudaMemsetAsync(b->d_fetched, 0, sizeof(unsigned long long), st));
         BM25X_CUDA_TRY(cudaEventRecord(b->ev0, st));
     }
+    SearchParams sp = index_params(ix);
+    sp.fetched = b->d_fetched;
+    sp.k = b->k;
+    sp.allow = b->d_allow;
+    sp.out_doc = b->out.doc;
+    sp.out_score = b->out.score;
+    sp.out_score64 = b->out.score64;
+    sp.out_payload = b->out.payload;
+    sp.out_n = b->out.n;
     for (int c = 0; c < kNumClasses; ++c) {
         Group &g = b->groups[c];
         if (!g.nq) continue;
-        SearchParams sp;
-        sp.post = d.post;
-        sp.pdoc = d.pdoc;
-        sp.champ = d.champ;
-        sp.champ_off = d.champ_off;
-        sp.seed_prune_min = ix->seed_prune_min;
-        sp.seed_dense_div = ix->seed_dense_div;
-        sp.post_off = d.post_off;
-        sp.df = d.df;
-        sp.blk_off = d.blk_off;
-        sp.blk = d.blk;
-        sp.blk_ub = d.blk_ub;
-        sp.s0f = d.s0f;
-        sp.s0d = d.s0d;
-        sp.s1d = d.s1d;
-        sp.s1f = d.s1f;
-        sp.payload = d.payload;
-        sp.ubd = d.ubd;
-        sp.prune = ix->prune;
-        sp.s1f_min = ix->s1f_min;
-        sp.fetched = b->d_fetched;
-        sp.n_docs = d.n_docs;
         sp.q_ids = g.d_ids;
         sp.q_off = g.d_off;
         sp.q_terms = g.d_terms;
         sp.nq = g.nq;
-        sp.k = b->k;
-        sp.allow = b->d_allow;
         sp.work_counter = g.d_counter;
-        sp.out_doc = b->out.doc;
-        sp.out_score = b->out.score;
-        sp.out_score64 = b->out.score64;
-        sp.out_payload = b->out.payload;
-        sp.out_n = b->out.n;
-        BM25X_CUDA_TRY(cudaMemsetAsync(g.d_counter, 0, sizeof(int), st));
         sp.q2 = g.d_q2;
         sp.resume = g.d_resume;
+        BM25X_CUDA_TRY(cudaMemsetAsync(g.d_counter, 0, sizeof(int), st));
         int rc = BM25X_OK;
         if (g.d_q2 && seeded_class(ix, g.M, b->k, b->d_allow)) {
             // seeded launch (champion lists + doc-id-only stream, no pruning); the queries it hands back (a list much
@@ -634,10 +654,7 @@ extern "C" int bm25x_merge_topk(uint32_t nq, uint32_t k, const uint32_t *doc_a, 
                                 const uint32_t *doc_b, const float *score_b, const double *score64_b,
                                 const uint16_t *payload_b, const uint32_t *n_b, uint32_t doc_base_b, uint32_t *out_doc,
                                 float *out_score, double *out_score64, uint16_t *out_payload, uint32_t *out_n) {
-    if (k == 0) {
-        bm25x_set_error("number of needed rows is set to 0");
-        return BM25X_ERR_LIMIT_ZERO;
-    }
+    if (const int rc = check_k(k, false); rc != BM25X_OK) return rc;
     if (nq && (!doc_a || !score64_a || !n_a || !doc_b || !score64_b || !n_b || !out_doc || !out_n) ||
         (out_score && (!score_a || !score_b)) || (out_payload && (!payload_a || !payload_b))) {
         bm25x_set_error("bm25x_merge_topk: null argument (f64 scores of both lists are required)");
@@ -685,27 +702,20 @@ extern "C" int bm25x_search_batch_growing(bm25x_index *sealed, bm25x_index *grow
                                           const uint8_t *allow_growing, uint32_t *out_doc, float *out_score,
                                           double *out_score64, uint16_t *out_payload, uint32_t *out_n,
                                           bm25x_search_stats *stats) {
-    if (!growing)
-        return bm25x_search_batch(sealed, nq, q_off, q_terms, k, allow_sealed, out_doc, out_score, out_score64,
-                                  out_payload, out_n, stats);
-    if (!sealed || sealed->d.n_terms != growing->d.n_terms || sealed->device != growing->device) {
-        bm25x_set_error("bm25x_search_batch_growing: the growing segment does not belong to this sealed index");
-        return BM25X_ERR_INVALID;
+    if (growing) {
+        if (!sealed || sealed->d.n_terms != growing->d.n_terms || sealed->device != growing->device) {
+            bm25x_set_error("bm25x_search_batch_growing: the growing segment does not belong to this sealed index");
+            return BM25X_ERR_INVALID;
+        }
+        if (const int rc = check_k(k, false); rc != BM25X_OK) return rc;
     }
-    if (k == 0) {
-        bm25x_set_error("number of needed rows is set to 0");
-        return BM25X_ERR_LIMIT_ZERO;
-    }
-    // both top-k lists merged on the device: equal scores keep the sealed list first (its ids are all below the base)
-    bm25x_index *seg[2] = {sealed, growing};
-    const uint32_t base[2] = {0, sealed->d.n_docs};
-    const uint8_t *allow[2] = {allow_sealed, allow_growing};
-    uint32_t live[2] = {0, 0};
-    const int rc = bm25x_merged_search("bm25x_search_batch_growing", 2, seg, base, allow, nq, q_off, q_terms, k,
-                                       {out_doc, out_score, out_score64, out_payload, out_n}, stats,
-                                       std::chrono::steady_clock::now(), live);
-    if (rc == BM25X_OK && stats) stats->queries = live[0];  // the sealed search's: a growing live query is a sealed one
-    return rc;
+    // both top-k lists merged on the device: equal scores keep the sealed list first (its ids are all below the base).
+    // stats->queries is the sealed search's: a growing live query is a sealed one.
+    SealedSide side;
+    side.ix = sealed;
+    return sealed_side_search("bm25x_search_batch_growing", side, growing, allow_sealed, allow_growing, false, nq, q_off,
+                              q_terms, k, {out_doc, out_score, out_score64, out_payload, out_n}, stats,
+                              std::chrono::steady_clock::now());
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -11,6 +11,9 @@
 
 #include "bm25x_build.h"
 
+// Lists one merge takes at most: the shards of a document-sharded index and its growing segment's handle.
+#define BM25X_MAX_LISTS (BM25X_MAX_SHARDS + 1)
+
 namespace {
 
 // Row r of shard s: (score64 x, global doc = local + base[s]).  Its rank in the merged list is r plus, for every other
@@ -80,19 +83,6 @@ __global__ void k_merge_shards(ShardRows in, uint32_t S, uint32_t nq, uint32_t k
     }
 }
 
-int launch_merge(int device, const ShardRows &in, uint32_t S, uint32_t nq, uint32_t k, const ResultRows &out,
-                 cudaStream_t st) {
-    const uint64_t total = (uint64_t)nq * S * k;
-    if (!total) return BM25X_OK;
-    int sms = 132;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-    const uint64_t want = (total + 255) / 256, cap = (uint64_t)sms * 32;
-    k_merge_shards<<<(unsigned)std::min(want, cap), 256, 0, st>>>(in, S, nq, k, out.doc, out.score, out.score64,
-                                                                  out.payload, out.n);
-    BM25X_CUDA_TRY(cudaGetLastError());
-    return BM25X_OK;
-}
-
 void set_shard(ShardRows &in, uint32_t s, const ResultRows &rows, uint32_t base) {
     in.doc[s] = rows.doc;
     in.score[s] = rows.score;
@@ -117,14 +107,47 @@ std::vector<uint8_t> allow_slice(const uint8_t *allow, uint32_t n_docs, uint32_t
     return out;
 }
 
-}  // namespace
+// The merge step: k_merge_shards over the S lists of `in` into device rows of its own on stream st of `device`, then ONE
+// copy of the merged rows to `host` and a synchronise.  merge_ms (or NULL): the kernel's time, between two events.  A
+// CUDA failure is refused as who's.
+int merge_step(const char *who, int device, const ShardRows &in, uint32_t S, uint32_t nq, uint32_t k,
+               const ResultRows &host, cudaStream_t st, float *merge_ms) {
+    ResultRows mo;
+    cudaEvent_t m0 = nullptr, m1 = nullptr;
+    cudaError_t e = mo.alloc(nq, k, st);
+    if (e == cudaSuccess && merge_ms) e = cudaEventCreate(&m0);
+    if (e == cudaSuccess && merge_ms) e = cudaEventCreate(&m1);
+    if (e == cudaSuccess && merge_ms) e = cudaEventRecord(m0, st);
+    const uint64_t total = (uint64_t)nq * S * k;
+    if (e == cudaSuccess && total) {
+        int sms = 132;
+        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+        const uint64_t want = (total + 255) / 256, cap = (uint64_t)sms * 32;
+        k_merge_shards<<<(unsigned)std::min(want, cap), 256, 0, st>>>(in, S, nq, k, mo.doc, mo.score, mo.score64,
+                                                                      mo.payload, mo.n);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess && merge_ms) e = cudaEventRecord(m1, st);
+    if (e == cudaSuccess) e = mo.copy_to(host, nq, k, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e == cudaSuccess && merge_ms) e = cudaEventElapsedTime(merge_ms, m0, m1);
+    mo.release(st);
+    if (m0) cudaEventDestroy(m0);
+    if (m1) cudaEventDestroy(m1);
+    if (e != cudaSuccess) {
+        bm25x_set_error("%s: %s", who, cudaGetErrorString(e));
+        return e == cudaErrorMemoryAllocation ? BM25X_ERR_OOM : BM25X_ERR_CUDA;
+    }
+    return BM25X_OK;
+}
 
 // The rows of S handles over consecutive doc ranges (list s: ids + base[s], base ascending) merged into one top-k list:
-// every handle's batch is prepared and run on its own library stream (the next one's canonicalisation overlaps the
-// kernels of the previous), the merge stream (handle 0's) waits for each run's done event and runs k_merge_shards, then
-// ONE copy brings the merged rows to `host`.  Rows of handles on other devices are copied peer to peer first.  stats:
-// sums over the handles plus the merge launch; h2d_ms = from t0 to the last run enqueued, d2h_ms = merge wait +
-// download; queries = sum of the handles' live queries (live[s] = handle s's, when live != NULL).
+// every handle's batch is prepared with its own allow[s] (NULL = all pass) and run on its own library stream (the next
+// one's canonicalisation overlaps the kernels of the previous), the merge stream (handle 0's) waits for each run's done
+// event, then the merge step.  Rows of handles on other devices are copied peer to peer first.  More than
+// BM25X_MAX_LISTS handles are refused.  Refusals of bm25x_batch_prepare, CUDA failures named by `who`.  stats: sums over
+// the handles plus the merge launch; h2d_ms = from t0 to the last run enqueued, d2h_ms = merge wait + download;
+// live[s] = handle s's live queries.
 int bm25x_merged_search(const char *who, uint32_t S, bm25x_index *const *handles, const uint32_t *base,
                         const uint8_t *const *allow, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms,
                         uint32_t k, const ResultRows &host, bm25x_search_stats *stats,
@@ -139,14 +162,10 @@ int bm25x_merged_search(const char *who, uint32_t S, bm25x_index *const *handles
     cudaStream_t ms = ix0->stream;  // the merge runs behind handle 0's kernels on its library stream
     std::vector<bm25x_batch *> bs(S, nullptr);
     std::vector<ResultRows> peer(S);  // rows of handles on other devices, copied to dev0
-    std::vector<cudaEvent_t> evs;
-    ResultRows mo;
     auto cleanup = [&](int code) {
         cudaSetDevice(dev0);
         cudaStreamSynchronize(ms);
         for (ResultRows &p : peer) p.release(ms);
-        mo.release(ms);
-        for (cudaEvent_t e : evs) cudaEventDestroy(e);
         for (bm25x_batch *b : bs)
             if (b) bm25x_batch_destroy(b);
         return code;
@@ -172,43 +191,18 @@ int bm25x_merged_search(const char *who, uint32_t S, bm25x_index *const *handles
         }
         set_shard(in, s, *rows, base[s]);
     }
-    if (e == cudaSuccess) e = mo.alloc(nq, k, ms);
-    cudaEvent_t m0 = nullptr, m1 = nullptr;
-    if (e == cudaSuccess && stats) {
-        e = cudaEventCreate(&m0);
-        if (e == cudaSuccess) evs.push_back(m0);
-        if (e == cudaSuccess) e = cudaEventCreate(&m1);
-        if (e == cudaSuccess) evs.push_back(m1);
-        if (e == cudaSuccess) e = cudaEventRecord(m0, ms);
-    }
     if (e != cudaSuccess) {
         bm25x_set_error("%s: %s", who, cudaGetErrorString(e));
         return cleanup(e == cudaErrorMemoryAllocation ? BM25X_ERR_OOM : BM25X_ERR_CUDA);
     }
-    rc = launch_merge(dev0, in, S, nq, k, mo, ms);
-    if (rc != BM25X_OK) return cleanup(rc);
-    if (stats) e = cudaEventRecord(m1, ms);
-    if (e == cudaSuccess) e = mo.copy_to(host, nq, k, ms);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ms);  // after the merge: every handle's kernels have finished too
-    if (e != cudaSuccess) {
-        bm25x_set_error("%s: %s", who, cudaGetErrorString(e));
-        return cleanup(BM25X_ERR_CUDA);
-    }
-    if (stats) {
+    float mms = 0.f;
+    rc = merge_step(who, dev0, in, S, nq, k, host, ms, stats ? &mms : nullptr);  // after it every kernel has finished
+    if (rc == BM25X_OK && stats) {
         memset(stats, 0, sizeof(*stats));
         for (uint32_t s = 0; s < S && rc == BM25X_OK; s++) {
             const uint32_t q0 = stats->queries;
             rc = bm25x_batch_add_stats(bs[s], stats);
-            if (live) live[s] = stats->queries - q0;
-        }
-        float mms = 0.f;
-        if (rc == BM25X_OK) {
-            cudaSetDevice(dev0);
-            e = cudaEventElapsedTime(&mms, m0, m1);
-            if (e != cudaSuccess) {
-                bm25x_set_error("%s: %s", who, cudaGetErrorString(e));
-                rc = BM25X_ERR_CUDA;
-            }
+            live[s] = stats->queries - q0;
         }
         stats->kernel_ms += mms;  // summed device time of the handles' kernels and the merge, not wall time
         stats->launches += (uint64_t)nq * S * k ? 1u : 0u;
@@ -218,27 +212,22 @@ int bm25x_merged_search(const char *who, uint32_t S, bm25x_index *const *handles
     return cleanup(rc);
 }
 
-int bm25x_sharded_merged_search(const char *who, bm25x_sharded_index *sx, bm25x_index *growing,
-                                const uint8_t *allow_growing, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms,
-                                uint32_t k, const uint8_t *allow, const ResultRows &host, bm25x_search_stats *stats,
-                                std::chrono::steady_clock::time_point t0) {
-    // ---- the refusals of bm25x_search_batch: its argument checks, then its canonicalisation slice by slice against the
-    // WHOLE segment's df (a query with 65 live terms is refused even when no shard sees more than 64) ----
-    if (nq && (!q_off || (!q_terms && q_off[nq] != 0))) {
-        bm25x_set_error("bm25x_batch_prepare: null argument");
-        return BM25X_ERR_INVALID;
-    }
-    if (k == 0) {
-        bm25x_set_error("number of needed rows is set to 0");  // scanners/default.rs:114-116
-        return BM25X_ERR_LIMIT_ZERO;
-    }
-    if (k > BM25X_MAX_K) {
-        bm25x_set_error("bm25x_batch_prepare: k=%u > BM25X_MAX_K=%d", k, BM25X_MAX_K);
-        return BM25X_ERR_UNSUPPORTED;
-    }
-    uint32_t n_live = 0;  // live queries of the whole index
-    int rc = BM25X_OK;
-    {
+}  // namespace
+
+int sealed_side_search(const char *who, const SealedSide &sealed, bm25x_index *growing, const uint8_t *allow_sealed,
+                       const uint8_t *allow_growing, bool count_growing, uint32_t nq, const uint32_t *q_off,
+                       const uint32_t *q_terms, uint32_t k, const ResultRows &host, bm25x_search_stats *stats,
+                       std::chrono::steady_clock::time_point t0) {
+    const bm25x_sharded_index *sx = sealed.sx;
+    if (!sx && !growing)
+        return bm25x_search_batch(sealed.ix, nq, q_off, q_terms, k, allow_sealed, host.doc, host.score, host.score64,
+                                  host.payload, host.n, stats);
+    // ---- a sharded side: the refusals of bm25x_search_batch, its request checks, then its canonicalisation slice by
+    // slice against the WHOLE segment's df (a query with 65 live terms is refused even when no shard sees more than 64) ----
+    uint32_t n_live = 0;  // live queries of the whole sharded segment
+    if (sx) {
+        int rc = check_queries(nq, q_off, q_terms);
+        if (rc == BM25X_OK) rc = check_k(k, true);
         const SlicePlan plan(sx->shards[0]->slice_min, nq);
         CanonQueries cq;
         for (uint32_t s = 0; s < plan.n && rc == BM25X_OK; s++) {
@@ -246,25 +235,31 @@ int bm25x_sharded_merged_search(const char *who, bm25x_sharded_index *sx, bm25x_
             rc = bm25x_canonicalise(sx->h_df.data(), sx->n_terms, e - a, q_off + a, q_terms, &cq);
             for (uint32_t i = 0; i < e - a; i++) n_live += cq.live[i] != 0;
         }
+        if (rc != BM25X_OK) return rc;
     }
-    if (rc != BM25X_OK) return rc;
-    const uint32_t S = sx->n_shards, L = S + (growing ? 1u : 0u);
-    std::vector<std::vector<uint8_t>> al(allow ? S : 0);
-    std::vector<const uint8_t *> as(L, nullptr);
-    for (uint32_t s = 0; s < S && allow; s++) {
-        al[s] = allow_slice(allow, sx->n_docs, sx->bounds[s], sx->bounds[s + 1]);
-        as[s] = al[s].data();
+    // ---- the lists: the sealed parts at their first ids, then the growing handle at n_docs() ----
+    const std::vector<SealPart> parts = sealed.parts();
+    const uint32_t S = (uint32_t)parts.size();
+    std::vector<bm25x_index *> hs;
+    std::vector<uint32_t> base;
+    std::vector<const uint8_t *> allow;
+    std::vector<std::vector<uint8_t>> slices(S);  // allow_sealed cut at a sharded side's bounds
+    for (uint32_t s = 0; s < S; s++) {
+        const SealPart &p = parts[s];
+        if (sx && allow_sealed) slices[s] = allow_slice(allow_sealed, sx->n_docs, p.first, p.first + p.n);
+        hs.push_back(p.h);
+        base.push_back(p.first);
+        allow.push_back(sx && allow_sealed ? slices[s].data() : allow_sealed);
     }
-    // the lists: the shards at their bounds, then the growing handle at n_docs(sx) (= bounds[S])
-    std::vector<bm25x_index *> hs(sx->shards.begin(), sx->shards.end());
     if (growing) {
         hs.push_back(growing);
-        as[S] = allow_growing;
+        base.push_back(sealed.n_docs());
+        allow.push_back(allow_growing);
     }
-    std::vector<uint32_t> live(L, 0);
-    rc = bm25x_merged_search(who, L, hs.data(), sx->bounds.data(), as.data(), nq, q_off, q_terms, k, host, stats, t0,
-                             live.data());
-    if (rc == BM25X_OK && stats) stats->queries = n_live + (growing ? live[S] : 0u);
+    std::vector<uint32_t> live(hs.size(), 0);
+    const int rc = bm25x_merged_search(who, (uint32_t)hs.size(), hs.data(), base.data(), allow.data(), nq, q_off, q_terms,
+                                       k, host, stats, t0, live.data());
+    if (rc == BM25X_OK && stats) stats->queries = (sx ? n_live : live[0]) + (growing && count_growing ? live[S] : 0u);
     return rc;
 }
 
@@ -276,9 +271,11 @@ extern "C" int bm25x_sharded_search_batch(bm25x_sharded_index *sx, uint32_t nq, 
         bm25x_set_error("bm25x_sharded_search_batch: null argument");
         return BM25X_ERR_INVALID;
     }
-    return bm25x_sharded_merged_search("bm25x_sharded_search_batch", sx, nullptr, nullptr, nq, q_off, q_terms, k, allow,
-                                       {out_doc, out_score, out_score64, out_payload, out_n}, stats,
-                                       std::chrono::steady_clock::now());
+    SealedSide side;
+    side.sx = sx;
+    return sealed_side_search("bm25x_sharded_search_batch", side, nullptr, allow, nullptr, false, nq, q_off, q_terms, k,
+                              {out_doc, out_score, out_score64, out_payload, out_n}, stats,
+                              std::chrono::steady_clock::now());
 }
 
 // ---- test / measurement hook: the merge kernel alone on host rows ----
@@ -287,10 +284,7 @@ extern "C" int bm25x_merge_shards(int device, uint32_t S, uint32_t nq, uint32_t 
                                   const uint32_t *n, uint32_t *out_doc, float *out_score, double *out_score64,
                                   uint16_t *out_payload, uint32_t *out_n, float *merge_ms) {
     const char *who = "bm25x_merge_shards";
-    if (k == 0) {
-        bm25x_set_error("number of needed rows is set to 0");
-        return BM25X_ERR_LIMIT_ZERO;
-    }
+    if (const int rc = check_k(k, false); rc != BM25X_OK) return rc;
     if (S == 0 || S > BM25X_MAX_SHARDS || k > BM25X_MAX_K) {
         bm25x_set_error("%s: n_shards=%u must be 1..%d and k=%u <= %d", who, S, BM25X_MAX_SHARDS, k, BM25X_MAX_K);
         return BM25X_ERR_INVALID;
@@ -306,36 +300,23 @@ extern "C" int bm25x_merge_shards(int device, uint32_t S, uint32_t nq, uint32_t 
     // the S shards' rows back to back: S * nq rows, on the host and in `src`
     const ResultRows host{const_cast<uint32_t *>(doc), const_cast<float *>(score), const_cast<double *>(score64),
                           const_cast<uint16_t *>(payload), const_cast<uint32_t *>(n)};
-    ResultRows src, mo;
-    cudaEvent_t m0 = nullptr, m1 = nullptr;
+    ResultRows src;
     cudaError_t e = src.alloc((size_t)nq * S, k, st);
-    if (e == cudaSuccess) e = mo.alloc(nq, k, st);
     if (e == cudaSuccess) e = host.copy_to(src, (size_t)nq * S, k, st);
-    ShardRows in;
-    memset(&in, 0, sizeof(in));
-    for (uint32_t s = 0; s < S; s++) set_shard(in, s, src.from((size_t)s * nq, k), nq ? doc_base[s] : 0);
-    if (e == cudaSuccess) e = cudaEventCreate(&m0);
-    if (e == cudaSuccess) e = cudaEventCreate(&m1);
-    if (e == cudaSuccess) e = cudaEventRecord(m0, st);
     int rc = BM25X_OK;
-    if (e == cudaSuccess) rc = launch_merge(device, in, S, nq, k, mo, st);
-    if (e == cudaSuccess && rc == BM25X_OK) e = cudaEventRecord(m1, st);
-    if (e == cudaSuccess && rc == BM25X_OK) e = mo.copy_to({out_doc, out_score, out_score64, out_payload, out_n}, nq, k, st);
-    if (e == cudaSuccess && rc == BM25X_OK) e = cudaStreamSynchronize(st);
-    if (e == cudaSuccess && rc == BM25X_OK && merge_ms) e = cudaEventElapsedTime(merge_ms, m0, m1);
-    cudaStreamSynchronize(st);
-    src.release(st);
-    mo.release(st);
-    cudaStreamSynchronize(st);
-    if (m0) cudaEventDestroy(m0);
-    if (m1) cudaEventDestroy(m1);
-    cudaStreamDestroy(st);
-    if (rc != BM25X_OK) return rc;
-    if (e != cudaSuccess) {
+    if (e == cudaSuccess) {
+        ShardRows in;
+        memset(&in, 0, sizeof(in));
+        for (uint32_t s = 0; s < S; s++) set_shard(in, s, src.from((size_t)s * nq, k), nq ? doc_base[s] : 0);
+        rc = merge_step(who, device, in, S, nq, k, {out_doc, out_score, out_score64, out_payload, out_n}, st, merge_ms);
+    } else {
         bm25x_set_error("%s: %s", who, cudaGetErrorString(e));
-        return e == cudaErrorMemoryAllocation ? BM25X_ERR_OOM : BM25X_ERR_CUDA;
+        rc = e == cudaErrorMemoryAllocation ? BM25X_ERR_OOM : BM25X_ERR_CUDA;
     }
-    return BM25X_OK;
+    src.release(st);
+    cudaStreamSynchronize(st);
+    cudaStreamDestroy(st);
+    return rc;
 }
 
 // ---- handle queries and options ----

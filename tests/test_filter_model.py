@@ -15,7 +15,6 @@ import numpy as np
 import pytest
 
 import util_filter as uf
-from test_gpu_margins import CASES
 
 KB = [(k1, b) for k1 in (1.2, 2.0) for b in (0.0, 0.75, 1.0)]
 
@@ -89,11 +88,11 @@ def test_exact_regime_is_a_point(orc):
     assert lo < hi
 
 
-@pytest.mark.parametrize("name", list(CASES))
+@pytest.mark.parametrize("name", list(uf.MARGIN_CASES))
 def test_near_threshold_fixtures_are_tight(orc, name):
     """Each GPU margin case: S_A < S_B with A first; F_B exact and below f32_rd(S_A) (kEps = 0 drops B) but not below
     f32_rd(S_A · (1 − 2^-18)) (the shipped kernel keeps B); and the model's S_A, S_B are the oracle's scores bit for bit."""
-    args = CASES[name][0]
+    args = uf.MARGIN_CASES[name][0]
     c = uf.near_threshold_case(orc, **args)
     assert c["a_doc"] < c["b_doc"] and c["S_a"] < c["S_b"]
     assert c["tight"] and c["keeps"] and c["max_keps"] is not None and c["max_keps"] < uf.KEPS

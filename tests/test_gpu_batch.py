@@ -13,10 +13,9 @@ import threading
 import numpy as np
 import pytest
 
-import _pkg
-from test_gpu_parity import _compare, _live_queries, _oracle_index, _PrefixOracle
 from util_cuda import device_synchronize, download, memset
-from util_parity import same_rows
+from util_lib import gpu_library, set_options  # noqa: F401  (gpu_library: the module fixture m)
+from util_parity import PrefixOracle, compare, live_queries, oracle_index, query_csr, same_rows
 
 pytestmark = pytest.mark.gpu
 
@@ -28,14 +27,6 @@ PATHS = dict(seeded=dict(_SEEDED, seed_prune_min=0xFFFFFFFF, seed_dense_div=0), 
              handback=dict(_SEEDED, seed_prune_min=64, seed_dense_div=64),       # skewed and dense queries handed back
              twophase=dict(seed=0, twophase=1, seed_max_terms=8, seed_prune_min=32768, seed_dense_div=64),
              plain=dict(seed=0, twophase=0, seed_max_terms=8, seed_prune_min=32768, seed_dense_div=64))
-
-
-@pytest.fixture(scope="module")
-def m():
-    mod = _pkg.load()
-    mod.load_library()
-    assert mod.device_count() >= 1, "no CUDA device: the engine has no CPU fallback"
-    return mod
 
 
 @pytest.fixture(scope="module")
@@ -53,12 +44,7 @@ def ix(m, corpus):
 
 @pytest.fixture(scope="module")
 def oix(orc, corpus):
-    return _PrefixOracle(_oracle_index(orc, corpus), max(KS))
-
-
-def _csr(qs):
-    q_off = np.cumsum([0] + [len(q) for q in qs]).astype(np.uint32)
-    return q_off, (np.concatenate(qs) if qs else np.zeros(0)).astype(np.uint32)
+    return PrefixOracle(oracle_index(orc, corpus), max(KS))
 
 
 def _canonical(q, df):
@@ -79,7 +65,7 @@ def mixed(m, corpus, ix):
     T = corpus.n_terms
     qs = []
     for counts, weighted in (([1, 2, 3, 4, 5, 8, 9, 16, 17, 32, 33, 64] * 4, False), ([1, 2, 3, 4, 5, 8] * 8, True)):
-        o, t = _live_queries(rng, df, counts, weighted=weighted)
+        o, t = live_queries(rng, df, counts, weighted=weighted)
         qs += [t[o[i]:o[i + 1]] for i in range(len(counts))]
     for i in rng.choice(len(qs), size=12, replace=False):  # duplicates and unknown ids around a live core
         junk = [m.TERM_MISSING, T, T + 9, 10 ** 7] + list(rng.choice(qs[i], size=min(len(qs[i]), 12)))
@@ -95,12 +81,7 @@ def mixed(m, corpus, ix):
     live = n_live > 0
     assert 4 <= (~live).sum() and any(len(q) != len(c) for q, c in zip(qs, canon) if len(c))
     allow = np.packbits(rng.random(corpus.n_docs) < 0.5, bitorder="little")
-    return _csr(qs) + (canon, live, allow)
-
-
-def _set(ix, **opts):
-    for name, value in opts.items():
-        ix.set_option(name, value)
+    return query_csr(qs) + (canon, live, allow)
 
 
 def _runs(mask):
@@ -127,8 +108,8 @@ def _poison(batch, live):
 
 
 def _check_oracle(res, oix, canon, k, allow, what):
-    c_off, c_terms = _csr(canon)
-    _compare(res, oix, c_off, c_terms, k, allow=allow, what=what)
+    c_off, c_terms = query_csr(canon)
+    compare(res, oix, c_off, c_terms, k, allow=allow, what=what)
 
 
 def _cls(n):
@@ -181,7 +162,7 @@ def test_rerun_rewrites_every_row(m, ix, oix, mixed, path):
                 df[c].max() >= n_docs // 64 + 1]
         assert 0 < len(back) < len(eligible), (len(back), len(eligible))
     for prune in (1, 0):
-        _set(ix, prune=prune, **PATHS[path])
+        set_options(ix, prune=prune, **PATHS[path])
         for k in KS:
             for al in (None, allow):
                 what = f"{path} prune={prune} k={k} allow={al is not None}"
@@ -209,7 +190,7 @@ def test_caller_streams_and_interleaved_batches(m, ix, mixed):
     prepare (the run waits for the upload)."""
     import torch
     q_off, q_terms, canon, live, allow = mixed
-    _set(ix, prune=1, **dict(PATHS["handback"], twophase=1))
+    set_options(ix, prune=1, **dict(PATHS["handback"], twophase=1))
     specs = [(10, None), (200, allow), (1025, None)]
     want = [ix.search_batch(q_off, q_terms, k, allow=al, want_payload=True) for k, al in specs]
     s1, s2 = torch.cuda.Stream(), torch.cuda.Stream()
@@ -250,7 +231,7 @@ def test_device_results_and_partial_fetch(m, ix, mixed):
     q_terms) returns those rows of the whole batch."""
     q_off, q_terms, canon, live, allow = mixed
     nq = len(q_off) - 1
-    _set(ix, prune=1, **PATHS["handback"])
+    set_options(ix, prune=1, **PATHS["handback"])
     k = 128
     b = ix.prepare(q_off, q_terms, k)
     b.run(timed=False)
@@ -272,16 +253,16 @@ def test_device_results_and_partial_fetch(m, ix, mixed):
 
     # prepare under `prep`, run under `run` (k = 10: every 2..8-term class may run seeded)
     k = 10
-    _set(ix, **PATHS["plain"])
+    set_options(ix, **PATHS["plain"])
     want = ix.search_batch(q_off, q_terms, k, want_payload=True)
     smt4 = dict(PATHS["handback"], seed_max_terms=4)
     for prep, run in ((PATHS["handback"], PATHS["plain"]), (PATHS["plain"], PATHS["handback"]),
                       (PATHS["plain"], PATHS["twophase"]), (PATHS["twophase"], PATHS["plain"]),
                       (PATHS["twophase"], PATHS["handback"]), (smt4, PATHS["handback"]), (PATHS["handback"], smt4)):
         for prune_prep, prune_run in ((1, 0), (0, 1)):
-            _set(ix, prune=prune_prep, **prep)
+            set_options(ix, prune=prune_prep, **prep)
             b = ix.prepare(q_off, q_terms, k)
-            _set(ix, prune=prune_run, **run)
+            set_options(ix, prune=prune_run, **run)
             st = b.run(timed=True)
             what = f"prepared {prep} prune={prune_prep}, run {run} prune={prune_run}"
             same_rows(b.fetch(want_payload=True), want, what)
@@ -290,7 +271,7 @@ def test_device_results_and_partial_fetch(m, ix, mixed):
     assert _launches(canon, k, None, PATHS["handback"], PATHS["plain"]) == len({_cls(len(c)) for c in canon if len(c)})
 
     # a slice of the offset array: rows a .. b-1 of the whole batch
-    _set(ix, prune=1, **PATHS["handback"])
+    set_options(ix, prune=1, **PATHS["handback"])
     for a, e in ((37, 121), (0, 1), (nq - 5, nq), (60, 60)):
         sub = ix.prepare(q_off[a:e + 1], q_terms, k)
         st = sub.run(timed=True)
@@ -312,11 +293,11 @@ def test_search_stats_restated(m, ix, mixed, path):
     df = ix.df()
     nq = len(q_off) - 1
     short = [i for i in range(nq) if len(canon[i]) <= 32]
-    s_off, s_terms = _csr([q_terms[q_off[i]:q_off[i + 1]] for i in short])
+    s_off, s_terms = query_csr([q_terms[q_off[i]:q_off[i + 1]] for i in short])
     sets = dict(mixed=(q_off, q_terms, canon), short=(s_off, s_terms, [canon[i] for i in short]))
     opts = PATHS[path]
     for prune in (1, 0):
-        _set(ix, prune=prune, **opts)
+        set_options(ix, prune=prune, **opts)
         for k in KS:
             for al in (None, allow):
                 for name, (qo, qt, cn) in sets.items():
@@ -348,7 +329,7 @@ def test_search_stats_restated(m, ix, mixed, path):
                     launches = sum(_launches(cn[a:e], k, al, opts) for a, e in zip(edges[:-1], edges[1:]))
                     assert _fields(cut) == want[:3] + (launches,), what
                     assert cut.postings_fetched == fetched, what
-    _set(ix, prune=1, slice_min=0)
+    set_options(ix, prune=1, slice_min=0)
 
 
 def test_concurrent_threads_one_index(m, corpus, ix, mixed):
@@ -362,7 +343,7 @@ def test_concurrent_threads_one_index(m, corpus, ix, mixed):
     q_off, q_terms, canon, live, allow = mixed
     nq = len(q_off) - 1
     opts = dict(PATHS["handback"], prune=1, slice_min=16)
-    _set(ix, **opts)
+    set_options(ix, **opts)
     rng = np.random.default_rng(311)
 
     def plan(t, sizes, first_kind):
@@ -371,7 +352,7 @@ def test_concurrent_threads_one_index(m, corpus, ix, mixed):
             kind = ("sliced", "split", "single")[(first_kind + j) % 3]
             size = min(size, 31) if kind == "single" else max(size, 32)  # nq >= 2 * slice_min: sliced
             idx = rng.choice(nq, size=size)
-            sub = _csr([q_terms[q_off[i]:q_off[i + 1]] for i in idx])
+            sub = query_csr([q_terms[q_off[i]:q_off[i + 1]] for i in idx])
             k = (10, 100, 224)[(t + j) % 3]
             calls.append((kind, sub, k, allow if (t + j) % 4 == 0 else None))
         return calls
@@ -442,7 +423,7 @@ def test_concurrent_threads_one_index(m, corpus, ix, mixed):
     plans = [plan(t, sizes, t % 3) for t in range(7)]
     wants = [expected(p) for p in plans]
     index = m.Index.from_corpus(corpus)  # fresh: its staging buffer grows during the threads
-    _set(index, **opts)
+    set_options(index, **opts)
     got = run_threads(index, plans, refuse=True)
     for t in range(len(plans)):
         for j, (g, w) in enumerate(zip(got[t], wants[t])):
@@ -454,13 +435,13 @@ def test_concurrent_threads_one_index(m, corpus, ix, mixed):
     wants = [expected(p) for p in plans]
     for r in range(2):
         index = m.Index.from_corpus(corpus)
-        _set(index, **opts)
+        set_options(index, **opts)
         got = run_threads(index, plans, refuse=False)
         for t in range(len(plans)):
             for j, (g, w) in enumerate(zip(got[t], wants[t])):
                 same_rows(g, w, f"fresh index {r} thread {t} call {j}")
         index.close()
-    _set(ix, slice_min=0)
+    set_options(ix, slice_min=0)
 
 
 def test_prepare_refusals(m, corpus, ix, mixed):
@@ -468,7 +449,7 @@ def test_prepare_refusals(m, corpus, ix, mixed):
     k > MAX_K (4), a replica that is not finalized (1).  A refused prepare leaves nothing behind: the next prepare on the
     same index works and answers as before."""
     q_off, q_terms, canon, live, allow = mixed
-    _set(ix, prune=1, **PATHS["handback"])
+    set_options(ix, prune=1, **PATHS["handback"])
     want = ix.search_batch(q_off, q_terms, 10, want_payload=True)
     rng = np.random.default_rng(321)
     q65 = np.sort(rng.choice(np.flatnonzero(ix.df() > 0), size=65, replace=False)).astype(np.uint32)

@@ -6,18 +6,11 @@ plain postings (all 13 device arrays), and searches on it are bit-exact against 
 import numpy as np
 import pytest
 
-import _pkg
-from test_gpu_parity import _compare, _oracle_index
+from util_corpora import BLOCK_CONFIGS
+from util_lib import gpu_library  # noqa: F401  (gpu_library: the module fixture m)
+from util_parity import compare, oracle_index
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def m():
-    mod = _pkg.load()
-    mod.load_library()
-    assert mod.device_count() >= 1, "no CUDA device: the engine has no CPU fallback"
-    return mod
 
 
 def _device_arrays(ix):
@@ -43,15 +36,7 @@ def _from_blocks(m, orc, c, **kw):
                                    eb.doc_off, eb.tf_off, eb.bytes[:eb.n_bytes], **args)
 
 
-CONFIGS = [
-    dict(name="C1", seed=0xB25C0DE1, n=1000, vocab=1000, lmin=32, lmax=32, zipf=0.0),      # only short (byte-packed) blocks
-    dict(name="zipf", seed=22, n=30000, vocab=5000, lmin=16, lmax=96, zipf=1.0),           # full + short blocks, wide bit widths
-    dict(name="dense", seed=23, n=5000, vocab=40, lmin=5, lmax=400, zipf=1.1),             # 1-2 bit deltas, large tf
-    dict(name="ties", seed=25, n=50000, vocab=200, lmin=16, lmax=16, zipf=0.0),
-]
-
-
-@pytest.mark.parametrize("cfg", CONFIGS, ids=[c["name"] for c in CONFIGS])
+@pytest.mark.parametrize("cfg", BLOCK_CONFIGS, ids=[c["name"] for c in BLOCK_CONFIGS])
 def test_blocks_index_identical_and_search_exact(m, orc, cfg):
     c = m.synth_corpus(cfg["seed"], cfg["n"], cfg["vocab"], cfg["lmin"], cfg["lmax"], cfg["zipf"])
     plain = m.Index.from_corpus(c)
@@ -60,9 +45,9 @@ def test_blocks_index_identical_and_search_exact(m, orc, cfg):
     for i, (a, b) in enumerate(zip(_device_arrays(plain), _device_arrays(ix))):
         assert np.array_equal(a, b), f"{cfg['name']}: device array {i} differs between CSR build and block ingest"
     q_off, q_terms = m.synth_queries(cfg["seed"] + 1000, 40, cfg["vocab"], 1, 8, c.post_off, cfg["zipf"])
-    oix = _oracle_index(orc, c)
+    oix = oracle_index(orc, c)
     for k in (1, 10, 100):
-        _compare(ix.search_batch(q_off, q_terms, k), oix, q_off, q_terms, k, what="blocks-" + cfg["name"])
+        compare(ix.search_batch(q_off, q_terms, k), oix, q_off, q_terms, k, what="blocks-" + cfg["name"])
     plain.close()
     ix.close()
 

@@ -2,19 +2,16 @@
 same documents, bit for bit, after every step of a seeded script of inserts, deletes and refreshes: every array of the
 segment's handle (the 13 of the layout, the doc-id copy and the champion lists), every output of its searches, its
 statistics, its refusals, concurrent searches while another thread inserts and deletes, and its device memory."""
-import ctypes
 import threading
 
 import numpy as np
 import pytest
 
-import _pkg
-from test_gpu_index_arrays import _growing_csr
-from test_gpu_parity import _oracle_index
-from test_gpu_zz_growing import _expect
-from util_cuda import cudart
-from util_index import CHAMP_L, assert_matches, fieldnorms, read_back, restate
-from util_parity import same_rows
+from util_cuda import free_bytes
+from util_index import CHAMP_L, assert_matches, fieldnorms, growing_csr, read_back, restate
+from util_lib import gpu_library  # noqa: F401  (gpu_library: the module fixture m)
+from util_parity import oracle_index, query_csr, same_rows
+from util_segment import growing_expect
 
 pytestmark = pytest.mark.gpu
 
@@ -23,20 +20,12 @@ KS = (1, 10, 128, 129, 224, 1024, 1025, 65535)
 
 
 @pytest.fixture(scope="module")
-def m():
-    mod = _pkg.load()
-    mod.load_library()
-    assert mod.device_count() >= 1, "no CUDA device: the engine has no CPU fallback"
-    return mod
-
-
-@pytest.fixture(scope="module")
 def world(m, orc):
     sealed = m.synth_corpus(0x5E6, 6000, 400, 8, 60, 0.8)
     ix = m.Index.from_corpus(sealed)
     sd = orc.GrowingDocs.from_corpus(orc.Corpus(sealed.n_docs, sealed.doc_len, sealed.n_terms, sealed.post_off,
                                                 sealed.post_doc, sealed.post_tf))
-    yield dict(sealed=sealed, ix=ix, sdocs=sd, oix=_oracle_index(orc, sealed))
+    yield dict(sealed=sealed, ix=ix, sdocs=sd, oix=oracle_index(orc, sealed))
     ix.close()
 
 
@@ -112,7 +101,7 @@ def _same_arrays(seg, ref, w, docs, form, with_payload, orc, what):
     a = docs.arrays()
     sdf = ix.df()
     g = orc.GrowingDocs(a["elem_off"], a["elem_term"], a["elem_tf"], a["doc_len"], a["deleted"])
-    off, doc, tf = _growing_csr(g, sealed.n_terms, sdf)
+    off, doc, tf = growing_csr(g, sealed.n_terms, sdf)
     stat = (sealed.n_docs, sdf, float(int(sealed.doc_len.astype(np.uint64).sum())) / sealed.n_docs)
     pay = a["payload"] if with_payload else None
     if form == "doc_len":
@@ -137,8 +126,7 @@ def _queries(rng, T, nq, lo=1, hi=8):
     qs.append([3, 3, 7, 0xFFFFFFFF, T + 5])                              # duplicate and missing terms
     qs.append(sorted(rng.choice(T, size=40, replace=False).tolist()))    # 33..64 live terms: two passes
     qs.append([])
-    q_off = np.cumsum([0] + [len(q) for q in qs]).astype(np.uint32)
-    return q_off, np.array([t for q in qs for t in q], np.uint32)
+    return query_csr(qs)
 
 
 def _search_both(seg, ix, ref, q_off, q_terms, k, allow=None, allow_g=None, allow_g_docs=None):
@@ -246,7 +234,7 @@ def run_script(orc, w, form, with_payload, prune, seed):
             q = q_terms[q_off[i]:q_off[i + 1]]
             if len(np.unique(q[q < sealed.n_terms])) > 32:
                 continue
-            ed, es = _expect(w["oix"], g, sealed.n_docs, q, 10)
+            ed, es = growing_expect(w["oix"], g, sealed.n_docs, q, 10)
             n = int(res["n"][i])
             assert res["doc"][i, :n].tolist() == ed and res["score64"][i, :n].tolist() == es, f"oracle q{i}"
     finally:
@@ -415,12 +403,6 @@ def test_concurrent_searches_see_whole_states(m, orc, world):
         seg.close()
 
 
-def _free_bytes():
-    free, total = ctypes.c_size_t(), ctypes.c_size_t()
-    assert cudart().cudaMemGetInfo(ctypes.byref(free), ctypes.byref(total)) == 0
-    return free.value
-
-
 def test_refreshes_free_their_memory(m, orc, world):
     w = world
     ix = w["ix"]
@@ -441,6 +423,6 @@ def test_refreshes_free_their_memory(m, orc, world):
         seg.close()
 
     run(3)  # loads every kernel of a refresh before the measurement
-    free = _free_bytes()
+    free = free_bytes()
     run(50)
-    assert _free_bytes() == free, "device memory of the segment not freed"
+    assert free_bytes() == free, "device memory of the segment not freed"

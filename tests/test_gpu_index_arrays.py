@@ -9,19 +9,12 @@ the whole segment's statistics)."""
 import numpy as np
 import pytest
 
-import _pkg
+from util_corpora import ADVERSARIAL_BOUNDS, adversarial_corpus
 from util_cuda import D2D, cudart, sm_count
-from util_index import (CHAMP_L, assert_matches, cache, champion_lists, fieldnorms, read_back, restate)
+from util_index import CHAMP_L, assert_matches, cache, check_shards, fieldnorms, growing_csr, read_back, restate
+from util_lib import gpu_library  # noqa: F401  (gpu_library: the module fixture m)
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def m():
-    mod = _pkg.load()
-    mod.load_library()
-    assert mod.device_count() >= 1, "no CUDA device: the engine has no CPU fallback"
-    return mod
 
 
 def _check(ix, r, what, skip=()):
@@ -276,21 +269,6 @@ def test_replica_refinalized(m, orc):
     src.close()
 
 
-def _growing_csr(g, T, sealed_df):
-    """The growing documents inverted, as search.rs:83-135 sees them: no posting from a deleted document, from a token the
-    sealed segment does not know, or from a term with no sealed posting."""
-    n = len(g.elem_off) - 1
-    owner = np.repeat(np.arange(n), np.diff(g.elem_off.astype(np.int64)))
-    term = g.elem_term.astype(np.int64)
-    keep = (g.deleted[owner] == 0) & (term < T)
-    keep[keep] = sealed_df[term[keep]] > 0
-    t, d, tf = term[keep], owner[keep], g.elem_tf[keep]
-    order = np.lexsort((d, t))
-    off = np.zeros(T + 1, np.uint64)
-    off[1:] = np.cumsum(np.bincount(t, minlength=T))
-    return off, d[order].astype(np.uint32), tf[order].astype(np.uint32)
-
-
 def test_growing_handle(m, orc):
     """bm25x_growing_create scores with the sealed segment's N, df and avgdl: its arrays against the restatement of its
     inverted documents with those statistics — norms from exact lengths and from stored norms, synthetic ctids of the
@@ -305,7 +283,7 @@ def test_growing_handle(m, orc):
     ix = m.Index.from_corpus(sealed)
     sdf = ix.df()
     stat = (sealed.n_docs, sdf, float(int(sealed.doc_len.astype(np.uint64).sum())) / sealed.n_docs)
-    off, doc, tf = _growing_csr(g, sealed.n_terms, sdf)
+    off, doc, tf = growing_csr(g, sealed.n_terms, sdf)
     assert np.count_nonzero(np.diff(off.astype(np.int64)) > 256) > 5
     fn = fieldnorms(orc, g.doc_len)
     ctid = np.random.default_rng(62).integers(0, 65535, size=(G, 3)).astype(np.uint16)
@@ -324,42 +302,6 @@ def test_growing_handle(m, orc):
     ix.close()
 
 
-def _local_csr(off, doc, tf, lo, hi):
-    o = off.astype(np.int64)
-    term = np.repeat(np.arange(len(o) - 1), np.diff(o))
-    keep = (doc >= lo) & (doc < hi)
-    loff = np.zeros(len(o), np.uint64)
-    loff[1:] = np.cumsum(np.bincount(term[keep], minlength=len(o) - 1))
-    return loff, (doc[keep] - lo).astype(np.uint32), tf[keep]
-
-
-def _check_shards(m, orc, c, sx, ix, k1, b, what):
-    """Every shard against the restatement of its local CSR with the whole segment's statistics; its score tables
-    byte-equal to the unsharded index's; its champion lists the whole ranking of each term restricted to its documents."""
-    N, T = int(c["n_docs"]), int(c["n_terms"])
-    off, doc, tf = c["post_off"], np.asarray(c["post_doc"]), np.asarray(c["post_tf"])
-    df = np.diff(off.astype(np.int64))
-    stat = (N, df, float(int(np.asarray(c["doc_len"], np.uint64).sum())) / N)
-    whole = read_back(ix.layout(), ix.derived())
-    rw = restate(orc, N, off, doc, tf, k1, b, doc_len=c["doc_len"])
-    bounds = sx.doc_bounds()
-    for s in range(len(bounds) - 1):
-        lo, hi = int(bounds[s]), int(bounds[s + 1])
-        lay, der = sx.shard_arrays(s)
-        got = read_back(lay, der)
-        loff, ldoc, ltf = _local_csr(off, doc, tf, lo, hi)
-        r = restate(orc, hi - lo, loff, ldoc, ltf, k1, b, doc_len=c["doc_len"][lo:hi], stat=stat, doc_base=lo)
-        assert_matches(got, lay, der, r, f"{what} shard {s} [{lo}, {hi})")
-        for key in ("s0d", "s0f", "s1d", "s1f"):
-            assert got[key].tobytes() == whole[key].tobytes(), f"{what} shard {s}: {key} differs from the whole index's"
-        inside = (doc >= lo) & (doc < hi)
-        sub = np.flatnonzero(inside)
-        champ, champ_off = champion_lists(rw.term[sub], doc[sub].astype(np.int64) - lo, (tf[sub].astype(np.int64) << 8) |
-                                          rw.fieldnorm[doc[sub]], rw.score[sub], np.bincount(rw.term[sub], minlength=T))
-        assert np.array_equal(got["champ_off"], champ_off), f"{what} shard {s}: champion offsets"
-        assert np.array_equal(got["champ"], champ.reshape(-1)), f"{what} shard {s}: not the whole ranking restricted"
-
-
 @pytest.mark.parametrize("S", [1, 3, 16])
 def test_shards_default_bounds(m, orc, S):
     c = m.synth_corpus(71, 30000, 2000, 4, 120, 0.8)
@@ -367,7 +309,7 @@ def test_shards_default_bounds(m, orc, S):
               post_tf=c.post_tf)
     ix = m.Index(**cd)
     sx = m.ShardedIndex(**cd, n_shards=S)
-    _check_shards(m, orc, cd, sx, ix, 1.2, 0.75, f"S={S}")
+    check_shards(m, orc, cd, sx, ix, 1.2, 0.75, f"S={S}")
     with pytest.raises(m.Bm25xError) as e:
         sx.shard_arrays(S)
     assert e.value.code == 1 and f"shard {S} of {S}" in str(e.value)
@@ -377,10 +319,9 @@ def test_shards_default_bounds(m, orc, S):
 
 def test_shards_adversarial_bounds(m, orc):
     """The bounds of test_gpu_sharded.py::test_adversarial_bounds: a one-document shard, a shard with no postings."""
-    from test_gpu_sharded import ADVERSARIAL_BOUNDS, _adversarial_corpus
-    c, _ = _adversarial_corpus()
+    c, _ = adversarial_corpus()
     ix = m.Index(**c)
     sx = m.ShardedIndex(**c, n_shards=len(ADVERSARIAL_BOUNDS) - 1, doc_bounds=ADVERSARIAL_BOUNDS)
-    _check_shards(m, orc, c, sx, ix, 1.2, 0.75, "adversarial")
+    check_shards(m, orc, c, sx, ix, 1.2, 0.75, "adversarial")
     sx.close()
     ix.close()

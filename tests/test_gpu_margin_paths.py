@@ -25,16 +25,15 @@ scores."""
 import numpy as np
 import pytest
 
-import _pkg
-from test_gpu_parity import _compare
-from test_gpu_paths import PATHS, _set
 import util_filter as uf
+from util_lib import gpu_library, set_options  # noqa: F401  (gpu_library: the module fixture m)
+from util_parity import KERNEL_PATHS, compare
 
 CLASSES = (1, 2, 3, 4, 8, 16, 32, 64)  # bm25x_batch_prepare: a query of n live terms runs in the first class >= n
 CHAMP_L = 128                          # BM25X_CHAMP_L: the seeded launch takes limits up to the champion-list length
 SUSPEND_MIN = 4096                     # BM25X_SUSPEND_MIN: postings left when a two-phase query is handed over
 
-SEEDED = dict(PATHS["seeded"], seed_max_terms=8)
+SEEDED = dict(KERNEL_PATHS["seeded"], seed_max_terms=8)
 HANDBACK = dict(SEEDED, seed_prune_min=0, seed_dense_div=0xFFFFFFFF)  # every list is "dense": all queries go back
 
 # name: (near_threshold_case arguments, flavour, index options, class M, KP, hit-list rows, launches)
@@ -51,14 +50,14 @@ CASES = {
     "seeded_8_k10": (dict(m=7, k=10, n_docs=1000000), "seeded", SEEDED, 8, 64, 0, 2),
     "seeded_8_k100": (dict(m=7, k=100, n_docs=1000000), "seeded", SEEDED, 8, 256, 0, 2),
     "seeded_dense": (dict(m=3, k=10, n_docs=60000, binade=8.0, dense=True), "seeded", SEEDED, 4, 64, 0, 2),
-    "resume_dense": (dict(m=3, k=10, n_docs=60000, binade=8.0, dense=True), "twophase", PATHS["twophase"], 4, 64, 0, 2),
-    "twophase_k128": (dict(m=3, k=128, n_docs=1000000), "twophase", PATHS["twophase"], 4, 256, 0, 2),
+    "resume_dense": (dict(m=3, k=10, n_docs=60000, binade=8.0, dense=True), "twophase", KERNEL_PATHS["twophase"], 4, 64, 0, 2),
+    "twophase_k128": (dict(m=3, k=128, n_docs=1000000), "twophase", KERNEL_PATHS["twophase"], 4, 256, 0, 2),
     "handback": (dict(m=3, k=10, n_docs=1000000), "handback", HANDBACK, 4, 64, 0, 2),
-    "plain_k224": (dict(m=3, k=224, n_docs=1000000), "plain", PATHS["plain"], 4, 256, 0, 1),
-    "plain_k225": (dict(m=3, k=225, n_docs=1000000), "plain", PATHS["plain"], 4, 2048, 0, 1),
-    "plain_k1024": (dict(m=3, k=1024, n_docs=1000000), "plain", PATHS["plain"], 4, 2048, 0, 1),
-    "plain_16_dense": (dict(m=15, k=10, n_docs=60000, binade=8.0, dense=True), "plain", PATHS["plain"], 16, 64, 0, 1),
-    "plain_32_dense": (dict(m=31, k=10, n_docs=60000, binade=8.0, dense=True), "plain", PATHS["plain"], 32, 64, 0, 1),
+    "plain_k224": (dict(m=3, k=224, n_docs=1000000), "plain", KERNEL_PATHS["plain"], 4, 256, 0, 1),
+    "plain_k225": (dict(m=3, k=225, n_docs=1000000), "plain", KERNEL_PATHS["plain"], 4, 2048, 0, 1),
+    "plain_k1024": (dict(m=3, k=1024, n_docs=1000000), "plain", KERNEL_PATHS["plain"], 4, 2048, 0, 1),
+    "plain_16_dense": (dict(m=15, k=10, n_docs=60000, binade=8.0, dense=True), "plain", KERNEL_PATHS["plain"], 16, 64, 0, 1),
+    "plain_32_dense": (dict(m=31, k=10, n_docs=60000, binade=8.0, dense=True), "plain", KERNEL_PATHS["plain"], 32, 64, 0, 1),
 }
 
 
@@ -79,14 +78,6 @@ def hit_rows(M, KP):
     warps = min(20, smem // ((off_hit + 8 + 127) & ~127))
     rows = min(32, (((smem // warps) & ~127) - (off_hit + 24)) // ((M + 1) * 4))
     return rows if rows >= 16 else 0
-
-
-def _hands_back(c, opts, prune):
-    """The seeded launch's test at query start: a list of n_docs / seed_dense_div postings or more (dense), or with pruning
-    on, a list of seed_prune_min or more that is 8 times the shortest (skewed)."""
-    mx, mn = int(max(c["df"])), int(min(c["df"]))
-    div = opts["seed_dense_div"]
-    return bool((prune and mx >= opts["seed_prune_min"] and mx // 8 >= mn) or (div and mx >= c["n_docs"] // div + 1))
 
 
 def _suspends_before_b(c):
@@ -120,7 +111,7 @@ def _where(name, c):
     if flavour in ("seeded", "handback"):
         assert 2 <= M <= 8 and k <= CHAMP_L and hit_rows(M, KP) == hcap
         for prune in (1, 0):
-            assert _hands_back(c, opts, prune) == (flavour == "handback"), prune
+            assert uf.hands_back(c, opts, prune) == (flavour == "handback"), prune
     else:
         assert hcap == 0
     if flavour == "twophase":
@@ -148,14 +139,6 @@ def test_margin_path_fixture(orc, name):
     assert os_[k] == c["S_a"] and os_[od.tolist().index(c["b_doc"])] == c["S_b"]
 
 
-@pytest.fixture(scope="module")
-def m():
-    mod = _pkg.load()
-    mod.load_library()
-    assert mod.device_count() >= 1, "no CUDA device: the engine has no CPU fallback"
-    return mod
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", list(CASES))
 def test_margin_keeps_b_on_every_instantiation(m, orc, name):
@@ -167,11 +150,11 @@ def test_margin_keeps_b_on_every_instantiation(m, orc, name):
     q_off = np.array([0, len(c["query"])], np.uint32)
     first = None
     for prune in (1, 0):
-        _set(ix, prune=prune, **opts)
+        set_options(ix, prune=prune, **opts)
         res = ix.search_batch(q_off, c["query"], k)
         assert res["stats"].launches == launches
         assert c["b_doc"] in res["doc"][0, :k].tolist(), f"{name} prune={prune}: B dropped by the filter"
-        _compare(res, oix, q_off, c["query"], k, what=f"{name} prune={prune}")
+        compare(res, oix, q_off, c["query"], k, what=f"{name} prune={prune}")
         if first is None:
             first = res
         else:

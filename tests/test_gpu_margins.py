@@ -27,37 +27,15 @@ So none of these alone changes a result while kEps = 2^-18; they matter only tog
 import numpy as np
 import pytest
 
-import _pkg
-from test_gpu_parity import _compare
-from test_gpu_paths import PATHS, _set
 import util_filter as uf
+from util_lib import gpu_library, set_options  # noqa: F401  (gpu_library: the module fixture m)
+from util_parity import compare
 
 pytestmark = pytest.mark.gpu
 
-# name: (near_threshold_case arguments, kernel path options, launches of the batch's one class)
-CASES = {
-    "plain_6_lanes": (dict(m=5, k=10, n_docs=1000000), PATHS["plain"], 1),    # class 8, KEEPW verification
-    "class_16": (dict(m=15, k=10, n_docs=1000000), PATHS["plain"], 1),        # filter_term loop
-    "class_32": (dict(m=31, k=10, n_docs=1000000), PATHS["plain"], 1),
-    "seeded_4_lanes": (dict(m=3, k=10, n_docs=1000000), PATHS["seeded"], 2),  # seeded launch + (empty) hand-back launch
-    "two_phase": (dict(m=3, k=10, n_docs=1000000), PATHS["twophase"], 2),     # suspend launch, resume launch (doc ids) finds B
-    "two_pass": (dict(m=8, k=10, n_docs=1000000, n_rare=32), PATHS["plain"], 1),  # 41 lanes: B holds group 1 only
-    "dense_window": (dict(m=4, k=10, n_docs=60000, binade=8.0, dense=True), PATHS["plain"], 1),
-    "hbm_pool": (dict(m=3, k=1025, n_docs=1000000), PATHS["plain"], 1),       # k = 1025: pool in HBM, lazy cut
-}
-
-
-@pytest.fixture(scope="module")
-def m():
-    mod = _pkg.load()
-    mod.load_library()
-    assert mod.device_count() >= 1, "no CUDA device: the engine has no CPU fallback"
-    return mod
-
-
-@pytest.mark.parametrize("name", list(CASES))
+@pytest.mark.parametrize("name", list(uf.MARGIN_CASES))
 def test_margin_keeps_the_later_better_document(m, orc, name):
-    args, opts, launches = CASES[name]
+    args, opts, launches = uf.MARGIN_CASES[name]
     c = uf.near_threshold_case(orc, **args)
     k = c["k"]
     assert c["tight"] and c["keeps"], "the model says kEps alone decides"
@@ -76,10 +54,10 @@ def test_margin_keeps_the_later_better_document(m, orc, name):
     assert os_[k] == c["S_a"] and os_[od.tolist().index(c["b_doc"])] == c["S_b"]
     first = None
     for prune in (1, 0):
-        _set(ix, prune=prune, **opts)
+        set_options(ix, prune=prune, **opts)
         res = ix.search_batch(q_off, c["query"], k)
         assert res["stats"].launches == launches
-        _compare(res, oix, q_off, c["query"], k, what=f"{name} prune={prune}")
+        compare(res, oix, q_off, c["query"], k, what=f"{name} prune={prune}")
         if first is None:
             first = res
         else:

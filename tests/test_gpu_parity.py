@@ -6,84 +6,11 @@ import os
 import numpy as np
 import pytest
 
-import _pkg
-from util_parity import check_topk, same_rows
+from util_corpora import PARITY_CONFIGS, TWO_PASS, csr_corpus, slt_corpus
+from util_lib import gpu_library  # noqa: F401  (gpu_library: the module fixture m)
+from util_parity import PrefixOracle, check_topk, compare, live_queries, oracle_index, query_csr, same_rows
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def m():
-    mod = _pkg.load()
-    mod.load_library()
-    assert mod.device_count() >= 1, "no CUDA device: the engine has no CPU fallback"
-    return mod
-
-
-def _oracle_index(orc, c):
-    return orc.OracleIndex(orc.Corpus(c.n_docs, c.doc_len, c.n_terms, c.post_off, c.post_doc, c.post_tf))
-
-
-def _compare(res, oix, q_off, q_terms, k, allow=None, what=""):
-    for i in range(len(q_off) - 1):
-        q = q_terms[q_off[i]:q_off[i + 1]]
-        od, os_, _ = oix.search_exhaustive(q, k, allow=allow)
-        n = int(res["n"][i])
-        assert n == len(od), f"{what} q{i}: n {n} != {len(od)}"
-        assert np.array_equal(res["doc"][i, :n], od), f"{what} q{i} k{k}: ids\n got {res['doc'][i, :n]}\nwant {od}"
-        assert np.array_equal(res["score64"][i, :n], os_), f"{what} q{i}: f64 scores not bit-exact"
-        assert np.array_equal(res["score"][i, :n], os_.astype(np.float32)), f"{what} q{i}: f32 scores"
-        assert np.all(res["doc"][i, n:] == 0xFFFFFFFF)
-
-
-class _PrefixOracle:
-    """OracleIndex.search_exhaustive at one large limit, memoised per (query, bitmap): the canonical order (score desc,
-    doc asc) is total, so the top-k of every smaller k is a prefix of it."""
-
-    def __init__(self, oix, kmax):
-        self.oix, self.kmax, self.memo = oix, kmax, {}
-
-    def search_exhaustive(self, q, k, allow=None):
-        assert k <= self.kmax
-        q = np.ascontiguousarray(q, dtype=np.uint32)
-        key = (q.tobytes(), None if allow is None else np.asarray(allow).tobytes())
-        if key not in self.memo:
-            self.memo[key] = self.oix.search_exhaustive(q, self.kmax, allow=allow)
-        od, os_, tg = self.memo[key]
-        return od[:k], os_[:k], tg
-
-
-def _live_queries(rng, df, counts, weighted=False):
-    """One query per entry of `counts` with exactly that many distinct terms of df > 0, ascending ids.  weighted: terms
-    drawn in proportion to df (head terms in most queries)."""
-    live = np.flatnonzero(df > 0)
-    p = df[live] / df[live].sum() if weighted else None
-    qs = [np.sort(rng.choice(live, size=n, replace=False, p=p)) for n in counts]
-    q_off = np.cumsum([0] + [len(q) for q in qs]).astype(np.uint32)
-    return q_off, np.concatenate(qs).astype(np.uint32)
-
-
-def _csr_corpus(rng, n_docs, lists, extra_len=0):
-    """Term-major CSR from explicit posting lists [(doc ids, tfs)]; a document's length is its Σ tf plus up to
-    `extra_len` tokens of terms outside the corpus (varied norms)."""
-    off = np.zeros(len(lists) + 1, dtype=np.uint64)
-    off[1:] = np.cumsum([len(d) for d, _ in lists])
-    post_doc = np.concatenate([np.asarray(d, np.uint32) for d, _ in lists])
-    post_tf = np.concatenate([np.asarray(t, np.uint32) for _, t in lists])
-    doc_len = np.bincount(post_doc, weights=post_tf, minlength=n_docs).astype(np.uint32)
-    if extra_len:
-        doc_len += rng.integers(0, extra_len + 1, size=n_docs).astype(np.uint32)
-    return doc_len, off, post_doc, post_tf
-
-
-TWO_PASS = [
-    # uniform vocabulary: df is not monotone in the term id, so the two groups interleave in id order
-    dict(name="uniform", seed=101, n=20000, vocab=1500, lmin=8, lmax=120, zipf=0.0, weighted=False),
-    # dense: 72 terms, long documents (dense windows in pass 0)
-    dict(name="dense", seed=102, n=4000, vocab=72, lmin=60, lmax=400, zipf=0.5, weighted=False),
-    # Zipf, terms drawn by df: head terms pruned while group 1 is probed
-    dict(name="zipf", seed=103, n=30000, vocab=3000, lmin=16, lmax=96, zipf=1.0, weighted=True),
-]
 
 
 @pytest.mark.parametrize("cfg", TWO_PASS, ids=[c["name"] for c in TWO_PASS])
@@ -97,7 +24,7 @@ def test_more_than_32_terms_two_passes(m, orc, cfg):
     df = ix.df()
     rng = np.random.default_rng(cfg["seed"])
     counts = [33, 40, 48, 63, 64] * 3
-    q_off, q_terms = _live_queries(rng, df, counts, weighted=cfg["weighted"])
+    q_off, q_terms = live_queries(rng, df, counts, weighted=cfg["weighted"])
     assert np.array_equal(np.diff(q_off), counts)
     if cfg["name"] == "uniform":  # the (df, id) split is not a cut in id order
         inter = 0
@@ -108,7 +35,7 @@ def test_more_than_32_terms_two_passes(m, orc, cfg):
         assert inter == len(counts)
     allow = np.packbits(rng.random(c.n_docs) < 0.3, bitorder="little")
     ks = (1, 10, 100, 225, 1000, 1025)
-    oix = _PrefixOracle(_oracle_index(orc, c), max(ks))
+    oix = PrefixOracle(oracle_index(orc, c), max(ks))
     for k in ks:
         for al in (None, allow):
             first = None
@@ -119,7 +46,7 @@ def test_more_than_32_terms_two_passes(m, orc, cfg):
                     res = ix.search_batch(q_off, q_terms, k, allow=al)
                     if first is None:
                         first = res
-                        _compare(res, oix, q_off, q_terms, k, allow=al, what=f"{cfg['name']} k={k} allow={al is not None}")
+                        compare(res, oix, q_off, q_terms, k, allow=al, what=f"{cfg['name']} k={k} allow={al is not None}")
                     else:
                         same_rows(res, first, f"{cfg['name']} k={k} twophase={two} prune={prune}")
     ix.close()
@@ -134,7 +61,7 @@ def test_more_than_32_terms_rarest_split_ties_and_refusals(m, orc):
     want_df = np.array([40] * 16 + [90] * 30 + list(rng.integers(200, 900, size=T - 46)))
     want_df = want_df[rng.permutation(T)]  # the boundary terms sit anywhere in id order
     lists = [(np.sort(rng.choice(n_docs, size=int(d), replace=False)), rng.integers(1, 5, size=int(d))) for d in want_df]
-    doc_len, off, pd_, pt = _csr_corpus(rng, n_docs, lists, extra_len=50)
+    doc_len, off, pd_, pt = csr_corpus(rng, n_docs, lists, extra_len=50)
     ix = m.Index(n_docs, doc_len, T, off, pd_, pt)
     oix = orc.OracleIndex(orc.Corpus(n_docs, doc_len, T, off, pd_, pt))
     assert np.array_equal(ix.df(), want_df)
@@ -142,12 +69,11 @@ def test_more_than_32_terms_rarest_split_ties_and_refusals(m, orc):
     qs = [np.concatenate([rare, tied, common[:18]]),                    # 64: the split cuts the df = 90 group at 16 of 30
           np.concatenate([rare[:6], tied, common[:4]]),                 # 40: 26 of the 30 tied terms in group 0
           np.concatenate([tied, common[:10]])]                          # 40: group 0 = the 30 tied + 2 common terms
-    q_off = np.cumsum([0] + [len(q) for q in qs]).astype(np.uint32)
-    q_terms = np.concatenate([np.sort(q) for q in qs]).astype(np.uint32)
+    q_off, q_terms = query_csr([np.sort(q) for q in qs])
     for k in (1, 10, 100, 1000, 1025):
         for prune in (1, 0):
             ix.set_option("prune", prune)
-            _compare(ix.search_batch(q_off, q_terms, k), oix, q_off, q_terms, k, what=f"tie split k={k} prune={prune}")
+            compare(ix.search_batch(q_off, q_terms, k), oix, q_off, q_terms, k, what=f"tie split k={k} prune={prune}")
     ix.set_option("prune", 1)
 
     # 80 raw terms, <= 64 live: the same rows as the canonical query
@@ -170,7 +96,7 @@ def test_more_than_32_terms_rarest_split_ties_and_refusals(m, orc):
         a = cix.search_batch(r_off, np.concatenate(raws), k)
         b = cix.search_batch(c_off, c_terms, k)
         same_rows(a, b, f"raw vs canonical k={k}")
-        _compare(b, _oracle_index(orc, c), c_off, c_terms, k, what=f"canonical k={k}")
+        compare(b, oracle_index(orc, c), c_off, c_terms, k, what=f"canonical k={k}")
     # 65 live terms: refused for the whole batch (two passes of 32 lanes cover 64)
     q65 = np.sort(rng.choice(live, size=65, replace=False)).astype(np.uint32)
     for q in (q65, np.concatenate([q65, q65[:10], [m.TERM_MISSING]]).astype(np.uint32)):
@@ -181,34 +107,23 @@ def test_more_than_32_terms_rarest_split_ties_and_refusals(m, orc):
     ix.close()
 
 
-CONFIGS = [
-    dict(name="C1", seed=0xB25C0DE1, n=1000, vocab=1000, lmin=32, lmax=32, zipf=0.0, nq=100, tmin=3, tmax=3),
-    dict(name="varlen", seed=21, n=20000, vocab=3000, lmin=1, lmax=300, zipf=0.0, nq=80, tmin=1, tmax=8),
-    dict(name="zipf", seed=22, n=30000, vocab=5000, lmin=16, lmax=96, zipf=1.0, nq=80, tmin=1, tmax=8),
-    dict(name="dense", seed=23, n=5000, vocab=40, lmin=5, lmax=400, zipf=1.1, nq=60, tmin=1, tmax=8),
-    dict(name="manyterms", seed=24, n=8000, vocab=600, lmin=8, lmax=64, zipf=0.8, nq=40, tmin=9, tmax=32),
-    dict(name="ties", seed=25, n=50000, vocab=200, lmin=16, lmax=16, zipf=0.0, nq=60, tmin=1, tmax=4),
-]
-
-
-@pytest.mark.parametrize("cfg", CONFIGS, ids=[c["name"] for c in CONFIGS])
+@pytest.mark.parametrize("cfg", PARITY_CONFIGS, ids=[c["name"] for c in PARITY_CONFIGS])
 def test_search_matches_oracle(m, orc, cfg):
     c = m.synth_corpus(cfg["seed"], cfg["n"], cfg["vocab"], cfg["lmin"], cfg["lmax"], cfg["zipf"])
     q_off, q_terms = m.synth_queries(cfg["seed"] + 1000, cfg["nq"], cfg["vocab"], cfg["tmin"], cfg["tmax"],
                                      c.post_off, cfg["zipf"])
     ix = m.Index.from_corpus(c)
-    oix = _oracle_index(orc, c)
+    oix = oracle_index(orc, c)
     for k in (1, 10, 100, 1000):
         res = ix.search_batch(q_off, q_terms, k)
-        _compare(res, oix, q_off, q_terms, k, what=cfg["name"])
+        compare(res, oix, q_off, q_terms, k, what=cfg["name"])
     ix.close()
 
 
 def test_golden_sqllogictest_ranking(m, orc, golden):
-    from test_oracle_golden import _slt_corpus
     for ids, want in [(list(range(1, 11)), golden["ranking_full_index"]), ([2, 4, 6, 8, 10], golden["ranking_even_ids"]),
                       ([1, 3, 5, 7, 9], golden["ranking_odd_ids"])]:
-        c, tid = _slt_corpus(orc, golden, ids)
+        c, tid = slt_corpus(orc, golden, ids)
         ix = m.Index(c.n_docs, c.doc_len, c.n_terms, c.post_off, c.post_doc, c.post_tf)
         docs, scores = ix.search([tid["postgresql"]], 10)
         assert [ids[d] for d in docs] == want
@@ -220,13 +135,12 @@ def test_golden_sqllogictest_ranking(m, orc, golden):
 def test_edge_cases(m, orc):
     c = m.synth_corpus(31, 3000, 100, 4, 40, 0.0)
     ix = m.Index.from_corpus(c)
-    oix = _oracle_index(orc, c)
+    oix = oracle_index(orc, c)
     # empty query, unknown terms, duplicates, unsorted, TERM_MISSING (search.rs:55-62)
     qs = [[], [1000000], [5, 5, 9, 5], [9, 5], [m.TERM_MISSING, 7], [3]]
-    q_off = np.cumsum([0] + [len(q) for q in qs]).astype(np.uint32)
-    q_terms = np.array([t for q in qs for t in q], dtype=np.uint32)
+    q_off, q_terms = query_csr(qs)
     res = ix.search_batch(q_off, q_terms, 7, want_payload=True)
-    _compare(res, oix, q_off, q_terms, 7, what="edge")
+    compare(res, oix, q_off, q_terms, 7, what="edge")
     assert res["n"][0] == 0 and res["n"][1] == 0
     assert np.array_equal(res["doc"][2], res["doc"][3])
     # payload default = synthetic ctid of the doc id
@@ -248,13 +162,13 @@ def test_edge_cases(m, orc):
 def test_prefilter_bitmap(m, orc):
     c = m.synth_corpus(41, 20000, 300, 8, 60, 0.9)
     ix = m.Index.from_corpus(c)
-    oix = _oracle_index(orc, c)
+    oix = oracle_index(orc, c)
     rng = np.random.default_rng(5)
     keep = rng.random(c.n_docs) < 0.2
     allow = np.packbits(keep, bitorder="little")
     q_off, q_terms = m.synth_queries(42, 40, 300, 1, 6, c.post_off, 0.9)
     res = ix.search_batch(q_off, q_terms, 25, allow=allow)
-    _compare(res, oix, q_off, q_terms, 25, allow=allow, what="prefilter")
+    compare(res, oix, q_off, q_terms, 25, allow=allow, what="prefilter")
     ix.close()
 
 
@@ -264,13 +178,13 @@ def test_pruning_on_off_identical(m, orc):
     c = m.synth_corpus(71, 60000, 3000, 24, 96, 1.0)
     q_off, q_terms = m.synth_queries(72, 200, 3000, 2, 8, c.post_off, 1.0)
     ix = m.Index.from_corpus(c)
-    oix = _oracle_index(orc, c)
+    oix = oracle_index(orc, c)
     on = ix.search_batch(q_off, q_terms, 10)
     ix.set_option("prune", 0)
     off = ix.search_batch(q_off, q_terms, 10)
     for key in ("doc", "score", "score64", "n"):
         assert np.array_equal(on[key], off[key]), key
-    _compare(on, oix, q_off, q_terms, 10, what="prune")
+    compare(on, oix, q_off, q_terms, 10, what="prune")
     if os.environ.get("BM25X_SEED_FORCE", "0") in ("", "0"):  # (a seeded launch never prunes: nothing to compare)
         assert 0 < on["stats"].postings_fetched < off["stats"].postings_fetched
     with pytest.raises(m.Bm25xError):
@@ -286,7 +200,7 @@ def test_kernel_paths_identical(m, orc, zipf):
     c = m.synth_corpus(81, 80000, 400 if zipf == 0.0 else 4000, 6, 40, zipf)
     q_off, q_terms = m.synth_queries(82, 160, c.n_terms, 2, 4, c.post_off, zipf)
     ix = m.Index.from_corpus(c)
-    oix = _oracle_index(orc, c)
+    oix = oracle_index(orc, c)
     for k in (1, 10, 100, 128, 129, 224):
         for prune in (1, 0):
             ix.set_option("prune", prune)
@@ -303,7 +217,7 @@ def test_kernel_paths_identical(m, orc, zipf):
             for name in ("seeded", "handback", "dense", "twophase"):
                 for key in ("doc", "score", "score64", "n"):
                     assert np.array_equal(got[name][key], got["plain"][key]), (name, key, k, prune)
-        _compare(got["seeded"], oix, q_off[:25], q_terms, k, what=f"paths k={k}")
+        compare(got["seeded"], oix, q_off[:25], q_terms, k, what=f"paths k={k}")
     ix.close()
 
 
@@ -332,7 +246,7 @@ def test_replica_same_device_identical(m, orc):
             a, b = ix.search_batch(q_off, q_terms, k), rep.search_batch(q_off, q_terms, k)
             for key in ("doc", "score", "score64", "n"):
                 assert np.array_equal(a[key], b[key]), (key, seed, k)
-    _compare(b, _oracle_index(orc, c), q_off[:30], q_terms, 100, what="replica")
+    compare(b, oracle_index(orc, c), q_off[:30], q_terms, 100, what="replica")
     rep.close()
     ix.close()
 
@@ -391,14 +305,14 @@ def test_sliced_search_batch_identical(m, orc):
             assert np.array_equal(one[key], cut[key]), key
         assert cut["stats"].queries == one["stats"].queries and cut["stats"].postings == one["stats"].postings
         assert cut["stats"].bytes_algo == one["stats"].bytes_algo and cut["stats"].launches >= one["stats"].launches
-    _compare(cut, _oracle_index(orc, c), q_off[:30], q_terms, 10, allow=allow, what="sliced")
+    compare(cut, oracle_index(orc, c), q_off[:30], q_terms, 10, allow=allow, what="sliced")
     ix.close()
 
 
 def test_evaluate_matches_oracle_bitwise(m, orc):
     c = m.synth_corpus(51, 5000, 400, 2, 120, 0.8)
     ix = m.Index.from_corpus(c)
-    oix = _oracle_index(orc, c)
+    oix = oracle_index(orc, c)
     rng = np.random.default_rng(7)
     docs, queries = [], []
     for _ in range(300):
@@ -418,7 +332,7 @@ def test_wand_reference_path_agrees_tie_aware(m, orc):
     the comparison a real reference run would need (SURVEY §8c)."""
     c = m.synth_corpus(61, 40000, 2000, 16, 80, 1.0)
     ix = m.Index.from_corpus(c)
-    oix = _oracle_index(orc, c)
+    oix = oracle_index(orc, c)
     q_off, q_terms = m.synth_queries(62, 50, 2000, 1, 8, c.post_off, 1.0)
     res = ix.search_batch(q_off, q_terms, 10)
     for i in range(50):
@@ -441,11 +355,11 @@ def test_config2_sample_1M_docs(m, orc):
     assert np.all(s[:, :-1] >= s[:, 1:])                                   # sortedness
     tie = s[:, :-1] == s[:, 1:]
     assert np.all(res["doc"][:, :-1][tie] < res["doc"][:, 1:][tie])        # canonical tie order
-    oix = _oracle_index(orc, c)
+    oix = oracle_index(orc, c)
     idx = np.arange(0, 10000, 97)
     sub_off = np.arange(len(idx) + 1, dtype=np.uint32)
     sub = {k: (v[idx] if isinstance(v, np.ndarray) else v) for k, v in res.items()}
-    _compare(sub, oix, sub_off, q_terms[idx], 10, what="C2")
+    compare(sub, oix, sub_off, q_terms[idx], 10, what="C2")
     ix.close()
 
 
@@ -468,8 +382,8 @@ def test_lookup_terms_16_byte_keys_then_search(m, orc):
     # a query in key space: unknown tokens are dropped, the rest searched — identical to the ordinal query
     q_off = np.array([0, len(ords)], dtype=np.uint32)
     res = ix.search_batch(q_off, ords, 10)
-    oix = _oracle_index(orc, c)
-    _compare(res, oix, np.array([0, 4], dtype=np.uint32), np.array([5, 17, 299, 0], dtype=np.uint32), 10, what="lookup")
+    oix = oracle_index(orc, c)
+    compare(res, oix, np.array([0, 4], dtype=np.uint32), np.array([5, 17, 299, 0], dtype=np.uint32), 10, what="lookup")
     ix.close()
     # keys must be strictly ascending (the reference's token address tree is sorted): rejected at create
     bad = keys.copy()

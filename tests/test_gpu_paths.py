@@ -7,32 +7,13 @@ test_gpu_parity.py::test_more_than_32_terms_two_passes."""
 import numpy as np
 import pytest
 
-import _pkg
-from test_gpu_parity import _compare, _csr_corpus, _live_queries, _oracle_index, _PrefixOracle
-from util_parity import same_rows
-from test_gpu_zz_growing import _expect, _setup
+from util_corpora import csr_corpus
 from util_index import assert_matches, read_back, restate
+from util_lib import gpu_library, set_options  # noqa: F401  (gpu_library: the module fixture m)
+from util_parity import KERNEL_PATHS, PrefixOracle, compare, live_queries, oracle_index, query_csr, same_rows
+from util_segment import growing_expect, growing_setup
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def m():
-    mod = _pkg.load()
-    mod.load_library()
-    assert mod.device_count() >= 1, "no CUDA device: the engine has no CPU fallback"
-    return mod
-
-
-# kernel paths of the 2..8-term classes, as index options (a seeded launch that keeps every query: no hand-back)
-PATHS = dict(seeded=dict(seed=1, twophase=0, seed_prune_min=0xFFFFFFFF, seed_dense_div=0),
-             twophase=dict(seed=0, twophase=1),
-             plain=dict(seed=0, twophase=0))
-
-
-def _set(ix, **opts):
-    for name, value in opts.items():
-        ix.set_option(name, value)
 
 
 def test_class_boundary_matrix_sliced(m, orc):
@@ -43,13 +24,12 @@ def test_class_boundary_matrix_sliced(m, orc):
     ix = m.Index.from_corpus(c)
     rng = np.random.default_rng(201)
     counts = [1, 2, 3, 4, 5, 8, 9, 16, 17, 32, 33, 64] * 6
-    q_off, q_terms = _live_queries(rng, ix.df(), counts)
+    q_off, q_terms = live_queries(rng, ix.df(), counts)
     qs = [q_terms[q_off[i]:q_off[i + 1]] for i in range(len(counts))] + [np.zeros(0, np.uint32),
                                                                           np.array([m.TERM_MISSING, 10 ** 7], np.uint32)]
     qs = [qs[i] for i in rng.permutation(len(qs))]
-    q_off = np.cumsum([0] + [len(q) for q in qs]).astype(np.uint32)
-    q_terms = np.concatenate(qs).astype(np.uint32)
-    oix = _PrefixOracle(_oracle_index(orc, c), 100)
+    q_off, q_terms = query_csr(qs)
+    oix = PrefixOracle(oracle_index(orc, c), 100)
     for k in (10, 100):
         ix.set_option("slice_min", 0)
         one = ix.search_batch(q_off, q_terms, k, want_payload=True)
@@ -58,7 +38,7 @@ def test_class_boundary_matrix_sliced(m, orc):
         assert cut["stats"].launches > one["stats"].launches
         same_rows(one, cut, f"sliced k={k}")
         assert np.array_equal(one["payload"], cut["payload"])
-        _compare(one, oix, q_off, q_terms, k, what=f"class matrix k={k}")
+        compare(one, oix, q_off, q_terms, k, what=f"class matrix k={k}")
     ix.close()
 
 
@@ -72,7 +52,7 @@ def test_limits_above_1024_hbm_pools(m, orc):
     df = ix.df()
     rng = np.random.default_rng(211)
     counts = [1, 3, 8] * 3
-    q_off, q_terms = _live_queries(rng, df, counts)
+    q_off, q_terms = live_queries(rng, df, counts)
     allow = np.packbits(rng.random(c.n_docs) < 0.6, bitorder="little")
     keep = np.unpackbits(allow, bitorder="little")[:c.n_docs].astype(bool)
 
@@ -84,7 +64,7 @@ def test_limits_above_1024_hbm_pools(m, orc):
     assert max(hits) > 65535 > min(hits), hits
     assert max(matches(i, allow) for i in range(len(counts))) > 65535
     ks = (1024, 1025, 5000, 65535)
-    oix = _PrefixOracle(_oracle_index(orc, c), max(ks))
+    oix = PrefixOracle(oracle_index(orc, c), max(ks))
     for k in ks:
         for al in (None, allow):
             ix.set_option("prune", 1)
@@ -92,20 +72,20 @@ def test_limits_above_1024_hbm_pools(m, orc):
             ix.set_option("prune", 0)
             off = ix.search_batch(q_off, q_terms, k, allow=al)
             same_rows(on, off, f"prune on/off k={k} allow={al is not None}")
-            _compare(on, oix, q_off, q_terms, k, allow=al, what=f"hbm pool k={k} allow={al is not None}")
+            compare(on, oix, q_off, q_terms, k, allow=al, what=f"hbm pool k={k} allow={al is not None}")
     ix.set_option("prune", 1)
     ix.close()
 
 
 def test_growing_segment_limit_2000(m, orc):
     """Sealed + growing search at a limit of the HBM-pool class: both top-2000 lists and their merge."""
-    sealed, g, ix, gix, oix = _setup(m, orc, 63, 3000, 3000, 60, 5, 1.0)
+    sealed, g, ix, gix, oix = growing_setup(m, orc, 63, 3000, 3000, 60, 5, 1.0)
     N = sealed.n_docs
     q_off, q_terms = m.synth_queries(1063, 24, 60, 1, 8, sealed.post_off, 1.0)
     both = ix.search_batch_growing(gix, q_off, q_terms, 2000)
     cut = 0
     for i in range(len(q_off) - 1):
-        ed, es = _expect(oix, g, N, q_terms[q_off[i]:q_off[i + 1]], 2000)
+        ed, es = growing_expect(oix, g, N, q_terms[q_off[i]:q_off[i + 1]], 2000)
         n = int(both["n"][i])
         assert n == len(ed) and both["doc"][i, :n].tolist() == ed, f"q{i} merged ids"
         assert both["score64"][i, :n].tolist() == es, f"q{i} merged f64 scores"
@@ -129,20 +109,20 @@ def test_seeded_5_to_8_terms(m, orc):
     n_live = np.diff(q_off)
     assert n_live.min() == 5 and n_live.max() == 8
     assert int(df[q_terms].max()) < min(c.n_docs // 64, 32768)  # the default hand-back thresholds
-    oix = _PrefixOracle(_oracle_index(orc, c), 129)
+    oix = PrefixOracle(oracle_index(orc, c), 129)
     for k in (1, 10, 127, 128, 129):
         got = {}
         for name, opts in dict(seed8=dict(seed=1, seed_max_terms=8), seed4=dict(seed=1, seed_max_terms=4),
                                off=dict(seed=0, seed_max_terms=8)).items():
             for prune in (1, 0):
-                _set(ix, prune=prune, **opts)
+                set_options(ix, prune=prune, **opts)
                 got[name, prune] = ix.search_batch(q_off, q_terms, k)
         for key, res in got.items():
             same_rows(res, got["off", 1], f"{key} k={k}")
         # one class (8) in the batch: a seeded launch and the launch of its hand-back list, else one launch
         assert got["seed8", 1]["stats"].launches == (2 if k <= 128 else 1)
         assert got["seed4", 1]["stats"].launches == 1
-        _compare(got["seed8", 1], oix, q_off[:41], q_terms, k, what=f"seeded 5..8 k={k}")
+        compare(got["seed8", 1], oix, q_off[:41], q_terms, k, what=f"seeded 5..8 k={k}")
     ix.close()
 
 
@@ -157,18 +137,18 @@ def test_k1_b_edges(m, orc, k1, b):
     ix = m.Index(c.n_docs, c.doc_len, c.n_terms, c.post_off, c.post_doc, c.post_tf, k1=k1, b=b)
     info = ix.info()
     assert (info.k1, info.b) == (k1, b)
-    oix = _PrefixOracle(orc.OracleIndex(orc.Corpus(c.n_docs, c.doc_len, c.n_terms, c.post_off, c.post_doc, c.post_tf,
+    oix = PrefixOracle(orc.OracleIndex(orc.Corpus(c.n_docs, c.doc_len, c.n_terms, c.post_off, c.post_doc, c.post_tf,
                                                    k1=k1, b=b)), 1000)
     q_off, q_terms = m.synth_queries(232, 120, c.n_terms, 1, 8, c.post_off, 0.6)
     for k in (1, 10, 128, 129, 224, 1000):
         got = {}
-        for name, opts in PATHS.items():
+        for name, opts in KERNEL_PATHS.items():
             for prune in (1, 0):
-                _set(ix, prune=prune, **opts)
+                set_options(ix, prune=prune, **opts)
                 got[name, prune] = ix.search_batch(q_off, q_terms, k)
         for key, res in got.items():
             same_rows(res, got["plain", 1], f"{key} k={k}")
-        _compare(got["seeded", 1], oix, q_off, q_terms, k, what=f"k1={k1} b={b} k={k}")
+        compare(got["seeded", 1], oix, q_off, q_terms, k, what=f"k1={k1} b={b} k={k}")
     ix.close()
 
 
@@ -187,23 +167,22 @@ def test_b0_tie_flood_at_champion_cut(m, orc):
     for _ in range(3):  # filler terms: document lengths (norms) vary
         d = np.sort(rng.choice(n_docs, size=2500, replace=False))
         lists.append((d, rng.integers(1, 7, size=len(d))))
-    doc_len, off, pd_, pt = _csr_corpus(rng, n_docs, lists, extra_len=300)
+    doc_len, off, pd_, pt = csr_corpus(rng, n_docs, lists, extra_len=300)
     T = len(lists)
     for k1 in (1.2, 2.0):
         ix = m.Index(n_docs, doc_len, T, off, pd_, pt, k1=k1, b=0.0)
-        oix = _PrefixOracle(orc.OracleIndex(orc.Corpus(n_docs, doc_len, T, off, pd_, pt, k1=k1, b=0.0)), 1001)
+        oix = PrefixOracle(orc.OracleIndex(orc.Corpus(n_docs, doc_len, T, off, pd_, pt, k1=k1, b=0.0)), 1001)
         qs = [[0], [0, 1], [2, 1], [0, 2], [0, 1, 2], [0, 3], [2, 4, 1]]
-        q_off = np.cumsum([0] + [len(q) for q in qs]).astype(np.uint32)
-        q_terms = np.array([t for q in qs for t in q], dtype=np.uint32)
+        q_off, q_terms = query_csr(qs)
         for k in (127, 128, 129, 1000):
             got = {}
             for name in ("seeded", "plain"):
                 for prune in (1, 0):
-                    _set(ix, prune=prune, **PATHS[name])
+                    set_options(ix, prune=prune, **KERNEL_PATHS[name])
                     got[name, prune] = ix.search_batch(q_off, q_terms, k)
             for key, res in got.items():
                 same_rows(res, got["plain", 1], f"{key} k1={k1} k={k}")
-            _compare(got["seeded", 1], oix, q_off, q_terms, k, what=f"tie flood k1={k1} k={k}")
+            compare(got["seeded", 1], oix, q_off, q_terms, k, what=f"tie flood k1={k1} k={k}")
             if k < 1000:  # the cut is inside a tie group: the last row of [0, 1] ties with rows it excludes
                 assert got["plain", 1]["score64"][1, k - 1] == oix.search_exhaustive(qs[1], k + 1)[1][k]
         ix.close()
@@ -215,7 +194,7 @@ def test_near_ties_at_the_kth_score(m, orc):
     0 < (s[i-1] - s[i]) / s[i] < 2^-17, then the GPU at limit k = i on every kernel path, pruning on and off."""
     c = m.synth_corpus(251, 20000, 300, 1, 300, 0.0)  # lists of ~5000 postings: crowded scores, thousands of near ties
     ix = m.Index.from_corpus(c)
-    oix = _oracle_index(orc, c)
+    oix = oracle_index(orc, c)
     q_off, q_terms = m.synth_queries(252, 300, c.n_terms, 1, 6, c.post_off, 0.0)
     ranking, cases = {}, []
     for qi in range(len(q_off) - 1):
@@ -237,9 +216,9 @@ def test_near_ties_at_the_kth_score(m, orc):
         sub_off = np.cumsum([0] + [int(q_off[i + 1] - q_off[i]) for i in qis]).astype(np.uint32)
         sub_terms = np.concatenate([q_terms[q_off[i]:q_off[i + 1]] for i in qis]).astype(np.uint32)
         first = None
-        for name, opts in PATHS.items():
+        for name, opts in KERNEL_PATHS.items():
             for prune in (1, 0):
-                _set(ix, prune=prune, **opts)
+                set_options(ix, prune=prune, **opts)
                 res = ix.search_batch(sub_off, sub_terms, k)
                 if first is None:
                     first = res

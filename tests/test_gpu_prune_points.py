@@ -25,13 +25,10 @@ runs the case with pruning on and off, compares both bit for bit with OracleInde
 import numpy as np
 import pytest
 
-import _pkg
 import util_filter as uf
 import util_prune as up
-from test_gpu_parity import _compare, _PrefixOracle
-from util_parity import same_rows
-from test_gpu_margin_paths import _hands_back
-from test_gpu_paths import _set
+from util_lib import gpu_library, set_options  # noqa: F401  (gpu_library: the module fixture m)
+from util_parity import PrefixOracle, compare, query_csr, same_rows
 
 SEEDED8 = dict(seed=1, twophase=0, seed_max_terms=8, seed_prune_min=0xFFFFFFFF, seed_dense_div=0)
 PLAIN = dict(seed=0, twophase=0)
@@ -46,14 +43,6 @@ def _cached(key, make):
     return _CACHE[key]
 
 
-@pytest.fixture(scope="module")
-def m():
-    mod = _pkg.load()
-    mod.load_library()
-    assert mod.device_count() >= 1, "no CUDA device: the engine has no CPU fallback"
-    return mod
-
-
 def _oracle(orc, c):
     return orc.OracleIndex(orc.Corpus(c.n_docs, c.doc_len, c.n_terms, c.post_off, c.post_doc, c.post_tf, k1=up.K1, b=up.B))
 
@@ -62,18 +51,14 @@ def _index(m, c):
     return m.Index(c.n_docs, c.doc_len, c.n_terms, c.post_off, c.post_doc, c.post_tf, k1=up.K1, b=up.B)
 
 
-def _qoff(qs):
-    return np.cumsum([0] + [len(q) for q in qs]).astype(np.uint32), np.concatenate(qs).astype(np.uint32)
-
-
 def _run_both(ix, oix, q_off, q_terms, k, opts, launches, what):
     """Pruning on and off: each against the oracle, both the same rows; returns (on, off)."""
     got = []
     for prune in (1, 0):
-        _set(ix, prune=prune, **opts)
+        set_options(ix, prune=prune, **opts)
         res = ix.search_batch(q_off, q_terms, k)
         assert res["stats"].launches == launches, (what, prune, res["stats"].launches)
-        _compare(res, oix, q_off, q_terms, k, what=f"{what} prune={prune}")
+        compare(res, oix, q_off, q_terms, k, what=f"{what} prune={prune}")
         got.append(res)
     same_rows(got[0], got[1], f"{what}: pruning on / off")
     return got
@@ -142,16 +127,16 @@ def test_ring_start_geometry(m, orc):
     c = _ring_fixture(orc)
     qs = _ring_queries(c)
     ix = _index(m, c)
-    oix = _PrefixOracle(_oracle(orc, c), 100)
+    oix = PrefixOracle(_oracle(orc, c), 100)
     for cls, queries in qs.items():
-        q_off, q_terms = _qoff(queries)
+        q_off, q_terms = query_csr(queries)
         seeded = cls == "seeded8"
         classes = {min(x for x in (8, 16, 32, 64) if x >= len(q)) for q in queries}
         for k in (10, 100):
             if seeded:  # the seeded launch's hand-back test at query start: it keeps every query
                 for q in queries:
                     for prune in (1, 0):
-                        assert not _hands_back(dict(df=c.df[q], n_docs=c.n_docs), SEEDED8, prune)
+                        assert not uf.hands_back(dict(df=c.df[q], n_docs=c.n_docs), SEEDED8, prune)
             launches = (2 if seeded else 1) * len(classes)
             _run_both(ix, oix, q_off, q_terms, k, SEEDED8 if seeded else PLAIN, launches, f"rings {cls} k={k}")
     ix.close()
@@ -240,7 +225,7 @@ def test_prune_point_gpu(m, orc, name):
     c, mo = _prune_fixture(orc, name)
     ix = _index(m, c)
     oix = _oracle(orc, c)
-    q_off, q_terms = _qoff([c.q])
+    q_off, q_terms = query_csr([c.q])
     on, off = _run_both(ix, oix, q_off, q_terms, k, PLAIN, 1, name)
     st_on, st_off = on["stats"], off["stats"]
     assert st_off.postings_fetched == st_off.postings
@@ -291,7 +276,7 @@ def test_probe_edges_model(orc, name):
 def test_probe_edges_gpu(m, orc, name):
     c = _probe_fixture(orc, name)
     ix = _index(m, c)
-    q_off, q_terms = _qoff([c.q])
+    q_off, q_terms = query_csr([c.q])
     for k in (10, 40):
         _run_both(ix, _oracle(orc, c), q_off, q_terms, k, PLAIN, 1, f"{name} k={k}")
     ix.close()
@@ -371,7 +356,7 @@ def test_pair_model(orc, name):
 def test_pair_gpu(m, orc, name, path):
     c = _pair_fixture(orc, name)
     ix = _index(m, c)
-    q_off, q_terms = _qoff([c.q])
+    q_off, q_terms = query_csr([c.q])
     on, _ = _run_both(ix, _oracle(orc, c), q_off, q_terms, c.k, PLAIN if path == "plain" else TWOPHASE,
                       1 if path == "plain" else 2, f"{name} {path}")
     assert c.y in on["doc"][0].tolist()
@@ -406,7 +391,7 @@ def test_two_pass_model(orc):
 def test_two_pass_gpu(m, orc):
     c = _two_pass_fixture(orc)
     ix = _index(m, c)
-    q_off, q_terms = _qoff([c.q])
+    q_off, q_terms = query_csr([c.q])
     on, _ = _run_both(ix, _oracle(orc, c), q_off, q_terms, c.k, PLAIN, 1, "two-pass")
     assert set(c.X) <= set(on["doc"][0].tolist())
     ix.close()

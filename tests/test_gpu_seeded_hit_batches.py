@@ -8,9 +8,9 @@ doc ids, f32 and f64 scores, counts and the unused slots (0xFFFFFFFF) must be th
 import numpy as np
 import pytest
 
-import _pkg
-from test_gpu_parity import _compare, _csr_corpus, _PrefixOracle
-from util_parity import same_rows
+from util_corpora import csr_corpus
+from util_lib import gpu_library, set_options  # noqa: F401  (gpu_library: the module fixture m)
+from util_parity import PrefixOracle, compare, query_csr, same_rows
 
 pytestmark = pytest.mark.gpu
 
@@ -19,37 +19,19 @@ PLAIN = dict(seed=0, twophase=0)
 KS = (1, 10, 64, 128)
 
 
-@pytest.fixture(scope="module")
-def m():
-    mod = _pkg.load()
-    mod.load_library()
-    assert mod.device_count() >= 1, "no CUDA device: the engine has no CPU fallback"
-    return mod
-
-
-def _set(ix, **opts):
-    for name, value in opts.items():
-        ix.set_option(name, value)
-
-
-def _queries(qs):
-    q_off = np.cumsum([0] + [len(q) for q in qs]).astype(np.uint32)
-    return q_off, np.array([t for q in qs for t in q], dtype=np.uint32)
-
-
 def _both_paths(m, ix, oix, qs, what, ks=KS):
     """Seeded and plain launches at every limit: identical rows, equal to the oracle."""
-    q_off, q_terms = _queries(qs)
+    q_off, q_terms = query_csr(qs)
     for k in ks:
         got = {}
         for name, opts in dict(seeded=SEEDED, plain=PLAIN).items():
             for prune in (1, 0):
-                _set(ix, prune=prune, **opts)
+                set_options(ix, prune=prune, **opts)
                 got[name, prune] = ix.search_batch(q_off, q_terms, k)
         for key, res in got.items():
             same_rows(res, got["plain", 1], f"{what} {key} k={k}")
             assert np.all(res["doc"][np.arange(k)[None, :] >= res["n"][:, None]] == 0xFFFFFFFF), f"{what} {key} k={k}"
-        _compare(got["seeded", 0], oix, q_off, q_terms, k, what=f"{what} k={k}")
+        compare(got["seeded", 0], oix, q_off, q_terms, k, what=f"{what} k={k}")
 
 
 def _correlated(rng, n_docs, groups, size, share, tf_hi, extra_len):
@@ -63,7 +45,7 @@ def _correlated(rng, n_docs, groups, size, share, tf_hi, extra_len):
             own = rng.choice(n_docs, size=size // 10, replace=False)
             d = np.unique(np.concatenate([pool[rng.random(size) < share], own]))
             lists.append((d, rng.integers(1, tf_hi + 1, size=len(d))))
-    return _csr_corpus(rng, n_docs, lists, extra_len=extra_len)
+    return csr_corpus(rng, n_docs, lists, extra_len=extra_len)
 
 
 @pytest.mark.parametrize("share", [0.5, 0.9])
@@ -77,7 +59,7 @@ def test_correlated_lists_fill_the_list_often(m, orc, share):
     T = len(off) - 1
     assert int(np.diff(off).max()) < n_docs // 64
     ix = m.Index(n_docs, doc_len, T, off, pd_, pt)
-    oix = _PrefixOracle(orc.OracleIndex(orc.Corpus(n_docs, doc_len, T, off, pd_, pt)), max(KS))
+    oix = PrefixOracle(orc.OracleIndex(orc.Corpus(n_docs, doc_len, T, off, pd_, pt)), max(KS))
     qs = []
     for g in range(6):
         base = 8 * g
@@ -103,10 +85,10 @@ def test_hits_only_in_the_last_window(m, orc):
     for _ in range(4):  # fillers: varied norms
         d = np.sort(rng.choice(n_docs, size=3000, replace=False))
         lists.append((d, rng.integers(1, 5, size=len(d))))
-    doc_len, off, pd_, pt = _csr_corpus(rng, n_docs, lists, extra_len=30)
+    doc_len, off, pd_, pt = csr_corpus(rng, n_docs, lists, extra_len=30)
     T = len(lists)
     ix = m.Index(n_docs, doc_len, T, off, pd_, pt)
-    oix = _PrefixOracle(orc.OracleIndex(orc.Corpus(n_docs, doc_len, T, off, pd_, pt)), max(KS))
+    oix = PrefixOracle(orc.OracleIndex(orc.Corpus(n_docs, doc_len, T, off, pd_, pt)), max(KS))
     qs = [[0, 1], [0, 2, 3], [0, 1, 2, 3], [1, 2, 3], [0, 1, 2, 3, 4, 5], [0, 1, 2, 3, 4, 5, 6, 7]]
     _both_paths(m, ix, oix, qs, "last window")
     ix.close()
@@ -132,10 +114,10 @@ def test_tie_flood_across_flushes(m, orc, k1):
     for _ in range(3):  # fillers: document lengths vary (irrelevant at b = 0, kept for the norms)
         d = np.sort(rng.choice(n_docs, size=5000, replace=False))
         lists.append((d, rng.integers(1, 7, size=len(d))))
-    doc_len, off, pd_, pt = _csr_corpus(rng, n_docs, lists, extra_len=200)
+    doc_len, off, pd_, pt = csr_corpus(rng, n_docs, lists, extra_len=200)
     T = len(lists)
     ix = m.Index(n_docs, doc_len, T, off, pd_, pt, k1=k1, b=0.0)
-    oix = _PrefixOracle(orc.OracleIndex(orc.Corpus(n_docs, doc_len, T, off, pd_, pt, k1=k1, b=0.0)), max(KS) + 1)
+    oix = PrefixOracle(orc.OracleIndex(orc.Corpus(n_docs, doc_len, T, off, pd_, pt, k1=k1, b=0.0)), max(KS) + 1)
     qs = [[0, 1], [0, 1, 2], [0, 1, 2, 3], [0, 4], [0, 1, 4], [1, 2, 3, 4], [0, 1, 2, 3, 4], [0, 1, 2, 3, 4, 5, 6, 7]]
     _both_paths(m, ix, oix, qs, f"tie flood k1={k1}")
     # the cut falls inside a tie group: the k-th row ties with the (k+1)-th the oracle ranks behind it
@@ -161,14 +143,14 @@ def test_seeds_held_by_another_run(m, orc):
     d3 = np.setdiff1d(rng.choice(n_docs, size=3000, replace=False), np.concatenate([d0, d1, d2]))
     lists = [(d0, tf0), (d1, rng.integers(1, 4, size=len(d1))), (d2, rng.integers(1, 4, size=len(d2))),
              (d3, np.full(len(d3), 9, np.uint32))]
-    doc_len, off, pd_, pt = _csr_corpus(rng, n_docs, lists, extra_len=20)
+    doc_len, off, pd_, pt = csr_corpus(rng, n_docs, lists, extra_len=20)
     T = len(lists)
     ix = m.Index(n_docs, doc_len, T, off, pd_, pt)
-    oix = _PrefixOracle(orc.OracleIndex(orc.Corpus(n_docs, doc_len, T, off, pd_, pt)), max(KS))
+    oix = PrefixOracle(orc.OracleIndex(orc.Corpus(n_docs, doc_len, T, off, pd_, pt)), max(KS))
     qs = [[0, 1], [0, 1, 2], [0, 1, 2, 3], [0, 3], [1, 2, 3]]
     _both_paths(m, ix, oix, qs, "seeds held twice")
-    q_off, q_terms = _queries(qs)
-    _set(ix, prune=0, **SEEDED)
+    q_off, q_terms = query_csr(qs)
+    set_options(ix, prune=0, **SEEDED)
     res = ix.search_batch(q_off, q_terms, 128)
     for i in range(len(qs)):
         n = int(res["n"][i])

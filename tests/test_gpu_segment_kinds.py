@@ -12,13 +12,13 @@ from types import SimpleNamespace
 import numpy as np
 import pytest
 
-import _pkg
-from test_gpu_parity import _live_queries
-from test_gpu_seal import Docs, World, _check_result, _check_searches, _keys, _new_docs, _pack, _sealed_docs
-from test_gpu_segment_steps import check_segment, first_docs
 from util_cuda import D2D, cudart
 from util_index import CHAMP_L, fieldnorms
+from util_lib import gpu_library  # noqa: F401  (gpu_library: the module fixture m)
 from util_maintain import maintain
+from util_parity import live_queries
+from util_segment import (Docs, World, check_result, check_searches, check_segment, first_docs, new_docs, pack,
+                          random_keys, sealed_docs)
 
 pytestmark = pytest.mark.gpu
 
@@ -28,24 +28,16 @@ N, T, N_NEW = 2500, 160, 6
 TIE, TIE_TF = 5, 7          # a term with 100 sealed and 60 growing postings of one tf, above every other tf of the corpus
 
 
-@pytest.fixture(scope="module")
-def m():
-    mod = _pkg.load()
-    mod.load_library()
-    assert mod.device_count() >= 1, "no CUDA device: the engine has no CPU fallback"
-    return mod
-
-
 def _corpus(orc, rng, keyed):
-    """test_gpu_seal's sealed documents, 100 of them with the tie term."""
-    docs, dead = _sealed_docs(rng, N, T)
+    """The sealed documents of util_segment.sealed_docs, 100 of them with the tie term."""
+    docs, dead = sealed_docs(rng, N, T)
     for d in range(100, 200):
         docs[d][TIE] = TIE_TF
     c = orc.Corpus.from_docs(docs, n_terms=T)
     return SimpleNamespace(docs=docs, dead=dead, off=c.post_off, doc=c.post_doc, tf=c.post_tf,
                            doc_len=c.doc_len + rng.integers(0, 5, size=N).astype(np.uint32),
                            payload=rng.integers(0, 65536, size=(N, 3)).astype(np.uint16),
-                           keys=np.array(sorted(_keys(rng, T).tolist()), np.uint8) if keyed else None)
+                           keys=np.array(sorted(random_keys(rng, T).tolist()), np.uint8) if keyed else None)
 
 
 def _world(m, c, k1, b, ix=None, keys=None):
@@ -55,14 +47,14 @@ def _world(m, c, k1, b, ix=None, keys=None):
 def _script(m, orc, rng, w, c, form, what):
     """The script on the sealed World w (closed at the end, with everything made from it)."""
     k1, b, keyed = w.k1, w.b, w.keys is not None
-    new_keys = _keys(rng, N_NEW, w.keys) if keyed else None
+    new_keys = random_keys(rng, N_NEW, w.keys) if keyed else None
     docs = Docs()
-    _new_docs(rng, w, c.dead, docs, 100, N_NEW)
+    new_docs(rng, w, c.dead, docs, 100, N_NEW)
     for i in range(60):                                          # the growing part of the tie group
         docs.add([TIE], [TIE_TF], i % 3, False, rng.integers(0, 65536, size=3).tolist())
     copy = sorted(c.docs[7].items())                             # a growing copy of sealed document 7
     docs.add([t for t, _ in copy], [f for _, f in copy], 0, False, [7, 7, 7])
-    _new_docs(rng, w, c.dead, docs, 50, N_NEW)
+    new_docs(rng, w, c.dead, docs, 50, N_NEW)
     seg = w.ix.growing_segment()
     made = [w.ix]
     try:
@@ -78,7 +70,7 @@ def _script(m, orc, rng, w, c, form, what):
         check_segment(orc, seg, w, docs, form, True, f"{what}, second refresh", k1, b)
         sdel = rng.random(N) < 0.1
         sdel[7] = False
-        got = seg.seal(sealed_deleted=_pack(sdel), new_keys=new_keys)
+        got = seg.seal(sealed_deleted=pack(sdel), new_keys=new_keys)
         made.append(got[0])
         r = maintain(N, w.off, w.doc, w.tf, docs.restated(orc, form, True), sealed_deleted=sdel, sealed_payload=w.payload,
                      sealed_keys=w.keys, new_keys=new_keys)
@@ -89,23 +81,23 @@ def _script(m, orc, rng, w, c, form, what):
         n_sealed = int((~sdel).sum())
         above = int(np.count_nonzero(r.post_tf[lo:hi] > TIE_TF))   # a growing tf of 2^24 - 1 now and then
         assert len(group) > CHAMP_L and 0 < np.count_nonzero(group < n_sealed) < CHAMP_L - above
-        rs = _check_result(m, orc, got[0], got[1:], r, f"{what}, seal", k1, b)
+        rs = check_result(m, orc, got[0], got[1:], r, f"{what}, seal", k1, b)
         if b == 0:   # the score is a function of tf alone: the list ends with the group's first new ids, growing ones last
             champ = rs.champ.reshape(-1, 2)[int(rs.champ_off[tie]):int(rs.champ_off[tie + 1]), 0]
             assert np.array_equal(champ[above:], group[:CHAMP_L - above]) and champ[-1] >= n_sealed
         a, s = got[0].info(), w.ix.info()
         assert (a.k1, a.b) == (s.k1, s.b) == (k1, b), f"{what}: the result's k1 / b"
-        _check_searches(orc, got[0], r, rng, f"{what}, seal", k1, b, ks=KS)
+        check_searches(orc, got[0], r, rng, f"{what}, seal", k1, b, ks=KS)
         # a segment on the result
         w2 = World.from_restated(m, r, got[0], k1, b)
         docs2 = Docs()
-        _new_docs(rng, w2, np.flatnonzero(w2.df == 0).tolist(), docs2, 80, N_NEW)
+        new_docs(rng, w2, np.flatnonzero(w2.df == 0).tolist(), docs2, 80, N_NEW)
         seg2 = w2.ix.growing_segment()
         try:
             seg2.insert(**docs2.kw(orc, form, True))
             g = w2.ix.growing(**docs2.kw(orc, form, True))
             try:
-                q_off, q_terms = _live_queries(rng, w2.df, [1, 2, 2, 3, 4, 5, 8, 12])
+                q_off, q_terms = live_queries(rng, w2.df, [1, 2, 2, 3, 4, 5, 8, 12])
                 for k in KS:
                     x = seg2.search_batch(q_off, q_terms, k, want_payload=True)
                     y = w2.ix.search_batch_growing(g, q_off, q_terms, k, want_payload=True)
@@ -173,7 +165,7 @@ def test_script_over_handle_kinds(m, orc, kind):
         try:
             seg.insert([0, 1], [T + 1], [1], doc_len=[1])
             with pytest.raises(m.Bm25xError) as e:
-                seg.seal(new_keys=_keys(rng, 2, c.keys))
+                seg.seal(new_keys=random_keys(rng, 2, c.keys))
             assert e.value.code == 1 and "without term keys" in str(e.value)
         finally:
             seg.close()
@@ -192,7 +184,7 @@ def test_evaluate_on_a_seals_result(m, orc):
     c = _corpus(orc, rng, False)
     w = _world(m, c, 1.2, 0.75)
     docs = Docs()
-    _new_docs(rng, w, c.dead, docs, 120, N_NEW)
+    new_docs(rng, w, c.dead, docs, 120, N_NEW)
     gone = int(np.flatnonzero((w.df > 0) & (w.df < 40))[0])                 # every document that holds it is deleted
     sdel = np.zeros(N, bool)
     sdel[w.doc[int(w.off[gone]):int(w.off[gone + 1])]] = True
@@ -205,7 +197,7 @@ def test_evaluate_on_a_seals_result(m, orc):
         seg.delete(np.array(victims, np.uint32))
         for v in victims:
             docs.deleted[v] = 1
-        got = seg.seal(sealed_deleted=_pack(sdel))
+        got = seg.seal(sealed_deleted=pack(sdel))
         r = maintain(N, w.off, w.doc, w.tf, docs.restated(orc, "doc_len", True), sealed_deleted=sdel,
                      sealed_payload=w.payload)
         df = np.diff(r.post_off.astype(np.int64))

@@ -12,21 +12,12 @@ from types import SimpleNamespace
 import numpy as np
 import pytest
 
-import _pkg
-from test_gpu_index_arrays import _growing_csr
-from test_gpu_seal import MODES, Docs, World, _check_result, _check_searches, _keys, _pack
-from util_index import assert_matches, read_back, restate
+from util_lib import gpu_library  # noqa: F401  (gpu_library: the module fixture m)
 from util_maintain import maintain
+from util_segment import (MODES, World, check_result, check_searches, check_segment, docs_from_postings, first_docs,
+                          pack, random_keys)
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def m():
-    mod = _pkg.load()
-    mod.load_library()
-    assert mod.device_count() >= 1, "no CUDA device: the engine has no CPU fallback"
-    return mod
 
 
 S = (0, 1, 31, 32, 33, 64, 65)                                   # every (source, next source) pair of these lengths
@@ -236,56 +227,6 @@ def _csr(lists, rng):
     return off, doc, rng.integers(1, 6, size=len(doc)).astype(np.uint32)
 
 
-def docs_from_postings(rng, n, term, ordinal, tf, extra_max=3):
-    """test_gpu_seal.Docs (arrays in place of its lists) of n growing documents holding the given postings; a length is
-    Σ tf plus up to extra_max."""
-    order = np.lexsort((term, ordinal))
-    docs = Docs()
-    docs.term, docs.tf = np.asarray(term, np.uint32)[order], np.asarray(tf, np.uint32)[order]
-    docs.off = np.concatenate([[0], np.cumsum(np.bincount(ordinal, minlength=n))]).tolist()
-    docs.extra = rng.integers(0, extra_max + 1, size=n)
-    docs.deleted = np.zeros(n, np.uint8)
-    docs.payload = rng.integers(0, 65536, size=(n, 3)).astype(np.uint16)
-    return docs
-
-
-def first_docs(docs, n):
-    """The first n documents of docs_from_postings' Docs, sharing their deleted flags."""
-    sub = Docs()
-    sub.off, sub.term, sub.tf = docs.off[:n + 1], docs.term[:docs.off[n]], docs.tf[:docs.off[n]]
-    sub.extra, sub.deleted, sub.payload = docs.extra[:n], docs.deleted[:n], docs.payload[:n]
-    return sub
-
-
-def check_segment(orc, seg, w, docs, form, with_payload, what, k1=1.2, b=0.75):
-    """Every array of the segment's handle: byte-equal to bm25x_growing_create's over the same documents and flags, and to
-    the CPU restatement of them with the sealed statistics of World w."""
-    kw = docs.kw(orc, form, with_payload)
-    ref = w.ix.growing(**kw)
-    try:
-        lay, der = seg.arrays()
-        got = read_back(lay, der)
-        g = SimpleNamespace(elem_off=kw["elem_off"], elem_term=kw["elem_term"], elem_tf=kw["elem_tf"], deleted=kw["deleted"])
-        off, doc, tf = _growing_csr(g, w.n_terms, w.df)
-        stat = (w.n_docs, w.df, float(w.sum_len) / w.n_docs)
-        if form == "doc_len":
-            r = restate(orc, docs.n, off, doc, tf, k1, b, stat=stat, doc_len=kw["doc_len"], payload=kw.get("payload"))
-            skip = ()
-        else:   # stored norms carry no length total
-            r = restate(orc, docs.n, off, doc, tf, k1, b, stat=stat, fieldnorm=kw["doc_fieldnorm"], sum_len=0,
-                        payload=kw.get("payload"))
-            skip = ("sum_doc_len",)
-        assert_matches(got, lay, der, r, what, skip)
-        want = read_back(ref.layout(), ref.derived())
-        for key in want:     # an array the restatement leaves empty is one unspecified placeholder slot
-            if getattr(r, key).size:
-                assert got[key].tobytes() == want[key].tobytes(), f"{what}: {key} differs from bm25x_growing_create's"
-        assert seg.info().n_postings == ref.info().n_postings == r.n_postings, what
-        return r
-    finally:
-        ref.close()
-
-
 @pytest.mark.parametrize("form", ["doc_len", "fieldnorm"])
 @pytest.mark.parametrize("size", list(SIZES))
 def test_step_edges(m, orc, size, form):
@@ -293,9 +234,9 @@ def test_step_edges(m, orc, size, form):
     rng, with_payload = c.rng, form == "fieldnorm"
     off, doc, tf = _csr([t.sealed for t in c.terms[:c.T]], rng)
     doc_len = (np.bincount(doc, weights=tf, minlength=c.NS) + rng.integers(0, 4, size=c.NS)).astype(np.uint32)
-    keys = np.array(sorted(_keys(rng, c.T).tolist()), np.uint8) if c.keyed else None
+    keys = np.array(sorted(random_keys(rng, c.T).tolist()), np.uint8) if c.keyed else None
     n_new = len(c.terms) - c.T
-    new_keys = _keys(rng, n_new, keys) if c.keyed else None
+    new_keys = random_keys(rng, n_new, keys) if c.keyed else None
     w = World(m, c.NS, off, doc, tf, doc_len, rng.integers(0, 65536, size=(c.NS, 3)).astype(np.uint16), keys)
     g = [np.r_[t.old, t.pend] for t in c.terms]
     goff, gord, gtf = _csr(g, rng)
@@ -312,13 +253,13 @@ def test_step_edges(m, orc, size, form):
         docs.deleted[c.gdel] = 1
         seg.refresh()
         check_segment(orc, seg, w, docs, form, with_payload, f"{what}, second refresh")
-        got = seg.seal(sealed_deleted=_pack(c.sdel), new_keys=new_keys)
+        got = seg.seal(sealed_deleted=pack(c.sdel), new_keys=new_keys)
         made.append(got[0])
         r = maintain(w.n_docs, w.off, w.doc, w.tf, docs.restated(orc, form, with_payload), sealed_deleted=c.sdel,
                      sealed_payload=w.payload, sealed_keys=w.keys, new_keys=new_keys)
-        _check_result(m, orc, got[0], got[1:], r, f"{what}, seal")
+        check_result(m, orc, got[0], got[1:], r, f"{what}, seal")
         # a cross-check, not the bar: searches over the constructed terms
-        _check_searches(orc, got[0], r, rng, f"{what}, seal", ks=(1, 10, 129),
+        check_searches(orc, got[0], r, rng, f"{what}, seal", ks=(1, 10, 129),
                         modes={k: MODES[k] for k in ("prune", "seed-forced")})
     finally:
         seg.close()

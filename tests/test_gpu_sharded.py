@@ -6,20 +6,12 @@ import threading
 import numpy as np
 import pytest
 
-import _pkg
-from test_gpu_parity import CONFIGS, TWO_PASS, _live_queries
-from util_parity import ROWS, same_rows
+from util_corpora import ADVERSARIAL_BOUNDS, PARITY_CONFIGS, SHARDED_PATHS, TWO_PASS, adversarial_corpus, corpus_dict
+from util_lib import gpu_library  # noqa: F401  (gpu_library: the module fixture m)
+from util_parity import ROWS, live_queries, query_csr, same_rows
 
 pytestmark = pytest.mark.gpu
 
-
-
-@pytest.fixture(scope="module")
-def m():
-    mod = _pkg.load()
-    mod.load_library()
-    assert mod.device_count() >= 1, "no CUDA device: the engine has no CPU fallback"
-    return mod
 
 
 def _both(ix, sx, q_off, q_terms, k, allow=None, what=""):
@@ -27,16 +19,6 @@ def _both(ix, sx, q_off, q_terms, k, allow=None, what=""):
     got = sx.search_batch(q_off, q_terms, k, allow=allow, want_payload=True)
     same_rows(got, want, what)
     return got, want
-
-
-def _csr(n_docs, lists, doc_len=None):
-    off = np.zeros(len(lists) + 1, np.uint64)
-    off[1:] = np.cumsum([len(d) for d, _ in lists])
-    post_doc = np.concatenate([np.asarray(d, np.uint32) for d, _ in lists])
-    post_tf = np.concatenate([np.asarray(t, np.uint32) for _, t in lists])
-    if doc_len is None:
-        doc_len = np.bincount(post_doc, weights=post_tf, minlength=n_docs).astype(np.uint32) + 1
-    return dict(n_docs=n_docs, doc_len=doc_len, n_terms=len(lists), post_off=off, post_doc=post_doc, post_tf=post_tf)
 
 
 def _default_bounds(post_doc, n_docs, n_shards):
@@ -53,7 +35,7 @@ def _default_bounds(post_doc, n_docs, n_shards):
     return np.array(b + [n_docs], np.uint32)
 
 
-@pytest.mark.parametrize("cfg", CONFIGS, ids=[c["name"] for c in CONFIGS])
+@pytest.mark.parametrize("cfg", PARITY_CONFIGS, ids=[c["name"] for c in PARITY_CONFIGS])
 def test_parity_shapes_every_shard_count(m, cfg):
     c = m.synth_corpus(cfg["seed"], cfg["n"], cfg["vocab"], cfg["lmin"], cfg["lmax"], cfg["zipf"])
     q_off, q_terms = m.synth_queries(cfg["seed"] + 1000, cfg["nq"], cfg["vocab"], cfg["tmin"], cfg["tmax"],
@@ -85,27 +67,10 @@ def test_default_bounds_skewed_corpus(m):
         sx.close()
 
 
-ADVERSARIAL_BOUNDS = [0, 997, 2001, 2002, 2003, 2301, 2600, 3333, 4000]
-
-
-def _adversarial_corpus():
-    """The corpus of test_adversarial_bounds, and its random generator for what the test draws next."""
-    rng = np.random.default_rng(3)
-    N = 4000
-    lists = []
-    for t in range(60):                                   # ordinary terms over [0, 2000) and [2600, 4000)
-        docs = np.sort(rng.choice(np.r_[0:2000, 2600:4000], size=int(rng.integers(5, 600)), replace=False))
-        lists.append((docs, rng.integers(1, 6, size=len(docs))))
-    lists.append((np.arange(2100, 2300), rng.integers(1, 4, size=200)))     # term 60: all postings in [2003, 2301)
-    lists.append((np.array([2001]), np.array([3])))                          # term 61: one document, shard [2001, 2002)
-    # [2301, 2600) holds no posting at all; [2002, 2003) has no query term
-    return _csr(N, lists, doc_len=rng.integers(1, 200, size=N).astype(np.uint32)), rng
-
-
 def test_adversarial_bounds(m):
     """A one-document shard, bounds off multiples of 8, a shard where every query term has local df 0, a shard holding
     all postings of a term, a shard with no postings at all — with and without a prefilter bitmap."""
-    c, rng = _adversarial_corpus()
+    c, rng = adversarial_corpus()
     N = c["n_docs"]
     bounds = ADVERSARIAL_BOUNDS
     ix = m.Index(**c)
@@ -113,8 +78,7 @@ def test_adversarial_bounds(m):
     assert np.array_equal(sx.doc_bounds(), bounds)
     qs = [[60], [61], [60, 61], [60, 3, 7], [61, 5], [1, 2, 3, 4], [9], [60, 61, 0, 1, 2, 3, 4, 5, 6]]
     qs += [list(rng.choice(62, size=int(rng.integers(1, 9)), replace=False)) for _ in range(40)]
-    q_off = np.cumsum([0] + [len(q) for q in qs]).astype(np.uint32)
-    q_terms = np.array([t for q in qs for t in q], np.uint32)
+    q_off, q_terms = query_csr(qs)
     allow = np.packbits(rng.random(N) < 0.4, bitorder="little")
     for k in (1, 7, 100, 300, 1025):
         for al in (None, allow):
@@ -134,10 +98,6 @@ def test_limits_across_the_pool_classes(m):
     ix.close()
 
 
-PATHS = dict(default={}, seed_off={"seed": 0}, seeded_forced={"seed_dense_div": 0, "seed_prune_min": 0xFFFFFFFF},
-             twophase={"seed": 0, "twophase": 1}, prune_off={"prune": 0})
-
-
 @pytest.mark.parametrize("zipf", [0.0, 1.0], ids=["uniform", "zipf"])
 def test_every_kernel_path_with_and_without_prefilter(m, zipf):
     c = m.synth_corpus(81, 80000, 400 if zipf == 0.0 else 4000, 6, 40, zipf)
@@ -145,7 +105,7 @@ def test_every_kernel_path_with_and_without_prefilter(m, zipf):
     allow = np.packbits(np.random.default_rng(9).random(c.n_docs) < 0.5, bitorder="little")
     ix = m.Index.from_corpus(c)
     sx = m.ShardedIndex.from_corpus(c, n_shards=4)
-    for name, opts in PATHS.items():
+    for name, opts in SHARDED_PATHS.items():
         for idx in (ix, sx):
             for o in ("seed", "twophase", "prune"):
                 idx.set_option(o, {"seed": 1, "twophase": 0, "prune": 1}[o])
@@ -170,7 +130,7 @@ def test_33_to_64_terms_split_differs_per_shard(m):
     df = ix.df()
     rng = np.random.default_rng(11)
     counts = list(range(33, 65)) * 2
-    q_off, q_terms = _live_queries(rng, df, counts)
+    q_off, q_terms = live_queries(rng, df, counts)
     bounds = np.array([0, 6001, 13007, c.n_docs], np.uint32)
     sx = m.ShardedIndex.from_corpus(c, n_shards=3, doc_bounds=bounds)
     # the rarest-32 group of a query by each shard's local df differs from the whole index's on some queries
@@ -198,13 +158,12 @@ def test_exact_ties_across_shard_boundaries_b0(m):
     N = 3000
     lists = [(np.sort(rng.choice(N, size=int(rng.integers(50, 900)), replace=False)), None) for _ in range(30)]
     lists = [(d, np.ones(len(d), np.uint32)) for d, _ in lists]
-    c = _csr(N, lists)
+    c = corpus_dict(N, lists)
     ix = m.Index(**c, b=0.0)
     bounds = [0, 333, 1001, 1002, 2222, N]
     sx = m.ShardedIndex(**c, b=0.0, n_shards=5, doc_bounds=bounds)
     qs = [list(rng.choice(30, size=int(rng.integers(1, 4)), replace=False)) for _ in range(50)]
-    q_off = np.cumsum([0] + [len(q) for q in qs]).astype(np.uint32)
-    q_terms = np.array([t for q in qs for t in q], np.uint32)
+    q_off, q_terms = query_csr(qs)
     crossing = 0
     for k in (5, 100, 1000):
         got, _ = _both(ix, sx, q_off, q_terms, k, what=f"b=0 ties k={k}")
@@ -244,10 +203,10 @@ def test_refusals_match_the_unsharded_index(m):
         qs = [list(qt[qo[i]:qo[i + 1]]) for i in range(nq)]
         for i in big_at:
             qs[i] = list(big)
-        qo = np.cumsum([0] + [len(q) for q in qs]).astype(np.uint32)
+        qo, qt = query_csr(qs)
         for i in backwards_at:
             qo[i + 1] = qo[i] - 1
-        return qo, np.array([t for q in qs for t in q], np.uint32)
+        return qo, qt
 
     # a sliced batch (4 slices of 16) whose only bad query, 40, is query 8 of the third slice
     for idx in (ix, sx):

@@ -2,28 +2,17 @@
 index built from the decoded CSR (byte-identical arrays, shard by shard), against the CPU restatement of every shard
 (tests/util_index.py), and against the unsharded stored-block ingest (bit-identical search rows on every kernel path, the
 same refusals for every corruption, wherever it sits relative to the shard bounds)."""
-import ctypes
 
 import numpy as np
 import pytest
 
-import _pkg
-from test_gpu_blocks import CONFIGS
-from test_gpu_index_arrays import _check_shards, _local_csr
-from test_gpu_sharded import ADVERSARIAL_BOUNDS, PATHS, _adversarial_corpus
-from util_cuda import cudart
-from util_index import DERIVED, LAYOUT, SCALARS, read_back, restate, assert_matches
-from util_parity import same_rows
+from util_corpora import ADVERSARIAL_BOUNDS, BLOCK_CONFIGS, SHARDED_PATHS, adversarial_corpus
+from util_cuda import free_bytes
+from util_index import DERIVED, LAYOUT, SCALARS, assert_matches, check_shards, local_csr, read_back, restate
+from util_lib import gpu_library, refused  # noqa: F401  (gpu_library: the module fixture m)
+from util_parity import query_csr, same_rows
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def m():
-    mod = _pkg.load()
-    mod.load_library()
-    assert mod.device_count() >= 1, "no CUDA device: the engine has no CPU fallback"
-    return mod
 
 
 def _dict(c):
@@ -71,7 +60,7 @@ def _rows(ix, sx, q_off, q_terms, k, allow=None, what=""):
 
 # ---- 1. arrays: byte-identical to bm25x_sharded_create on the decoded CSR ----
 
-@pytest.mark.parametrize("cfg", CONFIGS, ids=[c["name"] for c in CONFIGS])
+@pytest.mark.parametrize("cfg", BLOCK_CONFIGS, ids=[c["name"] for c in BLOCK_CONFIGS])
 def test_arrays_identical_to_sharded_create(m, orc, cfg):
     c = _dict(m.synth_corpus(cfg["seed"], cfg["n"], cfg["vocab"], cfg["lmin"], cfg["lmax"], cfg["zipf"]))
     blocks, _ = _encode(orc, c)
@@ -113,7 +102,7 @@ def test_bounds_against_blocks(m, orc):
     assert len(bounds) >= 6, bounds
     ix = m.Index(**c)
     sx = m.ShardedIndex.from_blocks(**blocks, n_shards=len(bounds) - 1, doc_bounds=bounds)
-    _check_shards(m, orc, c, sx, ix, 1.2, 0.75, f"block bounds {bounds}")
+    check_shards(m, orc, c, sx, ix, 1.2, 0.75, f"block bounds {bounds}")
     want = m.ShardedIndex(**c, n_shards=len(bounds) - 1, doc_bounds=bounds)
     _same_shards(sx, want, "block bounds")
     q_off, q_terms = m.synth_queries(1022, 100, 5000, 1, 8, c["post_off"], 1.0)
@@ -126,16 +115,15 @@ def test_bounds_against_blocks(m, orc):
 
 def test_adversarial_bounds(m, orc):
     """A one-document shard, a shard with no postings at all, terms with no postings in some shards."""
-    c, rng = _adversarial_corpus()
+    c, rng = adversarial_corpus()
     blocks, _ = _encode(orc, c)
     ix = m.Index(**c)
     sx = m.ShardedIndex.from_blocks(**blocks, n_shards=len(ADVERSARIAL_BOUNDS) - 1, doc_bounds=ADVERSARIAL_BOUNDS)
-    _check_shards(m, orc, c, sx, ix, 1.2, 0.75, "adversarial")
+    check_shards(m, orc, c, sx, ix, 1.2, 0.75, "adversarial")
     bix = m.Index.from_blocks(**blocks)
     qs = [[60], [61], [60, 61], [60, 3, 7], [61, 5], [1, 2, 3, 4]]
     qs += [list(rng.choice(62, size=int(rng.integers(1, 9)), replace=False)) for _ in range(30)]
-    q_off = np.cumsum([0] + [len(q) for q in qs]).astype(np.uint32)
-    q_terms = np.array([t for q in qs for t in q], np.uint32)
+    q_off, q_terms = query_csr(qs)
     allow = np.packbits(rng.random(c["n_docs"]) < 0.4, bitorder="little")
     for k in (1, 100, 1025):
         for al in (None, allow):
@@ -161,7 +149,7 @@ def test_stored_norms(m, orc):
     for s in range(4):
         lo, hi = bounds[s], bounds[s + 1]
         lay, der = sx.shard_arrays(s)
-        loff, ldoc, ltf = _local_csr(off, doc, tf, lo, hi)
+        loff, ldoc, ltf = local_csr(off, doc, tf, lo, hi)
         r = restate(orc, hi - lo, loff, ldoc, ltf, 1.2, 0.75, fieldnorm=fn[lo:hi], sum_len=total, stat=stat, doc_base=lo)
         assert_matches(read_back(lay, der), lay, der, r, f"stored norms shard {s}")
     q_off, q_terms = m.synth_queries(42, 60, 300, 1, 6, off, 0.7)
@@ -234,9 +222,9 @@ def test_wide_deltas_tf_limits_and_raw_tail(m, orc):
         ix.close()
     tfs[50] = 1 << 24
     blocks, _ = _two_block_token(orc, docs, tfs, N)
-    want = _refused(m, lambda: m.Index.from_blocks(**blocks))
+    want = refused(m, lambda: m.Index.from_blocks(**blocks))
     assert want[0] == 4 and "2^24" in want[1]
-    assert _refused(m, lambda: m.ShardedIndex.from_blocks(**blocks, n_shards=4, doc_bounds=bounds)) == want
+    assert refused(m, lambda: m.ShardedIndex.from_blocks(**blocks, n_shards=4, doc_bounds=bounds)) == want
 
 
 # ---- 4. search rows on every kernel path ----
@@ -248,7 +236,7 @@ def test_search_every_path(m, orc):
     allow = np.packbits(np.random.default_rng(9).random(c["n_docs"]) < 0.5, bitorder="little")
     ix = m.Index.from_blocks(**blocks)
     sx = m.ShardedIndex.from_blocks(**blocks, n_shards=3)
-    for name, opts in PATHS.items():
+    for name, opts in SHARDED_PATHS.items():
         for idx in (ix, sx):
             for o in ("seed", "twophase", "prune"):
                 idx.set_option(o, {"seed": 1, "twophase": 0, "prune": 1}[o])
@@ -265,18 +253,6 @@ def test_search_every_path(m, orc):
 
 # ---- 5. corruption: the unsharded ingest's refusals, wherever the corrupt block sits ----
 
-def _refused(m, fn):
-    with pytest.raises(m.Bm25xError) as e:
-        fn()
-    return e.value.code, str(e.value)
-
-
-def _free_bytes():
-    free, total = ctypes.c_size_t(), ctypes.c_size_t()
-    assert cudart().cudaMemGetInfo(ctypes.byref(free), ctypes.byref(total)) == 0
-    return free.value
-
-
 def _placements(doc_ids, N):
     """Bounds that cut the block holding doc_ids (ascending), and bounds whose last shard holds it whole."""
     a, z = int(doc_ids[0]), int(doc_ids[-1])
@@ -285,12 +261,12 @@ def _placements(doc_ids, N):
 
 
 def _same_refusal(m, blocks, doc_ids, what):
-    want = _refused(m, lambda: m.Index.from_blocks(**blocks))
+    want = refused(m, lambda: m.Index.from_blocks(**blocks))
     for where, b in _placements(doc_ids, blocks["n_docs"]).items():
-        free = _free_bytes()
-        got = _refused(m, lambda: m.ShardedIndex.from_blocks(**blocks, n_shards=2, doc_bounds=b))
+        free = free_bytes()
+        got = refused(m, lambda: m.ShardedIndex.from_blocks(**blocks, n_shards=2, doc_bounds=b))
         assert got == want, (what, where, got, want)
-        assert _free_bytes() == free, (what, where, "device memory not freed")
+        assert free_bytes() == free, (what, where, "device memory not freed")
     return want
 
 

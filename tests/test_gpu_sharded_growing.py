@@ -3,7 +3,7 @@
 Every case runs beside a twin: an unsharded index over the same corpus whose own segment receives the same inserts,
 deletes and refreshes.  After every step the sharded segment's rows (all five arrays) and its `queries` / `postings`
 equal the twin's, and its growing handle equals the twin's byte for byte, at 1..16 shards with default and adversarial
-bounds, every limit and the four option sets of test_gpu_seal.MODES.  Its seal equals, shard by shard and byte for byte,
+bounds, every limit and the four option sets of util_segment.MODES.  Its seal equals, shard by shard and byte for byte,
 bm25x_sharded_create over the restatement of maintain.rs (util_maintain) with the bounds the layout rule gives, its maps
 equal the restatement's and the twin's seal's, and its rows equal those of the twin's sealed index.  Then the layout
 edges, the refusals, a seal while other threads insert, delete and search, device memory and two devices."""
@@ -13,12 +13,12 @@ import threading
 import numpy as np
 import pytest
 
-from test_gpu_parity import _live_queries
-from test_gpu_seal import (DEFAULTS, KS, MODES, NONE, Docs, World, _free_bytes, _keys, _new_docs, _pack, _sealed_world,
-                           m)  # noqa: F401  (m: the module fixture)
+from util_cuda import free_bytes
 from util_index import read_back
+from util_lib import gpu_library  # noqa: F401  (gpu_library: the module fixture m)
 from util_maintain import MISSING, maintain
-from util_parity import ROWS, same_rows
+from util_parity import ROWS, live_queries, same_rows
+from util_segment import DEFAULTS, MODES, NONE, SEAL_KS, Docs, World, new_docs, pack, random_keys, sealed_world
 
 pytestmark = pytest.mark.gpu
 
@@ -62,7 +62,7 @@ def _search_pair(seg, twin, rng, w, q_off, q_terms, k, what, allow=True):
     n_g = seg.info().n_docs
     runs = [(None, None)]
     if allow:
-        runs.append((_pack(rng.random(w.n_docs) < 0.7), _pack(rng.random(max(n_g, 1)) < 0.7)))
+        runs.append((pack(rng.random(w.n_docs) < 0.7), pack(rng.random(max(n_g, 1)) < 0.7)))
     for al, ag in runs:
         a = seg.search_batch(q_off, q_terms, k, allow=al, allow_growing=ag, allow_growing_docs=max(n_g - 3, 0),
                              want_payload=True)
@@ -75,20 +75,20 @@ def _search_pair(seg, twin, rng, w, q_off, q_terms, k, what, allow=True):
 PARITY = [(S, kind) for S in (1, 2, 3, 8, 16) for kind in ("default", "adversarial") if S > 1 or kind == "default"]
 
 
-@pytest.mark.parametrize("k", KS)
+@pytest.mark.parametrize("k", SEAL_KS)
 @pytest.mark.parametrize("S,kind", PARITY)
 def test_search_parity(m, orc, S, kind, k):
     """Seeded scripts of inserts, deletes and refreshes; after every step the rows under every option set, and the growing
     handle's arrays, equal the twin's.  S = 16 with k = 65535 merges 17 lists."""
-    seed = 1000 * S + 10 * KS.index(k) + (kind == "adversarial")
+    seed = 1000 * S + 10 * SEAL_KS.index(k) + (kind == "adversarial")
     rng = np.random.default_rng(seed)
     form = ("doc_len", "fieldnorm")[seed % 2]
     with_payload = bool(seed // 2 % 2)
     keyed = bool(seed // 4 % 2)
-    w, dead = _sealed_world(m, orc, rng, 600, 90, keyed, with_payload)
+    w, dead = sealed_world(m, orc, rng, 600, 90, keyed, with_payload)
     sx = _sharded(m, w, S, _bounds(kind, S, w.n_docs))
     seg, twin = sx.growing_segment(), w.ix.growing_segment()
-    q_off, q_terms = _live_queries(rng, w.df, [1, 2, 2, 3, 4, 5, 8, 12, 40])
+    q_off, q_terms = live_queries(rng, w.df, [1, 2, 2, 3, 4, 5, 8, 12, 40])
     what = f"S={S} {kind} k={k} {form} payload={with_payload} keyed={keyed}"
     try:
         # before the first insert: the sharded search itself, stats included
@@ -101,7 +101,7 @@ def test_search_parity(m, orc, S, kind, k):
         docs = Docs()
         for step in range(3):
             lo = docs.n
-            _new_docs(rng, w, dead, docs, int(rng.integers(20, 90)), 4, p_deleted=0.1)
+            new_docs(rng, w, dead, docs, int(rng.integers(20, 90)), 4, p_deleted=0.1)
             kw = docs.kw(orc, form, with_payload, lo, docs.n)
             seg.insert(**kw)
             twin.insert(**kw)
@@ -133,7 +133,7 @@ def _new_bounds(old_bounds, sdel, n_growing_kept):
     return np.concatenate([[0], np.cumsum([kept[s] for s in keep])]).astype(np.uint32), keep
 
 
-def _check_sealed(m, orc, got, twin_got, r, old_bounds, sdel, old_devices, rng, what, ks=KS, modes=MODES):
+def _check_sealed(m, orc, got, twin_got, r, old_bounds, sdel, old_devices, rng, what, ks=SEAL_KS, modes=MODES):
     """The sharded seal `got` (ShardedIndex, maps) against bm25x_sharded_create over the restated corpus r with the
     layout rule's bounds and devices, against the restatement's maps and the twin's, and its rows against the twin's
     sealed index."""
@@ -163,7 +163,7 @@ def _check_sealed(m, orc, got, twin_got, r, old_bounds, sdel, old_devices, rng, 
     df = np.diff(r.post_off.astype(np.int64))
     if not (df > 0).any():
         return
-    q_off, q_terms = _live_queries(rng, df, [1, 2, 2, 3, 4, 5, 8, 12, 40][: 9 if (df > 0).sum() >= 40 else 5])
+    q_off, q_terms = live_queries(rng, df, [1, 2, 2, 3, 4, 5, 8, 12, 40][: 9 if (df > 0).sum() >= 40 else 5])
     try:
         for mode, opts in modes.items():
             _set_options((sx, tix), opts)
@@ -184,7 +184,7 @@ def test_seal_matches_restatement(m, orc, kind, form, with_payload, S):
     the restatement, shard by shard, and the twin's seal."""
     rng = np.random.default_rng(SEALS[(kind, form, with_payload, S)])
     keyed = kind == "keyed"
-    w, dead = _sealed_world(m, orc, rng, 1500, 140, keyed, with_payload)
+    w, dead = sealed_world(m, orc, rng, 1500, 140, keyed, with_payload)
     sx = _sharded(m, w, S, None)
     made = [sx, w.ix]
     seg = twin = None
@@ -194,7 +194,7 @@ def test_seal_matches_restatement(m, orc, kind, form, with_payload, S):
             old_bounds = sx.doc_bounds()
             seg, twin = sx.growing_segment(), w.ix.growing_segment()
             docs = Docs()
-            _new_docs(rng, w, dead, docs, 120, 5)
+            new_docs(rng, w, dead, docs, 120, 5)
             for lo, hi in ((0, 70), (70, docs.n)):
                 kw = docs.kw(orc, form, with_payload, lo, hi)
                 seg.insert(**kw)
@@ -208,12 +208,12 @@ def test_seal_matches_restatement(m, orc, kind, form, with_payload, S):
             for v in victims:
                 docs.deleted[int(v)] = 1
             sdel = rng.random(w.n_docs) < 0.1
-            new_keys = _keys(rng, 5, w.keys) if keyed else None
-            q_off, q_terms = _live_queries(rng, w.df, [1, 2, 3, 5])
+            new_keys = random_keys(rng, 5, w.keys) if keyed else None
+            q_off, q_terms = live_queries(rng, w.df, [1, 2, 3, 5])
             before = seg.search_batch(q_off, q_terms, 40, want_payload=True)
-            got = seg.seal(sealed_deleted=_pack(sdel), new_keys=new_keys)
+            got = seg.seal(sealed_deleted=pack(sdel), new_keys=new_keys)
             made.append(got[0])
-            twin_got = twin.seal(sealed_deleted=_pack(sdel), new_keys=new_keys)
+            twin_got = twin.seal(sealed_deleted=pack(sdel), new_keys=new_keys)
             made.append(twin_got[0])
             same_rows(before, seg.search_batch(q_off, q_terms, 40, want_payload=True), f"{what}: the old segment")
             r = maintain(w.n_docs, w.off, w.doc, w.tf, docs.restated(orc, form, with_payload), sealed_deleted=sdel,
@@ -238,7 +238,7 @@ def test_layout_edges(m, orc, case):
     """Every sealed document of one shard deleted (the first, a middle one, the last with and without growing
     survivors), a seal with no insert, and a 16-shard index."""
     rng = np.random.default_rng(61 + len(case))
-    w, dead = _sealed_world(m, orc, rng, 800, 100, False, True)
+    w, dead = sealed_world(m, orc, rng, 800, 100, False, True)
     S = 16 if case == "sixteen" else 4
     bounds = np.array([0, 150, 400, 650, 800], np.uint32) if S == 4 else None
     sx = _sharded(m, w, S, bounds)
@@ -248,7 +248,7 @@ def test_layout_edges(m, orc, case):
     try:
         docs = Docs()
         if case != "compaction":
-            _new_docs(rng, w, dead, docs, 60, 3)
+            new_docs(rng, w, dead, docs, 60, 3)
             seg.insert(**docs.kw(orc, "doc_len", True))
             twin.insert(**docs.kw(orc, "doc_len", True))
         if case == "last-without-growing":
@@ -259,9 +259,9 @@ def test_layout_edges(m, orc, case):
         s = {"first": 0, "middle": 2, "last-with-growing": 3, "last-without-growing": 3}.get(case)
         if s is not None:
             sdel[old_bounds[s]:old_bounds[s + 1]] = True
-        got = seg.seal(sealed_deleted=_pack(sdel))
+        got = seg.seal(sealed_deleted=pack(sdel))
         made.append(got[0])
-        twin_got = twin.seal(sealed_deleted=_pack(sdel))
+        twin_got = twin.seal(sealed_deleted=pack(sdel))
         made.append(twin_got[0])
         r = maintain(w.n_docs, w.off, w.doc, w.tf, docs.restated(orc, "doc_len", True), sealed_deleted=sdel,
                      sealed_payload=w.payload)
@@ -283,19 +283,19 @@ def test_refusals(m, orc):
     """bm25x_growing_seal's refusals with their codes and messages, named by bm25x_growing_seal_sharded; the cross-kind
     refusals; nothing changes on a refusal."""
     rng = np.random.default_rng(67)
-    w, dead = _sealed_world(m, orc, rng, 900, 100, True, True)
+    w, dead = sealed_world(m, orc, rng, 900, 100, True, True)
     sx = _sharded(m, w, 3, None)
     seg, plain = sx.growing_segment(), w.ix.growing_segment()
     L = m.load_library()
-    q_off, q_terms = _live_queries(rng, w.df, [1, 2, 3])
+    q_off, q_terms = live_queries(rng, w.df, [1, 2, 3])
     try:
         docs = Docs()
-        _new_docs(rng, w, dead, docs, 80, 4, p_deleted=0)
+        new_docs(rng, w, dead, docs, 80, 4, p_deleted=0)
         docs.add([w.n_terms + 2], [1], 0, False, [1, 2, 3])     # ordinal T + 2 for sure
         seg.insert(**docs.kw(orc, "doc_len", True))
         plain.insert(**docs.kw(orc, "doc_len", True))
         rows, info = seg.search_batch(q_off, q_terms, 20, want_payload=True), _snapshot(seg)
-        nk = _keys(rng, 4, w.keys)
+        nk = random_keys(rng, 4, w.keys)
 
         def refused(fn, code, text):
             with pytest.raises(m.Bm25xError) as e:
@@ -312,7 +312,7 @@ def test_refusals(m, orc):
         refused(lambda: seg.seal(new_keys=nk[:2]), 1, who + f"inserted term ordinal {first} >=")
         seg.delete(np.arange(docs.n))
         rows, info = seg.search_batch(q_off, q_terms, 20, want_payload=True), _snapshot(seg)
-        refused(lambda: seg.seal(new_keys=nk, sealed_deleted=_pack(np.ones(w.n_docs, bool))), 1,
+        refused(lambda: seg.seal(new_keys=nk, sealed_deleted=pack(np.ones(w.n_docs, bool))), 1,
                 who + "no document survives")
         # maps too short: refused with the sizes a retry needs
         for g_cap, t_cap in ((docs.n - 1, 1 << 20), (docs.n, w.n_terms)):
@@ -359,14 +359,14 @@ def test_seal_during_inserts_deletes_and_searches(m, orc):
     the seal equals the restatement of the state it reports (n_growing ordinals, the deleted set read off growing_map),
     and every search succeeds with the rows of one state of the script."""
     rng = np.random.default_rng(71)
-    w, dead = _sealed_world(m, orc, rng, 1500, 120, False, False)
+    w, dead = sealed_world(m, orc, rng, 1500, 120, False, False)
     sx = _sharded(m, w, 3, None)
-    q_off, q_terms = _live_queries(rng, w.df, [1, 2, 3, 4, 6, 9])
+    q_off, q_terms = live_queries(rng, w.df, [1, 2, 3, 4, 6, 9])
     docs = Docs()
     ops = []
     for i in range(8):
         lo = docs.n
-        _new_docs(rng, w, dead, docs, int(rng.integers(20, 100)), 3)
+        new_docs(rng, w, dead, docs, int(rng.integers(20, 100)), 3)
         ops.append(("insert", lo, docs.n))
         if i % 2:
             ops.append(("delete", rng.choice(docs.n, size=12, replace=False)))
@@ -445,12 +445,12 @@ def test_seal_during_inserts_deletes_and_searches(m, orc):
 
 def test_seals_free_their_memory(m, orc):
     rng = np.random.default_rng(73)
-    w, dead = _sealed_world(m, orc, rng, 1200, 110, True, False)
+    w, dead = sealed_world(m, orc, rng, 1200, 110, True, False)
     sx = _sharded(m, w, 3, None)
     docs = Docs()
-    _new_docs(rng, w, dead, docs, 150, 3)
-    nk = _keys(rng, 3, w.keys)
-    q_off, q_terms = _live_queries(rng, w.df, [1, 2, 3])
+    new_docs(rng, w, dead, docs, 150, 3)
+    nk = random_keys(rng, 3, w.keys)
+    q_off, q_terms = live_queries(rng, w.df, [1, 2, 3])
 
     def run(n_seal):
         seg = sx.growing_segment()
@@ -458,15 +458,15 @@ def test_seals_free_their_memory(m, orc):
         for i in range(n_seal):
             seg.delete([i])
             seg.search_batch(q_off, q_terms, 10)
-            nsx, *_ = seg.seal(sealed_deleted=_pack(rng.random(w.n_docs) < 0.1), new_keys=nk)
+            nsx, *_ = seg.seal(sealed_deleted=pack(rng.random(w.n_docs) < 0.1), new_keys=nk)
             nsx.close()
         seg.close()
 
     try:
         run(2)  # loads every kernel of a seal before the measurement
-        free = _free_bytes()
+        free = free_bytes()
         run(15)
-        assert _free_bytes() == free, "device memory of the sharded seal not freed"
+        assert free_bytes() == free, "device memory of the sharded seal not freed"
     finally:
         sx.close()
         w.ix.close()
@@ -477,25 +477,25 @@ def test_two_devices(m, orc):
     if m.device_count() < 2:
         pytest.skip("needs two CUDA devices")
     rng = np.random.default_rng(79)
-    w, dead = _sealed_world(m, orc, rng, 900, 100, False, True)
+    w, dead = sealed_world(m, orc, rng, 900, 100, False, True)
     sx = _sharded(m, w, 3, None, devices=[0, 1, 1])
     old_bounds = sx.doc_bounds()
     seg, twin = sx.growing_segment(), w.ix.growing_segment()
     made = [sx, w.ix]
     try:
         docs = Docs()
-        _new_docs(rng, w, dead, docs, 80, 3)
+        new_docs(rng, w, dead, docs, 80, 3)
         seg.insert(**docs.kw(orc, "doc_len", True))
         twin.insert(**docs.kw(orc, "doc_len", True))
         assert seg.info().device == 1
-        q_off, q_terms = _live_queries(rng, w.df, [1, 2, 3, 5, 8])
+        q_off, q_terms = live_queries(rng, w.df, [1, 2, 3, 5, 8])
         for k in (1, 10, 1025):
             _search_pair(seg, twin, rng, w, q_off, q_terms, k, f"two devices k={k}")
         _same_arrays(seg.arrays(), twin.arrays(), "two devices: growing handle")
         sdel = rng.random(w.n_docs) < 0.1
-        got = seg.seal(sealed_deleted=_pack(sdel))
+        got = seg.seal(sealed_deleted=pack(sdel))
         made.append(got[0])
-        twin_got = twin.seal(sealed_deleted=_pack(sdel))
+        twin_got = twin.seal(sealed_deleted=pack(sdel))
         made.append(twin_got[0])
         r = maintain(w.n_docs, w.off, w.doc, w.tf, docs.restated(orc, "doc_len", True), sealed_deleted=sdel,
                      sealed_payload=w.payload)

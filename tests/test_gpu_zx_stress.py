@@ -5,18 +5,10 @@ that a query pruned or that its rings were split again: test_gpu_prune_points.py
 import numpy as np
 import pytest
 
-import _pkg
-from test_gpu_parity import _compare, _oracle_index
+from util_lib import gpu_library  # noqa: F401  (gpu_library: the module fixture m)
+from util_parity import compare, oracle_index
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def m():
-    mod = _pkg.load()
-    mod.load_library()
-    assert mod.device_count() >= 1, "no CUDA device: the engine has no CPU fallback"
-    return mod
 
 
 def _cases():
@@ -42,7 +34,7 @@ def test_random_shapes_match_oracle(m, orc, cfg):
     q_off, q_terms = m.synth_queries(cfg["seed"] + 7, 24, cfg["vocab"], 1, tmax, c.post_off, cfg["zipf"])
     ix = m.Index.from_corpus(c)
     ix.set_option("prune", cfg["prune"])
-    oix = _oracle_index(orc, c)
+    oix = oracle_index(orc, c)
     res = ix.search_batch(q_off, q_terms, cfg["k"])
-    _compare(res, oix, q_off, q_terms, cfg["k"], what=str(cfg))
+    compare(res, oix, q_off, q_terms, cfg["k"], what=str(cfg))
     ix.close()

@@ -4,21 +4,10 @@ against the exhaustive oracle.  The corpora are the bench workloads (bench.py WO
 import numpy as np
 import pytest
 
-import _pkg
+from util_lib import gpu_library  # noqa: F401  (gpu_library: the module fixture m)
+from util_parity import oracle_index
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def m():
-    mod = _pkg.load()
-    mod.load_library()
-    assert mod.device_count() >= 1, "no CUDA device: the engine has no CPU fallback"
-    return mod
-
-
-def _oracle_index(orc, c):
-    return orc.OracleIndex(orc.Corpus(c.n_docs, c.doc_len, c.n_terms, c.post_off, c.post_doc, c.post_tf))
 
 
 def _properties(res, k, n_docs, what):
@@ -52,7 +41,7 @@ def test_config3_full_100k_queries_top100_and_top10(m, orc):
     c = m.synth_corpus(0xB25C0DE3, 10_000_000, 100_000, 128)
     q_off, q_terms = m.synth_queries(0xB25C0DE3 + 1000, 100_000, 100_000, 3, 3, c.post_off)
     ix = m.Index.from_corpus(c)
-    oix = _oracle_index(orc, c)
+    oix = oracle_index(orc, c)
     for k in (100, 10):
         res = ix.search_batch(q_off, q_terms, k)
         assert np.all(res["n"] == k)
@@ -78,7 +67,7 @@ def test_config4_zipf_8term_pruning_on_off(m, orc):
     for key in ("doc", "score", "score64", "n"):
         assert np.array_equal(on[key][:sub], off[key]), f"C4: pruning changed `{key}`"
     assert on["stats"].postings_fetched < on["stats"].postings
-    oix = _oracle_index(orc, c)
+    oix = oracle_index(orc, c)
     _sample_vs_oracle(on, oix, q_off, q_terms, 10, list(range(0, sub, 167)) + list(range(sub, 100_000, 9973)), "C4")
     ix.close()
 
@@ -96,6 +85,6 @@ def test_config5_25M_docs_mixed_queries(m, orc):
     res = ix.search_batch(q_off, q_terms, 10)
     assert np.all(res["n"] == 10)
     _properties(res, 10, c.n_docs, "C5")
-    oix = _oracle_index(orc, c)
+    oix = oracle_index(orc, c)
     _sample_vs_oracle(res, oix, q_off, q_terms, 10, range(0, 1_000_000, 15_873), "C5")              # 64 queries
     ix.close()

@@ -12,53 +12,27 @@ Each index holds ~7 bytes per document on the device (fieldnorm, payload): ~30 G
 one takes ~34 GB of host memory (the norms and the synthesised payload) and ~47 GB through the CSR path (plus 4-byte
 lengths), as measured on an H100 host; the sharded index builds one shard at a time.  Each build is skipped, saying so,
 when the free device or available host memory is short of that."""
-import ctypes
 import time
 from types import SimpleNamespace
 
 import numpy as np
 import pytest
 
-import _pkg
-from util_cuda import cudart, download
+from util_cuda import download
 from util_index import LAYOUT, ctid
-from util_parity import same_rows
-from util_sparse import (DOC_INF, FN_EMPTY, FN_TIE, MAX_N_DOCS, T31, SparseReference, assert_rows, full_fieldnorm,
-                         high_id_corpus, reference, sum_len_of)
+from util_lib import gpu_library  # noqa: F401  (gpu_library: the module fixture m)
+from util_parity import query_csr, same_rows
+from util_sparse import (B, DOC_INF, FN_EMPTY, FN_TIE, K1, MAX_N_DOCS, N_A, T31, Prefix, SparseReference, assert_rows,
+                         full_fieldnorm, high_id_corpus, high_id_queries, need, peak_host_gb, reference, sum_len_of)
 
 pytestmark = pytest.mark.gpu
 
-N_A = MAX_N_DOCS - 64       # index A: room for a growing segment of 64 documents, ids up to 0xFFFFFFFD
 N_B = MAX_N_DOCS            # sharded index B: the largest n_docs
-K1, B = 1.2, 0.75
 KS = (1, 10, 128, 129, 224, 1025)
-# kernel paths of the 2..8-term classes (test_gpu_paths.PATHS and the hand-back / dense options of
+# kernel paths of the 2..8-term classes (util_parity.KERNEL_PATHS and the hand-back / dense options of
 # test_gpu_parity.test_kernel_paths_identical): (seed, twophase, seed_prune_min, seed_dense_div)
 PATHS = dict(seeded=(1, 0, 0xFFFFFFFF, 0), handback=(1, 0, 64, 0), dense=(1, 0, 0xFFFFFFFF, 8), twophase=(0, 1, 0, 0),
              plain=(0, 0, 0, 0))
-
-
-@pytest.fixture(scope="module")
-def m():
-    mod = _pkg.load()
-    mod.load_library()
-    assert mod.device_count() >= 1, "no CUDA device: the engine has no CPU fallback"
-    return mod
-
-
-def _need(host_gb, dev_gb, what):
-    import psutil
-    free, total = ctypes.c_size_t(0), ctypes.c_size_t(0)
-    assert cudart().cudaMemGetInfo(ctypes.byref(free), ctypes.byref(total)) == 0
-    host = psutil.virtual_memory().available
-    if host < host_gb * 1e9 or free.value < dev_gb * 1e9:
-        pytest.skip(f"{what} needs {host_gb} GB of host and {dev_gb} GB of free device memory "
-                    f"({host / 1e9:.0f} GB / {free.value / 1e9:.0f} GB available)")
-
-
-def _peak_host_gb():
-    import resource
-    return resource.getrusage(resource.RUSAGE_SELF).ru_maxrss / 1e6
 
 
 _alive = {}  # the one large index alive at a time
@@ -71,7 +45,7 @@ def _build(name, make):
     t0 = time.perf_counter()
     ix = make()
     print(f"\n[high-id] {name}: built in {time.perf_counter() - t0:.1f} s, "
-          f"{ix.info().device_bytes / 1e9:.1f} GB on the device, host peak so far {_peak_host_gb():.1f} GB")
+          f"{ix.info().device_bytes / 1e9:.1f} GB on the device, host peak so far {peak_host_gb():.1f} GB")
     _alive[name] = ix
     return ix
 
@@ -83,7 +57,7 @@ def _close_last():
     for h in _alive.values():
         h.close()
     _alive.clear()
-    print(f"\n[high-id] module wall time {time.perf_counter() - t0:.0f} s, host peak {_peak_host_gb():.1f} GB")
+    print(f"\n[high-id] module wall time {time.perf_counter() - t0:.0f} s, host peak {peak_host_gb():.1f} GB")
 
 
 @pytest.fixture(scope="module")
@@ -104,7 +78,7 @@ def index_a(m, orc, corpus_a, encoded_a):
     """Index A from the stored blocks (norms + sum of lengths, as the pages hold them)."""
     c, _ = corpus_a
     eb = encoded_a
-    _need(45, 34, "index A (2^32 - 66 documents)")
+    need(45, 34, "index A (2^32 - 66 documents)")
 
     def make():
         fn = full_fieldnorm(c)
@@ -112,38 +86,6 @@ def index_a(m, orc, corpus_a, encoded_a):
                                    eb.doc_off, eb.tf_off, eb.bytes[:eb.n_bytes], doc_fieldnorm=fn,
                                    sum_doc_len=sum_len_of(orc, c), k1=K1, b=B)
     return _build("index A from blocks", make)
-
-
-def _queries(c, seed):
-    """Queries of 1, 2, 3, 4, 5-8, 9-16, 17-32 and 33-64 live terms over the corpus' kinds of terms."""
-    k = c.kinds
-    rng = np.random.default_rng(seed)
-    rand = lambda n: rng.choice(c.n_terms, n, replace=False)
-    qs = [[t] for t in k["tie"] + k["dense"][:2] + k["pad"] + k["wide"] + k["head"][:1] + k["fill"][-2:]]
-    qs += [[k["tie"][0], k["dense"][0]], [k["head"][0], k["tie"][1]], k["dense"][:2], [k["pad"][0], k["tie"][2]]]
-    qs += [k["dense"][:3], [k["head"][0], k["head"][1], k["tie"][0]], k["tie"]]
-    qs += [k["dense"][:4], k["pad"] + k["dense"][:2] + k["wide"], k["tie"] + k["pad"]]
-    qs += [k["dense"] + k["pad"], k["head"] + k["tie"], list(rand(5)), list(rand(8))]
-    qs += [k["dense"] + k["tie"] + list(rand(3)), list(rand(16)), list(rand(17)), list(rand(32)), list(rand(33)),
-           list(rand(64))]
-    qs = [np.unique(np.asarray(q, np.uint32)) for q in qs]
-    q_off = np.cumsum([0] + [len(q) for q in qs]).astype(np.uint32)
-    return q_off, np.concatenate(qs).astype(np.uint32), qs
-
-
-class _Prefix:
-    """SparseReference.search at one limit per (query, bitmap): every smaller limit's rows are a prefix."""
-
-    def __init__(self, ref, kmax):
-        self.ref, self.kmax, self.memo = ref, kmax, {}
-
-    def search(self, terms, k, allow=None):
-        key = (np.asarray(terms, np.uint32).tobytes(), id(allow))
-        if key not in self.memo:
-            self.memo[key] = self.ref.search(terms, self.kmax, allow=allow)
-        r = self.memo[key]
-        n = min(k, r.n)
-        return SimpleNamespace(doc=r.doc[:n], score64=r.score64[:n], score=r.score[:n], payload=r.payload[:n], n=n)
 
 
 def _set_path(ix, name):
@@ -220,8 +162,8 @@ def test_index_a_kernel_paths(index_a, corpus_a):
     scores, payload, empty slots)."""
     c, ref = corpus_a
     ix = index_a
-    q_off, q_terms, qs = _queries(c, 11)
-    pref = _Prefix(ref, max(KS))
+    q_off, q_terms, qs = high_id_queries(c, 11)
+    pref = Prefix(ref, max(KS))
     for k in KS:
         got = {}
         for name in PATHS:
@@ -245,7 +187,7 @@ def test_index_a_prefilter(index_a, corpus_a):
     c, ref = corpus_a
     ix = index_a
     rng = np.random.default_rng(5)
-    q_off, q_terms, qs = _queries(c, 12)
+    q_off, q_terms, qs = high_id_queries(c, 12)
     nbytes = (c.n_docs + 7) // 8
     assert c.n_docs % 8 != 0
     for flip in (0, 1):
@@ -257,7 +199,7 @@ def test_index_a_prefilter(index_a, corpus_a):
                 allow[d >> 3] |= np.uint8(1 << (d & 7))
             else:
                 allow[d >> 3] &= np.uint8(~(1 << (d & 7)) & 0xFF)
-        pref = _Prefix(ref, 1025)
+        pref = Prefix(ref, 1025)
         for k in (10, 129, 1025):
             for prune in (1, 0):
                 ix.set_option("prune", prune)
@@ -271,9 +213,8 @@ def test_index_a_hbm_pools(index_a, corpus_a):
     c, ref = corpus_a
     head = c.kinds["head"]
     qs = [np.array(head[:3], np.uint32), np.array(head, np.uint32), np.array(head[:2] + c.kinds["tie"], np.uint32)]
-    q_off = np.cumsum([0] + [len(q) for q in qs]).astype(np.uint32)
-    q_terms = np.concatenate(qs)
-    pref = _Prefix(ref, 65535)
+    q_off, q_terms = query_csr(qs)
+    pref = Prefix(ref, 65535)
     assert pref.search(qs[0], 65535).n == 65535
     for k in (1025, 65535):
         for prune in (1, 0):
@@ -317,8 +258,8 @@ def test_index_a_growing_ids_up_to_the_last(m, orc, index_a, corpus_a):
     both_off = np.concatenate([[0], np.cumsum([len(d) for d in lists_doc])])
     both = SparseReference(orc, N_A + G, both_off, np.concatenate(lists_doc), np.concatenate(lists_tf), K1, B, ref.sum_len,
                            post_fn=np.concatenate(lists_fn), norms=ref.norms, stat=(N_A, ref.df, ref.sum_len / N_A))
-    q_off, q_terms, qs = _queries(c, 13)
-    pref = _Prefix(both, 1025)
+    q_off, q_terms, qs = high_id_queries(c, 13)
+    pref = Prefix(both, 1025)
     top = 0
     for k in (1, 10, 129, 1025):
         res = index_a.search_batch_growing(gix, q_off, q_terms, k, want_payload=True)
@@ -338,7 +279,7 @@ def test_index_a_again_from_the_csr(m, orc, index_a, corpus_a):
     bits."""
     c, ref = corpus_a
     index_a.close()
-    _need(60, 34, "index A from the CSR (4-byte lengths of 2^32 - 66 documents)")
+    need(60, 34, "index A from the CSR (4-byte lengths of 2^32 - 66 documents)")
     L = orc.lib()
     length = np.array([L.orc_fieldnorm_to_length(f) for f in range(256)], dtype=np.uint32)
 
@@ -357,7 +298,7 @@ def test_sharded_index_b(m, orc):
     ids (payload = ctid of the global id), with and without a prefilter bitmap, at limits of every pool class.  (The
     balanced default bounds take an 8-byte prefix sum per document, 34 GB here: bm25x_sharded_create's default bounds are
     tested at smaller sizes by tests/test_gpu_sharded.py.)"""
-    _need(45, 34, "sharded index B (2^32 - 2 documents)")
+    need(45, 34, "sharded index B (2^32 - 2 documents)")
     c = high_id_corpus(N_B)
     ref = reference(orc, c, K1, B)
     L = orc.lib()
@@ -371,14 +312,14 @@ def test_sharded_index_b(m, orc):
                               doc_bounds=doc_bounds)
     sx = _build("sharded index B", make)
     assert np.array_equal(sx.doc_bounds(), doc_bounds)
-    q_off, q_terms, qs = _queries(c, 14)
+    q_off, q_terms, qs = high_id_queries(c, 14)
     rng = np.random.default_rng(6)
     allow = np.zeros((N_B + 7) // 8, np.uint8)
     on = c.live[rng.random(len(c.live)) < 0.5]
     np.bitwise_or.at(allow, on >> 3, (1 << (on & 7)).astype(np.uint8))
     allow[(T31 + 2) >> 3] |= np.uint8(1 << ((T31 + 2) & 7))
     for al in (None, allow):
-        pref = _Prefix(ref, 1025)
+        pref = Prefix(ref, 1025)
         for k in (1, 10, 129, 1025):
             res = sx.search_batch(q_off, q_terms, k, allow=al, want_payload=True)
             assert_rows(res, pref, qs, k, f"sharded k={k} allow={al is not None}", allow=al)

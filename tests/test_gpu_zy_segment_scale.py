@@ -14,18 +14,15 @@ bm25x_index_create over util_maintain's corpus and util_index.restate over the W
 against bm25x_search_batch_growing on the re-created handle, and on the result against the index built from the restated
 corpus, 50 of them against the oracle; device memory after the second case equal to that after the first.
 Measured on one H100 80GB HBM3 (700 W power limit): ~25 s per case, 53 s for the file, host peak 2.0 GB."""
-import ctypes
 
 import numpy as np
 import pytest
 
-import _pkg
-from test_gpu_parity import _compare
-from test_gpu_seal import World, _check_result, _keys, _pack
-from test_gpu_segment_steps import check_segment, docs_from_postings, first_docs
-from util_cuda import cudart, sm_count
+from util_cuda import free_bytes, sm_count
+from util_lib import gpu_library  # noqa: F401  (gpu_library: the module fixture m)
 from util_maintain import MISSING, maintain
-from util_parity import same_rows
+from util_parity import compare, same_rows
+from util_segment import World, check_result, check_segment, docs_from_postings, first_docs, pack, random_keys
 
 pytestmark = pytest.mark.gpu
 
@@ -35,27 +32,13 @@ ROWS = ("doc", "score", "score64", "n")
 free_after = {}                                                  # case -> free device bytes once everything is closed
 
 
-@pytest.fixture(scope="module")
-def m():
-    mod = _pkg.load()
-    mod.load_library()
-    assert mod.device_count() >= 1, "no CUDA device: the engine has no CPU fallback"
-    return mod
-
-
-def _free_bytes():
-    free, total = ctypes.c_size_t(), ctypes.c_size_t()
-    assert cudart().cudaMemGetInfo(ctypes.byref(free), ctypes.byref(total)) == 0
-    return free.value
-
-
 def _sealed(m, rng, T, keyed):
     c = m.synth_corpus(0x5CA1E, N_SEALED, T, 16, 48, 0.8)
     off = c.post_off.astype(np.int64)
     term = np.repeat(np.arange(T), np.diff(off))
     keep = (term < T // 2) | (rng.random(len(term)) < 0.06)      # the tail: 0-3 postings per term
     new_off = np.concatenate([[0], np.cumsum(np.bincount(term[keep], minlength=T))]).astype(np.uint64)
-    keys = np.array(sorted(_keys(np.random.default_rng(T), T).tolist()), np.uint8) if keyed else None
+    keys = np.array(sorted(random_keys(np.random.default_rng(T), T).tolist()), np.uint8) if keyed else None
     w = World(m, c.n_docs, new_off, c.post_doc[keep], c.post_tf[keep], c.doc_len.copy(), None, keys)
     c.free()
     return w
@@ -81,7 +64,7 @@ def test_more_terms_than_warps(m, orc, kind):
     w = _sealed(m, rng, T, keyed)
     assert w.df.max() > 100_000 and np.count_nonzero(w.df == 0) > 1000 and np.count_nonzero(w.df <= 3) > 10_000
     docs = _growing(m, orc, rng, T)
-    new_keys = _keys(np.random.default_rng(N_NEW), N_NEW, w.keys) if keyed else None   # both cases: the same documents
+    new_keys = random_keys(np.random.default_rng(N_NEW), N_NEW, w.keys) if keyed else None   # both cases: the same documents
     q_off, q_terms = m.synth_queries(0x5CA20, 2000, T, 1, 8, w.off, 0.8)
     seg = w.ix.growing_segment()
     got = ref = None
@@ -106,11 +89,11 @@ def test_more_terms_than_warps(m, orc, kind):
             docs.deleted[victims] = 1
             lo = hi
         sdel = rng.random(w.n_docs) < 0.1
-        got = seg.seal(sealed_deleted=_pack(sdel), new_keys=new_keys)
+        got = seg.seal(sealed_deleted=pack(sdel), new_keys=new_keys)
         r = maintain(w.n_docs, w.off, w.doc, w.tf, docs.restated(orc, "doc_len", True), sealed_deleted=sdel,
                      sealed_keys=w.keys, new_keys=new_keys)
         assert r.n_terms >= 3 * sms * 256, "k_splice's term loop takes fewer than three trips"
-        rs = _check_result(m, orc, got[0], got[1:], r, f"{kind}, seal")
+        rs = check_result(m, orc, got[0], got[1:], r, f"{kind}, seal")
         assert np.array_equal(got[0].df(), rs.df), f"{kind}: bm25x_index_get_df of the seal's result"
         ref = m.Index(r.n_docs, r.doc_len, r.n_terms, r.post_off, r.post_doc, r.post_tf, payload=r.payload,
                       term_keys=r.term_keys)
@@ -126,13 +109,13 @@ def test_more_terms_than_warps(m, orc, kind):
             rows = got[0].search_batch(q_off, q_new, k)
             same_rows(rows, ref.search_batch(q_off, q_new, k), f"{kind}, result k={k}")
             first = {key: rows[key][:50] for key in ROWS}
-            _compare(first, oix, q_off[:51], q_new, k, what=f"{kind}, result against the oracle k={k}")
+            compare(first, oix, q_off[:51], q_new, k, what=f"{kind}, result against the oracle k={k}")
     finally:
         seg.close()
         for ix in (got[0] if got else None, ref, w.ix):
             if ix is not None:
                 ix.close()
-    free_after[kind] = _free_bytes()
+    free_after[kind] = free_bytes()
 
 
 def test_device_memory_back_to_baseline():

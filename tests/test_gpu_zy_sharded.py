@@ -4,17 +4,9 @@ k = 10 and 100.  The whole index and four shards together hold about 31 GB of HB
 import numpy as np
 import pytest
 
-import _pkg
+from util_lib import gpu_library  # noqa: F401  (gpu_library: the module fixture m)
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def m():
-    mod = _pkg.load()
-    mod.load_library()
-    assert mod.device_count() >= 1, "no CUDA device: the engine has no CPU fallback"
-    return mod
 
 
 def test_c3_two_and_four_shards_identical(m):

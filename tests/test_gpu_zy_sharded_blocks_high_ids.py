@@ -8,23 +8,15 @@ from types import SimpleNamespace
 import numpy as np
 import pytest
 
-import _pkg
-from test_gpu_zy_high_doc_ids import B, K1, N_A, _Prefix, _need, _queries
-from util_sparse import T31, assert_rows, full_fieldnorm, high_id_corpus, reference, sum_len_of
+from util_lib import gpu_library  # noqa: F401  (gpu_library: the module fixture m)
+from util_sparse import (B, K1, N_A, T31, Prefix, assert_rows, full_fieldnorm, high_id_corpus, high_id_queries, need,
+                         reference, sum_len_of)
 
 pytestmark = pytest.mark.gpu
 
 
-@pytest.fixture(scope="module")
-def m():
-    mod = _pkg.load()
-    mod.load_library()
-    assert mod.device_count() >= 1, "no CUDA device: the engine has no CPU fallback"
-    return mod
-
-
 def test_sharded_from_blocks_above_2_31(m, orc):
-    _need(45, 34, "sharded index from blocks (2^32 - 66 documents)")
+    need(45, 34, "sharded index from blocks (2^32 - 66 documents)")
     c = high_id_corpus(N_A)
     ref = reference(orc, c, K1, B)
     eb = orc.EncodedBlocks(SimpleNamespace(n_terms=c.n_terms, post_off=c.post_off, post_doc=c.post_doc,
@@ -42,8 +34,8 @@ def test_sharded_from_blocks_above_2_31(m, orc):
     got = sx.search_batch(np.array([0, 1], np.uint32), np.array([w], np.uint32), 1025, want_payload=True)
     assert sorted(got["doc"][0, :int(got["n"][0])].tolist()) == ids.tolist()
     assert_rows(got, ref, [[w]], 1025, "wide term")
-    q_off, q_terms, qs = _queries(c, 15)
-    pref = _Prefix(ref, 1025)
+    q_off, q_terms, qs = high_id_queries(c, 15)
+    pref = Prefix(ref, 1025)
     for k in (1, 10, 129, 1025):
         res = sx.search_batch(q_off, q_terms, k, want_payload=True)
         assert_rows(res, pref, qs, k, f"sharded from blocks k={k}")

@@ -6,21 +6,12 @@ import subprocess
 import tempfile
 
 import numpy as np
-import pytest
 
-import _pkg
+from util_lib import host_library  # noqa: F401  (host_library: the module fixture m)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CALLS = ["bm25x_growing_open", "bm25x_growing_insert", "bm25x_growing_delete", "bm25x_growing_refresh",
          "bm25x_growing_get_info", "bm25x_growing_search_batch", "bm25x_growing_get_index", "bm25x_growing_close"]
-
-
-@pytest.fixture(scope="module")
-def m():
-    mod = _pkg.load()
-    mod.build_library()
-    mod.load_library()
-    return mod
 
 
 def test_growing_segment_symbols_exported(m):

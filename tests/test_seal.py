@@ -8,22 +8,13 @@ import tempfile
 from types import SimpleNamespace
 
 import numpy as np
-import pytest
 
-import _pkg
 from util_index import ctid
+from util_lib import host_library  # noqa: F401  (host_library: the module fixture m)
 from util_maintain import MISSING, maintain
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 NONE = 0xFFFFFFFF
-
-
-@pytest.fixture(scope="module")
-def m():
-    mod = _pkg.load()
-    mod.build_library()
-    mod.load_library()
-    return mod
 
 
 def test_seal_symbol_exported(m):

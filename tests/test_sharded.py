@@ -8,17 +8,9 @@ import re
 import numpy as np
 import pytest
 
-import _pkg
+from util_lib import host_library, refused  # noqa: F401  (host_library: the module fixture m)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-@pytest.fixture(scope="module")
-def m():
-    mod = _pkg.load()
-    mod.build_library()
-    mod.load_library()
-    return mod
 
 
 def _corpus(n_docs=40):
@@ -30,12 +22,6 @@ def _corpus(n_docs=40):
     post_tf = np.ones(len(post_doc), np.uint32)
     doc_len = np.bincount(post_doc, minlength=n_docs).astype(np.uint32) + 1
     return dict(n_docs=n_docs, doc_len=doc_len, n_terms=len(lists), post_off=off, post_doc=post_doc, post_tf=post_tf)
-
-
-def _refused(m, fn):
-    with pytest.raises(m.Bm25xError) as e:
-        fn()
-    return e.value.code, str(e.value)
 
 
 @pytest.mark.parametrize("n_shards, bounds, what", [
@@ -50,7 +36,7 @@ def _refused(m, fn):
 def test_malformed_shards_refused(m, n_shards, bounds, what):
     c = _corpus(12) if bounds == "small" else _corpus()
     bounds = None if bounds == "small" else bounds
-    code, msg = _refused(m, lambda: m.ShardedIndex(**c, n_shards=n_shards, doc_bounds=bounds))
+    code, msg = refused(m, lambda: m.ShardedIndex(**c, n_shards=n_shards, doc_bounds=bounds))
     assert code == 1 and what in msg and "bm25x_sharded_create" in msg, msg
 
 
@@ -75,34 +61,34 @@ def test_malformed_corpora_refused_as_index_create(m):
     cases.append((c, 4, "bm25x_index_create: term frequency >= 2^24 is not supported"))
     for c, code, what in cases:
         for n_shards in (1, 2, 0):   # the corpus is refused first, whatever the shard arguments
-            got, msg = _refused(m, lambda: m.ShardedIndex(**c, n_shards=n_shards))
+            got, msg = refused(m, lambda: m.ShardedIndex(**c, n_shards=n_shards))
             assert got == code and what in msg, (n_shards, msg)
 
 
 def test_refusals_before_the_device_check_match_index_create(m):
     """Refusals that bm25x_index_create makes before it looks for a device: the same code and the same message."""
     for kw in (dict(k1=-1.0), dict(b=1.5)):
-        want = _refused(m, lambda: m.Index(**_corpus(), **kw))
+        want = refused(m, lambda: m.Index(**_corpus(), **kw))
         assert want[0] == 1
-        assert _refused(m, lambda: m.ShardedIndex(**_corpus(), n_shards=2, **kw)) == want
+        assert refused(m, lambda: m.ShardedIndex(**_corpus(), n_shards=2, **kw)) == want
     c = _corpus()
     c["n_docs"], c["doc_len"] = 0, np.zeros(0, np.uint32)
     c["post_doc"] = c["post_doc"][:0]
     c["post_tf"] = c["post_tf"][:0]
     c["post_off"] = np.zeros(len(c["post_off"]), np.uint64)
-    want = _refused(m, lambda: m.Index(**c))
+    want = refused(m, lambda: m.Index(**c))
     assert want[0] == 1 and "empty or malformed corpus" in want[1]
-    assert _refused(m, lambda: m.ShardedIndex(**c, n_shards=1)) == want
+    assert refused(m, lambda: m.ShardedIndex(**c, n_shards=1)) == want
 
 
 def test_no_cpu_fallback(m):
     if m.device_count() > 0:
         pytest.skip("GPU present")
-    code, msg = _refused(m, lambda: m.ShardedIndex(**_corpus(), n_shards=2))
+    code, msg = refused(m, lambda: m.ShardedIndex(**_corpus(), n_shards=2))
     assert code == 2 and "no CPU fallback" in msg
-    code, msg = _refused(m, lambda: m.ShardedIndex(**_corpus(), n_shards=3, doc_bounds=[0, 7, 13, 40], devices=[0, 0, 0]))
+    code, msg = refused(m, lambda: m.ShardedIndex(**_corpus(), n_shards=3, doc_bounds=[0, 7, 13, 40], devices=[0, 0, 0]))
     assert code == 2 and "no CPU fallback" in msg
-    code, msg = _refused(m, lambda: m.merge_shards([dict(doc=np.zeros((1, 1), np.uint32), score=np.zeros((1, 1), np.float32),
+    code, msg = refused(m, lambda: m.merge_shards([dict(doc=np.zeros((1, 1), np.uint32), score=np.zeros((1, 1), np.float32),
                                                          score64=np.zeros((1, 1)), payload=np.zeros((1, 1, 3), np.uint16),
                                                          n=np.zeros(1, np.uint32))], [0], 1))
     assert code == 2 and "no CPU fallback" in msg

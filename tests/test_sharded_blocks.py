@@ -9,18 +9,10 @@ import re
 import numpy as np
 import pytest
 
-import _pkg
+from util_lib import host_library, refused  # noqa: F401  (host_library: the module fixture m)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 WHO = "bm25x_index_create_from_blocks"
-
-
-@pytest.fixture(scope="module")
-def m():
-    mod = _pkg.load()
-    mod.build_library()
-    mod.load_library()
-    return mod
 
 
 def _corpus(n_docs=600):
@@ -41,12 +33,6 @@ def _blocks(orc, c):
     return dict(n_docs=c["n_docs"], n_terms=c["n_terms"], term_blk_off=eb.term_blk_off, blk_min_doc=eb.blk_min,
                 blk_n=eb.blk_n, blk_meta_doc=eb.meta_doc, blk_meta_tf=eb.meta_tf, blk_doc_off=eb.doc_off,
                 blk_tf_off=eb.tf_off, data=eb.bytes[:eb.n_bytes], doc_len=c["doc_len"])
-
-
-def _refused(m, fn):
-    with pytest.raises(m.Bm25xError) as e:
-        fn()
-    return e.value.code, str(e.value)
 
 
 def _host_refusals(orc):
@@ -82,9 +68,9 @@ def test_block_refusals_match_index_from_blocks(m, orc):
     for blocks, code, msg, before_device in _host_refusals(orc):
         want = (code, f"bm25x error {code}: {msg}")
         if before_device or gpu:
-            assert _refused(m, lambda: m.Index.from_blocks(**blocks)) == want
+            assert refused(m, lambda: m.Index.from_blocks(**blocks)) == want
         for n_shards in (1, 2, 0):
-            got = _refused(m, lambda: m.ShardedIndex.from_blocks(**blocks, n_shards=n_shards))
+            got = refused(m, lambda: m.ShardedIndex.from_blocks(**blocks, n_shards=n_shards))
             assert got == want, (n_shards, got)
 
 
@@ -104,8 +90,8 @@ def test_shard_refusals_match_sharded_index(m, orc, n_shards, bounds):
                       blk_tf_off=eb.tf_off, data=eb.bytes[:eb.n_bytes], doc_len=c["doc_len"])
     else:
         blocks = _blocks(orc, c)
-    want = _refused(m, lambda: m.ShardedIndex(**c, n_shards=n_shards, doc_bounds=bounds))
-    got = _refused(m, lambda: m.ShardedIndex.from_blocks(**blocks, n_shards=n_shards, doc_bounds=bounds))
+    want = refused(m, lambda: m.ShardedIndex(**c, n_shards=n_shards, doc_bounds=bounds))
+    got = refused(m, lambda: m.ShardedIndex.from_blocks(**blocks, n_shards=n_shards, doc_bounds=bounds))
     assert want[0] == 1 and "bm25x_sharded_create" in want[1]
     assert got == want
 
@@ -114,9 +100,9 @@ def test_no_cpu_fallback(m, orc):
     if m.device_count() > 0:
         pytest.skip("GPU present")
     blocks = _blocks(orc, _corpus())
-    code, msg = _refused(m, lambda: m.ShardedIndex.from_blocks(**blocks, n_shards=2))
+    code, msg = refused(m, lambda: m.ShardedIndex.from_blocks(**blocks, n_shards=2))
     assert code == 2 and "no CPU fallback" in msg and "bm25x_index_create_sharded_from_blocks" in msg
-    code, msg = _refused(m, lambda: m.ShardedIndex.from_blocks(**blocks, n_shards=3, doc_bounds=[0, 7, 13, 600],
+    code, msg = refused(m, lambda: m.ShardedIndex.from_blocks(**blocks, n_shards=3, doc_bounds=[0, 7, 13, 600],
                                                                 devices=[0, 0, 0]))
     assert code == 2 and "no CPU fallback" in msg
 

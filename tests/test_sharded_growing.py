@@ -8,17 +8,9 @@ import re
 import numpy as np
 import pytest
 
-import _pkg
+from util_lib import host_library  # noqa: F401  (host_library: the module fixture m)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-@pytest.fixture(scope="module")
-def m():
-    mod = _pkg.load()
-    mod.build_library()
-    mod.load_library()
-    return mod
 
 
 def test_null_arguments_refused(m):

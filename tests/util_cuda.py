@@ -42,6 +42,12 @@ def device_synchronize():
     assert cudart().cudaDeviceSynchronize() == 0
 
 
+def free_bytes():
+    free, total = ctypes.c_size_t(), ctypes.c_size_t()
+    assert cudart().cudaMemGetInfo(ctypes.byref(free), ctypes.byref(total)) == 0
+    return free.value
+
+
 def sm_count(device=0):
     """Streaming multiprocessors of `device` (cudaDevAttrMultiProcessorCount)."""
     v = ctypes.c_int(0)

@@ -15,6 +15,8 @@ from fractions import Fraction
 
 import numpy as np
 
+from util_parity import KERNEL_PATHS
+
 F32 = np.float32
 U = 2.0 ** -24        # f32 unit roundoff
 KEPS = 2.0 ** -18     # kEps of k_search_ring: reject only when F < f32_rd(Sk·(1 − kEps) − …)
@@ -427,3 +429,25 @@ def _corpus(orc, dfs, s0d, s1d, m, k, n_docs, n_high, n_low, n_late, dense, n_ra
                 tight_pruned=F_probe < f32_rd(S_a),
                 keeps_pruned=F_probe >= FloT and (F_str is None or F_str >= Flo_p),
                 max_keps=largest_rejecting_keps(F_b, S_a))
+
+
+# The near-threshold cases of test_gpu_margins.py, one per kernel path the margin is load-bearing on.
+# name: (near_threshold_case arguments, kernel path options, launches of the batch's one class)
+MARGIN_CASES = {
+    "plain_6_lanes": (dict(m=5, k=10, n_docs=1000000), KERNEL_PATHS["plain"], 1),    # class 8, KEEPW verification
+    "class_16": (dict(m=15, k=10, n_docs=1000000), KERNEL_PATHS["plain"], 1),        # filter_term loop
+    "class_32": (dict(m=31, k=10, n_docs=1000000), KERNEL_PATHS["plain"], 1),
+    "seeded_4_lanes": (dict(m=3, k=10, n_docs=1000000), KERNEL_PATHS["seeded"], 2),  # seeded launch + (empty) hand-back launch
+    "two_phase": (dict(m=3, k=10, n_docs=1000000), KERNEL_PATHS["twophase"], 2),     # suspend launch, resume launch (doc ids) finds B
+    "two_pass": (dict(m=8, k=10, n_docs=1000000, n_rare=32), KERNEL_PATHS["plain"], 1),  # 41 lanes: B holds group 1 only
+    "dense_window": (dict(m=4, k=10, n_docs=60000, binade=8.0, dense=True), KERNEL_PATHS["plain"], 1),
+    "hbm_pool": (dict(m=3, k=1025, n_docs=1000000), KERNEL_PATHS["plain"], 1),       # k = 1025: pool in HBM, lazy cut
+}
+
+
+def hands_back(c, opts, prune):
+    """The seeded launch's test at query start: a list of n_docs / seed_dense_div postings or more (dense), or with pruning
+    on, a list of seed_prune_min or more that is 8 times the shortest (skewed)."""
+    mx, mn = int(max(c["df"])), int(min(c["df"]))
+    div = opts["seed_dense_div"]
+    return bool((prune and mx >= opts["seed_prune_min"] and mx // 8 >= mn) or (div and mx >= c["n_docs"] // div + 1))

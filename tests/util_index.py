@@ -194,3 +194,54 @@ def assert_matches(got, lay, der, r, what, skip=()):
             bad = np.flatnonzero(have != want)
             raise AssertionError(f"{what}: {name} differs at {len(bad)} entries, first {bad[:4].tolist()}: "
                                  f"device {have[bad[:4]].tolist()} restatement {want[bad[:4]].tolist()}")
+
+
+def growing_csr(g, T, sealed_df):
+    """The growing documents inverted, as search.rs:83-135 sees them: no posting from a deleted document, from a token the
+    sealed segment does not know, or from a term with no sealed posting."""
+    n = len(g.elem_off) - 1
+    owner = np.repeat(np.arange(n), np.diff(g.elem_off.astype(np.int64)))
+    term = g.elem_term.astype(np.int64)
+    keep = (g.deleted[owner] == 0) & (term < T)
+    keep[keep] = sealed_df[term[keep]] > 0
+    t, d, tf = term[keep], owner[keep], g.elem_tf[keep]
+    order = np.lexsort((d, t))
+    off = np.zeros(T + 1, np.uint64)
+    off[1:] = np.cumsum(np.bincount(t, minlength=T))
+    return off, d[order].astype(np.uint32), tf[order].astype(np.uint32)
+
+
+def local_csr(off, doc, tf, lo, hi):
+    o = off.astype(np.int64)
+    term = np.repeat(np.arange(len(o) - 1), np.diff(o))
+    keep = (doc >= lo) & (doc < hi)
+    loff = np.zeros(len(o), np.uint64)
+    loff[1:] = np.cumsum(np.bincount(term[keep], minlength=len(o) - 1))
+    return loff, (doc[keep] - lo).astype(np.uint32), tf[keep]
+
+
+def check_shards(m, orc, c, sx, ix, k1, b, what):
+    """Every shard against the restatement of its local CSR with the whole segment's statistics; its score tables
+    byte-equal to the unsharded index's; its champion lists the whole ranking of each term restricted to its documents."""
+    N, T = int(c["n_docs"]), int(c["n_terms"])
+    off, doc, tf = c["post_off"], np.asarray(c["post_doc"]), np.asarray(c["post_tf"])
+    df = np.diff(off.astype(np.int64))
+    stat = (N, df, float(int(np.asarray(c["doc_len"], np.uint64).sum())) / N)
+    whole = read_back(ix.layout(), ix.derived())
+    rw = restate(orc, N, off, doc, tf, k1, b, doc_len=c["doc_len"])
+    bounds = sx.doc_bounds()
+    for s in range(len(bounds) - 1):
+        lo, hi = int(bounds[s]), int(bounds[s + 1])
+        lay, der = sx.shard_arrays(s)
+        got = read_back(lay, der)
+        loff, ldoc, ltf = local_csr(off, doc, tf, lo, hi)
+        r = restate(orc, hi - lo, loff, ldoc, ltf, k1, b, doc_len=c["doc_len"][lo:hi], stat=stat, doc_base=lo)
+        assert_matches(got, lay, der, r, f"{what} shard {s} [{lo}, {hi})")
+        for key in ("s0d", "s0f", "s1d", "s1f"):
+            assert got[key].tobytes() == whole[key].tobytes(), f"{what} shard {s}: {key} differs from the whole index's"
+        inside = (doc >= lo) & (doc < hi)
+        sub = np.flatnonzero(inside)
+        champ, champ_off = champion_lists(rw.term[sub], doc[sub].astype(np.int64) - lo, (tf[sub].astype(np.int64) << 8) |
+                                          rw.fieldnorm[doc[sub]], rw.score[sub], np.bincount(rw.term[sub], minlength=T))
+        assert np.array_equal(got["champ_off"], champ_off), f"{what} shard {s}: champion offsets"
+        assert np.array_equal(got["champ"], champ.reshape(-1)), f"{what} shard {s}: not the whole ranking restricted"

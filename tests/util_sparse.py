@@ -8,12 +8,17 @@ oracle's Cache (util_index.cache); the posting-side arrays of a handle come from
 against OracleIndex.search_exhaustive and util_index.restate by tests/test_sparse_reference.py.
 
 high_id_corpus() builds the corpus of tests/test_gpu_zy_high_doc_ids.py: a few hundred thousand postings on documents
-placed on purpose across the 32-bit id space."""
+placed on purpose across the 32-bit id space; high_id_queries() the queries over it, and need() skips a test whose index
+does not fit in the host or device memory available."""
+import ctypes
 from types import SimpleNamespace
 
 import numpy as np
+import pytest
 
+from util_cuda import cudart
 from util_index import cache, ctid, restate_postings
+from util_parity import query_csr
 
 DOC_INF = 0xFFFFFFFF
 MAX_N_DOCS = 0xFFFFFFFE  # the largest n_docs the library accepts; the largest doc id is MAX_N_DOCS - 1
@@ -195,3 +200,56 @@ def reference(orc, c, k1, b):
     post_fn = c.live_fn[np.searchsorted(c.live, c.post_doc.astype(np.int64))]
     return SparseReference(orc, c.n_docs, c.post_off, c.post_doc, c.post_tf, k1, b, sum_len_of(orc, c), post_fn=post_fn,
                            norms=norms)
+
+
+# ---- the high-id indexes ----
+
+N_A = MAX_N_DOCS - 64       # index A: room for a growing segment of 64 documents, ids up to 0xFFFFFFFD
+K1, B = 1.2, 0.75
+
+
+def need(host_gb, dev_gb, what):
+    import psutil
+    free, total = ctypes.c_size_t(0), ctypes.c_size_t(0)
+    assert cudart().cudaMemGetInfo(ctypes.byref(free), ctypes.byref(total)) == 0
+    host = psutil.virtual_memory().available
+    if host < host_gb * 1e9 or free.value < dev_gb * 1e9:
+        pytest.skip(f"{what} needs {host_gb} GB of host and {dev_gb} GB of free device memory "
+                    f"({host / 1e9:.0f} GB / {free.value / 1e9:.0f} GB available)")
+
+
+def peak_host_gb():
+    import resource
+    return resource.getrusage(resource.RUSAGE_SELF).ru_maxrss / 1e6
+
+
+def high_id_queries(c, seed):
+    """Queries of 1, 2, 3, 4, 5-8, 9-16, 17-32 and 33-64 live terms over the corpus' kinds of terms."""
+    k = c.kinds
+    rng = np.random.default_rng(seed)
+    rand = lambda n: rng.choice(c.n_terms, n, replace=False)
+    qs = [[t] for t in k["tie"] + k["dense"][:2] + k["pad"] + k["wide"] + k["head"][:1] + k["fill"][-2:]]
+    qs += [[k["tie"][0], k["dense"][0]], [k["head"][0], k["tie"][1]], k["dense"][:2], [k["pad"][0], k["tie"][2]]]
+    qs += [k["dense"][:3], [k["head"][0], k["head"][1], k["tie"][0]], k["tie"]]
+    qs += [k["dense"][:4], k["pad"] + k["dense"][:2] + k["wide"], k["tie"] + k["pad"]]
+    qs += [k["dense"] + k["pad"], k["head"] + k["tie"], list(rand(5)), list(rand(8))]
+    qs += [k["dense"] + k["tie"] + list(rand(3)), list(rand(16)), list(rand(17)), list(rand(32)), list(rand(33)),
+           list(rand(64))]
+    qs = [np.unique(np.asarray(q, np.uint32)) for q in qs]
+    q_off, q_terms = query_csr(qs)
+    return q_off, q_terms, qs
+
+
+class Prefix:
+    """SparseReference.search at one limit per (query, bitmap): every smaller limit's rows are a prefix."""
+
+    def __init__(self, ref, kmax):
+        self.ref, self.kmax, self.memo = ref, kmax, {}
+
+    def search(self, terms, k, allow=None):
+        key = (np.asarray(terms, np.uint32).tobytes(), id(allow))
+        if key not in self.memo:
+            self.memo[key] = self.ref.search(terms, self.kmax, allow=allow)
+        r = self.memo[key]
+        n = min(k, r.n)
+        return SimpleNamespace(doc=r.doc[:n], score64=r.score64[:n], score=r.score[:n], payload=r.payload[:n], n=n)

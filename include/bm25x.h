@@ -118,6 +118,51 @@ typedef struct {
 } bm25x_blocks;
 int bm25x_index_create_from_blocks(const bm25x_blocks *blocks, int device, bm25x_index **out);
 
+/* ---- the inverse: a finalized index written out as the reference's stored segment, i.e. everything flush() writes for
+ * it (flush.rs:40-158) but the pages, tapes and address trees, which stay the caller's.  Encoded on the index's device:
+ * per token, blocks of 128 postings in doc order, the last one shorter (flush.rs:78-90; the index's own blocks); payloads
+ * in the codec of compression.rs:36-110 (full blocks bit-packed in the 4-lane vertical layout, doc ids delta-coded from
+ * the block's first id, width 32 raw; shorter blocks byte-packed, byte width 4 raw), per block the doc payload then the
+ * tf payload, blocks in token order.  The directory and `bytes` feed bm25x_index_create_from_blocks as they are (the
+ * doc_fieldnorm + sum_doc_len form: the handle keeps quantised norms, never exact lengths).
+ * n_docs, n_terms, n_blocks: those bm25x_index_get_info reports.  Every output array is optional (NULL: not written).
+ * bytes == NULL is a sizing call: it sets n_bytes and writes nothing else.  Refused with BM25X_ERR_INVALID: a null idx or
+ * out; term_key on an index without term keys (a finalized replica, a seal of one); a replica not finalized yet; a
+ * handle that scores with another segment's statistics, i.e. whose avgdl is not its Σlen / n_docs (bm25x_growing_create's
+ * handles score with the sealed segment's: flush would write other Wand pairs for their documents); bytes_cap < n_bytes (n_bytes is set, nothing else is written).  Every refusal, and every device allocation
+ * (BM25X_ERR_OOM), comes before the first output byte; after a later CUDA failure (BM25X_ERR_CUDA) the outputs are
+ * unspecified.  The handle is not changed, and the export runs on a stream of its own: searches on the same handle may
+ * run meanwhile.  Device memory beyond the index: about 35 bytes per block plus one payload chunk of at most 256 MiB. */
+typedef struct {
+    /* per document: DocumentTuple (tuples.rs:756-762) and JumpTuple (tuples.rs:141-160) */
+    uint8_t *doc_fieldnorm;        /* [n_docs] DocumentTuple.fieldnorm, or NULL */
+    uint16_t *payload;             /* [n_docs*3] DocumentTuple.payload: the stored ctid, the synthetic one when none was
+                                      given; or NULL */
+    uint64_t sum_doc_len;          /* out: JumpTuple.sum_of_document_lengths, the handle's Σlen */
+    /* per token: TokenTuple (flush.rs:126-135) */
+    uint8_t *term_key;             /* [n_terms*16] TokenTuple.id, or NULL; refused on an index without term keys */
+    uint32_t *tok_df;              /* [n_terms] TokenTuple.number_of_documents, or NULL */
+    uint8_t *tok_wand_fieldnorm;   /* [n_terms] TokenTuple.wand_fieldnorm: Wand::extend over the token's blocks in order
+                                      (flush.rs:111-112, bm25.rs:319-325); 255 for a token without postings; or NULL */
+    uint32_t *tok_wand_tf;         /* [n_terms] TokenTuple.wand_term_frequency; 0 for a token without postings; or NULL */
+    uint64_t *term_blk_off;        /* [n_terms+1] first block of each token, or NULL */
+    /* per block: SummaryTuple (flush.rs:113-120) + BlockTuple (flush.rs:91-100) */
+    uint32_t *blk_min_doc;         /* [n_blocks] SummaryTuple.min_document_id: the block's first doc id, or NULL */
+    uint32_t *blk_max_doc;         /* [n_blocks] SummaryTuple.max_document_id: its last, or NULL */
+    uint32_t *blk_n;               /* [n_blocks] SummaryTuple.number_of_documents, or NULL */
+    uint8_t *blk_meta_doc;         /* [n_blocks] BlockTuple.metadata_document_ids: flag << 7 | width, or NULL */
+    uint8_t *blk_meta_tf;          /* [n_blocks] BlockTuple.metadata_term_frequencies, or NULL */
+    uint64_t *blk_doc_off;         /* [n_blocks] byte offset of compressed_document_ids inside `bytes`, or NULL */
+    uint64_t *blk_tf_off;          /* [n_blocks] byte offset of compressed_term_frequencies inside `bytes`, or NULL */
+    uint8_t *blk_wand_fieldnorm;   /* [n_blocks] SummaryTuple.wand_fieldnorm: Wand over the block's postings in doc order
+                                      (bm25.rs:297-318), the first posting of the largest tf() (bm25.rs:291-295); or NULL */
+    uint32_t *blk_wand_tf;         /* [n_blocks] SummaryTuple.wand_term_frequency, or NULL */
+    uint8_t *bytes;                /* [bytes_cap] the concatenated block payloads, or NULL: a sizing call */
+    uint64_t bytes_cap;
+    uint64_t n_bytes;              /* out: the payload size, set by every call that gets past the argument checks */
+} bm25x_export;
+int bm25x_index_export_blocks(const bm25x_index *idx, bm25x_export *out);
+
 /* ---- replication across the GPUs of one box (queries shard, the index is replicated; NCCL broadcast at load
  * only).  The library stays NCCL-free: it exposes the device arrays, the caller moves the bytes (bench.py uses
  * torch.distributed.broadcast over NVLink).  Sender: bm25x_index_get_layout.  Receiver: bm25x_index_alloc_replica

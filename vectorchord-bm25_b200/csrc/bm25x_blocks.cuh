@@ -7,7 +7,8 @@
 //   * a token's last, shorter block: 1..4 little-endian bytes per value (bytepacking_u32_ordered.rs / _unordered.rs).
 // One warp decodes one block: lane `it` owns input vector `it` of the macro, i.e. values 4*it .. 4*it+3, so the delta
 // prefix sum is a 4-element local scan plus one warp scan.  The result is written straight into the engine's posting
-// layout {doc, tf << 8 | fieldnorm(doc)}.
+// layout {doc, tf << 8 | fieldnorm(doc)}.  The encoder of the same codec (bm25x_index_export_blocks) is at the end of
+// this file, with the same lane mapping.
 #pragma once
 
 #include "bm25x_build.h"
@@ -335,7 +336,201 @@ k_decode_shard_blocks(uint64_t n_blocks, const uint64_t *__restrict__ sel_off, u
     if (bad) atomicOr(err, bad);
 }
 
-}  // namespace
+// ---- export (bm25x_index_export_blocks, DESIGN §4.4): the encoder of the same codec, compress_document_ids /
+// compress_term_frequencies (compression.rs:36-110), over an index's own blocks.  One warp per block with the decoder's
+// lane mapping: lane `it` holds postings 4*it .. 4*it+3 ----
+
+// Metadata byte of a stream of n values whose OR has `bits` significant bits: the bit width of a full block, else the
+// byte width div_ceil(bits, 8).max(1) with the flag (compression.rs:43-62, bytepacking_u32_ordered.rs:29).
+__host__ __device__ __forceinline__ uint8_t stream_meta(uint32_t bits, uint32_t n) {
+    if (n == BM25X_BLOCK) return (uint8_t)bits;
+    const uint32_t by = (bits + 7u) / 8u;
+    return (uint8_t)(0x80u | (by ? by : 1u));
+}
+
+// Block g of an index (blocks of 128 postings per term, the last shorter) in the lane's registers: returns n, fills
+// doc / w (tf << 8 | fieldnorm) of postings 4*lane .. 4*lane+3, zero past n.
+__device__ __forceinline__ uint32_t load_block(uint64_t g, uint32_t lane, const uint64_t *__restrict__ blk_off,
+                                               uint32_t n_terms, const uint64_t *__restrict__ post_off,
+                                               const uint32_t *__restrict__ df, const Posting *__restrict__ post,
+                                               uint32_t doc[4], uint32_t w[4]) {
+    const uint32_t t = owner_of(blk_off, n_terms, g);
+    const uint64_t k = g - blk_off[t];
+    const uint64_t rest = df[t] - k * BM25X_BLOCK;
+    const uint32_t n = rest < BM25X_BLOCK ? (uint32_t)rest : BM25X_BLOCK;
+    const Posting *src = post + post_off[t] + k * BM25X_BLOCK;
+#pragma unroll
+    for (uint32_t l = 0; l < 4; l++) {
+        const uint32_t i = 4u * lane + l;
+        const Posting p = i < n ? src[i] : Posting{0u, 0u};
+        doc[l] = p.doc;
+        w[l] = p.w;
+    }
+    return n;
+}
+
+// The doc-id stream's values as compress_document_ids stores them: deltas from min_doc, or the ids themselves at bit width
+// 32 / byte width 4 (bitpacking_u32_ordered.rs:119-121, bytepacking_u32_ordered.rs:195).  Returns the OR of the deltas.
+__device__ __forceinline__ uint32_t doc_deltas(const uint32_t doc[4], uint32_t n, uint32_t lane, uint32_t min_doc,
+                                               uint32_t v[4]) {
+    const uint32_t before = __shfl_up_sync(0xFFFFFFFFu, doc[3], 1);
+    uint32_t acc = 0;
+#pragma unroll
+    for (uint32_t l = 0; l < 4; l++) {
+        const uint32_t prev = l ? doc[l - 1] : (lane ? before : min_doc);
+        v[l] = 4u * lane + l < n ? doc[l] - prev : 0u;
+        acc |= v[l];
+    }
+    return __reduce_or_sync(0xFFFFFFFFu, acc);
+}
+
+// Directory pass: per block its SummaryTuple (min / max from blk, n, the Wand pair) and the two metadata bytes.  wand_v =
+// the pair's tf() (bm25.rs:291-295: (tf·(k1+1)) / (tf + s1[fn]), k1p1 = k1 + 1), which the token pass folds.
+__global__ void __launch_bounds__(DEC_WARPS * 32)
+k_export_dir(uint64_t n_blocks, const uint64_t *__restrict__ blk_off, uint32_t n_terms,
+             const uint64_t *__restrict__ post_off, const uint32_t *__restrict__ df, const Posting *__restrict__ post,
+             const uint2 *__restrict__ blk, const double *__restrict__ s1d, double k1p1, uint32_t *__restrict__ min_doc,
+             uint32_t *__restrict__ max_doc, uint32_t *__restrict__ blk_n, uint8_t *__restrict__ meta_doc,
+             uint8_t *__restrict__ meta_tf, uint8_t *__restrict__ wand_fn, uint32_t *__restrict__ wand_tf,
+             double *__restrict__ wand_v) {
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
+    const uint64_t g = (uint64_t)blockIdx.x * DEC_WARPS + warp;
+    if (g >= n_blocks) return;  // whole warps leave
+    uint32_t doc[4], w[4], v[4];
+    const uint32_t n = load_block(g, lane, blk_off, n_terms, post_off, df, post, doc, w);
+    const uint2 mm = blk[g];
+    const uint32_t or_doc = doc_deltas(doc, n, lane, mm.x, v);
+    // Wand::push (bm25.rs:297-318): a posting replaces the pair only when its tf() is strictly greater, so the first
+    // posting of the largest tf() wins; the start pair (0.0, 255, 0) is never replaced by NaN
+    uint32_t or_tf = 0, pos = 0xFFFFFFFFu;
+    double best = 0.0;
+#pragma unroll
+    for (uint32_t l = 0; l < 4; l++) {
+        const uint32_t i = 4u * lane + l, tf = w[l] >> 8;
+        or_tf |= tf;
+        if (i >= n) continue;
+        const double tfd = (double)tf;
+        const double x = __ddiv_rn(__dmul_rn(tfd, k1p1), __dadd_rn(tfd, s1d[w[l] & 0xFFu]));
+        if (x > best) {
+            best = x;
+            pos = i;
+        }
+    }
+    or_tf = __reduce_or_sync(0xFFFFFFFFu, or_tf);
+    for (int o = 16; o > 0; o >>= 1) {  // arg-max; equal tf(): the earlier posting
+        const double ob = __shfl_xor_sync(0xFFFFFFFFu, best, o);
+        const uint32_t op = __shfl_xor_sync(0xFFFFFFFFu, pos, o);
+        if (ob > best || (ob == best && op < pos)) {
+            best = ob;
+            pos = op;
+        }
+    }
+    uint32_t mine = w[0];
+#pragma unroll
+    for (uint32_t l = 1; l < 4; l++)
+        if ((pos & 3u) == l) mine = w[l];
+    const uint32_t win = __shfl_sync(0xFFFFFFFFu, mine, (pos >> 2) & 31u);
+    if (lane == 0) {
+        min_doc[g] = mm.x;
+        max_doc[g] = mm.y;
+        blk_n[g] = n;
+        meta_doc[g] = stream_meta(32u - __clz(or_doc), n);
+        meta_tf[g] = stream_meta(32u - __clz(or_tf), n);
+        wand_fn[g] = pos == 0xFFFFFFFFu ? 255u : (uint8_t)(win & 0xFFu);
+        wand_tf[g] = pos == 0xFFFFFFFFu ? 0u : win >> 8;
+        wand_v[g] = best;
+    }
+}
+
+// Token pass: one warp per token folds its blocks' pairs with Wand::extend (bm25.rs:319-325) in block order: strictly
+// greater tf() replaces, so the earliest block wins; a token without blocks keeps (255, 0).
+__global__ void k_export_tokens(uint32_t n_terms, const uint64_t *__restrict__ blk_off, const double *__restrict__ wand_v,
+                                const uint8_t *__restrict__ wand_fn, const uint32_t *__restrict__ wand_tf,
+                                uint8_t *__restrict__ tok_fn, uint32_t *__restrict__ tok_tf) {
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint64_t t = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (t >= n_terms) return;  // whole warps leave
+    double best = 0.0;
+    uint64_t pos = ~0ull;
+    for (uint64_t g = blk_off[t] + lane; g < blk_off[t + 1]; g += 32)
+        if (wand_v[g] > best) {
+            best = wand_v[g];
+            pos = g;
+        }
+    for (int o = 16; o > 0; o >>= 1) {
+        const double ob = __shfl_xor_sync(0xFFFFFFFFu, best, o);
+        const uint64_t op = __shfl_xor_sync(0xFFFFFFFFu, pos, o);
+        if (ob > best || (ob == best && op < pos)) {
+            best = ob;
+            pos = op;
+        }
+    }
+    if (lane == 0) {
+        tok_fn[t] = pos == ~0ull ? 255u : wand_fn[pos];
+        tok_tf[t] = pos == ~0ull ? 0u : wand_tf[pos];
+    }
+}
+
+// One stream of a block, values v (4 per lane) under metadata `meta`, written to dst (byte-aligned).  Full block, width
+// 1..31: the compress! macro (bitpacking.rs:14-52) — value `it` of lane stream l at bit it*bw of that stream, output word
+// 4j + l holds its bits 32j .. 32j+31 — OR-ed together in the warp's shared stage (a value spans at most two words), then
+// copied out; width 32: the values as they are.  Shorter block: `width` little-endian bytes per value.
+__device__ __forceinline__ void encode_stream(uint32_t *stage, uint8_t meta, uint32_t n, uint32_t lane,
+                                              const uint32_t v[4], uint8_t *__restrict__ dst) {
+    const uint32_t width = meta & 0x7Fu;
+    if (meta >> 7) {
+#pragma unroll
+        for (uint32_t l = 0; l < 4; l++) {
+            const uint32_t i = 4u * lane + l;
+            if (i < n)
+                for (uint32_t k = 0; k < width; k++) dst[i * width + k] = (uint8_t)(v[l] >> (8u * k));
+        }
+        return;
+    }
+    if (width == 0) return;
+    if (width == 32) {
+#pragma unroll
+        for (uint32_t l = 0; l < 4; l++) stage[4u * lane + l] = v[l];
+    } else {
+        for (uint32_t i = lane; i < 4u * width; i += 32) stage[i] = 0u;
+        __syncwarp();
+        const uint32_t bit = lane * width, j = bit >> 5, cur = bit & 31u;
+#pragma unroll
+        for (uint32_t l = 0; l < 4; l++) {
+            atomicOr(stage + 4u * j + l, v[l] << cur);
+            if (cur + width > 32u) atomicOr(stage + 4u * (j + 1u) + l, v[l] >> (32u - cur));
+        }
+    }
+    __syncwarp();
+    const uint8_t *bytes = reinterpret_cast<const uint8_t *>(stage);  // little-endian words: the payload's byte order
+    for (uint32_t i = lane; i < 16u * width; i += 32) dst[i] = bytes[i];
+    __syncwarp();  // the stage is reused by the next stream
+}
+
+// Encode pass over the blocks [g0, g0 + n_blocks): block g's doc payload at out + doc_off[g] - base, its tf payload right
+// after it.  The metadata bytes are the directory pass's.
+__global__ void __launch_bounds__(DEC_WARPS * 32)
+k_export_encode(uint64_t g0, uint64_t n_blocks, const uint64_t *__restrict__ blk_off, uint32_t n_terms,
+                const uint64_t *__restrict__ post_off, const uint32_t *__restrict__ df, const Posting *__restrict__ post,
+                const uint2 *__restrict__ blk, const uint8_t *__restrict__ meta_doc, const uint8_t *__restrict__ meta_tf,
+                const uint64_t *__restrict__ doc_off, uint64_t base, uint8_t *__restrict__ out) {
+    __shared__ __align__(16) uint32_t stage[DEC_WARPS][BM25X_BLOCK];
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
+    const uint64_t g = g0 + (uint64_t)blockIdx.x * DEC_WARPS + warp;
+    if (g >= g0 + n_blocks) return;  // whole warps leave; no block-wide barrier below
+    uint32_t doc[4], w[4], v[4];
+    const uint32_t n = load_block(g, lane, blk_off, n_terms, post_off, df, post, doc, w);
+    const uint8_t md = meta_doc[g], mt = meta_tf[g];
+    doc_deltas(doc, n, lane, blk[g].x, v);
+    if (md == 32u || md == (0x80u | 4u))  // stored as they are
+#pragma unroll
+        for (uint32_t l = 0; l < 4; l++) v[l] = doc[l];
+    uint8_t *dst = out + (doc_off[g] - base);
+    encode_stream(stage[warp], md, n, lane, v, dst);
+#pragma unroll
+    for (uint32_t l = 0; l < 4; l++) v[l] = w[l] >> 8;
+    encode_stream(stage[warp], mt, n, lane, v, dst + stream_bytes(md, n));
+}
 
 // Ingest check: the stored SummaryTuple.(wand_fieldnorm, wand_term_frequency) of a block must evaluate to the block's
 // real maximum (it is the arg-max of the block's own postings, flush.rs:101-110); anything else is a corrupt index.
@@ -348,3 +543,5 @@ __global__ void k_check_block_wand(uint64_t n_blocks, const uint64_t *__restrict
     const uint32_t t = owner_of(blk_off, n_terms, g);
     if (!wand_pair_ok(wand_tf[g], wand_fn[g], s0d[t], s1d, blk_ub[g])) atomicOr(err, BM25X_BLKERR_WAND);
 }
+
+}  // namespace

@@ -241,6 +241,37 @@ int bm25x_search_batch(bm25x_index *idx, uint32_t nq, const uint32_t *q_off, con
                        const uint8_t *allow, uint32_t *out_doc, float *out_score, double *out_score64,
                        uint16_t *out_payload, uint32_t *out_n, bm25x_search_stats *stats);
 
+/* ---- Per-query candidate lists: each query's top-k over its own doc ids.  The reference's bm25::search
+ * (crates/bm25/src/search.rs:28-36) takes one filter per index scan, and every scan has its own WHERE clause and
+ * bm25.prefilter (src/index/fetcher.rs:181-215); here every query of the batch carries its own candidate list (a filter's
+ * qualifying rows, or the ids an ANN search returned for hybrid retrieval).
+ *   q_off, q_terms, k: as bm25x_search_batch (up to BM25X_MAX_QUERY_TERMS live terms).
+ *   c_off[nq+1], c_docs[]: query i's candidates are c_docs[c_off[i]..c_off[i+1]): doc ids in any order, duplicates
+ *     allowed (counted once), possibly none.
+ *   outputs: row i is bit for bit the row bm25x_search_batch returns for query i alone with `allow` = the bitmap of its
+ *     candidates: the candidates that hold a live query term, score desc then doc id asc, out_n[i] <= k, empty slots doc
+ *     0xFFFFFFFF with zeros elsewhere.  With k >= |C_i| the row holds every matching candidate with its score.
+ * Refusals, all before any device work (a refused call writes no output): those of bm25x_search_batch with its codes and
+ * messages (null arguments, k == 0, k > BM25X_MAX_K, q_off not monotone, > 64 live terms, replica not finalized); c_off
+ * not monotone and a candidate >= n_docs (BM25X_ERR_INVALID, the message names the query, the entry and the id); more
+ * than 2^31 - 1 candidates of live queries, or more than 2^31 - 1 queries, in one call (BM25X_ERR_UNSUPPORTED).
+ * Thread-safe on one handle, alongside the other searches.  The device sorts every query's candidates by doc id (CUB
+ * segmented sort), looks every (candidate, live term) pair up in the term's block table and then inside its 128-posting
+ * block, and sorts the scores per query (DESIGN §4.8).  Device memory beyond the rows: 24 B per candidate of a live query
+ * (4 B uploaded, 4 B for the sort's second doc-id buffer, 2 x 8 B of sort keys), 8 B per query and 4 B per live query
+ * term uploaded, plus CUB's temporary storage for the two segmented sorts.  Host memory: the upload goes through the
+ * handle's page-locked staging buffer, which bm25x_search_batch shares; it grows to 1.25x the largest upload the handle
+ * has made (about 4 B per candidate plus 8 B per query) and is kept until bm25x_index_destroy, so that repeated calls
+ * of that size do not pay a page-locked allocation each time.
+ * stats: queries = live queries; kernel_ms = device events around the sorts and kernels; launches = 4 when any live
+ * query has a candidate (two segmented sorts counted once each, the lookups, the rows), else 0; h2d_ms, d2h_ms as for
+ * bm25x_search_batch; postings = Σ df of the live terms, as elsewhere (no list is streamed here); postings_fetched =
+ * block-table entries plus postings the lookups read; bytes_algo = 8 B per (candidate, live term) lookup + 8 B per
+ * result slot + 16 B per query term. */
+int bm25x_search_candidates(bm25x_index *idx, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms,
+                            const uint32_t *c_off, const uint32_t *c_docs, uint32_t k, uint32_t *out_doc, float *out_score,
+                            double *out_score64, uint16_t *out_payload, uint32_t *out_n, bm25x_search_stats *stats);
+
 /* Split form of the same call, for pipelining and for timing the device part alone:
  * prepare = canonicalise + upload queries; run = kernels only, everything resident in HBM
  * (stream = cudaStream_t as void*, NULL = the library's stream; asynchronous unless stats != NULL);
@@ -343,6 +374,16 @@ int bm25x_growing_search_batch(bm25x_growing_segment *g, uint32_t nq, const uint
                                uint32_t k, const uint8_t *allow_sealed, const uint8_t *allow_growing,
                                uint32_t allow_growing_docs, uint32_t *out_doc, float *out_score, double *out_score64,
                                uint16_t *out_payload, uint32_t *out_n, bm25x_search_stats *stats);
+/* bm25x_search_candidates over the segment: candidate ids in the result id space (sealed ids below n_docs(sealed),
+ * growing ordinal o as n_docs(sealed) + o); a candidate at or past n_docs(sealed) + n_docs(segment) is refused
+ * (BM25X_ERR_INVALID).  A pending refresh runs first; deleted ordinals are never returned.  Every list (the sealed side's
+ * and the growing handle's) runs the candidate search at k over the candidates in its id range, and the lists are merged
+ * on the device as in bm25x_growing_search_batch, whose refusals, stats and behaviour before the first insert apply
+ * (with bm25x_search_candidates in place of bm25x_search_batch). */
+int bm25x_growing_search_candidates(bm25x_growing_segment *g, uint32_t nq, const uint32_t *q_off,
+                                    const uint32_t *q_terms, const uint32_t *c_off, const uint32_t *c_docs, uint32_t k,
+                                    uint32_t *out_doc, float *out_score, double *out_score64, uint16_t *out_payload,
+                                    uint32_t *out_n, bm25x_search_stats *stats);
 /* Test hook: the arrays of the segment's current handle, as bm25x_sharded_get_shard reports a shard's (either output may
  * be NULL); valid until the next refresh or close.  Refused before the first refresh of a non-empty segment. */
 int bm25x_growing_get_index(const bm25x_growing_segment *g, bm25x_index_layout *layout, bm25x_index_derived *derived);
@@ -424,6 +465,16 @@ int bm25x_sharded_lookup_terms(const bm25x_sharded_index *sx, const uint8_t *key
 int bm25x_sharded_search_batch(bm25x_sharded_index *sx, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms,
                                uint32_t k, const uint8_t *allow, uint32_t *out_doc, float *out_score, double *out_score64,
                                uint16_t *out_payload, uint32_t *out_n, bm25x_search_stats *stats);
+/* bm25x_search_candidates on a document-sharded index.  Named after bm25x_search_batch_growing rather than in the
+ * bm25x_sharded_* family: that family's prototypes are a fixed set, pinned by the binding's declaration test
+ * (tests/test_sharded.py), and this call takes the same sharded handle.  Candidates are global ids, routed by doc_bounds to their shard as
+ * local ids; every shard runs the candidate search at k and the lists are merged on shard 0's device.  Rows equal those
+ * of bm25x_search_candidates on an unsharded index of the same corpus.  Refusals are bm25x_sharded_search_batch's (the
+ * whole segment's canonicalisation first), then those of the candidate lists; stats as bm25x_sharded_search_batch. */
+int bm25x_search_candidates_sharded(bm25x_sharded_index *sx, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms,
+                                    const uint32_t *c_off, const uint32_t *c_docs, uint32_t k, uint32_t *out_doc,
+                                    float *out_score, double *out_score64, uint16_t *out_payload, uint32_t *out_n,
+                                    bm25x_search_stats *stats);
 /* A growing segment over a document-sharded index.  It scores with the whole segment's statistics (as every shard
  * does).  Its handle lives on the LAST shard's device.  After this call the segment is an ordinary
  * bm25x_growing_segment: insert, delete, refresh, get_info, get_index, search_batch and close take it unchanged, with

@@ -176,6 +176,10 @@ def load_library():
     L.bm25x_index_set_option.argtypes = [vp, C.c_char_p, C.c_int64]
     L.bm25x_search_batch.argtypes = [vp, C.c_uint32, u32p, u32p, C.c_uint32, u8p, u32p, f32p, f64p, u16p, u32p,
                                      C.POINTER(SearchStats)]
+    L.bm25x_search_candidates.argtypes = [vp, C.c_uint32, u32p, u32p, u32p, u32p, C.c_uint32, u32p, f32p, f64p, u16p,
+                                          u32p, C.POINTER(SearchStats)]
+    L.bm25x_search_candidates_sharded.argtypes = L.bm25x_search_candidates.argtypes
+    L.bm25x_growing_search_candidates.argtypes = L.bm25x_search_candidates.argtypes
     L.bm25x_batch_prepare.argtypes = [vp, C.c_uint32, u32p, u32p, C.c_uint32, u8p, C.POINTER(vp)]
     L.bm25x_batch_run.argtypes = [vp, vp, C.POINTER(SearchStats)]
     L.bm25x_batch_fetch.argtypes = [vp, u32p, f32p, f64p, u16p, u32p]
@@ -317,6 +321,21 @@ def _search_batch(fn, h, q_off, q_terms, k, allow, want_f64, want_payload, out):
     st = SearchStats()
     _check(fn(h, nq, _p(q_off, C.c_uint32), _p(q_terms, C.c_uint32), int(k), _p(al, C.c_uint8), *_rows_args(out),
               C.byref(st)))
+    out["stats"] = st
+    return out
+
+
+def _search_candidates(fn, h, q_off, q_terms, c_off, c_docs, k, want_f64, want_payload):
+    """bm25x_search_candidates or its sharded / growing form (the same signature) on host buffers."""
+    q_off = np.ascontiguousarray(q_off, dtype=np.uint32)
+    q_terms = np.ascontiguousarray(q_terms, dtype=np.uint32)
+    c_off = np.ascontiguousarray(c_off, dtype=np.uint32)
+    c_docs = np.ascontiguousarray(c_docs, dtype=np.uint32)
+    nq = len(q_off) - 1
+    out = _result_arrays(nq, max(int(k), 1), want_f64, want_payload)
+    st = SearchStats()
+    _check(fn(h, nq, _p(q_off, C.c_uint32), _p(q_terms, C.c_uint32), _p(c_off, C.c_uint32), _p(c_docs, C.c_uint32),
+              int(k), *_rows_args(out), C.byref(st)))
     out["stats"] = st
     return out
 
@@ -531,6 +550,13 @@ class Index:
         return _search_batch(load_library().bm25x_search_batch, self.h, q_off, q_terms, k, allow, want_f64, want_payload,
                              out)
 
+    def search_candidates(self, q_off, q_terms, c_off, c_docs, k, want_f64=True, want_payload=False):
+        """Per-query candidate lists (bm25x_search_candidates): query i's top-k over the doc ids
+        c_docs[c_off[i]:c_off[i+1]] (any order, duplicates counted once) — the rows search_batch returns for query i alone
+        with allow = the bitmap of its candidates.  Returns what search_batch returns."""
+        return _search_candidates(load_library().bm25x_search_candidates, self.h, q_off, q_terms, c_off, c_docs, k,
+                                  want_f64, want_payload)
+
     def search(self, query, k, allow=None):
         """One query, the shape of bm25::search(&index, k, &query, filter): [(score f64, doc id)] best first."""
         terms = query.terms if isinstance(query, Query) else np.asarray(query, dtype=np.uint32)
@@ -664,6 +690,12 @@ class GrowingSegment:
             *_rows_args(out), C.byref(st)))
         out["stats"] = st
         return out
+
+    def search_candidates(self, q_off, q_terms, c_off, c_docs, k, want_f64=True, want_payload=False):
+        """Index.search_candidates over sealed + growing (bm25x_growing_search_candidates): candidate ids in the result
+        id space, growing ordinal o as sealed.n_docs + o."""
+        return _search_candidates(load_library().bm25x_growing_search_candidates, self.h, q_off, q_terms, c_off, c_docs,
+                                  k, want_f64, want_payload)
 
     def seal(self, sealed_deleted=None, new_keys=None):
         """`maintain` (bm25x_growing_seal): a new sealed Index of the surviving sealed documents (ascending old id) and
@@ -828,6 +860,11 @@ class ShardedIndex:
     def search_batch(self, q_off, q_terms, k, allow=None, want_f64=True, want_payload=False, out=None):
         return _search_batch(load_library().bm25x_sharded_search_batch, self.h, q_off, q_terms, k, allow, want_f64,
                              want_payload, out)
+
+    def search_candidates(self, q_off, q_terms, c_off, c_docs, k, want_f64=True, want_payload=False):
+        """Index.search_candidates with global ids (bm25x_search_candidates_sharded)."""
+        return _search_candidates(load_library().bm25x_search_candidates_sharded, self.h, q_off, q_terms, c_off, c_docs,
+                                  k, want_f64, want_payload)
 
 
 def merge_shards(rows, doc_base, k, device=0):

@@ -169,16 +169,25 @@ struct SealedSide {
     }
 };
 
+// What each list of a sealed-side search selects: prefilter bitmaps (allow_sealed over the side's global ids,
+// allow_growing over the growing handle's ordinals; NULL = all pass), or, when c_off is set, candidate lists
+// (bm25x_search_candidates) in the result id space: sealed ids, then growing ordinal o as n_docs() + o.
+struct SideFilter {
+    const uint8_t *allow_sealed = nullptr, *allow_growing = nullptr;
+    const uint32_t *c_off = nullptr, *c_docs = nullptr;
+};
+
 // The search of a sealed side and, when `growing` is given, a growing handle over ids n_docs() + ordinal (bm25x_shards.cu).
-// One index without a growing handle: bm25x_search_batch.  Otherwise every part's top-k with its slice of allow_sealed
-// (global ids) and the growing handle's with allow_growing (its ordinals), merged on the device.  A sharded side first
-// makes bm25x_search_batch's request checks and canonicalises the queries against the whole segment, so that its
-// refusals are those of the unsharded index.  stats->queries = the live queries of the whole sealed segment, plus the
-// growing handle's when count_growing; h2d_ms is counted from t0.  CUDA failures are named by `who`.
-int sealed_side_search(const char *who, const SealedSide &sealed, bm25x_index *growing, const uint8_t *allow_sealed,
-                       const uint8_t *allow_growing, bool count_growing, uint32_t nq, const uint32_t *q_off,
-                       const uint32_t *q_terms, uint32_t k, const ResultRows &host, bm25x_search_stats *stats,
-                       std::chrono::steady_clock::time_point t0);
+// One index without a growing handle: bm25x_search_batch, or bm25x_search_candidates.  Otherwise every part's top-k and
+// the growing handle's, merged on the device: with its slice of allow_sealed / with allow_growing, or with the candidates
+// that fall in its id range, as local ids.  A sharded side first makes bm25x_search_batch's request checks and
+// canonicalises the queries against the whole segment, so that its refusals are those of the unsharded index; candidates
+// at or past the last id of the side and the growing handle are refused next.  stats->queries = the live queries of the
+// whole sealed segment, plus the growing handle's when count_growing; h2d_ms is counted from t0.  CUDA failures and the
+// candidates' refusals are named by `who`.
+int sealed_side_search(const char *who, const SealedSide &sealed, bm25x_index *growing, const SideFilter &f,
+                       bool count_growing, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms, uint32_t k,
+                       const ResultRows &host, bm25x_search_stats *stats, std::chrono::steady_clock::time_point t0);
 
 // The container of a document-sharded build, for both sources:after the host checks of the segment c (P postings, df, the
 // statistics st), every shard's device is checked with who's message; then prepare(device of shard 0, cum) runs the

@@ -211,13 +211,32 @@ struct ResultRows {
     }
 };
 
-// A prepared batch (bm25x_batch_prepare) seen from the sharded search: its output rows; a run on its index's stream between
-// the batch's timing events, without synchronising; the event that closes that run; after it has finished, its figures
-// added to *acc.
-const ResultRows &bm25x_batch_rows(const bm25x_batch *b);
-int bm25x_batch_run_timed(bm25x_batch *b);
-cudaEvent_t bm25x_batch_done_event(bm25x_batch *b);
-int bm25x_batch_add_stats(bm25x_batch *b, bm25x_search_stats *acc);
+// One list of a device merge (bm25x_merged_search): a search of one handle, enqueued on the handle's library stream between
+// timing events, without synchronising.  rows(): its device rows; done(): the event that closes its run; add_stats(): once
+// that has passed, its figures added to *acc.  Destroying it frees the search.  Both batch kinds are lists: the bitmap
+// search (bm25x_batch_list, bm25x_search.cu) and the candidate search (cand_list, bm25x_candidates.cu).
+struct ListRun {
+    virtual ~ListRun() {}
+    virtual const ResultRows &rows() const = 0;
+    virtual cudaEvent_t done() const = 0;
+    virtual int add_stats(bm25x_search_stats *acc) = 0;
+};
+// bm25x_batch_prepare of the queries on ix with the prefilter allow, then its timed run enqueued.
+int bm25x_batch_list(bm25x_index *ix, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms, uint32_t k,
+                     const uint8_t *allow, std::unique_ptr<ListRun> *out);
+// The candidate search of the queries on ix (query i's candidates: local ids c_docs[c_off[i]..c_off[i+1]), < its n_docs),
+// prepared as bm25x_search_candidates prepares it, then its timed run enqueued.  The refusals of bm25x_search_candidates.
+int cand_list(const char *who, bm25x_index *ix, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms,
+              const uint32_t *c_off, const uint32_t *c_docs, uint32_t k, std::unique_ptr<ListRun> *out);
+// The refusals of the candidate lists (bm25x_candidates.cu), named by who: c_off going backwards anywhere (checked over
+// all offsets before any entry is read), a null c_docs with entries, then a candidate >= n_ids.
+int check_candidates(const char *who, uint32_t nq, const uint32_t *c_off, const uint32_t *c_docs, uint64_t n_ids);
+
+// ix's page-locked staging buffer (bm25x_batch_prepare's, shared by the uploads of the handle) with room for `words`
+// u32, once the upload that last read it has finished; the caller holds ix->stage_mutex.  stage_upload: one copy of its
+// first `words` to d on ix->stream, recorded as the buffer's last reader.  stage_reserve refuses as `who`'s.
+int stage_reserve(bm25x_index *ix, const char *who, size_t words, uint32_t **out);
+cudaError_t stage_upload(bm25x_index *ix, void *d, size_t words);
 
 // The request checks of the searches and merges, with bm25x_search_batch's messages (bm25x_search.cu).  check_queries:
 // q_off when nq > 0, q_terms unless every query is empty.  check_k: k == 0, the reference's refusal

@@ -59,6 +59,10 @@ struct SearchParams {
     uint32_t *out_n;
 };
 
+// The fields of the search parameters that depend on the index handle alone: its device arrays and options
+// (bm25x_search.cu).
+SearchParams index_params(const bm25x_index *ix);
+
 namespace {
 
 constexpr uint32_t INF = BM25X_DOC_INF;
@@ -161,6 +165,40 @@ __device__ __forceinline__ void wpool_sort(const WPool<C> &pl, int n, int lane) 
             __syncwarp();
         }
     }
+}
+
+// ---- probes of one document in one term's list, without streaming it: the search kernel's probes of a term that is not
+// streamed any more (replaces Cursor::seek_block / seek of the reference's parked cursors, search.rs:412-466) and the
+// lookups of the candidate search (bm25x_candidates.cu): block table first (SummaryTuple.{min,max}_document_id), then inside
+// the 128-posting block.  `steps` counts the table entries / postings read (pruning statistics).
+// Returns l = 1 + index of the last block whose first document is <= doc (0: doc lies before the first block).
+__device__ __forceinline__ uint32_t probe_block(const SearchParams &p, uint64_t bbase, uint32_t nb, uint32_t doc,
+                                                uint32_t &steps) {
+    uint32_t l = 0, r = nb;
+    while (l < r) {
+        const uint32_t mid = (l + r) >> 1;
+        if (__ldg(&p.blk[bbase + mid].x) <= doc) l = mid + 1;
+        else r = mid;
+        steps++;
+    }
+    return l;
+}
+__device__ __forceinline__ uint32_t probe_in_block(const SearchParams &p, uint64_t pbase, uint32_t dfj, uint32_t block,
+                                                   uint32_t doc, uint32_t &steps) {
+    const uint32_t s = block * BM25X_BLOCK, e = min(s + BM25X_BLOCK, dfj);
+    const Posting *pp = p.post + pbase;
+    uint32_t l = s, r = e;
+    while (l < r) {
+        const uint32_t mid = (l + r) >> 1;
+        if (__ldg(&pp[mid].doc) < doc) l = mid + 1;
+        else r = mid;
+        steps++;
+    }
+    if (l < e) {
+        const Posting v = pp[l];
+        if (v.doc == doc) return v.w;
+    }
+    return 0u;
 }
 
 struct WFilter {

@@ -506,8 +506,38 @@ extern "C" int bm25x_growing_search_batch(bm25x_growing_segment *g, uint32_t nq,
         std::copy(allow_growing, allow_growing + ((size_t)n + 7) / 8, ag.begin());
         if (n & 7u) ag[n >> 3] &= (uint8_t)((1u << (n & 7u)) - 1u);
     }
-    return sealed_side_search("bm25x_growing_search_batch", g->sealed, cur.get(), allow_sealed,
-                              cur && allow_growing ? ag.data() : nullptr, true, nq, q_off, q_terms, k,
+    SideFilter f;
+    f.allow_sealed = allow_sealed;
+    f.allow_growing = cur && allow_growing ? ag.data() : nullptr;
+    return sealed_side_search("bm25x_growing_search_batch", g->sealed, cur.get(), f, true, nq, q_off, q_terms, k,
+                              {out_doc, out_score, out_score64, out_payload, out_n}, stats, t0);
+}
+
+extern "C" int bm25x_growing_search_candidates(bm25x_growing_segment *g, uint32_t nq, const uint32_t *q_off,
+                                               const uint32_t *q_terms, const uint32_t *c_off, const uint32_t *c_docs,
+                                               uint32_t k, uint32_t *out_doc, float *out_score, double *out_score64,
+                                               uint16_t *out_payload, uint32_t *out_n, bm25x_search_stats *stats) {
+    const char *who = "bm25x_growing_search_candidates";
+    if (!g || (nq && (!c_off || (!c_docs && c_off[nq] != 0)))) {
+        bm25x_set_error("%s: null argument", who);
+        return BM25X_ERR_INVALID;
+    }
+    if (const int rc = check_k(k, false); rc != BM25X_OK) return rc;  // before the refresh: a refused call leaves it pending
+    const auto t0 = std::chrono::steady_clock::now();
+    std::shared_ptr<bm25x_index> cur;
+    {
+        std::lock_guard<std::mutex> lock(g->mu);
+        const int rc = growing_refresh_locked(g);
+        if (rc != BM25X_OK) return rc;
+        cur = g->cur;
+    }
+    // before the first insert the sealed side alone answers: its ids are the only ones
+    if (!cur)
+        if (const int rc = check_candidates(who, nq, c_off, c_docs, g->sealed.n_docs()); rc != BM25X_OK) return rc;
+    SideFilter f;
+    f.c_off = c_off;
+    f.c_docs = c_docs;
+    return sealed_side_search(who, g->sealed, cur.get(), f, true, nq, q_off, q_terms, k,
                               {out_doc, out_score, out_score64, out_payload, out_n}, stats, t0);
 }
 

@@ -225,6 +225,38 @@ int check_k(uint32_t k, bool max_k) {
     return BM25X_OK;
 }
 
+int stage_reserve(bm25x_index *ix, const char *who, size_t words, uint32_t **out) {
+    if (ix->h_stage_words < words) {
+        if (ix->h_stage) {
+            cudaStreamSynchronize(ix->stream);  // an earlier batch's upload may still read it
+            cudaFreeHost(ix->h_stage);
+        }
+        ix->h_stage = nullptr;
+        ix->h_stage_words = 0;
+        const size_t cap = words + words / 4 + 1024;
+        const cudaError_t e = cudaMallocHost((void **)&ix->h_stage, cap * sizeof(uint32_t));
+        if (e != cudaSuccess) {
+            bm25x_set_error("%s: page-locked staging buffer: %s", who, cudaGetErrorString(e));
+            return BM25X_ERR_OOM;
+        }
+        ix->h_stage_words = cap;
+    } else if (ix->h_stage_busy) {
+        cudaEventSynchronize(ix->h_stage_free);  // the previous upload from this buffer has been issued; wait for it
+    }
+    *out = ix->h_stage;
+    return BM25X_OK;
+}
+
+cudaError_t stage_upload(bm25x_index *ix, void *d, size_t words) {
+    cudaError_t e = cudaMemcpyAsync(d, ix->h_stage, words * sizeof(uint32_t), cudaMemcpyHostToDevice, ix->stream);
+    if (e == cudaSuccess) {
+        if (!ix->h_stage_free) e = cudaEventCreateWithFlags(&ix->h_stage_free, cudaEventDisableTiming);
+        if (e == cudaSuccess) e = cudaEventRecord(ix->h_stage_free, ix->stream);
+        ix->h_stage_busy = true;
+    }
+    return e;
+}
+
 // Canonicalises the queries (bm25x_canonicalise), groups them by term-count class and uploads everything with ONE copy
 // from a page-locked staging buffer cached in the index handle.
 extern "C" int bm25x_batch_prepare(bm25x_index *ix, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms,
@@ -325,25 +357,11 @@ extern "C" int bm25x_batch_prepare(bm25x_index *ix, uint32_t nq, const uint32_t 
     }
     cudaStream_t st = ix->stream;
     std::lock_guard<std::mutex> stage_lock(ix->stage_mutex);  // the staging buffer is shared by the batches of this index
-    if (ix->h_stage_words < words) {
-        if (ix->h_stage) {
-            cudaStreamSynchronize(st);  // an earlier batch's upload may still read it
-            cudaFreeHost(ix->h_stage);
-        }
-        ix->h_stage = nullptr;
-        ix->h_stage_words = 0;
-        const size_t cap = words + words / 4 + 1024;
-        e = cudaMallocHost((void **)&ix->h_stage, cap * sizeof(uint32_t));
-        if (e != cudaSuccess) {
-            bm25x_set_error("bm25x_batch_prepare: page-locked staging buffer: %s", cudaGetErrorString(e));
-            delete b;
-            return BM25X_ERR_OOM;
-        }
-        ix->h_stage_words = cap;
-    } else if (ix->h_stage_busy) {
-        cudaEventSynchronize(ix->h_stage_free);  // the previous upload from this buffer has been issued; wait for it
+    uint32_t *hs = nullptr;
+    if (const int rc = stage_reserve(ix, "bm25x_batch_prepare", words, &hs); rc != BM25X_OK) {
+        delete b;
+        return rc;
     }
-    uint32_t *hs = ix->h_stage;
     for (int c = 0; c < kNumClasses; ++c) {
         hs[base_off[c]] = 0;
         hs[base_cnt[c]] = 0;
@@ -367,12 +385,7 @@ extern "C" int bm25x_batch_prepare(bm25x_index *ix, uint32_t nq, const uint32_t 
     b->postings = postings;
     uint32_t *d_q = nullptr;
     BTRY(batch_alloc(b, &d_q, words));
-    e = cudaMemcpyAsync(d_q, hs, words * sizeof(uint32_t), cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) {
-        if (!ix->h_stage_free) e = cudaEventCreateWithFlags(&ix->h_stage_free, cudaEventDisableTiming);
-        if (e == cudaSuccess) e = cudaEventRecord(ix->h_stage_free, st);
-        ix->h_stage_busy = true;
-    }
+    e = stage_upload(ix, d_q, words);
     for (int c = 0; c < kNumClasses; ++c) {
         Group &g = b->groups[c];
         g.d_ids = d_q + base_ids[c];
@@ -409,7 +422,7 @@ extern "C" int bm25x_batch_prepare(bm25x_index *ix, uint32_t nq, const uint32_t 
 }
 
 // The fields of the search kernels' parameters that depend on the index handle alone: its device arrays and options.
-static SearchParams index_params(const bm25x_index *ix) {
+SearchParams index_params(const bm25x_index *ix) {
     const DeviceIndex &d = ix->d;
     SearchParams sp;
     sp.post = d.post;
@@ -495,6 +508,8 @@ static int batch_enqueue(bm25x_batch *b, cudaStream_t st, bool timed) {
     return BM25X_OK;
 }
 
+static int bm25x_batch_add_stats(bm25x_batch *b, bm25x_search_stats *acc);
+
 extern "C" int bm25x_batch_run(bm25x_batch *b, void *stream_v, bm25x_search_stats *stats) {
     if (!b) {
         bm25x_set_error("bm25x_batch_run: null batch");
@@ -534,16 +549,27 @@ extern "C" int bm25x_batch_device_results(bm25x_batch *b, void **doc, void **sco
     return BM25X_OK;
 }
 
-const ResultRows &bm25x_batch_rows(const bm25x_batch *b) { return b->out; }
+// A batch as one list of a device merge (bm25x_merged_search).
+struct BatchList final : ListRun {
+    bm25x_batch *b;
+    explicit BatchList(bm25x_batch *b_) : b(b_) {}
+    ~BatchList() override { bm25x_batch_destroy(b); }
+    const ResultRows &rows() const override { return b->out; }
+    cudaEvent_t done() const override { return b->ev1; }
+    int add_stats(bm25x_search_stats *acc) override { return bm25x_batch_add_stats(b, acc); }
+};
 
-// An asynchronous timed run on the index's stream (the slices of search_batch_sliced, the shards of
-// bm25x_sharded_search_batch); bm25x_batch_add_stats reads its figures once it has finished.
-int bm25x_batch_run_timed(bm25x_batch *b) { return batch_enqueue(b, b->ix->stream, true); }
-
-cudaEvent_t bm25x_batch_done_event(bm25x_batch *b) { return b->ev1; }
+int bm25x_batch_list(bm25x_index *ix, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms, uint32_t k,
+                     const uint8_t *allow, std::unique_ptr<ListRun> *out) {
+    bm25x_batch *b = nullptr;
+    const int rc = bm25x_batch_prepare(ix, nq, q_off, q_terms, k, allow, &b);
+    if (rc != BM25X_OK) return rc;
+    out->reset(new BatchList(b));
+    return batch_enqueue(b, ix->stream, true);
+}
 
 // The figures of the batch's last timed run, added to *acc (bm25x_batch_run fills a zeroed one).
-int bm25x_batch_add_stats(bm25x_batch *b, bm25x_search_stats *acc) {
+static int bm25x_batch_add_stats(bm25x_batch *b, bm25x_search_stats *acc) {
     BM25X_CUDA_TRY(cudaSetDevice(b->ix->device));
     float ms = 0.f;
     unsigned long long fetched = 0;
@@ -713,8 +739,11 @@ extern "C" int bm25x_search_batch_growing(bm25x_index *sealed, bm25x_index *grow
     // stats->queries is the sealed search's: a growing live query is a sealed one.
     SealedSide side;
     side.ix = sealed;
-    return sealed_side_search("bm25x_search_batch_growing", side, growing, allow_sealed, allow_growing, false, nq, q_off,
-                              q_terms, k, {out_doc, out_score, out_score64, out_payload, out_n}, stats,
+    SideFilter f;
+    f.allow_sealed = allow_sealed;
+    f.allow_growing = allow_growing;
+    return sealed_side_search("bm25x_search_batch_growing", side, growing, f, false, nq, q_off, q_terms, k,
+                              {out_doc, out_score, out_score64, out_payload, out_n}, stats,
                               std::chrono::steady_clock::now());
 }
 

@@ -296,39 +296,6 @@ __device__ __forceinline__ uint32_t ring_find_pos(const typename C::RT *rg, uint
     return (l < e && ring_doc(rg, l & mask) == doc) ? l : INF;
 }
 
-// ---- probes of a term that is not streamed any more (candidates only; replaces Cursor::seek_block / seek of the
-// reference's parked cursors, search.rs:412-466): block table first (SummaryTuple.{min,max}_document_id), then inside
-// the 128-posting block.  `steps` counts the table entries / postings read (pruning statistics).
-// Returns l = 1 + index of the last block whose first document is <= doc (0: doc lies before the first block).
-__device__ __forceinline__ uint32_t probe_block(const SearchParams &p, uint64_t bbase, uint32_t nb, uint32_t doc,
-                                                uint32_t &steps) {
-    uint32_t l = 0, r = nb;
-    while (l < r) {
-        const uint32_t mid = (l + r) >> 1;
-        if (__ldg(&p.blk[bbase + mid].x) <= doc) l = mid + 1;
-        else r = mid;
-        steps++;
-    }
-    return l;
-}
-__device__ __forceinline__ uint32_t probe_in_block(const SearchParams &p, uint64_t pbase, uint32_t dfj, uint32_t block,
-                                                   uint32_t doc, uint32_t &steps) {
-    const uint32_t s = block * BM25X_BLOCK, e = min(s + BM25X_BLOCK, dfj);
-    const Posting *pp = p.post + pbase;
-    uint32_t l = s, r = e;
-    while (l < r) {
-        const uint32_t mid = (l + r) >> 1;
-        if (__ldg(&pp[mid].doc) < doc) l = mid + 1;
-        else r = mid;
-        steps++;
-    }
-    if (l < e) {
-        const Posting v = pp[l];
-        if (v.doc == doc) return v.w;
-    }
-    return 0u;
-}
-
 template <class C>
 __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_constant__ SearchParams p) {
     extern __shared__ __align__(128) uint8_t smem[];

@@ -7,6 +7,7 @@
 
 #include <algorithm>
 #include <chrono>
+#include <functional>
 #include <vector>
 
 #include "bm25x_build.h"
@@ -142,16 +143,15 @@ int merge_step(const char *who, int device, const ShardRows &in, uint32_t S, uin
 }
 
 // The rows of S handles over consecutive doc ranges (list s: ids + base[s], base ascending) merged into one top-k list:
-// every handle's batch is prepared with its own allow[s] (NULL = all pass) and run on its own library stream (the next
-// one's canonicalisation overlaps the kernels of the previous), the merge stream (handle 0's) waits for each run's done
-// event, then the merge step.  Rows of handles on other devices are copied peer to peer first.  More than
-// BM25X_MAX_LISTS handles are refused.  Refusals of bm25x_batch_prepare, CUDA failures named by `who`.  stats: sums over
-// the handles plus the merge launch; h2d_ms = from t0 to the last run enqueued, d2h_ms = merge wait + download;
-// live[s] = handle s's live queries.
+// make(s, &list) prepares handle s's search and enqueues its timed run on the handle's library stream (the next one's
+// preparation overlaps the kernels of the previous), the merge stream (handle 0's) waits for each list's done event, then
+// the merge step.  Rows of handles on other devices are copied peer to peer first.  More than BM25X_MAX_LISTS handles
+// are refused.  Refusals of make, CUDA failures named by `who`.  stats: sums over the lists plus the merge launch;
+// h2d_ms = from t0 to the last run enqueued, d2h_ms = merge wait + download; live[s] = list s's live queries.
 int bm25x_merged_search(const char *who, uint32_t S, bm25x_index *const *handles, const uint32_t *base,
-                        const uint8_t *const *allow, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms,
-                        uint32_t k, const ResultRows &host, bm25x_search_stats *stats,
-                        std::chrono::steady_clock::time_point t0, uint32_t *live) {
+                        const std::function<int(uint32_t, std::unique_ptr<ListRun> *)> &make, uint32_t nq, uint32_t k,
+                        const ResultRows &host, bm25x_search_stats *stats, std::chrono::steady_clock::time_point t0,
+                        uint32_t *live) {
     using clk = std::chrono::steady_clock;
     if (S == 0 || S > BM25X_MAX_LISTS) {
         bm25x_set_error("%s: %u lists to merge, must be 1..%d", who, S, BM25X_MAX_LISTS);
@@ -160,21 +160,17 @@ int bm25x_merged_search(const char *who, uint32_t S, bm25x_index *const *handles
     bm25x_index *ix0 = handles[0];
     const int dev0 = ix0->device;
     cudaStream_t ms = ix0->stream;  // the merge runs behind handle 0's kernels on its library stream
-    std::vector<bm25x_batch *> bs(S, nullptr);
+    std::vector<std::unique_ptr<ListRun>> lists(S);
     std::vector<ResultRows> peer(S);  // rows of handles on other devices, copied to dev0
     auto cleanup = [&](int code) {
         cudaSetDevice(dev0);
         cudaStreamSynchronize(ms);
         for (ResultRows &p : peer) p.release(ms);
-        for (bm25x_batch *b : bs)
-            if (b) bm25x_batch_destroy(b);
+        lists.clear();
         return code;
     };
     int rc = BM25X_OK;
-    for (uint32_t s = 0; s < S && rc == BM25X_OK; s++) {
-        rc = bm25x_batch_prepare(handles[s], nq, q_off, q_terms, k, allow[s], &bs[s]);
-        if (rc == BM25X_OK) rc = bm25x_batch_run_timed(bs[s]);
-    }
+    for (uint32_t s = 0; s < S && rc == BM25X_OK; s++) rc = make(s, &lists[s]);
     if (rc != BM25X_OK) return cleanup(rc);
     const auto t1 = clk::now();
     // ---- every handle's rows on dev0: read in place there, copied peer to peer from the other devices ----
@@ -182,8 +178,8 @@ int bm25x_merged_search(const char *who, uint32_t S, bm25x_index *const *handles
     memset(&in, 0, sizeof(in));
     cudaError_t e = cudaSetDevice(dev0);
     for (uint32_t s = 0; s < S && e == cudaSuccess; s++) {
-        e = cudaStreamWaitEvent(ms, bm25x_batch_done_event(bs[s]), 0);
-        const ResultRows *rows = &bm25x_batch_rows(bs[s]);
+        e = cudaStreamWaitEvent(ms, lists[s]->done(), 0);
+        const ResultRows *rows = &lists[s]->rows();
         if (e == cudaSuccess && handles[s]->device != dev0) {
             e = peer[s].alloc(nq, k, ms);
             if (e == cudaSuccess) e = rows->copy_to(peer[s], nq, k, ms);
@@ -201,7 +197,7 @@ int bm25x_merged_search(const char *who, uint32_t S, bm25x_index *const *handles
         memset(stats, 0, sizeof(*stats));
         for (uint32_t s = 0; s < S && rc == BM25X_OK; s++) {
             const uint32_t q0 = stats->queries;
-            rc = bm25x_batch_add_stats(bs[s], stats);
+            rc = lists[s]->add_stats(stats);
             live[s] = stats->queries - q0;
         }
         stats->kernel_ms += mms;  // summed device time of the handles' kernels and the merge, not wall time
@@ -212,16 +208,41 @@ int bm25x_merged_search(const char *who, uint32_t S, bm25x_index *const *handles
     return cleanup(rc);
 }
 
+// Candidate lists in the id space of consecutive ranges starting at first[0] = 0 < first[1] < ... < first[L] (the total),
+// cut into L candidate CSRs of local ids: list l takes query i's candidates in [first[l], first[l + 1]) as id - first[l],
+// in their order.  The offsets of the CSRs start at 0.
+struct RoutedCandidates {
+    std::vector<std::vector<uint32_t>> off, docs;
+};
+RoutedCandidates route_candidates(uint32_t nq, const uint32_t *c_off, const uint32_t *c_docs,
+                                  const std::vector<uint32_t> &first) {
+    const uint32_t L = (uint32_t)first.size() - 1;
+    RoutedCandidates r;
+    r.off.assign(L, std::vector<uint32_t>(nq + 1, 0));
+    r.docs.assign(L, {});
+    for (uint32_t i = 0; i < nq; i++) {
+        for (uint32_t j = c_off[i]; j < c_off[i + 1]; j++) {
+            const uint32_t d = c_docs[j];
+            const uint32_t l = (uint32_t)(std::upper_bound(first.begin() + 1, first.end() - 1, d) - (first.begin() + 1));
+            r.docs[l].push_back(d - first[l]);
+        }
+        for (uint32_t l = 0; l < L; l++) r.off[l][i + 1] = (uint32_t)r.docs[l].size();
+    }
+    return r;
+}
+
 }  // namespace
 
-int sealed_side_search(const char *who, const SealedSide &sealed, bm25x_index *growing, const uint8_t *allow_sealed,
-                       const uint8_t *allow_growing, bool count_growing, uint32_t nq, const uint32_t *q_off,
-                       const uint32_t *q_terms, uint32_t k, const ResultRows &host, bm25x_search_stats *stats,
-                       std::chrono::steady_clock::time_point t0) {
+int sealed_side_search(const char *who, const SealedSide &sealed, bm25x_index *growing, const SideFilter &f,
+                       bool count_growing, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms, uint32_t k,
+                       const ResultRows &host, bm25x_search_stats *stats, std::chrono::steady_clock::time_point t0) {
     const bm25x_sharded_index *sx = sealed.sx;
+    const bool cand = f.c_off != nullptr;
     if (!sx && !growing)
-        return bm25x_search_batch(sealed.ix, nq, q_off, q_terms, k, allow_sealed, host.doc, host.score, host.score64,
-                                  host.payload, host.n, stats);
+        return cand ? bm25x_search_candidates(sealed.ix, nq, q_off, q_terms, f.c_off, f.c_docs, k, host.doc, host.score,
+                                              host.score64, host.payload, host.n, stats)
+                    : bm25x_search_batch(sealed.ix, nq, q_off, q_terms, k, f.allow_sealed, host.doc, host.score,
+                                         host.score64, host.payload, host.n, stats);
     // ---- a sharded side: the refusals of bm25x_search_batch, its request checks, then its canonicalisation slice by
     // slice against the WHOLE segment's df (a query with 65 live terms is refused even when no shard sees more than 64) ----
     uint32_t n_live = 0;  // live queries of the whole sharded segment
@@ -242,23 +263,35 @@ int sealed_side_search(const char *who, const SealedSide &sealed, bm25x_index *g
     const uint32_t S = (uint32_t)parts.size();
     std::vector<bm25x_index *> hs;
     std::vector<uint32_t> base;
-    std::vector<const uint8_t *> allow;
-    std::vector<std::vector<uint8_t>> slices(S);  // allow_sealed cut at a sharded side's bounds
-    for (uint32_t s = 0; s < S; s++) {
-        const SealPart &p = parts[s];
-        if (sx && allow_sealed) slices[s] = allow_slice(allow_sealed, sx->n_docs, p.first, p.first + p.n);
+    for (const SealPart &p : parts) {
         hs.push_back(p.h);
         base.push_back(p.first);
-        allow.push_back(sx && allow_sealed ? slices[s].data() : allow_sealed);
     }
     if (growing) {
         hs.push_back(growing);
         base.push_back(sealed.n_docs());
-        allow.push_back(allow_growing);
     }
-    std::vector<uint32_t> live(hs.size(), 0);
-    const int rc = bm25x_merged_search(who, (uint32_t)hs.size(), hs.data(), base.data(), allow.data(), nq, q_off, q_terms,
-                                       k, host, stats, t0, live.data());
+    const uint32_t L = (uint32_t)hs.size();
+    std::vector<uint32_t> first(base);
+    first.push_back(sealed.n_docs() + (growing ? growing->d.n_docs : 0u));
+    if (cand) {
+        if (const int rc = check_candidates(who, nq, f.c_off, f.c_docs, first[L]); rc != BM25X_OK) return rc;
+    }
+    // bitmap search: allow_sealed cut at a sharded side's bounds; candidate search: the candidates routed to their lists
+    std::vector<std::vector<uint8_t>> slices(S);
+    const RoutedCandidates rc_lists = cand ? route_candidates(nq, f.c_off, f.c_docs, first) : RoutedCandidates();
+    auto make = [&](uint32_t s, std::unique_ptr<ListRun> *out) -> int {
+        if (cand)
+            return cand_list(who, hs[s], nq, q_off, q_terms, rc_lists.off[s].data(), rc_lists.docs[s].data(), k, out);
+        const uint8_t *allow = s < S ? f.allow_sealed : f.allow_growing;
+        if (s < S && sx && f.allow_sealed) {
+            slices[s] = allow_slice(f.allow_sealed, sx->n_docs, parts[s].first, parts[s].first + parts[s].n);
+            allow = slices[s].data();
+        }
+        return bm25x_batch_list(hs[s], nq, q_off, q_terms, k, allow, out);
+    };
+    std::vector<uint32_t> live(L, 0);
+    const int rc = bm25x_merged_search(who, L, hs.data(), base.data(), make, nq, k, host, stats, t0, live.data());
     if (rc == BM25X_OK && stats) stats->queries = (sx ? n_live : live[0]) + (growing && count_growing ? live[S] : 0u);
     return rc;
 }
@@ -273,7 +306,27 @@ extern "C" int bm25x_sharded_search_batch(bm25x_sharded_index *sx, uint32_t nq, 
     }
     SealedSide side;
     side.sx = sx;
-    return sealed_side_search("bm25x_sharded_search_batch", side, nullptr, allow, nullptr, false, nq, q_off, q_terms, k,
+    SideFilter f;
+    f.allow_sealed = allow;
+    return sealed_side_search("bm25x_sharded_search_batch", side, nullptr, f, false, nq, q_off, q_terms, k,
+                              {out_doc, out_score, out_score64, out_payload, out_n}, stats,
+                              std::chrono::steady_clock::now());
+}
+
+extern "C" int bm25x_search_candidates_sharded(bm25x_sharded_index *sx, uint32_t nq, const uint32_t *q_off,
+                                               const uint32_t *q_terms, const uint32_t *c_off, const uint32_t *c_docs,
+                                               uint32_t k, uint32_t *out_doc, float *out_score, double *out_score64,
+                                               uint16_t *out_payload, uint32_t *out_n, bm25x_search_stats *stats) {
+    if (!sx || (nq && (!c_off || (!c_docs && c_off[nq] != 0)))) {
+        bm25x_set_error("bm25x_search_candidates_sharded: null argument");
+        return BM25X_ERR_INVALID;
+    }
+    SealedSide side;
+    side.sx = sx;
+    SideFilter f;
+    f.c_off = c_off;
+    f.c_docs = c_docs;
+    return sealed_side_search("bm25x_search_candidates_sharded", side, nullptr, f, false, nq, q_off, q_terms, k,
                               {out_doc, out_score, out_score64, out_payload, out_n}, stats,
                               std::chrono::steady_clock::now());
 }

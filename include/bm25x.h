@@ -118,6 +118,38 @@ typedef struct {
 } bm25x_blocks;
 int bm25x_index_create_from_blocks(const bm25x_blocks *blocks, int device, bm25x_index **out);
 
+/* ---- the sealed segment from its DOCUMENTS: CREATE INDEX below the heap scan (ambuild → io::write → readers → build,
+ * src/index/bm25/am/am_build.rs:312-313, crates/bm25/src/io.rs:187-244), the inversion run on the GPU.  Documents are
+ * doc-major, in heap-scan order (doc id = position); each is a bm25vector Document: elements strictly ascending by key,
+ * tf != 0 (vector.rs:38-83).  Exactly one of elem_key / elem_term is given.
+ * The handle equals, array for array, the one bm25x_index_create builds from the reference's Segment of the same
+ * documents: records in input order, doc_len[d] = the saturating Σ tf of document d (Document::length), postings sorted
+ * by (key, doc); keyed: term_key = the distinct keys ascending bytewise (bm25x_lookup_terms, the export's term_key and the
+ * seal's new_keys work on it); keyless: n_terms as given (ordinals without postings keep df 0) and no keys.
+ * Refusals, every host one before any device is used (*out = NULL, no device memory left behind), named
+ * bm25x_index_create_from_documents: BM25X_ERR_INVALID for a null argument, both or neither of elem_key / elem_term,
+ * n_terms != 0 with keys, n_docs 0 or 0xFFFFFFFF, k1 / b out of range, elem_off[0] != 0, and naming the first offending
+ * document: elem_off going backwards, keys or ordinals not strictly ascending inside a document, an ordinal >= n_terms
+ * (BM25X_TERM_MISSING included), tf == 0; BM25X_ERR_UNSUPPORTED for tf >= 2^24.  Then the device check, and on the device,
+ * before the index is allocated, more than 0xFFFFFFFE distinct keys (BM25X_ERR_UNSUPPORTED); BM25X_ERR_OOM /
+ * BM25X_ERR_CUDA from the build steps.
+ * The device works in chunks of 2^22 elements (DESIGN §4.9).  Device memory beyond the index: 12 B per term (per-term
+ * cursors), per chunk 128 MiB keyless or 192 MiB keyed, CUB's temporary storage for one chunk's sort, and for a keyed
+ * build the vocabulary: 16 B per distinct key while the postings are written; the
+ * vocabulary pass before it holds up to 80 B per distinct key plus 80 B per element of one chunk (a list of (key, count)
+ * with room to double, and the sort's second buffer). */
+typedef struct {
+    uint32_t n_docs;            /* records, in heap-scan order: doc id = position (io.rs:193, readers) */
+    const uint64_t *elem_off;   /* [n_docs+1], elem_off[0] == 0, non-decreasing; E = elem_off[n_docs] may exceed 2^32 */
+    const uint8_t *elem_key;    /* [E*16] Element.key, strictly ascending (bytewise) inside a document: keyed build; or NULL */
+    const uint32_t *elem_term;  /* [E] term ordinal < n_terms, strictly ascending inside a document: keyless build; or NULL */
+    const uint32_t *elem_tf;    /* [E] Element.value, != 0 */
+    const uint16_t *payload;    /* [n_docs*3] Record payload (ctid), or NULL: the synthetic ctid, as bm25x_index_create */
+    uint32_t n_terms;           /* keyless: the vocabulary size (ordinals without postings keep df 0); keyed: must be 0 */
+    double k1, b;
+} bm25x_documents;
+int bm25x_index_create_from_documents(const bm25x_documents *docs, int device, bm25x_index **out);
+
 /* ---- the inverse: a finalized index written out as the reference's stored segment, i.e. everything flush() writes for
  * it (flush.rs:40-158) but the pages, tapes and address trees, which stay the caller's.  Encoded on the index's device:
  * per token, blocks of 128 postings in doc order, the last one shorter (flush.rs:78-90; the index's own blocks); payloads
@@ -450,6 +482,16 @@ int bm25x_sharded_create(const bm25x_corpus *whole, uint32_t n_shards, const uin
  * bm25x_sharded_index. */
 int bm25x_index_create_sharded_from_blocks(const bm25x_blocks *blocks, uint32_t n_shards, const uint32_t *doc_bounds,
                                            const int *devices, bm25x_sharded_index **out);
+/* The same document-sharded index, built from the documents (`docs` exactly as for bm25x_index_create_from_documents):
+ * equal to bm25x_sharded_create on that call's CSR with the same n_shards / doc_bounds / devices.  With doc_bounds == NULL
+ * the bounds are its balanced ones with c_d = the elements of document d (cum[d] = elem_off[d]).  Keyed: the vocabulary
+ * pass runs on devices[0] over every element, and the keys go with shard 0.  Then every shard's device counts its own df
+ * over its element range (the host sums them into the segment's df and statistics), and each shard inverts only
+ * [elem_off[lo], elem_off[hi]) with local doc ids.  Refusals: those of bm25x_index_create_from_documents (its codes and
+ * messages), then the shard arguments and devices with bm25x_sharded_create's messages, all before any device is used.
+ * Device memory per device beyond its shards: as bm25x_index_create_from_documents, for its own shards' documents. */
+int bm25x_index_create_sharded_from_documents(const bm25x_documents *docs, uint32_t n_shards, const uint32_t *doc_bounds,
+                                              const int *devices, bm25x_sharded_index **out);
 void bm25x_sharded_destroy(bm25x_sharded_index *sx);
 /* info as the unsharded index would report it (n_docs, n_terms, n_postings, sum_doc_len, avgdl, k1, b); device_bytes
  * and n_blocks summed over the shards; device = shard 0's.  doc_bounds_out[n_shards+1] or NULL. */

@@ -40,6 +40,12 @@ class _Blocks(C.Structure):
                 ("blk_wand_fieldnorm", C.POINTER(C.c_uint8)), ("blk_wand_tf", C.POINTER(C.c_uint32))]
 
 
+class _Documents(C.Structure):  # bm25x_documents
+    _fields_ = [("n_docs", C.c_uint32), ("elem_off", C.POINTER(C.c_uint64)), ("elem_key", C.POINTER(C.c_uint8)),
+                ("elem_term", C.POINTER(C.c_uint32)), ("elem_tf", C.POINTER(C.c_uint32)), ("payload", C.POINTER(C.c_uint16)),
+                ("n_terms", C.c_uint32), ("k1", C.c_double), ("b", C.c_double)]
+
+
 class Export(C.Structure):  # bm25x_export
     _fields_ = [("doc_fieldnorm", C.POINTER(C.c_uint8)), ("payload", C.POINTER(C.c_uint16)), ("sum_doc_len", C.c_uint64),
                 ("term_key", C.POINTER(C.c_uint8)), ("tok_df", C.POINTER(C.c_uint32)),
@@ -146,6 +152,7 @@ def load_library():
     L.bm25x_index_create.argtypes = [C.POINTER(_Corpus), C.c_int, C.POINTER(vp)]
     L.bm25x_index_create_from_blocks.argtypes = [C.POINTER(_Blocks), C.c_int, C.POINTER(vp)]
     L.bm25x_index_export_blocks.argtypes = [vp, C.POINTER(Export)]
+    L.bm25x_index_create_from_documents.argtypes = [C.POINTER(_Documents), C.c_int, C.POINTER(vp)]
     L.bm25x_growing_create.argtypes = [vp, C.POINTER(_GrowingDocs), C.POINTER(vp)]
     L.bm25x_search_batch_growing.argtypes = [vp, vp, C.c_uint32, u32p, u32p, C.c_uint32, u8p, u8p, u32p, f32p, f64p,
                                              u16p, u32p, C.POINTER(SearchStats)]
@@ -205,6 +212,8 @@ def load_library():
     L.bm25x_sharded_create.argtypes = [C.POINTER(_Corpus), C.c_uint32, u32p, C.POINTER(C.c_int), C.POINTER(vp)]
     L.bm25x_index_create_sharded_from_blocks.argtypes = [C.POINTER(_Blocks), C.c_uint32, u32p, C.POINTER(C.c_int),
                                                          C.POINTER(vp)]
+    L.bm25x_index_create_sharded_from_documents.argtypes = [C.POINTER(_Documents), C.c_uint32, u32p, C.POINTER(C.c_int),
+                                                            C.POINTER(vp)]
     L.bm25x_sharded_destroy.argtypes = [vp]
     L.bm25x_sharded_destroy.restype = None
     L.bm25x_sharded_get_info.argtypes = [vp, C.POINTER(IndexInfo), u32p, u32p]
@@ -295,6 +304,21 @@ def _blocks(keep, n_docs, n_terms, term_blk_off, blk_min_doc, blk_n, blk_meta_do
     if blk_wand_fieldnorm is not None and blk_wand_tf is not None:   # SummaryTuple.wand_* (checked against the blocks)
         c.blk_wand_fieldnorm = _kept(keep, blk_wand_fieldnorm, np.uint8, C.c_uint8)
         c.blk_wand_tf = _kept(keep, blk_wand_tf, np.uint32, C.c_uint32)
+    return c
+
+
+def _documents(keep, elem_off, elem_tf, elem_term, elem_key, n_terms, payload, k1, b):
+    c = _Documents()
+    c.elem_off = _kept(keep, elem_off, np.uint64, C.c_uint64)
+    c.n_docs = len(keep[-1]) - 1
+    c.elem_tf = _kept(keep, elem_tf, np.uint32, C.c_uint32)
+    if elem_term is not None:
+        c.elem_term = _kept(keep, elem_term, np.uint32, C.c_uint32)
+    if elem_key is not None:
+        c.elem_key = _kept(keep, elem_key, np.uint8, C.c_uint8)
+    if payload is not None:
+        c.payload = _kept(keep, payload, np.uint16, C.c_uint16)
+    c.n_terms, c.k1, c.b = int(n_terms), float(k1), float(b)
     return c
 
 
@@ -443,6 +467,22 @@ class Index:
         h = C.c_void_p()
         _check(load_library().bm25x_index_create_from_blocks(C.byref(c), device, C.byref(h)))
         return cls._adopt(h, n_docs, n_terms)
+
+    @classmethod
+    def from_documents(cls, elem_off, elem_tf, *, elem_term=None, elem_key=None, n_terms=0, payload=None, k1=1.2, b=0.75,
+                       device=0) -> "Index":
+        """Index from documents in heap-scan order (doc id = position), inverted on the GPU
+        (bm25x_index_create_from_documents): document d holds elements elem_off[d]..elem_off[d+1], each a term and its tf,
+        strictly ascending by term.  Exactly one of elem_term (ordinals < n_terms: keyless) or elem_key ([E, 16] keys:
+        keyed, the vocabulary is the distinct keys ascending).  The handle equals Index() on the reference's Segment of the
+        same documents."""
+        keep = []
+        c = _documents(keep, elem_off, elem_tf, elem_term, elem_key, n_terms, payload, k1, b)
+        h = C.c_void_p()
+        _check(load_library().bm25x_index_create_from_documents(C.byref(c), device, C.byref(h)))
+        info = IndexInfo()
+        _check(load_library().bm25x_index_get_info(h, C.byref(info)))
+        return cls._adopt(h, info.n_docs, info.n_terms)
 
     @classmethod
     def _adopt(cls, handle, n_docs, n_terms):
@@ -802,6 +842,23 @@ class ShardedIndex:
                                                                      devs, C.byref(self.h)))
         self.n_docs, self.n_terms = int(n_docs), int(n_terms)
         return self
+
+    @classmethod
+    def from_documents(cls, elem_off, elem_tf, *, elem_term=None, elem_key=None, n_terms=0, payload=None, k1=1.2, b=0.75,
+                       n_shards=2, doc_bounds=None, devices=None) -> "ShardedIndex":
+        """The sharded index from documents (Index.from_documents' arguments, bm25x_index_create_sharded_from_documents):
+        every shard's device inverts only its own documents' elements.  Equals ShardedIndex() on the Segment's CSR with the
+        same n_shards / doc_bounds / devices."""
+        keep = []
+        c = _documents(keep, elem_off, elem_tf, elem_term, elem_key, n_terms, payload, k1, b)
+        bounds = np.ascontiguousarray(doc_bounds, dtype=np.uint32) if doc_bounds is not None else None
+        devs = (C.c_int * int(n_shards))(*[int(d) for d in devices]) if devices is not None else None
+        h = C.c_void_p()
+        _check(load_library().bm25x_index_create_sharded_from_documents(C.byref(c), int(n_shards), _p(bounds, C.c_uint32),
+                                                                        devs, C.byref(h)))
+        info = IndexInfo()
+        _check(load_library().bm25x_sharded_get_info(h, C.byref(info), None, None))
+        return cls._adopt(h, info.n_docs, info.n_terms)
 
     @classmethod
     def _adopt(cls, handle, n_docs, n_terms):

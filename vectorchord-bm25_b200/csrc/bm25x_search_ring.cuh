@@ -27,7 +27,8 @@
 //             reference's operation order (Cache::evaluate, bm25.rs:355-358, summed over ascending terms) and enter
 //             the warp's pool.
 //   dense     windows in which the runs overlap heavily (head terms) are summed in a dense f32 accumulator indexed by
-//             doc - lo instead (the window is clamped to the accumulator size: a ring can be consumed partially).
+//             doc - lo instead (the window is clamped to the accumulator size: a ring can be consumed partially); plain
+//             kernel only.
 //   pruning   MaxScore-style, as v5 (token-level bounds; non-streamed terms are probed in HBM for candidates).
 //
 // Flavours (RCfg::FLAVOUR, RingFlavour in bm25x_common.h).  The above is the PLAIN kernel (RING_PLAIN; RING_HANDBACK =
@@ -157,6 +158,7 @@ struct RCfg {
     static constexpr size_t off_cand = off_pool_g + POOL_SMEM * 4;
     // seeded launches: the first k champions of the query's terms (doc, w) in shared memory, SST slots per term
     static constexpr uint32_t SST = KP_ <= 64 ? 32u : 128u;
+    static_assert(!SEEDED || SST > 32u || 64 + 32 * M_ <= LCAP, "k <= 32: the seeds of every term fit the list at once");
     static constexpr size_t off_seed = (off_cand + (size_t)LCAP * 2 + 7) & ~(size_t)7;
     static constexpr size_t off_hit = off_seed + (SEEDED ? (size_t)M_ * SST * 8 : 0);
     static constexpr size_t off_s1f = 0;  // CTA-shared: 1 KiB table first, then the warps
@@ -880,9 +882,11 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                 }
             }
             // ---- dense or sparse?  (expected number of documents held by two runs in this window) ----
+            // (not in seeded launches: their queries have no dense list, and a window whose runs happen to overlap
+            // is verified like any other — the dense sum only saves time, the verification is exact either way)
             bool dense = false;
             uint32_t span = 0;
-            if (C::M > 1) {
+            if (C::M > 1 && !C::SEEDED) {
                 const uint32_t n = e - rd;
                 const uint32_t S = __reduce_add_sync(FULL, n);
                 const uint32_t S2 = __reduce_add_sync(FULL, n * n);
@@ -1383,8 +1387,26 @@ __global__ void __launch_bounds__(C::THREADS, 1) k_search_ring(const __grid_cons
                     // rings hold every run's postings of the window, so the ONE verification site below tells whether
                     // another term holds the document
                     const uint32_t slices = (min(k, (uint32_t)BM25X_CHAMP_L) + 31u) >> 5;  // per term
+                    if constexpr (C::SST == 32u) {
+                        // k <= 32: one slice per term.  All M slices at once, their shared loads in flight together
+                        // (the list has room: nc <= 64 + 32·M <= LCAP)
+                        if (ss == 0u && nc <= 64u) {
+                            uint32_t d[C::M];
+#pragma unroll
+                            for (int jj = 0; jj < C::M; ++jj) d[jj] = seeds[jj * C::SST + lane].doc;
+#pragma unroll
+                            for (int jj = 0; jj < C::M; ++jj) {
+                                if (jj >= (int)m || ((ne_mask >> jj) & 1u)) continue;  // a pruned term's documents cannot enter
+                                const bool inw = d[jj] >= lo && d[jj] < hi;
+                                const uint32_t bal = __ballot_sync(FULL, inw);
+                                if (inw) cand[nc + __popc(bal & lt_mask)] = (uint16_t)((31u << 10) | (jj * C::SST + lane));
+                                nc += __popc(bal);
+                            }
+                            ss = (uint32_t)C::M;
+                        }
+                    }
 #pragma unroll 1
-                    while (ss < (uint32_t)C::M * slices && nc <= 64u) {
+                    while (C::SST > 32u && ss < (uint32_t)C::M * slices && nc <= 64u) {
                         uint32_t jj = ss, r = (uint32_t)lane;
                         if constexpr (C::SST > 32u) {
                             jj = ss / slices;

@@ -150,6 +150,59 @@ typedef struct {
 } bm25x_documents;
 int bm25x_index_create_from_documents(const bm25x_documents *docs, int device, bm25x_index **out);
 
+/* ---- documents and queries as PostgreSQL tsvectors, the type every way into the reference takes (bm25_ops is FOR TYPE
+ * tsvector, src/sql/finalize.sql:34-35): CREATE INDEX and aminsert cast each row with cast_tsvector_to_document, the
+ * index scan casts its query with cast_tsvector_to_query (src/datatype/tsvector.rs:84-105).  A batch of n tsvectors as
+ * the reference borrows them (TsVectorBorrowed, tsvector.rs:43-71; memory_tsvector.rs:30-51): vector i = its WordEntry
+ * words entries[ent_off[i] .. ent_off[i+1]) and its lexeme area bytes[byte_off[i] .. byte_off[i+1]), exactly what follows
+ * the datum's header.  Entry: bit 0 haspos, bits 1..11 len, bits 12..31 pos; the lexeme is area[pos .. pos+len), and with
+ * haspos its count is the native-endian u16 at area[pos+len rounded up to even] (the number of positions).
+ * Host refusals, all before any device is touched, BM25X_ERR_INVALID, the message naming the vector and the entry where
+ * there is one (the reference panics in each): null arguments (entries / bytes may be NULL when there are none), ent_off[0]
+ * or byte_off[0] != 0, offsets going backwards, a lexeme or a count running past its area, and in document mode an entry
+ * without positions ("tsvector must have positions", tsvector.rs:88). */
+typedef struct {
+    uint32_t n;
+    const uint64_t *ent_off;   /* [n+1], ent_off[0] == 0 */
+    const uint32_t *entries;   /* WordEntry: bit 0 haspos, bits 1..11 len, bits 12..31 pos */
+    const uint64_t *byte_off;  /* [n+1], byte_off[0] == 0 */
+    const uint8_t *bytes;
+} bm25x_tsvectors;
+/* The cast alone, on `device`: cast_tsvector_to_document (as_query == 0) or cast_tsvector_to_query of every vector.  Row i
+ * is out_off[i] .. out_off[i+1] of out_key ([.., 16] keys, ascending bytewise and distinct, vector::intern under seed) and,
+ * in document mode, out_tf (the saturating sum of the merged counts; not written in query mode, may be NULL there).  A cast
+ * never grows: size out_key and out_tf for ent_off[n] elements.  The output is bit for bit the restated casts over
+ * bm25x_intern.  Refusals: the host ones above; then, after the device work and before any output is written, a document
+ * element whose merged count is 0 (Document::new, vector.rs:51-64; BM25X_ERR_INVALID naming the vector).  The device works
+ * on chunks of whole vectors (at most 2^22 entries, 64 MiB of lexeme area and 2^22 vectors, or one larger vector; a vector
+ * of more than 2^31 - 1 entries is BM25X_ERR_UNSUPPORTED) and holds the cast until the end: 16 B (query) or 20 B
+ * (document) per entry, 4 B per vector (8 more in document mode), and per chunk about 60 B per entry plus its area and
+ * CUB's temporary storage. */
+int bm25x_cast_tsvectors(const bm25x_tsvectors *tsv, const uint8_t seed[32], int as_query, int device,
+                         uint64_t *out_off, uint8_t *out_key, uint32_t *out_tf);
+/* CREATE INDEX from the tsvectors (am_build.rs:722): the index bm25x_index_create_from_documents builds from the keyed
+ * documents the document cast gives, array for array; doc id = position (NULL rows are the caller's to leave out, as
+ * ambuild does), payload as there.  The keys never travel to the host: the cast leaves a device-resident keyed CSR that
+ * the build from documents reads chunk by chunk; only the row offsets and the document lengths come down (12 B per
+ * document).  Refusals (*out = NULL, no device memory left behind): the cast's; check_common's on n_docs (0 or 0xFFFFFFFF),
+ * k1 and b, on the host; on the device BM25X_ERR_UNSUPPORTED for a merged tf >= 2^24 (naming the first such document)
+ * and for more than 0xFFFFFFFE distinct keys, as the build from documents refuses them; BM25X_ERR_OOM / BM25X_ERR_CUDA.
+ * Device memory beyond the index: 20 B per tsvector entry (the cast, held through the build), one upload chunk of the cast
+ * (freed before the build starts), and the build from documents' own figures. */
+int bm25x_index_create_from_tsvectors(const bm25x_tsvectors *tsv, const uint8_t seed[32], const uint16_t *payload,
+                                      double k1, double b, int device, bm25x_index **out);
+/* Queries from tsvectors, ready for bm25x_search_batch, bm25x_search_candidates, bm25x_batch_prepare and the growing
+ * segment's searches as they are: for each vector the query cast (cast_tsvector_to_query) and then address_tokens::read
+ * (address_tokens.rs:61-98) on the index's device.  Row i = q_terms[q_off[i] .. q_off[i+1]) holds its distinct keys in
+ * key order as term ordinals, BM25X_TERM_MISSING for a key the vocabulary lacks (the searches drop those,
+ * search.rs:60-62).  Size q_terms for ent_off[n] terms.  The vocabulary goes to the device once per handle (16 B per term,
+ * kept until bm25x_index_destroy).  Refusals: the host ones above (query mode), then an index without term keys (a
+ * replica, a keyless build) with bm25x_lookup_terms' message, both before any device work; more than 2^32 - 1 output terms
+ * (BM25X_ERR_UNSUPPORTED), before any output is written.  Thread-safe alongside the searches on the same handle.  Device
+ * memory: 4 B per entry and 4 B per vector, held until the call returns, plus one upload chunk of the cast. */
+int bm25x_tsvector_queries(bm25x_index *idx, const uint8_t seed[32], const bm25x_tsvectors *tsv, uint32_t *q_off,
+                           uint32_t *q_terms);
+
 /* ---- the inverse: a finalized index written out as the reference's stored segment, i.e. everything flush() writes for
  * it (flush.rs:40-158) but the pages, tapes and address trees, which stay the caller's.  Encoded on the index's device:
  * per token, blocks of 128 postings in doc order, the last one shorter (flush.rs:78-90; the index's own blocks); payloads
@@ -252,7 +305,8 @@ int bm25x_lookup_terms(const bm25x_index *idx, const uint8_t *keys, uint32_t n, 
 
 /* vector::intern (crates/bm25/src/vector.rs:19-35): the 16-byte key of a token under the index's 32-byte seed.  Tokens
  * shorter than 16 bytes without a NUL byte are their own zero-padded key; all others are the first 16 bytes of
- * blake3::keyed_hash(seed, token) with a zero last byte replaced by 1.  Host-only (no device involved). */
+ * blake3::keyed_hash(seed, token) with a zero last byte replaced by 1.  Host-only (no device involved); the tsvector
+ * casts below intern whole batches on the device, bit for bit the same. */
 int bm25x_intern(const uint8_t seed[32], const uint8_t *token, size_t len, uint8_t key_out[BM25X_KEY_WIDTH]);
 /* Test hook: first 16 bytes of BLAKE3 keyed_hash(key, data) without the interning rules (known-answer tests). */
 int bm25x_blake3_keyed16(const uint8_t key[32], const uint8_t *data, size_t len, uint8_t out[16]);

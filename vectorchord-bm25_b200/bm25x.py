@@ -46,6 +46,11 @@ class _Documents(C.Structure):  # bm25x_documents
                 ("n_terms", C.c_uint32), ("k1", C.c_double), ("b", C.c_double)]
 
 
+class _Tsvectors(C.Structure):  # bm25x_tsvectors
+    _fields_ = [("n", C.c_uint32), ("ent_off", C.POINTER(C.c_uint64)), ("entries", C.POINTER(C.c_uint32)),
+                ("byte_off", C.POINTER(C.c_uint64)), ("bytes", C.POINTER(C.c_uint8))]
+
+
 class Export(C.Structure):  # bm25x_export
     _fields_ = [("doc_fieldnorm", C.POINTER(C.c_uint8)), ("payload", C.POINTER(C.c_uint16)), ("sum_doc_len", C.c_uint64),
                 ("term_key", C.POINTER(C.c_uint8)), ("tok_df", C.POINTER(C.c_uint32)),
@@ -153,6 +158,10 @@ def load_library():
     L.bm25x_index_create_from_blocks.argtypes = [C.POINTER(_Blocks), C.c_int, C.POINTER(vp)]
     L.bm25x_index_export_blocks.argtypes = [vp, C.POINTER(Export)]
     L.bm25x_index_create_from_documents.argtypes = [C.POINTER(_Documents), C.c_int, C.POINTER(vp)]
+    L.bm25x_cast_tsvectors.argtypes = [C.POINTER(_Tsvectors), u8p, C.c_int, C.c_int, u64p, u8p, u32p]
+    L.bm25x_index_create_from_tsvectors.argtypes = [C.POINTER(_Tsvectors), u8p, u16p, C.c_double, C.c_double, C.c_int,
+                                                    C.POINTER(vp)]
+    L.bm25x_tsvector_queries.argtypes = [vp, u8p, C.POINTER(_Tsvectors), u32p, u32p]
     L.bm25x_growing_create.argtypes = [vp, C.POINTER(_GrowingDocs), C.POINTER(vp)]
     L.bm25x_search_batch_growing.argtypes = [vp, vp, C.c_uint32, u32p, u32p, C.c_uint32, u8p, u8p, u32p, f32p, f64p,
                                              u16p, u32p, C.POINTER(SearchStats)]
@@ -322,6 +331,40 @@ def _documents(keep, elem_off, elem_tf, elem_term, elem_key, n_terms, payload, k
     return c
 
 
+def _tsvectors(keep, ent_off, entries, byte_off, data):
+    """bm25x_tsvectors over host arrays: vector i = WordEntry words entries[ent_off[i]:ent_off[i+1]] and lexeme area
+    data[byte_off[i]:byte_off[i+1]] (what follows each datum's header)."""
+    t = _Tsvectors()
+    t.ent_off = _kept(keep, ent_off, np.uint64, C.c_uint64)
+    t.n = len(keep[-1]) - 1
+    t.entries = _kept(keep, entries, np.uint32, C.c_uint32)
+    t.byte_off = _kept(keep, byte_off, np.uint64, C.c_uint64)
+    t.bytes = _kept(keep, np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray)) else data, np.uint8,
+                    C.c_uint8)
+    return t
+
+
+def _seed(seed):
+    assert len(seed) == 32
+    return (C.c_uint8 * 32).from_buffer_copy(bytes(seed))
+
+
+def cast_tsvectors(seed, ent_off, entries, byte_off, data, as_query=False, device=0):
+    """cast_tsvector_to_document (or, as_query, cast_tsvector_to_query) of every tsvector on the GPU
+    (bm25x_cast_tsvectors).  Returns (off u64 [n+1], keys u8 [E, 16], tf u32 [E] or None): row i = off[i]:off[i+1], its
+    keys ascending bytewise and distinct, tf the saturating sum of the merged position counts."""
+    keep = []
+    t = _tsvectors(keep, ent_off, entries, byte_off, data)
+    E = int(keep[0][-1]) if len(keep[0]) else 0
+    off = np.zeros(t.n + 1, np.uint64)
+    keys = np.zeros((max(E, 1), 16), np.uint8)
+    tf = None if as_query else np.zeros(max(E, 1), np.uint32)
+    _check(load_library().bm25x_cast_tsvectors(C.byref(t), _seed(seed), int(bool(as_query)), device, _p(off, C.c_uint64),
+                                               _p(keys, C.c_uint8), _p(tf, C.c_uint32)))
+    n = int(off[-1])
+    return off, keys[:n].copy(), None if tf is None else tf[:n].copy()
+
+
 def _result_arrays(nq, k, want_f64, want_payload):
     return {"doc": np.empty((nq, k), np.uint32), "score": np.empty((nq, k), np.float32),
             "score64": np.empty((nq, k), np.float64) if want_f64 else None,
@@ -485,6 +528,21 @@ class Index:
         return cls._adopt(h, info.n_docs, info.n_terms)
 
     @classmethod
+    def from_tsvectors(cls, seed, ent_off, entries, byte_off, data, *, payload=None, k1=1.2, b=0.75, device=0) -> "Index":
+        """CREATE INDEX from tsvectors (bm25x_index_create_from_tsvectors): the index from_documents builds from the keyed
+        documents of the document cast (doc id = position), the cast and the inversion on the GPU without the keys
+        coming to the host.  The tsvectors as cast_tsvectors takes them."""
+        keep = []
+        t = _tsvectors(keep, ent_off, entries, byte_off, data)
+        pay = _kept(keep, payload, np.uint16, C.c_uint16) if payload is not None else None
+        h = C.c_void_p()
+        _check(load_library().bm25x_index_create_from_tsvectors(C.byref(t), _seed(seed), pay, float(k1), float(b),
+                                                                device, C.byref(h)))
+        info = IndexInfo()
+        _check(load_library().bm25x_index_get_info(h, C.byref(info)))
+        return cls._adopt(h, info.n_docs, info.n_terms)
+
+    @classmethod
     def _adopt(cls, handle, n_docs, n_terms):
         self = cls.__new__(cls)
         self.h, self._keep, self.n_docs, self.n_terms = handle, None, int(n_docs), int(n_terms)
@@ -584,6 +642,19 @@ class Index:
         out = np.zeros(len(keys), dtype=np.uint32)
         _check(load_library().bm25x_lookup_terms(self.h, _p(keys, C.c_uint8), len(keys), _p(out, C.c_uint32)))
         return out
+
+    def tsvector_queries(self, seed, ent_off, entries, byte_off, data):
+        """Queries from tsvectors (bm25x_tsvector_queries): the query cast of each vector and its keys' ordinals in
+        this index's vocabulary (TERM_MISSING when absent), on the GPU.  Returns (q_off, q_terms) as search_batch and
+        search_candidates take them."""
+        keep = []
+        t = _tsvectors(keep, ent_off, entries, byte_off, data)
+        E = int(keep[0][-1]) if len(keep[0]) else 0
+        q_off = np.zeros(t.n + 1, np.uint32)
+        q_terms = np.zeros(max(E, 1), np.uint32)
+        _check(load_library().bm25x_tsvector_queries(self.h, _seed(seed), C.byref(t), _p(q_off, C.c_uint32),
+                                                     _p(q_terms, C.c_uint32)))
+        return q_off, q_terms[:int(q_off[-1])].copy()
 
     # ---- bm25::search for a batch (host buffers in, host buffers out) ----
     def search_batch(self, q_off, q_terms, k, allow=None, want_f64=True, want_payload=False, out=None):

@@ -122,6 +122,12 @@ cudaError_t index_finish_device(bm25x_index *ix);
 int upload_csr(bm25x_index *ix, const char *who, uint32_t T, uint64_t P, const uint64_t *post_off,
                const uint32_t *post_doc, const uint32_t *post_tf);
 
+// ---- the build from documents (bm25x_documents.cu) after its host checks: documents c as
+// bm25x_index_create_from_documents takes them and has checked them, doc_len[n_docs] their lengths.  The element arrays
+// may be device memory on `device` (the tsvector build's cast, bm25x_tsvector.cu); elem_off is host memory.  *out is
+// set on success; a CUDA failure is refused as `who`'s.
+int documents_build(const char *who, const bm25x_documents *c, const uint32_t *doc_len, int device, bm25x_index **out);
+
 // ---- host checks and helpers shared by the builders, with the messages their refusals give ----
 
 int cuda_refusal(const char *who, const char *step, cudaError_t e);

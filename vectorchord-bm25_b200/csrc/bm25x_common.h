@@ -114,6 +114,9 @@ struct bm25x_index {
     double *eval_idf = nullptr;
     uint32_t *eval_fn_len = nullptr;
     std::mutex eval_mutex;
+    // bm25x_tsvector_queries: h_keys as big-endian word pairs (Key128, 16 B per term), built on first use, kept on the device
+    void *key_vocab = nullptr;
+    std::mutex key_vocab_mutex;
 };
 
 // Document-sharded index (bm25x_sharded_*): shard s is an ordinary index over the documents [bounds[s], bounds[s+1]) with

@@ -22,25 +22,12 @@
 #include <cub/device/device_reduce.cuh>
 
 #include "bm25x_build.h"
+#include "bm25x_keys.cuh"
 
 namespace {
 
 constexpr uint64_t CHUNK = 1ull << 22;  // elements per chunk
 constexpr unsigned TPB = 256;
-
-// A 16-byte Element.key as two big-endian words: (hi, lo) order is the bytewise order of the key.
-struct Key128 {
-    uint64_t hi, lo;
-};
-__host__ __device__ __forceinline__ bool operator==(const Key128 &a, const Key128 &b) { return a.hi == b.hi && a.lo == b.lo; }
-struct Key128Bits {  // CUB's radix decomposer, most significant word first
-    __host__ __device__ ::cuda::std::tuple<uint64_t &, uint64_t &> operator()(Key128 &k) const { return {k.hi, k.lo}; }
-};
-
-__device__ __forceinline__ uint64_t bswap64(uint64_t x) {
-    return ((uint64_t)__byte_perm((uint32_t)x, 0, 0x0123) << 32) | __byte_perm((uint32_t)(x >> 32), 0, 0x0123);
-}
-__device__ __forceinline__ Key128 key_of(ulonglong2 raw) { return {bswap64(raw.x), bswap64(raw.y)}; }
 
 unsigned grid_of(uint64_t n) { return (unsigned)((n + TPB - 1) / TPB); }
 
@@ -143,18 +130,19 @@ struct GrowBuf {
     }
 };
 
-// Ordinals of elements [g, g + n) into term: keyless as given; keyed the keys (uploaded to kbuf) looked up in the device
-// vocabulary.  idx[i] = i when idx is given.
+// Ordinals of elements [g, g + n) into term: keyless as given; keyed the keys (copied to kbuf) looked up in the device
+// vocabulary.  idx[i] = i when idx is given.  The element arrays may be host or device memory: the copies follow the
+// addresses (a build from tsvectors hands its device-resident cast here).
 cudaError_t load_ordinals(const bm25x_documents *c, uint64_t g, uint64_t n, const Key128 *vocab, uint32_t T,
                           ulonglong2 *kbuf, uint32_t *term, uint32_t *idx) {
     cudaError_t e;
     if (c->elem_key) {
-        e = cudaMemcpy(kbuf, c->elem_key + g * 16, 16 * n, cudaMemcpyHostToDevice);
+        e = cudaMemcpy(kbuf, c->elem_key + g * 16, 16 * n, cudaMemcpyDefault);
         if (e != cudaSuccess) return e;
         k_key_ordinals<<<grid_of(n), TPB>>>(kbuf, n, vocab, T, term, idx);
         return cudaGetLastError();
     }
-    e = cudaMemcpy(term, c->elem_term + g, sizeof(uint32_t) * n, cudaMemcpyHostToDevice);
+    e = cudaMemcpy(term, c->elem_term + g, sizeof(uint32_t) * n, cudaMemcpyDefault);
     if (e != cudaSuccess || !idx) return e;
     k_iota<<<grid_of(n), TPB>>>(idx, n);
     return cudaGetLastError();
@@ -295,7 +283,7 @@ static int vocab_pass(const char *who, const bm25x_documents *c, int device, std
             if (e == cudaSuccess) e = cb[1].grow(cap, 0);
             if (e != cudaSuccess) break;
         }
-        e = cudaMemcpy(kb[0].p + V + A, c->elem_key + g * 16, 16 * n, cudaMemcpyHostToDevice);
+        e = cudaMemcpy(kb[0].p + V + A, c->elem_key + g * 16, 16 * n, cudaMemcpyDefault);
         if (e != cudaSuccess) break;
         k_keys_be<<<grid_of(n), TPB>>>(kb[0].p + V + A, cb[0].p + V + A, n);
         e = cudaGetLastError();
@@ -386,7 +374,7 @@ static int invert(const char *who, const bm25x_documents *c, const std::vector<u
                 h_sdoc.push_back(doc - lo);
             }
         sc.e = load_ordinals(c, g, n, vocab, T, kbuf, term[0], idx[0]);
-        if (sc.e == cudaSuccess) sc.e = cudaMemcpy(d_tf, c->elem_tf + g, sizeof(uint32_t) * n, cudaMemcpyHostToDevice);
+        if (sc.e == cudaSuccess) sc.e = cudaMemcpy(d_tf, c->elem_tf + g, sizeof(uint32_t) * n, cudaMemcpyDefault);
         if (sc.e == cudaSuccess)
             sc.e = cudaMemcpy(d_start, h_start.data(), sizeof(uint64_t) * h_start.size(), cudaMemcpyHostToDevice);
         if (sc.e == cudaSuccess)
@@ -405,6 +393,22 @@ static int invert(const char *who, const bm25x_documents *c, const std::vector<u
     return sc.e == cudaSuccess ? BM25X_OK : cuda_refusal(who, "document inversion", sc.e);
 }
 
+int documents_build(const char *who, const bm25x_documents *c, const uint32_t *doc_len, int device, bm25x_index **out) {
+    const uint32_t N = c->n_docs;
+    const uint64_t E = c->elem_off[N];
+    std::vector<uint8_t> keys;
+    std::vector<uint32_t> df;
+    int rc = c->elem_key ? vocab_pass(who, c, device, keys, df) : count_df(who, c, keys, c->n_terms, 0, E, device, df);
+    if (rc != BM25X_OK) return rc;
+    const uint32_t T = (uint32_t)df.size();
+    BuildMeta m{N, T, doc_len, c->payload, c->elem_key ? keys.data() : nullptr, c->k1, c->b, df.data(), E};
+    IndexGuard ix;
+    rc = index_begin(m, nullptr, device, ix);
+    if (rc == BM25X_OK) rc = invert(who, c, keys, 0, N, ix.get());
+    if (rc == BM25X_OK) *out = ix.release();
+    return rc;
+}
+
 extern "C" int bm25x_index_create_from_documents(const bm25x_documents *c, int device, bm25x_index **out) {
     const char *who = "bm25x_index_create_from_documents";
     if (out) *out = nullptr;
@@ -416,19 +420,7 @@ extern "C" int bm25x_index_create_from_documents(const bm25x_documents *c, int d
     int rc = validate_documents(c, doc_len);
     if (rc == BM25X_OK) rc = check_device(who, device);
     if (rc != BM25X_OK) return rc;
-    const uint32_t N = c->n_docs;
-    const uint64_t E = c->elem_off[N];
-    std::vector<uint8_t> keys;
-    std::vector<uint32_t> df;
-    rc = c->elem_key ? vocab_pass(who, c, device, keys, df) : count_df(who, c, keys, c->n_terms, 0, E, device, df);
-    if (rc != BM25X_OK) return rc;
-    const uint32_t T = (uint32_t)df.size();
-    BuildMeta m{N, T, doc_len.data(), c->payload, c->elem_key ? keys.data() : nullptr, c->k1, c->b, df.data(), E};
-    IndexGuard ix;
-    rc = index_begin(m, nullptr, device, ix);
-    if (rc == BM25X_OK) rc = invert(who, c, keys, 0, N, ix.get());
-    if (rc == BM25X_OK) *out = ix.release();
-    return rc;
+    return documents_build(who, c, doc_len.data(), device, out);
 }
 
 extern "C" int bm25x_index_create_sharded_from_documents(const bm25x_documents *c, uint32_t S, const uint32_t *doc_bounds,

@@ -803,6 +803,7 @@ extern "C" void bm25x_index_destroy(bm25x_index *ix) {
     cudaSetDevice(ix->device);
     if (ix->stream) cudaStreamSynchronize(ix->stream);
     for (void *p : ix->allocs) cudaFree(p);
+    cudaFree(ix->key_vocab);
     if (ix->h_stage) cudaFreeHost(ix->h_stage);
     if (ix->h_stage_free) cudaEventDestroy(ix->h_stage_free);
     if (ix->copy_stream) cudaStreamDestroy(ix->copy_stream);

@@ -6,7 +6,8 @@
 //
 // The reference takes BLAKE3 from the `blake3` crate (Cargo.lock: blake3 1.8.4), which is not vendored in
 // the reference tree; the function below restates the published BLAKE3 algorithm (keyed_hash mode, full chunk tree) in
-// portable C++.  Host code: keys are computed where the tokens are (the Rust side / the caller), never on the GPU.
+// portable C++.  Host code, one token per call; the tsvector casts intern whole batches on the GPU with the same
+// algorithm (bm25x_tsvector.cu), and the tests hold the two to the same bits.
 #include <stdint.h>
 #include <string.h>
 

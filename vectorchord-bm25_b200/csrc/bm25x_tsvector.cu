@@ -1,0 +1,533 @@
+// bm25x_tsvector.cu — the tsvector casts on the GPU (DESIGN §4.10): documents and queries taken as PostgreSQL tsvectors,
+// as every way into the reference takes them.
+//
+// cast_tsvector_to_document / cast_tsvector_to_query (src/datatype/tsvector.rs:84-105) intern every lexeme of a vector
+// (vector::intern, crates/bm25/src/vector.rs:19-35), sort by key and merge equal keys (document: the position counts
+// summed with saturation, tsvector.rs:107-127).  Here, over chunks of whole vectors:
+//   1. k_tsv_intern: one thread per WordEntry.  The lexeme is copied (short) or hashed (BLAKE3 keyed_hash in registers,
+//      at most 2 chunks + 1 parent), and the key goes out as Key128 tagged with its vector;
+//   2. a CUB radix sort by (vector, key) and a reduce by key with a saturating add merge the runs;
+//   3. k_tsv_emit writes each merged element at its place in the device-resident output (raw key bytes and tf, or the
+//      key's ordinal in an index's vocabulary), counts it into its vector's row and sums its vector's length.
+// Row offsets come from the row counts by a host scan once every chunk has run, so that a refused cast writes nothing.
+// The build from tsvectors hands the device-resident keyed CSR to the build from documents (documents_build): the keys
+// never travel to the host.
+#include <string.h>
+
+#include <algorithm>
+#include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_reduce.cuh>
+
+#include "bm25x_build.h"
+#include "bm25x_keys.cuh"
+
+namespace {
+
+constexpr uint64_t CHUNK_ENT = 1ull << 22;    // entries per upload chunk
+constexpr uint64_t CHUNK_BYTES = 1ull << 26;  // lexeme-area bytes per upload chunk
+constexpr uint64_t CHUNK_VEC = 1ull << 22;    // vectors per upload chunk (empty vectors cost no entry)
+constexpr unsigned TPB = 256;
+
+unsigned grid_of(uint64_t n) { return (unsigned)((n + TPB - 1) / TPB); }
+
+// ---- BLAKE3 keyed_hash, the first 16 bytes, of one lexeme of at most 2047 bytes (WordEntry.len has 11 bits) ----
+
+struct Seed {  // the 32-byte key as eight little-endian words, passed by value (kernel parameter space)
+    uint32_t w[8];
+};
+enum : uint32_t { CHUNK_START = 1, CHUNK_END = 2, PARENT = 4, ROOT = 8, KEYED_HASH = 16 };
+constexpr uint32_t IV0 = 0x6A09E667u, IV1 = 0xBB67AE85u, IV2 = 0x3C6EF372u, IV3 = 0xA54FF53Au;
+
+__device__ __forceinline__ uint32_t rotr(uint32_t x, int n) { return __funnelshift_r(x, x, n); }
+__device__ __forceinline__ void g(uint32_t &a, uint32_t &b, uint32_t &c, uint32_t &d, uint32_t mx, uint32_t my) {
+    a = a + b + mx;
+    d = rotr(d ^ a, 16);
+    c = c + d;
+    b = rotr(b ^ c, 12);
+    a = a + b + my;
+    d = rotr(d ^ a, 8);
+    c = c + d;
+    b = rotr(b ^ c, 7);
+}
+
+// The compression function: cv = the first 8 words of its output.  Every index is a constant once the rounds are
+// unrolled, so the state and the message stay in registers; the message permutation is register renaming.
+__device__ __forceinline__ void compress(uint32_t cv[8], const uint32_t block[16], uint32_t counter, uint32_t block_len,
+                                         uint32_t flags) {
+    uint32_t s[16] = {cv[0], cv[1], cv[2], cv[3], cv[4], cv[5], cv[6], cv[7], IV0, IV1, IV2, IV3, counter, 0u,
+                      block_len, flags};
+    uint32_t m[16];
+#pragma unroll
+    for (int i = 0; i < 16; i++) m[i] = block[i];
+#pragma unroll
+    for (int r = 0; r < 7; r++) {
+        g(s[0], s[4], s[8], s[12], m[0], m[1]);
+        g(s[1], s[5], s[9], s[13], m[2], m[3]);
+        g(s[2], s[6], s[10], s[14], m[4], m[5]);
+        g(s[3], s[7], s[11], s[15], m[6], m[7]);
+        g(s[0], s[5], s[10], s[15], m[8], m[9]);
+        g(s[1], s[6], s[11], s[12], m[10], m[11]);
+        g(s[2], s[7], s[8], s[13], m[12], m[13]);
+        g(s[3], s[4], s[9], s[14], m[14], m[15]);
+        const uint32_t t[16] = {m[2], m[6], m[3], m[10], m[7], m[0], m[4], m[13],
+                                m[1], m[11], m[12], m[5], m[9], m[14], m[15], m[8]};  // MSG_PERMUTATION
+#pragma unroll
+        for (int i = 0; i < 16; i++) m[i] = t[i];
+    }
+#pragma unroll
+    for (int i = 0; i < 8; i++) cv[i] = s[i] ^ s[i + 8];
+}
+
+// Block b of the message p[0..len): 64 bytes from offset 64 b, zero past len, as sixteen little-endian words.
+__device__ __forceinline__ void load_block(const uint8_t *__restrict__ p, uint32_t len, uint32_t b, uint32_t m[16]) {
+    const uint32_t off = 64 * b;
+#pragma unroll
+    for (int w = 0; w < 16; w++) {
+        uint32_t v = 0;
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+            const uint32_t at = off + 4 * w + j;
+            if (at < len) v |= (uint32_t)p[at] << (8 * j);
+        }
+        m[w] = v;
+    }
+}
+
+// The first four words of blake3::keyed_hash(seed, p[0..len)), len <= 2047: one chunk is the root; two chunks (1024
+// bytes, then the rest) are joined by a parent, which is the root.
+__device__ __forceinline__ void blake3_keyed16(const Seed &seed, const uint8_t *__restrict__ p, uint32_t len,
+                                               uint32_t out[4]) {
+    uint32_t cv[8], cv0[8], m[16];
+#pragma unroll
+    for (int i = 0; i < 8; i++) cv[i] = seed.w[i];
+    const bool two = len > 1024;
+    const uint32_t nb = len == 0 ? 1u : (len + 63) / 64;  // blocks over both chunks (chunk 0 holds 16 when two)
+    for (uint32_t b = 0; b < nb; b++) {
+        const uint32_t chunk = b >= 16 ? 1u : 0u, first = b - 16 * chunk;
+        if (b == 16) {
+#pragma unroll
+            for (int i = 0; i < 8; i++) {
+                cv0[i] = cv[i];
+                cv[i] = seed.w[i];
+            }
+        }
+        load_block(p, len, b, m);
+        const bool last = b + 1 == nb, chunk_last = last || (two && b == 15);
+        const uint32_t flags = KEYED_HASH | (first == 0 ? CHUNK_START : 0u) | (chunk_last ? CHUNK_END : 0u) |
+                               (last && !two ? ROOT : 0u);
+        compress(cv, m, chunk, min(64u, len - 64 * b), flags);
+    }
+    if (two) {
+#pragma unroll
+        for (int i = 0; i < 8; i++) {
+            m[i] = cv0[i];
+            m[i + 8] = cv[i];
+            cv[i] = seed.w[i];
+        }
+        compress(cv, m, 0, 64, KEYED_HASH | PARENT | ROOT);
+    }
+#pragma unroll
+    for (int i = 0; i < 4; i++) out[i] = cv[i];
+}
+
+// ---- the cast ----
+
+// A key tagged with the vector that holds it (the vector local to its chunk): sorted by (vec, hi, lo).
+struct VKey {
+    uint64_t hi, lo;
+    uint32_t vec;
+};
+struct VKeyBits {  // CUB's radix decomposer, most significant first
+    __host__ __device__ ::cuda::std::tuple<uint32_t &, uint64_t &, uint64_t &> operator()(VKey &k) const {
+        return {k.vec, k.hi, k.lo};
+    }
+};
+__host__ __device__ __forceinline__ bool operator==(const VKey &a, const VKey &b) {  // the merge's run test
+    return a.vec == b.vec && a.hi == b.hi && a.lo == b.lo;
+}
+struct SatAdd {  // Saturating<u32> sum (tsvector.rs:115-120)
+    __host__ __device__ uint32_t operator()(uint32_t a, uint32_t b) const {
+        const uint32_t s = a + b;
+        return s < a ? 0xFFFFFFFFu : s;
+    }
+};
+
+// One thread per entry of a chunk of nv vectors: entries of vector u are [eoff[u], eoff[u+1]) (rebased to the chunk),
+// its area bytes + boff[u] (rebased).  key[i] = the interned lexeme (vector::intern) tagged with u; cnt[i] = its
+// position count (document mode; the host checked that every entry has one).
+__global__ void k_tsv_intern(const uint32_t *__restrict__ ent, uint64_t n, const uint64_t *__restrict__ eoff,
+                             const uint64_t *__restrict__ boff, uint32_t nv, const uint8_t *__restrict__ bytes,
+                             const Seed seed, int as_query, VKey *__restrict__ key, uint32_t *__restrict__ cnt) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t u = owner_of(eoff, nv, i), e = ent[i];
+    const uint32_t len = (e >> 1) & 0x7FFu, pos = e >> 12;
+    const uint8_t *__restrict__ area = bytes + boff[u];
+    const uint8_t *__restrict__ lex = area + pos;
+    uint32_t w[4] = {0u, 0u, 0u, 0u};
+    bool nul = false;
+    if (len < 16) {
+#pragma unroll
+        for (uint32_t j = 0; j < 15; j++)
+            if (j < len) {
+                const uint32_t c = lex[j];
+                nul |= c == 0;
+                w[j >> 2] |= c << (8 * (j & 3));
+            }
+    }
+    if (len >= 16 || nul) {
+        blake3_keyed16(seed, lex, len, w);
+        if ((w[3] >> 24) == 0) w[3] |= 1u << 24;  // vector.rs:30-32: a hashed key never ends in a zero byte
+    }
+    VKey k;
+    k.hi = bswap64((uint64_t)w[0] | (uint64_t)w[1] << 32);
+    k.lo = bswap64((uint64_t)w[2] | (uint64_t)w[3] << 32);
+    k.vec = u;
+    key[i] = k;
+    if (!as_query) {
+        const uint32_t at = (pos + len + 1) & ~1u;  // SHORTALIGN(pos + len): the u16 count of the positions
+        cnt[i] = (uint32_t)area[at] | (uint32_t)area[at + 1] << 8;
+    }
+}
+
+// One thread per merged element i < *runs of a chunk whose vectors start at global vector v0 and whose elements go to
+// global element base + i: raw key bytes and tf (when given), or the ordinal of the key in the sorted vocabulary
+// (BM25X_TERM_MISSING when absent, address_tokens::read).  rows[v] counts the elements of vector v; document mode also
+// len[v] += tf, and the first vector with a merged tf of 0 / of 2^24 or more into flags[0] / flags[1].
+__global__ void k_tsv_emit(const VKey *__restrict__ key, const uint32_t *__restrict__ tf, const int64_t *__restrict__ runs,
+                           uint32_t v0, uint64_t base, int as_query, ulonglong2 *__restrict__ out_key,
+                           uint32_t *__restrict__ out_tf, const Key128 *__restrict__ vocab, uint32_t T,
+                           uint32_t *__restrict__ out_ord, uint32_t *__restrict__ rows, uint64_t *__restrict__ len,
+                           uint32_t *__restrict__ flags) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const bool live = i < (uint64_t)*runs;
+    const VKey k = live ? key[i] : VKey{0, 0, 0xFFFFFFFFu};
+    const uint32_t v = v0 + k.vec;
+    const uint32_t same = __match_any_sync(0xFFFFFFFFu, k.vec);
+    if (!live) return;
+    if ((threadIdx.x & 31) == (unsigned)(__ffs(same) - 1)) atomicAdd(&rows[v], (uint32_t)__popc(same));
+    const Key128 kk{k.hi, k.lo};
+    if (out_key) out_key[base + i] = raw_of(kk);
+    if (!as_query) {
+        const uint32_t t = tf[i];
+        if (out_tf) out_tf[base + i] = t;
+        atomicAdd((unsigned long long *)&len[v], (unsigned long long)t);
+        if (t == 0) atomicMin(&flags[0], v);
+        if (t >= (1u << 24)) atomicMin(&flags[1], v);
+    }
+    if (out_ord) {
+        uint32_t lo = 0, hi = T;
+        while (lo < hi) {
+            const uint32_t mid = (lo + hi) >> 1;
+            const Key128 w = vocab[mid];
+            if (w.hi < kk.hi || (w.hi == kk.hi && w.lo < kk.lo)) lo = mid + 1;
+            else hi = mid;
+        }
+        out_ord[base + i] = lo < T && vocab[lo] == kk ? lo : BM25X_TERM_MISSING;
+    }
+}
+
+// Raw keys → Key128 in place (an index's vocabulary as the lookups take it).
+__global__ void k_vocab_be(Key128 *__restrict__ keys, uint64_t n) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) keys[i] = key_of(reinterpret_cast<const ulonglong2 *>(keys)[i]);
+}
+
+// Every refusal of a batch of tsvectors that needs only the host (TsVectorBorrowed::iter's panics, tsvector.rs:55-71,
+// and "tsvector must have positions", tsvector.rs:88), named by who.
+int check_tsvectors(const char *who, const bm25x_tsvectors *t, int as_query) {
+    if (!t->ent_off || !t->byte_off) {
+        bm25x_set_error("%s: null argument", who);
+        return BM25X_ERR_INVALID;
+    }
+    const uint32_t n = t->n;
+    if (t->ent_off[0] != 0 || t->byte_off[0] != 0) {
+        bm25x_set_error("%s: invalid data: ent_off[0] and byte_off[0] must be 0", who);
+        return BM25X_ERR_INVALID;
+    }
+    for (uint32_t v = 0; v < n; v++)  // before any entry is read: the ranges must lie inside the arrays
+        if (t->ent_off[v + 1] < t->ent_off[v] || t->byte_off[v + 1] < t->byte_off[v]) {
+            bm25x_set_error("%s: invalid data: offsets not monotone at tsvector %u", who, v);
+            return BM25X_ERR_INVALID;
+        }
+    if ((!t->entries && t->ent_off[n]) || (!t->bytes && t->byte_off[n])) {
+        bm25x_set_error("%s: null argument", who);
+        return BM25X_ERR_INVALID;
+    }
+    // per vector: 0 = valid, else 1 + the fault (1 lexeme past the area, 2 count past the area, 3 no positions) and the
+    // entry (index inside the vector)
+    auto fault = [&](uint32_t v, uint64_t *entry) {
+        const uint64_t size = t->byte_off[v + 1] - t->byte_off[v];
+        for (uint64_t j = t->ent_off[v]; j < t->ent_off[v + 1]; j++) {
+            const uint32_t e = t->entries[j], len = (e >> 1) & 0x7FFu, pos = e >> 12;
+            *entry = j - t->ent_off[v];
+            if ((uint64_t)pos + len > size) return 1;
+            if (e & 1u) {
+                if ((((uint64_t)pos + len + 1) & ~1ull) + 2 > size) return 2;
+            } else if (!as_query) {
+                return 3;
+            }
+        }
+        return 0;
+    };
+    uint32_t first = 0xFFFFFFFFu;
+#pragma omp parallel for schedule(dynamic, 1024) reduction(min : first) num_threads(bm25x_host_threads(0))
+    for (uint32_t v = 0; v < n; v++) {
+        uint64_t j;
+        if (fault(v, &j)) first = std::min(first, v);
+    }
+    if (first == 0xFFFFFFFFu) return BM25X_OK;
+    uint64_t j = 0;
+    const int f = fault(first, &j);
+    const unsigned long long jj = (unsigned long long)j;
+    if (f == 1) bm25x_set_error("%s: invalid data: the lexeme of entry %llu of tsvector %u runs past its area", who, jj, first);
+    else if (f == 2)
+        bm25x_set_error("%s: invalid data: the position count of entry %llu of tsvector %u runs past its area", who, jj, first);
+    else bm25x_set_error("%s: invalid data: tsvector must have positions (entry %llu of tsvector %u)", who, jj, first);
+    return BM25X_ERR_INVALID;
+}
+
+// The cast of every vector on the current device.  Outputs held on the device: document mode the keyed CSR (raw keys
+// key[E'], tf[E']), query mode the keys, or (vocab given) the keys' ordinals ord[E'].  Host: off[n+1] the rows, len[n]
+// the saturating Σ tf of each row (document mode), and the first vector with a merged tf of 0 / >= 2^24.
+struct Cast {
+    Scratch sc;
+    ulonglong2 *key = nullptr;
+    uint32_t *tf = nullptr, *ord = nullptr;
+    std::vector<uint64_t> off;
+    std::vector<uint32_t> len;
+    uint32_t zero = 0xFFFFFFFFu, big = 0xFFFFFFFFu;
+    explicit Cast(int device) : sc(device) {}
+};
+
+int run_cast(const char *who, const bm25x_tsvectors *t, const uint8_t seed[32], int as_query, bool want_keys,
+             const Key128 *vocab, uint32_t T, Cast &c) {
+    Scratch &sc = c.sc;
+    const uint32_t n = t->n;
+    const uint64_t E = t->ent_off[n];
+    // the chunks: whole vectors, at most CHUNK_ENT entries, CHUNK_BYTES bytes and CHUNK_VEC vectors, or one vector
+    std::vector<uint32_t> cuts{0};
+    while (cuts.back() < n) {
+        const uint32_t a = cuts.back();
+        uint32_t b = a + 1;
+        while (b < n && b - a < CHUNK_VEC && t->ent_off[b + 1] - t->ent_off[a] <= CHUNK_ENT &&
+               t->byte_off[b + 1] - t->byte_off[a] <= CHUNK_BYTES)
+            b++;
+        cuts.push_back(b);
+    }
+    uint64_t ce = 0, cb = 0, cv = 0;
+    for (size_t k = 0; k + 1 < cuts.size(); k++) {
+        ce = std::max(ce, t->ent_off[cuts[k + 1]] - t->ent_off[cuts[k]]);
+        cb = std::max(cb, t->byte_off[cuts[k + 1]] - t->byte_off[cuts[k]]);
+        cv = std::max<uint64_t>(cv, cuts[k + 1] - cuts[k]);
+    }
+    if (ce > 0x7FFFFFFFull) {
+        bm25x_set_error("%s: a tsvector of %llu entries, more than the 2^31 - 1 one sort takes", who,
+                        (unsigned long long)ce);
+        return BM25X_ERR_UNSUPPORTED;
+    }
+    Seed sd;
+    for (int i = 0; i < 8; i++)
+        sd.w[i] = (uint32_t)seed[4 * i] | (uint32_t)seed[4 * i + 1] << 8 | (uint32_t)seed[4 * i + 2] << 16 |
+                  (uint32_t)seed[4 * i + 3] << 24;
+    sc.e = cudaSetDevice(sc.device);
+    if (want_keys) c.key = sc.alloc<ulonglong2>(E);
+    if (!as_query) c.tf = sc.alloc<uint32_t>(E);
+    if (vocab) c.ord = sc.alloc<uint32_t>(E);
+    uint32_t *rows = sc.alloc<uint32_t>(n), *flags = sc.alloc<uint32_t>(2);
+    uint64_t *len = as_query ? nullptr : sc.alloc<uint64_t>(n);
+    Scratch tmp(sc.device);  // the chunk buffers, freed before the caller goes on
+    uint32_t *d_ent = tmp.alloc<uint32_t>(ce), *cnt[2] = {tmp.alloc<uint32_t>(ce), tmp.alloc<uint32_t>(ce)};
+    uint8_t *d_bytes = tmp.alloc<uint8_t>(cb);
+    uint64_t *d_eoff = tmp.alloc<uint64_t>(cv + 1), *d_boff = tmp.alloc<uint64_t>(cv + 1);
+    VKey *key[2] = {tmp.alloc<VKey>(ce), tmp.alloc<VKey>(ce)};
+    int64_t *d_runs = tmp.alloc<int64_t>(1);
+    size_t sort_bytes = 0, red_bytes = 0;
+    if (tmp.e == cudaSuccess && ce) {
+        cub::DoubleBuffer<VKey> k(key[0], key[1]);
+        cub::DoubleBuffer<uint32_t> v(cnt[0], cnt[1]);
+        tmp.e = cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, k, v, (int)ce, VKeyBits{}, 0, 160);
+        if (tmp.e == cudaSuccess)
+            tmp.e = cub::DeviceReduce::ReduceByKey(nullptr, red_bytes, key[0], key[1], cnt[0], cnt[1], d_runs, SatAdd{},
+                                                   (int)ce);
+    }
+    void *temp = tmp.alloc<uint8_t>(std::max(sort_bytes, red_bytes));
+    if (sc.e == cudaSuccess) sc.e = tmp.e;
+    if (sc.e == cudaSuccess) sc.e = cudaMemset(rows, 0, sizeof(uint32_t) * (size_t)n);
+    if (sc.e == cudaSuccess) sc.e = cudaMemset(flags, 0xFF, 2 * sizeof(uint32_t));
+    if (sc.e == cudaSuccess && len) sc.e = cudaMemset(len, 0, sizeof(uint64_t) * (size_t)n);
+    std::vector<uint64_t> h_eoff, h_boff;
+    uint64_t base = 0;
+    for (size_t k = 0; k + 1 < cuts.size() && sc.e == cudaSuccess; k++) {
+        const uint32_t a = cuts[k], b = cuts[k + 1], nv = b - a;
+        const uint64_t e0 = t->ent_off[a], ne = t->ent_off[b] - e0, b0 = t->byte_off[a], nb = t->byte_off[b] - b0;
+        if (ne == 0) continue;
+        h_eoff.resize(nv + 1);
+        h_boff.resize(nv + 1);
+        for (uint32_t u = 0; u <= nv; u++) {
+            h_eoff[u] = t->ent_off[a + u] - e0;
+            h_boff[u] = t->byte_off[a + u] - b0;
+        }
+        sc.e = cudaMemcpy(d_ent, t->entries + e0, sizeof(uint32_t) * ne, cudaMemcpyHostToDevice);
+        if (sc.e == cudaSuccess && nb) sc.e = cudaMemcpy(d_bytes, t->bytes + b0, nb, cudaMemcpyHostToDevice);
+        if (sc.e == cudaSuccess) sc.e = cudaMemcpy(d_eoff, h_eoff.data(), sizeof(uint64_t) * (nv + 1), cudaMemcpyHostToDevice);
+        if (sc.e == cudaSuccess) sc.e = cudaMemcpy(d_boff, h_boff.data(), sizeof(uint64_t) * (nv + 1), cudaMemcpyHostToDevice);
+        if (sc.e != cudaSuccess) break;
+        k_tsv_intern<<<grid_of(ne), TPB>>>(d_ent, ne, d_eoff, d_boff, nv, d_bytes, sd, as_query, key[0], cnt[0]);
+        if (as_query) sc.e = cudaMemsetAsync(cnt[0], 0, sizeof(uint32_t) * ne);  // no counts: the merge still needs values
+        if (sc.e == cudaSuccess) sc.e = cudaGetLastError();
+        const int vbits = nv > 1 ? 32 - __builtin_clz(nv - 1) : 1;
+        cub::DoubleBuffer<VKey> kd(key[0], key[1]);
+        cub::DoubleBuffer<uint32_t> vd(cnt[0], cnt[1]);
+        if (sc.e == cudaSuccess)
+            sc.e = cub::DeviceRadixSort::SortPairs(temp, sort_bytes, kd, vd, (int)ne, VKeyBits{}, 0, 128 + vbits);
+        VKey *ko = kd.Alternate();
+        uint32_t *vo = vd.Alternate();
+        if (sc.e == cudaSuccess)
+            sc.e = cub::DeviceReduce::ReduceByKey(temp, red_bytes, kd.Current(), ko, vd.Current(), vo, d_runs, SatAdd{},
+                                                  (int)ne);
+        if (sc.e == cudaSuccess) {
+            k_tsv_emit<<<grid_of(ne), TPB>>>(ko, vo, d_runs, a, base, as_query, c.key, c.tf, vocab, T, c.ord, rows, len,
+                                             flags);
+            sc.e = cudaGetLastError();
+        }
+        int64_t runs = 0;
+        if (sc.e == cudaSuccess) sc.e = cudaMemcpy(&runs, d_runs, sizeof(runs), cudaMemcpyDeviceToHost);
+        base += (uint64_t)runs;
+    }
+    std::vector<uint32_t> h_rows(n);
+    if (sc.e == cudaSuccess && n) sc.e = cudaMemcpy(h_rows.data(), rows, sizeof(uint32_t) * n, cudaMemcpyDeviceToHost);
+    uint32_t h_flags[2] = {0xFFFFFFFFu, 0xFFFFFFFFu};
+    if (sc.e == cudaSuccess) sc.e = cudaMemcpy(h_flags, flags, sizeof(h_flags), cudaMemcpyDeviceToHost);
+    std::vector<uint64_t> h_len(len ? n : 0);
+    if (sc.e == cudaSuccess && len && n) sc.e = cudaMemcpy(h_len.data(), len, sizeof(uint64_t) * n, cudaMemcpyDeviceToHost);
+    if (sc.e != cudaSuccess) return cuda_refusal(who, "tsvector cast", sc.e);
+    c.off.assign((size_t)n + 1, 0);
+    for (uint32_t v = 0; v < n; v++) c.off[v + 1] = c.off[v] + h_rows[v];
+    c.len.resize(h_len.size());
+    for (size_t v = 0; v < h_len.size(); v++) c.len[v] = (uint32_t)std::min<uint64_t>(h_len[v], 0xFFFFFFFFu);
+    c.zero = h_flags[0];
+    c.big = h_flags[1];
+    if (c.zero != 0xFFFFFFFFu) {  // Document::new (vector.rs:51-64): an element of value 0 is invalid data
+        bm25x_set_error("%s: invalid data: a lexeme of tsvector %u has position counts that sum to 0", who, c.zero);
+        return BM25X_ERR_INVALID;
+    }
+    return BM25X_OK;
+}
+
+bool null_seed_or_tsv(const char *who, const bm25x_tsvectors *t, const uint8_t *seed) {
+    if (t && seed) return false;
+    bm25x_set_error("%s: null argument", who);
+    return true;
+}
+
+}  // namespace
+
+extern "C" int bm25x_cast_tsvectors(const bm25x_tsvectors *tsv, const uint8_t seed[32], int as_query, int device,
+                                    uint64_t *out_off, uint8_t *out_key, uint32_t *out_tf) {
+    const char *who = "bm25x_cast_tsvectors";
+    if (null_seed_or_tsv(who, tsv, seed)) return BM25X_ERR_INVALID;
+    if (!out_off || !out_key || (!as_query && !out_tf)) {
+        bm25x_set_error("%s: null argument", who);
+        return BM25X_ERR_INVALID;
+    }
+    int rc = check_tsvectors(who, tsv, as_query);
+    if (rc == BM25X_OK) rc = check_device(who, device);
+    if (rc != BM25X_OK) return rc;
+    Cast c(device);
+    rc = run_cast(who, tsv, seed, as_query, true, nullptr, 0, c);
+    if (rc != BM25X_OK) return rc;
+    const uint64_t E = c.off[tsv->n];
+    cudaError_t e = cudaSuccess;
+    if (E) e = cudaMemcpy(out_key, c.key, 16 * E, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess && E && !as_query) e = cudaMemcpy(out_tf, c.tf, sizeof(uint32_t) * E, cudaMemcpyDeviceToHost);
+    if (e != cudaSuccess) return cuda_refusal(who, "tsvector cast", e);
+    memcpy(out_off, c.off.data(), sizeof(uint64_t) * c.off.size());
+    return BM25X_OK;
+}
+
+extern "C" int bm25x_index_create_from_tsvectors(const bm25x_tsvectors *tsv, const uint8_t seed[32],
+                                                 const uint16_t *payload, double k1, double b, int device,
+                                                 bm25x_index **out) {
+    const char *who = "bm25x_index_create_from_tsvectors";
+    if (out) *out = nullptr;
+    if (null_seed_or_tsv(who, tsv, seed) || !out) {
+        bm25x_set_error("%s: null argument", who);
+        return BM25X_ERR_INVALID;
+    }
+    int rc = check_tsvectors(who, tsv, 0);
+    if (rc == BM25X_OK) rc = check_common(who, tsv->n, tsv->ent_off, k1, b, 0);
+    if (rc != BM25X_OK && rc != BM25X_ERR_CUDA) return rc;
+    rc = check_device(who, device);
+    if (rc != BM25X_OK) return rc;
+    Cast c(device);
+    rc = run_cast(who, tsv, seed, 0, true, nullptr, 0, c);
+    if (rc != BM25X_OK) return rc;
+    if (c.big != 0xFFFFFFFFu) {
+        bm25x_set_error("%s: term frequency >= 2^24 is not supported by the packed posting layout (document %u)", who,
+                        c.big);
+        return BM25X_ERR_UNSUPPORTED;
+    }
+    // the keyed documents of the cast, on the device: ascending keys and non-zero tf by construction
+    bm25x_documents d{};
+    d.n_docs = tsv->n;
+    d.elem_off = c.off.data();
+    d.elem_key = reinterpret_cast<const uint8_t *>(c.key);
+    d.elem_tf = c.tf;
+    d.payload = payload;
+    d.k1 = k1;
+    d.b = b;
+    return documents_build(who, &d, c.len.data(), device, out);
+}
+
+extern "C" int bm25x_tsvector_queries(bm25x_index *ix, const uint8_t seed[32], const bm25x_tsvectors *tsv, uint32_t *q_off,
+                                      uint32_t *q_terms) {
+    const char *who = "bm25x_tsvector_queries";
+    if (null_seed_or_tsv(who, tsv, seed) || !ix || !q_off) {
+        bm25x_set_error("%s: null argument", who);
+        return BM25X_ERR_INVALID;
+    }
+    int rc = check_tsvectors(who, tsv, 1);
+    if (rc != BM25X_OK) return rc;
+    if (!q_terms && tsv->ent_off[tsv->n]) {
+        bm25x_set_error("%s: null argument", who);
+        return BM25X_ERR_INVALID;
+    }
+    const uint32_t T = ix->d.n_terms;
+    if (ix->h_keys.empty() && T) {  // replicas and keyless builds: bm25x_lookup_terms' refusal
+        bm25x_set_error("bm25x_lookup_terms: index was created without term keys");
+        return BM25X_ERR_INVALID;
+    }
+    BM25X_CUDA_TRY(cudaSetDevice(ix->device));
+    {   // the vocabulary as Key128, built once per handle and freed with it (bm25x_index_destroy)
+        std::lock_guard<std::mutex> lk(ix->key_vocab_mutex);
+        if (!ix->key_vocab) {
+            Scratch v(ix->device);
+            Key128 *p = v.alloc<Key128>(T);
+            if (v.e == cudaSuccess && T) v.e = cudaMemcpy(p, ix->h_keys.data(), 16 * (size_t)T, cudaMemcpyHostToDevice);
+            if (v.e == cudaSuccess && T) {
+                k_vocab_be<<<grid_of(T), TPB>>>(p, T);
+                v.e = cudaGetLastError();
+            }
+            if (v.e == cudaSuccess) v.e = cudaDeviceSynchronize();
+            if (v.e != cudaSuccess) return cuda_refusal(who, "vocabulary upload", v.e);
+            v.ptrs.clear();  // kept: the handle owns it now
+            ix->key_vocab = p;
+        }
+    }
+    Cast c(ix->device);
+    rc = run_cast(who, tsv, seed, 1, false, (const Key128 *)ix->key_vocab, T, c);
+    if (rc != BM25X_OK) return rc;
+    const uint64_t E = c.off[tsv->n];
+    if (E > 0xFFFFFFFFull) {
+        bm25x_set_error("%s: %llu query terms, more than the 2^32 - 1 that u32 offsets address", who,
+                        (unsigned long long)E);
+        return BM25X_ERR_UNSUPPORTED;
+    }
+    if (E) {
+        const cudaError_t e = cudaMemcpy(q_terms, c.ord, sizeof(uint32_t) * E, cudaMemcpyDeviceToHost);
+        if (e != cudaSuccess) return cuda_refusal(who, "tsvector cast", e);
+    }
+    for (uint32_t v = 0; v <= tsv->n; v++) q_off[v] = (uint32_t)c.off[v];
+    return BM25X_OK;
+}

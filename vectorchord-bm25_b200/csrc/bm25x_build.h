@@ -94,6 +94,12 @@ struct Scratch {
         if (e == cudaSuccess && n) e = cudaMemcpy(p, h, sizeof(T) * n, cudaMemcpyHostToDevice);
         return p;
     }
+    // p, one of this scratch's allocations, handed to a longer-lived owner that frees it: no longer freed here.
+    template <typename T>
+    T *release(T *p) {
+        ptrs.erase(std::find(ptrs.begin(), ptrs.end(), (void *)p));
+        return p;
+    }
 };
 
 // One handle's documents and terms, from whichever source (CSR columns, reference-format blocks, a shard of either, a
@@ -134,6 +140,8 @@ int cuda_refusal(const char *who, const char *step, cudaError_t e);
 int check_device(const char *who, int device);
 int check_common(const char *who, uint32_t n_docs, const void *doc_len, double k1, double b, int device);
 int check_keys(const char *who, const uint8_t *term_key, uint32_t T);
+// address_tokens::read: the ordinal of the 16-byte key in the strictly ascending keys[0..T), or BM25X_TERM_MISSING.
+uint32_t key_ordinal(const uint8_t *keys, uint32_t T, const uint8_t *key);
 int check_shard_args(uint32_t N, uint32_t S, const uint32_t *doc_bounds);
 std::vector<uint32_t> shard_bounds(const uint32_t *doc_bounds, const std::vector<uint64_t> &cum, uint32_t N,
                                    uint32_t S);

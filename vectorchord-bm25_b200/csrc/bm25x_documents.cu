@@ -27,18 +27,6 @@
 namespace {
 
 constexpr uint64_t CHUNK = 1ull << 22;  // elements per chunk
-constexpr unsigned TPB = 256;
-
-unsigned grid_of(uint64_t n) { return (unsigned)((n + TPB - 1) / TPB); }
-
-// Raw keys (as uploaded) → Key128 in place; cnt[i] = 1 when cnt is given (the vocabulary pass's appended entries).
-__global__ void k_keys_be(Key128 *__restrict__ keys, uint32_t *__restrict__ cnt, uint64_t n) {
-    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const ulonglong2 raw = reinterpret_cast<const ulonglong2 *>(keys)[i];
-    keys[i] = key_of(raw);
-    if (cnt) cnt[i] = 1u;
-}
 
 // Ordinal of each raw key of a chunk: its position in the sorted vocabulary (which holds every key of the documents);
 // idx[i] = i when idx is given.
@@ -46,15 +34,7 @@ __global__ void k_key_ordinals(const ulonglong2 *__restrict__ raw, uint64_t n, c
                                uint32_t *__restrict__ term, uint32_t *__restrict__ idx) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const Key128 k = key_of(raw[i]);
-    uint32_t lo = 0, hi = T;
-    while (lo < hi) {
-        const uint32_t mid = (lo + hi) >> 1;
-        const Key128 v = vocab[mid];
-        if (v.hi < k.hi || (v.hi == k.hi && v.lo < k.lo)) lo = mid + 1;
-        else hi = mid;
-    }
-    term[i] = lo;
+    term[i] = key_rank(vocab, T, key_of(raw[i]));
     if (idx) idx[i] = (uint32_t)i;
 }
 
@@ -146,17 +126,6 @@ cudaError_t load_ordinals(const bm25x_documents *c, uint64_t g, uint64_t n, cons
     if (e != cudaSuccess || !idx) return e;
     k_iota<<<grid_of(n), TPB>>>(idx, n);
     return cudaGetLastError();
-}
-
-// The sorted vocabulary (host bytes, T keys) on the current device, as Key128.
-const Key128 *upload_vocab(Scratch &sc, const std::vector<uint8_t> &keys, uint32_t T) {
-    Key128 *v = sc.alloc<Key128>(T);
-    if (sc.e == cudaSuccess && T) sc.e = cudaMemcpy(v, keys.data(), 16 * (size_t)T, cudaMemcpyHostToDevice);
-    if (sc.e == cudaSuccess && T) {
-        k_keys_be<<<grid_of(T), TPB>>>(v, nullptr, T);
-        sc.e = cudaGetLastError();
-    }
-    return v;
 }
 
 }  // namespace
@@ -301,11 +270,10 @@ static int vocab_pass(const char *who, const bm25x_documents *c, int device, std
     if (e == cudaSuccess && V) e = cudaMemcpy(df.data(), cb[0].p, sizeof(uint32_t) * V, cudaMemcpyDeviceToHost);
     if (e != cudaSuccess) return cuda_refusal(who, "vocabulary pass", e);
     keys.resize((size_t)V * 16);
-    for (uint64_t t = 0; t < V; t++)
-        for (int b = 0; b < 8; b++) {
-            keys[t * 16 + b] = (uint8_t)(h[t].hi >> (56 - 8 * b));
-            keys[t * 16 + 8 + b] = (uint8_t)(h[t].lo >> (56 - 8 * b));
-        }
+    for (uint64_t t = 0; t < V; t++) {
+        const ulonglong2 raw = raw_of(h[t]);
+        memcpy(&keys[t * 16], &raw, 16);
+    }
     return BM25X_OK;
 }
 

@@ -582,15 +582,10 @@ static int seal_segment(const char *who, bm25x_growing_segment *g, bm25x_seal_ar
                 bm25x_set_error("%s: new key %u equals new key %u", who, x, y);
                 return BM25X_ERR_INVALID;
             }
-        for (uint32_t i = 0; i < K; i++) {  // address_tokens::read over the sealed keys, as bm25x_lookup_terms
-            uint32_t lo = 0, hi = T;
-            while (lo < hi) {
-                const uint32_t mid = (lo + hi) >> 1;
-                if (memcmp(skeys + (size_t)mid * 16, key_of(T + i), 16) < 0) lo = mid + 1;
-                else hi = mid;
-            }
-            if (lo < T && memcmp(skeys + (size_t)lo * 16, key_of(T + i), 16) == 0) {
-                bm25x_set_error("%s: new key %u equals the key of sealed term %u", who, i, lo);
+        for (uint32_t i = 0; i < K; i++) {
+            const uint32_t t = key_ordinal(skeys, T, key_of(T + i));
+            if (t != BM25X_TERM_MISSING) {
+                bm25x_set_error("%s: new key %u equals the key of sealed term %u", who, i, t);
                 return BM25X_ERR_INVALID;
             }
         }

@@ -459,6 +459,16 @@ int check_keys(const char *who, const uint8_t *term_key, uint32_t T) {
     return BM25X_OK;
 }
 
+uint32_t key_ordinal(const uint8_t *keys, uint32_t T, const uint8_t *key) {
+    uint32_t lo = 0, hi = T;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (memcmp(keys + (size_t)mid * 16, key, 16) < 0) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo < T && memcmp(keys + (size_t)lo * 16, key, 16) == 0 ? lo : BM25X_TERM_MISSING;
+}
+
 // Environment overrides of the option defaults (test matrix: BM25X_SEED=0 / BM25X_TWOPHASE=1 run the same tests through
 // the other kernel paths); bm25x_index_set_option still wins.
 static void apply_env_options(bm25x_index *ix) {
@@ -997,16 +1007,6 @@ extern "C" int bm25x_lookup_terms(const bm25x_index *ix, const uint8_t *keys, ui
         bm25x_set_error("bm25x_lookup_terms: index was created without term keys");
         return BM25X_ERR_INVALID;
     }
-    const uint8_t *base = ix->h_keys.data();
-    for (uint32_t i = 0; i < n; i++) {
-        const uint8_t *key = keys + (size_t)i * 16;
-        uint32_t lo = 0, hi = ix->d.n_terms;
-        while (lo < hi) {
-            uint32_t mid = (lo + hi) >> 1;
-            if (memcmp(base + (size_t)mid * 16, key, 16) < 0) lo = mid + 1;
-            else hi = mid;
-        }
-        out[i] = (lo < ix->d.n_terms && memcmp(base + (size_t)lo * 16, key, 16) == 0) ? lo : BM25X_TERM_MISSING;
-    }
+    for (uint32_t i = 0; i < n; i++) out[i] = key_ordinal(ix->h_keys.data(), ix->d.n_terms, keys + (size_t)i * 16);
     return BM25X_OK;
 }

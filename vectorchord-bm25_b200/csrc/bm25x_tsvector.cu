@@ -26,9 +26,6 @@ namespace {
 constexpr uint64_t CHUNK_ENT = 1ull << 22;    // entries per upload chunk
 constexpr uint64_t CHUNK_BYTES = 1ull << 26;  // lexeme-area bytes per upload chunk
 constexpr uint64_t CHUNK_VEC = 1ull << 22;    // vectors per upload chunk (empty vectors cost no entry)
-constexpr unsigned TPB = 256;
-
-unsigned grid_of(uint64_t n) { return (unsigned)((n + TPB - 1) / TPB); }
 
 // ---- BLAKE3 keyed_hash, the first 16 bytes, of one lexeme of at most 2047 bytes (WordEntry.len has 11 bits) ----
 
@@ -216,21 +213,9 @@ __global__ void k_tsv_emit(const VKey *__restrict__ key, const uint32_t *__restr
         if (t >= (1u << 24)) atomicMin(&flags[1], v);
     }
     if (out_ord) {
-        uint32_t lo = 0, hi = T;
-        while (lo < hi) {
-            const uint32_t mid = (lo + hi) >> 1;
-            const Key128 w = vocab[mid];
-            if (w.hi < kk.hi || (w.hi == kk.hi && w.lo < kk.lo)) lo = mid + 1;
-            else hi = mid;
-        }
-        out_ord[base + i] = lo < T && vocab[lo] == kk ? lo : BM25X_TERM_MISSING;
+        const uint32_t t = key_rank(vocab, T, kk);
+        out_ord[base + i] = t < T && vocab[t] == kk ? t : BM25X_TERM_MISSING;
     }
-}
-
-// Raw keys → Key128 in place (an index's vocabulary as the lookups take it).
-__global__ void k_vocab_be(Key128 *__restrict__ keys, uint64_t n) {
-    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) keys[i] = key_of(reinterpret_cast<const ulonglong2 *>(keys)[i]);
 }
 
 // Every refusal of a batch of tsvectors that needs only the host (TsVectorBorrowed::iter's panics, tsvector.rs:55-71,
@@ -503,16 +488,10 @@ extern "C" int bm25x_tsvector_queries(bm25x_index *ix, const uint8_t seed[32], c
         std::lock_guard<std::mutex> lk(ix->key_vocab_mutex);
         if (!ix->key_vocab) {
             Scratch v(ix->device);
-            Key128 *p = v.alloc<Key128>(T);
-            if (v.e == cudaSuccess && T) v.e = cudaMemcpy(p, ix->h_keys.data(), 16 * (size_t)T, cudaMemcpyHostToDevice);
-            if (v.e == cudaSuccess && T) {
-                k_vocab_be<<<grid_of(T), TPB>>>(p, T);
-                v.e = cudaGetLastError();
-            }
+            Key128 *p = upload_vocab(v, ix->h_keys, T);
             if (v.e == cudaSuccess) v.e = cudaDeviceSynchronize();
             if (v.e != cudaSuccess) return cuda_refusal(who, "vocabulary upload", v.e);
-            v.ptrs.clear();  // kept: the handle owns it now
-            ix->key_vocab = p;
+            ix->key_vocab = v.release(p);
         }
     }
     Cast c(ix->device);

@@ -474,6 +474,39 @@ int bm25x_growing_search_candidates(bm25x_growing_segment *g, uint32_t nq, const
  * be NULL); valid until the next refresh or close.  Refused before the first refresh of a non-empty segment. */
 int bm25x_growing_get_index(const bm25x_growing_segment *g, bm25x_index_layout *layout, bm25x_index_derived *derived);
 void bm25x_growing_close(bm25x_growing_segment *g);
+/* aminsert of tsvectors (src/index/bm25/am/mod.rs:261-287: cast_tsvector_to_document, then bm25::insert): vector i
+ * becomes ordinal n_docs + i.  The call equals bm25x_growing_insert of the restated rows: the document cast of each vector
+ * (bm25x_cast_tsvectors); each key as the ordinal of the sealed vocabulary (bm25x_lookup_terms, df 0 terms included), else
+ * the ordinal an earlier insert numbered it with, else a fresh one: n_terms(sealed) + K + r, K = the keys the segment held
+ * before the call, r = the key's rank among the call's fresh keys ascending bytewise; each row ascending by ordinal with
+ * the merged counts as tf; the norm in the segment's form (doc_len = the saturating Σ tf, or in doc_fieldnorm form
+ * length_to_fieldnorm of it); payload as given (NULL: the synthetic ctid of the ordinal); no deleted flags.
+ * From its first successful call on the segment OWNS its keys: bm25x_growing_insert refuses an ordinal >= n_terms(sealed)
+ * other than BM25X_TERM_MISSING (BM25X_ERR_INVALID, naming the document and the ordinal), and the seal takes the
+ * segment's keys as new_keys (args->new_keys must be NULL and n_new_keys 0, else BM25X_ERR_INVALID; n_source_terms =
+ * n_terms(sealed) + K).  Refusals, before any device work: null arguments; the tsvectors' host refusals (document mode);
+ * a sealed side without term keys (bm25x_lookup_terms' message); a segment that took ordinals >= n_terms(sealed) from
+ * bm25x_growing_insert (BM25X_ERR_INVALID: its numbering is the caller's).  After the cast: a merged count of 0; more
+ * than 2^31 - 1 elements or tsvectors in one call (BM25X_ERR_UNSUPPORTED); then everything bm25x_growing_insert refuses
+ * for the restated rows, with its codes and messages.  A refused call changes nothing and leaves no device memory behind.
+ * Concurrency: tsvector inserts are serialised with each other (fresh keys are numbered in commit order), and hold the
+ * segment's lock only for the host insert and the key commit, so searches do not wait on their device work.  Device
+ * memory on the segment's device, held until the call returns: the document cast's figures (bm25x_cast_tsvectors),
+ * 32 B per element whose key the sealed vocabulary lacks (compacted, sort buffer), 4 B per distinct such key, 16 B per
+ * element for the re-sort by ordinal, and CUB's temporary storage; the sealed vocabulary, 16 B per sealed term, once per
+ * index (bm25x_tsvector_queries' copy) or, over a document-sharded index, once per segment until bm25x_growing_close.
+ * Host: 16 B per owned key plus a hash table entry, until close. */
+int bm25x_growing_insert_tsvectors(bm25x_growing_segment *g, const uint8_t seed[32], const bm25x_tsvectors *tsv,
+                                   const uint16_t *payload);
+/* The keys the segment numbered: *n_out = K and key i (of ordinal n_terms(sealed) + i) at keys_out + 16 i.  cap < K is
+ * refused (BM25X_ERR_INVALID) with *n_out set and nothing written.  K = 0 for a segment without tsvector inserts. */
+int bm25x_growing_get_new_keys(const bm25x_growing_segment *g, uint32_t cap, uint8_t *keys_out, uint32_t *n_out);
+/* Queries from tsvectors for the segment's searches: bm25x_tsvector_queries over the sealed side (an index: equal to
+ * that call on it; a document-sharded index: the query cast plus bm25x_sharded_lookup_terms), with its refusals, named by
+ * this call.  Keys the segment numbered are BM25X_TERM_MISSING: before the seal they never match (search.rs:60-62).
+ * Thread-safe alongside inserts and searches. */
+int bm25x_growing_tsvector_queries(bm25x_growing_segment *g, const uint8_t seed[32], const bm25x_tsvectors *tsv,
+                                   uint32_t *q_off, uint32_t *q_terms);
 
 /* ---- the seal (`maintain`, crates/bm25/src/maintain.rs:27-311, called from amvacuumcleanup): a NEW sealed index on the
  * sealed index's device from the sealed documents not marked deleted (ascending old id, relabelled densely) followed by

@@ -178,6 +178,9 @@ def load_library():
     L.bm25x_growing_seal.argtypes = [vp, C.POINTER(SealArgs), C.POINTER(vp)]
     L.bm25x_growing_open_sharded.argtypes = [vp, C.POINTER(vp)]
     L.bm25x_growing_seal_sharded.argtypes = [vp, C.POINTER(SealArgs), C.POINTER(vp)]
+    L.bm25x_growing_insert_tsvectors.argtypes = [vp, u8p, C.POINTER(_Tsvectors), u16p]
+    L.bm25x_growing_get_new_keys.argtypes = [vp, C.c_uint32, u8p, u32p]
+    L.bm25x_growing_tsvector_queries.argtypes = [vp, u8p, C.POINTER(_Tsvectors), u32p, u32p]
     L.bm25x_merge_topk.argtypes = [C.c_uint32, C.c_uint32, u32p, f32p, f64p, u16p, u32p, u32p, f32p, f64p, u16p, u32p,
                                    C.c_uint32, u32p, f32p, f64p, u16p, u32p]
     L.bm25x_index_destroy.argtypes = [vp]
@@ -765,6 +768,42 @@ class GrowingSegment:
         keep = []
         g = _growing_docs(keep, elem_off, elem_term, elem_tf, doc_len, doc_fieldnorm, payload, deleted)
         _check(load_library().bm25x_growing_insert(self.h, C.byref(g)))
+
+    def insert_tsvectors(self, seed, ent_off, entries, byte_off, data, payload=None):
+        """aminsert of tsvectors (bm25x_growing_insert_tsvectors): each vector cast on the GPU and appended as the next
+        ordinal; keys the sealed vocabulary lacks are numbered by the segment (new_keys) and keyed by the seal.  The
+        tsvectors as cast_tsvectors takes them; payload [n, 3] ctids or None."""
+        keep = []
+        t = _tsvectors(keep, ent_off, entries, byte_off, data)
+        pay = _kept(keep, payload, np.uint16, C.c_uint16) if payload is not None else None
+        _check(load_library().bm25x_growing_insert_tsvectors(self.h, _seed(seed), C.byref(t), pay))
+
+    def new_keys(self):
+        """The keys the segment numbered (bm25x_growing_get_new_keys): uint8 [K, 16], row i the key of token ordinal
+        sealed.n_terms + i."""
+        L = load_library()
+        n = C.c_uint32()
+        while True:  # tsvector inserts may add keys between the sizing call and the copy
+            keys = np.zeros((max(n.value, 1), 16), np.uint8)
+            cap = n.value
+            rc = L.bm25x_growing_get_new_keys(self.h, cap, _p(keys, C.c_uint8), C.byref(n))
+            if rc != 0 and n.value > cap:
+                continue
+            _check(rc)
+            return keys[:n.value].copy()
+
+    def tsvector_queries(self, seed, ent_off, entries, byte_off, data):
+        """Queries from tsvectors for this segment's searches (bm25x_growing_tsvector_queries), shaped as
+        Index.tsvector_queries: ordinals of the sealed vocabulary, TERM_MISSING for every other key (the segment's own
+        included, until the seal)."""
+        keep = []
+        t = _tsvectors(keep, ent_off, entries, byte_off, data)
+        E = int(keep[0][-1]) if len(keep[0]) else 0
+        q_off = np.zeros(t.n + 1, np.uint32)
+        q_terms = np.zeros(max(E, 1), np.uint32)
+        _check(load_library().bm25x_growing_tsvector_queries(self.h, _seed(seed), C.byref(t), _p(q_off, C.c_uint32),
+                                                             _p(q_terms, C.c_uint32)))
+        return q_off, q_terms[:int(q_off[-1])].copy()
 
     def delete(self, ordinals):
         o = np.ascontiguousarray(ordinals, dtype=np.uint32)

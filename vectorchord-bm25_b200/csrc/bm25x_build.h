@@ -6,7 +6,9 @@
 // the growing segment's create, refresh and seal (bm25x_growing.cu).
 #pragma once
 
+#include <functional>
 #include <memory>
+#include <mutex>
 #include <vector>
 
 #include "bm25x_common.h"
@@ -133,6 +135,33 @@ int upload_csr(bm25x_index *ix, const char *who, uint32_t T, uint64_t P, const u
 // may be device memory on `device` (the tsvector build's cast, bm25x_tsvector.cu); elem_off is host memory.  *out is
 // set on success; a CUDA failure is refused as `who`'s.
 int documents_build(const char *who, const bm25x_documents *c, const uint32_t *doc_len, int device, bm25x_index **out);
+
+// ---- the tsvector casts of a growing segment (bm25x_tsvector.cu) ----
+
+// The host refusals of a batch of tsvectors (bm25x_tsvectors), named by who; as_query: the query cast's.
+int check_tsvectors(const char *who, const bm25x_tsvectors *t, int as_query);
+// A sealed vocabulary (T sorted 16-byte keys) and where its device copy lives: uploaded to `device` on first use into
+// *slot under *mu, freed by the slot's owner.
+struct TsvVocab {
+    int device;
+    const std::vector<uint8_t> *keys;
+    uint32_t T;
+    void **slot;
+    std::mutex *mu;
+};
+// Rows of a cast: row i = ord / tf [off[i], off[i+1]); len[i] = the saturating Σ tf of row i (document mode).
+struct TsvRows {
+    std::vector<uint64_t> off;
+    std::vector<uint32_t> ord, tf, len;
+};
+// number(nu, keys, ord): ord[i] = the ordinal of keys[16 i .. 16 i + 16) (the keys ascending and distinct), or a refusal.
+using TsvNumbering = std::function<int(uint32_t nu, const uint8_t *keys, uint32_t *ord)>;
+// The cast of t (checked) on v.device with each key's ordinal in v's vocabulary.  Query mode: BM25X_TERM_MISSING where
+// the vocabulary lacks the key.  Document mode: the keys it lacks go to `number` once each, and every row comes back
+// ascending by ordinal with the tf of its merged counts; more than 2^31 - 1 elements or tsvectors is
+// BM25X_ERR_UNSUPPORTED.  Refusals: the cast's, number's, CUDA failures named by who.
+int tsvector_rows(const char *who, const TsvVocab &v, const uint8_t seed[32], const bm25x_tsvectors *t, int as_query,
+                  const TsvNumbering &number, TsvRows &out);
 
 // ---- host checks and helpers shared by the builders, with the messages their refusals give ----
 

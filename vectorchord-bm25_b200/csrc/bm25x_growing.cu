@@ -1,11 +1,14 @@
 // bm25x_growing.cu — the growing segment (DESIGN §4.5): the one-shot handle of bm25x_growing_create, the mutable segment
 // with its inserts, deletes, refresh and search, and the seal into a new sealed index.  Every handle is built by the
-// contract of bm25x_build.h; the refresh and the seal splice with the kernels of bm25x_splice.cuh.
+// contract of bm25x_build.h; the refresh and the seal splice with the kernels of bm25x_splice.cuh.  Tsvector inserts
+// cast on the device (tsvector_rows, bm25x_tsvector.cu); the segment numbers the keys its sealed side lacks and hands
+// them to its seal.
 #include <string.h>
 
 #include <algorithm>
 #include <chrono>
 #include <memory>
+#include <unordered_map>
 #include <unordered_set>
 
 #include "bm25x_build.h"
@@ -168,6 +171,24 @@ extern "C" int bm25x_growing_create(const bm25x_index *sealed, const bm25x_growi
     return BM25X_OK;
 }
 
+// A 16-byte term key as two words, the key of the segment's key dictionary.
+struct Key16 {
+    uint64_t a, b;
+    bool operator==(const Key16 &o) const { return a == o.a && b == o.b; }
+};
+struct Key16Hash {
+    size_t operator()(const Key16 &k) const {
+        const uint64_t h = (k.a ^ (k.b * 0x9E3779B97F4A7C15ull)) * 0xBF58476D1CE4E5B9ull;
+        return (size_t)(h ^ (h >> 31));
+    }
+};
+static Key16 key16(const uint8_t *p) {
+    Key16 k;
+    memcpy(&k.a, p, 8);
+    memcpy(&k.b, p + 8, 8);
+    return k;
+}
+
 // ---- the mutable growing segment (DESIGN §4.5): the documents on the host as the reference's VectorTuples keep them
 // (norm, payload, deleted bit), their postings in one index handle on the sealed side's home device, brought up to date
 // by a refresh ----
@@ -197,9 +218,31 @@ struct bm25x_growing_segment {
     // the current handle over ordinals [0, n_indexed); a running search keeps its own reference, so that a refresh can
     // replace it meanwhile and the last holder destroys it
     std::shared_ptr<bm25x_index> cur;
+    // the keys the segment numbered (bm25x_growing_insert_tsvectors): key i has ordinal n_terms(sealed) + i.  The segment
+    // owns its keys from its first tsvector insert on.  num_mu is held across a whole tsvector insert, so that keys are
+    // numbered in commit order; the keys change under both locks.
+    std::mutex num_mu;
+    bool owns_keys = false;
+    std::vector<uint8_t> new_keys;
+    std::unordered_map<Key16, uint32_t, Key16Hash> key_ord;
+    // a sharded side's vocabulary on the home device (an index keeps its own, bm25x_index.key_vocab)
+    std::mutex vocab_mu;
+    void *key_vocab = nullptr;
 
     explicit bm25x_growing_segment(const SealedSide &s) : sealed(s), stats(s.stats()) {}
+    ~bm25x_growing_segment() {
+        if (!key_vocab) return;
+        cudaSetDevice(sealed.home().device);
+        cudaFree(key_vocab);
+    }
     uint32_t n_docs() const { return (uint32_t)deleted.size(); }
+    uint32_t n_keys() const { return (uint32_t)(new_keys.size() / 16); }
+    // the vocabulary tsvector_rows casts against
+    TsvVocab vocab() {
+        if (sealed.ix) return {sealed.ix->device, &sealed.ix->h_keys, sealed.ix->d.n_terms, &sealed.ix->key_vocab,
+                               &sealed.ix->key_vocab_mutex};
+        return {sealed.home().device, &sealed.keys(), sealed.n_terms(), &key_vocab, &vocab_mu};
+    }
 };
 
 extern "C" int bm25x_growing_open(bm25x_index *sealed, bm25x_growing_segment **out) {
@@ -232,12 +275,9 @@ extern "C" int bm25x_growing_open_sharded(bm25x_sharded_index *sealed, bm25x_gro
 
 extern "C" void bm25x_growing_close(bm25x_growing_segment *g) { delete g; }
 
-extern "C" int bm25x_growing_insert(bm25x_growing_segment *g, const bm25x_growing_docs *docs) {
-    if (!g || !docs) {
-        bm25x_set_error("bm25x_growing_insert: null argument");
-        return BM25X_ERR_INVALID;
-    }
-    std::lock_guard<std::mutex> lock(g->mu);
+// bm25x_growing_insert under g->mu.  sealed_only: every ordinal must be a sealed one or BM25X_TERM_MISSING (the segment
+// owns its keys).
+static int growing_insert_locked(bm25x_growing_segment *g, const bm25x_growing_docs *docs, bool sealed_only) {
     const int form = docs->doc_len ? 1 : docs->doc_fieldnorm ? 0 : -1;
     if (g->norm_form >= 0 && form >= 0 && form != g->norm_form) {
         bm25x_set_error("bm25x_growing_insert: documents with %s into a segment whose documents carry %s",
@@ -248,6 +288,16 @@ extern "C" int bm25x_growing_insert(bm25x_growing_segment *g, const bm25x_growin
     GrowingCsr csr;
     const int rc = invert_growing(g->sealed, docs, first, csr);
     if (rc != BM25X_OK) return rc;
+    for (uint32_t d = 0; sealed_only && d < G; d++)  // (invert_growing checked the offsets)
+        for (uint64_t e = docs->elem_off[d]; e < docs->elem_off[d + 1]; e++) {
+            const uint32_t t = docs->elem_term[e];
+            if (t >= g->sealed.n_terms() && t != BM25X_TERM_MISSING) {
+                bm25x_set_error("bm25x_growing_insert: document %u holds term ordinal %u >= n_terms(sealed)=%u, but the "
+                                "segment numbers its new terms itself (bm25x_growing_insert_tsvectors)", d, t,
+                                g->sealed.n_terms());
+                return BM25X_ERR_INVALID;
+            }
+        }
     g->norm_form = form;
     g->fieldnorm.resize((size_t)first + G);
     if (form) {
@@ -295,6 +345,142 @@ extern "C" int bm25x_growing_insert(bm25x_growing_segment *g, const bm25x_growin
         if (!form) g->sum_tf.push_back((uint32_t)std::min<uint64_t>(sum, 0xFFFFFFFFu));
     }
     g->pending = true;
+    return BM25X_OK;
+}
+
+extern "C" int bm25x_growing_insert(bm25x_growing_segment *g, const bm25x_growing_docs *docs) {
+    if (!g || !docs) {
+        bm25x_set_error("bm25x_growing_insert: null argument");
+        return BM25X_ERR_INVALID;
+    }
+    std::lock_guard<std::mutex> lock(g->mu);
+    return growing_insert_locked(g, docs, g->owns_keys);
+}
+
+// A segment that took ordinals >= n_terms(sealed) from bm25x_growing_insert cannot number keys itself (under g->mu).
+static int check_caller_numbered(const char *who, const bm25x_growing_segment *g) {
+    if (g->owns_keys || g->new_terms.empty()) return BM25X_OK;
+    bm25x_set_error("%s: the segment holds term ordinal %u >= n_terms(sealed)=%u from bm25x_growing_insert: its new terms "
+                    "are numbered by the caller", who, g->new_terms[0], g->sealed.n_terms());
+    return BM25X_ERR_INVALID;
+}
+
+// A sealed side without term keys: bm25x_lookup_terms' refusal (bm25x_sharded_lookup_terms gives the same).
+static int check_keyed(const SealedSide &s) {
+    if (!s.keys().empty() || !s.n_terms()) return BM25X_OK;
+    bm25x_set_error("bm25x_lookup_terms: index was created without term keys");
+    return BM25X_ERR_INVALID;
+}
+
+extern "C" int bm25x_growing_insert_tsvectors(bm25x_growing_segment *g, const uint8_t seed[32], const bm25x_tsvectors *tsv,
+                                              const uint16_t *payload) {
+    const char *who = "bm25x_growing_insert_tsvectors";
+    if (!g || !seed || !tsv) {
+        bm25x_set_error("%s: null argument", who);
+        return BM25X_ERR_INVALID;
+    }
+    int rc = check_tsvectors(who, tsv, 0);
+    if (rc == BM25X_OK) rc = check_keyed(g->sealed);
+    if (rc != BM25X_OK) return rc;
+    std::lock_guard<std::mutex> numbering(g->num_mu);
+    {
+        std::lock_guard<std::mutex> lock(g->mu);
+        rc = check_caller_numbered(who, g);
+        if (rc != BM25X_OK) return rc;
+    }
+    // the call's keys the sealed vocabulary lacks: the ordinal an earlier insert gave, or the next fresh one in key order
+    // (g->key_ord changes only under num_mu, held here)
+    const uint32_t T = g->sealed.n_terms(), K = g->n_keys();
+    std::vector<uint8_t> fresh;
+    auto number = [&](uint32_t nu, const uint8_t *keys, uint32_t *ord) {
+        for (uint32_t i = 0; i < nu; i++) {
+            const auto it = g->key_ord.find(key16(keys + (size_t)i * 16));
+            if (it != g->key_ord.end()) {
+                ord[i] = it->second;
+                continue;
+            }
+            const uint64_t t = (uint64_t)T + K + fresh.size() / 16;
+            if (t >= BM25X_TERM_MISSING) {
+                bm25x_set_error("%s: more than %u term ordinals (%u is BM25X_TERM_MISSING)", who, BM25X_TERM_MISSING,
+                                BM25X_TERM_MISSING);
+                return BM25X_ERR_UNSUPPORTED;
+            }
+            ord[i] = (uint32_t)t;
+            fresh.insert(fresh.end(), keys + (size_t)i * 16, keys + (size_t)i * 16 + 16);
+        }
+        return BM25X_OK;
+    };
+    TsvRows r;
+    rc = tsvector_rows(who, g->vocab(), seed, tsv, 0, number, r);
+    if (rc != BM25X_OK) return rc;
+    // the restated rows go in as bm25x_growing_insert takes them, with the norm in the segment's form
+    bm25x_growing_docs d{};
+    d.n_docs = tsv->n;
+    d.payload = payload;
+    d.elem_off = r.off.data();
+    d.elem_term = r.ord.data();
+    d.elem_tf = r.tf.data();
+    std::lock_guard<std::mutex> lock(g->mu);
+    std::vector<uint8_t> fn;
+    if (g->norm_form == 0) {
+        fn.resize(r.len.size());
+        for (size_t i = 0; i < fn.size(); i++) fn[i] = bm25x_length_to_fieldnorm(r.len[i]);
+        d.doc_fieldnorm = fn.data();
+    } else {
+        d.doc_len = r.len.data();
+    }
+    rc = check_caller_numbered(who, g);  // an ordinal insert may have come meanwhile
+    if (rc == BM25X_OK) rc = growing_insert_locked(g, &d, false);
+    if (rc != BM25X_OK) return rc;
+    for (size_t i = 0; i < fresh.size() / 16; i++) g->key_ord.emplace(key16(&fresh[i * 16]), (uint32_t)(T + K + i));
+    g->new_keys.insert(g->new_keys.end(), fresh.begin(), fresh.end());
+    g->owns_keys = true;
+    return BM25X_OK;
+}
+
+extern "C" int bm25x_growing_get_new_keys(const bm25x_growing_segment *g, uint32_t cap, uint8_t *keys_out, uint32_t *n_out) {
+    const char *who = "bm25x_growing_get_new_keys";
+    if (!g || !n_out || (cap && !keys_out)) {
+        bm25x_set_error("%s: null argument", who);
+        return BM25X_ERR_INVALID;
+    }
+    std::lock_guard<std::mutex> lock(g->mu);
+    const uint32_t K = g->n_keys();
+    *n_out = K;
+    if (cap < K) {
+        bm25x_set_error("%s: cap=%u below the segment's %u keys", who, cap, K);
+        return BM25X_ERR_INVALID;
+    }
+    if (K) memcpy(keys_out, g->new_keys.data(), g->new_keys.size());
+    return BM25X_OK;
+}
+
+extern "C" int bm25x_growing_tsvector_queries(bm25x_growing_segment *g, const uint8_t seed[32], const bm25x_tsvectors *tsv,
+                                              uint32_t *q_off, uint32_t *q_terms) {
+    const char *who = "bm25x_growing_tsvector_queries";
+    if (!g || !seed || !tsv || !q_off) {
+        bm25x_set_error("%s: null argument", who);
+        return BM25X_ERR_INVALID;
+    }
+    int rc = check_tsvectors(who, tsv, 1);
+    if (rc != BM25X_OK) return rc;
+    if (!q_terms && tsv->ent_off[tsv->n]) {
+        bm25x_set_error("%s: null argument", who);
+        return BM25X_ERR_INVALID;
+    }
+    rc = check_keyed(g->sealed);
+    if (rc != BM25X_OK) return rc;
+    // keys the segment numbered are not in the sealed vocabulary: BM25X_TERM_MISSING, as before the seal they never match
+    TsvRows r;
+    rc = tsvector_rows(who, g->vocab(), seed, tsv, 1, {}, r);
+    if (rc != BM25X_OK) return rc;
+    const uint64_t E = r.off[tsv->n];
+    if (E > 0xFFFFFFFFull) {
+        bm25x_set_error("%s: %llu query terms, more than the 2^32 - 1 that u32 offsets address", who, (unsigned long long)E);
+        return BM25X_ERR_UNSUPPORTED;
+    }
+    if (E) memcpy(q_terms, r.ord.data(), sizeof(uint32_t) * E);
+    for (uint32_t v = 0; v <= tsv->n; v++) q_off[v] = (uint32_t)r.off[v];
     return BM25X_OK;
 }
 
@@ -562,15 +748,18 @@ struct SealSnapshot {
 // until then bm25x_sharded_destroy holds it, so that a refusal frees every handle built so far.  Refusals and maps are
 // bm25x_growing_seal's, named by `who`.
 static int seal_segment(const char *who, bm25x_growing_segment *g, bm25x_seal_args *a, bm25x_sharded_index **out) {
-    const uint32_t NS = g->sealed.n_docs(), T = g->sealed.n_terms(), K = a->n_new_keys;
-    const bool keyed = !g->sealed.keys().empty();
-    // ---- the new keys: each unlike every sealed key and every other new key ----
+    const uint32_t NS = g->sealed.n_docs(), T = g->sealed.n_terms();
+    uint32_t K = a->n_new_keys;
+    bool keyed = !g->sealed.keys().empty();
+    // ---- the new keys: each unlike every sealed key and every other new key.  The caller's, or (taken with the
+    // snapshot below) those the segment owns, which are so by construction ----
     if (a->new_keys && !keyed) {
         bm25x_set_error("%s: new_keys given, but the sealed index was created without term keys", who);
         return BM25X_ERR_INVALID;
     }
-    const uint8_t *skeys = g->sealed.keys().data();
-    auto key_of = [&](uint32_t t) { return t < T ? skeys + (size_t)t * 16 : a->new_keys + (size_t)(t - T) * 16; };
+    const uint8_t *skeys = g->sealed.keys().data(), *nkeys = a->new_keys;
+    std::vector<uint8_t> owned;
+    auto key_of = [&](uint32_t t) { return t < T ? skeys + (size_t)t * 16 : nkeys + (size_t)(t - T) * 16; };
     auto key_less = [&](uint32_t x, uint32_t y) { return memcmp(key_of(x), key_of(y), 16) < 0; };
     if (K) {
         std::vector<uint32_t> order(K);
@@ -601,6 +790,17 @@ static int seal_segment(const char *who, bm25x_growing_segment *g, bm25x_seal_ar
     {
         std::lock_guard<std::mutex> lock(g->mu);
         const uint32_t NG = g->n_docs();
+        if (g->owns_keys) {
+            if (a->new_keys || a->n_new_keys) {
+                bm25x_set_error("%s: new_keys given, but the segment numbered its new terms itself "
+                                "(bm25x_growing_insert_tsvectors): it supplies their keys", who);
+                return BM25X_ERR_INVALID;
+            }
+            owned = g->new_keys;
+            nkeys = owned.data();
+            K = g->n_keys();
+            keyed = true;
+        }
         n_src = keyed ? T + K : std::max(T, g->term_end);
         if (keyed)
             for (uint32_t t : g->new_terms)

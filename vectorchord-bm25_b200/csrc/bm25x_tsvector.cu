@@ -11,12 +11,16 @@
 //      key's ordinal in an index's vocabulary), counts it into its vector's row and sums its vector's length.
 // Row offsets come from the row counts by a host scan once every chunk has run, so that a refused cast writes nothing.
 // The build from tsvectors hands the device-resident keyed CSR to the build from documents (documents_build): the keys
-// never travel to the host.
+// never travel to the host.  A growing segment's insert (tsvector_rows) numbers the keys its sealed vocabulary lacks:
+// k_tsv_missing compacts them, a radix sort and a unique give the call's distinct ones ascending, the host numbers
+// those, k_tsv_fresh hands each element its ordinal and a segmented sort puts every row back in ordinal order.
 #include <string.h>
 
 #include <algorithm>
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_reduce.cuh>
+#include <cub/device/device_segmented_sort.cuh>
+#include <cub/device/device_select.cuh>
 
 #include "bm25x_build.h"
 #include "bm25x_keys.cuh"
@@ -218,6 +222,32 @@ __global__ void k_tsv_emit(const VKey *__restrict__ key, const uint32_t *__restr
     }
 }
 
+// One thread per element of a document cast: the keys the vocabulary lacks (ord == BM25X_TERM_MISSING) as Key128,
+// appended at out[atomicAdd(n)] in any order (a sort follows); out == NULL counts them only.
+__global__ void k_tsv_missing(const ulonglong2 *__restrict__ key, const uint32_t *__restrict__ ord, uint64_t E,
+                              Key128 *__restrict__ out, uint32_t *__restrict__ n) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const bool miss = i < E && ord[i] == BM25X_TERM_MISSING;
+    const uint32_t b = __ballot_sync(0xFFFFFFFFu, miss);
+    if (!b) return;
+    const uint32_t lane = threadIdx.x & 31, leader = __ffs(b) - 1;
+    uint32_t at = 0;
+    if (lane == leader) at = atomicAdd(n, (uint32_t)__popc(b));
+    at = __shfl_sync(0xFFFFFFFFu, at, leader);
+    if (miss && out) out[at + __popc(b & ((1u << lane) - 1u))] = key_of(key[i]);
+}
+
+// One thread per element: a key the vocabulary lacks takes uord[its rank in u[0..nu)], the call's distinct missing keys
+// ascending.
+__global__ void k_tsv_fresh(const ulonglong2 *__restrict__ key, uint32_t *__restrict__ ord, uint64_t E,
+                            const Key128 *__restrict__ u, uint32_t nu, const uint32_t *__restrict__ uord) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= E || ord[i] != BM25X_TERM_MISSING) return;
+    ord[i] = uord[key_rank(u, nu, key_of(key[i]))];
+}
+
+}  // namespace
+
 // Every refusal of a batch of tsvectors that needs only the host (TsVectorBorrowed::iter's panics, tsvector.rs:55-71,
 // and "tsvector must have positions", tsvector.rs:88), named by who.
 int check_tsvectors(const char *who, const bm25x_tsvectors *t, int as_query) {
@@ -271,6 +301,8 @@ int check_tsvectors(const char *who, const bm25x_tsvectors *t, int as_query) {
     else bm25x_set_error("%s: invalid data: tsvector must have positions (entry %llu of tsvector %u)", who, jj, first);
     return BM25X_ERR_INVALID;
 }
+
+namespace {
 
 // The cast of every vector on the current device.  Outputs held on the device: document mode the keyed CSR (raw keys
 // key[E'], tf[E']), query mode the keys, or (vocab given) the keys' ordinals ord[E'].  Host: off[n+1] the rows, len[n]
@@ -406,7 +438,109 @@ bool null_seed_or_tsv(const char *who, const bm25x_tsvectors *t, const uint8_t *
     return true;
 }
 
+// v's vocabulary as Key128 on v.device, uploaded on first use and kept in *v.slot by its owner.  Leaves v.device current.
+int device_vocab(const char *who, const TsvVocab &v, const Key128 **out) {
+    cudaError_t e = cudaSetDevice(v.device);
+    if (e != cudaSuccess) return cuda_refusal(who, "vocabulary upload", e);
+    std::lock_guard<std::mutex> lk(*v.mu);
+    if (!*v.slot) {
+        Scratch s(v.device);
+        Key128 *p = upload_vocab(s, *v.keys, v.T);
+        if (s.e == cudaSuccess) s.e = cudaDeviceSynchronize();
+        if (s.e != cudaSuccess) return cuda_refusal(who, "vocabulary upload", s.e);
+        *v.slot = s.release(p);
+    }
+    *out = (const Key128 *)*v.slot;
+    return BM25X_OK;
+}
+
 }  // namespace
+
+int tsvector_rows(const char *who, const TsvVocab &v, const uint8_t seed[32], const bm25x_tsvectors *t, int as_query,
+                  const TsvNumbering &number, TsvRows &out) {
+    const Key128 *vocab = nullptr;
+    int rc = device_vocab(who, v, &vocab);
+    if (rc != BM25X_OK) return rc;
+    Cast c(v.device);
+    rc = run_cast(who, t, seed, as_query, !as_query, vocab, v.T, c);
+    if (rc != BM25X_OK) return rc;
+    const uint32_t n = t->n;
+    const uint64_t E = c.off[n];
+    Scratch &sc = c.sc;
+    uint32_t *ord = c.ord, *tf = c.tf;
+    if (!as_query) {
+        if (E > 0x7FFFFFFFull || n > 0x7FFFFFFFu) {  // the sorts below take int sizes
+            bm25x_set_error("%s: %llu elements in %u tsvectors, more than the 2^31 - 1 one insert sorts", who,
+                            (unsigned long long)E, n);
+            return BM25X_ERR_UNSUPPORTED;
+        }
+        // ---- the keys the vocabulary lacks: compacted, sorted and made distinct (U) ----
+        uint32_t *d_m = sc.alloc<uint32_t>(2), M = 0;
+        if (sc.e == cudaSuccess) sc.e = cudaMemset(d_m, 0, 2 * sizeof(uint32_t));
+        if (sc.e == cudaSuccess && E) {
+            k_tsv_missing<<<grid_of(E), TPB>>>(c.key, ord, E, nullptr, d_m);
+            sc.e = cudaGetLastError();
+        }
+        if (sc.e == cudaSuccess) sc.e = cudaMemcpy(&M, d_m, sizeof(M), cudaMemcpyDeviceToHost);
+        if (sc.e == cudaSuccess && M) {
+            Key128 *mk[2] = {sc.alloc<Key128>(M), sc.alloc<Key128>(M)};
+            cub::DoubleBuffer<Key128> kb(mk[0], mk[1]);
+            size_t sort_bytes = 0, uniq_bytes = 0;
+            if (sc.e == cudaSuccess)
+                sc.e = cub::DeviceRadixSort::SortKeys(nullptr, sort_bytes, kb, (int)M, Key128Bits{}, 0, 128);
+            if (sc.e == cudaSuccess) sc.e = cub::DeviceSelect::Unique(nullptr, uniq_bytes, mk[0], mk[1], d_m + 1, M);
+            void *temp = sc.alloc<uint8_t>(std::max(sort_bytes, uniq_bytes));
+            if (sc.e == cudaSuccess) sc.e = cudaMemset(d_m, 0, sizeof(uint32_t));
+            if (sc.e == cudaSuccess) {
+                k_tsv_missing<<<grid_of(E), TPB>>>(c.key, ord, E, mk[0], d_m);
+                sc.e = cudaGetLastError();
+            }
+            if (sc.e == cudaSuccess) sc.e = cub::DeviceRadixSort::SortKeys(temp, sort_bytes, kb, (int)M, Key128Bits{}, 0, 128);
+            Key128 *u = kb.Alternate();
+            if (sc.e == cudaSuccess) sc.e = cub::DeviceSelect::Unique(temp, uniq_bytes, kb.Current(), u, d_m + 1, M);
+            uint32_t nu = 0;
+            if (sc.e == cudaSuccess) sc.e = cudaMemcpy(&nu, d_m + 1, sizeof(nu), cudaMemcpyDeviceToHost);
+            std::vector<Key128> h_u(nu);
+            if (sc.e == cudaSuccess) sc.e = cudaMemcpy(h_u.data(), u, sizeof(Key128) * nu, cudaMemcpyDeviceToHost);
+            if (sc.e != cudaSuccess) return cuda_refusal(who, "tsvector cast", sc.e);
+            // ---- their ordinals, from the caller ----
+            std::vector<uint8_t> raw((size_t)nu * 16);
+            for (uint32_t i = 0; i < nu; i++) {
+                const ulonglong2 r = raw_of(h_u[i]);
+                memcpy(&raw[(size_t)i * 16], &r, 16);
+            }
+            std::vector<uint32_t> uord(nu);
+            rc = number(nu, raw.data(), uord.data());
+            if (rc != BM25X_OK) return rc;
+            const uint32_t *d_uord = sc.up(uord.data(), nu);
+            if (sc.e == cudaSuccess) {
+                k_tsv_fresh<<<grid_of(E), TPB>>>(c.key, ord, E, u, nu, d_uord);
+                sc.e = cudaGetLastError();
+            }
+            // ---- each row re-sorted by ordinal (only rows with a missing key can be out of order) ----
+            const uint64_t *d_off = sc.up(c.off.data(), (size_t)n + 1);
+            uint32_t *ord2 = sc.alloc<uint32_t>(E), *tf2 = sc.alloc<uint32_t>(E);
+            size_t seg_bytes = 0;
+            if (sc.e == cudaSuccess)
+                sc.e = cub::DeviceSegmentedSort::SortPairs(nullptr, seg_bytes, ord, ord2, tf, tf2, (int)E, (int)n, d_off,
+                                                          d_off + 1);
+            void *seg_temp = sc.alloc<uint8_t>(seg_bytes);
+            if (sc.e == cudaSuccess)
+                sc.e = cub::DeviceSegmentedSort::SortPairs(seg_temp, seg_bytes, ord, ord2, tf, tf2, (int)E, (int)n, d_off,
+                                                          d_off + 1);
+            ord = ord2;
+            tf = tf2;
+        }
+        out.tf.resize(E);
+        if (sc.e == cudaSuccess && E) sc.e = cudaMemcpy(out.tf.data(), tf, sizeof(uint32_t) * E, cudaMemcpyDeviceToHost);
+        out.len = std::move(c.len);
+    }
+    out.ord.resize(E);
+    if (sc.e == cudaSuccess && E) sc.e = cudaMemcpy(out.ord.data(), ord, sizeof(uint32_t) * E, cudaMemcpyDeviceToHost);
+    if (sc.e != cudaSuccess) return cuda_refusal(who, "tsvector cast", sc.e);
+    out.off = std::move(c.off);
+    return BM25X_OK;
+}
 
 extern "C" int bm25x_cast_tsvectors(const bm25x_tsvectors *tsv, const uint8_t seed[32], int as_query, int device,
                                     uint64_t *out_off, uint8_t *out_key, uint32_t *out_tf) {
@@ -483,19 +617,12 @@ extern "C" int bm25x_tsvector_queries(bm25x_index *ix, const uint8_t seed[32], c
         bm25x_set_error("bm25x_lookup_terms: index was created without term keys");
         return BM25X_ERR_INVALID;
     }
-    BM25X_CUDA_TRY(cudaSetDevice(ix->device));
-    {   // the vocabulary as Key128, built once per handle and freed with it (bm25x_index_destroy)
-        std::lock_guard<std::mutex> lk(ix->key_vocab_mutex);
-        if (!ix->key_vocab) {
-            Scratch v(ix->device);
-            Key128 *p = upload_vocab(v, ix->h_keys, T);
-            if (v.e == cudaSuccess) v.e = cudaDeviceSynchronize();
-            if (v.e != cudaSuccess) return cuda_refusal(who, "vocabulary upload", v.e);
-            ix->key_vocab = v.release(p);
-        }
-    }
+    // the vocabulary as Key128, built once per handle and freed with it (bm25x_index_destroy)
+    const Key128 *vocab = nullptr;
+    rc = device_vocab(who, {ix->device, &ix->h_keys, T, &ix->key_vocab, &ix->key_vocab_mutex}, &vocab);
+    if (rc != BM25X_OK) return rc;
     Cast c(ix->device);
-    rc = run_cast(who, tsv, seed, 1, false, (const Key128 *)ix->key_vocab, T, c);
+    rc = run_cast(who, tsv, seed, 1, false, vocab, T, c);
     if (rc != BM25X_OK) return rc;
     const uint64_t E = c.off[tsv->n];
     if (E > 0xFFFFFFFFull) {

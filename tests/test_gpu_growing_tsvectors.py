@@ -10,104 +10,12 @@ import numpy as np
 import pytest
 
 from util_cuda import free_bytes
-from util_index import DERIVED, LAYOUT, fieldnorms, read_back
+from util_growing_tsvector import MISSING, SEED, Twin, bm_of, same_seal, same_segment
+from util_index import fieldnorms, read_back
 from util_lib import gpu_library, refused  # noqa: F401  (gpu_library: the module fixture m)
-from util_parity import same_rows
 from util_tsvector import cast, pack_ids, pack_sorted, synthetic, word_table, write_tsvectors
 
 pytestmark = pytest.mark.gpu
-
-SEED = bytes((5 * i + 11) & 0xFF for i in range(32))
-KS = (1, 10, 128, 1025)
-MISSING = 0xFFFFFFFF
-
-
-def _bm(m):
-    return __import__(m.__name__ + ".bm25x", fromlist=["x"])
-
-
-class Twin:
-    """The restated inserts on a second segment over the same sealed side."""
-
-    def __init__(self, m, sealed):
-        self.m, self.sealed, self.T = m, sealed, sealed.n_terms
-        self.seg = sealed.growing_segment()
-        self.keys = {}                      # key bytes -> ordinal, for the keys the sealed vocabulary lacks
-
-    def rows(self, tsv):
-        off, keys, tf = cast(_bm(self.m).intern, SEED, tsv)
-        n = len(off) - 1
-        ords = self.sealed.lookup_terms(keys) if len(keys) else np.zeros(0, np.uint32)
-        miss = np.nonzero(ords == MISSING)[0]
-        fresh = sorted({bytes(keys[i]) for i in miss} - set(self.keys))
-        new = {k: self.T + len(self.keys) + r for r, k in enumerate(fresh)}
-        for i in miss:
-            k = bytes(keys[i])
-            ords[i] = self.keys[k] if k in self.keys else new[k]
-        vec = np.repeat(np.arange(n), np.diff(off.astype(np.int64)))
-        order = np.lexsort((ords, vec))
-        lens = np.bincount(vec, weights=tf.astype(np.float64), minlength=n) if len(vec) else np.zeros(n)
-        return off, ords[order], tf[order], np.minimum(lens, 0xFFFFFFFF).astype(np.uint32), new
-
-    def insert(self, orc, tsv, payload=None, form="doc_len"):
-        off, ords, tf, lens, new = self.rows(tsv)
-        norm = dict(doc_len=lens) if form == "doc_len" else dict(doc_fieldnorm=fieldnorms(orc, lens))
-        self.seg.insert(off, ords, tf, payload=payload, **norm)
-        self.keys.update(new)
-
-    def new_keys(self):
-        out = np.zeros((len(self.keys), 16), np.uint8)
-        for k, t in self.keys.items():
-            out[t - self.T] = np.frombuffer(k, np.uint8)
-        return out
-
-
-def _same_arrays(lay_a, der_a, lay_b, der_b, what):
-    a, b = read_back(lay_a, der_a), read_back(lay_b, der_b)
-    for name, _ in LAYOUT + DERIVED:
-        if (name in ("blk", "blk_ub") and lay_b.n_blocks == 0) or (name == "champ" and der_b.n_champ == 0):
-            continue
-        assert a[name].tobytes() == b[name].tobytes(), f"{what}: {name} differs"
-
-
-def _same_segment(seg, twin, queries, what):
-    """Arrays, info, keys and search rows of seg equal the twin's."""
-    assert np.array_equal(seg.new_keys(), twin.new_keys()), f"{what}: new keys"
-    seg.refresh()
-    twin.seg.refresh()
-    a, b = seg.info(), twin.seg.info()
-    for f, _ in type(b)._fields_:
-        assert getattr(a, f) == getattr(b, f), f"{what}: info.{f}"
-    if a.n_docs:
-        _same_arrays(*seg.arrays(), *twin.seg.arrays(), what)
-    q_off, q_terms = seg.tsvector_queries(SEED, **queries)
-    for k in KS:
-        same_rows(seg.search_batch(q_off, q_terms, k, want_payload=True),
-                  twin.seg.search_batch(q_off, q_terms, k, want_payload=True), f"{what} k={k}")
-
-
-def _same_seal(got, want, what):
-    """Two seals: maps, info, and every handle's arrays (each shard's for a sharded index)."""
-    ix_a, ix_b = got[0], want[0]
-    for x, y, name in zip(got[1:], want[1:], ("sealed_map", "growing_map", "term_map")):
-        assert np.array_equal(x, y), f"{what}: {name}"
-    a, b = ix_a.info(), ix_b.info()
-    for f, _ in type(b)._fields_:
-        assert getattr(a, f) == getattr(b, f), f"{what}: info.{f}"
-    if hasattr(ix_b, "shard_arrays"):
-        assert np.array_equal(ix_a.doc_bounds(), ix_b.doc_bounds()), what
-        for s in range(len(ix_b.doc_bounds()) - 1):
-            _same_arrays(*ix_a.shard_arrays(s), *ix_b.shard_arrays(s), f"{what} shard {s}")
-    else:
-        _same_arrays(ix_a.layout(), ix_a.derived(), ix_b.layout(), ix_b.derived(), what)
-    rng = np.random.default_rng(3)
-    T = a.n_terms
-    qs = [rng.choice(T, size=min(T, int(rng.integers(1, 6))), replace=False) for _ in range(40)]
-    q_off = np.cumsum([0] + [len(q) for q in qs]).astype(np.uint32)
-    q_terms = np.array([t for q in qs for t in q], np.uint32)
-    for k in KS:
-        same_rows(ix_a.search_batch(q_off, q_terms, k, want_payload=True),
-                  ix_b.search_batch(q_off, q_terms, k, want_payload=True), f"{what} sealed k={k}")
 
 
 # ---- the sealed sides ----
@@ -124,7 +32,7 @@ def _sealed(m, kind, rng):
     tsv = pack_sorted(docs)
     if kind == "index":
         return m.Index.from_tsvectors(SEED, **tsv), words
-    off, keys, tf = cast(_bm(m).intern, SEED, tsv)
+    off, keys, tf = cast(bm_of(m).intern, SEED, tsv)
     return m.ShardedIndex.from_documents(off, tf, elem_key=keys, n_shards=int(kind[-1])), words
 
 
@@ -176,25 +84,25 @@ def test_script_equals_twin_and_seals_alike(m, orc, kind, form):
             dead = rng.choice(seg.info().n_docs, size=3, replace=False).astype(np.uint32)
             seg.delete(dead)
             twin.seg.delete(dead)
-        _same_segment(seg, twin, _queries(rng, words, fresh), f"{kind} {form} step {step}")
+        same_segment(seg, twin, _queries(rng, words, fresh), f"{kind} {form} step {step}")
     # queries: the sealed side's own, with the segment's keys missing
     q = _queries(rng, words, fresh)
     q_off, q_terms = seg.tsvector_queries(SEED, **q)
     if kind == "index":
         w_off, w_terms = sealed.tsvector_queries(SEED, **q)
     else:
-        off, keys, _ = cast(_bm(m).intern, SEED, q, as_query=True)
+        off, keys, _ = cast(bm_of(m).intern, SEED, q, as_query=True)
         w_off, w_terms = off.astype(np.uint32), sealed.lookup_terms(keys)
     assert np.array_equal(q_off, w_off) and np.array_equal(q_terms, w_terms)
-    qo, qk, _ = cast(_bm(m).intern, SEED, q, as_query=True)
+    qo, qk, _ = cast(bm_of(m).intern, SEED, q, as_query=True)
     own = np.array([bytes(k) in twin.keys for k in qk], bool)
     assert own.any() and (q_terms[own] == MISSING).all()
     # the seal: the segment's keys against the caller's
     dele = np.packbits((np.arange(sealed.n_docs) % 7 == 3).astype(np.uint8), bitorder="little")
     got = seg.seal(sealed_deleted=dele)
     want = twin.seg.seal(sealed_deleted=dele, new_keys=twin.new_keys())
-    _same_seal(got, want, f"{kind} {form} seal")
-    doomed_keys = [bytes(k) for k in cast(_bm(m).intern, SEED, write_tsvectors([[(w, [1])] for w in doomed]))[1]]
+    same_seal(got, want, f"{kind} {form} seal")
+    doomed_keys = [bytes(k) for k in cast(bm_of(m).intern, SEED, write_tsvectors([[(w, [1])] for w in doomed]))[1]]
     assert all(got[3][twin.keys[k]] == MISSING for k in doomed_keys if k in twin.keys)
     assert len(got[3]) == sealed.n_terms + len(twin.keys)
 
@@ -223,14 +131,14 @@ def test_df0_sealed_key_and_large_batch(m, orc):
     seg.insert_tsvectors(SEED, **tsv)
     twin.insert(orc, tsv)
     assert len(twin.keys) == 1
-    _same_segment(seg, twin, tsv, "df0")
+    same_segment(seg, twin, tsv, "df0")
     # more than one cast chunk (2^22 entries), short and long lexemes
     big, bwords, _ = synthetic(rng, 150_000, 25, 35, 40_000, 0.02)
     assert int(big["ent_off"][-1]) > (1 << 22)
     seg.insert_tsvectors(SEED, **big)
     twin.insert(orc, big)
-    _same_segment(seg, twin, _queries(rng, short, bwords[:200]), "chunks")
-    _same_seal(seg.seal(), twin.seg.seal(new_keys=twin.new_keys()), "chunks seal")
+    same_segment(seg, twin, _queries(rng, short, bwords[:200]), "chunks")
+    same_seal(seg.seal(), twin.seg.seal(new_keys=twin.new_keys()), "chunks seal")
 
 
 def _expect_unchanged(seg, before, what):
@@ -245,7 +153,7 @@ def _state(seg):
 
 
 def test_refusals_change_nothing(m, orc):
-    bm = _bm(m)
+    bm = bm_of(m)
     L = m.load_library()
     rng = np.random.default_rng(8)
     sealed, words = _sealed(m, "index", rng)
@@ -327,10 +235,10 @@ def test_golden_end_to_end(m, orc, golden):
     seg.insert_tsvectors(SEED, **tsv, payload=pay[h:])
     twin.insert(orc, tsv, payload=pay[h:])
     query = pack_sorted([{golden["query"].encode(): [1]}])
-    _same_segment(seg, twin, query, "golden")
+    same_segment(seg, twin, query, "golden")
     ix, smap, gmap, tmap = seg.seal()
     full = m.Index.from_tsvectors(SEED, **_golden_tsvectors(golden, half + rest), payload=pay)
-    _same_seal((ix, smap, gmap, tmap), twin.seg.seal(new_keys=twin.new_keys()), "golden seal")
+    same_seal((ix, smap, gmap, tmap), twin.seg.seal(new_keys=twin.new_keys()), "golden seal")
     # the seal holds every passage, in id order: the query finds the passages the full build finds (a sealed survivor's
     # length is its number of postings, maintain.rs:356-360, so scores may differ from the full build's)
     assert ix.info().n_docs == full.info().n_docs == n and np.array_equal(tmap[:sealed.n_terms] != MISSING,
@@ -397,7 +305,7 @@ def test_concurrent_inserts(m, orc):
     assert len(got) == len(keys)
     want = set()
     for t in batches:
-        _, ks, _ = cast(_bm(m).intern, SEED, t)
+        _, ks, _ = cast(bm_of(m).intern, SEED, t)
         look = sealed.lookup_terms(ks)
         want |= {bytes(k) for k, o in zip(ks, look) if o == MISSING}
     assert got == want
@@ -405,5 +313,5 @@ def test_concurrent_inserts(m, orc):
     twin = Twin(m, sealed)
     for i in order:
         twin.insert(orc, batches[i], payload=tags[i])
-    _same_segment(seg, twin, q, "concurrent")
-    _same_seal(seg.seal(), twin.seg.seal(new_keys=twin.new_keys()), "concurrent seal")
+    same_segment(seg, twin, q, "concurrent")
+    same_seal(seg.seal(), twin.seg.seal(new_keys=twin.new_keys()), "concurrent seal")

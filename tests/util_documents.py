@@ -62,6 +62,34 @@ def segment(elem_off, elem_tf, elem_term=None, elem_key=None, n_terms=0):
                            post_doc=doc[order], post_tf=tf[order], term_keys=keys)
 
 
+CHUNK = 1 << 22  # elements per chunk of the device build (bm25x_documents.cu)
+
+
+def vocab_schedule(elem_key):
+    """The restated loop of vocab_pass over keyed elements: one event per chunk c, in order, ("grow", c, capacity,
+    kept) when the list is reallocated keeping its first `kept` entries, then ("defer", c, A) or ("compact", c, A) with
+    A the appended entries the chunk leaves.  A compaction leaves V = the distinct keys of every element so far, counted
+    from each key's first occurrence."""
+    E = len(elem_key)
+    _, ordinal = vocabulary(elem_key)
+    first = np.full(int(ordinal.max()) + 1 if E else 0, E, np.int64)
+    np.minimum.at(first, ordinal, np.arange(E, dtype=np.int64))
+    first.sort()
+    events, V, A, cap = [], 0, 0, 0
+    for c, g in enumerate(range(0, E, CHUNK)):
+        n = min(CHUNK, E - g)
+        if V + A + n > cap:
+            cap = 2 * (V + A + n)
+            events.append(("grow", c, cap, V + A))
+        A += n
+        if A >= max(V, CHUNK) or g + n == E:
+            events.append(("compact", c, A))
+            V, A = int(np.searchsorted(first, g + n)), 0
+        else:
+            events.append(("defer", c, A))
+    return events
+
+
 def csr_kwargs(s):
     """A segment() namespace as the keyword arguments of Index / ShardedIndex."""
     return dict(n_docs=s.n_docs, doc_len=s.doc_len, n_terms=s.n_terms, post_off=s.post_off, post_doc=s.post_doc,

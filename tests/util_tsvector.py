@@ -51,6 +51,20 @@ def pack_ids(vec_lens, word_flat, word_off, wid, npos):
     return dict(ent_off=ent_off, entries=entries, byte_off=byte_off, data=data)
 
 
+def assemble(vectors):
+    """A batch from (area u8, entries u32) per vector: the WordEntry words as given, each vector's lexeme area as given
+    (it may hold bytes no entry points at)."""
+    lens = [len(e) for _, e in vectors]
+    sizes = [len(a) for a, _ in vectors]
+    ent_off = np.zeros(len(vectors) + 1, np.uint64)
+    ent_off[1:] = np.cumsum(lens)
+    byte_off = np.zeros(len(vectors) + 1, np.uint64)
+    byte_off[1:] = np.cumsum(sizes)
+    entries = np.concatenate([np.asarray(e, np.uint32) for _, e in vectors]) if vectors else np.zeros(0, np.uint32)
+    data = np.concatenate([np.asarray(a, np.uint8) for a, _ in vectors]) if vectors else np.zeros(0, np.uint8)
+    return dict(ent_off=ent_off, entries=entries, byte_off=byte_off, data=data)
+
+
 def word_table(words):
     """A list of bytes as (flat u8, offsets [len + 1])."""
     off = np.zeros(len(words) + 1, np.int64)
@@ -139,6 +153,71 @@ def cast(intern, seed, tsv, as_query=False, keys=None):
         sums = np.add.reduceat(c, heads) if len(heads) else np.zeros(0, np.int64)
         tf = np.minimum(sums, 0xFFFFFFFF).astype(np.uint32)            # Saturating<u32>
     return off, ks[heads], tf
+
+
+CHUNK_ENT, CHUNK_BYTES, CHUNK_VEC = 1 << 22, 1 << 26, 1 << 22   # the cast's chunk limits (bm25x_tsvector.cu)
+
+
+def cast_cuts(tsv):
+    """The restated cut loop of run_cast: per chunk (a, b, rule, ne), vectors [a, b) holding ne entries, closed by
+    "end" (the batch), "vectors" (CHUNK_VEC of them), "single" (vector a alone exceeds a limit), "entries" or "bytes"
+    (vector b would take the chunk past CHUNK_ENT entries or CHUNK_BYTES lexeme-area bytes).  A chunk with ne == 0 is
+    skipped by the cast."""
+    ent = np.asarray(tsv["ent_off"], np.int64)
+    byt = np.asarray(tsv["byte_off"], np.int64)
+    n = len(ent) - 1
+    out, a = [], 0
+    while a < n:
+        # b = a + 1 + the vectors after a that fit: a prefix of a monotone test, found by binary search
+        stop = min(n, a + CHUNK_VEC)
+        b = a + 1
+        if b < stop:
+            lo = np.searchsorted(ent[b + 1:stop + 1], ent[a] + CHUNK_ENT, side="right")
+            hi = np.searchsorted(byt[b + 1:stop + 1], byt[a] + CHUNK_BYTES, side="right")
+            b += int(min(lo, hi))
+        if b == n:
+            rule = "end"
+        elif b - a == CHUNK_VEC:
+            rule = "vectors"
+        elif b == a + 1 and (ent[b] - ent[a] > CHUNK_ENT or byt[b] - byt[a] > CHUNK_BYTES):
+            rule = "single"
+        elif ent[b + 1] - ent[a] > CHUNK_ENT:
+            rule = "entries"
+        else:
+            rule = "bytes"
+        out.append((a, b, rule, int(ent[b] - ent[a])))
+        a = b
+    return out
+
+
+def byte_cut_batch(seed=21):
+    """Cut by bytes: areas of about 1 MiB (a few long lexemes, 1 000..2 047 bytes, at the front; the rest padding no entry
+    points into).  Chunk 0's 64 areas end exactly at CHUNK_BYTES; chunk 1's 64th vector would end one byte past it.
+    Returns (tsv, words, word id per entry)."""
+    rng = np.random.default_rng(seed)
+    words = list(dict.fromkeys(bytes(rng.integers(97, 123, int(rng.integers(1000, 2048)), dtype=np.uint8))
+                               for _ in range(300)))
+    M = 1 << 20
+    sizes = [M] * 64 + [M + 1] + [M] * 62 + [M] + [20_000, 0, 300_000, 0, 30_000]
+    vectors, wid_all = [], []
+    for v, size in enumerate(sizes):
+        if size == 0:
+            vectors.append((np.zeros(size, np.uint8), np.zeros(0, np.uint32)))
+            continue
+        k = int(rng.integers(1, 5 if size < M else 12))
+        wids = rng.choice(len(words), size=k, replace=False)
+        area, at = bytearray(), []
+        for w in wids:
+            at.append(len(area))
+            x = words[w]
+            area += x + (b"\0" if len(x) % 2 else b"") + int(rng.integers(1, 9)).to_bytes(2, "little")
+        assert len(area) <= size
+        area += bytes(size - len(area))
+        pick = rng.integers(0, k, int(rng.integers(20, 200)))
+        ents = np.array([(at[p] << 12) | (len(words[wids[p]]) << 1) | 1 for p in pick], np.uint32)
+        vectors.append((np.frombuffer(bytes(area), np.uint8), ents))
+        wid_all.append(wids[pick])
+    return assemble(vectors), words, np.concatenate(wid_all)
 
 
 def synthetic(rng, n, len_min, len_max, vocab, long_frac, max_pos=4, long_min=16, long_max=64):

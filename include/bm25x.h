@@ -646,7 +646,14 @@ int bm25x_check_vectors(uint32_t n, const uint32_t *off, const uint32_t *terms, 
 
 /* ---- bm25::evaluate (crates/bm25/src/evaluate.rs:22-74) behind `<&>` without an index scan
  * (src/index/operators.rs:22-55): pair p scores document [d_off[p], d_off[p+1]) (sorted distinct term ordinals
- * with tfs) against query [q_off[p], q_off[p+1]) (sorted distinct ordinals).  out[p] = positive f64 score. */
+ * with tfs) against query [q_off[p], q_off[p+1]) (sorted distinct ordinals).  out[p] = the f64 score, >= 0.
+ * It scores with the handle's own statistics: its N, df, avgdl, k1 and b.  The document's length is the saturating
+ * Σ tf (up to 2^32 - 1 per element and in sum), not a stored norm.  Query terms the document lacks, ordinals >= n_terms
+ * (BM25X_TERM_MISSING included) and terms of df 0 add nothing; a query has no term limit.  A replica's tables follow
+ * its latest bm25x_index_finalize_replica.
+ * BM25X_ERR_INVALID, writing nothing to out: a null argument, vectors that break bm25x_check_vectors, a replica not
+ * finalized, and a handle that scores with another segment's statistics (bm25x_growing_create's, or a replica of one;
+ * evaluate on the sealed index instead). */
 int bm25x_evaluate_batch(bm25x_index *idx, uint32_t n_pairs, const uint32_t *d_off, const uint32_t *d_terms,
                          const uint32_t *d_tfs, const uint32_t *q_off, const uint32_t *q_terms, double *out);
 

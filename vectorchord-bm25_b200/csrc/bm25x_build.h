@@ -63,6 +63,11 @@ struct Stats {
     Stats(uint32_t N, uint64_t sum_len, const uint32_t *df, uint32_t T, double k1, double b);
 };
 
+// Whether a handle scores with its own segment's statistics, avgdl = Σlen / N (flush.rs:52-66).  A handle of
+// bm25x_growing_create scores with the sealed segment's avgdl but holds its own documents' N, Σlen and df, and a replica
+// of one keeps that avgdl and Σlen through the layout.  The export and the evaluate refuse such handles.
+inline bool own_statistics(const bm25x_index *ix) { return ix->avgdl == (double)ix->sum_len / (double)ix->d.n_docs; }
+
 // A half-built handle: an early return destroys it, release() hands it out.
 struct IndexDestroy {
     void operator()(bm25x_index *ix) const { bm25x_index_destroy(ix); }

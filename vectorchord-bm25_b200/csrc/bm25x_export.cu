@@ -37,9 +37,9 @@ extern "C" int bm25x_index_export_blocks(const bm25x_index *ix, bm25x_export *ou
         bm25x_set_error("%s: replica not finalized", who);
         return BM25X_ERR_INVALID;
     }
-    // the Wand pairs flush writes use the segment's own avgdl = Σlen / N (flush.rs:52-66); a handle that scores with
-    // another segment's statistics (bm25x_growing_create's: the sealed segment's) has other s1 tables
-    if (!(ix->avgdl == (double)ix->sum_len / (double)N)) {
+    // the Wand pairs flush writes use the segment's own avgdl; a handle that scores with another segment's statistics
+    // has other s1 tables
+    if (!own_statistics(ix)) {
         bm25x_set_error("%s: the index scores with another segment's statistics (a growing handle); its Wand pairs would "
                         "not be the ones flush writes", who);
         return BM25X_ERR_INVALID;

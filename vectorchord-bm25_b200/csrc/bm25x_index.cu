@@ -937,6 +937,15 @@ extern "C" int bm25x_index_finalize_replica(bm25x_index *ix) {
     ix->h_df.resize(ix->d.n_terms);
     if (ix->d.n_terms)
         BM25X_CUDA_TRY(cudaMemcpy(ix->h_df.data(), ix->d.df, sizeof(uint32_t) * ix->d.n_terms, cudaMemcpyDeviceToHost));
+    {   // a refill brings another df: bm25x_evaluate_batch rebuilds its idf table from the new one on its next call (the
+        // fieldnorm -> length table depends on nothing and stays)
+        std::lock_guard<std::mutex> lk(ix->eval_mutex);
+        if (ix->eval_idf) {
+            ix->allocs.erase(std::find(ix->allocs.begin(), ix->allocs.end(), (void *)ix->eval_idf));
+            BM25X_CUDA_TRY(cudaFree(ix->eval_idf));
+            ix->eval_idf = nullptr;
+        }
+    }
     BM25X_CUDA_TRY(build_champions(ix));  // derived data: built here from the replicated arrays, on every call
     // s1f_min from the replicated arrays
     std::vector<uint8_t> h_fn(ix->d.n_docs);

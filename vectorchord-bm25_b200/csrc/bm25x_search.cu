@@ -797,27 +797,37 @@ extern "C" int bm25x_evaluate_batch(bm25x_index *ix, uint32_t n_pairs, const uin
         bm25x_set_error("bm25x_evaluate_batch: replica not finalized (bm25x_index_finalize_replica)");
         return BM25X_ERR_INVALID;
     }
+    // bm25::evaluate reads one segment's meta and tokens (evaluate.rs:22-74): a handle whose avgdl is another segment's
+    // while its N and df are its own matches no reference answer
+    if (!own_statistics(ix)) {
+        bm25x_set_error("bm25x_evaluate_batch: the index scores with another segment's statistics (a growing handle); "
+                        "evaluate on the sealed index");
+        return BM25X_ERR_INVALID;
+    }
     BM25X_CUDA_TRY(cudaSetDevice(ix->device));
     const uint32_t nd = d_off[n_pairs], nqt = q_off[n_pairs];
     const uint32_t T = ix->d.n_terms;
     {   // idf table (bm25.rs:285-289) with the host libm, like the reference's f64::ln, and the fieldnorm -> length table:
-        // they depend on the index alone — built once, kept on the device (freed with the handle)
+        // they depend on the index alone — built once, kept on the device (freed with the handle; the idf table is
+        // dropped by bm25x_index_finalize_replica and rebuilt here)
         std::lock_guard<std::mutex> lk(ix->eval_mutex);
+        if (!ix->eval_fn_len) {
+            uint32_t h_fn[256];
+            for (int f = 0; f < 256; ++f) h_fn[f] = bm25x_fieldnorm_to_length((uint8_t)f);
+            uint32_t *d_fn = nullptr;
+            BM25X_CUDA_TRY(cudaMalloc((void **)&d_fn, sizeof(h_fn)));
+            ix->allocs.push_back((void *)d_fn);
+            BM25X_CUDA_TRY(cudaMemcpy(d_fn, h_fn, sizeof(h_fn), cudaMemcpyHostToDevice));
+            ix->eval_fn_len = d_fn;
+        }
         if (!ix->eval_idf) {
             std::vector<double> h_idf(T ? T : 1);
             for (uint32_t t = 0; t < T; ++t)
                 h_idf[t] = log(((double)ix->d.n_docs + 1.0) / ((double)ix->h_df[t] + 0.5));
-            uint32_t h_fn[256];
-            for (int f = 0; f < 256; ++f) h_fn[f] = bm25x_fieldnorm_to_length((uint8_t)f);
             double *d_idf = nullptr;
-            uint32_t *d_fn = nullptr;
             BM25X_CUDA_TRY(cudaMalloc((void **)&d_idf, 8 * (size_t)(T ? T : 1)));
             ix->allocs.push_back((void *)d_idf);
-            BM25X_CUDA_TRY(cudaMalloc((void **)&d_fn, sizeof(h_fn)));
-            ix->allocs.push_back((void *)d_fn);
             BM25X_CUDA_TRY(cudaMemcpy(d_idf, h_idf.data(), 8 * (size_t)(T ? T : 1), cudaMemcpyHostToDevice));
-            BM25X_CUDA_TRY(cudaMemcpy(d_fn, h_fn, sizeof(h_fn), cudaMemcpyHostToDevice));
-            ix->eval_fn_len = d_fn;
             ix->eval_idf = d_idf;
         }
     }
@@ -845,7 +855,7 @@ extern "C" int bm25x_evaluate_batch(bm25x_index *ix, uint32_t n_pairs, const uin
     H(g_qoff, q_off, 4 * ((size_t)n_pairs + 1));
     H(g_qt, q_terms, 4 * (size_t)nqt);
     if (e == cudaSuccess) {
-        k_evaluate<<<(n_pairs + 127) / 128, 128>>>(n_pairs, g_doff, g_dt, g_df, g_qoff, g_qt, g_fn, g_idf, ix->d.s1d,
+        k_evaluate<<<(unsigned)(((uint64_t)n_pairs + 127) / 128), 128>>>(n_pairs, g_doff, g_dt, g_df, g_qoff, g_qt, g_fn, g_idf, ix->d.s1d,
                                                    ix->d.df, T, ix->k1, g_out);
         e = cudaGetLastError();
     }

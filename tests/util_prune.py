@@ -5,6 +5,7 @@ corpora built to reach those decisions on purpose.
                  two per streamed run, in proportion to df, with the branch each run took.
   first_window   the doc window of the first chunk: every run loads BM25X_RING_INIT postings, and the runs with postings
                  left in HBM bound the window by their last landed document.
+  windows        the windows of the first chunks (or of all of them) of a class of at most 8 terms, plain or seeded.
   pruned_lanes   the prune rule at a chunk boundary (util_filter.pruned_lanes, with ub_oth of a two-pass query's pass 0).
 
 Every corpus here uses b = 0 (the fieldnorm drops out of the score): a posting's score depends on its term's df and its
@@ -480,33 +481,40 @@ def pair_case(orc, n_p=2, seed=0):
     return c
 
 
-def windows(c, lanes, pruned_from, pruned, R=256, al=2, acc_docs=512, n_chunks=8):
-    """The doc windows of the first chunks of a class of at most 8 terms with fixed rings (R postings per run; the 2..4-term
-    classes: 8-byte rings, a 512-document dense accumulator): the first round loads BM25X_RING_INIT postings per run, a
-    window ends at the smallest last landed document of the runs with postings left in HBM (dense windows clamped to
-    the accumulator), and each refill tops the ring up (no top-up smaller than a quarter ring while a quarter is still
-    unread).  The lanes `pruned` (indices into `lanes`) leave at boundary `pruned_from` (1-based: chunk pruned_from
-    starts without them).  Returns per chunk (lo, hi, rd after it): rd = per lane, postings consumed."""
+def windows(c, lanes, pruned_from, pruned, R=256, al=2, acc_docs=512, n_chunks=8, first=INIT, clamp=True):
+    """The doc windows of a class of at most 8 terms (defaults: the plain kernel's fixed rings of R postings per run; the
+    2..4-term classes: 8-byte rings, a 512-document dense accumulator): the first round loads `first` postings per run
+    (BM25X_RING_INIT; None: a whole ring, as a seeded launch does), a window ends at the smallest last landed document of
+    the runs with postings left in HBM (dense windows clamped to the accumulator when `clamp`; a seeded launch never
+    clamps), and each refill tops the ring up (no top-up smaller than a quarter ring while a quarter is still unread).
+    R is one size for every run or one per lane (a class that sizes its rings per query).  The lanes `pruned` (indices
+    into `lanes`) leave at boundary `pruned_from` (1-based: chunk pruned_from starts without them).  Returns per chunk
+    (lo, hi, rd after it), the first n_chunks chunks or (None) every chunk up to the last one (hi = INF): rd = per lane,
+    postings consumed."""
     docs = [c.lists[t][0].astype(np.int64) for t in lanes]
     df = [len(d) for d in docs]
     dfpad = [(x + al - 1) & ~(al - 1) for x in df]
-    wr = [min(x, INIT) for x in dfpad]
+    R = list(R) if np.ndim(R) else [R] * len(lanes)
+    wr = [min(x, R[i] if first is None else first) for i, x in enumerate(dfpad)]
     rd = [0] * len(lanes)
     lo, out = 0, []
     INF = 0xFFFFFFFF
-    for chunk in range(1, n_chunks + 1):
+    chunk = 0
+    while n_chunks is None or chunk < n_chunks:
+        chunk += 1
         act = [i for i in range(len(lanes)) if not (chunk >= pruned_from and i in pruned)]
         lim = [int(docs[i][wr[i] - 1]) for i in act if wr[i] < df[i]]
         hi = min(lim) if lim else INF
         e = {i: (min(wr[i], df[i]) if hi == INF else rd[i] + int(np.searchsorted(docs[i][rd[i]:min(wr[i], df[i])], hi)))
              for i in act}
-        n = [e[i] - rd[i] for i in act]
-        S_, S2 = sum(n), sum(x * x for x in n)
-        hi_eff = hi if hi != INF else max((int(docs[i][e[i] - 1]) + 1 for i in act if e[i] > rd[i]), default=0)
-        span = max(hi_eff - lo, 0)
-        if len(act) > 1 and S_ * S_ - S2 > 2 * 48 * span and span > acc_docs:
-            hi = lo + acc_docs
-            e = {i: rd[i] + int(np.searchsorted(docs[i][rd[i]:e[i]], hi)) for i in act}
+        if clamp:
+            n = [e[i] - rd[i] for i in act]
+            S_, S2 = sum(n), sum(x * x for x in n)
+            hi_eff = hi if hi != INF else max((int(docs[i][e[i] - 1]) + 1 for i in act if e[i] > rd[i]), default=0)
+            span = max(hi_eff - lo, 0)
+            if len(act) > 1 and S_ * S_ - S2 > 2 * 48 * span and span > acc_docs:
+                hi = lo + acc_docs
+                e = {i: rd[i] + int(np.searchsorted(docs[i][rd[i]:e[i]], hi)) for i in act}
         for i in act:
             rd[i] = e[i]
         out.append((lo, hi, list(rd)))
@@ -515,8 +523,8 @@ def windows(c, lanes, pruned_from, pruned, R=256, al=2, acc_docs=512, n_chunks=8
             break
         for i in act:
             if wr[i] < dfpad[i]:
-                m = min((R - (wr[i] - rd[i])) & ~(al - 1), dfpad[i] - wr[i])
-                if m < R // 4 and wr[i] - rd[i] >= R // 4:
+                m = min((R[i] - (wr[i] - rd[i])) & ~(al - 1), dfpad[i] - wr[i])
+                if m < R[i] // 4 and wr[i] - rd[i] >= R[i] // 4:
                     m = 0
                 wr[i] += m
     return out

@@ -579,6 +579,39 @@ int bm25x_index_create_sharded_from_blocks(const bm25x_blocks *blocks, uint32_t 
  * Device memory per device beyond its shards: as bm25x_index_create_from_documents, for its own shards' documents. */
 int bm25x_index_create_sharded_from_documents(const bm25x_documents *docs, uint32_t n_shards, const uint32_t *doc_bounds,
                                               const int *devices, bm25x_sharded_index **out);
+/* The same document-sharded index, built from tsvectors (CREATE INDEX, am_build.rs:722, over a segment too large for one
+ * GPU): equal, shard for shard and array for array, to bm25x_index_create_sharded_from_documents on the keyed documents
+ * the document cast gives (doc id = position; bm25x_index_create_from_tsvectors), with the same payload, k1, b, n_shards,
+ * devices and the bounds this call reports (bm25x_sharded_get_info): n_terms = the distinct keys of the whole batch
+ * ascending bytewise, df / N / Σlen / avgdl the whole segment's, the keys with shard 0.  With doc_bounds == NULL the
+ * bounds are bm25x_sharded_create's balanced ones with c_d = the ENTRIES of tsvector d (cum[d] = ent_off[d]), known
+ * before any cast; for tsvectors with distinct lexemes (as PostgreSQL keeps them) that is the documents build's rule.
+ * Two passes, and no shard's keys leave its device but its distinct ones: each shard's slice is cast on its own device
+ * (the cast of bm25x_cast_tsvectors) and its distinct keys counted there; the host merges the shards' key lists into the
+ * vocabulary and sums their counts into df; each shard's device turns its keys into the vocabulary's ordinals and frees
+ * them; then the shards are built one after the other from (ordinal, tf).
+ * Refusals (*out = NULL; every shard built so far destroyed and every cast freed, no device memory left behind), in
+ * this order: null arguments; the tsvectors' host refusals (document mode); n of 0 or 0xFFFFFFFF, k1 and b
+ * (bm25x_index_create_from_tsvectors' messages); the shard arguments with bm25x_sharded_create's messages; every
+ * device (BM25X_ERR_CUDA).  Then, once EVERY shard is cast: the first vector (global numbering) with a merged count of 0
+ * (BM25X_ERR_INVALID), then the first document with a merged tf >= 2^24 (BM25X_ERR_UNSUPPORTED), then more than
+ * 0xFFFFFFFE distinct keys (BM25X_ERR_UNSUPPORTED), each with the unsharded call's message; BM25X_ERR_OOM /
+ * BM25X_ERR_CUDA.  Device memory per device, for each of its shards: 20 B per entry of its own slice and 12 B per
+ * tsvector (the cast), held until the vocabulary is known, plus the cast's chunk scratch while it runs and then the
+ * vocabulary pass's scratch (the shards' passes run one after the other, once every shard is cast); then 16 B per term
+ * of the vocabulary and 24 B per element while the ordinals are written; then 8 B per element (ordinal, tf) until that
+ * shard is built; plus its index and the build from documents' inversion figures.  Host: each shard's distinct keys
+ * (16 B each) and counts, the vocabulary (16 B per key), each shard's df (4 B per term), 12 B per tsvector. */
+int bm25x_index_create_sharded_from_tsvectors(const bm25x_tsvectors *tsv, const uint8_t seed[32],
+                                              const uint16_t *payload, double k1, double b, uint32_t n_shards,
+                                              const uint32_t *doc_bounds, const int *devices,
+                                              bm25x_sharded_index **out);
+/* bm25x_tsvector_queries on a document-sharded index: equal to that call on the unsharded index of the same corpus.  The
+ * query cast runs on shard 0's device against the segment's keys, which shard 0 holds; their device copy is made once
+ * per sharded index (16 B per term) and freed with it.  Refusals: bm25x_tsvector_queries', named by this call (a keyless
+ * sharded index: bm25x_lookup_terms' message).  Thread-safe alongside the searches on the same handle. */
+int bm25x_tsvector_queries_sharded(bm25x_sharded_index *sx, const uint8_t seed[32], const bm25x_tsvectors *tsv,
+                                   uint32_t *q_off, uint32_t *q_terms);
 void bm25x_sharded_destroy(bm25x_sharded_index *sx);
 /* info as the unsharded index would report it (n_docs, n_terms, n_postings, sum_doc_len, avgdl, k1, b); device_bytes
  * and n_blocks summed over the shards; device = shard 0's.  doc_bounds_out[n_shards+1] or NULL. */

@@ -226,6 +226,9 @@ def load_library():
                                                          C.POINTER(vp)]
     L.bm25x_index_create_sharded_from_documents.argtypes = [C.POINTER(_Documents), C.c_uint32, u32p, C.POINTER(C.c_int),
                                                             C.POINTER(vp)]
+    L.bm25x_index_create_sharded_from_tsvectors.argtypes = [C.POINTER(_Tsvectors), u8p, u16p, C.c_double, C.c_double,
+                                                             C.c_uint32, u32p, C.POINTER(C.c_int), C.POINTER(vp)]
+    L.bm25x_tsvector_queries_sharded.argtypes = [vp, u8p, C.POINTER(_Tsvectors), u32p, u32p]
     L.bm25x_sharded_destroy.argtypes = [vp]
     L.bm25x_sharded_destroy.restype = None
     L.bm25x_sharded_get_info.argtypes = [vp, C.POINTER(IndexInfo), u32p, u32p]
@@ -971,6 +974,26 @@ class ShardedIndex:
         return cls._adopt(h, info.n_docs, info.n_terms)
 
     @classmethod
+    def from_tsvectors(cls, seed, ent_off, entries, byte_off, data, *, payload=None, k1=1.2, b=0.75, n_shards=2,
+                       doc_bounds=None, devices=None) -> "ShardedIndex":
+        """The sharded index from tsvectors (Index.from_tsvectors' arguments, bm25x_index_create_sharded_from_tsvectors):
+        every shard's device casts only its own tsvectors and the vocabulary is merged from the shards' distinct keys.
+        Equals from_documents on the document cast with the same n_shards / devices and the bounds this index reports;
+        doc_bounds=None balances the shards by tsvector entries."""
+        keep = []
+        t = _tsvectors(keep, ent_off, entries, byte_off, data)
+        pay = _kept(keep, payload, np.uint16, C.c_uint16) if payload is not None else None
+        bounds = np.ascontiguousarray(doc_bounds, dtype=np.uint32) if doc_bounds is not None else None
+        devs = (C.c_int * int(n_shards))(*[int(d) for d in devices]) if devices is not None else None
+        h = C.c_void_p()
+        _check(load_library().bm25x_index_create_sharded_from_tsvectors(C.byref(t), _seed(seed), pay, float(k1), float(b),
+                                                                        int(n_shards), _p(bounds, C.c_uint32), devs,
+                                                                        C.byref(h)))
+        info = IndexInfo()
+        _check(load_library().bm25x_sharded_get_info(h, C.byref(info), None, None))
+        return cls._adopt(h, info.n_docs, info.n_terms)
+
+    @classmethod
     def _adopt(cls, handle, n_docs, n_terms):
         self = cls.__new__(cls)
         self.h, self.n_docs, self.n_terms = handle, int(n_docs), int(n_terms)
@@ -1023,6 +1046,18 @@ class ShardedIndex:
         out = np.zeros(len(keys), dtype=np.uint32)
         _check(load_library().bm25x_sharded_lookup_terms(self.h, _p(keys, C.c_uint8), len(keys), _p(out, C.c_uint32)))
         return out
+
+    def tsvector_queries(self, seed, ent_off, entries, byte_off, data):
+        """Index.tsvector_queries on this sharded index (bm25x_tsvector_queries_sharded): the query cast on shard 0's
+        device against the segment's keys.  Returns (q_off, q_terms) as search_batch takes them."""
+        keep = []
+        t = _tsvectors(keep, ent_off, entries, byte_off, data)
+        E = int(keep[0][-1]) if len(keep[0]) else 0
+        q_off = np.zeros(t.n + 1, np.uint32)
+        q_terms = np.zeros(max(E, 1), np.uint32)
+        _check(load_library().bm25x_tsvector_queries_sharded(self.h, _seed(seed), C.byref(t), _p(q_off, C.c_uint32),
+                                                             _p(q_terms, C.c_uint32)))
+        return q_off, q_terms[:int(q_off[-1])].copy()
 
     def search_batch(self, q_off, q_terms, k, allow=None, want_f64=True, want_payload=False, out=None):
         return _search_batch(load_library().bm25x_sharded_search_batch, self.h, q_off, q_terms, k, allow, want_f64,

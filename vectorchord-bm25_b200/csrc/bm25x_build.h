@@ -140,6 +140,17 @@ int upload_csr(bm25x_index *ix, const char *who, uint32_t T, uint64_t P, const u
 // may be device memory on `device` (the tsvector build's cast, bm25x_tsvector.cu); elem_off is host memory.  *out is
 // set on success; a CUDA failure is refused as `who`'s.
 int documents_build(const char *who, const bm25x_documents *c, const uint32_t *doc_len, int device, bm25x_index **out);
+// Its steps, which the sharded build from tsvectors (bm25x_tsvector.cu) runs shard by shard.  vocab_pass: the distinct
+// keys of c's elements ascending (host bytes, 16 B each) and each key's count, on `device`.  key_ordinals: term[i] = the
+// ordinal in keys[0..T) of raw key i (n 16-byte keys in device memory on `device`, each one of the vocabulary's).
+// invert: the postings of documents [lo, hi) of c, local ids, into the handle index_begin opened, then
+// index_finish_device; `keys` is read for a keyed c only.
+int vocab_pass(const char *who, const bm25x_documents *c, int device, std::vector<uint8_t> &keys,
+               std::vector<uint32_t> &df);
+cudaError_t key_ordinals(int device, const void *raw, uint64_t n, const std::vector<uint8_t> &keys, uint32_t T,
+                         uint32_t *term);
+int invert(const char *who, const bm25x_documents *c, const std::vector<uint8_t> &keys, uint32_t lo, uint32_t hi,
+           bm25x_index *ix);
 
 // ---- the tsvector casts of a growing segment (bm25x_tsvector.cu) ----
 
@@ -237,13 +248,13 @@ int sealed_side_search(const char *who, const SealedSide &sealed, bm25x_index *g
                        bool count_growing, uint32_t nq, const uint32_t *q_off, const uint32_t *q_terms, uint32_t k,
                        const ResultRows &host, bm25x_search_stats *stats, std::chrono::steady_clock::time_point t0);
 
-// The container of a document-sharded build, for both sources:after the host checks of the segment c (P postings, df, the
-// statistics st), every shard's device is checked with who's message; then prepare(device of shard 0, cum) runs the
+// The container of a document-sharded build, for every source: after the host checks of the segment c (P postings, df,
+// the statistics st), every shard's device is checked with who's message; then prepare(device of shard 0, cum) runs the
 // host work and refusals that need a device and, when doc_bounds is NULL, gives the postings per document for the balanced
-// bounds (shard_bounds); then the shards are built one at a time by build(s, device, lo, hi, ix).  On the first failure
-// everything built so far is destroyed.
+// bounds (shard_bounds); then the shards are built one at a time by build(s, device, lo, hi, ix).  c->n_terms, P, df and
+// st are read after prepare, which may set them.  On the first failure everything built so far is destroyed.
 template <typename Segment, typename Prepare, typename Build>
-int sharded_build(const char *who, const Segment *c, uint64_t P, const std::vector<uint32_t> &df, const Stats &st,
+int sharded_build(const char *who, const Segment *c, const uint64_t &P, const std::vector<uint32_t> &df, const Stats &st,
                   uint32_t S, const uint32_t *doc_bounds, const int *devices, Prepare prepare, Build build,
                   bm25x_sharded_index **out) {
     std::vector<int> dev(S, 0);

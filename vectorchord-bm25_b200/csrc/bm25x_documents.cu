@@ -207,8 +207,8 @@ static int validate_documents(const bm25x_documents *c, std::vector<uint32_t> &d
 // each key's df.  Every chunk's keys are appended to a device list of (key, count); the list is compacted (sort by key,
 // sum the counts of equal keys) when its appended part reaches its compacted part, so every entry is sorted a bounded
 // number of times whatever the vocabulary's size.
-static int vocab_pass(const char *who, const bm25x_documents *c, int device, std::vector<uint8_t> &keys,
-                      std::vector<uint32_t> &df) {
+int vocab_pass(const char *who, const bm25x_documents *c, int device, std::vector<uint8_t> &keys,
+               std::vector<uint32_t> &df) {
     const uint64_t E = c->elem_off[c->n_docs];
     cudaError_t e = cudaSetDevice(device);
     GrowBuf<Key128> kb[2];
@@ -302,8 +302,8 @@ static int count_df(const char *who, const bm25x_documents *c, const std::vector
 
 // The postings of documents [lo, hi) (local ids 0 .. hi - lo) written into the handle index_begin opened, chunk by chunk
 // in element order; then index_finish_device.
-static int invert(const char *who, const bm25x_documents *c, const std::vector<uint8_t> &keys, uint32_t lo, uint32_t hi,
-                  bm25x_index *ix) {
+int invert(const char *who, const bm25x_documents *c, const std::vector<uint8_t> &keys, uint32_t lo, uint32_t hi,
+           bm25x_index *ix) {
     DeviceIndex &d = ix->d;
     const uint32_t T = d.n_terms;
     const uint64_t e0 = c->elem_off[lo], e1 = c->elem_off[hi], ch = std::min(CHUNK, e1 - e0);
@@ -359,6 +359,19 @@ static int invert(const char *who, const bm25x_documents *c, const std::vector<u
     if (sc.e == cudaSuccess) sc.e = cudaDeviceSynchronize();
     if (sc.e == cudaSuccess) sc.e = index_finish_device(ix);
     return sc.e == cudaSuccess ? BM25X_OK : cuda_refusal(who, "document inversion", sc.e);
+}
+
+cudaError_t key_ordinals(int device, const void *raw, uint64_t n, const std::vector<uint8_t> &keys, uint32_t T,
+                         uint32_t *term) {
+    Scratch sc(device);
+    sc.e = cudaSetDevice(device);
+    const Key128 *vocab = upload_vocab(sc, keys, T);
+    if (sc.e == cudaSuccess && n) {
+        k_key_ordinals<<<grid_of(n), TPB>>>(static_cast<const ulonglong2 *>(raw), n, vocab, T, term, nullptr);
+        sc.e = cudaGetLastError();
+    }
+    if (sc.e == cudaSuccess) sc.e = cudaDeviceSynchronize();
+    return sc.e;
 }
 
 int documents_build(const char *who, const bm25x_documents *c, const uint32_t *doc_len, int device, bm25x_index **out) {

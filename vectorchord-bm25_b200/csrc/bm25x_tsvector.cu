@@ -11,12 +11,15 @@
 //      key's ordinal in an index's vocabulary), counts it into its vector's row and sums its vector's length.
 // Row offsets come from the row counts by a host scan once every chunk has run, so that a refused cast writes nothing.
 // The build from tsvectors hands the device-resident keyed CSR to the build from documents (documents_build): the keys
-// never travel to the host.  A growing segment's insert (tsvector_rows) numbers the keys its sealed vocabulary lacks:
+// never travel to the host.  The sharded build casts each shard's slice on its device and hands only its distinct keys
+// and their counts to the host, which merges them into the vocabulary; each shard's keys then become ordinals in place
+// and the build from documents inverts them without keys.  A growing segment's insert (tsvector_rows) numbers the keys its sealed vocabulary lacks:
 // k_tsv_missing compacts them, a radix sort and a unique give the call's distinct ones ascending, the host numbers
 // those, k_tsv_fresh hands each element its ordinal and a segmented sort puts every row back in ordinal order.
 #include <string.h>
 
 #include <algorithm>
+#include <queue>
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_reduce.cuh>
 #include <cub/device/device_segmented_sort.cuh>
@@ -317,11 +320,25 @@ struct Cast {
     explicit Cast(int device) : sc(device) {}
 };
 
+// Document::new (vector.rs:51-64): an element of value 0 is invalid data; v numbers the vector in the caller's batch.
+int zero_refusal(const char *who, uint32_t v) {
+    bm25x_set_error("%s: invalid data: a lexeme of tsvector %u has position counts that sum to 0", who, v);
+    return BM25X_ERR_INVALID;
+}
+
+// The refusal of a merged tf the packed posting layout cannot hold, naming the document.
+int big_tf_refusal(const char *who, uint32_t d) {
+    bm25x_set_error("%s: term frequency >= 2^24 is not supported by the packed posting layout (document %u)", who, d);
+    return BM25X_ERR_UNSUPPORTED;
+}
+
 int run_cast(const char *who, const bm25x_tsvectors *t, const uint8_t seed[32], int as_query, bool want_keys,
              const Key128 *vocab, uint32_t T, Cast &c) {
     Scratch &sc = c.sc;
     const uint32_t n = t->n;
-    const uint64_t E = t->ent_off[n];
+    // entries and bytes are read at the absolute offsets ent_off / byte_off give, so that a slice of a batch (its
+    // offsets + lo, entries and bytes as they are) casts in place; its outputs hold its own entries only
+    const uint64_t E = t->ent_off[n] - t->ent_off[0];
     // the chunks: whole vectors, at most CHUNK_ENT entries, CHUNK_BYTES bytes and CHUNK_VEC vectors, or one vector
     std::vector<uint32_t> cuts{0};
     while (cuts.back() < n) {
@@ -425,11 +442,7 @@ int run_cast(const char *who, const bm25x_tsvectors *t, const uint8_t seed[32], 
     for (size_t v = 0; v < h_len.size(); v++) c.len[v] = (uint32_t)std::min<uint64_t>(h_len[v], 0xFFFFFFFFu);
     c.zero = h_flags[0];
     c.big = h_flags[1];
-    if (c.zero != 0xFFFFFFFFu) {  // Document::new (vector.rs:51-64): an element of value 0 is invalid data
-        bm25x_set_error("%s: invalid data: a lexeme of tsvector %u has position counts that sum to 0", who, c.zero);
-        return BM25X_ERR_INVALID;
-    }
-    return BM25X_OK;
+    return c.zero != 0xFFFFFFFFu ? zero_refusal(who, c.zero) : BM25X_OK;
 }
 
 bool null_seed_or_tsv(const char *who, const bm25x_tsvectors *t, const uint8_t *seed) {
@@ -582,11 +595,7 @@ extern "C" int bm25x_index_create_from_tsvectors(const bm25x_tsvectors *tsv, con
     Cast c(device);
     rc = run_cast(who, tsv, seed, 0, true, nullptr, 0, c);
     if (rc != BM25X_OK) return rc;
-    if (c.big != 0xFFFFFFFFu) {
-        bm25x_set_error("%s: term frequency >= 2^24 is not supported by the packed posting layout (document %u)", who,
-                        c.big);
-        return BM25X_ERR_UNSUPPORTED;
-    }
+    if (c.big != 0xFFFFFFFFu) return big_tf_refusal(who, c.big);
     // the keyed documents of the cast, on the device: ascending keys and non-zero tf by construction
     bm25x_documents d{};
     d.n_docs = tsv->n;
@@ -599,13 +608,164 @@ extern "C" int bm25x_index_create_from_tsvectors(const bm25x_tsvectors *tsv, con
     return documents_build(who, &d, c.len.data(), device, out);
 }
 
-extern "C" int bm25x_tsvector_queries(bm25x_index *ix, const uint8_t seed[32], const bm25x_tsvectors *tsv, uint32_t *q_off,
-                                      uint32_t *q_terms) {
-    const char *who = "bm25x_tsvector_queries";
-    if (null_seed_or_tsv(who, tsv, seed) || !ix || !q_off) {
+// The sharded build from tsvectors: every shard's slice cast on its own device, one vocabulary merged on the host from
+// the shards' distinct keys, each shard's keys turned into that vocabulary's ordinals, then the shards built one after
+// the other from (ordinal, tf) alone.  A shard's keys never leave its device; only its distinct keys and their counts do.
+extern "C" int bm25x_index_create_sharded_from_tsvectors(const bm25x_tsvectors *tsv, const uint8_t seed[32],
+                                                         const uint16_t *payload, double k1, double b, uint32_t S,
+                                                         const uint32_t *doc_bounds, const int *devices,
+                                                         bm25x_sharded_index **out) {
+    const char *who = "bm25x_index_create_sharded_from_tsvectors";
+    if (out) *out = nullptr;
+    if (null_seed_or_tsv(who, tsv, seed) || !out) {
         bm25x_set_error("%s: null argument", who);
         return BM25X_ERR_INVALID;
     }
+    // every host check before any device is used: the tsvectors and the build's arguments as
+    // bm25x_index_create_from_tsvectors checks them, then the shard arguments as bm25x_sharded_create checks them
+    int rc = check_tsvectors(who, tsv, 0);
+    if (rc == BM25X_OK) rc = check_common(who, tsv->n, tsv->ent_off, k1, b, 0);
+    if (rc != BM25X_OK && rc != BM25X_ERR_CUDA) return rc;
+    const uint32_t N = tsv->n;
+    rc = check_shard_args(N, S, doc_bounds);
+    if (rc != BM25X_OK) return rc;
+    struct {
+        uint32_t n_docs, n_terms;
+        double k1, b;
+    } seg{N, 0, k1, b};  // n_terms: the merged vocabulary's size once prepare has run
+    uint64_t P = 0;
+    std::vector<uint8_t> keys;                       // the segment's vocabulary, 16 B per key
+    std::vector<uint32_t> df, len(N);                // the segment's df; each document's length (the cast's row sums)
+    std::vector<std::unique_ptr<Cast>> cast(S);      // shard s's cast: keyed, then (ordinals written) ord + tf
+    std::vector<std::vector<uint32_t>> df_s(S);      // shard s's df over the segment's vocabulary
+    Stats st(N, 0, nullptr, 0, k1, b);
+    auto prepare = [&](int, std::vector<uint64_t> *cum) {
+        std::vector<uint64_t> ent(tsv->ent_off, tsv->ent_off + (size_t)N + 1);  // c_d = the entries of tsvector d
+        const std::vector<uint32_t> bounds = shard_bounds(doc_bounds, ent, N, S);
+        // ---- every shard's slice cast on its device; refused only once every shard is cast, in the unsharded order ----
+        uint32_t zero = 0xFFFFFFFFu, big = 0xFFFFFFFFu;  // the first such vector, global numbering
+        for (uint32_t s = 0; s < S; s++) {
+            const uint32_t lo = bounds[s], hi = bounds[s + 1];
+            // the slice: run_cast reads entries and bytes at the offsets ent_off / byte_off give, so only those move
+            const bm25x_tsvectors t{hi - lo, tsv->ent_off + lo, tsv->entries, tsv->byte_off + lo, tsv->bytes};
+            cast[s].reset(new Cast(devices ? devices[s] : 0));
+            Cast &c = *cast[s];
+            const int rc = run_cast(who, &t, seed, 0, true, nullptr, 0, c);
+            if (rc != BM25X_OK && c.zero == 0xFFFFFFFFu) return rc;
+            if (rc != BM25X_OK || c.big != 0xFFFFFFFFu) {
+                if (c.zero != 0xFFFFFFFFu) zero = std::min(zero, lo + c.zero);
+                else big = std::min(big, lo + c.big);
+                cast[s].reset();
+                continue;
+            }
+            std::copy(c.len.begin(), c.len.end(), len.begin() + lo);
+            std::vector<uint32_t>().swap(c.len);
+        }
+        if (zero != 0xFFFFFFFFu) return zero_refusal(who, zero);
+        if (big != 0xFFFFFFFFu) return big_tf_refusal(who, big);
+        // ---- per shard, on its device: its distinct keys and their counts ----
+        std::vector<std::vector<uint8_t>> keys_s(S);
+        std::vector<std::vector<uint32_t>> cnt_s(S);
+        size_t total = 0;
+        for (uint32_t s = 0; s < S; s++) {
+            const Cast &c = *cast[s];
+            bm25x_documents d{};  // the slice's device-resident keyed CSR
+            d.n_docs = bounds[s + 1] - bounds[s];
+            d.elem_off = c.off.data();
+            d.elem_key = reinterpret_cast<const uint8_t *>(c.key);
+            d.elem_tf = c.tf;
+            const int rc = vocab_pass(who, &d, c.sc.device, keys_s[s], cnt_s[s]);
+            if (rc != BM25X_OK) return rc;
+            total += cnt_s[s].size();
+        }
+        // ---- the segment's vocabulary: the shards' ascending key lists merged (a heap of the S list heads), each
+        // shard key's global ordinal noted as it is taken ----
+        std::vector<size_t> at(S, 0);  // the next key of each list
+        std::vector<std::vector<uint32_t>> ord_s(S);
+        auto later = [&](uint32_t a, uint32_t b) {
+            const int c = memcmp(&keys_s[a][16 * at[a]], &keys_s[b][16 * at[b]], 16);
+            return c > 0 || (c == 0 && a > b);
+        };
+        std::priority_queue<uint32_t, std::vector<uint32_t>, decltype(later)> heads(later);
+        for (uint32_t s = 0; s < S; s++) {
+            ord_s[s].resize(cnt_s[s].size());
+            if (!cnt_s[s].empty()) heads.push(s);
+        }
+        keys.clear();
+        keys.reserve(16 * total);  // at most every shard's keys, distinct
+        while (!heads.empty()) {
+            const uint32_t s = heads.top();
+            heads.pop();
+            const uint8_t *k = &keys_s[s][16 * at[s]];
+            if (keys.empty() || memcmp(&keys[keys.size() - 16], k, 16) != 0) keys.insert(keys.end(), k, k + 16);
+            ord_s[s][at[s]] = (uint32_t)std::min<uint64_t>(keys.size() / 16 - 1, 0xFFFFFFFFull);
+            if (++at[s] < cnt_s[s].size()) heads.push(s);
+        }
+        std::vector<std::vector<uint8_t>>().swap(keys_s);
+        keys.shrink_to_fit();
+        const uint64_t V = keys.size() / 16;
+        if (V > 0xFFFFFFFEull) {  // vocab_pass's refusal
+            bm25x_set_error("%s: %llu distinct keys, more than the 2^32 - 2 term ordinals", who, (unsigned long long)V);
+            return BM25X_ERR_UNSUPPORTED;
+        }
+        const uint32_t T = (uint32_t)V;
+        // ---- each shard's counts at their global ordinals: its df; summed, the segment's ----
+        df.assign(T, 0);
+        for (uint32_t s = 0; s < S; s++) {
+            df_s[s].assign(T, 0);
+            for (size_t i = 0; i < cnt_s[s].size(); i++) {
+                df_s[s][ord_s[s][i]] = cnt_s[s][i];
+                df[ord_s[s][i]] += cnt_s[s][i];
+            }
+            std::vector<uint32_t>().swap(cnt_s[s]);
+            std::vector<uint32_t>().swap(ord_s[s]);
+        }
+        seg.n_terms = T;
+        st = Stats(N, doc_norms(N, len.data(), nullptr, 0, nullptr), df.data(), T, k1, b);
+        // ---- per shard, its keys as ordinals of the vocabulary; the keys freed ----
+        for (uint32_t s = 0; s < S; s++) {
+            Cast &c = *cast[s];
+            const uint64_t E = c.off.back();
+            P += E;
+            c.ord = c.sc.alloc<uint32_t>(E);
+            cudaError_t e = c.sc.e;
+            if (e == cudaSuccess && E) e = key_ordinals(c.sc.device, c.key, E, keys, T, c.ord);
+            if (e == cudaSuccess) e = cudaSetDevice(c.sc.device);
+            if (e == cudaSuccess) e = cudaFree(c.sc.release(c.key));
+            if (e != cudaSuccess) return cuda_refusal(who, "key ordinals", e);
+            c.key = nullptr;
+        }
+        if (cum) cum->swap(ent);
+        return BM25X_OK;
+    };
+    // one shard at a time, from its ordinals and tf; the term keys once, with shard 0
+    auto build = [&](uint32_t s, int device, uint32_t lo, uint32_t hi, IndexGuard &ix) {
+        Cast &c = *cast[s];
+        const uint32_t n = hi - lo, T = seg.n_terms;
+        BuildMeta m{n, T, len.data() + lo, payload ? payload + (size_t)lo * 3 : nullptr, s ? nullptr : keys.data(), k1, b,
+                    df_s[s].data(), c.off[n]};
+        m.doc_base = lo;
+        bm25x_documents d{};  // keyless: the cast's ordinals and tf, on the shard's device
+        d.n_docs = n;
+        d.elem_off = c.off.data();
+        d.elem_term = c.ord;
+        d.elem_tf = c.tf;
+        d.n_terms = T;
+        d.k1 = k1;
+        d.b = b;
+        int rc = index_begin(m, &st, device, ix);
+        if (rc == BM25X_OK) rc = invert(who, &d, keys, 0, n, ix.get());
+        cast[s].reset();
+        std::vector<uint32_t>().swap(df_s[s]);
+        return rc;
+    };
+    return sharded_build(who, &seg, P, df, st, S, doc_bounds, devices, prepare, build, out);
+}
+
+// Queries from tsvectors against the keys of ix (an index, or shard 0 of a document-sharded index, which holds the
+// segment's keys), after the null checks; refusals named by who.
+static int tsvector_queries(const char *who, bm25x_index *ix, const uint8_t seed[32], const bm25x_tsvectors *tsv,
+                            uint32_t *q_off, uint32_t *q_terms) {
     int rc = check_tsvectors(who, tsv, 1);
     if (rc != BM25X_OK) return rc;
     if (!q_terms && tsv->ent_off[tsv->n]) {
@@ -636,4 +796,25 @@ extern "C" int bm25x_tsvector_queries(bm25x_index *ix, const uint8_t seed[32], c
     }
     for (uint32_t v = 0; v <= tsv->n; v++) q_off[v] = (uint32_t)c.off[v];
     return BM25X_OK;
+}
+
+extern "C" int bm25x_tsvector_queries(bm25x_index *ix, const uint8_t seed[32], const bm25x_tsvectors *tsv, uint32_t *q_off,
+                                      uint32_t *q_terms) {
+    const char *who = "bm25x_tsvector_queries";
+    if (null_seed_or_tsv(who, tsv, seed) || !ix || !q_off) {
+        bm25x_set_error("%s: null argument", who);
+        return BM25X_ERR_INVALID;
+    }
+    return tsvector_queries(who, ix, seed, tsv, q_off, q_terms);
+}
+
+extern "C" int bm25x_tsvector_queries_sharded(bm25x_sharded_index *sx, const uint8_t seed[32], const bm25x_tsvectors *tsv,
+                                              uint32_t *q_off, uint32_t *q_terms) {
+    const char *who = "bm25x_tsvector_queries_sharded";
+    if (null_seed_or_tsv(who, tsv, seed) || !sx || !q_off) {
+        bm25x_set_error("%s: null argument", who);
+        return BM25X_ERR_INVALID;
+    }
+    // shard 0 holds the segment's keys, and its handle the device copy of them (uploaded once, freed with the index)
+    return tsvector_queries(who, sx->shards[0], seed, tsv, q_off, q_terms);
 }

@@ -689,6 +689,39 @@ int bm25x_check_vectors(uint32_t n, const uint32_t *off, const uint32_t *terms, 
  * evaluate on the sealed index instead). */
 int bm25x_evaluate_batch(bm25x_index *idx, uint32_t n_pairs, const uint32_t *d_off, const uint32_t *d_terms,
                          const uint32_t *d_tfs, const uint32_t *q_off, const uint32_t *q_terms, double *out);
+/* `<&>` from tsvectors in one call, what _bm25_evaluate(tsvector, bm25query) does (src/index/operators.rs:22-55): there
+ * are docs->n pairs, and out[p] = bm25::evaluate of cast_tsvector_to_document(docs[p]) against
+ * cast_tsvector_to_query(queries[pair_query ? pair_query[p] : p]), with the handle's N, df, avgdl, k1 and b.  Many rows
+ * against one query: queries->n == 1 and every pair_query entry 0.  Both casts run on the index's device against the
+ * copy of its vocabulary that bm25x_tsvector_queries keeps; the rows stay there in key order, known lexemes as their
+ * ordinals and unknown ones as BM25X_TERM_MISSING, which score nothing but count in the document's length
+ * (Document::length, vector.rs:77-83).  No key is numbered or re-sorted, and only out comes down.  A merged tf >= 2^24 is
+ * scored (evaluate has no packed posting layout).
+ * Refusals, BM25X_ERR_INVALID with out untouched, in this order and before any device work: a null argument (out may be
+ * NULL when docs->n == 0, pair_query may be NULL); the document tsvectors' host refusals (document mode, "tsvector must
+ * have positions" included), then the queries' (query mode); pair_query NULL with queries->n != docs->n, or an entry >=
+ * queries->n (naming the pair); a replica not finalized; a handle that scores with another segment's statistics (as
+ * bm25x_evaluate_batch); an index without term keys (bm25x_lookup_terms' message).  Then, after the casts and before out
+ * is written, the first document with a merged count of 0 (the cast's message).  BM25X_ERR_OOM / BM25X_ERR_CUDA from the
+ * device.  Thread-safe alongside the searches on the same handle; the idf table and the vocabulary copy are built once
+ * per handle.  Device memory until the call returns: 8 B per document element and 28 B per document tsvector, 4 B per
+ * query element and 16 B per query tsvector, 12 B per pair, plus one upload chunk of the cast (bm25x_cast_tsvectors);
+ * kept with the handle after the first call: 8 B (idf) and 16 B (vocabulary) per term. */
+int bm25x_evaluate_tsvectors(bm25x_index *idx, const uint8_t seed[32], const bm25x_tsvectors *docs,
+                             const bm25x_tsvectors *queries, const uint32_t *pair_query, double *out);
+/* bm25x_evaluate_batch and bm25x_evaluate_tsvectors on a document-sharded index: each returns exactly what its
+ * unsharded form returns on an index of the same corpus (the whole segment's N, df, avgdl, k1 and b), with its refusals,
+ * named by this call (there are no replicas or growing handles among sharded indexes).  Everything runs on shard 0's
+ * device, which holds the segment's keys and, for the tsvector call, their device copy (bm25x_tsvector_queries_sharded's).
+ * The whole segment's df and idf go to that device once per sharded index (12 B per term) and are freed by
+ * bm25x_sharded_destroy.  A keyless sharded index is served by the ordinal call and refused by the tsvector call
+ * (bm25x_lookup_terms' message).  Named in the bm25x_evaluate_* family rather than the bm25x_sharded_* one, whose
+ * prototypes are a fixed set (see bm25x_search_candidates_sharded). */
+int bm25x_evaluate_batch_sharded(bm25x_sharded_index *sx, uint32_t n_pairs, const uint32_t *d_off,
+                                 const uint32_t *d_terms, const uint32_t *d_tfs, const uint32_t *q_off,
+                                 const uint32_t *q_terms, double *out);
+int bm25x_evaluate_tsvectors_sharded(bm25x_sharded_index *sx, const uint8_t seed[32], const bm25x_tsvectors *docs,
+                                     const bm25x_tsvectors *queries, const uint32_t *pair_query, double *out);
 
 /* ---- synthetic corpus generator (bench/test utility; spec in DESIGN.md, mirrors tests/fuzz:168-205).
  * Fills a host CSR the caller frees with bm25x_synth_free. zipf_s == 0 ⇒ uniform vocabulary. */

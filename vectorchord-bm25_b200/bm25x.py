@@ -206,6 +206,9 @@ def load_library():
     L.bm25x_batch_destroy.argtypes = [vp]
     L.bm25x_batch_destroy.restype = None
     L.bm25x_evaluate_batch.argtypes = [vp, C.c_uint32, u32p, u32p, u32p, u32p, u32p, f64p]
+    L.bm25x_evaluate_batch_sharded.argtypes = L.bm25x_evaluate_batch.argtypes
+    L.bm25x_evaluate_tsvectors.argtypes = [vp, u8p, C.POINTER(_Tsvectors), C.POINTER(_Tsvectors), u32p, f64p]
+    L.bm25x_evaluate_tsvectors_sharded.argtypes = L.bm25x_evaluate_tsvectors.argtypes
     L.bm25x_check_vectors.argtypes = [C.c_uint32, u32p, u32p, u32p]
     L.bm25x_synth_generate.argtypes = [C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_double,
                                        C.c_int, C.POINTER(_Synth)]
@@ -719,21 +722,42 @@ class Index:
 
     # ---- bm25::evaluate for a batch of (document, query) pairs ----
     def evaluate_batch(self, docs, queries):
-        d_off = np.zeros(len(docs) + 1, np.uint32)
-        q_off = np.zeros(len(docs) + 1, np.uint32)
-        for i, (d, q) in enumerate(zip(docs, queries)):
-            d_off[i + 1] = d_off[i] + len(d.terms)
-            q_off[i + 1] = q_off[i] + len(q.terms)
-        cat = lambda xs: np.ascontiguousarray(np.concatenate(xs) if xs else np.zeros(0), dtype=np.uint32)
-        d_terms, d_tfs, q_terms = cat([d.terms for d in docs]), cat([d.tfs for d in docs]), cat([q.terms for q in queries])
-        out = np.zeros(len(docs), np.float64)
-        _check(load_library().bm25x_evaluate_batch(self.h, len(docs), _p(d_off, C.c_uint32), _p(d_terms, C.c_uint32),
-                                                   _p(d_tfs, C.c_uint32), _p(q_off, C.c_uint32),
-                                                   _p(q_terms, C.c_uint32), _p(out, C.c_double)))
-        return out
+        return _evaluate_batch(load_library().bm25x_evaluate_batch, self.h, docs, queries)
 
     def evaluate(self, document: Document, query: Query) -> float:
         return float(self.evaluate_batch([document], [query])[0])
+
+    def evaluate_tsvectors(self, seed, docs, queries, pair_query=None):
+        """`<&>` from tsvectors (bm25x_evaluate_tsvectors): out[p] = bm25::evaluate of document tsvector p against query
+        tsvector pair_query[p] (p when None), both cast on the GPU against this index's keys."""
+        return _evaluate_tsvectors(load_library().bm25x_evaluate_tsvectors, self.h, seed, docs, queries, pair_query)
+
+
+def _evaluate_batch(fn, h, docs, queries):
+    """bm25x_evaluate_batch or its sharded form (the same signature) on lists of Document and Query."""
+    d_off = np.zeros(len(docs) + 1, np.uint32)
+    q_off = np.zeros(len(docs) + 1, np.uint32)
+    for i, (d, q) in enumerate(zip(docs, queries)):
+        d_off[i + 1] = d_off[i] + len(d.terms)
+        q_off[i + 1] = q_off[i] + len(q.terms)
+    cat = lambda xs: np.ascontiguousarray(np.concatenate(xs) if xs else np.zeros(0), dtype=np.uint32)
+    d_terms, d_tfs, q_terms = cat([d.terms for d in docs]), cat([d.tfs for d in docs]), cat([q.terms for q in queries])
+    out = np.zeros(len(docs), np.float64)
+    _check(fn(h, len(docs), _p(d_off, C.c_uint32), _p(d_terms, C.c_uint32), _p(d_tfs, C.c_uint32),
+              _p(q_off, C.c_uint32), _p(q_terms, C.c_uint32), _p(out, C.c_double)))
+    return out
+
+
+def _evaluate_tsvectors(fn, h, seed, docs, queries, pair_query):
+    """bm25x_evaluate_tsvectors or its sharded form.  docs, queries: tsvector batches, each a dict of the arguments
+    cast_tsvectors takes (ent_off, entries, byte_off, data); pair_query: u32 [docs n] or None."""
+    keep = []
+    d = _tsvectors(keep, **docs)
+    q = _tsvectors(keep, **queries)
+    pq = None if pair_query is None else _kept(keep, pair_query, np.uint32, C.c_uint32)
+    out = np.zeros(max(d.n, 1), np.float64)
+    _check(fn(h, _seed(seed), C.byref(d), C.byref(q), pq, _p(out, C.c_double)))
+    return out[:d.n]
 
 
 def _growing_docs(keep, elem_off, elem_term, elem_tf, doc_len, doc_fieldnorm, payload, deleted):
@@ -1058,6 +1082,15 @@ class ShardedIndex:
         _check(load_library().bm25x_tsvector_queries_sharded(self.h, _seed(seed), C.byref(t), _p(q_off, C.c_uint32),
                                                              _p(q_terms, C.c_uint32)))
         return q_off, q_terms[:int(q_off[-1])].copy()
+
+    def evaluate_batch(self, docs, queries):
+        """Index.evaluate_batch with the whole segment's statistics (bm25x_evaluate_batch_sharded)."""
+        return _evaluate_batch(load_library().bm25x_evaluate_batch_sharded, self.h, docs, queries)
+
+    def evaluate_tsvectors(self, seed, docs, queries, pair_query=None):
+        """Index.evaluate_tsvectors on this sharded index (bm25x_evaluate_tsvectors_sharded), on shard 0's device."""
+        return _evaluate_tsvectors(load_library().bm25x_evaluate_tsvectors_sharded, self.h, seed, docs, queries,
+                                   pair_query)
 
     def search_batch(self, q_off, q_terms, k, allow=None, want_f64=True, want_payload=False, out=None):
         return _search_batch(load_library().bm25x_sharded_search_batch, self.h, q_off, q_terms, k, allow, want_f64,

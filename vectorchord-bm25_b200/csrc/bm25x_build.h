@@ -165,6 +165,25 @@ struct TsvVocab {
     void **slot;
     std::mutex *mu;
 };
+// The cast of a batch on one device (run_cast, bm25x_tsvector.cu).  Outputs held on the device, freed with the object:
+// document mode the keyed CSR (raw keys key[E'], tf[E']), query mode the keys, or (a vocabulary given) the keys'
+// ordinals ord[E'].  Host: off[n+1] the rows, len[n] the saturating Σ tf of each row (document mode), and the first
+// vector with a merged tf of 0 / >= 2^24.
+struct TsvCast {
+    Scratch sc;
+    ulonglong2 *key = nullptr;
+    uint32_t *tf = nullptr, *ord = nullptr;
+    std::vector<uint64_t> off;
+    std::vector<uint32_t> len;
+    uint32_t zero = 0xFFFFFFFFu, big = 0xFFFFFFFFu;
+    explicit TsvCast(int device) : sc(device) {}
+};
+// The cast of t (checked) on v.device, left there without keys: c.ord the ordinal of each key in v's vocabulary
+// (BM25X_TERM_MISSING where it lacks the key; each row in key order, so known ordinals ascend with BM25X_TERM_MISSING
+// among them), c.tf in document mode, and c.off.  Refusals: the cast's (a document element whose merged count is 0, after
+// the device work), CUDA failures named by who.  A merged tf >= 2^24 is not refused (c.big names it).
+int tsvector_cast(const char *who, const TsvVocab &v, const uint8_t seed[32], const bm25x_tsvectors *t, int as_query,
+                  TsvCast &c);
 // Rows of a cast: row i = ord / tf [off[i], off[i+1]); len[i] = the saturating Σ tf of row i (document mode).
 struct TsvRows {
     std::vector<uint64_t> off;

@@ -130,6 +130,11 @@ struct bm25x_sharded_index {
     uint64_t n_post = 0, sum_len = 0;
     double k1 = 1.2, b = 0.75, avgdl = 0;
     std::vector<uint32_t> h_df;
+    // bm25x_evaluate_*_sharded: the whole segment's df and idf on shard 0's device, built on first use, freed by
+    // bm25x_sharded_destroy
+    uint32_t *eval_df = nullptr;
+    double *eval_idf = nullptr;
+    std::mutex eval_mutex;
 };
 
 // ---- internal to the host library (bm25x_search.cu, bm25x_shards.cu, bm25x_growing.cu) ----

@@ -696,6 +696,11 @@ extern "C" int bm25x_index_create(const bm25x_corpus *c, int device, bm25x_index
 // that scores with the whole segment's statistics ----
 extern "C" void bm25x_sharded_destroy(bm25x_sharded_index *sx) {
     if (!sx) return;
+    if (sx->eval_df || sx->eval_idf) {
+        cudaSetDevice(sx->shards[0]->device);
+        cudaFree(sx->eval_df);
+        cudaFree(sx->eval_idf);
+    }
     for (bm25x_index *ix : sx->shards) bm25x_index_destroy(ix);
     delete sx;
 }

@@ -24,47 +24,6 @@
 
 #include "bm25x_device.cuh"
 
-namespace {
-
-// ---------------------------------------------------------------------------------------------
-// bm25::evaluate (crates/bm25/src/evaluate.rs:22-74): one thread per (document, query) pair.
-__global__ void k_evaluate(uint32_t n_pairs, const uint32_t *__restrict__ d_off, const uint32_t *__restrict__ d_terms,
-                           const uint32_t *__restrict__ d_tfs, const uint32_t *__restrict__ q_off,
-                           const uint32_t *__restrict__ q_terms, const uint32_t *__restrict__ fn_len,
-                           const double *__restrict__ idf, const double *__restrict__ s1d, const uint32_t *__restrict__ df,
-                           uint32_t n_terms, double k1, double *__restrict__ out) {
-    uint32_t pidx = blockIdx.x * blockDim.x + threadIdx.x;
-    if (pidx >= n_pairs) return;
-    uint32_t a = d_off[pidx], b = d_off[pidx + 1];
-    uint64_t len = 0;  // Document::length(): saturating Σ tf (vector.rs:77-83)
-    for (uint32_t i = a; i < b; ++i) {
-        len += d_tfs[i];
-        if (len > 0xFFFFFFFFull) len = 0xFFFFFFFFull;
-    }
-    int lo = 0, hi = 256;  // length_to_fieldnorm, bm25.rs:278-283
-    while (lo < hi) {
-        int mid = (lo + hi) >> 1;
-        if (fn_len[mid] <= (uint32_t)len) lo = mid + 1;
-        else hi = mid;
-    }
-    const int fn = lo - 1;
-    uint32_t cursor = a;
-    double result = 0.0;
-    const double k1p1 = __dadd_rn(k1, 1.0);
-    for (uint32_t qi = q_off[pidx]; qi < q_off[pidx + 1]; ++qi) {
-        uint32_t key = q_terms[qi];
-        while (cursor < b && d_terms[cursor] < key) cursor++;
-        if (!(cursor < b && d_terms[cursor] == key)) continue;
-        if (key >= n_terms || df[key] == 0) continue;  // address_tokens::read → None
-        double tfd = (double)d_tfs[cursor];
-        double tfv = __ddiv_rn(__dmul_rn(tfd, k1p1), __dadd_rn(tfd, s1d[fn]));  // bm25.rs:291-295
-        result = __dadd_rn(result, __dmul_rn(idf[key], tfv));
-    }
-    out[pidx] = result;
-}
-
-}  // namespace
-
 // =============================================================================================
 // Host side
 // =============================================================================================
@@ -745,130 +704,4 @@ extern "C" int bm25x_search_batch_growing(bm25x_index *sealed, bm25x_index *grow
     return sealed_side_search("bm25x_search_batch_growing", side, growing, f, false, nq, q_off, q_terms, k,
                               {out_doc, out_score, out_score64, out_payload, out_n}, stats,
                               std::chrono::steady_clock::now());
-}
-
-// ---------------------------------------------------------------------------------------------
-uint32_t bm25x_fieldnorm_to_length(uint8_t fn);
-
-// Invariants of the reference's vector types (crates/bm25/src/vector.rs:46-134): a Document / Query holds strictly
-// ascending keys, a Document's term frequencies are non-zero (`Document::new` / `Query::new` → expect("invalid data")).
-// Host only; bm25x_evaluate_batch applies it to both sides of every pair (its kernel merges the two sorted lists).
-extern "C" int bm25x_check_vectors(uint32_t n, const uint32_t *off, const uint32_t *terms, const uint32_t *tfs) {
-    if (n && (!off || (!terms && off[n] != 0))) {
-        bm25x_set_error("bm25x_check_vectors: null argument");
-        return BM25X_ERR_INVALID;
-    }
-    for (uint32_t i = 0; i < n; ++i) {
-        if (off[i + 1] < off[i]) {
-            bm25x_set_error("invalid data: offsets not monotone at vector %u", i);
-            return BM25X_ERR_INVALID;
-        }
-        for (uint32_t j = off[i]; j < off[i + 1]; ++j) {
-            if (j > off[i] && terms[j] <= terms[j - 1]) {
-                bm25x_set_error("invalid data: keys of vector %u are not strictly ascending", i);
-                return BM25X_ERR_INVALID;
-            }
-            if (tfs && tfs[j] == 0) {
-                bm25x_set_error("invalid data: zero term frequency in vector %u", i);
-                return BM25X_ERR_INVALID;
-            }
-        }
-    }
-    return BM25X_OK;
-}
-
-extern "C" int bm25x_evaluate_batch(bm25x_index *ix, uint32_t n_pairs, const uint32_t *d_off, const uint32_t *d_terms,
-                                    const uint32_t *d_tfs, const uint32_t *q_off, const uint32_t *q_terms, double *out) {
-    if (!ix || (n_pairs && (!d_off || !q_off || !out))) {
-        bm25x_set_error("bm25x_evaluate_batch: null argument");
-        return BM25X_ERR_INVALID;
-    }
-    if (n_pairs == 0) return BM25X_OK;
-    if (d_off[n_pairs] != 0 && !d_tfs) {
-        bm25x_set_error("bm25x_evaluate_batch: null argument");
-        return BM25X_ERR_INVALID;
-    }
-    {   // Document / Query invariants (vector.rs:46-134)
-        int vrc = bm25x_check_vectors(n_pairs, d_off, d_terms, d_tfs);
-        if (vrc == BM25X_OK) vrc = bm25x_check_vectors(n_pairs, q_off, q_terms, nullptr);
-        if (vrc != BM25X_OK) return vrc;
-    }
-    if (ix->h_df.size() != ix->d.n_terms) {
-        bm25x_set_error("bm25x_evaluate_batch: replica not finalized (bm25x_index_finalize_replica)");
-        return BM25X_ERR_INVALID;
-    }
-    // bm25::evaluate reads one segment's meta and tokens (evaluate.rs:22-74): a handle whose avgdl is another segment's
-    // while its N and df are its own matches no reference answer
-    if (!own_statistics(ix)) {
-        bm25x_set_error("bm25x_evaluate_batch: the index scores with another segment's statistics (a growing handle); "
-                        "evaluate on the sealed index");
-        return BM25X_ERR_INVALID;
-    }
-    BM25X_CUDA_TRY(cudaSetDevice(ix->device));
-    const uint32_t nd = d_off[n_pairs], nqt = q_off[n_pairs];
-    const uint32_t T = ix->d.n_terms;
-    {   // idf table (bm25.rs:285-289) with the host libm, like the reference's f64::ln, and the fieldnorm -> length table:
-        // they depend on the index alone — built once, kept on the device (freed with the handle; the idf table is
-        // dropped by bm25x_index_finalize_replica and rebuilt here)
-        std::lock_guard<std::mutex> lk(ix->eval_mutex);
-        if (!ix->eval_fn_len) {
-            uint32_t h_fn[256];
-            for (int f = 0; f < 256; ++f) h_fn[f] = bm25x_fieldnorm_to_length((uint8_t)f);
-            uint32_t *d_fn = nullptr;
-            BM25X_CUDA_TRY(cudaMalloc((void **)&d_fn, sizeof(h_fn)));
-            ix->allocs.push_back((void *)d_fn);
-            BM25X_CUDA_TRY(cudaMemcpy(d_fn, h_fn, sizeof(h_fn), cudaMemcpyHostToDevice));
-            ix->eval_fn_len = d_fn;
-        }
-        if (!ix->eval_idf) {
-            std::vector<double> h_idf(T ? T : 1);
-            for (uint32_t t = 0; t < T; ++t)
-                h_idf[t] = log(((double)ix->d.n_docs + 1.0) / ((double)ix->h_df[t] + 0.5));
-            double *d_idf = nullptr;
-            BM25X_CUDA_TRY(cudaMalloc((void **)&d_idf, 8 * (size_t)(T ? T : 1)));
-            ix->allocs.push_back((void *)d_idf);
-            BM25X_CUDA_TRY(cudaMemcpy(d_idf, h_idf.data(), 8 * (size_t)(T ? T : 1), cudaMemcpyHostToDevice));
-            ix->eval_idf = d_idf;
-        }
-    }
-    uint32_t *g_doff = nullptr, *g_dt = nullptr, *g_df = nullptr, *g_qoff = nullptr, *g_qt = nullptr;
-    uint32_t *const g_fn = ix->eval_fn_len;
-    double *const g_idf = ix->eval_idf;
-    double *g_out = nullptr;
-    int rc = BM25X_OK;
-    cudaError_t e = cudaSuccess;
-    auto A = [&](void **p, size_t bytes) {
-        if (e == cudaSuccess) e = cudaMalloc(p, bytes ? bytes : 4);
-    };
-    A((void **)&g_doff, 4 * ((size_t)n_pairs + 1));
-    A((void **)&g_dt, 4 * (size_t)nd);
-    A((void **)&g_df, 4 * (size_t)nd);
-    A((void **)&g_qoff, 4 * ((size_t)n_pairs + 1));
-    A((void **)&g_qt, 4 * (size_t)nqt);
-    A((void **)&g_out, 8 * (size_t)n_pairs);
-    auto H = [&](void *dst, const void *src, size_t bytes) {
-        if (e == cudaSuccess && bytes) e = cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice);
-    };
-    H(g_doff, d_off, 4 * ((size_t)n_pairs + 1));
-    H(g_dt, d_terms, 4 * (size_t)nd);
-    H(g_df, d_tfs, 4 * (size_t)nd);
-    H(g_qoff, q_off, 4 * ((size_t)n_pairs + 1));
-    H(g_qt, q_terms, 4 * (size_t)nqt);
-    if (e == cudaSuccess) {
-        k_evaluate<<<(unsigned)(((uint64_t)n_pairs + 127) / 128), 128>>>(n_pairs, g_doff, g_dt, g_df, g_qoff, g_qt, g_fn, g_idf, ix->d.s1d,
-                                                   ix->d.df, T, ix->k1, g_out);
-        e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = cudaMemcpy(out, g_out, 8 * (size_t)n_pairs, cudaMemcpyDeviceToHost);
-    if (e != cudaSuccess) {
-        bm25x_set_error("bm25x_evaluate_batch: %s", cudaGetErrorString(e));
-        rc = BM25X_ERR_CUDA;
-    }
-    cudaFree(g_doff);
-    cudaFree(g_dt);
-    cudaFree(g_df);
-    cudaFree(g_qoff);
-    cudaFree(g_qt);
-    cudaFree(g_out);
-    return rc;
 }

@@ -307,19 +307,6 @@ int check_tsvectors(const char *who, const bm25x_tsvectors *t, int as_query) {
 
 namespace {
 
-// The cast of every vector on the current device.  Outputs held on the device: document mode the keyed CSR (raw keys
-// key[E'], tf[E']), query mode the keys, or (vocab given) the keys' ordinals ord[E'].  Host: off[n+1] the rows, len[n]
-// the saturating Σ tf of each row (document mode), and the first vector with a merged tf of 0 / >= 2^24.
-struct Cast {
-    Scratch sc;
-    ulonglong2 *key = nullptr;
-    uint32_t *tf = nullptr, *ord = nullptr;
-    std::vector<uint64_t> off;
-    std::vector<uint32_t> len;
-    uint32_t zero = 0xFFFFFFFFu, big = 0xFFFFFFFFu;
-    explicit Cast(int device) : sc(device) {}
-};
-
 // Document::new (vector.rs:51-64): an element of value 0 is invalid data; v numbers the vector in the caller's batch.
 int zero_refusal(const char *who, uint32_t v) {
     bm25x_set_error("%s: invalid data: a lexeme of tsvector %u has position counts that sum to 0", who, v);
@@ -333,7 +320,7 @@ int big_tf_refusal(const char *who, uint32_t d) {
 }
 
 int run_cast(const char *who, const bm25x_tsvectors *t, const uint8_t seed[32], int as_query, bool want_keys,
-             const Key128 *vocab, uint32_t T, Cast &c) {
+             const Key128 *vocab, uint32_t T, TsvCast &c) {
     Scratch &sc = c.sc;
     const uint32_t n = t->n;
     // entries and bytes are read at the absolute offsets ent_off / byte_off give, so that a slice of a batch (its
@@ -469,12 +456,19 @@ int device_vocab(const char *who, const TsvVocab &v, const Key128 **out) {
 
 }  // namespace
 
+int tsvector_cast(const char *who, const TsvVocab &v, const uint8_t seed[32], const bm25x_tsvectors *t, int as_query,
+                  TsvCast &c) {
+    const Key128 *vocab = nullptr;
+    const int rc = device_vocab(who, v, &vocab);
+    return rc == BM25X_OK ? run_cast(who, t, seed, as_query, false, vocab, v.T, c) : rc;
+}
+
 int tsvector_rows(const char *who, const TsvVocab &v, const uint8_t seed[32], const bm25x_tsvectors *t, int as_query,
                   const TsvNumbering &number, TsvRows &out) {
     const Key128 *vocab = nullptr;
     int rc = device_vocab(who, v, &vocab);
     if (rc != BM25X_OK) return rc;
-    Cast c(v.device);
+    TsvCast c(v.device);
     rc = run_cast(who, t, seed, as_query, !as_query, vocab, v.T, c);
     if (rc != BM25X_OK) return rc;
     const uint32_t n = t->n;
@@ -566,7 +560,7 @@ extern "C" int bm25x_cast_tsvectors(const bm25x_tsvectors *tsv, const uint8_t se
     int rc = check_tsvectors(who, tsv, as_query);
     if (rc == BM25X_OK) rc = check_device(who, device);
     if (rc != BM25X_OK) return rc;
-    Cast c(device);
+    TsvCast c(device);
     rc = run_cast(who, tsv, seed, as_query, true, nullptr, 0, c);
     if (rc != BM25X_OK) return rc;
     const uint64_t E = c.off[tsv->n];
@@ -592,7 +586,7 @@ extern "C" int bm25x_index_create_from_tsvectors(const bm25x_tsvectors *tsv, con
     if (rc != BM25X_OK && rc != BM25X_ERR_CUDA) return rc;
     rc = check_device(who, device);
     if (rc != BM25X_OK) return rc;
-    Cast c(device);
+    TsvCast c(device);
     rc = run_cast(who, tsv, seed, 0, true, nullptr, 0, c);
     if (rc != BM25X_OK) return rc;
     if (c.big != 0xFFFFFFFFu) return big_tf_refusal(who, c.big);
@@ -636,7 +630,7 @@ extern "C" int bm25x_index_create_sharded_from_tsvectors(const bm25x_tsvectors *
     uint64_t P = 0;
     std::vector<uint8_t> keys;                       // the segment's vocabulary, 16 B per key
     std::vector<uint32_t> df, len(N);                // the segment's df; each document's length (the cast's row sums)
-    std::vector<std::unique_ptr<Cast>> cast(S);      // shard s's cast: keyed, then (ordinals written) ord + tf
+    std::vector<std::unique_ptr<TsvCast>> cast(S);   // shard s's cast: keyed, then (ordinals written) ord + tf
     std::vector<std::vector<uint32_t>> df_s(S);      // shard s's df over the segment's vocabulary
     Stats st(N, 0, nullptr, 0, k1, b);
     auto prepare = [&](int, std::vector<uint64_t> *cum) {
@@ -648,8 +642,8 @@ extern "C" int bm25x_index_create_sharded_from_tsvectors(const bm25x_tsvectors *
             const uint32_t lo = bounds[s], hi = bounds[s + 1];
             // the slice: run_cast reads entries and bytes at the offsets ent_off / byte_off give, so only those move
             const bm25x_tsvectors t{hi - lo, tsv->ent_off + lo, tsv->entries, tsv->byte_off + lo, tsv->bytes};
-            cast[s].reset(new Cast(devices ? devices[s] : 0));
-            Cast &c = *cast[s];
+            cast[s].reset(new TsvCast(devices ? devices[s] : 0));
+            TsvCast &c = *cast[s];
             const int rc = run_cast(who, &t, seed, 0, true, nullptr, 0, c);
             if (rc != BM25X_OK && c.zero == 0xFFFFFFFFu) return rc;
             if (rc != BM25X_OK || c.big != 0xFFFFFFFFu) {
@@ -668,7 +662,7 @@ extern "C" int bm25x_index_create_sharded_from_tsvectors(const bm25x_tsvectors *
         std::vector<std::vector<uint32_t>> cnt_s(S);
         size_t total = 0;
         for (uint32_t s = 0; s < S; s++) {
-            const Cast &c = *cast[s];
+            const TsvCast &c = *cast[s];
             bm25x_documents d{};  // the slice's device-resident keyed CSR
             d.n_docs = bounds[s + 1] - bounds[s];
             d.elem_off = c.off.data();
@@ -724,7 +718,7 @@ extern "C" int bm25x_index_create_sharded_from_tsvectors(const bm25x_tsvectors *
         st = Stats(N, doc_norms(N, len.data(), nullptr, 0, nullptr), df.data(), T, k1, b);
         // ---- per shard, its keys as ordinals of the vocabulary; the keys freed ----
         for (uint32_t s = 0; s < S; s++) {
-            Cast &c = *cast[s];
+            TsvCast &c = *cast[s];
             const uint64_t E = c.off.back();
             P += E;
             c.ord = c.sc.alloc<uint32_t>(E);
@@ -740,7 +734,7 @@ extern "C" int bm25x_index_create_sharded_from_tsvectors(const bm25x_tsvectors *
     };
     // one shard at a time, from its ordinals and tf; the term keys once, with shard 0
     auto build = [&](uint32_t s, int device, uint32_t lo, uint32_t hi, IndexGuard &ix) {
-        Cast &c = *cast[s];
+        TsvCast &c = *cast[s];
         const uint32_t n = hi - lo, T = seg.n_terms;
         BuildMeta m{n, T, len.data() + lo, payload ? payload + (size_t)lo * 3 : nullptr, s ? nullptr : keys.data(), k1, b,
                     df_s[s].data(), c.off[n]};
@@ -778,11 +772,8 @@ static int tsvector_queries(const char *who, bm25x_index *ix, const uint8_t seed
         return BM25X_ERR_INVALID;
     }
     // the vocabulary as Key128, built once per handle and freed with it (bm25x_index_destroy)
-    const Key128 *vocab = nullptr;
-    rc = device_vocab(who, {ix->device, &ix->h_keys, T, &ix->key_vocab, &ix->key_vocab_mutex}, &vocab);
-    if (rc != BM25X_OK) return rc;
-    Cast c(ix->device);
-    rc = run_cast(who, tsv, seed, 1, false, vocab, T, c);
+    TsvCast c(ix->device);
+    rc = tsvector_cast(who, {ix->device, &ix->h_keys, T, &ix->key_vocab, &ix->key_vocab_mutex}, seed, tsv, 1, c);
     if (rc != BM25X_OK) return rc;
     const uint64_t E = c.off[tsv->n];
     if (E > 0xFFFFFFFFull) {

@@ -423,7 +423,8 @@ int bm25x_merge_topk(uint32_t nq, uint32_t k, const uint32_t *doc_a, const float
  * over sealed + growing is one call (both handles' kernels, one device merge, one download) and refreshes first when
  * anything is pending.  Every call may come from any thread: a search sees one state of the segment, with every insert
  * and delete that returned before it started and never part of one; a handle a running search still holds is destroyed
- * when that search ends.  The sealed index must outlive the segment. */
+ * when that search ends.  The sealed index must outlive the segment, or the rebind to its successor
+ * (bm25x_growing_rebind). */
 typedef struct bm25x_growing_segment bm25x_growing_segment;
 typedef struct {
     uint32_t n_docs;        /* ordinals handed out (deleted ones included) */
@@ -645,7 +646,8 @@ int bm25x_search_candidates_sharded(bm25x_sharded_index *sx, uint32_t nq, const 
  * bm25x_sharded_search_batch (the whole segment's canonicalisation first) and merges the shards' lists and the growing
  * handle's, growing ordinal o as n_docs(whole) + o, allow_sealed over global ids; stats: queries = live queries of the
  * whole segment plus the growing handle's, the rest sums over the shards, the growing handle and the merge launch.
- * Before the first insert it is bm25x_sharded_search_batch, stats included.  The sharded index must outlive the segment;
+ * Before the first insert it is bm25x_sharded_search_batch, stats included.  The sharded index must outlive the segment,
+ * or the rebind to its successor (bm25x_growing_rebind_sharded);
  * bm25x_growing_seal refuses the segment (BM25X_ERR_INVALID). */
 int bm25x_growing_open_sharded(bm25x_sharded_index *sealed, bm25x_growing_segment **out);
 /* The seal of a segment opened with bm25x_growing_open_sharded.  The result is a new document-sharded index.  args,
@@ -659,6 +661,57 @@ int bm25x_growing_open_sharded(bm25x_sharded_index *sealed, bm25x_growing_segmen
  * fit (bounds are not rebalanced).  The old sharded index and the segment are not changed; an unsharded segment is
  * refused (BM25X_ERR_INVALID). */
 int bm25x_growing_seal_sharded(bm25x_growing_segment *g, bm25x_seal_args *args, bm25x_sharded_index **out);
+/* ---- the rebind: the segment goes on over the index its latest seal built, as the reference's segment goes on after
+ * `maintain` rewrote the sealed segment in place.  The ordinals the seal folded in ([0, n_folded)) leave the segment;
+ * old ordinal n_folded + i becomes ordinal i.  Afterwards the segment equals, array for array, field for field and row
+ * for row, bm25x_growing_open (or _open_sharded) on the new index followed by ONE insert of the carried documents
+ * restated: each keeps its stored payload (the synthetic ctid of its OLD ordinal when none was given), its norm in the
+ * segment's form and its deleted flag; each element is translated and the rows re-sorted by the new ordinal:
+ *   - keyless index: the ordinal is unchanged (the seal keeps keyless ordinals stable);
+ *   - a segment that owns its keys (bm25x_growing_insert_tsvectors): the element's key becomes its ordinal in the new
+ *     vocabulary when the new index has it, else an owned key again, n_terms(new) + r, r its rank ascending bytewise
+ *     among the carried keys the new vocabulary lacks (the numbering of one tsvector insert into a fresh segment);
+ *   - keyed index, ordinals numbered by the caller: the seal's term map.  A carried ordinal >= n_source_terms (no key
+ *     is known for it) or whose key vanished in the seal is refused (BM25X_ERR_INVALID, naming the first carried
+ *     document and the ordinal): the caller inserts those documents again;
+ *   - BM25X_TERM_MISSING stays missing.
+ * A carried document deleted before the rebind keeps no element: its postings are gone, so its keys are not carried.
+ * The carried documents then score with the new index's N, df and avgdl, as the reference's do after `maintain`.
+ * late_deleted is the seal's growing map applied to the folded ordinals deleted since its snapshot: the caller ORs it
+ * into allow_sealed and the next seal's sealed_deleted.
+ * The call accepts only the handle the segment's latest successful seal returned, named by a serial number every index
+ * and sharded handle gets when it is created (an address may be reused).  Until the rebind the segment keeps the record
+ * of that seal: 4 B per folded ordinal and 4 B per source term on the host; a later seal replaces it, a rebind clears
+ * it.  Refusals change nothing but this: the call refreshes the segment first, as a search does, so a refusal that
+ * comes after the refresh (the keyed refusals, the tf one, BM25X_ERR_OOM / BM25X_ERR_CUDA) leaves it refreshed (get_info's pending
+ * 0, the handle of the same documents rebuilt); the documents, the seal's record and every row stay as they were.
+ * Refusals: null arguments; no seal to rebind to, or a handle that is not the latest seal's
+ * result; an unsharded segment given to _sharded or the reverse; the keyed refusals above; a carried posting with
+ * tf >= 2^24 on a term the new index holds (BM25X_ERR_UNSUPPORTED, as the insert of the restated documents refuses it);
+ * BM25X_ERR_OOM / BM25X_ERR_CUDA.  Concurrency: the call is ordered with tsvector inserts and holds the segment's lock while it
+ * refreshes and builds the carried documents' handle, then swaps sealed side, statistics and handle in one step.  Every
+ * search, candidate search and tsvector query takes that binding as one, so it sees the old one or the new one, never a
+ * mix; ordinal arguments (delete, allow_growing, candidate ids) are read against the binding the call locks.  The call
+ * returns once every call that took the old binding has released it (a seal in flight included): the old index may then
+ * be destroyed.  A seal that began before the rebind and would take its snapshot after it is refused (BM25X_ERR_INVALID,
+ * "seal it again"); a seal whose snapshot came before the rebind returns its index but leaves no record, so a rebind to
+ * that index is refused ("no seal to rebind to").  Device memory at the peak, on the new home device (the index, or its
+ * last shard): the old handle and the new one, plus scratch: 4.125 B per old ordinal (the bitmap of the folded and
+ * deleted ordinals, the map of the carried ones), 12 B per term of the old handle (the count and its scan), 8 B per old
+ * source term (the offsets of the postings going up), 4 B per new term, n_carried / 8 B, and 8 B per carried posting
+ * that moves between the handle and the host (down through the host or up from it).  When the seal dropped the old last
+ * shard and the new last shard is on another device, every carried posting goes through the host: the scratch of the
+ * old ordinals and old terms is then on the old device. */
+typedef struct {
+    uint8_t *late_deleted;    /* out, [ceil(n_docs(new)/8)] or NULL: bit d set = new sealed document d is a growing
+                                 ordinal the seal folded in and the segment deleted after the seal's snapshot; every
+                                 other bit written 0 (the layout of `allow` / sealed_deleted) */
+    uint32_t n_late_deleted;  /* out */
+    uint32_t n_folded;        /* out: the seal's n_growing */
+    uint32_t n_carried;       /* out: ordinals carried over: old ordinal n_folded + i becomes ordinal i */
+} bm25x_rebind_args;
+int bm25x_growing_rebind(bm25x_growing_segment *g, bm25x_index *sealed, bm25x_rebind_args *a);
+int bm25x_growing_rebind_sharded(bm25x_growing_segment *g, bm25x_sharded_index *sealed, bm25x_rebind_args *a);
 /* Test hook: the arrays of shard s (0 <= s < n_shards) as bm25x_index_get_layout / bm25x_index_get_derived report them
  * for an index: local doc ids, local n_docs / n_postings / df, the whole segment's avgdl and score tables.  The shard
  * handle itself stays internal.  Either output may be NULL. */

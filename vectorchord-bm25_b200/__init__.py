@@ -7,9 +7,10 @@ falls back to a CPU implementation: if the library or an H100 is missing, calls 
 """
 from .bm25x import (Bm25xError, Index, Batch, SearchStats, IndexLayout, IndexDerived, synth_corpus, synth_queries, load_library, build_library,
                     device_count, Document, Query, MAX_K, MAX_QUERY_TERMS, TERM_MISSING, merge_topk, check_vectors, Broker,
-                    ShardedIndex, MAX_SHARDS, merge_shards, GrowingSegment, GrowingInfo, SealArgs, Export, cast_tsvectors)
+                    ShardedIndex, MAX_SHARDS, merge_shards, GrowingSegment, GrowingInfo, SealArgs, RebindArgs, Export,
+                    cast_tsvectors)
 
 __all__ = ["Bm25xError", "Index", "Batch", "SearchStats", "IndexLayout", "IndexDerived", "synth_corpus", "synth_queries", "load_library",
            "build_library", "device_count", "Document", "Query", "MAX_K", "MAX_QUERY_TERMS", "TERM_MISSING", "merge_topk",
            "check_vectors", "Broker", "ShardedIndex", "MAX_SHARDS", "merge_shards",
-           "GrowingSegment", "GrowingInfo", "SealArgs", "Export", "cast_tsvectors"]
+           "GrowingSegment", "GrowingInfo", "SealArgs", "RebindArgs", "Export", "cast_tsvectors"]

@@ -82,6 +82,11 @@ class SealArgs(C.Structure):  # bm25x_seal_args
                 ("n_source_terms", C.c_uint32)]
 
 
+class RebindArgs(C.Structure):  # bm25x_rebind_args
+    _fields_ = [("late_deleted", C.POINTER(C.c_uint8)), ("n_late_deleted", C.c_uint32), ("n_folded", C.c_uint32),
+                ("n_carried", C.c_uint32)]
+
+
 class IndexInfo(C.Structure):
     _fields_ = [("n_docs", C.c_uint32), ("n_terms", C.c_uint32), ("n_postings", C.c_uint64),
                 ("sum_doc_len", C.c_uint64), ("avgdl", C.c_double), ("k1", C.c_double), ("b", C.c_double),
@@ -178,6 +183,8 @@ def load_library():
     L.bm25x_growing_seal.argtypes = [vp, C.POINTER(SealArgs), C.POINTER(vp)]
     L.bm25x_growing_open_sharded.argtypes = [vp, C.POINTER(vp)]
     L.bm25x_growing_seal_sharded.argtypes = [vp, C.POINTER(SealArgs), C.POINTER(vp)]
+    L.bm25x_growing_rebind.argtypes = [vp, vp, C.POINTER(RebindArgs)]
+    L.bm25x_growing_rebind_sharded.argtypes = [vp, vp, C.POINTER(RebindArgs)]
     L.bm25x_growing_insert_tsvectors.argtypes = [vp, u8p, C.POINTER(_Tsvectors), u16p]
     L.bm25x_growing_get_new_keys.argtypes = [vp, C.c_uint32, u8p, u32p]
     L.bm25x_growing_tsvector_queries.argtypes = [vp, u8p, C.POINTER(_Tsvectors), u32p, u32p]
@@ -909,6 +916,20 @@ class GrowingSegment:
                 _check(L.bm25x_index_get_info(h, C.byref(info)))
                 ix = Index._adopt(h, info.n_docs, info.n_terms)
             return ix, smap, gmap[:a.n_growing].copy(), tmap[:a.n_source_terms].copy()
+
+    def rebind(self, new_index):
+        """The segment goes on over new_index, the Index (or ShardedIndex) its latest seal returned
+        (bm25x_growing_rebind / _sharded): the ordinals the seal folded in leave it, ordinal n_folded + i becomes i.
+        Returns the new ids of the folded documents deleted after the seal's snapshot, ascending (to OR into
+        allow_sealed and the next seal's sealed_deleted).  self.sealed then is new_index; the old index may be closed."""
+        L = load_library()
+        late = np.zeros(max((new_index.n_docs + 7) // 8, 1), np.uint8)
+        a = RebindArgs()
+        a.late_deleted = _p(late, C.c_uint8)
+        call = L.bm25x_growing_rebind_sharded if self.sharded else L.bm25x_growing_rebind
+        _check(call(self.h, new_index.h, C.byref(a)))
+        self.sealed = new_index
+        return np.flatnonzero(np.unpackbits(late, bitorder="little")[:new_index.n_docs]).astype(np.uint32)
 
     def close(self):
         if getattr(self, "h", None):

@@ -6,6 +6,7 @@
 
 #include <algorithm>
 #include <array>
+#include <atomic>
 #include <chrono>
 #include <memory>
 #include <mutex>
@@ -83,7 +84,15 @@ struct DeviceIndex {
     uint16_t *payload = nullptr;    // [n_docs*3]
 };
 
+// A number no other index or sharded handle of this process has had: the growing segment names its seal's result by it
+// (bm25x_growing_rebind), since a destroyed handle's address may come back with the next one.
+inline uint64_t bm25x_next_serial() {
+    static std::atomic<uint64_t> n{0};
+    return ++n;
+}
+
 struct bm25x_index {
+    const uint64_t serial = bm25x_next_serial();
     int device = 0;
     int sm_count = 0;
     DeviceIndex d;
@@ -122,6 +131,7 @@ struct bm25x_index {
 // Document-sharded index (bm25x_sharded_*): shard s is an ordinary index over the documents [bounds[s], bounds[s+1]) with
 // local ids, built with the whole segment's statistics (one Stats object), so it scores with the same s0 / s1 bits.
 struct bm25x_sharded_index {
+    const uint64_t serial = bm25x_next_serial();
     uint32_t n_shards = 0;
     std::vector<uint32_t> bounds;        // [n_shards+1]
     std::vector<bm25x_index *> shards;   // [n_shards]

@@ -7,6 +7,7 @@
 
 #include <algorithm>
 #include <chrono>
+#include <future>
 #include <memory>
 #include <unordered_map>
 #include <unordered_set>
@@ -189,13 +190,52 @@ static Key16 key16(const uint8_t *p) {
     return k;
 }
 
+// What a segment is bound to: its sealed side, the statistics it scores with (the sealed segment's, computed once) and,
+// over a document-sharded side, that side's vocabulary on the home device (an index keeps its own,
+// bm25x_index.key_vocab).  A call that reads the sealed side outside the segment's lock takes the binding under it,
+// together with the handle, and holds its reference until it returns; a rebind swaps both in one step, then waits until
+// the last holder of the old binding has dropped it (`released`, set by the rebind, fires in the destructor).
+struct Binding {
+    SealedSide sealed;
+    Stats stats;
+    int device;
+    std::mutex vocab_mu;
+    void *key_vocab = nullptr;
+    std::promise<void> *released = nullptr;
+
+    explicit Binding(const SealedSide &s) : sealed(s), stats(s.stats()), device(s.home().device) {}
+    ~Binding() {
+        if (key_vocab) {
+            cudaSetDevice(device);
+            cudaFree(key_vocab);
+        }
+        if (released) released->set_value();
+    }
+    // the vocabulary tsvector_rows casts against
+    TsvVocab vocab() {
+        if (sealed.ix) return {sealed.ix->device, &sealed.ix->h_keys, sealed.ix->d.n_terms, &sealed.ix->key_vocab,
+                               &sealed.ix->key_vocab_mutex};
+        return {device, &sealed.keys(), sealed.n_terms(), &key_vocab, &vocab_mu};
+    }
+};
+
+// The record of a segment's latest successful seal, what its rebind needs (serial == 0: none): the serial of the handle
+// it returned, its n_growing, growing map and term map.
+struct SealRecord {
+    uint64_t serial = 0;
+    uint32_t n_growing = 0;
+    std::vector<uint32_t> gmap, tmap;
+};
+
 // ---- the mutable growing segment (DESIGN §4.5): the documents on the host as the reference's VectorTuples keep them
 // (norm, payload, deleted bit), their postings in one index handle on the sealed side's home device, brought up to date
 // by a refresh ----
 struct bm25x_growing_segment {
-    SealedSide sealed;
-    Stats stats;                       // the sealed segment's, computed once
+    const bool sharded;                // opened over a document-sharded index (a rebind keeps the kind)
     mutable std::mutex mu;             // guards everything below; a refresh runs under it
+    // the binding (changed by a rebind only, under mu and num_mu)
+    std::shared_ptr<Binding> bind;
+    SealRecord last_seal;
     int norm_form = -1;                // -1: no insert yet; 1: doc_len; 0: doc_fieldnorm
     std::vector<uint8_t> fieldnorm;    // per ordinal
     std::vector<uint32_t> doc_len;     // per ordinal (doc_len form only)
@@ -225,23 +265,16 @@ struct bm25x_growing_segment {
     bool owns_keys = false;
     std::vector<uint8_t> new_keys;
     std::unordered_map<Key16, uint32_t, Key16Hash> key_ord;
-    // a sharded side's vocabulary on the home device (an index keeps its own, bm25x_index.key_vocab)
-    std::mutex vocab_mu;
-    void *key_vocab = nullptr;
 
-    explicit bm25x_growing_segment(const SealedSide &s) : sealed(s), stats(s.stats()) {}
-    ~bm25x_growing_segment() {
-        if (!key_vocab) return;
-        cudaSetDevice(sealed.home().device);
-        cudaFree(key_vocab);
-    }
+    explicit bm25x_growing_segment(const SealedSide &s) : sharded(s.sx != nullptr), bind(std::make_shared<Binding>(s)) {}
     uint32_t n_docs() const { return (uint32_t)deleted.size(); }
     uint32_t n_keys() const { return (uint32_t)(new_keys.size() / 16); }
-    // the vocabulary tsvector_rows casts against
-    TsvVocab vocab() {
-        if (sealed.ix) return {sealed.ix->device, &sealed.ix->h_keys, sealed.ix->d.n_terms, &sealed.ix->key_vocab,
-                               &sealed.ix->key_vocab_mutex};
-        return {sealed.home().device, &sealed.keys(), sealed.n_terms(), &key_vocab, &vocab_mu};
+    // the sealed side, under mu or num_mu
+    const SealedSide &sealed() const { return bind->sealed; }
+    // the binding, for a call that reads it outside the lock
+    std::shared_ptr<Binding> binding() const {
+        std::lock_guard<std::mutex> lock(mu);
+        return bind;
     }
 };
 
@@ -286,15 +319,15 @@ static int growing_insert_locked(bm25x_growing_segment *g, const bm25x_growing_d
     }
     const uint32_t first = g->n_docs(), G = docs->n_docs;
     GrowingCsr csr;
-    const int rc = invert_growing(g->sealed, docs, first, csr);
+    const int rc = invert_growing(g->sealed(), docs, first, csr);
     if (rc != BM25X_OK) return rc;
     for (uint32_t d = 0; sealed_only && d < G; d++)  // (invert_growing checked the offsets)
         for (uint64_t e = docs->elem_off[d]; e < docs->elem_off[d + 1]; e++) {
             const uint32_t t = docs->elem_term[e];
-            if (t >= g->sealed.n_terms() && t != BM25X_TERM_MISSING) {
+            if (t >= g->sealed().n_terms() && t != BM25X_TERM_MISSING) {
                 bm25x_set_error("bm25x_growing_insert: document %u holds term ordinal %u >= n_terms(sealed)=%u, but the "
                                 "segment numbers its new terms itself (bm25x_growing_insert_tsvectors)", d, t,
-                                g->sealed.n_terms());
+                                g->sealed().n_terms());
                 return BM25X_ERR_INVALID;
             }
         }
@@ -323,8 +356,8 @@ static int growing_insert_locked(bm25x_growing_segment *g, const bm25x_growing_d
     g->pend_doc.insert(g->pend_doc.end(), csr.doc.begin(), csr.doc.end());
     g->pend_tf.insert(g->pend_tf.end(), csr.tf.begin(), csr.tf.end());
     // the seal's share: dormant postings, Σ tf (doc_fieldnorm form), new ordinals
-    const uint32_t T = g->sealed.n_terms();
-    const std::vector<uint32_t> &sdf = g->sealed.df();
+    const uint32_t T = g->sealed().n_terms();
+    const std::vector<uint32_t> &sdf = g->sealed().df();
     for (uint32_t d = 0; d < G; d++) {
         const bool live = !(docs->deleted && docs->deleted[d]);
         uint64_t sum = 0;
@@ -361,7 +394,7 @@ extern "C" int bm25x_growing_insert(bm25x_growing_segment *g, const bm25x_growin
 static int check_caller_numbered(const char *who, const bm25x_growing_segment *g) {
     if (g->owns_keys || g->new_terms.empty()) return BM25X_OK;
     bm25x_set_error("%s: the segment holds term ordinal %u >= n_terms(sealed)=%u from bm25x_growing_insert: its new terms "
-                    "are numbered by the caller", who, g->new_terms[0], g->sealed.n_terms());
+                    "are numbered by the caller", who, g->new_terms[0], g->sealed().n_terms());
     return BM25X_ERR_INVALID;
 }
 
@@ -380,9 +413,11 @@ extern "C" int bm25x_growing_insert_tsvectors(bm25x_growing_segment *g, const ui
         return BM25X_ERR_INVALID;
     }
     int rc = check_tsvectors(who, tsv, 0);
-    if (rc == BM25X_OK) rc = check_keyed(g->sealed);
     if (rc != BM25X_OK) return rc;
+    // num_mu also holds the binding: only a rebind changes it, and a rebind takes num_mu first
     std::lock_guard<std::mutex> numbering(g->num_mu);
+    rc = check_keyed(g->sealed());
+    if (rc != BM25X_OK) return rc;
     {
         std::lock_guard<std::mutex> lock(g->mu);
         rc = check_caller_numbered(who, g);
@@ -390,7 +425,7 @@ extern "C" int bm25x_growing_insert_tsvectors(bm25x_growing_segment *g, const ui
     }
     // the call's keys the sealed vocabulary lacks: the ordinal an earlier insert gave, or the next fresh one in key order
     // (g->key_ord changes only under num_mu, held here)
-    const uint32_t T = g->sealed.n_terms(), K = g->n_keys();
+    const uint32_t T = g->sealed().n_terms(), K = g->n_keys();
     std::vector<uint8_t> fresh;
     auto number = [&](uint32_t nu, const uint8_t *keys, uint32_t *ord) {
         for (uint32_t i = 0; i < nu; i++) {
@@ -411,7 +446,7 @@ extern "C" int bm25x_growing_insert_tsvectors(bm25x_growing_segment *g, const ui
         return BM25X_OK;
     };
     TsvRows r;
-    rc = tsvector_rows(who, g->vocab(), seed, tsv, 0, number, r);
+    rc = tsvector_rows(who, g->bind->vocab(), seed, tsv, 0, number, r);
     if (rc != BM25X_OK) return rc;
     // the restated rows go in as bm25x_growing_insert takes them, with the norm in the segment's form
     bm25x_growing_docs d{};
@@ -468,11 +503,12 @@ extern "C" int bm25x_growing_tsvector_queries(bm25x_growing_segment *g, const ui
         bm25x_set_error("%s: null argument", who);
         return BM25X_ERR_INVALID;
     }
-    rc = check_keyed(g->sealed);
+    const std::shared_ptr<Binding> bind = g->binding();
+    rc = check_keyed(bind->sealed);
     if (rc != BM25X_OK) return rc;
     // keys the segment numbered are not in the sealed vocabulary: BM25X_TERM_MISSING, as before the seal they never match
     TsvRows r;
-    rc = tsvector_rows(who, g->vocab(), seed, tsv, 1, {}, r);
+    rc = tsvector_rows(who, bind->vocab(), seed, tsv, 1, {}, r);
     if (rc != BM25X_OK) return rc;
     const uint64_t E = r.off[tsv->n];
     if (E > 0xFFFFFFFFull) {
@@ -592,9 +628,9 @@ static int splice_finish(Scratch &sc, const char *who, bm25x_index *ix, const ui
 static int growing_refresh_locked(bm25x_growing_segment *g) {
     const char *who = "bm25x_growing_refresh";
     if (!g->pending) return BM25X_OK;
-    const bm25x_index &home = g->sealed.home();
-    const std::vector<uint8_t> &keys = g->sealed.keys();
-    const uint32_t N = g->n_docs(), T = g->sealed.n_terms();
+    const bm25x_index &home = g->sealed().home();
+    const std::vector<uint8_t> &keys = g->sealed().keys();
+    const uint32_t N = g->n_docs(), T = g->sealed().n_terms();
     const int device = home.device;
     // ---- the sources: the current handle's lists, then the postings inserted since, against the deleted ordinals ----
     Scratch sc(device);
@@ -614,10 +650,10 @@ static int growing_refresh_locked(bm25x_growing_segment *g) {
                 home.k1, home.b, df.data(), P};
     m.fieldnorm = g->norm_form ? nullptr : g->fieldnorm.data();
     IndexGuard ix;
-    int rc = index_begin(m, &g->stats, device, ix);
+    int rc = index_begin(m, &g->bind->stats, device, ix);
     if (rc == BM25X_OK) rc = splice_finish(sc, who, ix.get(), nullptr, src);
     if (rc != BM25X_OK) return rc;
-    growing_options(ix.get(), g->sealed);
+    growing_options(ix.get(), g->sealed());
     g->cur.reset(ix.release(), IndexDestroy());
     std::vector<uint32_t>().swap(g->pend_term);
     std::vector<uint32_t>().swap(g->pend_doc);
@@ -647,7 +683,7 @@ extern "C" int bm25x_growing_get_info(const bm25x_growing_segment *g, bm25x_grow
     out->n_postings = g->cur ? g->cur->d.n_post : 0;
     out->device_bytes = g->cur ? g->cur->device_bytes : 0;
     out->pending = g->pending ? 1u : 0u;
-    out->device = g->sealed.home().device;
+    out->device = g->sealed().home().device;
     return BM25X_OK;
 }
 
@@ -678,11 +714,14 @@ extern "C" int bm25x_growing_search_batch(bm25x_growing_segment *g, uint32_t nq,
     }
     if (const int rc = check_k(k, false); rc != BM25X_OK) return rc;  // before the refresh: a refused call leaves it pending
     const auto t0 = std::chrono::steady_clock::now();
-    std::shared_ptr<bm25x_index> cur;  // this search's state of the segment (NULL: nothing inserted yet)
+    // this search's state of the segment: its binding and its handle (NULL: nothing inserted yet), taken as one
+    std::shared_ptr<Binding> bind;
+    std::shared_ptr<bm25x_index> cur;
     {
         std::lock_guard<std::mutex> lock(g->mu);
         const int rc = growing_refresh_locked(g);
         if (rc != BM25X_OK) return rc;
+        bind = g->bind;
         cur = g->cur;
     }
     std::vector<uint8_t> ag;  // allow_growing over the handle's ordinals: the caller's bits below allow_growing_docs
@@ -695,7 +734,7 @@ extern "C" int bm25x_growing_search_batch(bm25x_growing_segment *g, uint32_t nq,
     SideFilter f;
     f.allow_sealed = allow_sealed;
     f.allow_growing = cur && allow_growing ? ag.data() : nullptr;
-    return sealed_side_search("bm25x_growing_search_batch", g->sealed, cur.get(), f, true, nq, q_off, q_terms, k,
+    return sealed_side_search("bm25x_growing_search_batch", bind->sealed, cur.get(), f, true, nq, q_off, q_terms, k,
                               {out_doc, out_score, out_score64, out_payload, out_n}, stats, t0);
 }
 
@@ -710,20 +749,22 @@ extern "C" int bm25x_growing_search_candidates(bm25x_growing_segment *g, uint32_
     }
     if (const int rc = check_k(k, false); rc != BM25X_OK) return rc;  // before the refresh: a refused call leaves it pending
     const auto t0 = std::chrono::steady_clock::now();
+    std::shared_ptr<Binding> bind;
     std::shared_ptr<bm25x_index> cur;
     {
         std::lock_guard<std::mutex> lock(g->mu);
         const int rc = growing_refresh_locked(g);
         if (rc != BM25X_OK) return rc;
+        bind = g->bind;
         cur = g->cur;
     }
     // before the first insert the sealed side alone answers: its ids are the only ones
     if (!cur)
-        if (const int rc = check_candidates(who, nq, c_off, c_docs, g->sealed.n_docs()); rc != BM25X_OK) return rc;
+        if (const int rc = check_candidates(who, nq, c_off, c_docs, bind->sealed.n_docs()); rc != BM25X_OK) return rc;
     SideFilter f;
     f.c_off = c_off;
     f.c_docs = c_docs;
-    return sealed_side_search(who, g->sealed, cur.get(), f, true, nq, q_off, q_terms, k,
+    return sealed_side_search(who, bind->sealed, cur.get(), f, true, nq, q_off, q_terms, k,
                               {out_doc, out_score, out_score64, out_payload, out_n}, stats, t0);
 }
 
@@ -748,16 +789,18 @@ struct SealSnapshot {
 // until then bm25x_sharded_destroy holds it, so that a refusal frees every handle built so far.  Refusals and maps are
 // bm25x_growing_seal's, named by `who`.
 static int seal_segment(const char *who, bm25x_growing_segment *g, bm25x_seal_args *a, bm25x_sharded_index **out) {
-    const uint32_t NS = g->sealed.n_docs(), T = g->sealed.n_terms();
+    const std::shared_ptr<Binding> bind = g->binding();  // held to the end: a rebind waits for it
+    const SealedSide &sealed = bind->sealed;
+    const uint32_t NS = sealed.n_docs(), T = sealed.n_terms();
     uint32_t K = a->n_new_keys;
-    bool keyed = !g->sealed.keys().empty();
+    bool keyed = !sealed.keys().empty();
     // ---- the new keys: each unlike every sealed key and every other new key.  The caller's, or (taken with the
     // snapshot below) those the segment owns, which are so by construction ----
     if (a->new_keys && !keyed) {
         bm25x_set_error("%s: new_keys given, but the sealed index was created without term keys", who);
         return BM25X_ERR_INVALID;
     }
-    const uint8_t *skeys = g->sealed.keys().data(), *nkeys = a->new_keys;
+    const uint8_t *skeys = sealed.keys().data(), *nkeys = a->new_keys;
     std::vector<uint8_t> owned;
     auto key_of = [&](uint32_t t) { return t < T ? skeys + (size_t)t * 16 : nkeys + (size_t)(t - T) * 16; };
     auto key_less = [&](uint32_t x, uint32_t y) { return memcmp(key_of(x), key_of(y), 16) < 0; };
@@ -789,6 +832,10 @@ static int seal_segment(const char *who, bm25x_growing_segment *g, bm25x_seal_ar
     uint32_t n_src;
     {
         std::lock_guard<std::mutex> lock(g->mu);
+        if (g->bind != bind) {
+            bm25x_set_error("%s: the segment was rebound while the seal began: seal it again", who);
+            return BM25X_ERR_INVALID;
+        }
         const uint32_t NG = g->n_docs();
         if (g->owns_keys) {
             if (a->new_keys || a->n_new_keys) {
@@ -842,7 +889,7 @@ static int seal_segment(const char *who, bm25x_growing_segment *g, bm25x_seal_ar
     uint32_t N = ns_keep;
     for (uint32_t o = 0; o < NG; o++) gmap[o] = s.deleted[o] ? BM25X_DOC_INF : N++;
     // ---- per part: its survivors' new ids [new_lo, new_lo + n_new) (the last part's include the growing survivors) ----
-    const std::vector<SealPart> parts = g->sealed.parts();
+    const std::vector<SealPart> parts = sealed.parts();
     const uint32_t NP = (uint32_t)parts.size();
     std::vector<uint32_t> new_lo(NP + 1, 0);
     for (uint32_t p = 0; p < NP; p++) {
@@ -934,7 +981,7 @@ static int seal_segment(const char *who, bm25x_growing_segment *g, bm25x_seal_ar
     for (uint32_t d = 0; d < N; d++) sum_len += len[d];
     // ---- rules 5 and 7: ONE set of statistics for the new segment; per part that keeps a document, a new handle on its
     // device scoring with them, its survivors spliced into it, then what every index derives from them ----
-    const double k1 = g->sealed.home().k1, b = g->sealed.home().b;
+    const double k1 = sealed.home().k1, b = sealed.home().b;
     const Stats st(N, sum_len, df.data(), TN, k1, b);
     std::unique_ptr<bm25x_sharded_index, void (*)(bm25x_sharded_index *)> sx(new bm25x_sharded_index(),
                                                                              bm25x_sharded_destroy);
@@ -970,6 +1017,16 @@ static int seal_segment(const char *who, bm25x_growing_segment *g, bm25x_seal_ar
     if (a->sealed_map) std::copy(smap.begin(), smap.end(), a->sealed_map);
     if (a->growing_map) std::copy(gmap.begin(), gmap.end(), a->growing_map);
     if (a->term_map) std::copy(tmap.begin(), tmap.end(), a->term_map);
+    {
+        // the record a rebind to this result needs; a seal that a rebind overtook leaves none (its ordinals are gone)
+        std::lock_guard<std::mutex> lock(g->mu);
+        if (g->bind == bind) {
+            g->last_seal.serial = g->sharded ? sx->serial : sx->shards[0]->serial;
+            g->last_seal.n_growing = NG;
+            g->last_seal.gmap = std::move(gmap);
+            g->last_seal.tmap = std::move(tmap);
+        }
+    }
     *out = sx.release();
     return BM25X_OK;
 }
@@ -981,7 +1038,7 @@ extern "C" int bm25x_growing_seal(bm25x_growing_segment *g, bm25x_seal_args *a, 
         return BM25X_ERR_INVALID;
     }
     *out = nullptr;
-    if (g->sealed.sx) {
+    if (g->sharded) {
         bm25x_set_error("%s: the segment was opened over a document-sharded index: seal it with bm25x_growing_seal_sharded",
                         who);
         return BM25X_ERR_INVALID;
@@ -1002,9 +1059,281 @@ extern "C" int bm25x_growing_seal_sharded(bm25x_growing_segment *g, bm25x_seal_a
         return BM25X_ERR_INVALID;
     }
     *out = nullptr;
-    if (!g->sealed.sx) {
+    if (!g->sharded) {
         bm25x_set_error("%s: the segment was opened over an unsharded index: seal it with bm25x_growing_seal", who);
         return BM25X_ERR_INVALID;
     }
     return seal_segment(who, g, a, out);
+}
+
+// ---- the rebind (DESIGN §4.5): the segment goes on over the index its latest seal built.  The ordinals the seal folded
+// in leave it, the carried ones are renumbered from 0 and their elements translated to the new vocabulary; the carried
+// postings of the new handle come from the current handle on the device and from the host's dormant list ----
+
+// How a carried element's term is translated: the segment's numbering of its terms.
+enum class Numbering { KEYLESS, OWNED, CALLER };
+
+static int rebind_segment(const char *who, bm25x_growing_segment *g, const SealedSide &side, uint64_t serial,
+                          bm25x_rebind_args *a) {
+    std::unique_lock<std::mutex> numbering(g->num_mu);  // ordered with the tsvector inserts, which read the binding
+    std::unique_lock<std::mutex> lock(g->mu);
+    const SealRecord &rec = g->last_seal;
+    if (!rec.serial) {
+        bm25x_set_error("%s: no seal to rebind to (no seal of the segment has succeeded since it was opened or last "
+                        "rebound)", who);
+        return BM25X_ERR_INVALID;
+    }
+    if (rec.serial != serial) {
+        bm25x_set_error("%s: the index is not the one the segment's latest seal returned", who);
+        return BM25X_ERR_INVALID;
+    }
+    int rc = growing_refresh_locked(g);
+    if (rc != BM25X_OK) return rc;
+    const Binding &ob = *g->bind;
+    const uint32_t NG = rec.n_growing, N = g->n_docs(), NC = N - NG;
+    const uint32_t To = ob.sealed.n_terms(), Tn = side.n_terms(), K = g->n_keys();
+    const std::vector<uint32_t> &ndf = side.df();
+    const Numbering kind = g->owns_keys ? Numbering::OWNED : ob.sealed.keys().empty() ? Numbering::KEYLESS
+                                                                                       : Numbering::CALLER;
+    const uint32_t n_old = std::max(To + K, g->term_end);  // the old source-term space
+    // a term the new handle holds: one with postings in the new index (a growing handle leaves the others out)
+    auto live_new = [&](uint32_t u) { return u < Tn && ndf[u] != 0; };
+    const bm25x_index *cur = NC ? g->cur.get() : nullptr;
+    const int od = ob.device, nd = side.home().device;
+    const bool same = od == nd;
+    // ---- the carried ordinals: old o >= NG becomes o - NG; a folded or deleted ordinal gives no posting ----
+    std::vector<uint8_t> gone(N);
+    std::vector<uint32_t> cmap(N);
+    for (uint32_t o = 0; o < N; o++) {
+        gone[o] = o < NG || g->deleted[o];
+        cmap[o] = o < NG ? BM25X_DOC_INF : o - NG;
+    }
+    const std::vector<uint32_t> bits = deleted_bitmap(gone);
+    // ---- the current handle's carried survivors per term (k_splice_count), on its device ----
+    Scratch sco(od);
+    sco.e = cudaSetDevice(od);
+    SpliceSources hs{};
+    std::vector<uint32_t> hcnt;
+    if (cur) {
+        hs.s[0] = handle_source(cur, sco.up(bits.data(), bits.size()), sco.up(cmap.data(), N));
+        hcnt = splice_count(sco, cur->sm_count, To, hs);
+        if (sco.e != cudaSuccess) return cuda_refusal(who, "count", sco.e);
+    }
+    hcnt.resize(To, 0);
+    std::vector<uint32_t> dcnt(n_old, 0);  // the carried dormant postings per term
+    for (size_t i = 0; i < g->dorm_doc.size(); i++)
+        if (!gone[g->dorm_doc[i]]) dcnt[g->dorm_term[i]]++;
+    // ---- the translation of every old term a carried posting holds ----
+    std::vector<uint32_t> xl(n_old, BM25X_TERM_MISSING);
+    std::vector<uint8_t> owned;  // OWNED: the carried keys the new vocabulary lacks, ascending
+    if (kind == Numbering::KEYLESS) {
+        for (uint32_t t = 0; t < n_old; t++) xl[t] = t;
+    } else if (kind == Numbering::CALLER) {
+        for (uint32_t t = 0; t < n_old && t < (uint32_t)rec.tmap.size(); t++) xl[t] = rec.tmap[t];
+    } else {
+        const uint8_t *okeys = ob.sealed.keys().data(), *nkeys = side.keys().data();
+        auto key_of = [&](uint32_t t) { return t < To ? okeys + (size_t)t * 16 : g->new_keys.data() + (size_t)(t - To) * 16; };
+        std::vector<uint32_t> lack;
+        for (uint32_t t = 0; t < n_old; t++) {
+            if (!(t < To ? hcnt[t] : 0) && !dcnt[t]) continue;
+            xl[t] = key_ordinal(nkeys, Tn, key_of(t));
+            if (xl[t] == BM25X_TERM_MISSING) lack.push_back(t);
+        }
+        std::sort(lack.begin(), lack.end(), [&](uint32_t x, uint32_t y) { return memcmp(key_of(x), key_of(y), 16) < 0; });
+        if ((uint64_t)Tn + lack.size() >= BM25X_TERM_MISSING) {
+            bm25x_set_error("%s: more than %u term ordinals (%u is BM25X_TERM_MISSING)", who, BM25X_TERM_MISSING,
+                            BM25X_TERM_MISSING);
+            return BM25X_ERR_UNSUPPORTED;
+        }
+        for (uint32_t r = 0; r < (uint32_t)lack.size(); r++) {
+            xl[lack[r]] = Tn + r;
+            owned.insert(owned.end(), key_of(lack[r]), key_of(lack[r]) + 16);
+        }
+    }
+    // ---- down: the carried postings of the handle's terms the new handle does not keep (across devices: all of them),
+    // compacted on the device by k_splice_emit at the offsets of their scan, then one download ----
+    std::vector<uint64_t> down_off((size_t)To + 1, 0);
+    for (uint32_t t = 0; t < To; t++)
+        down_off[(size_t)t + 1] = down_off[t] + (!same || !live_new(xl[t]) ? hcnt[t] : 0);
+    const uint64_t D = down_off[To];
+    std::vector<uint32_t> dn_term(D), dn_doc(D), dn_tf(D);
+    if (D) {
+        const uint64_t *d_off = sco.up(down_off.data(), down_off.size());
+        uint32_t *d_doc = sco.alloc<uint32_t>(D), *d_tf = sco.alloc<uint32_t>(D);
+        if (sco.e == cudaSuccess) {
+            k_splice_emit<<<splice_grid(To, cur->sm_count), 256>>>(To, hs.s[0], d_off, d_doc, d_tf);
+            sco.e = cudaGetLastError();
+        }
+        if (sco.e == cudaSuccess) sco.e = cudaMemcpy(dn_doc.data(), d_doc, sizeof(uint32_t) * D, cudaMemcpyDeviceToHost);
+        if (sco.e == cudaSuccess) sco.e = cudaMemcpy(dn_tf.data(), d_tf, sizeof(uint32_t) * D, cudaMemcpyDeviceToHost);
+        if (sco.e != cudaSuccess) return cuda_refusal(who, "carry", sco.e);
+        for (uint32_t t = 0; t < To; t++)
+            std::fill(dn_term.begin() + down_off[t], dn_term.begin() + down_off[(size_t)t + 1], t);
+    }
+    // ---- the carried postings on the host (down, then dormant; a term has postings in one of them only): a keyed
+    // caller-numbered term without a new ordinal is refused, a term the new handle keeps goes up, any other stays
+    // dormant under its new ordinal ----
+    if (kind == Numbering::CALLER) {
+        uint64_t worst = ~0ull;  // (carried ordinal, old term) of the first carried posting without a new ordinal
+        for (uint64_t i = 0; i < D; i++)
+            if (xl[dn_term[i]] == BM25X_TERM_MISSING) worst = std::min(worst, (uint64_t)dn_doc[i] << 32 | dn_term[i]);
+        for (size_t i = 0; i < g->dorm_doc.size(); i++) {
+            const uint32_t o = g->dorm_doc[i], t = g->dorm_term[i];
+            if (!gone[o] && xl[t] == BM25X_TERM_MISSING) worst = std::min(worst, (uint64_t)(o - NG) << 32 | t);
+        }
+        if (worst != ~0ull) {
+            const uint32_t o = (uint32_t)(worst >> 32) + NG, t = (uint32_t)worst;
+            if (t >= rec.tmap.size())
+                bm25x_set_error("%s: growing ordinal %u holds term ordinal %u >= n_source_terms=%u of the seal: no key is "
+                                "known for it (insert the document again)", who, o, t, (uint32_t)rec.tmap.size());
+            else
+                bm25x_set_error("%s: growing ordinal %u holds term ordinal %u, whose key vanished in the seal (insert the "
+                                "document again)", who, o, t);
+            return BM25X_ERR_INVALID;
+        }
+    }
+    std::vector<uint32_t> up_term, up_doc, up_tf, nd_term, nd_doc, nd_tf;
+    bool big = false;
+    auto route = [&](uint32_t t, uint32_t d, uint32_t f) {
+        const uint32_t u = xl[t];
+        if (live_new(u)) {
+            big |= f >= (1u << 24);
+            up_term.push_back(t);
+            up_doc.push_back(d);
+            up_tf.push_back(f);
+        } else {
+            nd_term.push_back(u);
+            nd_doc.push_back(d);
+            nd_tf.push_back(f);
+        }
+    };
+    for (uint64_t i = 0; i < D; i++) route(dn_term[i], dn_doc[i], dn_tf[i]);
+    for (size_t i = 0; i < g->dorm_doc.size(); i++)
+        if (!gone[g->dorm_doc[i]]) route(g->dorm_term[i], g->dorm_doc[i] - NG, g->dorm_tf[i]);
+    if (big) {  // what the insert of the restated documents refuses
+        bm25x_set_error("%s: term frequency >= 2^24 is not supported by the packed posting layout", who);
+        return BM25X_ERR_UNSUPPORTED;
+    }
+    // ---- the new handle: new term u from old term src_of[u], its survivors in the handle (same device) and those that
+    // came up, opened with the new statistics on the new home device ----
+    const auto nb = std::make_shared<Binding>(side);
+    IndexGuard ix;
+    if (NC) {
+        std::unique_ptr<Scratch> other;
+        Scratch &scn = same ? sco : *(other = std::make_unique<Scratch>(nd));
+        scn.e = cudaSetDevice(nd);
+        std::vector<uint32_t> src_of(Tn, BM25X_TERM_MISSING), df(Tn, 0), ucnt(n_old, 0);
+        for (uint32_t t : up_term) ucnt[t]++;
+        uint64_t P = 0;
+        for (uint32_t t = 0; t < n_old; t++)
+            if (live_new(xl[t])) {
+                src_of[xl[t]] = t;
+                P += df[xl[t]] = (same && t < To ? hcnt[t] : 0) + ucnt[t];
+            }
+        const std::vector<uint32_t> zero(((size_t)NC + 31) / 32, 0);
+        SpliceSources src{};
+        if (same) src.s[0] = hs.s[0];
+        src.s[1] = grouped_source(scn, n_old, up_term, up_doc, up_tf, scn.up(zero.data(), zero.size()), nullptr);
+        if (scn.e != cudaSuccess) return cuda_refusal(who, "carry", scn.e);
+        const std::vector<uint8_t> &keys = side.keys();
+        BuildMeta m{NC, Tn, g->norm_form ? g->doc_len.data() + NG : nullptr, g->payload.data() + (size_t)NG * 3,
+                    keys.empty() ? nullptr : keys.data(), side.home().k1, side.home().b, df.data(), P};
+        m.fieldnorm = g->norm_form ? nullptr : g->fieldnorm.data() + NG;
+        rc = index_begin(m, &nb->stats, nd, ix);
+        if (rc == BM25X_OK) rc = splice_finish(scn, who, ix.get(), scn.up(src_of.data(), Tn), src);
+        if (rc != BM25X_OK) return rc;
+        growing_options(ix.get(), side);
+    }
+    // ---- commit: nothing is refused from here on ----
+    const uint32_t NN = side.n_docs();
+    uint32_t n_late = 0;
+    if (a->late_deleted) memset(a->late_deleted, 0, ((size_t)NN + 7) / 8);
+    for (uint32_t o = 0; o < NG; o++)
+        if (g->deleted[o] && rec.gmap[o] != BM25X_DOC_INF) {
+            n_late++;
+            if (a->late_deleted) a->late_deleted[rec.gmap[o] >> 3] |= (uint8_t)(1u << (rec.gmap[o] & 7u));
+        }
+    a->n_late_deleted = n_late;
+    a->n_folded = NG;
+    a->n_carried = NC;
+    g->fieldnorm.erase(g->fieldnorm.begin(), g->fieldnorm.begin() + NG);
+    if (g->norm_form == 1) g->doc_len.erase(g->doc_len.begin(), g->doc_len.begin() + NG);
+    if (g->norm_form == 0) g->sum_tf.erase(g->sum_tf.begin(), g->sum_tf.begin() + NG);
+    g->payload.erase(g->payload.begin(), g->payload.begin() + (size_t)NG * 3);
+    g->deleted.erase(g->deleted.begin(), g->deleted.begin() + NG);
+    g->n_deleted = (uint32_t)std::count(g->deleted.begin(), g->deleted.end(), (uint8_t)1);
+    // the dormant postings as one insert of the carried documents appends them: by document, then by term
+    std::vector<uint32_t> perm(nd_term.size());
+    for (uint32_t i = 0; i < (uint32_t)perm.size(); i++) perm[i] = i;
+    std::sort(perm.begin(), perm.end(), [&](uint32_t x, uint32_t y) {
+        return nd_doc[x] != nd_doc[y] ? nd_doc[x] < nd_doc[y] : nd_term[x] < nd_term[y];
+    });
+    g->dorm_term.resize(perm.size());
+    g->dorm_doc.resize(perm.size());
+    g->dorm_tf.resize(perm.size());
+    for (size_t i = 0; i < perm.size(); i++) {
+        g->dorm_term[i] = nd_term[perm[i]];
+        g->dorm_doc[i] = nd_doc[perm[i]];
+        g->dorm_tf[i] = nd_tf[perm[i]];
+    }
+    // the carried ordinals >= n_terms(new), in the order they first come in the carried documents (every one of them is
+    // dormant; a keyed caller-numbered segment has none)
+    g->new_terms.clear();
+    g->new_seen.clear();
+    g->term_end = 0;
+    for (uint32_t u : g->dorm_term)
+        if (u >= Tn && g->new_seen.insert(u).second) {
+            g->new_terms.push_back(u);
+            g->term_end = std::max(g->term_end, u + 1);
+        }
+    if (kind == Numbering::OWNED) {
+        g->new_keys = std::move(owned);
+        g->key_ord.clear();
+        for (uint32_t r = 0; r < g->n_keys(); r++) g->key_ord.emplace(key16(&g->new_keys[(size_t)r * 16]), Tn + r);
+    }
+    if (ix) g->cur.reset(ix.release(), IndexDestroy());
+    else g->cur.reset();
+    g->last_seal = SealRecord();
+    std::shared_ptr<Binding> old = std::move(g->bind);
+    g->bind = nb;
+    // ---- the old binding's holders finish with it; its last one fires `released` ----
+    std::promise<void> released;
+    std::future<void> done = released.get_future();
+    old->released = &released;
+    lock.unlock();
+    numbering.unlock();
+    old.reset();
+    done.wait();
+    return BM25X_OK;
+}
+
+extern "C" int bm25x_growing_rebind(bm25x_growing_segment *g, bm25x_index *sealed, bm25x_rebind_args *a) {
+    const char *who = "bm25x_growing_rebind";
+    if (!g || !sealed || !a) {
+        bm25x_set_error("%s: null argument", who);
+        return BM25X_ERR_INVALID;
+    }
+    if (g->sharded) {
+        bm25x_set_error("%s: the segment was opened over a document-sharded index: rebind it with "
+                        "bm25x_growing_rebind_sharded", who);
+        return BM25X_ERR_INVALID;
+    }
+    SealedSide side;
+    side.ix = sealed;
+    return rebind_segment(who, g, side, sealed->serial, a);
+}
+
+extern "C" int bm25x_growing_rebind_sharded(bm25x_growing_segment *g, bm25x_sharded_index *sealed, bm25x_rebind_args *a) {
+    const char *who = "bm25x_growing_rebind_sharded";
+    if (!g || !sealed || !a) {
+        bm25x_set_error("%s: null argument", who);
+        return BM25X_ERR_INVALID;
+    }
+    if (!g->sharded) {
+        bm25x_set_error("%s: the segment was opened over an unsharded index: rebind it with bm25x_growing_rebind", who);
+        return BM25X_ERR_INVALID;
+    }
+    SealedSide side;
+    side.sx = sealed;
+    return rebind_segment(who, g, side, sealed->serial, a);
 }

@@ -1,6 +1,7 @@
 // bm25x_splice.cuh — the term-major postings of a new index handle spliced from lists already on the device
-// (DESIGN §4.5): the refresh of a mutable growing segment (bm25x_growing_refresh) and its seal (bm25x_growing_seal).
-// The refresh is the seal's splice with identity maps and no sealed source.
+// (DESIGN §4.5): the refresh of a mutable growing segment (bm25x_growing_refresh), its seal (bm25x_growing_seal) and its
+// rebind (bm25x_growing_rebind).  The refresh is the seal's splice with identity maps and no sealed source; the rebind's
+// splice takes the carried postings of the current handle and those coming up from the host.
 //
 // A term's postings come from up to three disjoint sources, each read in doc order; a later source's doc ids (after its
 // map) are above every earlier source's, so a term's survivors stay ascending when written source by source:
@@ -76,6 +77,39 @@ __global__ void k_splice_count(uint32_t n, const SpliceSources src, uint32_t *__
         }
         c = __reduce_add_sync(0xFFFFFFFFu, c);
         if (lane == 0) df[t] = c;
+    }
+}
+
+// The reverse direction, for a rebind (bm25x_growing_rebind): the survivors of the handle-form source q for the terms
+// t < n that out_off selects (out_off[t + 1] > out_off[t]; out_off is the exclusive scan of k_splice_count's df over the
+// selected terms, 0 for the others), written at out_off[t] as (map[doc], tf) in doc order, so that one download brings
+// them to the host, which reads each posting's term off out_off.  The same order-preserving ballot / popc compaction as
+// k_splice.
+__global__ void k_splice_emit(uint32_t n, const SpliceSrc q, const uint64_t *__restrict__ out_off,
+                              uint32_t *__restrict__ out_doc, uint32_t *__restrict__ out_tf) {
+    const uint32_t lane = threadIdx.x & 31u, warps = gridDim.x * (blockDim.x >> 5), lt = (1u << lane) - 1u;
+    for (uint32_t t = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); t < n; t += warps) {
+        uint64_t pos = out_off[t];
+        if (out_off[t + 1] == pos) continue;
+        const uint64_t b = q.off[t], e = b + q.df[t];
+        for (uint64_t base = b; base < e; base += 32) {
+            const uint64_t i = base + lane;
+            Posting p;
+            p.doc = 0;
+            p.w = 0;
+            bool keep = false;
+            if (i < e) {
+                p = q.post[i];
+                keep = !splice_deleted(q.del, p.doc);
+            }
+            const uint32_t m = __ballot_sync(0xFFFFFFFFu, keep);
+            if (keep) {
+                const uint64_t at = pos + __popc(m & lt);
+                out_doc[at] = q.map ? q.map[p.doc] : p.doc;
+                out_tf[at] = p.w >> 8;
+            }
+            pos += __popc(m);
+        }
     }
 }
 
